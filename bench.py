@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- rows scanned/sec for Pinot's filter -> project -> GROUP BY aggregate path on B200 (BASELINE.json metric:
+"""bench.py -- rows scanned/sec for Pinot's filter -> project -> GROUP BY aggregate path on H100 (BASELINE.json metric:
 "rows scanned/sec per box, filter+groupby on 100M-row segments, 1/2/4/8 GPU").
 
 Table (per GPU): 8 segments x 100 M rows, 8 dict-encoded fixed-bit INT columns c0..c7 (cardinalities 10 .. 1 000 000 ->
@@ -27,6 +27,11 @@ Table (per GPU): 8 segments x 100 M rows, 8 dict-encoded fixed-bit INT columns c
 
 Multi-GPU (torchrun, one rank per GPU): segments shard whole per GPU, no data-path collective; weak scaling:
 value = total rows of all ranks / max-over-ranks time.
+
+--steps K sets the number of timed steps of every device leg (headline, per-segment blocks, c2) and of the reference arm.
+--dump-outputs DIR writes the headline's results block of the last timed step as DIR/<name>.npy (float64, rows sorted by
+group key): group_key_c3, sum_c5, count.  The tables are generated from fixed seeds, so the same arguments give the same
+inputs on every run and two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -83,7 +88,7 @@ def bytes_per_row() -> float:
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     FIELDS = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
               "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -138,7 +143,18 @@ def measured_peak_gbs():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except (KeyError, ValueError):
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3)"
+
+
+def dump_outputs(out_dir: str, table) -> None:
+    """The headline's results block ({group key: [sum, count]}) as float64 arrays, rows sorted by group key."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    keys = sorted(table)
+    cols = {"group_key_c3": [k if k != () else -1 for k in keys], "sum_c5": [table[k][0] for k in keys],
+            "count": [table[k][1] for k in keys]}
+    for name, values in cols.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), np.asarray(values, dtype=np.float64))
 
 
 def cpu_model() -> str:
@@ -239,9 +255,12 @@ def main():
     ap.add_argument("--c2-selectivity", type=float, default=0.25)
     ap.add_argument("--e2e-steps", type=int, default=3)
     ap.add_argument("--cpu-threads", type=int, default=0, help="0 = all host cores")
-    ap.add_argument("--reference-seconds", type=float, default=120.0, help="time budget of the --impl reference steps")
     ap.add_argument("--quick", action="store_true", help="tuning runs: skip the c2, e2e and cpu_baseline legs")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the headline's results block of the last timed step as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
     args.warmup = max(args.warmup, 3)
 
     rank = int(os.environ.get("RANK", "0"))
@@ -261,7 +280,7 @@ def main():
               "segments_per_gpu": args.segments, "rows_per_segment": args.rows, "selectivity": args.selectivity,
               "groups": CARDS[3], "touched_bits_per_row": int(bpr * 8),
               "l2_policy": f"inputs larger than L2 (touched columns = {args.segments * args.rows * bpr / 1e9:.2f} GB per step "
-                           "per GPU vs 126 MB L2)",
+                           "per GPU vs 50 MB L2 on an H100)",
               "parallelism": f"segments sharded {args.segments}/GPU x {world} GPU, group tables reduced once"}
 
     # ---------------------------------------------------------------------------------------------- reference arm
@@ -269,10 +288,7 @@ def main():
         cores = args.cpu_threads or (os.cpu_count() or 1)
         table = CpuTable(args.segments, args.rows, 0, cores)
         table.run(q_gb)  # warm-up / page-in
-        times = []
-        t_start = time.perf_counter()
-        while len(times) < max(1, args.steps) and (not times or time.perf_counter() - t_start < args.reference_seconds):
-            times.append(table.run(q_gb)[0])
+        times = [table.run(q_gb)[0] for _ in range(args.steps)]
         sec = statistics.mean(times)
         val = table.rows / sec
         line = {"impl": "reference", "metric": METRIC, "value": val, "unit": "rows/s", "n_gpus": args.gpus,
@@ -289,7 +305,7 @@ def main():
         print(json.dumps(line))
         return 0
 
-    # ---------------------------------------------------------------------------------------------- B200 arm
+    # ---------------------------------------------------------------------------------------------- device arm
     import torch
     from pinot_b200.plan_maker import B200Context, B200PlanMaker, IndexSegment
 
@@ -383,6 +399,8 @@ def main():
         gb_table = block_table(gb_out)
         assert gb_table == block_table(gb_first), "non-deterministic result across steps"
         matched = sum(c for _, c in gb_table.values())
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, gb_table)
     gb_out = gb_first = None   # blocks alias native results: dropped before the context closes
     if rank == 0:
         expect = rows_per_step * world * args.selectivity
@@ -405,11 +423,11 @@ def main():
     def gb_blocks_step():
         blocks = pm.execute_segments(segs, q_gb)
         return blocks, blocks[0].device_ms
-    seg_blocks, _, sb_elapsed, sb_kms, _ = timed(gb_blocks_step, max(20, args.steps // 10))
-    sb_steps = max(20, args.steps // 10)
+    sb_steps = args.steps
+    seg_blocks, _, sb_elapsed, sb_kms, _ = timed(gb_blocks_step, sb_steps)
 
     # ---- c2: the aggregation-only scan ----
-    c2_steps = max(20, args.steps // 3)
+    c2_steps = args.steps
     c2_out, c2_first, c2_elapsed, c2_kms, _ = timed(c2_step, c2_steps)
     assert c2_out == c2_first, "non-deterministic c2 result"
     c2_achieved = rows_per_step * bpr / (c2_kms * 1e-3) / 1e9
@@ -487,25 +505,13 @@ def main():
                "parity": f"per-segment and combined group tables of the device == the oracle's on all {table.rows} rows "
                          "(COUNT exact, SUM within 1e-6 relative); c2 result == oracle"}
 
-    # dram__bytes_read.sum + dram__bytes_write.sum of ONE launch of the scan kernel, from the committed `ncu --set full`
-    # captures of these same workloads (profiles/): only quoted when this run IS that workload
-    def traffic_of(name, sel):
-        tpath = os.path.join(ROOT, "profiles", name)
-        if os.path.exists(tpath):
-            tj = json.load(open(tpath))
-            if tj.get("segments") == args.segments and tj.get("rows_per_segment") == args.rows and abs(tj.get("selectivity", -1) - sel) < 1e-9:
-                return tj["dram_bytes_per_launch"], tj["source"]
-        return None, None
-    gb_traffic, gb_traffic_src = traffic_of("r2_gb_traffic.json", args.selectivity)
-    c2_traffic, c2_traffic_src = traffic_of("r2_c2_traffic.json", args.c2_selectivity)
-
     if rank == 0:
         alg = rows_per_step * bpr
         line = {"metric": METRIC, "value": value, "unit": "rows/s", "n_gpus": world, "steps": args.steps,
                 "warmup": args.warmup, "ms_per_step": gb_ms, "higher_is_better": True, "scaling": "weak",
                 "vs_baseline": None, "dtype": "int64", "data": "synthetic", "config": config,
                 "roofline": {"bound": "hbm", "achieved": gb_achieved, "peak": peak, "unit": "GB/s",
-                             "frac": gb_achieved / peak, "traffic": gb_traffic, "traffic_source": gb_traffic_src,
+                             "frac": gb_achieved / peak,
                              "peak_source": peak_src,
                              "kernel": "pb200::scan_kernel<6,true> (group-by, W=6 warps, 2 CTAs/SM)", "kernel_ms": gb_kms,
                              "algorithmic_bytes_per_launch": alg},
@@ -525,7 +531,7 @@ def main():
                 "c2": {"query": c2_query_text(args.c2_selectivity), "value": rows_per_step * world / (c2_elapsed / c2_steps),
                        "ms_per_step": c2_elapsed / c2_steps * 1e3, "steps": c2_steps,
                        "roofline": {"bound": "hbm", "achieved": c2_achieved, "peak": peak, "unit": "GB/s",
-                                    "frac": c2_achieved / peak, "traffic": c2_traffic, "traffic_source": c2_traffic_src,
+                                    "frac": c2_achieved / peak,
                                     "kernel": "pb200::scan_kernel<6,false> (aggregation only)", "kernel_ms": c2_kms,
                                     "algorithmic_bytes_per_launch": alg},
                        "result": {"sum_c5": c2_out[0], "count": c2_out[1], "scope": "rank 0's segments"}},

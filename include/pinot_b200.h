@@ -1,5 +1,5 @@
 /*
- * pinot_b200.h -- C-ABI of libpinot_b200.so: the B200-native implementation of Apache Pinot's per-segment
+ * pinot_b200.h -- C-ABI of libpinot_b200.so: the H100-native (sm_90a) implementation of Apache Pinot's per-segment
  * scan -> filter -> project -> (group-by) aggregate operator chain.
  *
  * This is the drop-in boundary.  In the reference the path is entered through the plan-maker plugin seam

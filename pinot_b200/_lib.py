@@ -1,7 +1,7 @@
 """ctypes binding of libpinot_b200.so (include/pinot_b200.h + include/pinot_b200_host.h).
 
 There is NO fallback: if the shared library is missing or no CUDA device is present, importing / initialising fails
-loudly.  The library is built in-tree by ``python -m pinot_b200.build`` (nvcc, sm_100a).
+loudly.  The library is built in-tree by ``python -m pinot_b200.build`` (nvcc, sm_90a).
 """
 from __future__ import annotations
 

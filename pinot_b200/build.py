@@ -1,4 +1,4 @@
-"""Builds pinot_b200/libpinot_b200.so in-tree with nvcc for sm_100a (no torch, no JIT cache: the .so travels with the repo).
+"""Builds pinot_b200/libpinot_b200.so in-tree with nvcc for sm_90a (no torch, no JIT cache: the .so travels with the repo).
 
     python -m pinot_b200.build            # incremental
     python -m pinot_b200.build --force
@@ -18,7 +18,7 @@ SCAN_KERNELS = ["w6_agg", "w8_agg", "w8_agg_nodefer", "w6_gb1", "w8_gb1", "w6_gb
 SOURCES = [f"pb200_scan_k_{k}.cu" for k in SCAN_KERNELS] + ["pb200_api.cu", "pb200_domain.cu", "pb200_extract.cu", "pb200_comm.cu", "pb200_roaring.cu", "pb200_synth.cu",
                                                              "host/plan_maker.cpp", "host/star_tree.cpp", "host/datatable.cpp", "host/segment_cache.cpp", "host/raw_forward.cpp", "host/filtered_agg.cpp"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
          "-Xptxas", "-v", "--expt-relaxed-constexpr"]
 
 
@@ -53,7 +53,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     with ThreadPoolExecutor(max_workers=min(len(SOURCES), os.cpu_count() or 4)) as ex:
         objs = list(ex.map(compile_one, SOURCES))
     tmp = LIB + ".tmp"  # link beside the target, then rename: a reader (or a repo snapshot) never sees a half-written .so
-    cmd = [NVCC, "-shared", "-o", tmp, *objs, "-cudart", "static", "-gencode", "arch=compute_100a,code=sm_100a", "-ldl"]
+    cmd = [NVCC, "-shared", "-o", tmp, *objs, "-cudart", "static", "-gencode", "arch=compute_90a,code=sm_90a", "-ldl"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

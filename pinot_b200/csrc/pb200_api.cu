@@ -164,10 +164,10 @@ __global__ void fwd_words_to_native_kernel(uint4* __restrict__ p, size_t n16) {
     p[i] = x;
   }
 }
-static cudaError_t fwd_words_to_native(void* p, size_t bytes, cudaStream_t st) {  // bytes: the padded allocation (multiple of 16)
+static cudaError_t fwd_words_to_native(void* p, size_t bytes, int sm_count, cudaStream_t st) {  // bytes: the padded allocation (multiple of 16)
   const size_t n16 = bytes / 16;
   if (!n16) return cudaSuccess;
-  const int blocks = (int)std::min<size_t>((n16 + 255) / 256, 148 * 16);
+  const int blocks = (int)std::min<size_t>((n16 + 255) / 256, (size_t)sm_count * 16);
   fwd_words_to_native_kernel<<<blocks, 256, 0, st>>>((uint4*)p, n16);
   return cudaGetLastError();
 }
@@ -298,8 +298,8 @@ extern "C" int32_t pb200_init(int32_t device, pb200_ctx** out) {
   PB200_CUDA(cudaGetDeviceProperties(&prop, device));
   ctx->sm_count = prop.multiProcessorCount;
   ctx->max_smem_optin = (int)prop.sharedMemPerBlockOptin;
-  if (prop.major < 9) {
-    set_error("device sm_%d%d: this library is built for sm_100a (TMA bulk copies + mbarrier)", prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0) {  // sm_90a code loads on compute capability 9.0 only
+    set_error("device sm_%d%d: this library is built for sm_90a (TMA bulk copies + mbarrier)", prop.major, prop.minor);
     delete ctx;
     return PB200_E_UNSUPPORTED;
   }
@@ -466,7 +466,7 @@ extern "C" int32_t pb200_segment_register(pb200_ctx* ctx, const char* name, int3
         // dictionary conversion below and the next column's set-up (pageable buffers are staged synchronously by the
         // runtime); the stream is drained once at the end of the registration
         PB200_CUDA(cudaMemcpyAsync(c.fwd, d.fwd, need, cudaMemcpyHostToDevice, up));
-        PB200_CUDA(fwd_words_to_native(c.fwd, c.fwd_alloc_bytes, up));
+        PB200_CUDA(fwd_words_to_native(c.fwd, c.fwd_alloc_bytes, ctx->sm_count, up));
       }
     } else if (d.fwd_kind == PB200_FWD_DICT_SORTED) {
       // SortedIndexReaderImpl: expand (start,end) pairs into a fixed-bit dictId stream so every kernel sees one format
@@ -488,7 +488,7 @@ extern "C" int32_t pb200_segment_register(pb200_ctx* ctx, const char* name, int3
       }
       { void* fp = nullptr; int rc = dev_alloc(ctx, c.fwd_alloc_bytes, &fp); if (rc) return fail(rc); c.fwd = (uint32_t*)fp; }
       PB200_CUDA(cudaMemcpyAsync(c.fwd, packed.data(), c.fwd_alloc_bytes, cudaMemcpyHostToDevice, up));  // pageable source: staged before the call returns
-      PB200_CUDA(fwd_words_to_native(c.fwd, c.fwd_alloc_bytes, up));
+      PB200_CUDA(fwd_words_to_native(c.fwd, c.fwd_alloc_bytes, ctx->sm_count, up));
       c.fwd_kind = PB200_FWD_DICT_FIXEDBIT;
     } else if (d.fwd_kind == PB200_FWD_RAW_FIXEDBYTE) {
       // BaseChunkForwardIndexReader header :60-106; only PASS_THROUGH 4-byte values are accelerated
@@ -508,7 +508,7 @@ extern "C" int32_t pb200_segment_register(pb200_ctx* ctx, const char* name, int3
       { void* fp = nullptr; int rc = dev_alloc(ctx, c.fwd_alloc_bytes, &fp); if (rc) return fail(rc); c.fwd = (uint32_t*)fp; }
       PB200_CUDA(cudaMemsetAsync(c.fwd, 0, c.fwd_alloc_bytes, up));
       PB200_CUDA(cudaMemcpyAsync(c.fwd, p + start, 4ull * num_docs, cudaMemcpyHostToDevice, up));
-      PB200_CUDA(fwd_words_to_native(c.fwd, c.fwd_alloc_bytes, up));
+      PB200_CUDA(fwd_words_to_native(c.fwd, c.fwd_alloc_bytes, ctx->sm_count, up));
     } else {
       set_error("column %d: unknown forward index kind %d", i, d.fwd_kind);
       return fail(PB200_E_INVALID);
@@ -881,7 +881,7 @@ static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment*
   // CTA tile = W warps x 1024 rows; every warp streams its own 1024-row slices through a private TMA ring.
   // W = 6 (aggregation only): 192-thread CTAs, two per SM, 168 registers, no spills (32 of them hold the software-pipelined
   // dictionary gathers).  Group-by: the survivor-queue path needs ~120 registers; W = 6 with two CTAs per SM leaves room
-  // for a 3-deep ring (measured on C3/range: 2.26 ms vs 2.95 ms at W = 8); falls back to one CTA when the rows are too wide
+  // for a 3-deep ring (faster than W = 8 on C3/range); falls back to one CTA when the rows are too wide
   // for two 2-deep rings.
   const Tuning tune = [&]() { std::lock_guard<std::mutex> g(ctx->mu); return ctx->tune; }();
   int cw = tune.warps, stages = 0, ctas_per_sm = 1;
@@ -896,8 +896,7 @@ static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment*
   for (int a = 0; a < kMaxAggs; a++) q.smem_slot[a] = -1;
   if (plan.group_by && tune.smem_groups) {
     // Small key spaces only: there the global table's few addresses serialise in L2, while for thousands of groups the
-    // fire-and-forget global REDs beat shared atomics that must return the old low word (measured on C3/range, 10 000
-    // groups: 3.6 ms global vs 4.4 ms shared).
+    // fire-and-forget global REDs beat shared atomics that must return the old low word.
     const long long smem_groups_max = tune.smem_groups_max;
     long long gmax = 1;
     for (int s = 0; s < nseg && gmax > 0; s++) {
@@ -1283,7 +1282,7 @@ static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment*
       } else {
         groups = (long long)space;
         // Small dense tables are SPREAD: entry of raw key k sits at k * stride.  A 10 000-group table is 80 KB = 312 of the
-        // 256-byte chunks the L2 address hash distributes over ~184 slices -- some slices own three chunks, some none, and
+        // 256-byte chunks the L2 address hash distributes over the L2 slices -- some slices own three chunks, some none, and
         // every surviving row sends a reduction to them (ncu: hottest slice 75 % tag-request utilisation vs 56 % average).
         // With one entry per 128 bytes the same reductions spread over >= 4096 chunks.  Costs table bytes (<= 2 MB each,
         // memset + extraction scan), no instruction in the kernel: the stride is folded into the key multipliers.
@@ -1490,7 +1489,7 @@ static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment*
     for (int r = 0; r < nres; r++) {
       const pb200_result::Dense& d = res[r]->dense;
       if (d.pack_agg < 0) continue;
-      const int vb = (int)std::max<long long>(1, std::min<long long>((d.groups + 1023) / 1024, 148 * 4));
+      const int vb = (int)std::max<long long>(1, std::min<long long>((d.groups + 1023) / 1024, (long long)ctx->sm_count * 4));
       carrier_verify_kernel<<<vb, 256, 0, st>>>((const unsigned long long*)d.isum[d.pack_agg], d.groups, d.pack_shift, dev_verify + 4 * r);
     }
   PB200_CUDA(cudaMemcpyAsync(pin_back, accum_buf.p, acc_bytes, cudaMemcpyDeviceToHost, st));

@@ -309,7 +309,7 @@ extern "C" int32_t pb200_segment_bind_domain(pb200_ctx* ctx, pb200_segment* seg,
       cudaError_t e = cudaMemcpyAsync(remap_dev, w.remap.data(), w.remap.size() * 4, cudaMemcpyHostToDevice, st);
       if (e == cudaSuccess) e = cudaMemsetAsync(nf, 0, nbytes, st);
       if (e == cudaSuccess && groups > 0) {
-        const int blocks = (int)std::min<long long>((groups + 255) / 256, 148 * 16);
+        const int blocks = (int)std::min<long long>((groups + 255) / 256, (long long)ctx->sm_count * 16);
         reencode_kernel<<<blocks, 256, 0, st>>>(c.fwd, c.bits, (uint32_t*)nf, dc.bits, (const uint32_t*)remap_dev,
                                                 (uint32_t)c.cardinality, seg->num_docs, groups);
         e = cudaGetLastError();

@@ -13,8 +13,8 @@
 //           -- no host conversion loop; accessors read (or hand out) columns of that pinned block.
 // Small results (worst case <= kSpeculativeBytes) do all three launches back to back, write STRAIGHT into the mapped
 // pinned block and synchronise ONCE.  Larger ones read the group counts first, size the block exactly, compact into a
-// device staging buffer and move it with ONE DMA copy: device stores into mapped host memory reach ~5 GB/s (measured:
-// 1 M groups x 48 B in 9.2 ms, 100 000 groups in 0.77 ms), the copy engine ~50 GB/s.
+// device staging buffer and move it with ONE DMA copy: device stores into mapped host memory are far slower than the
+// copy engine.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -314,7 +314,7 @@ int extract_groups(pb200_ctx* ctx, pb200_result* const* Rs, int nres, cudaStream
       if (rows) {
         DevBufRaw g(ctx);
         if ((rc = g.alloc(rows * wpg * 4))) return rc;
-        const int gb2 = (int)std::max<size_t>(1, std::min<size_t>((rows * wpg + 255) / 256, 148 * 8));
+        const int gb2 = (int)std::max<size_t>(1, std::min<size_t>((rows * wpg + 255) / 256, (size_t)ctx->sm_count * 8));
         gather_bitset_rows_kernel<<<gb2, 256, 0, st>>>(d.dbits[a], reinterpret_cast<const uint32_t*>(out + e.off_idx), (long long)rows, (int)wpg, (uint32_t*)g.p);
         PB200_CUDA(cudaMemcpyAsync(bits.data(), g.p, rows * wpg * 4, cudaMemcpyDeviceToHost, st));
         PB200_CUDA(cudaStreamSynchronize(st));

@@ -208,7 +208,7 @@ __device__ __forceinline__ void smem_add64(uint32_t* lo, uint32_t* hi, uint32_t 
 // dictId range predicate -> 32-bit row mask.
 // Mask building through the carry flag: compare = one subtract whose carry-out lands in CC.CF, and `addc m, m, m`
 // shifts it into the mask (m = 2m + CF) -- 2 instructions per value (IADD3 + IMAD.X, the second one on the FMA pipe)
-// instead of ISETP + SEL + OR.  After `sub.cc.u32 t, a, b` ptxas / sm_100a leave CF = 1 iff there was NO borrow, i.e.
+// instead of ISETP + SEL + OR.  After `sub.cc.u32 t, a, b` ptxas / sm_90a leave CF = 1 iff there was NO borrow, i.e.
 // a >= b (the hardware carry of a + ~b + 1; measured by tests/workloads/cc_probe and guarded by every parity test).
 // Four chains of 8 values (rows 8k .. 8k+7 in chain k, first row in the chain's highest bit) keep the adds independent;
 // the chains are concatenated and bit-reversed once per leaf.

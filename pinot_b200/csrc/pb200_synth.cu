@@ -143,7 +143,7 @@ int synth_build_inverted(pb200_ctx* ctx, cudaStream_t st, DeviceColumn& col, lon
   uint32_t* dcounts = nullptr;
   PB200_CUDA(cudaMalloc(&dcounts, (size_t)card * nchunks * 4));
   PB200_CUDA(cudaMemsetAsync(dcounts, 0, (size_t)card * nchunks * 4, st));
-  inv_count_kernel<<<148 * 8, 256, 0, st>>>(col.fwd, col.bits, num_docs, nchunks, dcounts);
+  inv_count_kernel<<<ctx->sm_count * 8, 256, 0, st>>>(col.fwd, col.bits, num_docs, nchunks, dcounts);
   std::vector<uint32_t> counts((size_t)card * nchunks);
   PB200_CUDA(cudaMemcpyAsync(counts.data(), dcounts, counts.size() * 4, cudaMemcpyDeviceToHost, st));
   PB200_CUDA(cudaStreamSynchronize(st));
@@ -189,7 +189,7 @@ int synth_build_inverted(pb200_ctx* ctx, cudaStream_t st, DeviceColumn& col, lon
   if (!jobs.empty()) {
     PB200_CUDA(cudaMalloc(&djobs, jobs.size() * sizeof(ContainerJob)));
     PB200_CUDA(cudaMemcpyAsync(djobs, jobs.data(), jobs.size() * sizeof(ContainerJob), cudaMemcpyHostToDevice, st));
-    int grid = (int)std::min<size_t>(jobs.size(), 148 * 16);
+    int grid = (int)std::min<size_t>(jobs.size(), (size_t)ctx->sm_count * 16);
     inv_fill_kernel<<<grid, 256, 0, st>>>(col.fwd, col.bits, num_docs, djobs, (long long)jobs.size(), col.inv);
     PB200_CUDA(cudaGetLastError());
   }
@@ -227,7 +227,7 @@ extern "C" int32_t pb200_synth_segment(pb200_ctx* ctx, const char* name, int32_t
     if (e != cudaSuccess) { set_error("cudaMalloc(%llu) failed: %s", (unsigned long long)alloc, cudaGetErrorString(e)); cleanup(false); cudaGetLastError(); return PB200_E_NOMEM; }
     fwds.push_back(fwd);
     long long groups = tiles * (kMaxTileRows / 32);
-    synth_fwd_kernel<<<148 * 8, 256, 0, st>>>(fwd, groups, num_docs, bits, (uint32_t)sc.cardinality, sc.seed);
+    synth_fwd_kernel<<<ctx->sm_count * 8, 256, 0, st>>>(fwd, groups, num_docs, bits, (uint32_t)sc.cardinality, sc.seed);
     cudaMemsetAsync((unsigned char*)fwd + (alloc - 64), 0, 64, st);
     unsigned char* dict = nullptr;
     e = cudaMalloc(&dict, 4ull * sc.cardinality);

@@ -9,7 +9,7 @@
 // (little-endian) byte order -- the byte swap of the big-endian file words is done ONCE when the segment is uploaded
 // (fwd_words_to_native in pb200_api.cu) instead of once per value group per query (a PRMT per word otherwise).
 //
-// B200 mapping: ONE THREAD owns one such group (32 rows).  Its B words sit contiguously in shared memory (the tile was
+// GPU mapping: ONE THREAD owns one such group (32 rows).  Its B words sit contiguously in shared memory (the tile was
 // brought in by a TMA bulk copy, so the layout is the HBM layout); lane l of a warp reads words
 // [l*B, (l+1)*B).  With the widest naturally aligned load (LDS.128 when B%4==0, LDS.64 when B%2==0, else LDS.32) the
 // lane stride is an odd multiple of the access width for every B except 8, 16 and 24, i.e. bank-conflict free; all

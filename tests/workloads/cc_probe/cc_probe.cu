@@ -1,4 +1,4 @@
-// probe: `sub.cc.u32 t,a,b; addc.u32 m,m,m` yields m = 2m + (a >= b) on sm_100a (CF = hardware carry = no borrow)
+// probe: `sub.cc.u32 t,a,b; addc.u32 m,m,m` yields m = 2m + (a >= b) on sm_90a (CF = hardware carry = no borrow)
 #include <cstdint>
 #include <cstdio>
 #include <vector>
