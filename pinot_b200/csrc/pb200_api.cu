@@ -880,23 +880,78 @@ static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment*
   const size_t hdr_bytes = (sizeof(SmemHeader) + 127) / 128 * 128;
   // CTA tile = W warps x 1024 rows; every warp streams its own 1024-row slices through a private TMA ring.
   // W = 6 (aggregation only): 192-thread CTAs, two per SM, 168 registers, no spills (32 of them hold the software-pipelined
-  // dictionary gathers).  Group-by: the survivor-queue path needs ~120 registers; W = 6 with two CTAs per SM leaves room
-  // for a 3-deep ring (faster than W = 8 on C3/range); falls back to one CTA when the rows are too wide
-  // for two 2-deep rings.
+  // dictionary gathers).  Group-by: the survivor-queue path needs 144-145 registers (ptxas, sm_90a); W = 6 with two CTAs per
+  // SM leaves room for a 3-deep ring (faster than W = 8 on C3/range); falls back to one CTA when the rows are too wide
+  // for two 2-deep rings, or when a shared-memory group table needs the room (below).
   const Tuning tune = [&]() { std::lock_guard<std::mutex> g(ctx->mu); return ctx->tune; }();
   int cw = tune.warps, stages = 0, ctas_per_sm = 1;
   q.sparse_max = tune.sparse_max;
   q.sparse_max_agg = tune.sparse_max_agg >= 0 ? tune.sparse_max_agg : (plan.group_by ? std::min(q.sparse_max, 2) : q.sparse_max);
   ctas_per_sm = tune.ctas_per_sm;  // default 2: the group-by kernel needs < 168 registers, two 192-thread CTAs per SM
   const size_t warp_stage_bytes = (size_t)128 * max_bits_sum;
-  size_t extra_bytes = (q.conj ? 0 : (size_t)cw * 32 * kMaxStack * 4) + (plan.group_by ? (size_t)cw * 2048 : (size_t)nagg * cw * 32 * 16);
+  auto extra_for = [&](int w) { return (q.conj ? 0 : (size_t)w * 32 * kMaxStack * 4) + (plan.group_by ? (size_t)w * 2048 : (size_t)nagg * w * 32 * 16); };
+  size_t extra_bytes = extra_for(cw);
   q.queue_max = plan.group_by ? 1024 : 0;  // every group-by slice goes through the survivor queue
-  // CTA-private group tables in shared memory when the key space is small and every function is COUNT or an integer SUM
+
+  // ---- count carrier.  Every RED into the global tables is an L2 read-modify-write, and on this path the L2 request
+  // rate is the bound.  When the query needs the per-group row count (COUNT / AVG, or only as the group-exists marker)
+  // and sums an INT dictionary column, the count rides in the upper bits of that sum: each row adds
+  // (value - vmin) + 2^shift with ONE reduction (or, in a shared-memory table, one 8-byte entry instead of 12).
+  //   Fields: sum field = `shift` bits, count field = 64 - shift bits, balanced so that both overflow at about the
+  //   same rows per group: shift = ceil((64 + bits(R)) / 2), R = vmax - vmin + 1 from the dictionary (a 20-bit value
+  //   range leaves 22 bits = 4 M rows per group; a full 32-bit range 65 535).
+  //   Either field CAN overflow; both are detected EXACTLY after the launch from one number: a sum field overflow
+  //   carries into the count field (counts only grow: value - vmin >= 0), a count overflow drops 2^(64-shift) from
+  //   it, so  sum_g count_g == matched docs  iff neither happened -- the two cannot cancel because the carries total
+  //   at most docs x R / 2^shift < 2^(64-shift) when docs x R < 2^64 (the admission test below).  On a mismatch the
+  //   submission runs again with a separate COUNT table (kRetryWithoutCountCarrier); results are exact either way.
+  // Decided per result (r) here, before the shared-memory table is sized; the result tables below apply it.
+  struct Carrier { int agg = -1; int shift = 0; long long vmin = 0; };
+  auto count_carrier = [&](int r) -> Carrier {
+    Carrier cr;
+    if (!plan.group_by || !allow_count_carrier || (query->flags & PB200_Q_NO_COUNT_CARRIER) || !tune.pack_count) return cr;
+    const bool deferred = merge && (query->flags & PB200_Q_DEFER_FINALIZE);
+    const int reduce_world = deferred ? std::max(query->reduce_world, 1) : 1;
+    unsigned long long docs = 0;
+    for (int s = 0; s < nseg; s++) if (merge || s == r) docs += (unsigned long long)segments[s]->num_docs;
+    // a table that will be summed with the other GPUs' tables: the admission test covers the docs of ALL of them
+    if (deferred) docs = query->merged_docs_bound > 0 ? (unsigned long long)query->merged_docs_bound : docs * (unsigned long long)reduce_world;
+    auto bits_of = [](unsigned long long x) { int b = 0; while (b < 64 && (x >> b)) b++; return b; };
+    for (int a = 0; a < nagg; a++) {
+      const int fn = q.aggs[a].function;
+      if ((fn != PB200_AGG_SUM && fn != PB200_AGG_AVG) || q.aggs[a].val_kind != VAL_DICT_I32) continue;
+      long long vmin = std::numeric_limits<long long>::max(), vmax = std::numeric_limits<long long>::min();
+      bool ok = true;
+      for (int s = 0; s < nseg && ok; s++) {
+        if (!merge && s != r) continue;
+        const DeviceColumn& c = segments[s]->cols[query->aggs[a].column];
+        if (c.dict_host.size() < 4ull * std::max(c.cardinality, 1) || c.stored_type != PB200_INT) { ok = false; break; }
+        // the other GPUs must subtract the SAME minimum: only a table-wide (domain) dictionary guarantees that
+        if (reduce_world > 1 && !c.dict_shared) { ok = false; break; }
+        int32_t v0, v1;   // sorted dictionary: first / last entry
+        memcpy(&v0, c.dict_host.data(), 4);
+        memcpy(&v1, c.dict_host.data() + 4ull * (c.cardinality - 1), 4);
+        vmin = std::min<long long>(vmin, v0);
+        vmax = std::max<long long>(vmax, v1);
+      }
+      if (!ok) continue;
+      const int rbits = bits_of((unsigned long long)(vmax - vmin));   // value - vmin fits rbits bits
+      if (bits_of(docs) + rbits > 63) continue;                        // docs x R < 2^63: the detection is airtight
+      cr.agg = a;
+      cr.shift = tune.pack_shift > 0 ? tune.pack_shift : (64 + rbits + 1) / 2;
+      cr.vmin = vmin;
+      break;
+    }
+    return cr;
+  };
+
+  // CTA-private group tables in shared memory when the key space fits next to a 2-deep ring and every function is
+  // COUNT or an integer SUM.  A survivor then costs shared atomics instead of a global RED.  Measured on H100 with
+  // 10 000 groups (DESIGN.md section 3.1): one 8-warp CTA per SM with the table and the pipelined last batch runs the
+  // headline scan in 1.83 ms, two 6-warp CTAs with the global table in 2.11.
   q.smem_groups = 0;
   for (int a = 0; a < kMaxAggs; a++) q.smem_slot[a] = -1;
   if (plan.group_by && tune.smem_groups) {
-    // Small key spaces only: there the global table's few addresses serialise in L2, while for thousands of groups the
-    // fire-and-forget global REDs beat shared atomics that must return the old low word.
     const long long smem_groups_max = tune.smem_groups_max;
     long long gmax = 1;
     for (int s = 0; s < nseg && gmax > 0; s++) {
@@ -913,17 +968,32 @@ static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment*
       if ((fn == PB200_AGG_SUM || fn == PB200_AGG_AVG) && (vk == VAL_DICT_I32 || vk == VAL_RAW_I32)) q.smem_slot[a] = (int8_t)nsum++;
       else ok = false;
     }
+    // no count array when every result of the launch carries its counts in a sum
+    bool all_carry = ok;
+    for (int r = 0; r < (merge ? 1 : nseg) && all_carry; r++) all_carry = count_carrier(r).agg >= 0;
+    q.smem_count = all_carry ? 0 : 1;
     const long long gstride = gmax | 1;
-    const size_t copy_bytes = ok ? (size_t)gstride * 4 * (1 + 2 * nsum) : 0;
-    // room left after a 2-deep ring; the table may take at most 64 KB of it
-    const long long room = (long long)ctx->max_smem_optin / ctas_per_sm - (long long)hdr_bytes - (long long)extra_bytes - 1024 - 256 - (long long)(2 * warp_stage_bytes * cw);
-    if (ok && room >= (long long)copy_bytes) {
+    const size_t copy_bytes = ok ? (size_t)gstride * 4 * (q.smem_count + 2 * nsum) : 0;
+    // room left after a 2-deep ring
+    auto room_for = [&](int w, int ctas) {
+      return (long long)ctx->max_smem_optin / ctas - (long long)hdr_bytes - (long long)extra_for(w) - 1024 - 256 - (long long)(2 * warp_stage_bytes * w);
+    };
+    bool fits = ok && room_for(cw, ctas_per_sm) >= (long long)copy_bytes;
+    if (ok && !fits && room_for(8, 1) >= (long long)copy_bytes) {
+      // a table too large for the configured CTA: one CTA of 8 warps per SM.  With 6 warps the CTA hides too little
+      // latency (10 000 groups on H100: 2.20 ms against 2.11 for the global table at 2 CTAs/SM; 8 warps: 1.83).
+      cw = 8; ctas_per_sm = 1; extra_bytes = extra_for(8); fits = true;
+    }
+    if (fits) {
+      // replicated copies (fewer same-address conflicts) for small key spaces: they may take at most 64 KB
+      const long long room = room_for(cw, ctas_per_sm);
       int copies = 1;
       while (copies < 32 && (long long)copy_bytes * copies * 2 <= std::min<long long>(room, 64 << 10)) copies *= 2;
       if (tune.smem_copies > 0) copies = std::max(1, std::min(copies, tune.smem_copies));
       q.smem_groups = (int32_t)gmax;
       q.smem_copies = copies;
       q.smem_gstride = (int32_t)gstride;
+      q.smem_merged = merge ? 1 : 0;
       extra_bytes += copy_bytes * copies;
     } else {
       for (int a = 0; a < kMaxAggs; a++) q.smem_slot[a] = -1;
@@ -1150,13 +1220,13 @@ static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment*
       lf.code = leaf_code(lf.kind, lf.cmp, lf.negate, has_slot ? sd.slots[lf.slot].bits : 0, has_slot ? sd.slots[lf.slot].stage_words : 0u);
     }
     // software-pipelined aggregations go LAST (nothing is waited on after them).  Aggregation only: q.defer_agg.
-    // Group-by (dense / hash tables, not the CTA-private shared tables): up to two of {SUM / AVG over a 4-byte
-    // dictionary, MIN, MAX} -- the kernel issues their loads for the last queue batch and reduces one tile later.
+    // Group-by: up to two of {SUM / AVG over a 4-byte dictionary, MIN, MAX} -- the kernel issues their loads for the
+    // last queue batch and reduces one tile later (into the global table, or the CTA's shared table: integer sums only).
     bool pipelined[kMaxAggs] = {};
     int npipe = 0;
     if (!plan.group_by) {
       if (q.defer_agg >= 0) pipelined[q.defer_agg] = true;
-    } else if (tune.gb_defer && q.smem_groups == 0) {
+    } else if (tune.gb_defer) {
       for (int a = 0; a < nagg && npipe < 2; a++) {
         if (q.aggs[a].slot < 0) continue;
         const int fn = q.aggs[a].function, vk = q.aggs[a].val_kind;
@@ -1311,54 +1381,19 @@ static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment*
         has_minmax |= q.aggs[a].function == PB200_AGG_MIN || q.aggs[a].function == PB200_AGG_MAX;
       }
       bool need_seen = !need_count && !has_minmax && !hashed;  // a hash table's keys mark the groups that exist
-      // ---- count carrier.  Every RED into the tables is an L2 read-modify-write, and on this path the L2 sector rate is
-      // the bound (lts__t_sectors ~ 3.7x the streamed bytes at 10 % selectivity, profiles/r2_*).  When the query needs the
-      // per-group row count (COUNT / AVG, or only as the group-exists marker) and sums an INT dictionary column, the
-      // count rides in the upper bits of that sum: each row adds (value - vmin) + 2^shift with ONE reduction.
-      //   Fields: sum field = `shift` bits, count field = 64 - shift bits, balanced so that both overflow at about the
-      //   same rows per group: shift = ceil((64 + bits(R)) / 2), R = vmax - vmin + 1 from the dictionary (a 20-bit value
-      //   range leaves 22 bits = 4 M rows per group; a full 32-bit range 65 535).
-      //   Either field CAN overflow; both are detected EXACTLY after the launch from one number: a sum field overflow
-      //   carries into the count field (counts only grow: value - vmin >= 0), a count overflow drops 2^(64-shift) from
-      //   it, so  sum_g count_g == matched docs  iff neither happened -- the two cannot cancel because the carries total
-      //   at most docs x R / 2^shift < 2^(64-shift) when docs x R < 2^64 (the admission test below).  On a mismatch the
-      //   submission runs again with a separate COUNT table (kRetryWithoutCountCarrier); results are exact either way.
+      // ---- count carrier (see count_carrier above) ----
       d.pack_agg = -1;
       const bool deferred = merge && (query->flags & PB200_Q_DEFER_FINALIZE);
       d.reduce_world = deferred ? std::max(query->reduce_world, 1) : 1;
-      if (allow_count_carrier && !(query->flags & PB200_Q_NO_COUNT_CARRIER) && tune.pack_count && q.smem_groups == 0 &&
-          (need_count || need_seen)) {
-        unsigned long long docs = 0;
-        for (int s = 0; s < nseg; s++) if (merge || s == r) docs += (unsigned long long)segments[s]->num_docs;
-        // a table that will be summed with the other GPUs' tables: the admission test covers the docs of ALL of them
-        if (deferred) docs = query->merged_docs_bound > 0 ? (unsigned long long)query->merged_docs_bound : docs * (unsigned long long)d.reduce_world;
-        auto bits_of = [](unsigned long long x) { int b = 0; while (b < 64 && (x >> b)) b++; return b; };
-        for (int a = 0; a < nagg && d.pack_agg < 0; a++) {
-          const int fn = q.aggs[a].function;
-          if ((fn != PB200_AGG_SUM && fn != PB200_AGG_AVG) || q.aggs[a].val_kind != VAL_DICT_I32) continue;
-          long long vmin = std::numeric_limits<long long>::max(), vmax = std::numeric_limits<long long>::min();
-          bool ok = true;
-          for (int s = 0; s < nseg && ok; s++) {
-            if (!merge && s != r) continue;
-            const DeviceColumn& c = segments[s]->cols[query->aggs[a].column];
-            if (c.dict_host.size() < 4ull * std::max(c.cardinality, 1) || c.stored_type != PB200_INT) { ok = false; break; }
-            // the other GPUs must subtract the SAME minimum: only a table-wide (domain) dictionary guarantees that
-            if (d.reduce_world > 1 && !c.dict_shared) { ok = false; break; }
-            int32_t v0, v1;   // sorted dictionary: first / last entry
-            memcpy(&v0, c.dict_host.data(), 4);
-            memcpy(&v1, c.dict_host.data() + 4ull * (c.cardinality - 1), 4);
-            vmin = std::min<long long>(vmin, v0);
-            vmax = std::max<long long>(vmax, v1);
-          }
-          if (!ok) continue;
-          const int rbits = bits_of((unsigned long long)(vmax - vmin));   // value - vmin fits rbits bits
-          if (bits_of(docs) + rbits > 63) continue;                        // docs x R < 2^63: the detection is airtight
-          d.pack_agg = a;
-          d.pack_shift = tune.pack_shift > 0 ? tune.pack_shift : (64 + rbits + 1) / 2;
-          d.pack_vmin = vmin;
+      if (need_count || need_seen) {
+        const Carrier cr = count_carrier(r);
+        if (cr.agg >= 0) {
+          d.pack_agg = cr.agg; d.pack_shift = cr.shift; d.pack_vmin = cr.vmin;
+          need_count = false; need_seen = false;
         }
-        if (d.pack_agg >= 0) { need_count = false; need_seen = false; }
       }
+      // a shared-memory table without a count array relies on every result carrying its counts
+      if (q.smem_groups && !q.smem_count && d.pack_agg < 0) { set_error("internal: shared-memory group table has no count array"); return PB200_E_INVALID; }
       long long n_i64 = need_count ? 1 : 0, n_f64 = 0, n_max = need_seen ? 1 : 0, n_min = 0;
       for (int a = 0; a < nagg; a++) {
         const int fn = q.aggs[a].function, vk = q.aggs[a].val_kind;

@@ -165,7 +165,9 @@ struct QueryDesc {
   int32_t total_tiles;     // CTA tiles in this launch
   // CTA-private group table in shared memory (group-by with a small key space and COUNT / integer SUM only): rows
   // update it with native 32-bit shared atomics and it is merged into the global dense table once per segment.
-  // Layout at byte offset smem_table_off: count u32[G], then per summed aggregation lo u32[G], hi u32[G].
+  // Layout at byte offset smem_table_off: count u32[G] (when smem_count), then per summed aggregation lo u32[G],
+  // hi u32[G].  A sum that carries its group's row count (SegDesc.sum_addend) needs no count array: with the carrier
+  // admitted for every result of the launch an entry is 8 bytes, and the flushed table equals what global REDs build.
   int32_t smem_groups;     // 0 = off, else the size G of the dense key space (max over the launch's segments)
   uint32_t smem_table_off;
   // the table is replicated `smem_copies` (power of two) times, lane l updates copy l % copies: same-address conflicts
@@ -177,7 +179,8 @@ struct QueryDesc {
   uint32_t queue_off;
   int32_t queue_max;
   int8_t smem_slot[kMaxAggs];  // aggregation -> index of its (lo, hi) pair, -1: none (COUNT)
-  int8_t pad_tail[2];
+  int8_t smem_count;           // 1: the shared table has a count array
+  int8_t smem_merged;          // 1: every segment of the launch adds into the same global table (flush at exit only)
   int32_t reserved_tail[2];
 };
 

@@ -61,7 +61,7 @@ struct Tuning {
   int stages = 0;                // PB200_STAGES (0: as many as fit)
   int grid = 0;                  // PB200_GRID (0: SMs x CTAs per SM)
   int smem_groups = 1;           // !PB200_NO_SMEM_GROUPS
-  long long smem_groups_max = 2048;  // PB200_SMEM_GROUPS_MAX
+  long long smem_groups_max = 1ll << 24;  // PB200_SMEM_GROUPS_MAX: cap on top of the shared-memory budget (default: none)
   int smem_copies = 0;           // PB200_SMEM_COPIES (0: as many as fit)
   long long dense_max = 1ll << 24;   // PB200_DENSE_MAX: dense group table up to this many raw keys, hash table beyond
   int defer = 1;                 // !PB200_NO_DEFER: software-pipelined gathers, aggregation-only kernel

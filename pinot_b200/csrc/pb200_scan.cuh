@@ -192,14 +192,15 @@ __device__ __forceinline__ bool hash_slot(const SegDesc& sd, unsigned long long 
   return false;
 }
 
-// 64-bit signed accumulate into a CTA-private shared-memory table kept as two u32 words: shared 64-bit atomic adds
-// compile to a CAS spin loop (ATOMS.CAST.SPIN.64) while 32-bit ones are native, and the high word only moves on a
-// carry or a negative addend.
-__device__ __forceinline__ void smem_add64(uint32_t* lo, uint32_t* hi, uint32_t g, int x) {
+// 64-bit accumulate (modulo 2^64, like the global table's red.add.u64) into a CTA-private shared-memory table kept as
+// two u32 words: shared 64-bit atomic adds compile to a CAS spin loop (ATOMS.CAST.SPIN.64) while 32-bit ones are
+// native.  The high word gets the addend's high word plus the carry out of the low word; for a plain 32-bit value that
+// is nonzero only on a carry or a negative addend, for a count-carrying addend (2^shift + ...) on every row.
+__device__ __forceinline__ void smem_add64(uint32_t* lo, uint32_t* hi, uint32_t g, unsigned long long x) {
   const uint32_t xl = (uint32_t)x;
   const uint32_t old = atomicAdd(lo + g, xl);
-  const int h = (x >> 31) + ((uint32_t)(old + xl) < xl ? 1 : 0);  // sign extension + carry out of the low word
-  if (h) atomicAdd(hi + g, (uint32_t)h);
+  const uint32_t h = (uint32_t)(x >> 32) + ((uint32_t)(old + xl) < xl ? 1u : 0u);
+  if (h) atomicAdd(hi + g, h);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -287,7 +288,7 @@ struct MinMaxLeft {
 // Shared-memory layout (dynamic):
 //   [SmemHeader][W x num_stages x stage_words][filter stack (generic filters only)]
 //   [acc64: num_aggs x threads x 8 B][accmm: num_aggs x threads x 8 B]                        (aggregation-only kernel)
-//   [survivor queue: W x 1024 u16][group table copies: count, (lo, hi) per sum -- optional]     (group-by kernel)
+//   [survivor queue: W x 1024 u16][group table copies: [count,] (lo, hi) per sum -- optional]   (group-by kernel)
 // acc64/accmm are the per-thread running aggregates; they live in shared memory (private slot per thread, touched once
 // per tile) instead of registers so that two CTAs fit on an SM.
 template <int W, bool GROUPBY, bool DEFER = !GROUPBY, int MINB = (GROUPBY ? 1 : 2)>
@@ -325,7 +326,7 @@ scan_kernel(const __grid_constant__ QueryDesc q, const __grid_constant__ TmaTabl
     int nsl = 0;
 #pragma unroll
     for (int a = 0; a < kMaxAggs; ++a) nsl = max(nsl, (int)q.smem_slot[a] + 1);
-    for (uint32_t i = threadIdx.x; i < TA * (1u + 2u * nsl); i += W * 32) tcnt[i] = 0u;
+    for (uint32_t i = threadIdx.x; i < TA * ((uint32_t)q.smem_count + 2u * nsl); i += W * 32) tcnt[i] = 0u;
   }
   if (threadIdx.x < kMaxAggs) hdr->aggs[threadIdx.x] = q.aggs[threadIdx.x];
   if (threadIdx.x < kMaxSlots) hdr->slot_roles[threadIdx.x] = q.slot_roles[threadIdx.x];
@@ -442,11 +443,18 @@ scan_kernel(const __grid_constant__ QueryDesc q, const __grid_constant__ TmaTabl
               } else {
                 // device INT dictionaries are biased (value + 2^31): the addend removes the bias -- or, when this sum
                 // CARRIES the group's row count (SegDesc.sum_addend), re-bases the value to (value - min) + 2^shift
-                unsigned long long* t = reinterpret_cast<unsigned long long*>(sd.g_isum[a]);
                 const unsigned long long addend = sd.sum_addend[a];
+                if (TG) {
+                  uint32_t* lo = tcnt + tcopy + TA * ((uint32_t)q.smem_count + 2u * q.smem_slot[a]);
 #pragma unroll
-                for (int u = 0; u < kQB; ++u)
-                  if ((pend_ok >> u) & 1u) red_add_u64(t + pg[u], (unsigned long long)px[k][u] + addend);
+                  for (int u = 0; u < kQB; ++u)
+                    if ((pend_ok >> u) & 1u) smem_add64(lo, lo + TA, pg[u], (unsigned long long)px[k][u] + addend);
+                } else {
+                  unsigned long long* t = reinterpret_cast<unsigned long long*>(sd.g_isum[a]);
+#pragma unroll
+                  for (int u = 0; u < kQB; ++u)
+                    if ((pend_ok >> u) & 1u) red_add_u64(t + pg[u], (unsigned long long)px[k][u] + addend);
+                }
               }
             } else if (fn == 2) {
               uint32_t* t = sd.g_min[a];
@@ -502,26 +510,31 @@ scan_kernel(const __grid_constant__ QueryDesc q, const __grid_constant__ TmaTabl
     }
   };
   reset_acc();
-  // merges the CTA-private group table into the segment's dense global table and clears it (whole CTA, between barriers)
+  // merges the CTA-private group table into the segment's dense global table and clears it (whole CTA, between barriers).
+  // Zero entries are skipped: adding 0 changes no global entry, and most groups of a CTA's table are empty when the
+  // key space is large.
   auto table_flush = [&]() {
     for (uint32_t g = threadIdx.x; g < TG; g += W * 32) {
-      uint32_t c = 0;
-      for (int r = 0; r < q.smem_copies; ++r) { c += tcnt[r * q.smem_gstride + g]; tcnt[r * q.smem_gstride + g] = 0u; }
-      if (c == 0u) continue;
-      if (sd.g_count) atomicAdd(sd.g_count + g, (unsigned long long)c);
-      else if (sd.g_seen) sd.g_seen[g] = 1u;
+      if (q.smem_count) {
+        uint32_t c = 0;
+        for (int r = 0; r < q.smem_copies; ++r) { c += tcnt[r * q.smem_gstride + g]; tcnt[r * q.smem_gstride + g] = 0u; }
+        if (c != 0u) {
+          if (sd.g_count) atomicAdd(sd.g_count + g, (unsigned long long)c);
+          else if (sd.g_seen) sd.g_seen[g] = 1u;
+        }
+      }
 #pragma unroll
       for (int a = 0; a < kMaxAggs; ++a) {
         const int k = q.smem_slot[a];
         if (k < 0 || a >= q.num_aggs) continue;
-        uint32_t* lo = tcnt + TA * (1u + 2u * k);
+        uint32_t* lo = tcnt + TA * ((uint32_t)q.smem_count + 2u * k);
         unsigned long long v = 0;
         for (int r = 0; r < q.smem_copies; ++r) {
           const uint32_t i = r * q.smem_gstride + g;
           v += (unsigned long long)lo[i] | (unsigned long long)lo[TA + i] << 32;
           lo[i] = 0u; lo[TA + i] = 0u;
         }
-        atomicAdd(reinterpret_cast<unsigned long long*>(sd.g_isum[a] + g), v);
+        if (v != 0ull) atomicAdd(reinterpret_cast<unsigned long long*>(sd.g_isum[a] + g), v);
       }
     }
   };
@@ -535,7 +548,8 @@ scan_kernel(const __grid_constant__ QueryDesc q, const __grid_constant__ TmaTabl
       while (T >= tt.seg[ns].end_tile) ++ns;
       if (sidx >= 0) flush();
       consumer_bar_sync(kConsumers);  // everyone done reading the old descriptor
-      if (GROUPBY && TG && sidx >= 0) { table_flush(); consumer_bar_sync(kConsumers); }
+      // a merged submission accumulates every segment into the same global table: its CTA table is flushed once, at exit
+      if (GROUPBY && TG && sidx >= 0 && !q.smem_merged) { table_flush(); consumer_bar_sync(kConsumers); }
       const uint32_t* src = reinterpret_cast<const uint32_t*>(segs + ns);
       uint32_t* dstw = reinterpret_cast<uint32_t*>(&hdr->seg);
       for (int i = threadIdx.x; i < (int)(sizeof(SegDesc) / 4); i += kConsumers) dstw[i] = __ldg(src + i);
@@ -757,8 +771,10 @@ scan_kernel(const __grid_constant__ QueryDesc q, const __grid_constant__ TmaTabl
             }
           }
           if (TG) {
+            if (q.smem_count) {
 #pragma unroll
-            for (int u = 0; u < kQB; ++u) if (ok[u]) atomicAdd(tcnt + tcopy + g[u], 1u);
+              for (int u = 0; u < kQB; ++u) if (ok[u]) atomicAdd(tcnt + tcopy + g[u], 1u);
+            }
           } else if (sd.g_count) {
 #pragma unroll
             for (int u = 0; u < kQB; ++u) if (ok[u]) red_add_u64(sd.g_count + g[u], 1ull);
@@ -828,9 +844,9 @@ scan_kernel(const __grid_constant__ QueryDesc q, const __grid_constant__ TmaTabl
                   x[u] = vk == VAL_DICT_I32 ? (long long)((unsigned long long)__ldg(static_cast<const uint32_t*>(sd.dict[a]) + id[u]) + sd.sum_addend[a])
                                             : (long long)(int)id[u];
                 if (TG) {
-                  uint32_t* lo = tcnt + tcopy + TA * (1u + 2u * q.smem_slot[a]);
+                  uint32_t* lo = tcnt + tcopy + TA * ((uint32_t)q.smem_count + 2u * q.smem_slot[a]);
 #pragma unroll
-                  for (int u = 0; u < kQB; ++u) if (ok[u]) smem_add64(lo, lo + TA, g[u], (int)x[u]);
+                  for (int u = 0; u < kQB; ++u) if (ok[u]) smem_add64(lo, lo + TA, g[u], (unsigned long long)x[u]);
                 } else {
                   unsigned long long* gs = reinterpret_cast<unsigned long long*>(sd.g_isum[a]);
 #pragma unroll
