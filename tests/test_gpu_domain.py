@@ -9,6 +9,7 @@ Oracle side: each segment through the CPU oracle with its OWN dictionaries, merg
 import numpy as np
 import pytest
 
+from exact_ref import check_exact
 from gpu_util import assert_tables_equal, oracle_table, to_device
 from pinot_b200 import sql
 from pinot_b200.plan_maker import B200Context, B200PlanMaker, DictionaryDomain, UnsupportedQueryError
@@ -102,6 +103,7 @@ def test_merge_refused_when_dictionaries_differ(oracle, ctx, pm):
         got = pm.execute_segments([da, db], q, merge=True)[0]
         want = combine([x.function for x in q.aggregations], [oracle_table(s, q, oracle.execute(s, q)) for s in (a, b)])
         assert_tables_equal(q, device_table(da, q, got), want, "value-space merge")
+        check_exact(oracle, [a, b], q, device_table(da, q, got), "value-space merge")
     finally:
         da.destroy()
         db.destroy()
@@ -140,6 +142,7 @@ def test_domain_merge_equals_oracle_merge_by_value(oracle, ctx, pm, sizes):
                 assert_tables_equal(q, device_table(d, q, blk), w, "bound, per segment: " + text)
             merged = pm.execute_segments(devs, q, merge=True)[0]
             assert_tables_equal(q, device_table(devs[0], q, merged), combine(fns, want_blocks), "merged by value: " + text)
+            check_exact(oracle, segs, q, device_table(devs[0], q, merged), "merged by value: " + text)
     finally:
         for d in devs:
             d.destroy()

@@ -5,6 +5,7 @@ restatement on the reference's own FilteredAggregationsTest queries)."""
 import numpy as np
 import pytest
 
+from exact_ref import check_exact
 from gpu_util import assert_tables_equal, check_query, gpu_table, oracle_table, to_device
 from pinot_b200 import sql
 from pinot_b200.plan_maker import B200Context, B200PlanMaker
@@ -86,6 +87,7 @@ def test_filtered_aggregations_over_merged_segments(oracle, ctx, pm):
             block = pm.execute_segments(devs, q, merge=True)[0]
             want = combine([a.function for a in q.aggregations], [oracle_table(s, q, oracle.execute(s, q)) for s in segs])
             assert_tables_equal(q, gpu_table(segs[0], q, block, devs[0]), want, "merged: " + text)
+            check_exact(oracle, segs, q, gpu_table(segs[0], q, block, devs[0]), "merged: " + text)
             assert block.stats.num_docs_scanned == sum(oracle.execute(s, q).stats[0] for s in segs), text
     finally:
         for d in devs:

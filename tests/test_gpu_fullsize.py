@@ -13,7 +13,6 @@ import threading
 import numpy as np
 import pytest
 
-from gpu_util import SUM_REL_TOL
 from pinot_b200 import sql
 from pinot_b200.plan_maker import B200Context, B200PlanMaker, IndexSegment
 
@@ -22,6 +21,10 @@ pytestmark = pytest.mark.gpu
 ROWS = 100_000_000
 COLS = [("d1", 10, True), ("d2", 20, True), ("d3", 50, True), ("g", 10_000, False), ("m", 100_000, False),
         ("f", 10_000, False), ("g2", 100, False), ("h", 1_000_000, False)]
+
+
+def _max_abs_value(spec):
+    return max(abs(spec["value_base"]), abs(spec["value_base"] + spec["value_step"] * (spec["cardinality"] - 1)))
 
 
 def specs(seed0):
@@ -121,6 +124,11 @@ FULL_QUERIES = [
 def test_full_size_segment_equals_oracle(oracle, ctx, big, name, text):
     dev, host, parts = big
     q = sql.parse(text, num_groups_limit=2_000_000)
+    # every partial sum of the oracle's Java-order double is an integer below rows x max|value| < 2^53, so it is exact:
+    # the device's integer sums must equal it bit for bit
+    for agg in q.aggregations:
+        if agg.function in ("SUM", "AVG"):
+            assert ROWS * _max_abs_value(next(s for s in specs(0) if s["name"] == agg.column)) < 2 ** 53, agg.column
     want, want_docs = oracle_tables(oracle, parts, q)
     block = B200PlanMaker(ctx).make_segment_plan_node(dev, q).run().next_block()
     got = device_table(block, q)
@@ -129,12 +137,8 @@ def test_full_size_segment_equals_oracle(oracle, ctx, big, name, text):
     for key, wv in want.items():
         gv = got[key]
         for a, agg in enumerate(q.aggregations):
-            if agg.function == "SUM":
-                assert gv[a] == wv[a] or abs(gv[a] - wv[a]) <= SUM_REL_TOL * abs(wv[a]), (name, key, gv[a], wv[a])
-            elif agg.function == "AVG":
-                assert gv[a][1] == wv[a][1] and abs(gv[a][0] - wv[a][0]) <= SUM_REL_TOL * abs(wv[a][0]), (name, key)
-            else:   # COUNT / MIN / MAX: bit exact
-                assert gv[a] == wv[a], (name, key, agg.function, gv[a], wv[a])
+            # SUM, AVG (sum and count), COUNT, MIN, MAX: bit exact
+            assert gv[a] == wv[a], (name, key, agg.function, gv[a], wv[a])
 
 
 def test_full_size_generators_agree(oracle, big):

@@ -3,6 +3,7 @@ import numpy as np
 import pytest
 
 import golden_cases as G
+from exact_ref import check_exact
 from gpu_util import assert_tables_equal, check_query, gpu_table, oracle_table, to_device
 from pinot_b200 import sql
 from pinot_b200.plan_maker import B200Context, B200PlanMaker, IndexSegment, UnsupportedQueryError
@@ -233,9 +234,11 @@ def test_multi_segment_single_submission_and_device_merge(oracle, ctx, pm):
             blocks = pm.execute_segments(devs, q)
             for s, b, w in zip(segs, blocks, want_blocks):
                 assert_tables_equal(q, gpu_table(s, q, b), w, text)
+                check_exact(oracle, [s], q, gpu_table(s, q, b), text)
             merged = pm.execute_segments(devs, q, merge=True)
             assert len(merged) == 1
             assert_tables_equal(q, gpu_table(segs[0], q, merged[0]), combine(fns, want_blocks), "merged " + text)
+            check_exact(oracle, segs, q, gpu_table(segs[0], q, merged[0]), "merged " + text)
             if q.is_group_by:
                 # deferred extraction (what a cross-GPU reduce of the dense tables sits between): tables first, groups later
                 from pinot_b200 import _lib
@@ -273,6 +276,7 @@ def test_more_segments_than_one_launch_holds(oracle, ctx, pm):
             merged = gpu_table(seg, q, pm.execute_segments([dev] * k, q, merge=True)[0])
             fns = [a.function for a in q.aggregations]
             assert_tables_equal(q, merged, combine(fns, [want] * k), "merged x37 " + text)
+            check_exact(oracle, [seg] * k, q, merged, "merged x37 " + text)
     finally:
         dev.destroy()
 

@@ -11,6 +11,7 @@ import os
 import numpy as np
 import pytest
 
+from exact_ref import check_exact
 from gpu_util import assert_tables_equal, check_query, gpu_table, oracle_table, to_device
 from pinot_b200 import sql
 from pinot_b200.plan_maker import B200Context, B200PlanMaker, IndexSegment
@@ -103,6 +104,7 @@ def test_raw_group_by_merged_over_segments_by_value(oracle, ctx, pm):
         block = pm.execute_segments(devs, q, merge=True)[0]
         want = combine([a.function for a in q.aggregations], [oracle_table(s, q, oracle.execute(s, q)) for s in segs])
         assert_tables_equal(q, gpu_table(segs[0], q, block, devs[0]), want, "merged raw group-by")
+        check_exact(oracle, segs, q, gpu_table(segs[0], q, block, devs[0]), "merged raw group-by")
     finally:
         for d in devs:
             d.destroy()

@@ -4,6 +4,7 @@ route forced through pb200_tuning_set("smem_groups", 0)."""
 import numpy as np
 import pytest
 
+from exact_ref import check_exact
 from gpu_util import assert_tables_equal, check_query, gpu_table, oracle_table, to_device
 from pinot_b200 import sql
 from pinot_b200.plan_maker import B200Context, B200PlanMaker
@@ -85,6 +86,7 @@ def test_10000_groups_merged_segments_with_ragged_tails(oracle, ctx, pm, smem_gr
             merged = pm.execute_segments(devs, q, merge=True)
             assert len(merged) == 1 and merged[0].count_carrier, text
             assert_tables_equal(q, gpu_table(segs[0], q, merged[0]), combine(fns, want), f"smem={smem_groups} merged: {text}")
+            check_exact(oracle, segs, q, gpu_table(segs[0], q, merged[0]), f"smem={smem_groups} merged: {text}")
     finally:
         for d in devs:
             d.destroy()
@@ -108,6 +110,7 @@ def test_carrier_count_overflow_inside_a_cta_table_falls_back(oracle, ctx, pm):
         merged = pm.execute_segments([dev, dev, dev], q, merge=True)[0]
         assert not merged.count_carrier
         assert_tables_equal(q, gpu_table(seg, q, merged), combine(["SUM", "COUNT"], [oracle_table(seg, q, oracle.execute(seg, q))] * 3), "merged overflow")
+        check_exact(oracle, [seg] * 3, q, gpu_table(seg, q, merged), "merged overflow")
     finally:
         ctx.set_tuning("pack_shift", 0)
         dev.destroy()
