@@ -1372,15 +1372,19 @@ static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment*
       d.num_groups_limit = query->num_groups_limit;
       for (int a = 0; a < nagg; a++) { d.aggs.push_back(query->aggs[a]); d.val_kind.push_back(q.aggs[a].val_kind); d.agg_cols.push_back(q.aggs[a].slot < 0 ? nullptr : &seg->cols[query->aggs[a].column]); }
       // one block per element kind
-      // the exact per-group count is kept only when a function needs it; otherwise a MIN/MAX table (or a flag table)
-      // marks the groups that exist -- one atomic less per surviving row
+      // the exact per-group count is kept only when a function needs it; otherwise a dictionary MIN/MAX table (or a flag
+      // table) marks the groups that exist -- one atomic less per surviving row.  A raw INT MIN/MAX table cannot: every
+      // u32 is a value there, the empty entry included (max_offset in pb200_desc.h)
       bool need_count = tune.always_count != 0;
-      bool has_minmax = false;
+      auto marks_groups = [&](int a) {
+        return (q.aggs[a].function == PB200_AGG_MIN || q.aggs[a].function == PB200_AGG_MAX) && q.aggs[a].val_kind != VAL_RAW_I32;
+      };
+      bool has_marker = false;
       for (int a = 0; a < nagg; a++) {
         need_count |= q.aggs[a].function == PB200_AGG_COUNT || q.aggs[a].function == PB200_AGG_AVG;
-        has_minmax |= q.aggs[a].function == PB200_AGG_MIN || q.aggs[a].function == PB200_AGG_MAX;
+        has_marker |= marks_groups(a);
       }
-      bool need_seen = !need_count && !has_minmax && !hashed;  // a hash table's keys mark the groups that exist
+      bool need_seen = !need_count && !has_marker && !hashed;  // a hash table's keys mark the groups that exist
       // ---- count carrier (see count_carrier above) ----
       d.pack_agg = -1;
       const bool deferred = merge && (query->flags & PB200_Q_DEFER_FINALIZE);
@@ -1431,8 +1435,8 @@ static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment*
           if (sum_in_double(vk)) d.dsum[a] = (double*)d.f64_block + (fi++) * groups;
           else d.isum[a] = (long long*)d.i64_block + (ii++) * groups;
           if (a == d.pack_agg) d.exists_packed = (const unsigned long long*)d.isum[a];
-        } else if (fn == PB200_AGG_MIN) { d.gmin[a] = (uint32_t*)d.u32min_block + (ni++) * groups; if (!need_count && !d.exists_max && !d.exists_min) d.exists_min = d.gmin[a]; }
-        else if (fn == PB200_AGG_MAX) { d.gmax[a] = (uint32_t*)d.u32max_block + (xi++) * groups; if (!need_count && !d.exists_max && !d.exists_min) d.exists_max = d.gmax[a]; }
+        } else if (fn == PB200_AGG_MIN) { d.gmin[a] = (uint32_t*)d.u32min_block + (ni++) * groups; if (!need_count && marks_groups(a) && !d.exists_max && !d.exists_min) d.exists_min = d.gmin[a]; }
+        else if (fn == PB200_AGG_MAX) { d.gmax[a] = (uint32_t*)d.u32max_block + (xi++) * groups; if (!need_count && marks_groups(a) && !d.exists_max && !d.exists_min) d.exists_max = d.gmax[a]; }
         else if (fn == PB200_AGG_DISTINCTCOUNT) {  // one dictId bitset per group / slot
           const DeviceColumn& c = seg->cols[query->aggs[a].column];
           const unsigned long long words = ((unsigned long long)c.cardinality + 31) / 32;
@@ -1609,10 +1613,13 @@ static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment*
         else if (fn == PB200_AGG_SUM || fn == PB200_AGG_AVG) {
           d = sum_in_double(vk) ? acc.dsum[a] : (double)acc.isum[a];
           l = (int64_t)acc.count;
-        } else if (fn == PB200_AGG_MIN) {
-          if (acc.min_id[a] == 0xFFFFFFFFu || acc.count == 0) d = INFINITY; else { id = (int32_t)acc.min_id[a]; d = c->dict_host.empty() && vk != VAL_RAW_I32 ? (double)id : value_of(acc.min_id[a]); }
-        } else if (fn == PB200_AGG_MAX) {
-          if (acc.max_id_plus1[a] == 0) d = -INFINITY; else { id = (int32_t)(acc.max_id_plus1[a] - 1); d = c->dict_host.empty() && vk != VAL_RAW_I32 ? (double)id : value_of(acc.max_id_plus1[a] - 1); }
+        } else if (fn == PB200_AGG_MIN || fn == PB200_AGG_MAX) {
+          // raw INT: 0xFFFFFFFF / 0 are INT_MAX / INT_MIN as well as "no row" (max_offset): only the count tells
+          const bool mn = fn == PB200_AGG_MIN;
+          const uint32_t x = mn ? acc.min_id[a] : acc.max_id_plus1[a] - max_offset(vk);
+          const bool empty = acc.count == 0 || (vk != VAL_RAW_I32 && (mn ? acc.min_id[a] == 0xFFFFFFFFu : acc.max_id_plus1[a] == 0));
+          if (empty) d = mn ? INFINITY : -INFINITY;
+          else { id = (int32_t)x; d = c->dict_host.empty() && vk != VAL_RAW_I32 ? (double)id : value_of(x); }
         } else if (fn == PB200_AGG_DISTINCTCOUNT) {
           int maxbits = c->bits;
           if (merge) for (int t = 0; t < nseg; t++) maxbits = std::max(maxbits, segments[t]->cols[query->aggs[a].column].bits);

@@ -6,7 +6,11 @@
 //   int64 block   COUNT / integer SUM (and count-carrying sums)   ncclSum
 //   double block  FLOAT / DOUBLE / LONG sums                        ncclSum
 //   u32max block  MAX as dictId + 1, 0 = empty                      ncclMax on ncclUint32
+//                 (raw INT: value ^ 0x80000000, 0 = INT_MIN or empty; group-exists flags)
 //   u32min block  MIN as dictId, 0xFFFFFFFF = empty                 ncclMin on ncclUint32
+//                 (raw INT: value ^ 0x80000000, 0xFFFFFFFF = INT_MAX or empty)
+// A raw INT entry's emptiness is never read from the entry: the group's count, seen flag, carrier or hash key tells
+// (max_offset in pb200_desc.h).  Both stay neutral elements of their reduce, so the reduces are the same for both kinds.
 // pb200_result_combine issues ALL of a result's reduces as ONE NCCL group on the context's stream, reads the carrier verdict
 // that rides behind the int64 block (pb200_api.cu), and lets the root extract the groups -- one library call per rank and
 // query instead of four Python-driven collectives, a tensor-alias step and a second call for the extraction.

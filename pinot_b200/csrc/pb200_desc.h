@@ -33,6 +33,13 @@ enum : int32_t { VAL_NONE = 0, VAL_DICT_I32 = 1, VAL_DICT_I64 = 2, VAL_DICT_F32 
 // int64 accumulator (|v| x rows < 2^31 x 2^31, cannot wrap).
 __host__ __device__ constexpr bool sum_in_double(int vk) { return vk == VAL_DICT_F32 || vk == VAL_DICT_F64 || vk == VAL_DICT_I64; }
 
+// MIN / MAX entries hold an order-preserving u32: the dictId, or for a raw INT column x = value ^ 0x80000000.  A MIN entry
+// starts at 0xFFFFFFFF, a MAX entry at 0; MAX stores x + max_offset(vk).  DictIds are below 2^31, so dictId + 1 never
+// wraps and 0 / 0xFFFFFFFF mean "no row".  A raw INT spans all of u32 (INT_MAX is 0xFFFFFFFF, INT_MIN is 0): its MAX is
+// stored as x, and whether the group has a row at all comes from its count, seen flag, count carrier or hash key -- never
+// from a raw MIN / MAX entry.
+__host__ __device__ constexpr uint32_t max_offset(int vk) { return vk == VAL_RAW_I32 ? 0u : 1u; }
+
 struct SlotDesc {
   const uint32_t* data;  // device: packed words, padded to whole tiles
   int32_t bits;          // 1..32 (32 = raw big-endian 32-bit values)
@@ -70,8 +77,8 @@ struct AggAccum {
   unsigned long long count;             // matched docs
   long long isum[kMaxAggs];             // exact integer sums (INT / LONG dictionaries)
   double dsum[kMaxAggs];                // FLOAT / DOUBLE sums
-  uint32_t min_id[kMaxAggs];            // dictId (or order-preserving raw encoding); 0xFFFFFFFF = empty
-  uint32_t max_id_plus1[kMaxAggs];      // dictId + 1; 0 = empty
+  uint32_t min_id[kMaxAggs];            // dictId (or order-preserving raw encoding); 0xFFFFFFFF = empty (raw: count == 0)
+  uint32_t max_id_plus1[kMaxAggs];      // dictId + 1; 0 = empty (raw INT: the encoding itself, see max_offset)
 };
 
 struct SegDesc {
@@ -91,7 +98,7 @@ struct SegDesc {
   AggAccum* accum;                     // aggregation-only output
   // dense group table (group-by): indexed by raw key = sum_j dictId_j * mult_j
   unsigned long long* g_count;   // per-group row count; NULL when no COUNT / AVG needs it
-  uint32_t* g_seen;              // then: group-exists flags (NULL if a MIN/MAX table already tells)
+  uint32_t* g_seen;              // then: group-exists flags (NULL if a dictionary MIN/MAX table already tells)
   long long* g_isum[kMaxAggs];
   double* g_dsum[kMaxAggs];
   uint32_t* g_min[kMaxAggs];

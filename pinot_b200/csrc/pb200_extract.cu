@@ -31,9 +31,9 @@ constexpr size_t kSpeculativeBytes = 512ull << 10;
 constexpr unsigned long long kNoCol = ~0ull;
 
 struct ExtractDesc {
-  const unsigned long long* count;   // existence markers, see NonEmpty below
+  const unsigned long long* count;   // existence markers, see non_empty() below
   const uint32_t* seen;
-  const uint32_t* maxk;
+  const uint32_t* maxk;              // dictionary MIN / MAX tables only (a raw INT entry has no empty value)
   const uint32_t* mink;
   const unsigned long long* hkeys;
   const unsigned long long* packed;  // count-carrying sum table (pb200_api.cu): sum(value - vmin) + count << shift
@@ -154,10 +154,12 @@ __global__ void __launch_bounds__(kExtractThreads) extract_write_kernel(const Ex
         lv = (long long)cnt;
       } else if (fn == PB200_AGG_MIN || fn == PB200_AGG_MAX) {
         const uint32_t t = static_cast<const uint32_t*>(d.src[a])[g];
-        const bool empty = fn == PB200_AGG_MIN ? t == 0xFFFFFFFFu : t == 0u;
+        // every row of a submission reaches each of its functions, so a group that exists has a MIN / MAX.  Raw INT entries
+        // are all values (max_offset): 0xFFFFFFFF / 0 are INT_MAX / INT_MIN there, never "empty"
+        const bool empty = vk != VAL_RAW_I32 && (fn == PB200_AGG_MIN ? t == 0xFFFFFFFFu : t == 0u);
         if (empty) dv = fn == PB200_AGG_MIN ? INFINITY : -INFINITY;
         else {
-          const uint32_t x = fn == PB200_AGG_MIN ? t : t - 1u;
+          const uint32_t x = fn == PB200_AGG_MIN ? t : t - max_offset(vk);
           id = (int32_t)x;
           if (vk == VAL_RAW_I32) dv = (double)(int32_t)(x ^ 0x80000000u);
           else if (!d.dict[a]) dv = (double)x;

@@ -462,8 +462,9 @@ scan_kernel(const __grid_constant__ QueryDesc q, const __grid_constant__ TmaTabl
               for (int u = 0; u < kQB; ++u) if (((pend_ok >> u) & 1u) && pq[k][u] < px[k][u]) atomicMin(t + pg[u], pq[k][u]);
             } else {
               uint32_t* t = sd.g_max[a];
+              const uint32_t inc = max_offset(vk);
 #pragma unroll
-              for (int u = 0; u < kQB; ++u) if (((pend_ok >> u) & 1u) && pq[k][u] + 1u > px[k][u]) atomicMax(t + pg[u], pq[k][u] + 1u);
+              for (int u = 0; u < kQB; ++u) if (((pend_ok >> u) & 1u) && pq[k][u] + inc > px[k][u]) atomicMax(t + pg[u], pq[k][u] + inc);
             }
           }
         }
@@ -705,7 +706,7 @@ scan_kernel(const __grid_constant__ QueryDesc q, const __grid_constant__ TmaTabl
         } else if (fn == 2 || fn == 3) {
           const uint32_t x = id ^ (vk == VAL_RAW_I32 ? 0x80000000u : 0u);
           uint2 mmx = accmm[a * kConsumers + group];
-          mmx.x = min(mmx.x, x); mmx.y = max(mmx.y, x + 1u);
+          mmx.x = min(mmx.x, x); mmx.y = max(mmx.y, x + max_offset(vk));
           accmm[a * kConsumers + group] = mmx;
         } else if (fn == 5) {
           atomicOr(sd.distinct_bits[a] + (id >> 5), 1u << (id & 31));
@@ -862,6 +863,7 @@ scan_kernel(const __grid_constant__ QueryDesc q, const __grid_constant__ TmaTabl
               // MIN / MAX tables change for only O(log n) of a group's rows: read the current entries first, then issue
               // a reduction only where the row can win (a stale read costs a redundant reduction, never a wrong result)
               const uint32_t bias = vk == VAL_RAW_I32 ? 0x80000000u : 0u;
+              const uint32_t inc = max_offset(vk);
               uint32_t* tab = fn == 2 ? sd.g_min[a] : sd.g_max[a];
               uint32_t cur[kQB];
 #pragma unroll
@@ -870,7 +872,7 @@ scan_kernel(const __grid_constant__ QueryDesc q, const __grid_constant__ TmaTabl
               for (int u = 0; u < kQB; ++u) {
                 const uint32_t x = id[u] ^ bias;
                 if (fn == 2) { if (x < cur[u]) atomicMin(tab + g[u], x); }
-                else { if (x + 1u > cur[u]) atomicMax(tab + g[u], x + 1u); }
+                else { if (x + inc > cur[u]) atomicMax(tab + g[u], x + inc); }
               }
             }
           }
@@ -946,11 +948,11 @@ scan_kernel(const __grid_constant__ QueryDesc q, const __grid_constant__ TmaTabl
                 double* slot = reinterpret_cast<double*>(acc64 + a * kConsumers + group);
                 *slot += acc;
               }
-            } else if (fn == 2 || fn == 3) {  // raw INT: signed -> unsigned order
+            } else if (fn == 2 || fn == 3) {  // raw INT: signed -> unsigned order, MAX stored without the +1 (max_offset)
               uint32_t tmn = 0xFFFFFFFFu, tmx = 0u;
 #pragma unroll
               for (int j = 0; j < 32; ++j)
-                if ((m >> j) & 1u) { const uint32_t x = v[j] ^ 0x80000000u; tmn = min(tmn, x); tmx = max(tmx, x + 1u); }
+                if ((m >> j) & 1u) { const uint32_t x = v[j] ^ 0x80000000u; tmn = min(tmn, x); tmx = max(tmx, x); }
               uint2 mmx = accmm[a * kConsumers + group];
               mmx.x = min(mmx.x, tmn); mmx.y = max(mmx.y, tmx);
               accmm[a * kConsumers + group] = mmx;

@@ -15,6 +15,10 @@ ones after ``DictionaryDomain`` binding, see ``global_domain``) and the tables m
     u32max    MAX as (dictId + 1), 0 = empty          MAX              MaxAggregationFunction.merge
     u32min    MIN as dictId, 0xFFFFFFFF = empty       MIN              MinAggregationFunction.merge
 
+A raw INT column's MIN / MAX entries hold value ^ 0x80000000 (MAX without the + 1): 0 and 0xFFFFFFFF are INT_MIN and
+INT_MAX there as well as "empty", and the group's count, seen flag, count carrier or hash key says whether it exists.
+The empty values are still the neutral elements of MAX / MIN, so the reduce is the same for both kinds.
+
 ``torch.distributed`` (NCCL over NVLink / NVSwitch) is plumbing only: the tensors handed to it alias the library's own
 device buffers (``pb200_result_device_buffers``), nothing is copied.  The tables are O(groups), not O(rows): the
 exchange is latency-bound (C4: 100 000 groups x (8+8+4) B = 2 MB per rank).

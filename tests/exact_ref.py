@@ -1,9 +1,10 @@
-"""Exact reference for SUM / AVG / COUNT, independent of the oracle's aggregation code, and the comparator that holds the
-device's results to it.
+"""Exact reference for COUNT / SUM / AVG / MIN / MAX / DISTINCTCOUNT, independent of the oracle's aggregation code, and the
+comparator that holds the device's results to it.
 
 The oracle accumulates SUM in Java order in a `double`, so it states parity with the reference but cannot tell an exact
-integer sum from a nearly exact one.  Here the rows come from the oracle's filter (pinned to the reference's goldens), the
-values and group keys straight from the segment's columns, and the arithmetic is exact:
+integer sum from a nearly exact one; its MIN / MAX fold doubles, so it cannot tell which row won either.  Here the rows
+come from the oracle's filter (pinned to the reference's goldens), the values and group keys straight from the segment's
+columns, and the arithmetic is exact:
 
 * INT columns (dictionary or raw): per-group sums in int64 (exact while rows x 2^31 < 2^63); the device must return
   `float(exact)`, the correctly rounded double, bit for bit.
@@ -12,13 +13,24 @@ values and group keys straight from the segment's columns, and the arithmetic is
   gamma_n * A of S, gamma_n = n u / (1 - n u), u = 2^-53.  That bound holds for every summation order (a LONG's
   rounding to double included) and does not depend on |S|, so cancelling values are no false alarm.
 * COUNT and the AVG count: equal.
+* MIN / MAX: the stored value of the group's smallest / largest row (int for INT / LONG, float for FLOAT / DOUBLE).  A
+  dictionary column is ordered by its dictionary (the smallest / largest dictId, Pinot's order for every type); a raw
+  column numerically.  A group without a row: +inf / -inf.  The device must return `float(value)` (round to nearest:
+  LONG beyond 2^53), bit for bit.  STRING MIN / MAX come back as dictIds, not values, and are left to the oracle
+  comparison.
+* DISTINCTCOUNT: the set of the group's distinct values, equal.
 
 Merged results: the reference runs over the union of the segments' rows, keyed by value (not a sum of per-segment floats).
+
+Out of scope: NaN and -0.0 in FLOAT / DOUBLE columns.  np.unique (the test segment builder) merges -0.0 with +0.0 and
+sorts NaN last, while the reference's Math.min / Math.max propagate NaN and its group-by `<` keeps whichever zero came
+first; which one the product follows is not settled here, so no test feeds those values.
 """
 from __future__ import annotations
 
 import dataclasses
 import math
+import struct
 from dataclasses import dataclass
 from fractions import Fraction
 from typing import Dict, List, Optional, Sequence
@@ -112,9 +124,57 @@ def _float_sums(values: np.ndarray, gidx: np.ndarray, groups: int):
     return s, a
 
 
+def _extremes(oracle, segs, docs, column: str, sel: np.ndarray, gidx: np.ndarray, groups: int, fn: str) -> list:
+    """Per group, the MIN / MAX stored value of `column` over the selected rows (+-inf: no row).
+    Inside a segment the order is its dictionary's (smallest / largest dictId) or, raw, the numeric one; across segments
+    the winners are compared by value."""
+    pick = np.minimum if fn == "MIN" else np.maximum
+    best, have = None, np.zeros(groups, dtype=bool)
+    at = 0
+    for s, d in zip(segs, docs):
+        m = sel[at:at + len(d)]
+        g = gidx[at:at + len(d)][m]
+        at += len(d)
+        if not len(g):
+            continue
+        c = s.column(column)
+        present = np.zeros(groups, dtype=bool)
+        present[g] = True
+        some_row = np.zeros(groups, dtype=np.int64)   # the start value of a present group is one of its own rows
+        some_row[g] = np.arange(len(g))
+        if c.has_dictionary:
+            ids = _dict_ids(oracle, s, c, d[m]).astype(np.int64)
+            win = ids[some_row]
+            pick.at(win, g, ids)
+            v = _dictionary(c)[win]
+        else:
+            vals = np.asarray(c.raw_values)[d[m]]
+            v = vals[some_row]
+            pick.at(v, g, vals)
+        if best is None:
+            best = v.copy()
+        else:
+            both = have & present
+            best[both] = pick(best[both], v[both])
+            best[present & ~have] = v[present & ~have]
+        have |= present
+    empty = math.inf if fn == "MIN" else -math.inf
+    if best is None:
+        return [empty] * groups
+    return [best[i].item() if have[i] else empty for i in range(groups)]
+
+
+def _distinct_sets(values: np.ndarray, gidx: np.ndarray, groups: int) -> List[frozenset]:
+    order = np.argsort(gidx, kind="stable")
+    bounds = np.searchsorted(gidx[order], np.arange(groups + 1))
+    sv = values[order]
+    return [frozenset(_key_value(x) for x in np.unique(sv[bounds[g]:bounds[g + 1]]).tolist()) for g in range(groups)]
+
+
 def reference(oracle, segs: Sequence[sb.SegmentData], q) -> Dict[tuple, list]:
     """{group key values: [per aggregation]} over the union of the segments' rows: COUNT -> int, SUM / AVG -> ExactSum,
-    other functions -> None.  Keys are the value tuples reduce_util.normalise produces."""
+    MIN / MAX -> stored value or +-inf (None for STRING), DISTINCTCOUNT -> frozenset of values.  Keys are the value tuples
+    reduce_util.normalise produces."""
     docs = [oracle.filter_doc_ids(s, q)[0].astype(np.int64) for s in segs]
     # group index of every matched row: per column, values -> codes over the union, then mixed radix
     if q.group_by:
@@ -142,20 +202,28 @@ def reference(oracle, segs: Sequence[sb.SegmentData], q) -> Dict[tuple, list]:
     groups = len(keys)
     cols = [[None] * groups for _ in q.aggregations]
     for a, agg in enumerate(q.aggregations):
-        if agg.function not in ("COUNT", "SUM", "AVG"):
+        dt = segs[0].column(agg.column).data_type if agg.column is not None else None
+        if agg.function not in ("COUNT", "SUM", "AVG", "MIN", "MAX", "DISTINCTCOUNT"):
+            continue
+        if agg.function in ("MIN", "MAX") and dt == sb.STRING:
             continue
         if agg.filter is not None:   # FILTER (WHERE ...): the main filter's rows that the clause matches too
             cq = dataclasses.replace(q, filter=agg.filter)
             sel = np.concatenate([np.isin(d, oracle.filter_doc_ids(s, cq)[0]) for s, d in zip(segs, docs)])
         else:
             sel = np.ones(len(gidx), dtype=bool)
+        if agg.function in ("MIN", "MAX"):
+            cols[a] = _extremes(oracle, segs, docs, agg.column, sel, gidx, groups, agg.function)
+            continue
         g = gidx[sel]
         counts = [int(x) for x in np.bincount(g, minlength=groups)]
         if agg.function == "COUNT":
             cols[a] = counts
             continue
         vals = np.concatenate([column_values(oracle, s, agg.column, d) for s, d in zip(segs, docs)])[sel]
-        dt = segs[0].column(agg.column).data_type
+        if agg.function == "DISTINCTCOUNT":
+            cols[a] = _distinct_sets(vals, g, groups)
+            continue
         if dt == sb.INT:
             cols[a] = [ExactSum("int", s, None, n) for s, n in zip(_exact_int_sums(vals, g, groups), counts)]
         elif dt == sb.LONG:
@@ -182,24 +250,31 @@ def check_sum(got: float, ref: ExactSum) -> bool:
     return sum_within_bound(got, ref)
 
 
-def assert_sums_exact(q, got: Dict[tuple, list], ref: Dict[tuple, list], what: str = "") -> None:
+def same_double(got: float, ref: float) -> bool:
+    """Bit-for-bit equality of two doubles (0.0 and -0.0 differ, an infinity only equals itself)."""
+    return struct.pack("<d", got) == struct.pack("<d", ref)
+
+
+def assert_exact(q, got: Dict[tuple, list], ref: Dict[tuple, list], what: str = "") -> None:
     """Per aggregation: COUNT equal; SUM / AVG over INT bit-exact (AVG: and its count equal); over LONG / FLOAT / DOUBLE
-    within gamma_n * A of the exact sum.  MIN / MAX / DISTINCTCOUNT are left to the oracle comparison."""
+    within gamma_n * A of the exact sum; MIN / MAX bit-exact; DISTINCTCOUNT the same set of values."""
     assert set(got) == set(ref), f"{what}: group keys differ from the exact reference: {len(got)} vs {len(ref)}"
     for key, rv in ref.items():
         gv = got[key]
         for a, agg in enumerate(q.aggregations):
             fn, r = agg.function, rv[a]
-            if fn == "COUNT":
-                assert gv[a] == r, (what, key, fn, gv[a], r)
+            if fn in ("COUNT", "DISTINCTCOUNT"):
+                assert gv[a] == r, (what, key, fn, agg.column, gv[a], r)
             elif fn in ("SUM", "AVG"):
                 s = gv[a] if fn == "SUM" else gv[a][0]
                 if fn == "AVG":
                     assert gv[a][1] == r.n, (what, key, "AVG count", gv[a][1], r.n)
                 assert check_sum(s, r), (what, key, fn, agg.column, r.kind, repr(s), r.s, r.n)
+            elif fn in ("MIN", "MAX") and r is not None:
+                assert same_double(gv[a], float(r)), (what, key, fn, agg.column, float(gv[a]).hex(), float(r).hex(), r)
 
 
 def check_exact(oracle, segs: Sequence[sb.SegmentData], q, got: Dict[tuple, list], what: str = "") -> Dict[tuple, list]:
     ref = reference(oracle, segs, q)
-    assert_sums_exact(q, got, ref, what)
+    assert_exact(q, got, ref, what)
     return ref

@@ -1,6 +1,8 @@
 """Helpers shared by the -m gpu tests: run one query through the product (C-ABI) and through the oracle, compare."""
 from __future__ import annotations
 
+import contextlib
+
 from exact_ref import check_exact
 from pinot_b200.plan_maker import IndexSegment
 from reduce_util import normalise
@@ -9,6 +11,23 @@ from reduce_util import normalise
 # everything else equal.  It is not the exactness check: integer SUMs are held bit-exact, and floating sums to the gamma_n
 # bound, by tests/exact_ref.py (check_query runs both).
 SUM_REL_TOL = 1e-6
+
+# pb200_tuning_set knobs at their library defaults: what tuned() restores
+TUNING_DEFAULTS = {"warps": 6, "defer": 1, "gb_defer": 1, "sparse_max_agg": -1, "smem_groups": 1, "smem_copies": 0,
+                   "pack_count": 1, "pack_shift": 0, "dense_max": 1 << 24, "table_stride": 0, "grid": 0, "ctas_per_sm": 2,
+                   "raw_dict_max": 1 << 20, "always_count": 0}
+
+
+@contextlib.contextmanager
+def tuned(ctx, **knobs):
+    """Sets tuning knobs for the body of a `with` and restores their defaults afterwards, also when the body fails."""
+    try:
+        for name, value in knobs.items():
+            ctx.set_tuning(name, value)
+        yield
+    finally:
+        for name in knobs:
+            ctx.set_tuning(name, TUNING_DEFAULTS[name])
 
 
 def to_device(ctx, seg_data) -> IndexSegment:

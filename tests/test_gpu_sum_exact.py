@@ -6,13 +6,11 @@ above 2^53, the count carrier with a negative minimum over the full 32-bit range
 Each route is forced with pb200_tuning_set and the knob is restored in a `finally`.  Every docstring names the host rule in
 pinot_b200/csrc/pb200_api.cu (pb200_execute) that sends the query down that route.  Segment sizes cover ragged tails and
 the tile edges of both CTA widths (6 x 1024 and 8 x 1024 rows)."""
-import contextlib
-
 import numpy as np
 import pytest
 
 from exact_ref import check_exact
-from gpu_util import check_query, gpu_table, to_device
+from gpu_util import check_query, gpu_table, to_device, tuned
 from pinot_b200 import sql
 from pinot_b200.plan_maker import B200Context, B200PlanMaker
 
@@ -23,9 +21,6 @@ SIZES = [1, 31, 33, 6_143, 6_144, 6_145, 8_191, 8_192, 8_193, 16_385, 50_000]
 VALUE_SETS = ["int_max", "int_min", "five", "heavy", "cancel"]
 G = 24            # small key space "k": a replicated shared-memory table
 GB = 10_000       # large key space "kb": one 8-warp CTA per SM with the table (segments of >= GB rows hold every key)
-TUNING_DEFAULTS = {"warps": 6, "defer": 1, "gb_defer": 1, "sparse_max_agg": -1, "smem_groups": 1, "smem_copies": 0,
-                   "pack_count": 1, "pack_shift": 0, "dense_max": 1 << 24, "table_stride": 0, "grid": 0, "ctas_per_sm": 2,
-                   "raw_dict_max": 1 << 20}
 
 AGG_QUERIES = ["SELECT SUM(v), COUNT(*), AVG(v) FROM t WHERE w < 7",
                "SELECT SUM(v) FROM t"]
@@ -35,17 +30,6 @@ GB_QUERIES = ["SELECT SUM(v), COUNT(*) FROM t WHERE w < 7 GROUP BY {k}",
 RAW_QUERIES = ["SELECT SUM(r), COUNT(*), AVG(r) FROM t WHERE w < 7",
                "SELECT SUM(r), COUNT(*) FROM t WHERE w < 7 GROUP BY k",
                "SELECT AVG(r), SUM(v) FROM t GROUP BY k"]
-
-
-@contextlib.contextmanager
-def tuned(ctx, **knobs):
-    try:
-        for name, value in knobs.items():
-            ctx.set_tuning(name, value)
-        yield
-    finally:
-        for name in knobs:
-            ctx.set_tuning(name, TUNING_DEFAULTS[name])
 
 
 def _values(vset, k, rng):
