@@ -35,7 +35,9 @@ extern "C" {
 #endif
 
 #define PB200_ABI_VERSION 3 /* 2: pb200_query.reduce_world / merged_docs_bound, domains, tuning, pb200_result_meta.reserved bits;
-                              3: pb200_comm_*, pb200_result_columns, doc masks, pb200h_query.agg_filter_* (the host query struct grew) */
+                              3: pb200_comm_*, pb200_result_columns, doc masks, pb200h_query.agg_filter_* (the host query struct grew);
+                                 pb200_order_by / pb200_execute_ordered / pb200h_execute_ordered were added later without a
+                                 version change: they are new symbols and structs, no existing one changed */
 
 enum {
   PB200_OK = 0,
@@ -228,6 +230,30 @@ typedef struct {
  * (core/operator/query/GroupByOperator.java:101-140, AggregationOperator.java:64-80). */
 int32_t pb200_execute(pb200_ctx* ctx, const pb200_query* query, pb200_segment* const* segments,
                       int32_t num_segments, pb200_result** results);
+
+/* ---- ORDER BY ... LIMIT of group-by results (GroupByCombineOperator's IndexedTable / TableResizer trim) ---------------- */
+/* An order item compares the FINAL value of an aggregation (COUNT, SUM, MIN / MAX with +-inf for a group without rows,
+ * AVG = sum / count or -inf at count 0, DISTINCTCOUNT = set size; doubles like Double.compare) or the dictId of a group-by
+ * column; rows equal on every item are ordered by their group-key values ascending, in GROUP BY column order.  The rows of
+ * an ordered result come back in that order, and only the first trim_size of them (trim_size <= 0: all, sorted).  The
+ * numGroupsLimit check applies to the untrimmed group count; num_groups is the number of rows kept. */
+#define PB200_MAX_ORDER_BY 8
+enum { PB200_ORDER_AGG = 0, PB200_ORDER_GROUP_BY = 1 };
+typedef struct {
+  int32_t kind;       /* PB200_ORDER_AGG: index into pb200_query.aggs; PB200_ORDER_GROUP_BY: index into group_by_columns */
+  int32_t index;
+  int32_t descending; /* 0: ASC, else DESC */
+} pb200_order_item;
+typedef struct {
+  int32_t num_items;  /* 1 .. PB200_MAX_ORDER_BY */
+  int32_t trim_size;  /* rows kept per result; <= 0: sort without trimming */
+  pb200_order_item items[PB200_MAX_ORDER_BY];
+} pb200_order_by;
+/* pb200_execute with the group-by results ordered and trimmed on the device (order == NULL: exactly pb200_execute).  A
+ * PB200_Q_DEFER_FINALIZE result keeps the spec: pb200_result_finalize and pb200_result_combine apply it when they extract.
+ * Aggregation-only queries ignore it.  A bad item index or num_items outside 1..8: PB200_E_INVALID. */
+int32_t pb200_execute_ordered(pb200_ctx* ctx, const pb200_query* query, const pb200_order_by* order,
+                              pb200_segment* const* segments, int32_t num_segments, pb200_result** results);
 
 /* ---- results (the data a GroupByResultsBlock / AggregationResultsBlock is built from) ---------------------------- */
 enum { PB200_REGIME_NONE = 0, PB200_REGIME_ARRAY = 1, PB200_REGIME_INT_MAP = 2, PB200_REGIME_LONG_MAP = 3,

@@ -177,6 +177,12 @@ enum {
  * super.makeSegmentPlanNode(). */
 int32_t pb200h_execute(pb200_ctx* ctx, const pb200h_query* query, pb200h_segment* const* segments,
                        int32_t num_segments, pb200_result** results, int32_t* operator_kinds);
+/* pb200h_execute with the group-by results ordered and trimmed (pb200_order_by of include/pinot_b200.h; group-by indices
+ * refer to query->group_by, aggregation indices to query->aggs).  Results built on the host (star-tree, FILTER clauses) are
+ * ordered and trimmed on the host by the same rule.  order == NULL: exactly pb200h_execute. */
+int32_t pb200h_execute_ordered(pb200_ctx* ctx, const pb200h_query* query, const pb200_order_by* order,
+                               pb200h_segment* const* segments, int32_t num_segments, pb200_result** results,
+                               int32_t* operator_kinds);
 /* The result as the server -> broker wire format: DataTableImplV4 bytes (pinot-common/.../datatable/DataTableImplV4.java:49-81)
  * exactly as GroupByResultsBlock.getDataTable() / AggregationResultsBlock.getDataTable() build them for the same rows
  * (GroupByResultsBlock.java:186-236): typed group-key values (STRING keys through the DataTable's own string dictionary),

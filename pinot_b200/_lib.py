@@ -107,6 +107,18 @@ class HQuery(C.Structure):
                 ("agg_filter_start", C.POINTER(C.c_int32)), ("agg_filter_count", C.POINTER(C.c_int32))]
 
 
+MAX_ORDER_BY = 8
+ORDER_AGG, ORDER_GROUP_BY = 0, 1
+
+
+class OrderItem(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("index", C.c_int32), ("descending", C.c_int32)]
+
+
+class OrderBy(C.Structure):
+    _fields_ = [("num_items", C.c_int32), ("trim_size", C.c_int32), ("items", OrderItem * MAX_ORDER_BY)]
+
+
 class HStarMetric(C.Structure):
     _fields_ = [("function", C.c_int32), ("reserved", C.c_int32), ("column", C.c_char_p), ("fwd", C.c_void_p),
                 ("fwd_bytes", C.c_uint64)]
@@ -115,13 +127,13 @@ class HStarMetric(C.Structure):
 # every symbol include/pinot_b200.h and include/pinot_b200_host.h declare (checked by tests/test_abi.py)
 EXPORTED_SYMBOLS = [
     "pb200_init", "pb200_shutdown", "pb200_last_error", "pb200_abi_version", "pb200_device_info", "pb200_tuning_set",
-    "pb200_segment_register", "pb200_segment_release", "pb200_segment_device_bytes", "pb200_execute",
+    "pb200_segment_register", "pb200_segment_release", "pb200_segment_device_bytes", "pb200_execute", "pb200_execute_ordered",
     "pb200_result_meta_get", "pb200_result_group_keys", "pb200_result_agg", "pb200_result_agg_dict_ids",
     "pb200_result_distinct", "pb200_result_fetch", "pb200_result_free", "pb200_result_device_buffers", "pb200_result_finalize",
     "pb200_synth_segment", "pb200_segment_read_index", "pb200_segment_column_info",
     "pb200h_segment_create", "pb200h_segment_adopt", "pb200h_segment_load_dir", "pb200h_segment_destroy",
     "pb200h_segment_device", "pb200h_segment_num_docs", "pb200h_segment_num_columns", "pb200h_segment_column_index",
-    "pb200h_segment_column_name", "pb200h_segment_column_info", "pb200h_dictionary_get", "pb200h_execute",
+    "pb200h_segment_column_name", "pb200h_segment_column_info", "pb200h_dictionary_get", "pb200h_execute", "pb200h_execute_ordered",
     "pb200h_explain", "pb200h_startree_attach", "pb200h_domain_build", "pb200h_segment_bind_domain",
     "pb200h_result_to_datatable", "pb200h_cache_create", "pb200h_cache_acquire", "pb200h_cache_release", "pb200h_cache_evict",
     "pb200h_cache_stats", "pb200h_cache_destroy",
@@ -152,6 +164,7 @@ def load() -> C.CDLL:
     L.pb200_segment_device_bytes.restype = i64
     L.pb200_segment_device_bytes.argtypes = [vp]
     L.pb200_execute.argtypes = [vp, C.POINTER(Query), C.POINTER(vp), i32, C.POINTER(vp)]
+    L.pb200_execute_ordered.argtypes = [vp, C.POINTER(Query), C.POINTER(OrderBy), C.POINTER(vp), i32, C.POINTER(vp)]
     L.pb200_result_meta_get.argtypes = [vp, C.POINTER(ResultMeta)]
     L.pb200_result_group_keys.argtypes = [vp, vp]
     L.pb200_result_agg.argtypes = [vp, i32, vp, vp]
@@ -180,6 +193,8 @@ def load() -> C.CDLL:
     L.pb200h_segment_column_info.argtypes = [vp, i32, C.POINTER(i32)]
     L.pb200h_dictionary_get.argtypes = [vp, i32, i32, C.POINTER(C.c_double), C.POINTER(i64), C.c_char_p, i32]
     L.pb200h_execute.argtypes = [vp, C.POINTER(HQuery), C.POINTER(vp), i32, C.POINTER(vp), C.POINTER(i32)]
+    L.pb200h_execute_ordered.argtypes = [vp, C.POINTER(HQuery), C.POINTER(OrderBy), C.POINTER(vp), i32, C.POINTER(vp),
+                                         C.POINTER(i32)]
     L.pb200h_explain.argtypes = [vp, C.POINTER(HQuery), vp, C.c_char_p, i32]
     L.pb200h_startree_attach.argtypes = [vp, vp, vp, C.c_uint64, i32, i32, C.POINTER(C.c_char_p), C.POINTER(vp),
                                          C.POINTER(C.c_uint64), i32, C.POINTER(HStarMetric)]

@@ -15,6 +15,7 @@ from __future__ import annotations
 
 import argparse
 import json
+import struct
 import sys
 from typing import Dict, List
 
@@ -57,11 +58,24 @@ def merge_blocks(query, segments, blocks) -> Dict[tuple, list]:
     return out
 
 
+def _order_value(v):
+    """Sort key of a final value: doubles in Double.compare order (-0.0 before 0.0), other values as they are."""
+    if isinstance(v, float):
+        u = struct.unpack("<Q", struct.pack("<d", v))[0]
+        return u ^ 0xFFFFFFFFFFFFFFFF if u >> 63 else u | (1 << 63)
+    return v
+
+
 def final_rows(query, table: Dict[tuple, list]) -> List[list]:
-    """Broker-side extraction of final results + LIMIT (no ORDER BY: Pinot returns an arbitrary LIMIT-sized subset; here the
-    rows are sorted by key to make the output stable)."""
+    """Broker-side extraction of final results + ORDER BY + LIMIT.  ORDER BY compares final values (AVG = sum / count,
+    DISTINCTCOUNT = set size) and breaks ties by the key values ascending, in GROUP BY column order -- the library's order.
+    Without ORDER BY Pinot returns an arbitrary LIMIT-sized subset; here the rows are sorted by key to make the output
+    stable."""
+    from .sql import resolve_order_by
+    items = resolve_order_by(query) if query.is_group_by else []
     rows = []
-    for key in sorted(table, key=lambda k: tuple(str(x) for x in k)):
+    keys = sorted(table) if items else sorted(table, key=lambda k: tuple(str(x) for x in k))
+    for key in keys:
         vals = []
         for agg, v in zip(query.aggregations, table[key]):
             if agg.function == "AVG":
@@ -71,6 +85,10 @@ def final_rows(query, table: Dict[tuple, list]) -> List[list]:
             else:
                 vals.append(v)
         rows.append(list(key) + vals)
+    k = len(query.group_by)
+    for kind, index, asc in reversed(items):  # stable passes, last item first
+        col = index if kind == "GROUP_BY" else k + index
+        rows.sort(key=lambda r: _order_value(r[col]), reverse=not asc)
     return rows[: query.limit]
 
 

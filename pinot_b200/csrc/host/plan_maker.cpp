@@ -662,11 +662,18 @@ extern "C" int32_t pb200h_explain(pb200_ctx* ctx, const pb200h_query* q, pb200h_
 
 extern "C" int32_t pb200h_execute(pb200_ctx* ctx, const pb200h_query* q, pb200h_segment* const* segs, int32_t nseg,
                                   pb200_result** results, int32_t* kinds) {
+  return pb200h_execute_ordered(ctx, q, nullptr, segs, nseg, results, kinds);
+}
+
+extern "C" int32_t pb200h_execute_ordered(pb200_ctx* ctx, const pb200h_query* q, const pb200_order_by* order,
+                                          pb200h_segment* const* segs, int32_t nseg, pb200_result** results, int32_t* kinds) {
   if (!ctx || !q || !segs || !results || nseg <= 0) { set_error("invalid argument to pb200h_execute"); return PB200_E_INVALID; }
   if (q->num_aggs <= 0) { set_error("selection queries are outside this path"); return PB200_E_UNSUPPORTED; }
+  if (int vrc = pb200::order_validate(order, q->num_aggs, q->num_group_by)) return vrc;
+  if (q->num_group_by == 0) order = nullptr;  // aggregation only: one row, nothing to order
   if (q->agg_filter_count && q->agg_filter_start && q->agg_filter_nodes)
     for (int a = 0; a < q->num_aggs; a++)
-      if (q->agg_filter_count[a] > 0) return execute_filtered(ctx, *q, segs, nseg, results, kinds);  // host/filtered_agg.cpp
+      if (q->agg_filter_count[a] > 0) return execute_filtered(ctx, *q, order, segs, nseg, results, kinds);  // host/filtered_agg.cpp
   const bool merge = q->merge_segments != 0;
   // resolve columns by name against segment 0 (all segments of a table share the schema)
   const pb200h_segment& s0 = *segs[0];
@@ -715,7 +722,15 @@ extern "C" int32_t pb200h_execute(pb200_ctx* ctx, const pb200h_query* q, pb200h_
       for (auto& st : segs[s]->star_trees) {
         int rc = try_star_tree(ctx, *segs[s], *st, *q, &star_results[s]);
         if (rc < 0) { for (auto r : star_results) if (r) pb200_result_free(r); return rc; }
-        if (rc == 1) { kind[s] = PB200H_OP_STAR_TREE; break; }
+        if (rc == 1) {
+          kind[s] = PB200H_OP_STAR_TREE;
+          if (order) {  // the star-tree's own submission computes other functions: order by the query's, on the host
+            std::vector<int32_t> fns(q->num_aggs);
+            for (int a = 0; a < q->num_aggs; a++) fns[a] = q->aggs[a].function;
+            pb200::order_rows_host(star_results[s], *order, fns.data());
+          }
+          break;
+        }
       }
     }
   }
@@ -742,7 +757,7 @@ extern "C" int32_t pb200h_execute(pb200_ctx* ctx, const pb200h_query* q, pb200h_
     dq.filter = flat.data();
     dq.group_by_columns = gb.data();
     dq.aggs = aggs.data();
-    int rc = pb200_execute(ctx, &dq, dsegs.data(), (int)dsegs.size(), dev_results.data());
+    int rc = pb200_execute_ordered(ctx, &dq, order, dsegs.data(), (int)dsegs.size(), dev_results.data());
     if (rc) { for (auto r : star_results) if (r) pb200_result_free(r); return rc; }
   }
   if (merge) { results[0] = dev_results[0]; return PB200_OK; }

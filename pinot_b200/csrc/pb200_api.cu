@@ -690,13 +690,19 @@ cudaError_t launch_scan_variant(const ScanVariant& v, size_t smem_bytes, int gri
 // after the launch) -- the caller runs the submission again with separate COUNT reductions.
 constexpr int kRetryWithoutCountCarrier = 1;
 static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment* const* segments, int32_t nseg,
-                        pb200_result** results, bool allow_count_carrier);
+                        pb200_result** results, bool allow_count_carrier, const pb200_order_by* order);
+
+extern "C" int32_t pb200_execute_ordered(pb200_ctx* ctx, const pb200_query* query, const pb200_order_by* order,
+                                         pb200_segment* const* segments, int32_t nseg, pb200_result** results) {
+  if (query) { const int vrc = order_validate(order, query->num_aggs, query->num_group_by); if (vrc) return vrc; }
+  int rc = execute_impl(ctx, query, segments, nseg, results, true, order);
+  if (rc == kRetryWithoutCountCarrier) rc = execute_impl(ctx, query, segments, nseg, results, false, order);
+  return rc;
+}
 
 extern "C" int32_t pb200_execute(pb200_ctx* ctx, const pb200_query* query, pb200_segment* const* segments,
                                  int32_t nseg, pb200_result** results) {
-  int rc = execute_impl(ctx, query, segments, nseg, results, true);
-  if (rc == kRetryWithoutCountCarrier) rc = execute_impl(ctx, query, segments, nseg, results, false);
-  return rc;
+  return pb200_execute_ordered(ctx, query, nullptr, segments, nseg, results);
 }
 
 // Per result: {sum over the table of the carried counts, largest low (sum) field, largest carried count} -- pb200_execute's verification.
@@ -719,7 +725,7 @@ __global__ void carrier_verify_kernel(const unsigned long long* __restrict__ tab
 }
 
 static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment* const* segments, int32_t nseg,
-                        pb200_result** results, bool allow_count_carrier) {
+                        pb200_result** results, bool allow_count_carrier, const pb200_order_by* order) {
   if (!ctx || !query || !segments || !results || nseg <= 0) { set_error("invalid argument to pb200_execute"); return PB200_E_INVALID; }
   const double t_enter = now_ms();
   PB200_CUDA(cudaSetDevice(ctx->device));
@@ -1640,6 +1646,7 @@ static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment*
     }
   }
   const bool defer_finalize = merge && (query->flags & PB200_Q_DEFER_FINALIZE);
+  if (plan.group_by && order) for (int r = 0; r < nres; r++) res[r]->order = *order;  // a deferred result keeps it for its extraction
   const double t_results = now_ms();
   if (plan.group_by && defer_finalize) {
     for (int r = 0; r < nres; r++) { res[r]->meta.num_groups = 0; res[r]->dbl.assign(nagg, {}); res[r]->lng.assign(nagg, {}); res[r]->ids.assign(nagg, {}); res[r]->distinct.assign(nagg, {}); }

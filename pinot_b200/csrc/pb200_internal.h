@@ -140,6 +140,7 @@ struct pb200_result {
     const int64_t* lng[pb200::kMaxAggs] = {};      // NULL: all zero
     const int32_t* ids[pb200::kMaxAggs] = {};      // NULL: all -1
   } view;
+  pb200_order_by order{};                        // ORDER BY spec of a group-by result (num_items 0: none), applied at extraction
   std::vector<int32_t> agg_functions;            // PB200_AGG_* per aggregation (set by pb200_execute)
   std::vector<int32_t> keys;                     // [G x k]
   std::vector<std::vector<double>> dbl;          // per agg [rows]
@@ -210,6 +211,11 @@ struct DevBufRaw {  // RAII pooled device buffer
 // pb200_extract.cu: non-empty groups of the results' device tables -> final layout in pinned memory (all results at once)
 int extract_groups(pb200_ctx* ctx, pb200_result* const* results, int nres, cudaStream_t st);
 void result_materialize(pb200_result* R);  // view -> the std::vector fields
+// pb200_order_by checks shared by the device and host entry points: PB200_OK or PB200_E_INVALID (message set)
+int order_validate(const pb200_order_by* order, int num_aggs, int num_group_by);
+// Orders and trims a host-built group-by result (rows in its std::vector fields or view) by `order`; fns = PB200_AGG_* per
+// aggregation.  Same keys as the device sort (pb200_order.h); the result's rows end up in its std::vector fields.
+void order_rows_host(pb200_result* R, const pb200_order_by& order, const int32_t* fns);
 
 // pb200_roaring.cu
 // One serialized RoaringBitmap (posting list of one dictId) to be OR-ed into `mask` (1 bit per doc, bit j of 32-bit

@@ -227,7 +227,8 @@ def _combine_with_sets(backend, segments, query, dist, dst):
     columns are bound to one dictionary domain (global_domain) -- the caller's precondition, as for every cross-GPU merge."""
     import numpy as np
     from .plan_maker import ResultsBlock
-    block = backend.pm.execute_segments(segments, query, merge=True)[0]
+    # every group of every rank: a rank-level trim before this merge by key could drop a group of the global top rows
+    block = backend.pm.execute_segments(segments, query, merge=True, ordered=False)[0]
     fns = [a.function for a in query.aggregations]
     rows = 1 if block.num_groups < 0 else block.num_groups
     mine = {}

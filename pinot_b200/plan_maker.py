@@ -409,6 +409,23 @@ def _marshal_query(q: QueryContext, merge: bool, reduce_world: int = 0, no_count
     return hq, (c_nodes, c_lits, gb, gb_names, aggs, keep, c_agg_nodes, c_starts, c_counts)
 
 
+def order_spec(q: QueryContext, merge: bool):
+    """pb200_order_by of a GROUP BY query with an ORDER BY (None otherwise).  Trim: max(5 * LIMIT, option) rows when the
+    option (min_server_group_trim_size for a merged result, min_segment_group_trim_size per segment) is > 0, else sorted
+    without trimming -- Pinot's table capacity rule for the combine step."""
+    from .sql import resolve_order_by
+    if not q.is_group_by or not q.order_by:
+        return None
+    items = resolve_order_by(q)
+    if len(items) > _lib.MAX_ORDER_BY:
+        raise ValueError(f"ORDER BY has {len(items)} items, at most {_lib.MAX_ORDER_BY} are supported")
+    option = q.min_server_group_trim_size if merge else q.min_segment_group_trim_size
+    spec = _lib.OrderBy(len(items), max(5 * q.limit, option) if option > 0 else 0)
+    for i, (kind, index, asc) in enumerate(items):
+        spec.items[i] = _lib.OrderItem(_lib.ORDER_GROUP_BY if kind == "GROUP_BY" else _lib.ORDER_AGG, index, int(not asc))
+    return spec
+
+
 class _NativeResult:
     """Owner of a native pb200_result whose columns numpy arrays alias (views=True): freed with the block (or release())."""
 
@@ -565,11 +582,14 @@ class B200PlanMaker:
 
     def execute_segments(self, segments: Sequence[IndexSegment], query: QueryContext, merge: bool = False,
                          keep_handle: bool = False, reduce_world: int = 0, merged_docs_bound: int = 0,
-                         no_count_carrier: bool = False, defer: Optional[bool] = None, views: bool = False) -> List[ResultsBlock]:
+                         no_count_carrier: bool = False, defer: Optional[bool] = None, views: bool = False,
+                         ordered: bool = True) -> List[ResultsBlock]:
         """All segments of one query in ONE device submission (makeInstancePlan-level batching).  With merge=True the
         segments (sharing dictionaries) are combined on the device and one block is returned; with keep_handle=True as
         well, a group-by block comes back WITHOUT its groups extracted (PB200_Q_DEFER_FINALIZE): its dense device tables
-        are meant to be reduced across GPUs (pinot_b200.distributed.combine_across_ranks), which extracts on the root."""
+        are meant to be reduced across GPUs (pinot_b200.distributed.combine_across_ranks), which extracts on the root.
+        A GROUP BY query with an ORDER BY gets its rows ordered and trimmed by the library (order_spec; a deferred block
+        when it is extracted); ordered=False returns every group in the library's row order."""
         # merge + keep_handle: the caller reduces the dense tables across GPUs first; groups are extracted afterwards
         # defer=False with keep_handle=True: extracted blocks that keep their native handle (to_datatable); release() them
         if defer is None:
@@ -586,7 +606,11 @@ class B200PlanMaker:
         nres = 1 if merge else n
         res = (C.c_void_p * nres)()
         kinds = (C.c_int32 * n)()
-        _lib.check(self.ctx.lib.pb200h_execute(self.ctx.handle, C.byref(hq), segs, n, res, kinds))
+        spec = order_spec(query, merge) if ordered else None
+        if spec is None:
+            _lib.check(self.ctx.lib.pb200h_execute(self.ctx.handle, C.byref(hq), segs, n, res, kinds))
+        else:
+            _lib.check(self.ctx.lib.pb200h_execute_ordered(self.ctx.handle, C.byref(hq), C.byref(spec), segs, n, res, kinds))
         # views=True: the blocks' arrays alias the native results' pinned memory (no copy); keep the block alive while you
         # use them and drop it before the context closes
         blocks = [_read_result(self.ctx, C.c_void_p(res[i]), query, kinds[i if not merge else 0], keep_handle, views)

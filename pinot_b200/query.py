@@ -67,6 +67,10 @@ class QueryContext:
     max_initial_result_holder_capacity: int = DEFAULT_MAX_INITIAL_RESULT_HOLDER_CAPACITY
     and_scan_reordering: bool = False
     use_star_tree: bool = True  # query option useStarTree
+    # GROUP BY ... ORDER BY ... LIMIT n trims to max(5 * n, option) groups (option > 0; else no trim): the merged result
+    # (query options minServerGroupTrimSize, default 5000) and per-segment results (minSegmentGroupTrimSize, default off)
+    min_server_group_trim_size: int = 5000
+    min_segment_group_trim_size: int = -1
 
     @property
     def is_group_by(self) -> bool:

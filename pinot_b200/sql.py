@@ -153,6 +153,29 @@ class _Parser:
         raise SqlError(f"unsupported operator {op}")
 
 
+def resolve_order_by(query: QueryContext) -> List[tuple]:
+    """ORDER BY expressions -> [(kind, index, ascending)]: kind "GROUP_BY" indexes query.group_by, "AGG" indexes
+    query.aggregations (the first one the expression names).  Anything else is refused: ORDER BY on expressions or on
+    functions that are not in the SELECT list is outside this path."""
+    out = []
+    for expr, asc in query.order_by:
+        if expr in query.group_by:
+            out.append(("GROUP_BY", query.group_by.index(expr), asc))
+            continue
+        m = re.fullmatch(r"([A-Za-z_$][A-Za-z0-9_$]*)\((\*|[A-Za-z_$][A-Za-z0-9_$]*)\)", expr)
+        found = None
+        if m:
+            fn, col = m.group(1).upper(), m.group(2)
+            for a, agg in enumerate(query.aggregations):
+                if agg.function == fn and (fn == "COUNT" or agg.column == col):
+                    found = a
+                    break
+        if found is None:
+            raise SqlError(f"ORDER BY {expr}: neither a GROUP BY column nor an aggregation of the SELECT list")
+        out.append(("AGG", found, asc))
+    return out
+
+
 def parse(sql: str, **options) -> QueryContext:
     """SQL text -> QueryContext (filter already run through the broker-side filter optimizers)."""
     p = _Parser(sql)
@@ -219,5 +242,7 @@ def parse(sql: str, **options) -> QueryContext:
             raise SqlError(f"column {c} must appear in GROUP BY (selection queries are outside this path)")
     if not aggs:
         raise SqlError("only aggregation / group-by queries are on this path")
-    return QueryContext(aggregations=aggs, filter=optimize_filter(flt), group_by=group_by, table=table, limit=limit,
-                        order_by=order_by, **options)
+    query = QueryContext(aggregations=aggs, filter=optimize_filter(flt), group_by=group_by, table=table, limit=limit,
+                         order_by=order_by, **options)
+    resolve_order_by(query)
+    return query
