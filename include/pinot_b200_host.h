@@ -116,8 +116,11 @@ enum { PB200H_AND = 0, PB200H_OR = 1, PB200H_NOT = 2, PB200H_EQ = 3, PB200H_NEQ 
        PB200H_RANGE = 7 };
 
 typedef struct {
-  int64_t i;     /* INT / LONG columns */
-  double d;      /* FLOAT / DOUBLE columns */
+  /* `d`: every numeric literal rounded to double (FLOAT columns compare (float)d).  `i`: the literal when it is an
+     int64, so that (double)i == d; INT / LONG columns compare by exact value: `i` then, else a fractional `d` (no
+     integer equals it), else (an integral or infinite `d`) a literal beyond the int64 range on the side of d */
+  int64_t i;
+  double d;
   const char* s; /* STRING columns */
 } pb200h_literal;
 

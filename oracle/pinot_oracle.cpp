@@ -354,6 +354,16 @@ RawChunkHeader parse_raw_header(const uint8_t* b, int64_t len) {
   return h;
 }
 
+// INT / LONG value vs literal by exact numeric value (NumericalFilterOptimizer: a fractional literal equals no integer,
+// range bounds become ceil / floor, a literal beyond the column's range makes the predicate constant).  `d` is the
+// literal rounded to double, `i` the literal when it is an int64 ((double)i == d); otherwise a fractional `d` is the
+// literal and an integral or infinite one lies beyond int64 on its side.
+int cmp_integral(int64_t v, const po_literal_t& l) {
+  if ((double)l.i == l.d) return v < l.i ? -1 : v > l.i ? 1 : 0;
+  if (std::isfinite(l.d) && l.d != std::floor(l.d)) return (double)v < l.d ? -1 : 1;   // |d| < 2^52: rounding v keeps its side
+  return l.d > 0 ? -1 : 1;
+}
+
 struct Column {
   const po_column_t* c;
   RawChunkHeader raw;
@@ -436,8 +446,8 @@ struct Column {
       int mid = (lo + hi) >> 1;
       int cmp;
       switch (c->data_type) {
-        case PO_INT: { int64_t v = dict_int(mid); cmp = v < lit.i ? -1 : v > lit.i ? 1 : 0; break; }
-        case PO_LONG: { int64_t v = dict_long(mid); cmp = v < lit.i ? -1 : v > lit.i ? 1 : 0; break; }
+        case PO_INT: cmp = cmp_integral(dict_int(mid), lit); break;
+        case PO_LONG: cmp = cmp_integral(dict_long(mid), lit); break;
         case PO_FLOAT: { float v = dict_float(mid), t = (float)lit.d; cmp = v < t ? -1 : v > t ? 1 : 0; break; }
         case PO_DOUBLE: { double v = dict_double_raw(mid); cmp = v < lit.d ? -1 : v > lit.d ? 1 : 0; break; }
         default: { int r = dict_string(mid).compare(lit.s ? lit.s : ""); cmp = r < 0 ? -1 : r > 0 ? 1 : 0; }
@@ -445,6 +455,15 @@ struct Column {
       if (cmp < 0) lo = mid + 1; else if (cmp > 0) hi = mid - 1; else return mid;
     }
     return -(lo + 1);
+  }
+  // raw value at `doc` vs a literal in the column's type (the *RawValueBased*PredicateEvaluators): INT / LONG exact,
+  // FLOAT as float, DOUBLE as double
+  int raw_compare(int doc, const po_literal_t& lit) const {
+    switch (c->data_type) {
+      case PO_INT: case PO_LONG: return cmp_integral(raw_as_long(doc), lit);
+      case PO_FLOAT: { float v = (float)raw_as_double(doc), t = (float)lit.d; return v < t ? -1 : v > t ? 1 : 0; }
+      default: { double v = raw_as_double(doc); return v < lit.d ? -1 : v > lit.d ? 1 : 0; }
+    }
   }
   // BitmapInvertedIndexReader.getDocIds (seglocal/segment/index/readers/BitmapInvertedIndexReader.java:45-62)
   bool inverted_bitmap(int dict_id, const uint8_t** p, int64_t* len) const {
@@ -474,17 +493,18 @@ struct Predicate {
   int card = 0;
   // raw (no dictionary) numeric predicate
   bool raw = false;
-  double lo = 0, hi = 0; bool lo_inc = true, hi_inc = true, lo_unb = true, hi_unb = true;
-  std::vector<double> raw_values;
+  po_literal_t lo{}, hi{}; bool lo_inc = true, hi_inc = true, lo_unb = true, hi_unb = true;
+  std::vector<po_literal_t> raw_values;
 
   bool apply(int dict_id) const { return is_range ? (start <= dict_id && end > dict_id) : lut[dict_id] != 0; }
-  bool apply_raw(double v) const {
+  bool apply_raw(const Column& col, int doc) const {
     if (is_range) {
-      if (!lo_unb && (lo_inc ? v < lo : v <= lo)) return false;
-      if (!hi_unb && (hi_inc ? v > hi : v >= hi)) return false;
+      if (!lo_unb) { int c = col.raw_compare(doc, lo); if (lo_inc ? c < 0 : c <= 0) return false; }
+      if (!hi_unb) { int c = col.raw_compare(doc, hi); if (hi_inc ? c > 0 : c >= 0) return false; }
       return true;
     }
-    bool in = std::find(raw_values.begin(), raw_values.end(), v) != raw_values.end();
+    bool in = false;
+    for (const po_literal_t& l : raw_values) in |= col.raw_compare(doc, l) == 0;
     return exclusive ? !in : in;
   }
   int num_matching() const {  // getNumMatchingItems (negative for exclusive predicates)
@@ -500,10 +520,6 @@ struct Predicate {
   }
 };
 
-double lit_as_double(const Column& col, const po_literal_t& l) {
-  return (col.c->data_type == PO_INT || col.c->data_type == PO_LONG) ? (double)l.i : l.d;
-}
-
 Predicate make_predicate(const Column& col, const po_filter_node_t& n, const po_literal_t* lits) {
   Predicate p;
   p.type = n.type;
@@ -515,11 +531,11 @@ Predicate make_predicate(const Column& col, const po_filter_node_t& n, const po_
       p.is_range = true;
       p.lo_unb = n.lower_unbounded; p.hi_unb = n.upper_unbounded;
       p.lo_inc = n.lower_inclusive; p.hi_inc = n.upper_inclusive;
-      if (!p.lo_unb) p.lo = lit_as_double(col, v[0]);
-      if (!p.hi_unb) p.hi = lit_as_double(col, v[1]);
+      if (!p.lo_unb) p.lo = v[0];
+      if (!p.hi_unb) p.hi = v[1];
     } else {
       p.exclusive = n.type == PO_NEQ || n.type == PO_NOT_IN;
-      for (int i = 0; i < n.num_values; i++) p.raw_values.push_back(lit_as_double(col, v[i]));
+      for (int i = 0; i < n.num_values; i++) p.raw_values.push_back(v[i]);
     }
     return p;
   }
@@ -596,14 +612,14 @@ struct ScanIterator : DocIdIterator {
   int match_values(int limit, int* doc_ids) {  // DictIdMatcher.matchValues / raw matchers
     int m = 0;
     if (pred.raw) {
-      for (int i = 0; i < limit; i++) if (pred.apply_raw(col.raw_as_double(doc_ids[i]))) doc_ids[m++] = doc_ids[i];
+      for (int i = 0; i < limit; i++) if (pred.apply_raw(col, doc_ids[i])) doc_ids[m++] = doc_ids[i];
       return m;
     }
     col.read_dict_ids(num_docs, doc_ids, limit, dict_buf);
     for (int i = 0; i < limit; i++) if (pred.apply(dict_buf[i])) doc_ids[m++] = doc_ids[i];
     return m;
   }
-  bool does_match(int doc) { return pred.raw ? pred.apply_raw(col.raw_as_double(doc)) : pred.apply(col.get_dict_id(doc)); }
+  bool does_match(int doc) { return pred.raw ? pred.apply_raw(col, doc) : pred.apply(col.get_dict_id(doc)); }
   int next() override {
     if (cursor >= first_mismatch) {
       int limit, bs = 0;

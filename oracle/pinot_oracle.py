@@ -5,6 +5,7 @@ Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / ``--impl refe
 from __future__ import annotations
 
 import ctypes as C
+import math
 import os
 import subprocess
 from dataclasses import dataclass, field
@@ -281,10 +282,17 @@ class Oracle:
                 b = v.encode("utf-8") if isinstance(v, str) else bytes(v)
                 keep.append(b)
                 return _Literal(0, 0.0, b)
-            if col.data_type in (sb.INT, sb.LONG):
-                # NumericalFilterOptimizer semantics are the caller's business; tests use integral literals here
-                return _Literal(int(v), float(v), None)
-            return _Literal(0, float(v), None)
+            # d = the literal rounded to double, i = the literal when it is an int64 (else 0): INT / LONG compare by
+            # exact value (pinot_oracle.cpp cmp_integral)
+            if isinstance(v, (int, np.integer)):
+                iv = int(v)
+                try:
+                    d = float(iv)
+                except OverflowError:
+                    d = math.copysign(math.inf, iv)
+                return _Literal(iv if -(1 << 63) <= iv < (1 << 63) else 0, d, None)
+            d = float(v)
+            return _Literal(int(d) if d.is_integer() and -2.0 ** 63 <= d < 2.0 ** 63 else 0, d, None)
 
         def encode(node_list):
             out = []

@@ -17,6 +17,17 @@ using pb200::set_error;
 inline uint32_t hbe32(const unsigned char* p) { return (uint32_t)p[0] << 24 | (uint32_t)p[1] << 16 | (uint32_t)p[2] << 8 | p[3]; }
 inline uint64_t hbe64(const unsigned char* p) { return (uint64_t)hbe32(p) << 32 | hbe32(p + 4); }
 
+// Stored INT / LONG value vs a predicate literal, by exact numeric value (-1, 0, 1).  `d` is the literal rounded to
+// double; when it is an int64, `i` holds it exactly and (double)i == d.  Otherwise a fractional `d` is the literal
+// itself (it equals no integer) and an integral or infinite one lies beyond the int64 range on its side.  This is what
+// the reference's broker (NumericalFilterOptimizer) makes of `intCol >= 2.5` or `longCol < 1e19` before a server sees
+// them.
+inline int compare_integral(int64_t v, const pb200h_literal& l) {
+  if ((double)l.i == l.d) return v < l.i ? -1 : v > l.i;
+  if (std::isfinite(l.d) && l.d != std::floor(l.d)) return (double)v < l.d ? -1 : 1;   // |d| < 2^52: rounding v keeps its side
+  return l.d > 0 ? -1 : 1;
+}
+
 struct HostColumn {
   std::string name;
   int data_type = 0, has_dictionary = 0, bits = 0, cardinality = 0, is_sorted = 0, entry_bytes = 0;
@@ -57,8 +68,8 @@ struct HostColumn {
     while (lo <= hi) {
       int mid = (lo + hi) >> 1, cmp;
       switch (data_type) {
-        case PB200_INT: { int64_t v = get_int(mid); cmp = v < l.i ? -1 : v > l.i; break; }
-        case PB200_LONG: { int64_t v = get_long(mid); cmp = v < l.i ? -1 : v > l.i; break; }
+        case PB200_INT: cmp = compare_integral(get_int(mid), l); break;
+        case PB200_LONG: cmp = compare_integral(get_long(mid), l); break;
         case PB200_FLOAT: { float v = get_float(mid), t = (float)l.d; cmp = v < t ? -1 : v > t; break; }
         case PB200_DOUBLE: { double v = get_double(mid); cmp = v < l.d ? -1 : v > l.d; break; }
         default: { int r = get_string(mid).compare(l.s ? l.s : ""); cmp = r < 0 ? -1 : r > 0; }

@@ -67,11 +67,15 @@ bool raw_leaf(const HostColumn& c, const pb200h_filter_node& n, const pb200h_lit
   const pb200h_literal* v = lits + n.values_offset;
   if (n.type == PB200H_RANGE) {
     d.op = PB200_F_RAW_RANGE;
-    d.raw_lo = n.lower_unbounded ? 0.0 : (double)v[0].i; d.raw_hi = n.upper_unbounded ? 0.0 : (double)v[1].i;
+    // the literals' doubles: fractional bounds reach pb200_execute as they are (it takes ceil / floor), and every int32
+    // bound is exact (compare_integral)
+    d.raw_lo = n.lower_unbounded ? 0.0 : v[0].d;
+    d.raw_hi = n.upper_unbounded ? 0.0 : v[1].d;
     d.raw_flags = (n.lower_unbounded ? 1 : 0) | (n.upper_unbounded ? 2 : 0) | (n.lower_inclusive ? 0 : 4) | (n.upper_inclusive ? 0 : 8);
     return true;
   }
-  if (n.type == PB200H_EQ) { d.op = PB200_F_RAW_RANGE; d.raw_lo = d.raw_hi = (double)v[0].i; d.raw_flags = 0; return true; }
+  // EQ with a fractional literal: [ceil, floor] is empty
+  if (n.type == PB200H_EQ) { d.op = PB200_F_RAW_RANGE; d.raw_lo = d.raw_hi = v[0].d; d.raw_flags = 0; return true; }
   return false;
 }
 

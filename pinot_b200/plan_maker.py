@@ -16,6 +16,7 @@ marshals.  There is no CPU fallback: queries outside the accelerated set raise `
 from __future__ import annotations
 
 import ctypes as C
+import math
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional, Sequence, Tuple
 
@@ -338,6 +339,24 @@ class ResultsBlock:
         return out
 
 
+INT64_MIN, INT64_MAX = -(1 << 63), (1 << 63) - 1
+
+
+def numeric_literal(v) -> Tuple[int, float]:
+    """(i, d) of pb200h_literal for a number: d = the literal rounded to double, i = the literal when it is an int64 (so
+    (double)i == d), else 0 -- the host then compares INT / LONG values with the fraction `d` or knows the literal lies
+    beyond int64 (a ctypes int64 field would wrap it silently)."""
+    if isinstance(v, (int, np.integer)):
+        v = int(v)
+        try:
+            d = float(v)
+        except OverflowError:
+            d = math.copysign(math.inf, v)
+        return (v if INT64_MIN <= v <= INT64_MAX else 0), d
+    d = float(v)
+    return (int(d) if d.is_integer() and INT64_MIN <= d < 2.0 ** 63 else 0), d
+
+
 def _marshal_query(q: QueryContext, merge: bool, reduce_world: int = 0, no_count_carrier: bool = False,
                    merged_docs_bound: int = 0):
     nodes = postfix(q.filter)
@@ -352,8 +371,7 @@ def _marshal_query(q: QueryContext, merge: bool, reduce_world: int = 0, no_count
         if isinstance(v, bytes):
             keep.append(v)
             return _lib.HLiteral(0, 0.0, v)
-        iv = int(v) if float(v).is_integer() else int(np.floor(v))
-        return _lib.HLiteral(iv, float(v), None)
+        return _lib.HLiteral(*numeric_literal(v), None)
 
     def encode(node_list):
         out = []
