@@ -12,7 +12,7 @@
 // A raw INT entry's emptiness is never read from the entry: the group's count, seen flag, carrier or hash key tells
 // (max_offset in pb200_desc.h).  Both stay neutral elements of their reduce, so the reduces are the same for both kinds.
 // pb200_result_combine issues ALL of a result's reduces as ONE NCCL group on the context's stream, reads the carrier verdict
-// that rides behind the int64 block (pb200_api.cu), and lets the root extract the groups -- one library call per rank and
+// that rides behind the int64 block (pb200_plan.cpp), and lets the root extract the groups -- one library call per rank and
 // query instead of four Python-driven collectives, a tensor-alias step and a second call for the extraction.
 //
 // NCCL is bound at RUN time (dlopen "libnccl.so.2"): the library loads and every single-GPU entry point works on a box

@@ -1,4 +1,4 @@
-// pb200_desc.h -- launch descriptors shared by the host planner (pb200_api.cu) and the scan kernels.
+// pb200_desc.h -- launch descriptors shared by the host planner (pb200_plan.cpp), the launch (pb200_api.cu) and the scan kernels.
 #pragma once
 #include <cstdint>
 
@@ -113,7 +113,7 @@ struct SegDesc {
   unsigned long long group_mult64[kMaxGroupBy];
   // group-by SUM / AVG over an INT dictionary: the 64-bit value added to the table is (zero-extended biased dictionary
   // word) + sum_addend[a].  Plain sums: -2^31 (removes the bias).  The sum that CARRIES the row count of its group
-  // (pb200_api.cu "count carrier"): 2^shift - biased(min value), i.e. one reduction adds (value - min) to the low `shift`
+  // (pb200_plan.cpp "count carrier"): 2^shift - biased(min value), i.e. one reduction adds (value - min) to the low `shift`
   // bits and 1 to the bits above them -- the separate COUNT reduction (an L2 read-modify-write per surviving row) is gone.
   unsigned long long sum_addend[kMaxAggs];
 };

@@ -43,7 +43,7 @@ struct ExtractDesc {
   const uint32_t* maxk;              // dictionary MIN / MAX tables only (a raw INT entry has no empty value)
   const uint32_t* mink;
   const unsigned long long* hkeys;
-  const unsigned long long* packed;  // count-carrying sum table (pb200_api.cu): sum(value - vmin) + count << shift
+  const unsigned long long* packed;  // count-carrying sum table (pb200_plan.cpp): sum(value - vmin) + count << shift
   long long pack_vmin;
   int32_t pack_agg, pack_shift;
   long long groups;                  // table entries (dense: raw key space x stride, hash: capacity)

@@ -27,6 +27,8 @@ void set_error(const char* fmt, ...);
 // Upper bound of the scan kernel's tile (consumer warps x 1024 rows).  Forward indexes are padded so that whole tiles
 // of any size up to this can be streamed.
 constexpr int kMaxTileRows = 8192;
+// words a device doc mask needs: whole tiles + one spare tile (the kernel reads masks tile-wise) + a tail
+inline size_t doc_mask_words(long long num_docs) { return (((size_t)num_docs + kMaxTileRows - 1) / kMaxTileRows + 1) * (kMaxTileRows / 32) + 8; }
 
 struct DeviceColumn {
   int fwd_kind = 0, stored_type = 0, bits = 0, cardinality = 0;
@@ -52,11 +54,12 @@ struct DeviceColumn {
 
 namespace pb200 {
 // Tuning knobs of the scan kernel launch.  Read from the environment ONCE, at pb200_init (PB200_W, PB200_CTAS, ... --
-// DESIGN.md section 3.1), changeable afterwards with pb200_tuning_set(); pb200_execute itself never calls getenv.
+// DESIGN.md section 3.1), changeable afterwards with pb200_tuning_set(); read by the scan planner (plan_scan,
+// pb200_plan.cpp), which pb200_execute calls with a copy taken under the context's lock -- neither calls getenv.
 struct Tuning {
   int warps = 6;                 // PB200_W: 6 | 8 warps per CTA
   int sparse_max = 4;            // PB200_SPARSE_MAX
-  int sparse_max_agg = -1;       // PB200_SPARSE_MAX_AGG (-1: rule in pb200_execute)
+  int sparse_max_agg = -1;       // PB200_SPARSE_MAX_AGG (-1: rule in plan_scan)
   int ctas_per_sm = 2;           // PB200_CTAS
   int stages = 0;                // PB200_STAGES (0: as many as fit)
   int grid = 0;                  // PB200_GRID (0: SMs x CTAs per SM)
@@ -66,7 +69,7 @@ struct Tuning {
   long long dense_max = 1ll << 24;   // PB200_DENSE_MAX: dense group table up to this many raw keys, hash table beyond
   int defer = 1;                 // !PB200_NO_DEFER: software-pipelined gathers, aggregation-only kernel
   int gb_defer = 1;              // !PB200_NO_GB_DEFER: software-pipelined last queue batch, group-by kernel
-  int pack_count = 1;            // !PB200_NO_PACK_COUNT: group-by COUNT carried inside an INT SUM's reductions (pb200_api.cu)
+  int pack_count = 1;            // !PB200_NO_PACK_COUNT: group-by COUNT carried inside an INT SUM's reductions (pb200_plan.cpp)
   int table_stride = 0;          // PB200_TABLE_STRIDE: dense group tables hold raw key k at k * stride (0 = auto, 1 = off)
   int pack_shift = 0;            // PB200_PACK_SHIFT: force the carrier's count shift (tests of the overflow fallback); 0 = from the doc count
   int skip = 1;                  // !PB200_NO_SKIP: bitmap-driven slice skipping
@@ -151,13 +154,13 @@ struct pb200_result {
   struct Dense {
     pb200_ctx* ctx = nullptr;
     long long groups = 0;                        // table entries: dense key space x stride, or hash capacity
-    int stride = 1;                              // dense tables: raw key k lives at entry k * stride (pb200_api.cu)
+    int stride = 1;                              // dense tables: raw key k lives at entry k * stride (pb200_plan.cpp)
     bool live = false;                           // device tables still allocated
     unsigned long long* count = nullptr;         // NULL when no COUNT / AVG
     uint32_t* seen = nullptr;                    // group-exists flags (inside the u32max block) or NULL
     uint32_t* exists_max = nullptr;              // a MAX table doubling as the group-exists marker, or NULL
     uint32_t* exists_min = nullptr;              // a MIN table doubling as the group-exists marker, or NULL
-    // count carrier (pb200_api.cu): aggregation pack_agg's int64 table holds  sum(value - pack_vmin) + count << pack_shift
+    // count carrier (pb200_plan.cpp): aggregation pack_agg's int64 table holds  sum(value - pack_vmin) + count << pack_shift
     int pack_agg = -1, pack_shift = 0;
     long long pack_vmin = 0;
     const unsigned long long* exists_packed = nullptr;  // that table: non-zero <=> the group exists

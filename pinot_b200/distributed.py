@@ -160,7 +160,7 @@ class DeviceBackend:
 def combine_tables(backend, block, query, dist, dst: int = 0):
     """All ranks call this with their merged, unextracted block: reduce of the tables to `dst`, which extracts the groups.
 
-    Count-carrying sums ("count carrier", pb200_api.cu: the per-group row count rides in the upper bits of an INT sum)
+    Count-carrying sums ("count carrier", pb200_plan.cpp: the per-group row count rides in the upper bits of an INT sum)
     add field by field in the same int64 reduce; whether that is safe is decided per rank BEFORE the reduce (the rank's
     largest sum field must leave room for the other ranks': block.carrier_unsafe) and agreed on with one 4-byte MAX
     all-reduce that travels with the tables.  Returns (result or None, retry): retry == True on EVERY rank iff some rank

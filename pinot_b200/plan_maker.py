@@ -308,7 +308,7 @@ class ResultsBlock:
     device_ms: float = 0.0
     operator_kind: str = "AGGREGATION"
     handle: Optional[C.c_void_p] = None  # kept only for merged results (multi-GPU combine)
-    count_carrier: bool = False  # the per-group row counts rode in an INT sum's reductions (pb200_api.cu)
+    count_carrier: bool = False  # the per-group row counts rode in an INT sum's reductions (pb200_plan.cpp)
     carrier_unsafe: bool = False  # deferred result: that sum may overflow in the cross-GPU reduce, rerun without carrier
     flag_slot: bool = False  # the int64 table block ends with this rank's unsafe verdict: all-reduce it with the tables
 

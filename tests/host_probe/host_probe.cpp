@@ -2,12 +2,14 @@
 // CPU test suite can compare it with the oracle:
 //   * pb200h::StarTree::parse / traverse   (StarTreeFilterOperator's traversal as the product runs it)
 //   * pb200h::matching_dict_ids             (PredicateEvaluator resolution: value-space predicate -> dictIds)
+//   * pb200::plan_scan                       (every decision about a scan launch, on segments built from metadata)
 // Built by tests/test_host_logic_cpu.py with g++ against the in-tree library; nothing here ships.
 #include <cstdint>
 #include <cstring>
 #include <vector>
 
 #include "../../pinot_b200/csrc/host/host_internal.h"
+#include "../../pinot_b200/csrc/pb200_plan.h"
 
 extern "C" {
 
@@ -116,6 +118,115 @@ int32_t probe_synthesize_dictionary(const unsigned char* values_be, int32_t data
   memcpy(fwd_out, fwd.data(), fwd.size());
   *cardinality = card; *bits = nb;
   return 1;
+}
+
+// ---- pb200::plan_scan over segments made of column metadata alone (no device memory: resident pointers are sentinels) ----
+typedef struct {
+  int32_t fwd_kind, stored_type, bits, cardinality;
+  int32_t dict_native;        // 1: the column has a device dictionary (a sentinel pointer, never dereferenced)
+  int32_t dict_shared;        // dictionary of a bound domain
+  int32_t has_inv;            // an inverted index whose every dictId has a non-empty posting list
+  int32_t reserved;
+  uint64_t dict_hash;
+  const void* dict_host;      // native little-endian dictionary values (INT: 4 bytes each), or NULL
+  uint64_t dict_host_bytes;
+} probe_col;
+
+enum { PP_RES = 40, PP_SEG = 40, PP_CHUNK = 4 };
+typedef struct {  // every field int64: tests/test_scan_plan_cpu.py mirrors this list
+  int64_t warps, ctas_per_sm, stages, stage_words, tile_rows, smem_bytes, queue_off, smem_table_off, queue_max;
+  int64_t sparse_max, sparse_max_agg, defer_agg, conj, num_slots, num_leaves, num_nodes, use_pipe;
+  int64_t smem_groups, smem_copies, smem_gstride, smem_count, smem_merged, smem_slot[pb200::kMaxAggs];
+  int64_t variant[4];  // warps, group_by, defer, min_blocks
+  int64_t num_chunks, chunk_first_seg[PP_CHUNK], chunk_num_segs[PP_CHUNK], chunk_total_tiles[PP_CHUNK], chunk_grid[PP_CHUNK];
+  int64_t nres, projected, num_leaf_buffers, in_filter[PP_RES];
+  int64_t hashed[PP_RES], groups[PP_RES], stride[PP_RES], carrier_agg[PP_RES], carrier_shift[PP_RES], carrier_vmin[PP_RES];
+  int64_t need_count[PP_RES], need_seen[PP_RES], exists_min[PP_RES], exists_max[PP_RES], reduce_world[PP_RES];
+  int64_t flag_slot[PP_RES], tail_slots[PP_RES], i64_elems[PP_RES], f64_elems[PP_RES], u32max_elems[PP_RES], u32min_elems[PP_RES];
+  int64_t dwords[PP_RES * pb200::kMaxAggs], distinct_words[PP_RES * pb200::kMaxAggs];
+  int64_t seg_first_tile[PP_SEG], seg_num_tiles[PP_SEG], seg_stage_tx[PP_SEG], seg_num_agg_codes[PP_SEG], seg_num_defer_codes[PP_SEG];
+  int64_t seg_agg_code[PP_SEG * pb200::kMaxAggs];
+  int64_t seg_leaf_kind[PP_SEG * pb200::kMaxLeaves], seg_leaf_cmp[PP_SEG * pb200::kMaxLeaves], seg_leaf_negate[PP_SEG * pb200::kMaxLeaves];
+  int64_t seg_leaf_lo[PP_SEG * pb200::kMaxLeaves], seg_leaf_span[PP_SEG * pb200::kMaxLeaves], seg_leaf_slot[PP_SEG * pb200::kMaxLeaves];
+} probe_plan;
+
+int64_t probe_plan_size(void) { return (int64_t)sizeof(probe_plan); }
+
+// cols: nseg x ncols; knobs: nknobs pb200_tuning_set (name, value) pairs.  Returns plan_scan's status.
+int32_t probe_plan_scan(int32_t sm_count, int32_t max_smem_optin, const char* const* knob_names, const int64_t* knob_values,
+                        int32_t nknobs, const pb200_query* query, const probe_col* cols, int32_t ncols, const int32_t* num_docs,
+                        int32_t nseg, int32_t allow_count_carrier, probe_plan* out) {
+  using namespace pb200;
+  pb200_ctx ctx;
+  for (int i = 0; i < nknobs; i++) if (int rc = pb200_tuning_set(&ctx, knob_names[i], knob_values[i])) return rc;
+  static uint32_t sentinel[4];
+  std::vector<pb200_segment> segs(nseg);
+  std::vector<pb200_segment*> ptrs(nseg);
+  for (int s = 0; s < nseg; s++) {
+    segs[s].num_docs = num_docs[s];
+    segs[s].cols.resize(ncols);
+    for (int k = 0; k < ncols; k++) {
+      const probe_col& p = cols[(size_t)s * ncols + k];
+      DeviceColumn& c = segs[s].cols[k];
+      c.fwd_kind = p.fwd_kind; c.stored_type = p.stored_type; c.bits = p.bits; c.cardinality = p.cardinality;
+      c.fwd = sentinel;
+      c.dict_native = p.dict_native ? sentinel : nullptr;
+      c.dict_shared = p.dict_shared != 0;
+      c.dict_hash = p.dict_hash;
+      if (p.dict_host) c.dict_host.assign((const unsigned char*)p.dict_host, (const unsigned char*)p.dict_host + p.dict_host_bytes);
+      if (p.has_inv) {
+        c.inv = (unsigned char*)sentinel;
+        for (int id = 0; id <= c.cardinality; id++) c.inv_offsets.push_back(4u * (c.cardinality + 1) + 8u * id);
+      }
+    }
+    ptrs[s] = &segs[s];
+  }
+  ScanPlan plan;
+  const int rc = plan_scan(ctx.tune, DeviceLimits{sm_count, max_smem_optin}, query, ptrs.data(), nseg, allow_count_carrier != 0, &plan);
+  memset(out, 0, sizeof *out);
+  if (rc) return rc;
+  const QueryDesc& q = plan.q;
+  probe_plan& o = *out;
+  o.warps = plan.warps; o.ctas_per_sm = plan.ctas_per_sm; o.stages = q.num_stages; o.stage_words = q.stage_words;
+  o.tile_rows = q.tile_rows; o.smem_bytes = (int64_t)plan.smem_bytes; o.queue_off = q.queue_off; o.smem_table_off = q.smem_table_off;
+  o.queue_max = q.queue_max; o.sparse_max = q.sparse_max; o.sparse_max_agg = q.sparse_max_agg; o.defer_agg = q.defer_agg;
+  o.conj = q.conj; o.num_slots = q.num_slots; o.num_leaves = q.num_leaves; o.num_nodes = q.num_nodes; o.use_pipe = q.use_pipe;
+  o.smem_groups = q.smem_groups; o.smem_copies = q.smem_copies; o.smem_gstride = q.smem_gstride; o.smem_count = q.smem_count;
+  o.smem_merged = q.smem_merged;
+  for (int a = 0; a < kMaxAggs; a++) o.smem_slot[a] = q.smem_slot[a];
+  o.variant[0] = plan.variant.warps; o.variant[1] = plan.variant.group_by; o.variant[2] = plan.variant.defer; o.variant[3] = plan.variant.min_blocks;
+  o.num_chunks = (int64_t)plan.chunks.size();
+  for (size_t c = 0; c < plan.chunks.size() && c < PP_CHUNK; c++) {
+    o.chunk_first_seg[c] = plan.chunks[c].first_seg; o.chunk_num_segs[c] = plan.chunks[c].num_segs;
+    o.chunk_total_tiles[c] = plan.chunks[c].total_tiles; o.chunk_grid[c] = plan.chunks[c].grid;
+  }
+  o.nres = plan.nres; o.projected = plan.projected; o.num_leaf_buffers = (int64_t)plan.leaf_buffers.size();
+  for (int r = 0; r < plan.nres && r < PP_RES; r++) {
+    o.in_filter[r] = plan.in_filter[r];
+    for (int a = 0; a < kMaxAggs && !plan.distinct_words.empty() && a < (int)plan.distinct_words[r].size(); a++)
+      o.distinct_words[r * kMaxAggs + a] = (int64_t)plan.distinct_words[r][a];
+    if (plan.tables.empty()) continue;
+    const TableLayout& t = plan.tables[r];
+    o.hashed[r] = t.hashed; o.groups[r] = t.groups; o.stride[r] = t.stride; o.carrier_agg[r] = t.carrier.agg;
+    o.carrier_shift[r] = t.carrier.shift; o.carrier_vmin[r] = t.carrier.vmin; o.need_count[r] = t.need_count;
+    o.need_seen[r] = t.need_seen; o.exists_min[r] = t.exists_min; o.exists_max[r] = t.exists_max; o.reduce_world[r] = t.reduce_world;
+    o.flag_slot[r] = t.flag_slot; o.tail_slots[r] = t.tail_slots; o.i64_elems[r] = t.i64_elems; o.f64_elems[r] = t.f64_elems;
+    o.u32max_elems[r] = t.u32max_elems; o.u32min_elems[r] = t.u32min_elems;
+    for (int a = 0; a < kMaxAggs; a++) o.dwords[r * kMaxAggs + a] = t.dwords[a];
+  }
+  for (int s = 0; s < nseg && s < PP_SEG; s++) {
+    const SegDesc& sd = plan.segs[s];
+    o.seg_first_tile[s] = sd.first_tile; o.seg_num_tiles[s] = sd.num_tiles; o.seg_stage_tx[s] = sd.stage_tx;
+    o.seg_num_agg_codes[s] = sd.num_agg_codes; o.seg_num_defer_codes[s] = sd.num_defer_codes;
+    for (int a = 0; a < kMaxAggs; a++) o.seg_agg_code[s * kMaxAggs + a] = sd.agg_code[a];
+    for (int l = 0; l < kMaxLeaves; l++) {
+      const LeafDesc& lf = sd.leaves[l];
+      o.seg_leaf_kind[s * kMaxLeaves + l] = lf.kind; o.seg_leaf_cmp[s * kMaxLeaves + l] = lf.cmp;
+      o.seg_leaf_negate[s * kMaxLeaves + l] = lf.negate; o.seg_leaf_lo[s * kMaxLeaves + l] = lf.lo;
+      o.seg_leaf_span[s * kMaxLeaves + l] = lf.span; o.seg_leaf_slot[s * kMaxLeaves + l] = lf.slot;
+    }
+  }
+  return PB200_OK;
 }
 
 }  // extern "C"

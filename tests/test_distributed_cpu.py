@@ -80,7 +80,7 @@ class OracleBackend:
         carrier = -1
         if not no_count_carrier and (need_count or not has_minmax):
             carrier = next((a for a, ag in enumerate(query.aggregations) if ag.function in ("SUM", "AVG")), -1)
-        # the library's field sizing (pb200_api.cu "count carrier"): balanced fields from the dictionary's value range
+        # the library's field sizing (pb200_plan.cpp "count carrier"): balanced fields from the dictionary's value range
         dv = segments[0].column(query.aggregations[carrier].column).dict_values if carrier >= 0 else np.zeros(1, dtype=np.int64)
         vmin, rbits = int(dv.min()), int(int(dv.max()) - int(dv.min())).bit_length()
         shift = self.force_shift or (64 + rbits + 1) // 2

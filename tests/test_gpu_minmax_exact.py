@@ -12,7 +12,7 @@ values at the extremes of their types:
   matches), so the kernel runs and the small segments come back without a row.
 
 Each route is forced with pb200_tuning_set (tuned() restores the knob).  Every docstring names the host rule in
-pinot_b200/csrc/pb200_api.cu (pb200_execute) that picks the route.  Segment sizes cover ragged tails and the tile edges
+pinot_b200/csrc/pb200_plan.cpp (plan_scan) that picks the route.  Segment sizes cover ragged tails and the tile edges
 of both CTA widths (6 x 1024 and 8 x 1024 rows).  For dictionary columns the C-ABI dictId of every MIN / MAX must be the
 id of the reference's value."""
 import numpy as np

@@ -4,7 +4,7 @@ whose shared-table low word wraps many times, mixed signs whose group totals lan
 above 2^53, the count carrier with a negative minimum over the full 32-bit range, and a carrier entry that wraps to zero.
 
 Each route is forced with pb200_tuning_set and the knob is restored in a `finally`.  Every docstring names the host rule in
-pinot_b200/csrc/pb200_api.cu (pb200_execute) that sends the query down that route.  Segment sizes cover ragged tails and
+pinot_b200/csrc/pb200_plan.cpp (plan_scan) that sends the query down that route.  Segment sizes cover ragged tails and
 the tile edges of both CTA widths (6 x 1024 and 8 x 1024 rows)."""
 import numpy as np
 import pytest
