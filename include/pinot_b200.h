@@ -255,6 +255,48 @@ typedef struct {
 int32_t pb200_execute_ordered(pb200_ctx* ctx, const pb200_query* query, const pb200_order_by* order,
                               pb200_segment* const* segments, int32_t num_segments, pb200_result** results);
 
+/* ---- selection: SELECT columns WHERE ... [ORDER BY columns] LIMIT n (SelectionOnlyOperator, SelectionOrderByOperator) -- */
+/* Without order items: per segment, the first `limit` matching docs in doc-id order with the values of the selected
+ * columns.  With PB200_Q_MERGE_SEGMENTS one result: the segments are taken in submission order and each contributes a
+ * doc-order prefix of its matches (one of the outcomes the reference's selection-only combine can produce).
+ * With order items: per segment, the top `limit` rows by the order columns' values, ties by doc id ascending (the
+ * reference keeps the lower doc ids among equal keys); merged, the segments' tops are merged by value with ties broken by
+ * (segment index in the submission, doc id).  Value order: dictionary order (dictId order inside a segment, value order
+ * across segments; STRING: the dictionary's byte order), numeric order for raw INT / FLOAT columns; NaN and -0.0 are out
+ * of scope.  Order columns need not be selected.
+ * Columns may have different dictionaries in different segments.  A selected column comes back typed: INT / LONG / STRING
+ * as int64 (STRING: the dictId, looked up in the dictionary of the row's segment), FLOAT / DOUBLE as double; raw INT /
+ * FLOAT columns read their 32-bit values.  limit 0 returns no rows, only the statistics; limit above
+ * PB200_MAX_SELECT_LIMIT, or more than 65 535 segments, is PB200_E_UNSUPPORTED; more than PB200_MAX_ORDER_BY order items
+ * is PB200_E_INVALID.
+ * Statistics (device semantics): num_docs_scanned = matched docs in the doc range that was scanned.  Without ORDER BY a
+ * segment is first scanned over a prefix of whole tiles (at least 2^20 docs); only where that prefix holds fewer than
+ * `limit` matches is the whole segment scanned, and then the whole segment is the scanned range.  With ORDER BY every doc
+ * is scanned.  num_entries_scanned_in_filter = scanned docs x scan leaves; num_entries_scanned_post_filter = rows x
+ * num_columns.  device_ms = the scan launches; pb200_last_phases gives the host time of the scan and select phases. */
+#define PB200_MAX_SELECT_LIMIT 1000000
+typedef struct {
+  int32_t column;     /* column id */
+  int32_t descending; /* 0: ASC, else DESC */
+} pb200_select_order;
+typedef struct {
+  int32_t num_columns;
+  const int32_t* columns;   /* column ids, in output order */
+  int32_t num_order_items;  /* 0 .. PB200_MAX_ORDER_BY */
+  pb200_select_order order[PB200_MAX_ORDER_BY];
+  int64_t limit;            /* 0 .. PB200_MAX_SELECT_LIMIT */
+} pb200_selection;
+/* filter_only: the filter part of a pb200_query (num_filter_nodes, filter, PB200_Q_PER_SEGMENT_FILTER in its flags; its
+ * group-by and aggregation fields are ignored).  flags: PB200_Q_MERGE_SEGMENTS or 0.  Writes num_segments results (one
+ * when merged). */
+int32_t pb200_execute_selection(pb200_ctx* ctx, const pb200_query* filter_only, const pb200_selection* selection,
+                                pb200_segment* const* segments, int32_t num_segments, int32_t flags, pb200_result** results);
+/* The rows of a selection result: doc ids and the index (in the submission) of each row's segment, and per selected
+ * column a pointer to `rows` int64 or double values (see pb200_execute_selection).  Any output may be NULL; columns
+ * receives num_columns pointers.  Valid until pb200_result_free(result).  PB200_E_INVALID for other results. */
+int32_t pb200_result_selection(const pb200_result* result, int64_t* rows, const int32_t** doc_ids,
+                               const int32_t** segment_index, const void** columns);
+
 /* ---- results (the data a GroupByResultsBlock / AggregationResultsBlock is built from) ---------------------------- */
 enum { PB200_REGIME_NONE = 0, PB200_REGIME_ARRAY = 1, PB200_REGIME_INT_MAP = 2, PB200_REGIME_LONG_MAP = 3,
        PB200_REGIME_ARRAY_MAP = 4 };

@@ -186,6 +186,26 @@ int32_t pb200h_execute(pb200_ctx* ctx, const pb200h_query* query, pb200h_segment
 int32_t pb200h_execute_ordered(pb200_ctx* ctx, const pb200h_query* query, const pb200_order_by* order,
                                pb200h_segment* const* segments, int32_t num_segments, pb200_result** results,
                                int32_t* operator_kinds);
+/* ---- selection (SELECT columns WHERE ... LIMIT n; pb200_execute_selection of include/pinot_b200.h) --------------- */
+typedef struct {
+  const char* column;
+  int32_t descending;
+} pb200h_select_order;
+typedef struct {
+  int32_t num_columns;
+  const char* const* columns;  /* by name, in output order (SELECT * is resolved by the caller) */
+  int32_t num_order_items;     /* 0 .. PB200_MAX_ORDER_BY (order columns need not be selected) */
+  pb200h_select_order order[PB200_MAX_ORDER_BY];
+  int64_t limit;
+} pb200h_selection;
+/* The filter and merge_segments of `query` (its group-by and aggregation fields are ignored) with the rows of `selection`
+ * (ORDER BY semantics: pb200_execute_selection; a merged ORDER BY merges the segments' tops by value).
+ * Predicates are resolved per segment like pb200h_execute; a segment whose filter folds to EMPTY is never scanned (its
+ * result has no rows; merged: it contributes none), star-trees are never used.  results[] receives num_segments
+ * handles (one when merge_segments); read them with pb200_result_selection -- segment_index refers to `segments`. */
+int32_t pb200h_execute_selection(pb200_ctx* ctx, const pb200h_query* query, const pb200h_selection* selection,
+                                 pb200h_segment* const* segments, int32_t num_segments, pb200_result** results);
+
 /* The result as the server -> broker wire format: DataTableImplV4 bytes (pinot-common/.../datatable/DataTableImplV4.java:49-81)
  * exactly as GroupByResultsBlock.getDataTable() / AggregationResultsBlock.getDataTable() build them for the same rows
  * (GroupByResultsBlock.java:186-236): typed group-key values (STRING keys through the DataTable's own string dictionary),

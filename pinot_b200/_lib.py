@@ -119,6 +119,27 @@ class OrderBy(C.Structure):
     _fields_ = [("num_items", C.c_int32), ("trim_size", C.c_int32), ("items", OrderItem * MAX_ORDER_BY)]
 
 
+class SelectOrder(C.Structure):
+    _fields_ = [("column", C.c_int32), ("descending", C.c_int32)]
+
+
+class Selection(C.Structure):
+    _fields_ = [("num_columns", C.c_int32), ("columns", C.POINTER(C.c_int32)), ("num_order_items", C.c_int32),
+                ("order", SelectOrder * MAX_ORDER_BY), ("limit", C.c_int64)]
+
+
+class HSelectOrder(C.Structure):
+    _fields_ = [("column", C.c_char_p), ("descending", C.c_int32)]
+
+
+class HSelection(C.Structure):
+    _fields_ = [("num_columns", C.c_int32), ("columns", C.POINTER(C.c_char_p)), ("num_order_items", C.c_int32),
+                ("order", HSelectOrder * MAX_ORDER_BY), ("limit", C.c_int64)]
+
+
+MAX_SELECT_LIMIT = 1_000_000
+
+
 class HStarMetric(C.Structure):
     _fields_ = [("function", C.c_int32), ("reserved", C.c_int32), ("column", C.c_char_p), ("fwd", C.c_void_p),
                 ("fwd_bytes", C.c_uint64)]
@@ -140,6 +161,7 @@ EXPORTED_SYMBOLS = [
     "pb200_domain_create", "pb200_domain_from_segments", "pb200_domain_column_info", "pb200_domain_dictionary",
     "pb200_domain_release", "pb200_segment_bind_domain", "pb200_segment_local_ids",
     "pb200_last_phases", "pb200_result_columns", "pb200_doc_mask_upload", "pb200_doc_mask_free", "pb200_roaring_validate", "pb200_comm_unique_id", "pb200_comm_init", "pb200_comm_shutdown", "pb200_result_combine",
+    "pb200_execute_selection", "pb200_result_selection", "pb200h_execute_selection",
 ]
 
 _LIB = None
@@ -198,6 +220,9 @@ def load() -> C.CDLL:
     L.pb200h_explain.argtypes = [vp, C.POINTER(HQuery), vp, C.c_char_p, i32]
     L.pb200h_startree_attach.argtypes = [vp, vp, vp, C.c_uint64, i32, i32, C.POINTER(C.c_char_p), C.POINTER(vp),
                                          C.POINTER(C.c_uint64), i32, C.POINTER(HStarMetric)]
+    L.pb200_execute_selection.argtypes = [vp, C.POINTER(Query), C.POINTER(Selection), C.POINTER(vp), i32, i32, C.POINTER(vp)]
+    L.pb200_result_selection.argtypes = [vp, C.POINTER(i64), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]
+    L.pb200h_execute_selection.argtypes = [vp, C.POINTER(HQuery), C.POINTER(HSelection), C.POINTER(vp), i32, C.POINTER(vp)]
     L.pb200_result_columns.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]
     L.pb200_roaring_validate.argtypes = [vp, C.c_uint64, C.c_int64]
     L.pb200_doc_mask_upload.argtypes = [vp, i32, vp, C.c_int64, C.POINTER(vp)]

@@ -106,6 +106,8 @@ def main(argv=None) -> int:
     from ._lib import Pb200Error
     from .plan_maker import B200Context, B200PlanMaker, DictionaryDomain, IndexSegment
 
+    if sql.is_selection(args.sql):
+        return _selection(args, sql.parse_selection(args.sql))
     query = sql.parse(args.sql, num_groups_limit=args.num_groups_limit)
     ctx = B200Context(args.device)
     segments, domain = [], None
@@ -148,6 +150,39 @@ def main(argv=None) -> int:
             s.destroy()
         if domain is not None:
             domain.release()
+        ctx.close()
+
+
+def _selection(args, query) -> int:
+    """SELECT columns ... LIMIT n: one device submission, segments taken in the order given (their dictionaries may
+    differ: values are decoded per row's segment)."""
+    from ._lib import Pb200Error
+    from .plan_maker import B200Context, B200PlanMaker, IndexSegment
+
+    ctx = B200Context(args.device)
+    segments = []
+    try:
+        for d in args.segment_dir:
+            segments.append(IndexSegment.load(ctx, d))
+        try:
+            block = B200PlanMaker(ctx).execute_selection(segments, query, merge=True)
+        except Pb200Error as e:
+            sys.stderr.write(f"{e}\n")
+            return 2
+        rows = [[c[i].item() if hasattr(c[i], "item") else c[i] for c in block.columns] for i in range(block.num_rows)]
+        stats = {"numDocsScanned": block.stats.num_docs_scanned, "totalDocs": sum(s.num_docs for s in segments),
+                 "numSegments": len(segments), "deviceMs": round(block.device_ms, 4), "operators": ["SELECTION"]}
+        if args.json:
+            print(json.dumps({"columns": block.names, "rows": rows, "stats": stats}, default=str))
+        else:
+            print("\t".join(block.names))
+            for r in rows:
+                print("\t".join(str(x) for x in r))
+            print(f"-- {json.dumps(stats)}", file=sys.stderr)
+        return 0
+    finally:
+        for s in segments:
+            s.destroy()
         ctx.close()
 
 

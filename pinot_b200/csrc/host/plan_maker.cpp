@@ -774,3 +774,81 @@ extern "C" int32_t pb200h_execute_ordered(pb200_ctx* ctx, const pb200h_query* q,
   }
   return PB200_OK;
 }
+
+namespace {
+// A selection result without rows, built on the host (every doc of the segments is filtered out before any scan).
+pb200_result* empty_selection(pb200h_segment* const* segs, int s0, int s1, int ncols) {
+  pb200_result* R = new pb200_result();
+  R->selection.present = true;
+  R->selection.columns.assign(ncols, nullptr);
+  R->meta.regime = PB200_REGIME_NONE;
+  for (int s = s0; s < s1; s++) R->meta.num_total_docs += segs[s]->num_docs;
+  return R;
+}
+}  // namespace
+
+extern "C" int32_t pb200h_execute_selection(pb200_ctx* ctx, const pb200h_query* q, const pb200h_selection* sel,
+                                            pb200h_segment* const* segs, int32_t nseg, pb200_result** results) {
+  if (!ctx || !q || !sel || !segs || !results || nseg <= 0) { set_error("invalid argument to pb200h_execute_selection"); return PB200_E_INVALID; }
+  if (sel->num_columns < 0 || (sel->num_columns > 0 && !sel->columns)) { set_error("selection: bad column list"); return PB200_E_INVALID; }
+  const pb200h_segment& s0 = *segs[0];
+  std::vector<int32_t> cols(sel->num_columns);
+  for (int k = 0; k < sel->num_columns; k++) {
+    cols[k] = s0.column_index(sel->columns[k]);
+    if (cols[k] < 0) { set_error("unknown selected column '%s'", sel->columns[k] ? sel->columns[k] : "(null)"); return PB200_E_INVALID; }
+  }
+  pb200_selection dsel;
+  memset(&dsel, 0, sizeof dsel);
+  dsel.num_columns = sel->num_columns;
+  dsel.columns = cols.data();
+  dsel.limit = sel->limit;
+  if (sel->num_order_items < 0 || sel->num_order_items > PB200_MAX_ORDER_BY) { set_error("selection ORDER BY with %d items (1..%d)", sel->num_order_items, PB200_MAX_ORDER_BY); return PB200_E_INVALID; }
+  dsel.num_order_items = sel->num_order_items;
+  for (int k = 0; k < sel->num_order_items; k++) {
+    dsel.order[k].column = s0.column_index(sel->order[k].column);
+    dsel.order[k].descending = sel->order[k].descending;
+    if (dsel.order[k].column < 0) { set_error("unknown ORDER BY column '%s'", sel->order[k].column ? sel->order[k].column : "(null)"); return PB200_E_INVALID; }
+  }
+  if (sel->limit < 0) { set_error("selection: negative LIMIT"); return PB200_E_INVALID; }
+  if (sel->limit > PB200_MAX_SELECT_LIMIT) { set_error("selection LIMIT %lld above %d", (long long)sel->limit, PB200_MAX_SELECT_LIMIT); return PB200_E_UNSUPPORTED; }
+  const bool merge = q->merge_segments != 0;
+  std::vector<SegmentFilter> filters(nseg);
+  std::vector<int> dev_idx;
+  for (int s = 0; s < nseg; s++) {
+    if (segs[s]->cols.size() != s0.cols.size()) { set_error("segments do not share a schema"); return PB200_E_INVALID; }
+    for (int k = 0; k < sel->num_columns; k++) {
+      const HostColumn &a = s0.cols[cols[k]], &b = segs[s]->cols[cols[k]];
+      if (a.name != b.name || a.data_type != b.data_type) { set_error("segment %d: column '%s' is not at the position it has in segment 0", s, sel->columns[k]); return PB200_E_INVALID; }
+    }
+    if (int rc = build_segment_filter(*segs[s], *q, filters[s], nullptr)) return rc;
+    if (!filters[s].root_empty) dev_idx.push_back(s);
+  }
+  const int nres = merge ? 1 : nseg;
+  std::vector<pb200_result*> dev_results(merge ? 1 : dev_idx.size(), nullptr);
+  if (!dev_idx.empty()) {
+    std::vector<pb200_filter_node> flat;
+    std::vector<pb200_segment*> dsegs;
+    for (int s : dev_idx) { flat.insert(flat.end(), filters[s].nodes.begin(), filters[s].nodes.end()); dsegs.push_back(segs[s]->dev); }
+    pb200_query dq;
+    memset(&dq, 0, sizeof dq);
+    dq.num_filter_nodes = q->num_filter_nodes;
+    dq.flags = PB200_Q_PER_SEGMENT_FILTER;
+    dq.filter = flat.data();
+    int rc = pb200_execute_selection(ctx, &dq, &dsel, dsegs.data(), (int)dsegs.size(), merge ? PB200_Q_MERGE_SEGMENTS : 0, dev_results.data());
+    if (rc) return rc;
+    // rows name their segment by its position in the device submission: map it back to `segs`
+    for (pb200_result* R : dev_results)
+      for (int64_t i = 0; i < R->selection.rows; i++) R->selection.segment_index[i] = dev_idx[R->selection.segment_index[i]];
+  }
+  if (merge) {
+    results[0] = dev_idx.empty() ? empty_selection(segs, 0, nseg, sel->num_columns) : dev_results[0];
+    results[0]->meta.num_total_docs = 0;
+    for (int s = 0; s < nseg; s++) results[0]->meta.num_total_docs += segs[s]->num_docs;
+    return PB200_OK;
+  }
+  size_t di = 0;
+  for (int s = 0; s < nres; s++)
+    results[s] = (di < dev_idx.size() && dev_idx[di] == s) ? dev_results[di++] : empty_selection(segs, s, s + 1, sel->num_columns);
+  return PB200_OK;
+}
+

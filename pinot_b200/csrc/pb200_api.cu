@@ -27,6 +27,9 @@ static thread_local char g_error[1024] = "";
 static thread_local double g_phase_ms[PB200_NUM_PHASES] = {};
 static inline double now_ms() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
 
+void set_phase_ms(int phase, double ms) { g_phase_ms[phase] = ms; }
+double host_ms() { return now_ms(); }
+
 void set_error(const char* fmt, ...) {
   va_list ap;
   va_start(ap, fmt);
@@ -622,6 +625,52 @@ cudaError_t launch_scan_variant(const ScanVariant& v, size_t smem_bytes, int gri
 }
 }  // namespace pb200
 
+namespace pb200 {
+// Device buffers of the plan's filter leaves: LUTs, doc masks, range lists, and every posting list decoded by ONE launch;
+// the leaf descriptors in plan.segs point at them.  They live in `temps` until the caller is done with the launch.
+int bind_leaf_buffers(pb200_ctx* ctx, ScanPlan& plan, cudaStream_t st, std::vector<std::unique_ptr<DevBufRaw>>& temps) {
+  std::vector<DecodeJob> decode_jobs;
+  auto temp = [&](size_t bytes, void** p) -> int {
+    temps.emplace_back(new DevBufRaw(ctx));
+    const int rc = temps.back()->alloc(bytes);
+    *p = temps.back()->p;
+    return rc;
+  };
+  for (const LeafBuffer& b : plan.leaf_buffers) {
+    void* vp = nullptr;
+    if (int rc = temp(b.words * 4, &vp)) return rc;
+    uint32_t* p = static_cast<uint32_t*>(vp);
+    LeafDesc& lf = plan.segs[b.seg].leaves[b.leaf];
+    if (b.kind == LeafBuffer::DOC_RANGES) lf.ranges = reinterpret_cast<const int32_t*>(p); else lf.bits = p;
+    switch (b.kind) {
+      case LeafBuffer::LUT:
+        PB200_CUDA(cudaMemcpyAsync(p, b.lut.data(), b.words * 4, cudaMemcpyHostToDevice, st));
+        PB200_CUDA(cudaStreamSynchronize(st));
+        break;
+      case LeafBuffer::INV_MASK:
+        PB200_CUDA(cudaMemsetAsync(p, 0, b.words * 4, st));
+        for (DecodeJob j : b.jobs) { j.mask = p; decode_jobs.push_back(j); }
+        break;
+      case LeafBuffer::DOC_MASK:
+        PB200_CUDA(cudaMemsetAsync(p + b.src_words, 0, (b.words - b.src_words) * 4, st));
+        PB200_CUDA(cudaMemcpyAsync(p, b.src, b.src_words * 4, cudaMemcpyHostToDevice, st));
+        PB200_CUDA(cudaStreamSynchronize(st));  // caller's buffer may be a temporary
+        break;
+      case LeafBuffer::DOC_RANGES:
+        PB200_CUDA(cudaMemcpyAsync(p, b.src, b.src_words * 4, cudaMemcpyHostToDevice, st));
+        PB200_CUDA(cudaStreamSynchronize(st));
+        break;
+    }
+  }
+  if (!decode_jobs.empty()) {
+    void* jobs_dev = nullptr;
+    if (int rc = temp(sizeof(DecodeJob) * decode_jobs.size(), &jobs_dev)) return rc;
+    if (int rc = roaring_decode_batch(ctx, st, decode_jobs, jobs_dev)) return rc;
+  }
+  return PB200_OK;
+}
+}  // namespace pb200
+
 // Internal return code of execute_impl: a count-carrying sum overflowed its field (detected exactly, see the verification
 // after the launch) -- the caller runs the submission again with separate COUNT reductions.
 constexpr int kRetryWithoutCountCarrier = 1;
@@ -689,46 +738,8 @@ static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment*
     ~ResultCleanup() { if (armed) for (auto& x : *r) if (x) pb200_result_free(x.release()); }
   } cleanup{&res};
 
-  // ---- bind the leaf buffers: LUTs, doc masks, range lists, and every posting list decoded by ONE launch ----
   std::vector<std::unique_ptr<DevBufRaw>> temps;  // freed after the launch
-  std::vector<DecodeJob> decode_jobs;
-  auto temp = [&](size_t bytes, void** p) -> int {
-    temps.emplace_back(new DevBufRaw(ctx));
-    const int rc = temps.back()->alloc(bytes);
-    *p = temps.back()->p;
-    return rc;
-  };
-  for (const LeafBuffer& b : plan.leaf_buffers) {
-    void* vp = nullptr;
-    if (int rc = temp(b.words * 4, &vp)) return rc;
-    uint32_t* p = static_cast<uint32_t*>(vp);
-    LeafDesc& lf = plan.segs[b.seg].leaves[b.leaf];
-    if (b.kind == LeafBuffer::DOC_RANGES) lf.ranges = reinterpret_cast<const int32_t*>(p); else lf.bits = p;
-    switch (b.kind) {
-      case LeafBuffer::LUT:
-        PB200_CUDA(cudaMemcpyAsync(p, b.lut.data(), b.words * 4, cudaMemcpyHostToDevice, st));
-        PB200_CUDA(cudaStreamSynchronize(st));
-        break;
-      case LeafBuffer::INV_MASK:
-        PB200_CUDA(cudaMemsetAsync(p, 0, b.words * 4, st));
-        for (DecodeJob j : b.jobs) { j.mask = p; decode_jobs.push_back(j); }
-        break;
-      case LeafBuffer::DOC_MASK:
-        PB200_CUDA(cudaMemsetAsync(p + b.src_words, 0, (b.words - b.src_words) * 4, st));
-        PB200_CUDA(cudaMemcpyAsync(p, b.src, b.src_words * 4, cudaMemcpyHostToDevice, st));
-        PB200_CUDA(cudaStreamSynchronize(st));  // caller's buffer may be a temporary
-        break;
-      case LeafBuffer::DOC_RANGES:
-        PB200_CUDA(cudaMemcpyAsync(p, b.src, b.src_words * 4, cudaMemcpyHostToDevice, st));
-        PB200_CUDA(cudaStreamSynchronize(st));
-        break;
-    }
-  }
-  if (!decode_jobs.empty()) {
-    void* jobs_dev = nullptr;
-    if (int rc = temp(sizeof(DecodeJob) * decode_jobs.size(), &jobs_dev)) return rc;
-    if (int rc = roaring_decode_batch(ctx, st, decode_jobs, jobs_dev)) return rc;
-  }
+  if (int rc = bind_leaf_buffers(ctx, plan, st, temps)) return rc;
 
   // ---- bind the outputs ----
   AggAccum init_acc;

@@ -188,8 +188,20 @@ struct QueryDesc {
   int8_t smem_slot[kMaxAggs];  // aggregation -> index of its (lo, hi) pair, -1: none (COUNT)
   int8_t smem_count;           // 1: the shared table has a count array
   int8_t smem_merged;          // 1: every segment of the launch adds into the same global table (flush at exit only)
+  // Selection launches (pb200_select.cu): the launch-wide match mask, as two 32-bit halves (lo, hi) of the pointer because
+  // the field is only 4-byte aligned.  Non-NULL: every thread stores its final 32-row mask at word
+  // (T * W + warp) * 32 + lane, T the launch tile.  NULL (both halves 0) in every aggregation launch.
   int32_t reserved_tail[2];
 };
+
+__host__ __device__ inline uint32_t* selection_mask_of(const QueryDesc& q) {
+  return reinterpret_cast<uint32_t*>((unsigned long long)(uint32_t)q.reserved_tail[1] << 32 | (uint32_t)q.reserved_tail[0]);
+}
+inline void set_selection_mask(QueryDesc& q, uint32_t* p) {
+  const unsigned long long v = reinterpret_cast<unsigned long long>(p);
+  q.reserved_tail[0] = (int32_t)(uint32_t)v;
+  q.reserved_tail[1] = (int32_t)(uint32_t)(v >> 32);
+}
 
 // ---- shared-memory header of the scan kernel (the host sizes the dynamic shared memory with it) ----
 constexpr int kMaxWarps = 8;    // warps per CTA (all of them consume; there is no producer warp)

@@ -15,6 +15,9 @@
 namespace pb200 {
 
 void set_error(const char* fmt, ...);
+// pb200_last_phases of the calling thread: one phase's host wall-clock (PB200_PHASE_*), and the clock it is read from
+void set_phase_ms(int phase, double ms);
+double host_ms();
 #define PB200_CUDA(call)                                                                         \
   do {                                                                                           \
     cudaError_t e__ = (call);                                                                    \
@@ -143,6 +146,15 @@ struct pb200_result {
     const int64_t* lng[pb200::kMaxAggs] = {};      // NULL: all zero
     const int32_t* ids[pb200::kMaxAggs] = {};      // NULL: all -1
   } view;
+  // Selection result (pb200_select.cu): rows in a pinned block shared by the results of one submission
+  struct Selection {
+    bool present = false;
+    std::shared_ptr<pb200::PinnedBlock> block;
+    int64_t rows = 0;
+    int32_t* doc_ids = nullptr;
+    int32_t* segment_index = nullptr;
+    std::vector<const void*> columns;            // int64 or double [rows] each
+  } selection;
   pb200_order_by order{};                        // ORDER BY spec of a group-by result (num_items 0: none), applied at extraction
   std::vector<int32_t> agg_functions;            // PB200_AGG_* per aggregation (set by pb200_execute)
   std::vector<int32_t> keys;                     // [G x k]

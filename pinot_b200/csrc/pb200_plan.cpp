@@ -704,6 +704,110 @@ int plan_scan(const Tuning& tune, DeviceLimits lim, const pb200_query* query, pb
   return PB200_OK;
 }
 
+int plan_selection(const Tuning& tune, DeviceLimits lim, const pb200_query* filter_only, const pb200_selection* sel,
+                   pb200_segment* const* segments, int nseg, bool prefix, SelectionPlan* out) {
+  if (!filter_only || !sel || !segments || !out || nseg <= 0) { set_error("invalid argument to pb200_execute_selection"); return PB200_E_INVALID; }
+  if (sel->limit < 0 || sel->num_columns < 0 || (sel->num_columns > 0 && !sel->columns)) { set_error("selection: bad limit or column list"); return PB200_E_INVALID; }
+  if (sel->limit > PB200_MAX_SELECT_LIMIT) { set_error("selection LIMIT %lld above %d", (long long)sel->limit, PB200_MAX_SELECT_LIMIT); return PB200_E_UNSUPPORTED; }
+  if (sel->num_order_items < 0 || sel->num_order_items > PB200_MAX_ORDER_BY) { set_error("selection ORDER BY with %d items (1..%d)", sel->num_order_items, PB200_MAX_ORDER_BY); return PB200_E_INVALID; }
+  // the select phase puts the segment index in gridDim.y
+  if (nseg > kMaxSelectSegments) { set_error("selection over %d segments: at most %d per submission", nseg, kMaxSelectSegments); return PB200_E_UNSUPPORTED; }
+  // the scan: the caller's filter, COUNT(*) (matched docs per segment), one result per segment
+  static const pb200_agg kCount = {PB200_AGG_COUNT, -1};
+  pb200_query q = *filter_only;
+  q.num_group_by = 0;
+  q.group_by_columns = nullptr;
+  q.num_aggs = 1;
+  q.aggs = &kCount;
+  q.flags = filter_only->flags & PB200_Q_PER_SEGMENT_FILTER;
+  q.reduce_world = 0;
+  q.merged_docs_bound = 0;
+  SelectionPlan& p = *out;
+  p = SelectionPlan();
+  if (int rc = plan_scan(tune, lim, &q, segments, nseg, false, &p.scan)) return rc;
+  ScanPlan& plan = p.scan;
+  p.limit = sel->limit;
+
+  // ---- selected and order columns: one value kind for all segments ----
+  const int ncols = (int)segments[0]->cols.size();
+  auto kind_of = [&](int c, const char* what, int* out_kind) -> int {
+    if (c < 0 || c >= ncols) { set_error("%s column %d out of range", what, c); return PB200_E_INVALID; }
+    int kind = -1;
+    for (int s = 0; s < nseg; s++) {
+      const DeviceColumn& dc = segments[s]->cols[c];
+      int ks;
+      if (dc.fwd_kind != PB200_FWD_DICT_FIXEDBIT && dc.fwd_kind != PB200_FWD_RAW_FIXEDBYTE) ks = -1;
+      else if (dc.bits == 32 && !dc.dict_native) ks = dc.stored_type == PB200_INT ? SEL_RAW_I32 : dc.stored_type == PB200_FLOAT ? SEL_RAW_F32 : -1;
+      else if (dc.stored_type == PB200_STRING) ks = SEL_DICT_ID;
+      else if (!dc.dict_native) ks = -1;
+      else ks = dc.stored_type == PB200_INT ? SEL_DICT_I32 : dc.stored_type == PB200_LONG ? SEL_DICT_I64
+              : dc.stored_type == PB200_FLOAT ? SEL_DICT_F32 : SEL_DICT_F64;
+      if (ks < 0) { set_error("%s column %d of segment %d has no device dictionary or raw 32-bit values: not accelerated", what, c, s); return PB200_E_UNSUPPORTED; }
+      if (kind >= 0 && ks != kind) { set_error("%s column %d is stored differently in segment %d than in segment 0", what, c, s); return PB200_E_UNSUPPORTED; }
+      kind = ks;
+    }
+    *out_kind = kind;
+    return PB200_OK;
+  };
+  for (int k = 0; k < sel->num_columns; k++) {
+    int kind = 0;
+    if (int rc = kind_of(sel->columns[k], "selected", &kind)) return rc;
+    p.columns.push_back(sel->columns[k]);
+    p.kinds.push_back(kind);
+  }
+  for (int k = 0; k < sel->num_order_items; k++) {
+    int kind = 0;
+    if (int rc = kind_of(sel->order[k].column, "ORDER BY", &kind)) return rc;
+    p.order_cols.push_back(sel->order[k].column);
+    p.order_kinds.push_back(kind);
+    p.order_desc.push_back(sel->order[k].descending != 0);
+  }
+  // a COUNT(*) launch has no deferred gathers: at 8 warps it runs the variant without them (the one that stores the mask)
+  if (plan.variant.warps == 8) plan.variant.defer = false;
+  // the top rows by value can sit anywhere in a segment: ORDER BY scans every doc
+  if (!p.order_cols.empty()) prefix = false;
+
+  // ---- scanned range: a prefix of whole tiles, or the whole segment ----
+  const long long tile_rows = plan.q.tile_rows;
+  const long long prefix_tiles = (std::max(kSelectPrefixRows, 2 * p.limit) + tile_rows - 1) / tile_rows;
+  p.scan_docs.resize(nseg);
+  for (int s = 0; s < nseg; s++) {
+    SegDesc& sd = plan.segs[s];
+    const long long leaves_per_doc = sd.num_docs > 0 ? plan.in_filter[s] / sd.num_docs : 0;
+    p.scan_docs[s] = sd.num_docs;
+    if (prefix && sd.num_tiles > prefix_tiles) {
+      sd.num_tiles = prefix_tiles;
+      p.scan_docs[s] = prefix_tiles * tile_rows;
+      p.prefix = true;
+    }
+    plan.in_filter[s] = leaves_per_doc * p.scan_docs[s];
+  }
+  // launch chunks over the (possibly shortened) tile ranges -- the grouping of segments into chunks is plan_scan's
+  long long cursor = 0;
+  p.mask_word_off.resize(nseg);
+  for (LaunchChunk& ch : plan.chunks) {
+    long long c_tiles = 0;
+    p.chunk_word_off.push_back(cursor * tile_rows / 32);
+    for (int s = ch.first_seg; s < ch.first_seg + ch.num_segs; s++) {
+      plan.segs[s].first_tile = c_tiles;
+      p.mask_word_off[s] = (cursor + c_tiles) * tile_rows / 32;
+      c_tiles += plan.segs[s].num_tiles;
+    }
+    ch.total_tiles = (int)c_tiles;
+    ch.grid = tune.grid > 0 ? tune.grid : (int)std::min<long long>((long long)lim.sm_count * plan.ctas_per_sm, std::max<long long>(c_tiles, 1));
+    cursor += c_tiles;
+  }
+  p.mask_words = cursor * tile_rows / 32;
+  return PB200_OK;
+}
+
+std::vector<int> selection_rescan(const SelectionPlan& p, pb200_segment* const* segments, const std::vector<long long>& matches) {
+  std::vector<int> out;
+  for (size_t s = 0; s < p.scan_docs.size(); s++)
+    if (p.scan_docs[s] < segments[s]->num_docs && matches[s] < p.limit) out.push_back((int)s);
+  return out;
+}
+
 TmaTable tma_table(const ScanPlan& plan, const LaunchChunk& c) {
   TmaTable tt;
   memset(&tt, 0, sizeof tt);

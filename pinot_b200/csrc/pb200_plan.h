@@ -82,10 +82,47 @@ struct ScanPlan {
 int plan_scan(const Tuning& tune, DeviceLimits lim, const pb200_query* query, pb200_segment* const* segments, int nseg,
               bool allow_count_carrier, ScanPlan* out);
 
+// ---- selection (pb200_execute_selection): plan_scan with COUNT(*) as the only aggregation, plus the match mask ----
+constexpr long long kSelectPrefixRows = 1ll << 20;  // first pass of a selection without ORDER BY: at least this many docs
+constexpr int kMaxSelectSegments = 65535;           // segments of one selection submission (gridDim.y of the select phase)
+// how a selected column's value is produced at a doc (pb200_select.cu gather)
+enum : int32_t { SEL_DICT_I32 = 0, SEL_DICT_I64 = 1, SEL_DICT_F32 = 2, SEL_DICT_F64 = 3, SEL_DICT_ID = 4, SEL_RAW_I32 = 5,
+                 SEL_RAW_F32 = 6 };
+inline bool selection_kind_is_double(int k) { return k == SEL_DICT_F32 || k == SEL_DICT_F64 || k == SEL_RAW_F32; }
+
+struct SelectionPlan {
+  ScanPlan scan;                          // the launch; segments keep their submission order and results are per segment
+  std::vector<int> columns;               // selected column ids
+  std::vector<int> kinds;                 // SEL_* per selected column (the same in every segment)
+  std::vector<int> order_cols, order_kinds;  // ORDER BY items: column id, SEL_* kind
+  std::vector<bool> order_desc;
+  long long limit = 0;
+  // Launch-wide match mask: doc d of segment s is bit d % 32 of word mask_word_off[s] + d / 32 (bit j of word w = doc
+  // 32w + j inside the segment, the PB200_F_DOC_MASK layout).  Chunk c's launch writes from word chunk_word_off[c] on.
+  std::vector<long long> mask_word_off;
+  std::vector<long long> chunk_word_off;
+  long long mask_words = 0;
+  std::vector<long long> scan_docs;       // per segment: docs [0, scan_docs) scanned (a prefix, or num_docs)
+  bool prefix = false;                    // some segment is scanned over a prefix only
+};
+
+// prefix: scan each segment over its first max(kSelectPrefixRows, 2 x limit) docs rounded up to whole tiles (selection
+// without ORDER BY: the first `limit` matches are usually there; with ORDER BY every doc is scanned).  PB200_OK or the PB200_E_* code of
+// pb200_execute_selection for this input.  No CUDA runtime call.
+int plan_selection(const Tuning& tune, DeviceLimits lim, const pb200_query* filter_only, const pb200_selection* sel,
+                   pb200_segment* const* segments, int nseg, bool prefix, SelectionPlan* out);
+// Segments a prefix pass must scan again over all their docs: prefix shorter than the segment and fewer than `limit`
+// matches in it (matches[s] = matched docs of segment s in the prefix).
+std::vector<int> selection_rescan(const SelectionPlan& p, pb200_segment* const* segments, const std::vector<long long>& matches);
+
 // DictionaryBasedGroupKeyGenerator's key-holder regime for these group-by cardinalities (informational)
 int regime_of(const std::vector<int>& cards, int array_threshold);
 
 // The TMA table of chunk `c` (device pointers as bound into plan.segs).
 TmaTable tma_table(const ScanPlan& plan, const LaunchChunk& c);
+
+// pb200_api.cu: allocates and fills the device buffers plan.leaf_buffers lists on `st` and points the leaf descriptors of
+// plan.segs at them; the buffers stay in `temps` until the launch that reads them is done.
+int bind_leaf_buffers(pb200_ctx* ctx, ScanPlan& plan, cudaStream_t st, std::vector<std::unique_ptr<DevBufRaw>>& temps);
 
 }  // namespace pb200

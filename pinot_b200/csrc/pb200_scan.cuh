@@ -674,6 +674,12 @@ scan_kernel(const __grid_constant__ QueryDesc q, const __grid_constant__ TmaTabl
         m &= stk[0];
       }
     }
+    // selection launches: the thread's final mask (bit j = row row0 + j; zero for skipped slices and rows past the
+    // segment) into the launch-wide doc-id set, one coalesced store per thread and tile.  Selections run the
+    // aggregation-only variants without deferred gathers at 8 warps (plan_selection), so that variant alone carries it.
+    if constexpr (!GROUPBY && !(W == 8 && DEFER)) {
+      if ((q.reserved_tail[0] | q.reserved_tail[1]) != 0) selection_mask_of(q)[((size_t)T * W + warp) * 32 + lane] = m;
+    }
 
     drain();  // the previous tile's gathers have had this tile's whole filter phase to arrive
     drain_gb();

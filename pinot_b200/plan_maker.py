@@ -635,3 +635,85 @@ class B200PlanMaker:
                   for i in range(nres)]
         self.last_device_ms = blocks[0].device_ms
         return blocks
+
+    def execute_selection(self, segments: Sequence[IndexSegment], query, merge: bool = False):
+        """A selection query (sql.SelectionQuery) over the segments in ONE device submission: per segment its first
+        `limit` matching docs in doc order (merge=True: one block, segments taken in submission order), or with an ORDER BY
+        its top `limit` rows by value, ties by doc id (merge=True: the tops merged by value, ties by (segment, doc id)).  Returns a list of
+        SelectionResultsBlock, one per segment, or one block when merged."""
+        columns = query.columns if query.columns is not None else sorted(segments[0].column_names)
+        if len(query.order_by) > _lib.MAX_ORDER_BY:
+            raise ValueError(f"ORDER BY has {len(query.order_by)} items, at most {_lib.MAX_ORDER_BY} are supported")
+        hq, _keep = _marshal_query(QueryContext(aggregations=[], filter=query.filter), merge)
+        names = [c.encode() for c in columns]
+        cnames = (C.c_char_p * max(1, len(names)))(*names)
+        onames = [c.encode() for c, _ in query.order_by]
+        sel = _lib.HSelection(len(columns), cnames, len(onames))
+        for k, (name, (_, asc)) in enumerate(zip(onames, query.order_by)):
+            sel.order[k] = _lib.HSelectOrder(name, int(not asc))
+        sel.limit = int(query.limit)
+        n = len(segments)
+        segs = (C.c_void_p * n)(*[s.handle for s in segments])
+        nres = 1 if merge else n
+        res = (C.c_void_p * nres)()
+        _lib.check(self.ctx.lib.pb200h_execute_selection(self.ctx.handle, C.byref(hq), C.byref(sel), segs, n, res))
+        blocks = [_read_selection(self.ctx, C.c_void_p(res[i]), segments, columns) for i in range(nres)]
+        self.last_device_ms = blocks[0].device_ms
+        return blocks[0] if merge else blocks
+
+
+@dataclass
+class SelectionResultsBlock:
+    """What a SelectionResultsBlock is built from: the selected columns' values per row (INT / LONG as int64, FLOAT /
+    DOUBLE as float64, STRING as str), the doc id and the segment (index into the submitted segments) of every row."""
+    names: List[str]
+    columns: List[np.ndarray]
+    doc_ids: np.ndarray
+    segment_index: np.ndarray
+    stats: ExecutionStatistics
+    device_ms: float = 0.0
+
+    @property
+    def num_rows(self) -> int:
+        return len(self.doc_ids)
+
+
+def _read_selection(ctx: B200Context, handle, segments: Sequence[IndexSegment], columns: Sequence[str]) -> SelectionResultsBlock:
+    L = ctx.lib
+    try:
+        meta = _lib.ResultMeta()
+        _lib.check(L.pb200_result_meta_get(handle, C.byref(meta)))
+        rows = C.c_int64()
+        docs, segi = C.c_void_p(), C.c_void_p()
+        cols = (C.c_void_p * max(1, len(columns)))()
+        _lib.check(L.pb200_result_selection(handle, C.byref(rows), C.byref(docs), C.byref(segi), cols))
+        n = int(rows.value)
+
+        def copy(ptr, ctype, dtype):
+            if n == 0 or not ptr:
+                return np.zeros(0, dtype=dtype)
+            return np.ctypeslib.as_array(C.cast(ptr, C.POINTER(ctype)), shape=(n,)).astype(dtype, copy=True)
+        doc_ids = copy(docs.value, C.c_int32, np.int32)
+        seg_index = copy(segi.value, C.c_int32, np.int32)
+        out = []
+        for k, name in enumerate(columns):
+            info = segments[0].column_info(name)
+            if info["data_type"] in (_lib.FLOAT, _lib.DOUBLE):
+                out.append(copy(cols[k], C.c_double, np.float64))
+            elif info["data_type"] == _lib.STRING:   # dictIds of the row's segment -> the dictionary's strings
+                ids = copy(cols[k], C.c_int64, np.int64)
+                cache: Dict[Tuple[int, int], str] = {}
+                vals = np.empty(n, dtype=object)
+                for i in range(n):
+                    key = (int(seg_index[i]), int(ids[i]))
+                    if key not in cache:
+                        cache[key] = segments[key[0]].dictionary_value(name, key[1])
+                    vals[i] = cache[key]
+                out.append(vals)
+            else:
+                out.append(copy(cols[k], C.c_int64, np.int64))
+        stats = ExecutionStatistics(meta.num_docs_scanned, meta.num_entries_scanned_in_filter,
+                                    meta.num_entries_scanned_post_filter, meta.num_total_docs)
+        return SelectionResultsBlock(list(columns), out, doc_ids, seg_index, stats, float(meta.device_ms))
+    finally:
+        L.pb200_result_free(handle)

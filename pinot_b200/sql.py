@@ -8,6 +8,7 @@ stays Java).  This module exists so the parity tests read like the reference's
 
     SELECT item[, item...] FROM table [WHERE cond] [GROUP BY col[, col...]] [ORDER BY expr [ASC|DESC], ...] [LIMIT n]
     item  := COUNT(*) | FN(col) | col            (plain columns are allowed only when they are group-by keys)
+    selection (parse_selection): SELECT * | col[, col...] FROM table [WHERE cond] [ORDER BY col [ASC|DESC], ...] [LIMIT n]
     cond  := cond AND cond | cond OR cond | NOT cond | (cond) | col op literal | col BETWEEN a AND b
              | col [NOT] IN (literal, ...)
     op    := = | != | <> | < | <= | > | >=
@@ -15,6 +16,7 @@ stays Java).  This module exists so the parity tests read like the reference's
 from __future__ import annotations
 
 import re
+from dataclasses import dataclass, field
 from typing import List, Optional
 
 from .query import Aggregation, Filter, FilterNode, Predicate, QueryContext, optimize_filter
@@ -246,3 +248,70 @@ def parse(sql: str, **options) -> QueryContext:
                          order_by=order_by, **options)
     resolve_order_by(query)
     return query
+
+
+@dataclass
+class SelectionQuery:
+    """SELECT columns FROM table WHERE ... [ORDER BY col [ASC|DESC], ...] LIMIT n (the reference's selection query shape).
+    columns None: SELECT * (the segment's columns in name order)."""
+    columns: Optional[List[str]]
+    filter: Optional[FilterNode] = None
+    order_by: List[tuple] = field(default_factory=list)  # (column, ascending)
+    limit: int = 10
+    table: str = "testTable"
+
+
+def is_selection(sql: str) -> bool:
+    """True when the select list holds no aggregation function (the statement is a selection query)."""
+    p = _Parser(sql)
+    if not p.take_kw("SELECT"):
+        return False
+    while p.peek()[0] is not None and not p.kw("FROM"):
+        k, v = p.peek()
+        p.i += 1
+        if k == "id" and v.upper() in _FUNCTIONS and p.take_op("("):
+            return False
+    return True
+
+
+def parse_selection(sql: str) -> SelectionQuery:
+    """SQL text of a selection query -> SelectionQuery (filter run through the broker-side filter optimizers)."""
+    p = _Parser(sql)
+    p.expect_kw("SELECT")
+    columns: Optional[List[str]] = []
+    if p.take_op("*"):
+        columns = None
+    else:
+        while True:
+            name = p.ident()
+            if name.upper() in _FUNCTIONS and p.peek() == ("op", "("):
+                raise SqlError(f"{name}(...) in a selection query: aggregations go through parse()")
+            columns.append(name)
+            if not p.take_op(","):
+                break
+    p.expect_kw("FROM")
+    table = p.ident()
+    flt: Optional[FilterNode] = None
+    if p.take_kw("WHERE"):
+        flt = p.cond()
+    if p.kw("GROUP"):
+        raise SqlError("GROUP BY needs an aggregation in the select list")
+    order_by = []
+    if p.take_kw("ORDER"):
+        p.expect_kw("BY")
+        while True:
+            name = p.ident()
+            asc = not p.take_kw("DESC")
+            if asc:
+                p.take_kw("ASC")
+            order_by.append((name, asc))
+            if not p.take_op(","):
+                break
+    limit = 10
+    if p.take_kw("LIMIT"):
+        limit = p.literal()
+        if not isinstance(limit, int) or limit < 0:
+            raise SqlError(f"LIMIT must be a non-negative integer, got {limit!r}")
+    if p.peek()[0] is not None:
+        raise SqlError(f"trailing tokens: {p.toks[p.i:]}")
+    return SelectionQuery(columns=columns, filter=optimize_filter(flt), order_by=order_by, limit=limit, table=table)
