@@ -297,6 +297,30 @@ int32_t pb200_execute_selection(pb200_ctx* ctx, const pb200_query* filter_only, 
 int32_t pb200_result_selection(const pb200_result* result, int64_t* rows, const int32_t** doc_ids,
                                const int32_t** segment_index, const void** columns);
 
+/* ---- DISTINCT: SELECT DISTINCT columns WHERE ... [ORDER BY columns] LIMIT n (DistinctOperator) -------------------- */
+/* `distinct` is a pb200_selection: its columns are the DISTINCT columns (1..8), its order items name some of them (an
+ * order item on any other column is PB200_E_INVALID).  A row is one distinct tuple of the columns' values over the
+ * matching docs, and carries the tuple's FIRST OCCURRENCE: the doc id and segment index of the first matching doc holding
+ * it, in (segment index in the submission, doc id) order.
+ * Without order items: the first `limit` tuples in order of first occurrence.  With order items: the top `limit` tuples
+ * by the items (value order as for pb200_execute_selection, DESC reversed), ties by first occurrence ascending.
+ * Per segment (flags 0) each result uses that segment's docs only; PB200_Q_MERGE_SEGMENTS gives one result over all
+ * segments and needs every DISTINCT column to have one dictionary across them (bind the segments to a domain), otherwise
+ * PB200_E_UNSUPPORTED as for group-by merges.
+ * Values come back as for a selection (read them with pb200_result_selection): INT / LONG / STRING (the dictId) as
+ * int64, FLOAT / DOUBLE as double.  PB200_E_UNSUPPORTED (the caller runs the stock operator): a column without dictIds
+ * (a raw column streamed as 32-bit values; a raw column whose dictionary was synthesised at load is accepted), a key
+ * space (product of the columns' cardinalities) above 2^24 for one result, tables above 2^27 entries over all results of
+ * the call, more than 8 columns, limit above PB200_MAX_SELECT_LIMIT, more than 65 535 segments.
+ * Statistics (device semantics): num_docs_scanned = matched docs in the scanned range; num_entries_scanned_in_filter =
+ * scanned docs x scan leaves; num_entries_scanned_post_filter = matched docs x num_columns (every matched doc's key is
+ * read).  Without order items each segment is first scanned over selection's prefix (at least 2^20 docs, whole tiles);
+ * a result is final when at least `limit` of its tuples first occur before the prefix end of its earliest truncated
+ * segment, otherwise its truncated segments are scanned in full.  With order items every doc is scanned.
+ * device_ms = the scan launches and the table builds; pb200_last_phases reports PLAN, DEVICE_WAIT, EXTRACT and TOTAL. */
+int32_t pb200_execute_distinct(pb200_ctx* ctx, const pb200_query* filter_only, const pb200_selection* distinct,
+                               pb200_segment* const* segments, int32_t num_segments, int32_t flags, pb200_result** results);
+
 /* ---- results (the data a GroupByResultsBlock / AggregationResultsBlock is built from) ---------------------------- */
 enum { PB200_REGIME_NONE = 0, PB200_REGIME_ARRAY = 1, PB200_REGIME_INT_MAP = 2, PB200_REGIME_LONG_MAP = 3,
        PB200_REGIME_ARRAY_MAP = 4 };

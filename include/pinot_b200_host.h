@@ -205,6 +205,11 @@ typedef struct {
  * handles (one when merge_segments); read them with pb200_result_selection -- segment_index refers to `segments`. */
 int32_t pb200h_execute_selection(pb200_ctx* ctx, const pb200h_query* query, const pb200h_selection* selection,
                                  pb200h_segment* const* segments, int32_t num_segments, pb200_result** results);
+/* SELECT DISTINCT (pb200_execute_distinct of include/pinot_b200.h): `distinct` names the DISTINCT columns and order
+ * items (an order item must be one of the columns: PB200_E_INVALID otherwise).  Filters, EMPTY segments and results as
+ * for pb200h_execute_selection; merge_segments needs the DISTINCT columns bound to one domain. */
+int32_t pb200h_execute_distinct(pb200_ctx* ctx, const pb200h_query* query, const pb200h_selection* distinct,
+                                pb200h_segment* const* segments, int32_t num_segments, pb200_result** results);
 
 /* The result as the server -> broker wire format: DataTableImplV4 bytes (pinot-common/.../datatable/DataTableImplV4.java:49-81)
  * exactly as GroupByResultsBlock.getDataTable() / AggregationResultsBlock.getDataTable() build them for the same rows

@@ -162,6 +162,7 @@ EXPORTED_SYMBOLS = [
     "pb200_domain_release", "pb200_segment_bind_domain", "pb200_segment_local_ids",
     "pb200_last_phases", "pb200_result_columns", "pb200_doc_mask_upload", "pb200_doc_mask_free", "pb200_roaring_validate", "pb200_comm_unique_id", "pb200_comm_init", "pb200_comm_shutdown", "pb200_result_combine",
     "pb200_execute_selection", "pb200_result_selection", "pb200h_execute_selection",
+    "pb200_execute_distinct", "pb200h_execute_distinct",
 ]
 
 _LIB = None
@@ -223,6 +224,8 @@ def load() -> C.CDLL:
     L.pb200_execute_selection.argtypes = [vp, C.POINTER(Query), C.POINTER(Selection), C.POINTER(vp), i32, i32, C.POINTER(vp)]
     L.pb200_result_selection.argtypes = [vp, C.POINTER(i64), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]
     L.pb200h_execute_selection.argtypes = [vp, C.POINTER(HQuery), C.POINTER(HSelection), C.POINTER(vp), i32, C.POINTER(vp)]
+    L.pb200_execute_distinct.argtypes = [vp, C.POINTER(Query), C.POINTER(Selection), C.POINTER(vp), i32, i32, C.POINTER(vp)]
+    L.pb200h_execute_distinct.argtypes = [vp, C.POINTER(HQuery), C.POINTER(HSelection), C.POINTER(vp), i32, C.POINTER(vp)]
     L.pb200_result_columns.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]
     L.pb200_roaring_validate.argtypes = [vp, C.c_uint64, C.c_int64]
     L.pb200_doc_mask_upload.argtypes = [vp, i32, vp, C.c_int64, C.POINTER(vp)]

@@ -106,6 +106,8 @@ def main(argv=None) -> int:
     from ._lib import Pb200Error
     from .plan_maker import B200Context, B200PlanMaker, DictionaryDomain, IndexSegment
 
+    if sql.is_distinct(args.sql):
+        return _distinct(args, sql.parse_distinct(args.sql))
     if sql.is_selection(args.sql):
         return _selection(args, sql.parse_selection(args.sql))
     query = sql.parse(args.sql, num_groups_limit=args.num_groups_limit)
@@ -183,6 +185,49 @@ def _selection(args, query) -> int:
     finally:
         for s in segments:
             s.destroy()
+        ctx.close()
+
+
+def _distinct(args, query) -> int:
+    """SELECT DISTINCT columns ... LIMIT n.  --merge-on-device: the segments are bound to one domain over the DISTINCT
+    columns and answered in one merged call; otherwise one per-segment call, merged by value (merge_distinct_blocks)."""
+    from ._lib import Pb200Error
+    from .plan_maker import B200Context, B200PlanMaker, DictionaryDomain, IndexSegment, merge_distinct_blocks
+
+    ctx = B200Context(args.device)
+    segments, domain = [], None
+    try:
+        for d in args.segment_dir:
+            segments.append(IndexSegment.load(ctx, d))
+        pm = B200PlanMaker(ctx)
+        try:
+            if args.merge_on_device and len(segments) > 1:
+                domain = DictionaryDomain.build(ctx, segments, list(dict.fromkeys(query.columns)))
+                for s in segments:
+                    s.bind_domain(domain)
+                block = pm.execute_distinct(segments, query, merge=True)
+            else:
+                block = merge_distinct_blocks(pm.execute_distinct(segments, query), query.order_by, query.limit)
+        except Pb200Error as e:
+            sys.stderr.write(f"{e}\n")
+            return 2
+        rows = [[c[i].item() if hasattr(c[i], "item") else c[i] for c in block.columns] for i in range(block.num_rows)]
+        stats = {"numDocsScanned": block.stats.num_docs_scanned, "totalDocs": sum(s.num_docs for s in segments),
+                 "numSegments": len(segments), "deviceMs": round(block.device_ms, 4), "operators": ["DISTINCT"]}
+        if args.json:
+            print(json.dumps({"columns": block.names, "rows": rows, "stats": stats}, default=str))
+        else:
+            print("\t".join(block.names))
+            for r in rows:
+                print("\t".join(str(x) for x in r))
+            print(f"-- {json.dumps(stats)}", file=sys.stderr)
+        return 0
+    finally:
+        block = None
+        for s in segments:
+            s.destroy()
+        if domain is not None:
+            domain.release()
         ctx.close()
 
 

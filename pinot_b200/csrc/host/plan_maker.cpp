@@ -785,11 +785,13 @@ pb200_result* empty_selection(pb200h_segment* const* segs, int s0, int s1, int n
   for (int s = s0; s < s1; s++) R->meta.num_total_docs += segs[s]->num_docs;
   return R;
 }
-}  // namespace
 
-extern "C" int32_t pb200h_execute_selection(pb200_ctx* ctx, const pb200h_query* q, const pb200h_selection* sel,
-                                            pb200h_segment* const* segs, int32_t nseg, pb200_result** results) {
-  if (!ctx || !q || !sel || !segs || !results || nseg <= 0) { set_error("invalid argument to pb200h_execute_selection"); return PB200_E_INVALID; }
+// pb200h_execute_selection and pb200h_execute_distinct: names resolved, filters folded per segment, `device` (the C-ABI
+// call) run over the segments whose filter is not EMPTY, segment indexes mapped back to `segs`.
+using RowsDeviceCall = int32_t (*)(pb200_ctx*, const pb200_query*, const pb200_selection*, pb200_segment* const*, int32_t, int32_t,
+                                   pb200_result**);
+int32_t execute_rows(pb200_ctx* ctx, const pb200h_query* q, const pb200h_selection* sel, pb200h_segment* const* segs, int32_t nseg,
+                     pb200_result** results, RowsDeviceCall device) {
   if (sel->num_columns < 0 || (sel->num_columns > 0 && !sel->columns)) { set_error("selection: bad column list"); return PB200_E_INVALID; }
   const pb200h_segment& s0 = *segs[0];
   std::vector<int32_t> cols(sel->num_columns);
@@ -834,7 +836,7 @@ extern "C" int32_t pb200h_execute_selection(pb200_ctx* ctx, const pb200h_query* 
     dq.num_filter_nodes = q->num_filter_nodes;
     dq.flags = PB200_Q_PER_SEGMENT_FILTER;
     dq.filter = flat.data();
-    int rc = pb200_execute_selection(ctx, &dq, &dsel, dsegs.data(), (int)dsegs.size(), merge ? PB200_Q_MERGE_SEGMENTS : 0, dev_results.data());
+    int rc = device(ctx, &dq, &dsel, dsegs.data(), (int)dsegs.size(), merge ? PB200_Q_MERGE_SEGMENTS : 0, dev_results.data());
     if (rc) return rc;
     // rows name their segment by its position in the device submission: map it back to `segs`
     for (pb200_result* R : dev_results)
@@ -850,5 +852,26 @@ extern "C" int32_t pb200h_execute_selection(pb200_ctx* ctx, const pb200h_query* 
   for (int s = 0; s < nres; s++)
     results[s] = (di < dev_idx.size() && dev_idx[di] == s) ? dev_results[di++] : empty_selection(segs, s, s + 1, sel->num_columns);
   return PB200_OK;
+}
+}  // namespace
+
+extern "C" int32_t pb200h_execute_selection(pb200_ctx* ctx, const pb200h_query* q, const pb200h_selection* sel,
+                                            pb200h_segment* const* segs, int32_t nseg, pb200_result** results) {
+  if (!ctx || !q || !sel || !segs || !results || nseg <= 0) { set_error("invalid argument to pb200h_execute_selection"); return PB200_E_INVALID; }
+  return execute_rows(ctx, q, sel, segs, nseg, results, pb200_execute_selection);
+}
+
+extern "C" int32_t pb200h_execute_distinct(pb200_ctx* ctx, const pb200h_query* q, const pb200h_selection* distinct,
+                                           pb200h_segment* const* segs, int32_t nseg, pb200_result** results) {
+  if (!ctx || !q || !distinct || !segs || !results || nseg <= 0) { set_error("invalid argument to pb200h_execute_distinct"); return PB200_E_INVALID; }
+  // also when every segment's filter folds to EMPTY and nothing reaches the device
+  for (int k = 0; k < distinct->num_order_items && k < PB200_MAX_ORDER_BY; k++) {
+    const char* name = distinct->order[k].column;
+    bool found = false;
+    for (int c = 0; c < distinct->num_columns && name && distinct->columns && !found; c++)
+      found = distinct->columns[c] && strcmp(distinct->columns[c], name) == 0;
+    if (!found) { set_error("DISTINCT ORDER BY column '%s' is not one of the DISTINCT columns", name ? name : "(null)"); return PB200_E_INVALID; }
+  }
+  return execute_rows(ctx, q, distinct, segs, nseg, results, pb200_execute_distinct);
 }
 

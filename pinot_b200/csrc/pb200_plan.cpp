@@ -55,6 +55,23 @@ int regime_of(const std::vector<int>& cards, int array_threshold) {
   return product > array_threshold ? PB200_REGIME_INT_MAP : PB200_REGIME_ARRAY;
 }
 
+// One result for all segments == a merge of dictId-indexed state (group tables, MIN / MAX ids, DISTINCTCOUNT bitsets,
+// DISTINCT tables).  That is only a merge BY VALUE (GroupByCombineOperator.java:130-146, AggregationFunction.merge) when
+// the column has the same dictionary everywhere: compare content hashes, not cardinalities.  Bound segments
+// (pb200_domain_*) pass by construction; anything else is refused so that the caller combines per-segment results itself.
+bool same_dictionary(pb200_segment* const* segments, int nseg, int col, const char* what) {
+  const DeviceColumn& c0 = segments[0]->cols[col];
+  for (int s = 1; s < nseg; s++) {
+    const DeviceColumn& c = segments[s]->cols[col];
+    if (c.dict_hash != c0.dict_hash || c.cardinality != c0.cardinality || c.stored_type != c0.stored_type) {
+      set_error("PB200_Q_MERGE_SEGMENTS: %s column %d has a different dictionary in segment %d than in segment 0 "
+                "(bind the segments to a pb200_domain first)", what, col, s);
+      return false;
+    }
+  }
+  return true;
+}
+
 int plan_scan(const Tuning& tune, DeviceLimits lim, const pb200_query* query, pb200_segment* const* segments, int nseg,
               bool allow_count_carrier, ScanPlan* out) {
   if (!query || !segments || !out || nseg <= 0) { set_error("invalid argument to pb200_execute"); return PB200_E_INVALID; }
@@ -73,32 +90,16 @@ int plan_scan(const Tuning& tune, DeviceLimits lim, const pb200_query* query, pb
   }
 
   if (merge && nseg > 1) {
-    // One result for all segments == a merge of dictId-indexed state (group tables, MIN / MAX ids, DISTINCTCOUNT bitsets).
-    // That is only a merge BY VALUE (GroupByCombineOperator.java:130-146, AggregationFunction.merge) when the column has
-    // the same dictionary everywhere: compare content hashes, not cardinalities.  Bound segments (pb200_domain_*) pass by
-    // construction; anything else is refused so that the caller combines per-segment results itself.
-    auto same_dictionary = [&](int col, const char* what) -> bool {
-      const DeviceColumn& c0 = segments[0]->cols[col];
-      for (int s = 1; s < nseg; s++) {
-        const DeviceColumn& c = segments[s]->cols[col];
-        if (c.dict_hash != c0.dict_hash || c.cardinality != c0.cardinality || c.stored_type != c0.stored_type) {
-          set_error("PB200_Q_MERGE_SEGMENTS: %s column %d has a different dictionary in segment %d than in segment 0 "
-                    "(bind the segments to a pb200_domain first)", what, col, s);
-          return false;
-        }
-      }
-      return true;
-    };
     for (int g = 0; g < ngb; g++) {
       const int c = query->group_by_columns[g];
-      if (c >= 0 && c < ncols && !same_dictionary(c, "group-by")) return PB200_E_UNSUPPORTED;
+      if (c >= 0 && c < ncols && !same_dictionary(segments, nseg, c, "group-by")) return PB200_E_UNSUPPORTED;
     }
     for (int a = 0; a < nagg; a++) {
       const pb200_agg& ag = query->aggs[a];
       if (ag.function != PB200_AGG_MIN && ag.function != PB200_AGG_MAX && ag.function != PB200_AGG_DISTINCTCOUNT) continue;
       if (ag.column < 0 || ag.column >= ncols) continue;
       if (segments[0]->cols[ag.column].bits == 32 && !segments[0]->cols[ag.column].dict_native) continue;  // raw values, no ids
-      if (!same_dictionary(ag.column, ag.function == PB200_AGG_DISTINCTCOUNT ? "DISTINCTCOUNT" : "MIN/MAX")) return PB200_E_UNSUPPORTED;
+      if (!same_dictionary(segments, nseg, ag.column, ag.function == PB200_AGG_DISTINCTCOUNT ? "DISTINCTCOUNT" : "MIN/MAX")) return PB200_E_UNSUPPORTED;
     }
   }
 
@@ -805,6 +806,86 @@ std::vector<int> selection_rescan(const SelectionPlan& p, pb200_segment* const* 
   std::vector<int> out;
   for (size_t s = 0; s < p.scan_docs.size(); s++)
     if (p.scan_docs[s] < segments[s]->num_docs && matches[s] < p.limit) out.push_back((int)s);
+  return out;
+}
+
+int plan_distinct(const Tuning& tune, DeviceLimits lim, const pb200_query* filter_only, const pb200_selection* distinct,
+                  pb200_segment* const* segments, int nseg, bool merge, bool prefix, DistinctPlan* out) {
+  if (!filter_only || !distinct || !segments || !out || nseg <= 0) { set_error("invalid argument to pb200_execute_distinct"); return PB200_E_INVALID; }
+  const int nkeys = distinct->num_columns;
+  if (nkeys <= 0 || !distinct->columns) { set_error("DISTINCT needs at least one column"); return PB200_E_INVALID; }
+  if (nkeys > kMaxDistinctColumns) { set_error("DISTINCT over %d columns (at most %d)", nkeys, kMaxDistinctColumns); return PB200_E_UNSUPPORTED; }
+  if (distinct->num_order_items < 0 || distinct->num_order_items > PB200_MAX_ORDER_BY) { set_error("DISTINCT ORDER BY with %d items (1..%d)", distinct->num_order_items, PB200_MAX_ORDER_BY); return PB200_E_INVALID; }
+  DistinctPlan& p = *out;
+  p = DistinctPlan();
+  // every order item names a DISTINCT column (SQL: ORDER BY items of a SELECT DISTINCT must appear in the select list)
+  std::vector<bool> ordered_col(nkeys, false);
+  for (int k = 0; k < distinct->num_order_items; k++) {
+    const int key = (int)(std::find(distinct->columns, distinct->columns + nkeys, distinct->order[k].column) - distinct->columns);
+    if (key == nkeys) { set_error("DISTINCT ORDER BY column %d is not one of the DISTINCT columns", distinct->order[k].column); return PB200_E_INVALID; }
+    if (ordered_col[key]) continue;
+    ordered_col[key] = true;
+    p.order_key.push_back(key);
+    p.order_desc.push_back(distinct->order[k].descending != 0);
+  }
+  if (int rc = plan_selection(tune, lim, filter_only, distinct, segments, nseg, prefix, &p.sel)) return rc;
+  // key columns: dictIds (a raw column streamed as 32-bit values has none)
+  for (int k = 0; k < nkeys; k++) {
+    const int col = distinct->columns[k];
+    for (int s = 0; s < nseg; s++) {
+      const DeviceColumn& c = segments[s]->cols[col];
+      if (c.bits > 31 || c.cardinality <= 0 || c.fwd_kind != PB200_FWD_DICT_FIXEDBIT) {
+        set_error("DISTINCT column %d is not dictionary-encoded in segment %d: not accelerated", col, s);
+        return PB200_E_UNSUPPORTED;
+      }
+    }
+    if (merge && nseg > 1 && !same_dictionary(segments, nseg, col, "DISTINCT")) return PB200_E_UNSUPPORTED;
+  }
+  p.nres = merge ? 1 : nseg;
+  p.cards.resize(nseg);
+  p.mult.resize(nseg);
+  for (int s = 0; s < nseg; s++) {
+    long long space = 1;
+    for (int k = 0; k < nkeys; k++) {
+      const int card = segments[s]->cols[distinct->columns[k]].cardinality;
+      p.cards[s].push_back(card);
+      p.mult[s].push_back((uint32_t)space);
+      space *= card;
+      if (space > kMaxDistinctKeys) {
+        set_error("DISTINCT key space of segment %d above %lld entries: not accelerated", s, kMaxDistinctKeys);
+        return PB200_E_UNSUPPORTED;
+      }
+    }
+    if (!merge || s == 0) {
+      p.table_off.push_back(p.table_entries);
+      p.table_size.push_back(space);
+      p.table_entries += space;
+    }
+  }
+  if (p.table_entries > kMaxDistinctEntries) {
+    set_error("DISTINCT tables of %lld entries in one call (at most %lld)", p.table_entries, kMaxDistinctEntries);
+    return PB200_E_UNSUPPORTED;
+  }
+  return PB200_OK;
+}
+
+std::vector<unsigned long long> distinct_bounds(const DistinctPlan& p, pb200_segment* const* segments) {
+  const int nseg = (int)p.sel.scan_docs.size();
+  std::vector<unsigned long long> bound(p.nres, kDistinctEmpty);
+  for (int s = nseg - 1; s >= 0; s--)   // the earliest truncated segment of each result wins
+    if (p.sel.scan_docs[s] < segments[s]->num_docs)
+      bound[p.nres == 1 ? 0 : s] = (unsigned long long)s << 32 | (unsigned long long)p.sel.scan_docs[s];
+  return bound;
+}
+
+std::vector<int> distinct_rescan(const DistinctPlan& p, pb200_segment* const* segments, const std::vector<long long>& below) {
+  const int nseg = (int)p.sel.scan_docs.size();
+  const std::vector<unsigned long long> bound = distinct_bounds(p, segments);
+  std::vector<int> out;
+  for (int s = 0; s < nseg; s++) {
+    const int r = p.nres == 1 ? 0 : s;
+    if (p.sel.scan_docs[s] < segments[s]->num_docs && bound[r] != kDistinctEmpty && below[r] < p.sel.limit) out.push_back(s);
+  }
   return out;
 }
 

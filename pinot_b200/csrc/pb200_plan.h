@@ -115,6 +115,40 @@ int plan_selection(const Tuning& tune, DeviceLimits lim, const pb200_query* filt
 // matches in it (matches[s] = matched docs of segment s in the prefix).
 std::vector<int> selection_rescan(const SelectionPlan& p, pb200_segment* const* segments, const std::vector<long long>& matches);
 
+// ---- DISTINCT (pb200_execute_distinct): a selection scan, then a dense first-occurrence table per result ----
+constexpr int kMaxDistinctColumns = 8;                 // the group-by limit
+constexpr long long kMaxDistinctKeys = 1ll << 24;      // raw key space of one result's table
+constexpr long long kMaxDistinctEntries = 1ll << 27;   // table entries of all results of one call
+constexpr unsigned long long kDistinctEmpty = ~0ull;   // table entry without a match; else segment << 32 | doc
+
+struct DistinctPlan {
+  SelectionPlan sel;                      // the scan: columns = the DISTINCT columns, order items as given
+  int nres = 0;
+  // [segment][key column]: cardinality and multiplier, raw key = sum_k dictId_k x mult_k, mult_k = prod_{j<k} card_j
+  // (merged: the same in every segment, their dictionaries are one)
+  std::vector<std::vector<int>> cards;
+  std::vector<std::vector<uint32_t>> mult;
+  std::vector<long long> table_off, table_size;   // per result: first entry in the call's table block, entries
+  long long table_entries = 0;
+  std::vector<int> order_key;             // per order item kept: index of its column among the key columns
+  std::vector<bool> order_desc;           // (an item repeating an earlier item's column is dropped: it orders nothing)
+};
+
+// PB200_OK or the PB200_E_* code of pb200_execute_distinct for this input (refusals: see include/pinot_b200.h).  merge:
+// one result over all segments.  prefix as for plan_selection (ignored with order items).  No CUDA runtime call.
+int plan_distinct(const Tuning& tune, DeviceLimits lim, const pb200_query* filter_only, const pb200_selection* distinct,
+                  pb200_segment* const* segments, int nseg, bool merge, bool prefix, DistinctPlan* out);
+// The prefix-final rule.  bound[r]: (segment << 32 | prefix end) of the earliest segment of result r whose scan was cut
+// short, kDistinctEmpty when none was.  Every position before the bound has been scanned, so result r is final when at
+// least `limit` of its table's entries lie below it (below[r]).  Returns the truncated segments of every result that is
+// not final, to be scanned again in full into the same tables.
+std::vector<unsigned long long> distinct_bounds(const DistinctPlan& p, pb200_segment* const* segments);
+std::vector<int> distinct_rescan(const DistinctPlan& p, pb200_segment* const* segments, const std::vector<long long>& below);
+
+// PB200_Q_MERGE_SEGMENTS over dictIds: true when column `col` has the same dictionary in every segment; otherwise sets
+// the error ("`what` column ... bind the segments to a pb200_domain first") and returns false.
+bool same_dictionary(pb200_segment* const* segments, int nseg, int col, const char* what);
+
 // DictionaryBasedGroupKeyGenerator's key-holder regime for these group-by cardinalities (informational)
 int regime_of(const std::vector<int>& cards, int array_threshold);
 
@@ -124,5 +158,10 @@ TmaTable tma_table(const ScanPlan& plan, const LaunchChunk& c);
 // pb200_api.cu: allocates and fills the device buffers plan.leaf_buffers lists on `st` and points the leaf descriptors of
 // plan.segs at them; the buffers stay in `temps` until the launch that reads them is done.
 int bind_leaf_buffers(pb200_ctx* ctx, ScanPlan& plan, cudaStream_t st, std::vector<std::unique_ptr<DevBufRaw>>& temps);
+
+// pb200_select.cu: one scan launch of a selection plan on `st`: fills `mask` (p.mask_words words) and the matched docs of
+// each segment, adds the scan's CUDA-event time to *ms; ends in a stream synchronisation.
+int run_selection_scan(pb200_ctx* ctx, cudaStream_t st, SelectionPlan& p, DevBufRaw& mask, std::vector<long long>& matches,
+                       float* ms);
 
 }  // namespace pb200

@@ -38,11 +38,11 @@
 #include "pb200_internal.h"
 #include "pb200_plan.h"
 #include "pb200_scan_launch.h"
+#include "pb200_select.cuh"
 
 namespace pb200 {
 namespace {
 
-constexpr size_t kMappedBytes = 512ull << 10;
 constexpr int kSelThreads = 256;
 constexpr int kHistBits = 12;                 // order-key histogram: the key's top 12 bits
 constexpr int kHistBins = 1 << kHistBits;
@@ -58,23 +58,6 @@ struct SelSeg {            // one segment of the select phase
   uint32_t thresh;         // ORDER BY: largest first-key bucket compacted (kHistBins - 1: every match)
   int32_t seg;             // index in the submission
 };
-struct SelCol {            // one column (selected or order item) of one segment
-  const uint32_t* fwd;     // resident forward index, native word order (pb200_unpack.cuh)
-  const void* dict;        // device dictionary (INT: biased by 2^31) or NULL
-  int32_t bits, kind;      // kind: SEL_*
-  int32_t desc, pad;       // order items: DESC
-};
-
-// the stored 32-bit word at `doc`: dictId, or the raw value (MSB-first bit stream; a value may straddle two words)
-__device__ __forceinline__ uint32_t read_at(const SelCol& c, int32_t doc) {
-  const unsigned long long bit = (unsigned long long)doc * (unsigned)c.bits;
-  const uint32_t* p = c.fwd + (bit >> 5);
-  const int sh = (int)(bit & 31u);
-  const uint32_t hi = __ldg(p);
-  const uint32_t lo = sh + c.bits > 32 ? __ldg(p + 1) : 0u;
-  const uint32_t x = __funnelshift_l(lo, hi, sh);
-  return c.bits == 32 ? x : x >> (32 - c.bits);
-}
 // order-preserving 32-bit key (see the file comment)
 __device__ __forceinline__ uint32_t order_key(const SelCol& c, int32_t doc) {
   const uint32_t x = read_at(c, doc);
@@ -177,18 +160,7 @@ __global__ void sel_gather_kernel(const int32_t* __restrict__ docs, const int32_
     oseg[i] = s;
     for (int k = 0; k < ncols; k++) {
       const SelCol col = cols[(size_t)s * ncols + k];
-      const uint32_t id = read_at(col, d);
-      unsigned long long v;
-      switch (col.kind) {
-        case SEL_DICT_I32: v = (unsigned long long)(long long)(int32_t)(__ldg(static_cast<const uint32_t*>(col.dict) + id) ^ 0x80000000u); break;
-        case SEL_DICT_I64: v = (unsigned long long)__ldg(static_cast<const long long*>(col.dict) + id); break;
-        case SEL_DICT_F32: v = (unsigned long long)__double_as_longlong((double)__ldg(static_cast<const float*>(col.dict) + id)); break;
-        case SEL_DICT_F64: v = (unsigned long long)__double_as_longlong(__ldg(static_cast<const double*>(col.dict) + id)); break;
-        case SEL_RAW_I32: v = (unsigned long long)(long long)(int32_t)id; break;
-        case SEL_RAW_F32: v = (unsigned long long)__double_as_longlong((double)__int_as_float((int)id)); break;
-        default: v = (unsigned long long)id; break;  // SEL_DICT_ID: STRING dictIds
-      }
-      ocol[(size_t)k * rows + i] = v;
+      ocol[(size_t)k * rows + i] = sel_value(col, read_at(col, d));
     }
   }
 }
@@ -198,7 +170,8 @@ struct EventPair {
   ~EventPair() { give_event(c, a); give_event(c, b); }
 };
 
-// One scan launch of a selection plan: fills `mask` (p.mask_words words) and the matched docs of each segment.
+}  // namespace
+
 int run_selection_scan(pb200_ctx* ctx, cudaStream_t st, SelectionPlan& p, DevBufRaw& mask, std::vector<long long>& matches,
                        float* ms) {
   ScanPlan& plan = p.scan;
@@ -240,6 +213,8 @@ int run_selection_scan(pb200_ctx* ctx, cudaStream_t st, SelectionPlan& p, DevBuf
   *ms += t;
   return PB200_OK;
 }
+
+namespace {
 
 // By-value comparison of two output rows on one order item (merged ORDER BY over segments whose dictionaries may differ).
 int compare_item(const pb200_segment* const* segments, int col, int kind, bool desc, const unsigned long long* v, int32_t sa,
@@ -446,7 +421,7 @@ extern "C" int32_t pb200_execute_selection(pb200_ctx* ctx, const pb200_query* fi
       pick = pk;
     }
     unsigned char* dst = nullptr;
-    const bool mapped = out_bytes <= kMappedBytes;
+    const bool mapped = out_bytes <= kSelMappedBytes;
     if (mapped) {
       void* dp = nullptr;
       PB200_CUDA(cudaHostGetDevicePointer(&dp, block->p, 0));

@@ -661,6 +661,32 @@ class B200PlanMaker:
         self.last_device_ms = blocks[0].device_ms
         return blocks[0] if merge else blocks
 
+    def execute_distinct(self, segments: Sequence[IndexSegment], query, merge: bool = False):
+        """A DISTINCT query (sql.DistinctQuery) over the segments in ONE device submission: per segment its first `limit`
+        distinct tuples in order of first occurrence, or with an ORDER BY its top `limit` tuples, ties by first
+        occurrence.  merge=True: one block over all segments (every DISTINCT column bound to one domain; otherwise
+        UnsupportedQueryError) -- merge_distinct_blocks combines per-segment blocks by value instead.  Returns a list of
+        DistinctResultsBlock, one per segment, or one block when merged."""
+        columns = list(query.columns)
+        if len(query.order_by) > _lib.MAX_ORDER_BY:
+            raise ValueError(f"ORDER BY has {len(query.order_by)} items, at most {_lib.MAX_ORDER_BY} are supported")
+        hq, _keep = _marshal_query(QueryContext(aggregations=[], filter=query.filter), merge)
+        names = [c.encode() for c in columns]
+        cnames = (C.c_char_p * max(1, len(names)))(*names)
+        onames = [c.encode() for c, _ in query.order_by]
+        sel = _lib.HSelection(len(columns), cnames, len(onames))
+        for k, (name, (_, asc)) in enumerate(zip(onames, query.order_by)):
+            sel.order[k] = _lib.HSelectOrder(name, int(not asc))
+        sel.limit = int(query.limit)
+        n = len(segments)
+        segs = (C.c_void_p * n)(*[s.handle for s in segments])
+        nres = 1 if merge else n
+        res = (C.c_void_p * nres)()
+        _lib.check(self.ctx.lib.pb200h_execute_distinct(self.ctx.handle, C.byref(hq), C.byref(sel), segs, n, res))
+        blocks = [_read_selection(self.ctx, C.c_void_p(res[i]), segments, columns, DistinctResultsBlock) for i in range(nres)]
+        self.last_device_ms = blocks[0].device_ms
+        return blocks[0] if merge else blocks
+
 
 @dataclass
 class SelectionResultsBlock:
@@ -678,7 +704,42 @@ class SelectionResultsBlock:
         return len(self.doc_ids)
 
 
-def _read_selection(ctx: B200Context, handle, segments: Sequence[IndexSegment], columns: Sequence[str]) -> SelectionResultsBlock:
+@dataclass
+class DistinctResultsBlock(SelectionResultsBlock):
+    """What a DistinctResultsBlock is built from: one row per distinct tuple, values typed as in a selection, doc_ids /
+    segment_index = the tuple's first occurrence."""
+
+
+def merge_distinct_blocks(blocks: Sequence[SelectionResultsBlock], order_by=(), limit: int = 10) -> DistinctResultsBlock:
+    """By-value merge of per-segment DISTINCT blocks of one submission (segment_index refers to that submission): the
+    union of their tuples, each with its earliest (segment, doc) occurrence, ordered by first occurrence or by `order_by`
+    ([(column, ascending)], ties by first occurrence), then the first `limit`.  Exact, because each segment's block holds
+    its own first (or top) `limit` tuples."""
+    names = list(blocks[0].names)
+    first: Dict[tuple, tuple] = {}
+    for b in blocks:
+        for i in range(b.num_rows):
+            key = tuple(c[i].item() if hasattr(c[i], "item") else c[i] for c in b.columns)
+            occ = (int(b.segment_index[i]), int(b.doc_ids[i]))
+            if key not in first or occ < first[key]:
+                first[key] = occ
+    rows = sorted(first.items(), key=lambda kv: kv[1])
+    for col, asc in reversed(list(order_by)):   # stable passes, last item first
+        k = names.index(col)
+        rows.sort(key=lambda kv: kv[0][k], reverse=not asc)
+    rows = rows[:limit]
+    columns = []
+    for k, c in enumerate(blocks[0].columns):
+        vals = [kv[0][k] for kv in rows]
+        columns.append(np.array(vals, dtype=object) if c.dtype == object else np.array(vals, dtype=c.dtype))
+    stats = ExecutionStatistics(*(sum(getattr(b.stats, f) for b in blocks) for f in
+                                  ("num_docs_scanned", "num_entries_scanned_in_filter", "num_entries_scanned_post_filter", "num_total_docs")))
+    return DistinctResultsBlock(names, columns, np.array([kv[1][1] for kv in rows], dtype=np.int32),
+                                np.array([kv[1][0] for kv in rows], dtype=np.int32), stats, sum(b.device_ms for b in blocks[:1]))
+
+
+def _read_selection(ctx: B200Context, handle, segments: Sequence[IndexSegment], columns: Sequence[str],
+                    block_class=SelectionResultsBlock) -> SelectionResultsBlock:
     L = ctx.lib
     try:
         meta = _lib.ResultMeta()
@@ -714,6 +775,6 @@ def _read_selection(ctx: B200Context, handle, segments: Sequence[IndexSegment], 
                 out.append(copy(cols[k], C.c_int64, np.int64))
         stats = ExecutionStatistics(meta.num_docs_scanned, meta.num_entries_scanned_in_filter,
                                     meta.num_entries_scanned_post_filter, meta.num_total_docs)
-        return SelectionResultsBlock(list(columns), out, doc_ids, seg_index, stats, float(meta.device_ms))
+        return block_class(list(columns), out, doc_ids, seg_index, stats, float(meta.device_ms))
     finally:
         L.pb200_result_free(handle)

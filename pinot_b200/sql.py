@@ -9,6 +9,8 @@ stays Java).  This module exists so the parity tests read like the reference's
     SELECT item[, item...] FROM table [WHERE cond] [GROUP BY col[, col...]] [ORDER BY expr [ASC|DESC], ...] [LIMIT n]
     item  := COUNT(*) | FN(col) | col            (plain columns are allowed only when they are group-by keys)
     selection (parse_selection): SELECT * | col[, col...] FROM table [WHERE cond] [ORDER BY col [ASC|DESC], ...] [LIMIT n]
+    distinct (parse_distinct): SELECT DISTINCT col[, col...] FROM table [WHERE cond] [ORDER BY col [ASC|DESC], ...] [LIMIT n]
+                  (every ORDER BY column must be a DISTINCT column)
     cond  := cond AND cond | cond OR cond | NOT cond | (cond) | col op literal | col BETWEEN a AND b
              | col [NOT] IN (literal, ...)
     op    := = | != | <> | < | <= | > | >=
@@ -315,3 +317,65 @@ def parse_selection(sql: str) -> SelectionQuery:
     if p.peek()[0] is not None:
         raise SqlError(f"trailing tokens: {p.toks[p.i:]}")
     return SelectionQuery(columns=columns, filter=optimize_filter(flt), order_by=order_by, limit=limit, table=table)
+
+
+@dataclass
+class DistinctQuery:
+    """SELECT DISTINCT columns FROM table WHERE ... [ORDER BY col [ASC|DESC], ...] LIMIT n (the reference's DISTINCT
+    query shape).  Every order column is one of `columns`."""
+    columns: List[str]
+    filter: Optional[FilterNode] = None
+    order_by: List[tuple] = field(default_factory=list)  # (column, ascending)
+    limit: int = 10
+    table: str = "testTable"
+
+
+def is_distinct(sql: str) -> bool:
+    """True when the statement starts with SELECT DISTINCT."""
+    p = _Parser(sql)
+    return p.take_kw("SELECT") and p.kw("DISTINCT")
+
+
+def parse_distinct(sql: str) -> DistinctQuery:
+    """SQL text of a SELECT DISTINCT query -> DistinctQuery (filter run through the broker-side filter optimizers)."""
+    p = _Parser(sql)
+    p.expect_kw("SELECT")
+    p.expect_kw("DISTINCT")
+    if p.peek() == ("op", "*"):
+        raise SqlError("DISTINCT * is not supported: name the columns")
+    columns: List[str] = []
+    while True:
+        name = p.ident()
+        if p.peek() == ("op", "("):
+            raise SqlError(f"{name}(...) in a DISTINCT select list: functions and expressions are not supported")
+        columns.append(name)
+        if not p.take_op(","):
+            break
+    p.expect_kw("FROM")
+    table = p.ident()
+    flt: Optional[FilterNode] = None
+    if p.take_kw("WHERE"):
+        flt = p.cond()
+    if p.kw("GROUP"):
+        raise SqlError("GROUP BY in a DISTINCT query")
+    order_by = []
+    if p.take_kw("ORDER"):
+        p.expect_kw("BY")
+        while True:
+            name = p.ident()
+            if name not in columns:
+                raise SqlError(f"ORDER BY {name}: a DISTINCT query can only order by its selected columns")
+            asc = not p.take_kw("DESC")
+            if asc:
+                p.take_kw("ASC")
+            order_by.append((name, asc))
+            if not p.take_op(","):
+                break
+    limit = 10
+    if p.take_kw("LIMIT"):
+        limit = p.literal()
+        if not isinstance(limit, int) or limit < 0:
+            raise SqlError(f"LIMIT must be a non-negative integer, got {limit!r}")
+    if p.peek()[0] is not None:
+        raise SqlError(f"trailing tokens: {p.toks[p.i:]}")
+    return DistinctQuery(columns=columns, filter=optimize_filter(flt), order_by=order_by, limit=limit, table=table)
