@@ -185,9 +185,9 @@ typedef struct {
 #define PB200_NODE_IDS_ON_DEVICE 1
 
 /* Aggregation functions accelerated on this path (core/query/aggregation/function/{Count,Sum,Min,Max,Avg,
- * DistinctCount}AggregationFunction.java). */
+ * DistinctCount,Percentile}AggregationFunction.java).  PERCENTILE takes its percentile through pb200_execute_args. */
 enum { PB200_AGG_COUNT = 0, PB200_AGG_SUM = 1, PB200_AGG_MIN = 2, PB200_AGG_MAX = 3, PB200_AGG_AVG = 4,
-       PB200_AGG_DISTINCTCOUNT = 5 };
+       PB200_AGG_DISTINCTCOUNT = 5, PB200_AGG_PERCENTILE = 6 };
 
 typedef struct {
   int32_t function; /* PB200_AGG_* */
@@ -254,6 +254,30 @@ typedef struct {
  * Aggregation-only queries ignore it.  A bad item index or num_items outside 1..8: PB200_E_INVALID. */
 int32_t pb200_execute_ordered(pb200_ctx* ctx, const pb200_query* query, const pb200_order_by* order,
                               pb200_segment* const* segments, int32_t num_segments, pb200_result** results);
+
+/* ---- PERCENTILE(col, p): exact percentiles from per-group dictId histograms ------------------------------------------ */
+/* pb200_execute_ordered with one argument per aggregation: agg_args[a] is the percentile p (0 <= p <= 100, fractions
+ * allowed) of a PB200_AGG_PERCENTILE aggregation and is ignored for the other functions.  agg_args == NULL is
+ * pb200_execute_ordered, which refuses PERCENTILE with PB200_E_INVALID (as does a p outside [0, 100] or NaN).
+ * Semantics (PercentileAggregationFunction.extractFinalResult): the n values of the column over the group's matched rows,
+ * as doubles, sorted ascending; n == 0: -inf; p == 100: the largest; otherwise the value at index
+ * (int64)((double)n * p / 100.0), clamped to n - 1.  The column must carry dictIds (INT / LONG / FLOAT / DOUBLE
+ * dictionaries, raw columns whose dictionary was synthesised at load): a dictionary is sorted, so a histogram of counts
+ * over dictIds is the sorted value list.  Several PERCENTILEs of one column share one histogram.
+ * Results: pb200_result_agg gives the value (double column) and n (long column), pb200_result_agg_dict_ids the selected
+ * dictId (-1 when n == 0), so that a LONG beyond 2^53 can be looked up exactly; ORDER BY compares the double value.
+ * PB200_E_UNSUPPORTED (the caller runs the stock operator): STRING columns, raw columns streamed as 32-bit values,
+ * histograms above 2^28 entries over all results of the call (aggregation only: 2^bits per result; group-by: table
+ * entries x cardinality), a result over 2^32 docs or more, PB200_Q_DEFER_FINALIZE; a PB200_Q_MERGE_SEGMENTS submission
+ * needs the column's dictionary to be the same in every segment.  NaN and -0.0 are out of scope, as for MIN / MAX. */
+int32_t pb200_execute_args(pb200_ctx* ctx, const pb200_query* query, const pb200_order_by* order, const double* agg_args,
+                           pb200_segment* const* segments, int32_t num_segments, pb200_result** results);
+/* The histogram behind PERCENTILE aggregation `agg` in row `row`: its non-zero bins ascending by dictId (counts > 0), the
+ * intermediate for merging per-segment results by value (the analogue of pb200_result_distinct).  Returns the number of
+ * bins (or < 0 on error) and writes at most `capacity` of them; either output may be NULL.  The histograms are copied from
+ * the device on the first call for a result, so a caller that reads only the final values pays nothing for them. */
+int64_t pb200_result_histogram(const pb200_result* result, int32_t agg, int32_t row, int32_t* dict_ids, int64_t* counts,
+                               int64_t capacity);
 
 /* ---- selection: SELECT columns WHERE ... [ORDER BY columns] LIMIT n (SelectionOnlyOperator, SelectionOrderByOperator) -- */
 /* Without order items: per segment, the first `limit` matching docs in doc-id order with the values of the selected
@@ -368,7 +392,8 @@ int32_t pb200_result_columns(const pb200_result* result, const int32_t** keys, c
 int32_t pb200_result_free(pb200_result* result);
 
 /* ---- multi-GPU combine support (dense group tables with shared dictionaries) ----------------------------------- */
-/* Device pointers + element counts of the dense accumulator arrays of a merged group-by result, so that the caller's
+/* Results with DISTINCTCOUNT bitsets or PERCENTILE histograms are refused (PB200_E_UNSUPPORTED).
+ * Device pointers + element counts of the dense accumulator arrays of a merged group-by result, so that the caller's
  * collective layer (torch.distributed / NCCL) can all-reduce them in place across ranks:
  *   kind 0: int64 sums/counts (reduce SUM)   kind 1: double sums (SUM)   kind 2: uint32 max-encoded (reduce MAX)
  * After the collective, pb200_result_finalize() re-extracts the groups on the root rank. */

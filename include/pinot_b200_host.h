@@ -186,6 +186,12 @@ int32_t pb200h_execute(pb200_ctx* ctx, const pb200h_query* query, pb200h_segment
 int32_t pb200h_execute_ordered(pb200_ctx* ctx, const pb200h_query* query, const pb200_order_by* order,
                                pb200h_segment* const* segments, int32_t num_segments, pb200_result** results,
                                int32_t* operator_kinds);
+/* pb200h_execute_ordered with one argument per aggregation (pb200_execute_args: the percentile of a PERCENTILE).
+ * PERCENTILE in a query with any FILTER (WHERE ...) clause is PB200_E_UNSUPPORTED; agg_args == NULL refuses PERCENTILE
+ * with PB200_E_INVALID. */
+int32_t pb200h_execute_args(pb200_ctx* ctx, const pb200h_query* query, const pb200_order_by* order, const double* agg_args,
+                            pb200h_segment* const* segments, int32_t num_segments, pb200_result** results,
+                            int32_t* operator_kinds);
 /* ---- selection (SELECT columns WHERE ... LIMIT n; pb200_execute_selection of include/pinot_b200.h) --------------- */
 typedef struct {
   const char* column;

@@ -16,7 +16,7 @@ E_INVALID, E_UNSUPPORTED, E_CUDA, E_NOMEM, E_LIMIT = -1, -2, -3, -4, -5
 
 INT, LONG, FLOAT, DOUBLE, STRING = 0, 1, 2, 3, 4
 FWD_DICT_FIXEDBIT, FWD_DICT_SORTED, FWD_RAW_FIXEDBYTE = 0, 1, 2
-AGG_CODES = {"COUNT": 0, "SUM": 1, "MIN": 2, "MAX": 3, "AVG": 4, "DISTINCTCOUNT": 5}
+AGG_CODES = {"COUNT": 0, "SUM": 1, "MIN": 2, "MAX": 3, "AVG": 4, "DISTINCTCOUNT": 5, "PERCENTILE": 6}
 FILTER_CODES = {"AND": 0, "OR": 1, "NOT": 2, "EQ": 3, "NEQ": 4, "IN": 5, "NOT_IN": 6, "RANGE": 7}
 REGIMES = {0: "NONE", 1: "ARRAY", 2: "INT_MAP", 3: "LONG_MAP", 4: "ARRAY_MAP"}
 OPERATOR_KINDS = {0: "AGGREGATION", 1: "GROUP_BY", 2: "NON_SCAN_AGGREGATION", 3: "EMPTY", 4: "STAR_TREE"}
@@ -163,6 +163,7 @@ EXPORTED_SYMBOLS = [
     "pb200_last_phases", "pb200_result_columns", "pb200_doc_mask_upload", "pb200_doc_mask_free", "pb200_roaring_validate", "pb200_comm_unique_id", "pb200_comm_init", "pb200_comm_shutdown", "pb200_result_combine",
     "pb200_execute_selection", "pb200_result_selection", "pb200h_execute_selection",
     "pb200_execute_distinct", "pb200h_execute_distinct",
+    "pb200_execute_args", "pb200h_execute_args", "pb200_result_histogram",
 ]
 
 _LIB = None
@@ -188,6 +189,10 @@ def load() -> C.CDLL:
     L.pb200_segment_device_bytes.argtypes = [vp]
     L.pb200_execute.argtypes = [vp, C.POINTER(Query), C.POINTER(vp), i32, C.POINTER(vp)]
     L.pb200_execute_ordered.argtypes = [vp, C.POINTER(Query), C.POINTER(OrderBy), C.POINTER(vp), i32, C.POINTER(vp)]
+    L.pb200_execute_args.argtypes = [vp, C.POINTER(Query), C.POINTER(OrderBy), C.POINTER(C.c_double), C.POINTER(vp), i32,
+                                     C.POINTER(vp)]
+    L.pb200_result_histogram.restype = i64
+    L.pb200_result_histogram.argtypes = [vp, i32, i32, vp, vp, i64]
     L.pb200_result_meta_get.argtypes = [vp, C.POINTER(ResultMeta)]
     L.pb200_result_group_keys.argtypes = [vp, vp]
     L.pb200_result_agg.argtypes = [vp, i32, vp, vp]
@@ -218,6 +223,8 @@ def load() -> C.CDLL:
     L.pb200h_execute.argtypes = [vp, C.POINTER(HQuery), C.POINTER(vp), i32, C.POINTER(vp), C.POINTER(i32)]
     L.pb200h_execute_ordered.argtypes = [vp, C.POINTER(HQuery), C.POINTER(OrderBy), C.POINTER(vp), i32, C.POINTER(vp),
                                          C.POINTER(i32)]
+    L.pb200h_execute_args.argtypes = [vp, C.POINTER(HQuery), C.POINTER(OrderBy), C.POINTER(C.c_double), C.POINTER(vp), i32,
+                                      C.POINTER(vp), C.POINTER(i32)]
     L.pb200h_explain.argtypes = [vp, C.POINTER(HQuery), vp, C.c_char_p, i32]
     L.pb200h_startree_attach.argtypes = [vp, vp, vp, C.c_uint64, i32, i32, C.POINTER(C.c_char_p), C.POINTER(vp),
                                          C.POINTER(C.c_uint64), i32, C.POINTER(HStarMetric)]

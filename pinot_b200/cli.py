@@ -22,7 +22,8 @@ from typing import Dict, List
 
 def merge_blocks(query, segments, blocks) -> Dict[tuple, list]:
     """{key values: [intermediate per aggregation]} over all blocks: COUNT -> int, SUM / MIN / MAX -> float,
-    AVG -> (sum, count), DISTINCTCOUNT -> set of values (GroupByCombineOperator / AggregationFunction.merge)."""
+    AVG -> (sum, count), DISTINCTCOUNT -> set of values, PERCENTILE -> (p, {value: count}) from the per-segment
+    histograms, or its final float for a block merged on the device (GroupByCombineOperator / AggregationFunction.merge)."""
     out: Dict[tuple, list] = {}
     for seg, b in zip(segments, blocks):
         rows = 1 if b.num_groups < 0 else b.num_groups
@@ -37,6 +38,13 @@ def merge_blocks(query, segments, blocks) -> Dict[tuple, list]:
                     vals.append((float(b.doubles[a][g]), int(b.longs[a][g])))
                 elif fn == "DISTINCTCOUNT":
                     vals.append({seg.dictionary_value(agg.column, int(d)) for d in b.distinct[(a, g)]})
+                elif fn == "PERCENTILE" and (a, g) in b.histograms:
+                    ids, counts = b.histograms[(a, g)]
+                    hist: Dict[float, int] = {}
+                    for d, c in zip(ids, counts):
+                        v = float(seg.dictionary_value(agg.column, int(d)))
+                        hist[v] = hist.get(v, 0) + int(c)
+                    vals.append((agg.arg, hist))
                 else:
                     vals.append(float(b.doubles[a][g]))
             cur = out.get(key)
@@ -53,6 +61,9 @@ def merge_blocks(query, segments, blocks) -> Dict[tuple, list]:
                     cur[a] = max(cur[a], vals[a])
                 elif fn == "AVG":
                     cur[a] = (cur[a][0] + vals[a][0], cur[a][1] + vals[a][1])
+                elif fn == "PERCENTILE" and isinstance(cur[a], tuple):
+                    for v, c in vals[a][1].items():
+                        cur[a][1][v] = cur[a][1].get(v, 0) + c
                 else:
                     cur[a] |= vals[a]
     return out
@@ -71,6 +82,7 @@ def final_rows(query, table: Dict[tuple, list]) -> List[list]:
     DISTINCTCOUNT = set size) and breaks ties by the key values ascending, in GROUP BY column order -- the library's order.
     Without ORDER BY Pinot returns an arbitrary LIMIT-sized subset; here the rows are sorted by key to make the output
     stable."""
+    from .query import percentile_of_counts
     from .sql import resolve_order_by
     items = resolve_order_by(query) if query.is_group_by else []
     rows = []
@@ -82,6 +94,8 @@ def final_rows(query, table: Dict[tuple, list]) -> List[list]:
                 vals.append(v[0] / v[1] if v[1] else float("-inf"))
             elif agg.function == "DISTINCTCOUNT":
                 vals.append(len(v))
+            elif agg.function == "PERCENTILE" and isinstance(v, tuple):
+                vals.append(percentile_of_counts(v))
             else:
                 vals.append(v)
         rows.append(list(key) + vals)
@@ -120,7 +134,7 @@ def main(argv=None) -> int:
         try:
             if args.merge_on_device and len(segments) > 1:
                 cols = list(dict.fromkeys(list(query.group_by) + [a.column for a in query.aggregations
-                                                                  if a.column and a.function in ("MIN", "MAX", "DISTINCTCOUNT")]))
+                                                                  if a.column and a.function in ("MIN", "MAX", "DISTINCTCOUNT", "PERCENTILE")]))
                 if cols:
                     domain = DictionaryDomain.build(ctx, segments, cols)
                     for s in segments:

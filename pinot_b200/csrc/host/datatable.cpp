@@ -75,6 +75,11 @@ extern "C" int64_t pb200h_result_to_datatable(const pb200h_query* q, const pb200
   if (pb200_result_meta_get(R, &meta)) return PB200_E_INVALID;
   const int ngb = q->num_group_by, nagg = q->num_aggs;
   if (meta.num_group_by != ngb || meta.num_aggs != nagg) { set_error("result does not belong to this query"); return PB200_E_INVALID; }
+  for (int a = 0; a < nagg; a++)
+    if (q->aggs[a].function == PB200_AGG_PERCENTILE) {  // its intermediate is the reference's DoubleArrayList of values
+      set_error("PERCENTILE intermediates are not written as DataTable objects");
+      return PB200_E_UNSUPPORTED;
+    }
   const size_t rows = meta.num_groups < 0 ? 1 : (size_t)meta.num_groups;
   // ---- intermediates through the C-ABI accessors ----
   std::vector<int32_t> keys(rows * (size_t)std::max(ngb, 1));

@@ -233,6 +233,7 @@ pb200_result* host_result(const pb200h_segment& seg, const pb200h_query& q, bool
       case PB200_AGG_SUM: case PB200_AGG_AVG: d = 0; l = 0; break;
       case PB200_AGG_MIN: if (empty) d = INFINITY; else { id = c->to_device_id(0); d = c->as_double(0); } break;
       case PB200_AGG_MAX: if (empty) d = -INFINITY; else { id = c->to_device_id(c->cardinality - 1); d = c->as_double(c->cardinality - 1); } break;
+      case PB200_AGG_PERCENTILE: d = -INFINITY; break;   // only reached for an empty match (never answered without a scan)
       case PB200_AGG_DISTINCTCOUNT: {
         std::vector<int32_t> ids;
         if (!empty) for (int i = 0; i < c->cardinality; i++) ids.push_back(c->to_device_id(i));
@@ -671,10 +672,30 @@ extern "C" int32_t pb200h_execute(pb200_ctx* ctx, const pb200h_query* q, pb200h_
 
 extern "C" int32_t pb200h_execute_ordered(pb200_ctx* ctx, const pb200h_query* q, const pb200_order_by* order,
                                           pb200h_segment* const* segs, int32_t nseg, pb200_result** results, int32_t* kinds) {
+  return pb200h_execute_args(ctx, q, order, nullptr, segs, nseg, results, kinds);
+}
+
+extern "C" int32_t pb200h_execute_args(pb200_ctx* ctx, const pb200h_query* q, const pb200_order_by* order, const double* agg_args,
+                                       pb200h_segment* const* segs, int32_t nseg, pb200_result** results, int32_t* kinds) {
   if (!ctx || !q || !segs || !results || nseg <= 0) { set_error("invalid argument to pb200h_execute"); return PB200_E_INVALID; }
   if (q->num_aggs <= 0) { set_error("selection queries are outside this path"); return PB200_E_UNSUPPORTED; }
   if (int vrc = pb200::order_validate(order, q->num_aggs, q->num_group_by)) return vrc;
   if (q->num_group_by == 0) order = nullptr;  // aggregation only: one row, nothing to order
+  bool any_clause = false;   // some aggregation has a FILTER (WHERE ...) clause
+  if (q->agg_filter_count && q->agg_filter_start && q->agg_filter_nodes)
+    for (int a = 0; a < q->num_aggs; a++) any_clause |= q->agg_filter_count[a] > 0;
+  for (int a = 0; a < q->num_aggs; a++) {
+    if (q->aggs[a].function != PB200_AGG_PERCENTILE) continue;
+    // the same checks as the device path, made before any segment can be answered on the host
+    if (!agg_args) { set_error("PERCENTILE (aggregation %d) needs its percentile: call pb200h_execute_args", a); return PB200_E_INVALID; }
+    if (!(agg_args[a] >= 0.0 && agg_args[a] <= 100.0)) { set_error("PERCENTILE (aggregation %d): percentile %g outside [0, 100]", a, agg_args[a]); return PB200_E_INVALID; }
+    // FILTER clauses run as one submission per clause (host/filtered_agg.cpp), which carries no percentiles: a PERCENTILE
+    // anywhere in such a query -- with its own clause or next to another function's -- goes to the stock operator
+    if (any_clause) {
+      set_error("PERCENTILE in a query with FILTER (WHERE ...) clauses is not accelerated");
+      return PB200_E_UNSUPPORTED;
+    }
+  }
   if (q->agg_filter_count && q->agg_filter_start && q->agg_filter_nodes)
     for (int a = 0; a < q->num_aggs; a++)
       if (q->agg_filter_count[a] > 0) return execute_filtered(ctx, *q, order, segs, nseg, results, kinds);  // host/filtered_agg.cpp
@@ -761,7 +782,7 @@ extern "C" int32_t pb200h_execute_ordered(pb200_ctx* ctx, const pb200h_query* q,
     dq.filter = flat.data();
     dq.group_by_columns = gb.data();
     dq.aggs = aggs.data();
-    int rc = pb200_execute_ordered(ctx, &dq, order, dsegs.data(), (int)dsegs.size(), dev_results.data());
+    int rc = pb200_execute_args(ctx, &dq, order, agg_args, dsegs.data(), (int)dsegs.size(), dev_results.data());
     if (rc) { for (auto r : star_results) if (r) pb200_result_free(r); return rc; }
   }
   if (merge) { results[0] = dev_results[0]; return PB200_OK; }

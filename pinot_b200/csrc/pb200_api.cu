@@ -16,6 +16,7 @@
 #include <memory>
 
 #include "pb200_internal.h"
+#include "pb200_percentile.h"
 #include "pb200_plan.h"
 #include "pb200_scan_launch.h"
 #include "pb200_unpack.cuh"
@@ -675,14 +676,19 @@ int bind_leaf_buffers(pb200_ctx* ctx, ScanPlan& plan, cudaStream_t st, std::vect
 // after the launch) -- the caller runs the submission again with separate COUNT reductions.
 constexpr int kRetryWithoutCountCarrier = 1;
 static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment* const* segments, int32_t nseg,
-                        pb200_result** results, bool allow_count_carrier, const pb200_order_by* order);
+                        pb200_result** results, bool allow_count_carrier, const pb200_order_by* order, const double* agg_args);
+
+extern "C" int32_t pb200_execute_args(pb200_ctx* ctx, const pb200_query* query, const pb200_order_by* order, const double* agg_args,
+                                      pb200_segment* const* segments, int32_t nseg, pb200_result** results) {
+  if (query) { const int vrc = order_validate(order, query->num_aggs, query->num_group_by); if (vrc) return vrc; }
+  int rc = execute_impl(ctx, query, segments, nseg, results, true, order, agg_args);
+  if (rc == kRetryWithoutCountCarrier) rc = execute_impl(ctx, query, segments, nseg, results, false, order, agg_args);
+  return rc;
+}
 
 extern "C" int32_t pb200_execute_ordered(pb200_ctx* ctx, const pb200_query* query, const pb200_order_by* order,
                                          pb200_segment* const* segments, int32_t nseg, pb200_result** results) {
-  if (query) { const int vrc = order_validate(order, query->num_aggs, query->num_group_by); if (vrc) return vrc; }
-  int rc = execute_impl(ctx, query, segments, nseg, results, true, order);
-  if (rc == kRetryWithoutCountCarrier) rc = execute_impl(ctx, query, segments, nseg, results, false, order);
-  return rc;
+  return pb200_execute_args(ctx, query, order, nullptr, segments, nseg, results);
 }
 
 extern "C" int32_t pb200_execute(pb200_ctx* ctx, const pb200_query* query, pb200_segment* const* segments,
@@ -710,7 +716,7 @@ __global__ void carrier_verify_kernel(const unsigned long long* __restrict__ tab
 }
 
 static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment* const* segments, int32_t nseg,
-                        pb200_result** results, bool allow_count_carrier, const pb200_order_by* order) {
+                        pb200_result** results, bool allow_count_carrier, const pb200_order_by* order, const double* agg_args) {
   if (!ctx || !query || !segments || !results || nseg <= 0) { set_error("invalid argument to pb200_execute"); return PB200_E_INVALID; }
   const double t_enter = now_ms();
   PB200_CUDA(cudaSetDevice(ctx->device));
@@ -721,7 +727,7 @@ static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment*
   const Tuning tune = [&]() { std::lock_guard<std::mutex> g(ctx->mu); return ctx->tune; }();
   ScanPlan plan;
   {
-    const int rc = plan_scan(tune, DeviceLimits{ctx->sm_count, ctx->max_smem_optin}, query, segments, nseg, allow_count_carrier, &plan);
+    const int rc = plan_scan(tune, DeviceLimits{ctx->sm_count, ctx->max_smem_optin}, query, segments, nseg, allow_count_carrier, &plan, agg_args);
     if (rc) return rc;
   }
   const QueryDesc& q = plan.q;
@@ -731,7 +737,13 @@ static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment*
   cudaStream_t st = take_stream(ctx);
   struct StreamReturn { pb200_ctx* c; cudaStream_t s; ~StreamReturn() { give_stream(c, s); } } stream_return{ctx, st};
   std::vector<std::unique_ptr<pb200_result>> res;
-  for (int r = 0; r < nres; r++) res.emplace_back(new pb200_result());
+  for (int r = 0; r < nres; r++) {
+    res.emplace_back(new pb200_result());
+    res.back()->pct.ctx = ctx;
+    for (int a = 0; a < nagg; a++) res.back()->pct.rep[a] = plan.pct_rep[a];
+  }
+  bool any_pct = false;
+  for (int a = 0; a < nagg; a++) any_pct |= plan.pct_rep[a] >= 0;
   struct ResultCleanup {  // frees dense device state if we fail midway
     std::vector<std::unique_ptr<pb200_result>>* r;
     bool armed = true;
@@ -752,12 +764,14 @@ static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment*
     ~PinnedScratch() { pinned_free(c, p, bytes); }
   } pacc{ctx};
   {
-    int rc = pinned_alloc(ctx, 2 * (sizeof(AggAccum) + 32) * nres, &pacc.p, &pacc.bytes);
+    int rc = pinned_alloc(ctx, 2 * (sizeof(AggAccum) + 32 + (any_pct && !plan.group_by ? 8 * kMaxAggs : 0)) * nres, &pacc.p, &pacc.bytes);
     if (rc) return rc;
   }
   // block layout (device and both pinned halves): nres AggAccum records, then 4 words per result for the count-carrier
-  // verification {sum of carried counts, largest sum field, largest carried count, unused}
-  const size_t acc_bytes = (sizeof(AggAccum) + 32) * nres;
+  // verification {sum of carried counts, largest sum field, largest carried count, unused}, then (aggregation-only
+  // PERCENTILE) per result kMaxAggs selected dictIds and kMaxAggs value counts, u32 each -- read back with the accumulators
+  const size_t pct_bytes = any_pct && !plan.group_by ? 8ull * kMaxAggs * nres : 0;
+  const size_t acc_bytes = (sizeof(AggAccum) + 32) * nres + pct_bytes;
   unsigned char* const pin_init = static_cast<unsigned char*>(pacc.p);
   unsigned char* const pin_back = pin_init + acc_bytes;
   AggAccum* host_acc = reinterpret_cast<AggAccum*>(pin_back);
@@ -772,6 +786,8 @@ static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment*
     PB200_CUDA(cudaMemcpyAsync(accum_buf.p, pin_init, acc_bytes, cudaMemcpyHostToDevice, st));
   }
   unsigned long long* const dev_verify = reinterpret_cast<unsigned long long*>(static_cast<unsigned char*>(accum_buf.p) + sizeof(AggAccum) * nres);
+  uint32_t* const dev_pct = reinterpret_cast<uint32_t*>(static_cast<unsigned char*>(accum_buf.p) + (sizeof(AggAccum) + 32) * nres);
+  const uint32_t* const host_pct = reinterpret_cast<const uint32_t*>(pin_back + (sizeof(AggAccum) + 32) * nres);
   for (int s = 0; s < nseg; s++) plan.segs[s].accum = (AggAccum*)accum_buf.p + (merge ? 0 : s);
   std::vector<std::vector<std::unique_ptr<DevBufRaw>>> distinct_bufs(nres);  // aggregation only: DISTINCTCOUNT bitsets
   if (!plan.group_by) {
@@ -789,6 +805,19 @@ static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment*
     for (int s = 0; s < nseg; s++)
       for (int a = 0; a < nagg; a++)
         if (distinct_bufs[merge ? 0 : s][a]) plan.segs[s].distinct_bits[a] = (uint32_t*)distinct_bufs[merge ? 0 : s][a]->p;
+    // PERCENTILE: one dictId histogram per result and column, owned by the result from here on
+    for (int r = 0; r < nres; r++)
+      for (int a = 0; a < nagg; a++) {
+        const size_t entries = plan.hist_entries[r][a];
+        if (!entries) continue;
+        pb200_result::Pct& p = res[r]->pct;
+        if (int rc = dev_alloc(ctx, entries * 4, (void**)&p.hist[a])) return rc;
+        PB200_CUDA(cudaMemsetAsync(p.hist[a], 0, entries * 4, st));
+        p.entries[a] = (uint32_t)entries;
+      }
+    for (int s = 0; s < nseg; s++)
+      for (int a = 0; a < nagg; a++)
+        if (res[merge ? 0 : s]->pct.hist[a]) plan.segs[s].distinct_bits[a] = res[merge ? 0 : s]->pct.hist[a];
   } else {
     // group tables to the plan's layout; they belong to the results from here on
     for (int r = 0; r < nres; r++) {
@@ -838,6 +867,16 @@ static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment*
           if ((rc = dev_alloc(ctx, bytes, (void**)&d.dbits[a]))) return rc;
           PB200_CUDA(cudaMemsetAsync(d.dbits[a], 0, bytes, st));
           d.dwords[a] = t.dwords[a];
+        } else if (fn == PB200_AGG_PERCENTILE) {  // one dictId histogram per group / slot (owner), a dictId per entry (each)
+          pb200_result::Pct& p = res[r]->pct;
+          if (t.hist_per_group[a]) {
+            const size_t entries = (size_t)t.hist_per_group[a] * t.groups;
+            if ((rc = dev_alloc(ctx, entries * 4, (void**)&p.hist[a]))) return rc;
+            PB200_CUDA(cudaMemsetAsync(p.hist[a], 0, entries * 4, st));
+            p.entries[a] = t.hist_per_group[a];
+            if ((rc = dev_alloc(ctx, (size_t)t.groups * 4, (void**)&p.n[a]))) return rc;
+          }
+          if ((rc = dev_alloc(ctx, (size_t)t.groups * 4, (void**)&p.ids[a]))) return rc;
         }
       }
       if (d.pack_agg >= 0) d.exists_packed = (const unsigned long long*)d.isum[d.pack_agg];
@@ -850,6 +889,7 @@ static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment*
       sd.g_count = d.count;
       sd.g_seen = d.seen;
       for (int a = 0; a < nagg; a++) { sd.g_isum[a] = d.isum[a]; sd.g_dsum[a] = d.dsum[a]; sd.g_min[a] = d.gmin[a]; sd.g_max[a] = d.gmax[a]; sd.distinct_bits[a] = d.dbits[a]; }
+      for (int a = 0; a < nagg; a++) if (res[merge ? 0 : s]->pct.hist[a]) sd.distinct_bits[a] = res[merge ? 0 : s]->pct.hist[a];
       sd.h_keys = d.hkeys;
       sd.h_ctl = d.hctl;
     }
@@ -882,6 +922,31 @@ static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment*
   }
   if (le != cudaSuccess) { set_error("scan kernel launch failed: %s (smem %zu B, grid %d)", cudaGetErrorString(le), plan.smem_bytes, grid); return PB200_E_CUDA; }
   PB200_CUDA(cudaEventRecord(e1, st));
+
+  // ---- PERCENTILE finalize: histograms -> selected dictIds, queued behind the scan (aggregation only: into the block
+  //      that is read back with the accumulators; group-by: per table entry, read by the extraction) ----
+  std::vector<std::unique_ptr<DevBufRaw>> pct_temps;
+  for (int r = 0; r < nres && any_pct; r++)
+    for (int a = 0; a < nagg; a++) {
+      pb200_result::Pct& p = res[r]->pct;
+      if (!p.hist[a]) continue;
+      PercentileJob job;
+      job.hist = p.hist[a];
+      job.E = p.entries[a];
+      if (plan.group_by) {
+        job.rows = plan.tables[r].groups;
+        job.n_out = p.n[a];
+      } else {
+        job.rows = 1;
+        job.n_out = dev_pct + (size_t)r * 2 * kMaxAggs + kMaxAggs + a;
+      }
+      for (int b = 0; b < nagg; b++) {
+        if (plan.pct_rep[b] != a) continue;
+        job.p[job.np] = plan.pct_p[b];
+        job.ids[job.np++] = plan.group_by ? p.ids[b] : dev_pct + (size_t)r * 2 * kMaxAggs + b;
+      }
+      if (int prc = percentile_finalize(ctx, st, job, pct_temps)) return prc;
+    }
 
   // ---- verify the count carriers ----
   if (plan.group_by)
@@ -972,6 +1037,10 @@ static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment*
           const bool empty = acc.count == 0 || (vk != VAL_RAW_I32 && (mn ? acc.min_id[a] == 0xFFFFFFFFu : acc.max_id_plus1[a] == 0));
           if (empty) d = mn ? INFINITY : -INFINITY;
           else { id = (int32_t)x; d = c->dict_host.empty() && vk != VAL_RAW_I32 ? (double)id : value_of(x); }
+        } else if (fn == PB200_AGG_PERCENTILE) {
+          const uint32_t x = host_pct[(size_t)r * 2 * kMaxAggs + a];
+          if (x == ~0u) d = -INFINITY;   // no matched row
+          else { id = (int32_t)x; d = value_of(x); l = host_pct[(size_t)r * 2 * kMaxAggs + kMaxAggs + plan.pct_rep[a]]; }
         } else if (fn == PB200_AGG_DISTINCTCOUNT) {
           const size_t words = plan.distinct_words[r][a];
           std::vector<uint32_t> bits(words);
@@ -1004,6 +1073,8 @@ static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment*
         dev_free(ctx, d.hkeys); dev_free(ctx, d.hctl);
         d.hkeys = nullptr; d.hctl = nullptr;
         for (int a = 0; a < kMaxAggs; a++) { dev_free(ctx, d.dbits[a]); d.dbits[a] = nullptr; }
+        pb200_result::Pct& p = res[r]->pct;   // the histograms stay for pb200_result_histogram
+        for (int a = 0; a < kMaxAggs; a++) { dev_free(ctx, p.ids[a]); dev_free(ctx, p.n[a]); p.ids[a] = p.n[a] = nullptr; }
         d.i64_block = d.f64_block = d.u32max_block = d.u32min_block = nullptr;
         d.live = false;
       }
@@ -1036,6 +1107,11 @@ extern "C" int32_t pb200_result_device_buffers(pb200_result* R, int32_t kind, vo
   if (!R || !p || !n) { set_error("null argument"); return PB200_E_INVALID; }
   pb200_result::Dense& d = R->dense;
   if (d.hkeys) { set_error("hash group tables of different GPUs are not element-wise reducible"); return PB200_E_UNSUPPORTED; }
+  for (int a = 0; a < kMaxAggs; a++)
+    if (R->pct.hist[a]) {
+      set_error("PERCENTILE keeps dictId histograms on the device: a cross-GPU reduce of the tables would drop the other ranks' values");
+      return PB200_E_UNSUPPORTED;
+    }
   for (int a = 0; a < kMaxAggs; a++)
     if (d.dbits[a]) {  // per-group DISTINCTCOUNT bitsets are not one of the four reducible blocks: never reduce "around" them
       set_error("group-by DISTINCTCOUNT keeps per-group dictId bitsets on the device: a cross-GPU reduce of the tables would drop the other ranks' sets");
@@ -1146,6 +1222,7 @@ extern "C" int32_t pb200_result_free(pb200_result* R) {
   if (!R) return PB200_OK;
   pb200_result::Dense& d = R->dense;
   if (d.ctx) { dev_free(d.ctx, d.i64_block); dev_free(d.ctx, d.f64_block); dev_free(d.ctx, d.u32max_block); dev_free(d.ctx, d.u32min_block); dev_free(d.ctx, d.hkeys); dev_free(d.ctx, d.hctl); for (int a = 0; a < kMaxAggs; a++) dev_free(d.ctx, d.dbits[a]); }
+  if (R->pct.ctx) for (int a = 0; a < kMaxAggs; a++) { dev_free(R->pct.ctx, R->pct.hist[a]); dev_free(R->pct.ctx, R->pct.ids[a]); dev_free(R->pct.ctx, R->pct.n[a]); }
   delete R;
   return PB200_OK;
 }

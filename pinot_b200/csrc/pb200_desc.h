@@ -40,6 +40,15 @@ __host__ __device__ constexpr bool sum_in_double(int vk) { return vk == VAL_DICT
 // from a raw MIN / MAX entry.
 __host__ __device__ constexpr uint32_t max_offset(int vk) { return vk == VAL_RAW_I32 ? 0u : 1u; }
 
+// PERCENTILE(col, p) over n > 0 sorted values (PercentileAggregationFunction.extractFinalResult): p == 100 selects the
+// largest, otherwise index (int64)((double)n * p / 100.0) -- product, division, truncation, in that order -- clamped to
+// n - 1 (rounding near p = 100 can reach n, where the reference would throw).
+__host__ __device__ inline long long percentile_index(long long n, double p) {
+  if (p == 100.0) return n - 1;
+  const long long k = (long long)((double)n * p / 100.0);
+  return k < n - 1 ? k : n - 1;
+}
+
 struct SlotDesc {
   const uint32_t* data;  // device: packed words, padded to whole tiles
   int32_t bits;          // 1..32 (32 = raw big-endian 32-bit values)
@@ -93,7 +102,12 @@ struct SegDesc {
   SlotDesc slots[kMaxSlots];
   LeafDesc leaves[kMaxLeaves];
   const void* dict[kMaxAggs];          // native (little-endian) dictionary value array of the aggregation's column
-  uint32_t* distinct_bits[kMaxAggs];   // DISTINCTCOUNT: bitset over dictIds (group-by: one of distinct_words[a] words per group / slot)
+  // per-group dictId tables, indexed by the aggregation (group-by: distinct_words[a] entries per group / slot):
+  //   DISTINCTCOUNT: bitset over dictIds, distinct_words[a] = words per group;
+  //   PERCENTILE:    u32 histogram of dictId counts, distinct_words[a] = entries per group (the column's cardinality);
+  //                  aggregation only: 1 when the warps count into private shared-memory histograms first (at most
+  //                  64 dictIds, in the aggregation's accumulator slots), else 0
+  uint32_t* distinct_bits[kMaxAggs];
   uint32_t distinct_words[kMaxAggs];
   AggAccum* accum;                     // aggregation-only output
   // dense group table (group-by): indexed by raw key = sum_j dictId_j * mult_j

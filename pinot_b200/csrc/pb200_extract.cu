@@ -64,6 +64,7 @@ struct ExtractDesc {
   unsigned long long idx_cap;        // untrimmed row bound: min(entries, numGroupsLimit + 1)
   const uint32_t* dbits[kMaxAggs];   // DISTINCTCOUNT per-group bitsets (an ORDER BY key is the popcount of a row)
   uint32_t dwords[kMaxAggs];
+  const uint32_t* pct_n[kMaxAggs];   // PERCENTILE: values per table entry (src[a] holds the selected dictIds)
 };
 
 __device__ __forceinline__ bool non_empty(const ExtractDesc& d, long long i) {
@@ -125,6 +126,17 @@ __device__ __forceinline__ unsigned long long group_count(const ExtractDesc& d, 
 
 // aggregation a of entry g as the result's columns hold it: double value, long (count), MIN / MAX dictId.  DISTINCTCOUNT
 // leaves zeros (the set sizes are filled in on the host from the gathered bitsets)
+// value of dictId x of aggregation a's column
+__device__ __forceinline__ double dict_value(const ExtractDesc& d, int a, uint32_t x) {
+  const int vk = d.vk[a];
+  if (vk == VAL_RAW_I32) return (double)(int32_t)(x ^ 0x80000000u);
+  if (!d.dict[a]) return (double)x;
+  if (vk == VAL_DICT_I32) return (double)(int32_t)(static_cast<const uint32_t*>(d.dict[a])[x] ^ 0x80000000u);  // device copy is biased
+  if (vk == VAL_DICT_I64) return (double)static_cast<const long long*>(d.dict[a])[x];
+  if (vk == VAL_DICT_F32) return (double)static_cast<const float*>(d.dict[a])[x];
+  return static_cast<const double*>(d.dict[a])[x];
+}
+
 __device__ __forceinline__ void agg_values(const ExtractDesc& d, int a, long long g, unsigned long long cnt, double& dv,
                                            long long& lv, int32_t& id) {
   const int fn = d.fn[a], vk = d.vk[a];
@@ -147,13 +159,13 @@ __device__ __forceinline__ void agg_values(const ExtractDesc& d, int a, long lon
     else {
       const uint32_t x = fn == PB200_AGG_MIN ? t : t - max_offset(vk);
       id = (int32_t)x;
-      if (vk == VAL_RAW_I32) dv = (double)(int32_t)(x ^ 0x80000000u);
-      else if (!d.dict[a]) dv = (double)x;
-      else if (vk == VAL_DICT_I32) dv = (double)(int32_t)(static_cast<const uint32_t*>(d.dict[a])[x] ^ 0x80000000u);  // device copy is biased
-      else if (vk == VAL_DICT_I64) dv = (double)static_cast<const long long*>(d.dict[a])[x];
-      else if (vk == VAL_DICT_F32) dv = (double)static_cast<const float*>(d.dict[a])[x];
-      else dv = static_cast<const double*>(d.dict[a])[x];
+      dv = dict_value(d, a, x);
     }
+  } else if (fn == PB200_AGG_PERCENTILE) {  // finalized from the histogram (pb200_percentile.cu): dictId, ~0 = no row
+    const uint32_t x = static_cast<const uint32_t*>(d.src[a])[g];
+    lv = d.pct_n[a][g];
+    if (x == ~0u) dv = -INFINITY;
+    else { id = (int32_t)x; dv = dict_value(d, a, x); }
   }
 }
 
@@ -289,13 +301,14 @@ static size_t layout_result(const pb200_result::Dense& d, ExtractDesc& e, size_t
   e.cap_rows = rows;
   e.off_keys = take(4, rows * (size_t)std::max(e.ngb, 1));
   bool need_idx = false;
-  for (int a = 0; a < e.nagg; a++) need_idx |= d.dbits[a] != nullptr;
+  for (int a = 0; a < e.nagg; a++) need_idx |= d.dbits[a] != nullptr || e.fn[a] == PB200_AGG_PERCENTILE;
   e.off_idx = need_idx ? take(4, rows) : kNoCol;
   for (int a = 0; a < e.nagg; a++) {
     const int fn = e.fn[a];
     e.off_dbl[a] = take(8, rows);
-    e.off_lng[a] = (fn == PB200_AGG_COUNT || fn == PB200_AGG_AVG || fn == PB200_AGG_SUM || fn == PB200_AGG_DISTINCTCOUNT) ? take(8, rows) : kNoCol;
-    e.off_ids[a] = (fn == PB200_AGG_MIN || fn == PB200_AGG_MAX) ? take(4, rows) : kNoCol;
+    e.off_lng[a] = (fn == PB200_AGG_COUNT || fn == PB200_AGG_AVG || fn == PB200_AGG_SUM || fn == PB200_AGG_DISTINCTCOUNT ||
+                    fn == PB200_AGG_PERCENTILE) ? take(8, rows) : kNoCol;
+    e.off_ids[a] = (fn == PB200_AGG_MIN || fn == PB200_AGG_MAX || fn == PB200_AGG_PERCENTILE) ? take(4, rows) : kNoCol;
   }
   return off;
 }
@@ -364,6 +377,7 @@ int extract_groups(pb200_ctx* ctx, pb200_result* const* Rs, int nres, cudaStream
       if (fn == PB200_AGG_SUM || fn == PB200_AGG_AVG) e.src[a] = sum_in_double(vk) ? (const void*)d.dsum[a] : (const void*)d.isum[a];
       else if (fn == PB200_AGG_MIN) e.src[a] = d.gmin[a];
       else if (fn == PB200_AGG_MAX) e.src[a] = d.gmax[a];
+      else if (fn == PB200_AGG_PERCENTILE) { e.src[a] = Rs[r]->pct.ids[a]; e.pct_n[a] = Rs[r]->pct.n[Rs[r]->pct.rep[a]]; }
       const DeviceColumn* c = d.agg_cols[a];
       e.dict[a] = (c && vk != VAL_RAW_I32 && !c->dict_host.empty()) ? c->dict_native : nullptr;
     }
@@ -491,6 +505,7 @@ int extract_groups(pb200_ctx* ctx, pb200_result* const* Rs, int nres, cudaStream
     v.block = pin;
     v.rows = kept_rows(R, n[r]);
     v.keys = reinterpret_cast<const int32_t*>(out + e.off_keys);
+    R->pct.row_entry = e.off_idx == kNoCol ? nullptr : reinterpret_cast<const uint32_t*>(out + e.off_idx);
     for (int a = 0; a < nagg; a++) {
       v.dbl[a] = e.off_dbl[a] == kNoCol ? nullptr : reinterpret_cast<const double*>(out + e.off_dbl[a]);
       v.lng[a] = e.off_lng[a] == kNoCol ? nullptr : reinterpret_cast<const int64_t*>(out + e.off_lng[a]);

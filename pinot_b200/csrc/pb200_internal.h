@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cstdint>
 #include <map>
 #include <memory>
@@ -155,6 +156,18 @@ struct pb200_result {
     int32_t* segment_index = nullptr;
     std::vector<const void*> columns;            // int64 or double [rows] each
   } selection;
+  // PERCENTILE (pb200_percentile.cu): the histograms stay on the device until pb200_result_histogram copies them
+  struct Pct {
+    Pct() { std::fill(rep, rep + pb200::kMaxAggs, -1); }
+    pb200_ctx* ctx = nullptr;
+    int rep[pb200::kMaxAggs];                    // aggregation -> owner of its histogram (-1: not a PERCENTILE)
+    uint32_t* hist[pb200::kMaxAggs] = {};        // owners: device histogram, one row per result row / table entry
+    uint32_t entries[pb200::kMaxAggs] = {};      // owners: entries per row
+    uint32_t* ids[pb200::kMaxAggs] = {};         // group-by: selected dictId per table entry (device, ~0: no row)
+    uint32_t* n[pb200::kMaxAggs] = {};           // group-by, owners: values per table entry (device)
+    const uint32_t* row_entry = nullptr;         // group-by: table entry of each extracted row (inside view.block)
+    std::vector<uint32_t> host[pb200::kMaxAggs]; // owners: histogram rows of the result's rows, copied on first use
+  } pct;
   pb200_order_by order{};                        // ORDER BY spec of a group-by result (num_items 0: none), applied at extraction
   std::vector<int32_t> agg_functions;            // PB200_AGG_* per aggregation (set by pb200_execute)
   std::vector<int32_t> keys;                     // [G x k]

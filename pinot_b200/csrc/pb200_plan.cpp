@@ -73,7 +73,7 @@ bool same_dictionary(pb200_segment* const* segments, int nseg, int col, const ch
 }
 
 int plan_scan(const Tuning& tune, DeviceLimits lim, const pb200_query* query, pb200_segment* const* segments, int nseg,
-              bool allow_count_carrier, ScanPlan* out) {
+              bool allow_count_carrier, ScanPlan* out, const double* agg_args) {
   if (!query || !segments || !out || nseg <= 0) { set_error("invalid argument to pb200_execute"); return PB200_E_INVALID; }
   const bool per_seg_filter = query->flags & PB200_Q_PER_SEGMENT_FILTER;
   const bool merge = query->flags & PB200_Q_MERGE_SEGMENTS;
@@ -96,10 +96,12 @@ int plan_scan(const Tuning& tune, DeviceLimits lim, const pb200_query* query, pb
     }
     for (int a = 0; a < nagg; a++) {
       const pb200_agg& ag = query->aggs[a];
-      if (ag.function != PB200_AGG_MIN && ag.function != PB200_AGG_MAX && ag.function != PB200_AGG_DISTINCTCOUNT) continue;
+      if (ag.function != PB200_AGG_MIN && ag.function != PB200_AGG_MAX && ag.function != PB200_AGG_DISTINCTCOUNT &&
+          ag.function != PB200_AGG_PERCENTILE) continue;
       if (ag.column < 0 || ag.column >= ncols) continue;
       if (segments[0]->cols[ag.column].bits == 32 && !segments[0]->cols[ag.column].dict_native) continue;  // raw values, no ids
-      if (!same_dictionary(segments, nseg, ag.column, ag.function == PB200_AGG_DISTINCTCOUNT ? "DISTINCTCOUNT" : "MIN/MAX")) return PB200_E_UNSUPPORTED;
+      const char* what = ag.function == PB200_AGG_DISTINCTCOUNT ? "DISTINCTCOUNT" : ag.function == PB200_AGG_PERCENTILE ? "PERCENTILE" : "MIN/MAX";
+      if (!same_dictionary(segments, nseg, ag.column, what)) return PB200_E_UNSUPPORTED;
     }
   }
 
@@ -114,6 +116,8 @@ int plan_scan(const Tuning& tune, DeviceLimits lim, const pb200_query* query, pb
   q.num_segments = nseg;
   q.num_aggs = nagg;
   q.num_group_by = ngb;
+  plan.pct_p.assign(nagg, std::numeric_limits<double>::quiet_NaN());
+  plan.pct_rep.assign(nagg, -1);
 
   // ---- slots: filter scan columns, then group-by keys, then aggregation arguments ----
   const pb200_filter_node* f0 = query->filter;
@@ -149,8 +153,30 @@ int plan_scan(const Tuning& tune, DeviceLimits lim, const pb200_query* query, pb
     q.aggs[a].slot = -1;
     q.aggs[a].val_kind = VAL_NONE;
     if (ag.function == PB200_AGG_COUNT) continue;
-    if (ag.function < 0 || ag.function > PB200_AGG_DISTINCTCOUNT) { set_error("unknown aggregation function %d", ag.function); return PB200_E_INVALID; }
+    if (ag.function < 0 || ag.function > PB200_AGG_PERCENTILE) { set_error("unknown aggregation function %d", ag.function); return PB200_E_INVALID; }
     if (ag.column < 0 || ag.column >= ncols) { set_error("aggregation column %d out of range", ag.column); return PB200_E_INVALID; }
+    if (ag.function == PB200_AGG_PERCENTILE) {
+      // the percentile travels beside the query (pb200_execute_args); PercentileAggregationFunction takes 0 <= p <= 100
+      if (!agg_args) {   // pb200_execute / pb200_execute_ordered carry no percentile
+        set_error("unknown aggregation function %d without arguments: PERCENTILE (aggregation %d) takes its percentile through pb200_execute_args", ag.function, a);
+        return PB200_E_INVALID;
+      }
+      const double pv = agg_args[a];
+      if (!(pv >= 0.0 && pv <= 100.0)) { set_error("PERCENTILE (aggregation %d): percentile %g outside [0, 100]", a, pv); return PB200_E_INVALID; }
+      if (plan.defer_finalize) { set_error("PERCENTILE histograms are not reducible across GPUs (PB200_Q_DEFER_FINALIZE)"); return PB200_E_UNSUPPORTED; }
+      for (int t = 0; t < nseg; t++) {
+        const DeviceColumn& pc = segments[t]->cols[ag.column];
+        if (pc.stored_type == PB200_STRING) { set_error("PERCENTILE over STRING column %d", ag.column); return PB200_E_UNSUPPORTED; }
+        if (pc.bits > 31 || !pc.dict_native || pc.cardinality <= 0) {
+          set_error("PERCENTILE over column %d: no dictIds in segment %d (raw values): not accelerated", ag.column, t);
+          return PB200_E_UNSUPPORTED;
+        }
+      }
+      plan.pct_p[a] = pv;
+      plan.pct_rep[a] = a;
+      for (int b = 0; b < a; b++)   // PERCENTILEs of one column share the first one's histogram
+        if (query->aggs[b].function == PB200_AGG_PERCENTILE && query->aggs[b].column == ag.column) { plan.pct_rep[a] = b; break; }
+    }
     int s = slot_of(plan, ag.column, ROLE_AGG);
     if (s < 0) { set_error("too many distinct columns (max %d)", kMaxSlots); return PB200_E_UNSUPPORTED; }
     q.aggs[a].slot = s;
@@ -541,6 +567,7 @@ int plan_scan(const Tuning& tune, DeviceLimits lim, const pb200_query* query, pb
     for (int pass = 0; pass < 2; pass++)
       for (int a = 0; a < nagg; a++) {
         if (q.aggs[a].slot < 0 || pipelined[a] != (pass == 1)) continue;
+        if (plan.pct_rep[a] >= 0 && plan.pct_rep[a] != a) continue;   // reads another PERCENTILE's histogram
         const SlotDesc& sl = sd.slots[q.aggs[a].slot];
         sd.agg_code[n++] = agg_code(a, q.aggs[a].function, q.aggs[a].val_kind, sl.bits, sl.stage_words);
       }
@@ -562,7 +589,31 @@ int plan_scan(const Tuning& tune, DeviceLimits lim, const pb200_query* query, pb
     }
   }
 
+  bool any_pct = false;
+  for (int a = 0; a < nagg; a++) any_pct |= plan.pct_rep[a] >= 0;
+  if (any_pct) {
+    // histogram bins are u32: a result over 2^32 docs could wrap one
+    for (int r = 0; r < nres; r++) {
+      unsigned long long docs = 0;
+      for (int s = 0; s < nseg; s++) if (merge || s == r) docs += (unsigned long long)segments[s]->num_docs;
+      if (docs >= (1ull << 32)) { set_error("PERCENTILE over %llu docs in one result: histogram bins are 32-bit", docs); return PB200_E_UNSUPPORTED; }
+    }
+  }
   if (!plan.group_by) {
+    // PERCENTILE: one histogram of 2^bits u32 entries per result and column (every representable dictId is addressable)
+    plan.hist_entries.assign(nres, std::vector<size_t>(nagg, 0));
+    for (int r = 0; r < nres; r++)
+      for (int a = 0; a < nagg; a++) {
+        if (plan.pct_rep[a] != a) continue;
+        int maxbits = 0;
+        for (int s = 0; s < nseg; s++) if (merge || s == r) maxbits = std::max(maxbits, segments[s]->cols[query->aggs[a].column].bits);
+        plan.hist_entries[r][a] = (size_t)1 << maxbits;
+        plan.hist_total += 1ll << maxbits;
+      }
+    // few dictIds: warp-private shared-memory histograms (SegDesc.distinct_words as the flag)
+    for (int s = 0; s < nseg; s++)
+      for (int a = 0; a < nagg; a++)
+        if (plan.pct_rep[a] == a) plan.segs[s].distinct_words[a] = segments[s]->cols[query->aggs[a].column].cardinality <= kHistWarpPrivateMaxCard ? 1u : 0u;
     // DISTINCTCOUNT: one dictId bitset per result; a merged result's bitset must hold the dictIds of every segment
     plan.distinct_words.assign(nres, std::vector<size_t>(nagg, 0));
     for (int r = 0; r < nres; r++)
@@ -608,7 +659,7 @@ int plan_scan(const Tuning& tune, DeviceLimits lim, const pb200_query* query, pb
         // With one entry per 128 bytes the same reductions spread over >= 4096 chunks.  Costs table bytes (<= 2 MB each,
         // memset + extraction scan), no instruction in the kernel: the stride is folded into the key multipliers.
         bool any_bitset = false;
-        for (int a = 0; a < nagg; a++) any_bitset |= q.aggs[a].function == PB200_AGG_DISTINCTCOUNT;
+        for (int a = 0; a < nagg; a++) any_bitset |= q.aggs[a].function == PB200_AGG_DISTINCTCOUNT || q.aggs[a].function == PB200_AGG_PERCENTILE;
         if (q.smem_groups == 0 && !any_bitset && tune.table_stride != 1) {
           long long s = 1;
           if (tune.table_stride > 1) s = tune.table_stride;
@@ -655,6 +706,11 @@ int plan_scan(const Tuning& tune, DeviceLimits lim, const pb200_query* query, pb
             return PB200_E_UNSUPPORTED;
           }
           t.dwords[a] = (uint32_t)words;
+        } else if (fn == PB200_AGG_PERCENTILE && plan.pct_rep[a] == a) {  // one dictId histogram per group / slot
+          const int card = seg->cols[query->aggs[a].column].cardinality;
+          t.hist_per_group[a] = (uint32_t)card;
+          plan.hist_total += (long long)card * t.groups;
+          if ((unsigned long long)card * (unsigned long long)t.groups > (unsigned long long)kMaxHistogramEntries) break;  // refused below
         }
       }
       t.i64_elems = ii * t.groups; t.f64_elems = fi * t.groups; t.u32max_elems = xi * t.groups; t.u32min_elems = ni * t.groups;
@@ -674,12 +730,17 @@ int plan_scan(const Tuning& tune, DeviceLimits lim, const pb200_query* query, pb
       for (int a = 0; a < nagg; a++) {
         sd.sum_addend[a] = 0ull - (1ull << 31);  // plain INT-dictionary sum: remove the device copy's bias
         if (a == t.carrier.agg) sd.sum_addend[a] = (1ull << t.carrier.shift) - (unsigned long long)((uint32_t)(int32_t)t.carrier.vmin ^ 0x80000000u);
-        sd.distinct_words[a] = t.dwords[a];
+        sd.distinct_words[a] = plan.pct_rep[a] >= 0 ? t.hist_per_group[a] : t.dwords[a];
       }
       for (int g = 0; g < ngb; g++) { sd.group_mult[g] = t.mult[g] * (uint32_t)t.stride; sd.group_mult64[g] = t.mult64[g]; }  // hash tables: stride 1
       sd.h_mask = t.hashed ? (uint32_t)(t.groups - 1) : 0u;
       sd.h_limit = query->num_groups_limit;
     }
+  }
+
+  if (plan.hist_total > kMaxHistogramEntries) {
+    set_error("PERCENTILE histograms of %lld entries in one call (at most %lld)", plan.hist_total, kMaxHistogramEntries);
+    return PB200_E_UNSUPPORTED;
   }
 
   // ---- launch chunks of <= kMaxLaunchSegs segments (their TMA table travels in the kernel parameters) ----

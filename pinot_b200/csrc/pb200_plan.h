@@ -54,6 +54,7 @@ struct TableLayout {
   long long i64_elems = 0, f64_elems = 0, u32max_elems = 0, u32min_elems = 0;
   int index[kMaxAggs] = {};
   uint32_t dwords[kMaxAggs] = {};   // DISTINCTCOUNT: bitset words per group
+  uint32_t hist_per_group[kMaxAggs] = {};  // PERCENTILE (the histogram's owner, ScanPlan::pct_rep): entries per group
 };
 
 // One kernel launch: segments [first_seg, first_seg + num_segs), their tiles numbered from 0
@@ -74,13 +75,25 @@ struct ScanPlan {
   std::vector<LeafBuffer> leaf_buffers;
   std::vector<TableLayout> tables;                    // group-by: one per result
   std::vector<std::vector<size_t>> distinct_words;    // aggregation only: [result][agg] DISTINCTCOUNT bitset words (0: none)
+  // PERCENTILE: percentile of aggregation a (NaN: not a PERCENTILE) and the aggregation whose histogram it reads -- the
+  // first PERCENTILE of its column, the only one with an agg code (-1: not a PERCENTILE)
+  std::vector<double> pct_p;
+  std::vector<int> pct_rep;
+  std::vector<std::vector<size_t>> hist_entries;      // aggregation only: [result][agg] histogram entries of an owner (0: none)
+  long long hist_total = 0;                           // histogram entries of all results of the call
   std::vector<long long> in_filter;                   // per result: num_entries_scanned_in_filter
   int projected = 0;                                  // num_entries_scanned_post_filter = matched docs x this
 };
 
-// PB200_OK, or the PB200_E_* code of pb200_execute for this input (message set with set_error).
+// PB200_OK, or the PB200_E_* code of pb200_execute_args for this input (message set with set_error).  agg_args: one per
+// aggregation, the percentile of a PERCENTILE (NULL: PERCENTILE is refused, as pb200_execute does).
+constexpr long long kMaxHistogramEntries = 1ll << 28;  // PERCENTILE histogram entries of one call (u32 each)
+// Aggregation-only PERCENTILE over at most this many dictIds: each warp counts into a private histogram in its own
+// accumulator slots in shared memory (32 threads x 8 bytes = 64 u32 bins), flushed once per segment, instead of one
+// same-address L2 reduction per row (DESIGN.md section 3.7 has the measurements)
+constexpr int kHistWarpPrivateMaxCard = 64;
 int plan_scan(const Tuning& tune, DeviceLimits lim, const pb200_query* query, pb200_segment* const* segments, int nseg,
-              bool allow_count_carrier, ScanPlan* out);
+              bool allow_count_carrier, ScanPlan* out, const double* agg_args = nullptr);
 
 // ---- selection (pb200_execute_selection): plan_scan with COUNT(*) as the only aggregation, plus the match mask ----
 constexpr long long kSelectPrefixRows = 1ll << 20;  // first pass of a selection without ORDER BY: at least this many docs

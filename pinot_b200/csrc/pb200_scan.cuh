@@ -162,6 +162,9 @@ __device__ __forceinline__ void red_add_u64(unsigned long long* p, unsigned long
 __device__ __forceinline__ void red_add_f64(double* p, double v) {
   asm volatile("red.global.add.f64 [%0], %1;" ::"l"(p), "d"(v) : "memory");
 }
+__device__ __forceinline__ void red_add_u32(uint32_t* p, uint32_t v) {
+  asm volatile("red.global.add.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
 
 // Hash group table: slot of `key` in the open-addressing table (linear probing, 64-bit CAS on the key itself -- exact,
 // no fingerprints).  Returns false once the table holds more than h_limit groups (the caller's result is then discarded:
@@ -505,6 +508,12 @@ scan_kernel(const __grid_constant__ QueryDesc q, const __grid_constant__ TmaTabl
           const uint2 mm = accmm[a * kConsumers + group];
           if (fn == 2) { uint32_t v = warp_min(mm.x); if (lane == 0) atomicMin(&sd.accum->min_id[a], v); }
           else { uint32_t v = warp_max(mm.y); if (lane == 0) atomicMax(&sd.accum->max_id_plus1[a], v); }
+        } else if (fn == 6 && sd.distinct_words[a]) {
+          // the warp-private PERCENTILE histogram: this thread's slot holds bins 2 * lane and 2 * lane + 1
+          __syncwarp();
+          const unsigned long long bins = acc64[a * kConsumers + group];
+          if ((uint32_t)bins) red_add_u32(sd.distinct_bits[a] + 2 * lane, (uint32_t)bins);
+          if ((uint32_t)(bins >> 32)) red_add_u32(sd.distinct_bits[a] + 2 * lane + 1, (uint32_t)(bins >> 32));
         }
       }
       reset_acc();
@@ -716,6 +725,9 @@ scan_kernel(const __grid_constant__ QueryDesc q, const __grid_constant__ TmaTabl
           accmm[a * kConsumers + group] = mmx;
         } else if (fn == 5) {
           atomicOr(sd.distinct_bits[a] + (id >> 5), 1u << (id & 31));
+        } else if (fn == 6) {  // PERCENTILE: the result's dictId histogram (the sorted value list of the reference)
+          if (!GROUPBY && sd.distinct_words[a]) atomicAdd(reinterpret_cast<uint32_t*>(acc64 + a * kConsumers + warp * 32) + id, 1u);
+          else red_add_u32(sd.distinct_bits[a] + id, 1u);
         }
       }
     };
@@ -865,6 +877,11 @@ scan_kernel(const __grid_constant__ QueryDesc q, const __grid_constant__ TmaTabl
               const size_t wpg = sd.distinct_words[a];
 #pragma unroll
               for (int u = 0; u < kQB; ++u) if (ok[u]) atomicOr(bits + (size_t)g[u] * wpg + (id[u] >> 5), 1u << (id[u] & 31u));
+            } else if (fn == 6) {  // PERCENTILE: the group's dictId histogram (DoubleArrayList of values per group in the reference)
+              uint32_t* hist = sd.distinct_bits[a];
+              const size_t epg = sd.distinct_words[a];
+#pragma unroll
+              for (int u = 0; u < kQB; ++u) if (ok[u]) red_add_u32(hist + (size_t)g[u] * epg + id[u], 1u);
             } else if (fn == 2 || fn == 3) {
               // MIN / MAX tables change for only O(log n) of a group's rows: read the current entries first, then issue
               // a reduction only where the row can win (a stale read costs a redundant reduction, never a wrong result)
@@ -967,6 +984,21 @@ scan_kernel(const __grid_constant__ QueryDesc q, const __grid_constant__ TmaTabl
 #pragma unroll
               for (int j = 0; j < 32; ++j)
                 if ((m >> j) & 1u) atomicOr(bits + (v[j] >> 5), 1u << (v[j] & 31));
+            } else if (fn == 6) {  // PERCENTILE: dictId histogram
+              if (sd.distinct_words[a]) {
+                // at most 64 dictIds (plan_scan): same-address reductions would serialise in L2, so the warp counts into
+                // a private 64-bin histogram in its own accumulator slots (shared-memory atomics), added to the
+                // result's histogram once per segment (flush)
+                uint32_t* wh = reinterpret_cast<uint32_t*>(acc64 + a * kConsumers + warp * 32);
+#pragma unroll
+                for (int j = 0; j < 32; ++j)
+                  if ((m >> j) & 1u) atomicAdd(wh + v[j], 1u);
+              } else {   // one reduction per surviving row
+                uint32_t* hist = sd.distinct_bits[a];
+#pragma unroll
+                for (int j = 0; j < 32; ++j)
+                  if ((m >> j) & 1u) red_add_u32(hist + v[j], 1u);
+              }
             }
           }
         }

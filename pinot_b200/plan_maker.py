@@ -311,6 +311,9 @@ class ResultsBlock:
     count_carrier: bool = False  # the per-group row counts rode in an INT sum's reductions (pb200_plan.cpp)
     carrier_unsafe: bool = False  # deferred result: that sum may overflow in the cross-GPU reduce, rerun without carrier
     flag_slot: bool = False  # the int64 table block ends with this rank's unsafe verdict: all-reduce it with the tables
+    # PERCENTILE of per-segment results: (agg, row) -> (dictIds ascending, counts) of the row's non-zero histogram bins,
+    # the intermediate a by-value merge adds up (cli.merge_blocks)
+    histograms: Dict[Tuple[int, int], Tuple[np.ndarray, np.ndarray]] = field(default_factory=dict)
 
     def release(self, ctx: "B200Context") -> None:
         """Frees the native result of a block executed with keep_handle=True (or views=True: the arrays die with it)."""
@@ -324,7 +327,7 @@ class ResultsBlock:
             self.handle = None
 
     def get_results(self, query: QueryContext) -> List[object]:
-        """AggregationResultsBlock.getResults(): Long for COUNT, Double for SUM/MIN/MAX, (sum, count) for AVG,
+        """AggregationResultsBlock.getResults(): Long for COUNT, Double for SUM/MIN/MAX/PERCENTILE, (sum, count) for AVG,
         set size for DISTINCTCOUNT -- row 0 (aggregation only)."""
         out = []
         for a, agg in enumerate(query.aggregations):
@@ -484,14 +487,15 @@ def _read_views(ctx: B200Context, handle, q: QueryContext, meta):
     return keys, doubles, longs, ids
 
 
-def _read_result(ctx: B200Context, handle, q: QueryContext, kind: int, keep_handle: bool, views: bool = False) -> ResultsBlock:
+def _read_result(ctx: B200Context, handle, q: QueryContext, kind: int, keep_handle: bool, views: bool = False,
+                 histograms: bool = False) -> ResultsBlock:
     L = ctx.lib
     meta = _lib.ResultMeta()
     _lib.check(L.pb200_result_meta_get(handle, C.byref(meta)))
     g = meta.num_groups
     rows = 1 if g < 0 else g
     k = len(q.group_by)
-    if views and not any(a.function == "DISTINCTCOUNT" for a in q.aggregations):
+    if views and not any(a.function in ("DISTINCTCOUNT", "PERCENTILE") for a in q.aggregations):
         keys, doubles, longs, ids = _read_views(ctx, handle, q, meta)
         stats = ExecutionStatistics(meta.num_docs_scanned, meta.num_entries_scanned_in_filter,
                                     meta.num_entries_scanned_post_filter, meta.num_total_docs)
@@ -520,10 +524,21 @@ def _read_result(ctx: B200Context, handle, q: QueryContext, kind: int, keep_hand
                 if n < 0:
                     _lib.check(int(n))
                 distinct[(a, row)] = buf
+    hists = {}
+    for a, agg in enumerate(q.aggregations):
+        if agg.function == "PERCENTILE" and histograms:
+            for row in range(rows):
+                n = L.pb200_result_histogram(handle, a, row, None, None, 0)
+                if n < 0:
+                    _lib.check(int(n))
+                hid, hcnt = np.zeros(int(n), dtype=np.int32), np.zeros(int(n), dtype=np.int64)
+                _lib.check(min(0, int(L.pb200_result_histogram(handle, a, row, _ptr(hid), _ptr(hcnt), int(n)))))
+                hists[(a, row)] = (hid, hcnt)
     stats = ExecutionStatistics(meta.num_docs_scanned, meta.num_entries_scanned_in_filter,
                                 meta.num_entries_scanned_post_filter, meta.num_total_docs)
     block = ResultsBlock(g, _lib.REGIMES[meta.regime], bool(meta.groups_limit_reached), stats, keys, doubles, longs,
                          ids, distinct, meta.device_ms, _lib.OPERATOR_KINDS.get(kind, "AGGREGATION"))
+    block.histograms = hists
     block.count_carrier = bool(meta.reserved & 1)
     block.carrier_unsafe = bool(meta.reserved & 2)
     block.flag_slot = bool(meta.reserved & 4)
@@ -625,14 +640,20 @@ class B200PlanMaker:
         res = (C.c_void_p * nres)()
         kinds = (C.c_int32 * n)()
         spec = order_spec(query, merge) if ordered else None
-        if spec is None:
+        pct = [a.function == "PERCENTILE" for a in query.aggregations]
+        if any(pct):
+            # one argument per aggregation: the percentile of each PERCENTILE (pb200h_execute_args)
+            args = (C.c_double * len(pct))(*[float(a.arg) if is_p else 0.0 for a, is_p in zip(query.aggregations, pct)])
+            _lib.check(self.ctx.lib.pb200h_execute_args(self.ctx.handle, C.byref(hq), C.byref(spec) if spec is not None else None,
+                                                        args, segs, n, res, kinds))
+        elif spec is None:
             _lib.check(self.ctx.lib.pb200h_execute(self.ctx.handle, C.byref(hq), segs, n, res, kinds))
         else:
             _lib.check(self.ctx.lib.pb200h_execute_ordered(self.ctx.handle, C.byref(hq), C.byref(spec), segs, n, res, kinds))
         # views=True: the blocks' arrays alias the native results' pinned memory (no copy); keep the block alive while you
         # use them and drop it before the context closes
-        blocks = [_read_result(self.ctx, C.c_void_p(res[i]), query, kinds[i if not merge else 0], keep_handle, views)
-                  for i in range(nres)]
+        blocks = [_read_result(self.ctx, C.c_void_p(res[i]), query, kinds[i if not merge else 0], keep_handle, views,
+                               histograms=not merge) for i in range(nres)]
         self.last_device_ms = blocks[0].device_ms
         return blocks
 

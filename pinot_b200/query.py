@@ -45,14 +45,40 @@ FilterNode = Union[Filter, Predicate]
 
 @dataclass
 class Aggregation:
-    function: str  # COUNT | SUM | MIN | MAX | AVG | DISTINCTCOUNT
+    function: str  # COUNT | SUM | MIN | MAX | AVG | DISTINCTCOUNT | PERCENTILE
     column: Optional[str] = None  # None for COUNT(*)
     # FILTER (WHERE ...) clause of this function (QueryContext.getFilteredAggregationFunctions: Pair<function, FilterContext>);
     # evaluated together with the query's own filter (AggregationFunctionUtils.buildFilteredAggregationInfos)
     filter: Optional["FilterNode"] = None
+    arg: Optional[float] = None  # PERCENTILE: the percentile, 0 <= p <= 100
 
     def __str__(self):
+        if self.function == "PERCENTILE":
+            return f"percentile({self.column}, {self.arg:g})"
         return f"{self.function.lower()}({self.column or '*'})"
+
+
+def percentile_index(n: int, p: float) -> int:
+    """PercentileAggregationFunction.extractFinalResult's index among n > 0 sorted values: the largest at p == 100,
+    otherwise int((double)n * p / 100.0) -- product, division, truncation -- clamped to n - 1."""
+    if p == 100.0:
+        return n - 1
+    return min(int(float(n) * float(p) / 100.0), n - 1)
+
+
+def percentile_of_counts(counts) -> float:
+    """PERCENTILE over a {value: count} multiset (the by-value merge of per-segment histograms); -inf when empty.
+    `counts` is (p, {value: count})."""
+    p, hist = counts
+    n = sum(hist.values())
+    if n == 0:
+        return float("-inf")
+    k = percentile_index(n, p)
+    for v in sorted(hist):
+        k -= hist[v]
+        if k < 0:
+            return float(v)
+    raise AssertionError("unreachable")
 
 
 @dataclass

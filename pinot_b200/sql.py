@@ -7,7 +7,8 @@ stays Java).  This module exists so the parity tests read like the reference's
 ``pinot-core/src/test/java/org/apache/pinot/queries/BaseQueriesTest.java:97-102``).  Grammar:
 
     SELECT item[, item...] FROM table [WHERE cond] [GROUP BY col[, col...]] [ORDER BY expr [ASC|DESC], ...] [LIMIT n]
-    item  := COUNT(*) | FN(col) | col            (plain columns are allowed only when they are group-by keys)
+    item  := COUNT(*) | FN(col) | PERCENTILE(col, p) | PERCENTILE<n>(col) | col
+             (plain columns are allowed only when they are group-by keys; 0 <= p <= 100, fractions allowed)
     selection (parse_selection): SELECT * | col[, col...] FROM table [WHERE cond] [ORDER BY col [ASC|DESC], ...] [LIMIT n]
     distinct (parse_distinct): SELECT DISTINCT col[, col...] FROM table [WHERE cond] [ORDER BY col [ASC|DESC], ...] [LIMIT n]
                   (every ORDER BY column must be a DISTINCT column)
@@ -26,7 +27,22 @@ from .query import Aggregation, Filter, FilterNode, Predicate, QueryContext, opt
 _TOKEN = re.compile(r"\s*(?:(\d+\.\d+(?:[eE][-+]?\d+)?|-?\d+\.\d+|-?\d+)|'((?:[^']|'')*)'|(<=|>=|<>|!=|[=<>(),*])|"
                     r"([A-Za-z_$][A-Za-z0-9_$]*))")
 
-_FUNCTIONS = {"COUNT", "SUM", "MIN", "MAX", "AVG", "DISTINCTCOUNT"}
+_FUNCTIONS = {"COUNT", "SUM", "MIN", "MAX", "AVG", "DISTINCTCOUNT", "PERCENTILE"}
+_PERCENTILE_N = re.compile(r"PERCENTILE(\d+)")
+
+
+def _is_function(name: str) -> bool:
+    return name.upper() in _FUNCTIONS or _PERCENTILE_N.fullmatch(name.upper()) is not None
+
+
+def _percentile_arg(value) -> float:
+    """The percentile of PERCENTILE(col, p) / PERCENTILE<n>(col): a numeric literal in [0, 100]."""
+    if isinstance(value, bool) or not isinstance(value, (int, float)):
+        raise SqlError(f"PERCENTILE needs a numeric percentile, got {value!r}")
+    p = float(value)
+    if not 0.0 <= p <= 100.0:
+        raise SqlError(f"PERCENTILE percentile {value!r} is outside [0, 100]")
+    return p
 
 
 class SqlError(ValueError):
@@ -81,6 +97,17 @@ class _Parser:
     def expect_op(self, op):
         if not self.take_op(op):
             raise SqlError(f"expected {op!r}, got {self.peek()}")
+
+    def percentile_call(self, name: str):
+        """After `name(`: the column and percentile of PERCENTILE(col, p) or PERCENTILE<n>(col), up to the `)`."""
+        col = self.ident()
+        m = _PERCENTILE_N.fullmatch(name.upper())
+        if m:
+            p = _percentile_arg(int(m.group(1)))
+        else:
+            self.expect_op(",")
+            p = _percentile_arg(self.literal())
+        return col, p
 
     def ident(self) -> str:
         k, v = self.peek()
@@ -166,12 +193,13 @@ def resolve_order_by(query: QueryContext) -> List[tuple]:
         if expr in query.group_by:
             out.append(("GROUP_BY", query.group_by.index(expr), asc))
             continue
-        m = re.fullmatch(r"([A-Za-z_$][A-Za-z0-9_$]*)\((\*|[A-Za-z_$][A-Za-z0-9_$]*)\)", expr)
+        m = re.fullmatch(r"([A-Za-z_$][A-Za-z0-9_$]*)\((\*|[A-Za-z_$][A-Za-z0-9_$]*)(?:,(.+))?\)", expr)
         found = None
         if m:
             fn, col = m.group(1).upper(), m.group(2)
+            arg = None if m.group(3) is None else float(m.group(3))
             for a, agg in enumerate(query.aggregations):
-                if agg.function == fn and (fn == "COUNT" or agg.column == col):
+                if agg.function == fn and (fn == "COUNT" or agg.column == col) and (fn != "PERCENTILE" or agg.arg == arg):
                     found = a
                     break
         if found is None:
@@ -188,9 +216,12 @@ def parse(sql: str, **options) -> QueryContext:
     plain: List[str] = []
     while True:
         name = p.ident()
-        if name.upper() in _FUNCTIONS and p.take_op("("):
+        if _is_function(name) and p.take_op("("):
             fn = name.upper()
-            if p.take_op("*"):
+            if fn.startswith("PERCENTILE"):
+                col, pct = p.percentile_call(name)
+                aggs.append(Aggregation("PERCENTILE", col, arg=pct))
+            elif p.take_op("*"):
                 if fn != "COUNT":
                     raise SqlError(f"{fn}(*) is not valid")
                 aggs.append(Aggregation("COUNT", None))
@@ -225,9 +256,14 @@ def parse(sql: str, **options) -> QueryContext:
             name = p.ident()
             expr = name
             if p.take_op("("):
-                inner = "*" if p.take_op("*") else p.ident()
-                p.expect_op(")")
-                expr = f"{name.lower()}({inner})"
+                if _is_function(name) and name.upper().startswith("PERCENTILE"):
+                    inner, pct = p.percentile_call(name)
+                    p.expect_op(")")
+                    expr = f"percentile({inner},{pct!r})"
+                else:
+                    inner = "*" if p.take_op("*") else p.ident()
+                    p.expect_op(")")
+                    expr = f"{name.lower()}({inner})"
             asc = True
             if p.take_kw("DESC"):
                 asc = False
@@ -271,7 +307,7 @@ def is_selection(sql: str) -> bool:
     while p.peek()[0] is not None and not p.kw("FROM"):
         k, v = p.peek()
         p.i += 1
-        if k == "id" and v.upper() in _FUNCTIONS and p.take_op("("):
+        if k == "id" and _is_function(v) and p.take_op("("):
             return False
     return True
 
@@ -286,7 +322,7 @@ def parse_selection(sql: str) -> SelectionQuery:
     else:
         while True:
             name = p.ident()
-            if name.upper() in _FUNCTIONS and p.peek() == ("op", "("):
+            if _is_function(name) and p.peek() == ("op", "("):
                 raise SqlError(f"{name}(...) in a selection query: aggregations go through parse()")
             columns.append(name)
             if not p.take_op(","):
