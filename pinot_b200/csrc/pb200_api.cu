@@ -310,6 +310,7 @@ extern "C" int32_t pb200_init(int32_t device, pb200_ctx** out) {
     t.dense_max = env_i("PB200_DENSE_MAX", t.dense_max);
     t.defer = getenv("PB200_NO_DEFER") ? 0 : 1;
     t.gb_defer = getenv("PB200_NO_GB_DEFER") ? 0 : 1;
+    t.spec = getenv("PB200_NO_SPEC") ? 0 : 1;
     t.pack_count = getenv("PB200_NO_PACK_COUNT") ? 0 : 1;
     t.pack_shift = (int)env_i("PB200_PACK_SHIFT", 0);
     t.table_stride = (int)env_i("PB200_TABLE_STRIDE", 0);
@@ -338,6 +339,7 @@ extern "C" int32_t pb200_tuning_set(pb200_ctx* ctx, const char* name, int64_t va
   else if (n == "dense_max") t.dense_max = value;
   else if (n == "defer") t.defer = value != 0;
   else if (n == "gb_defer") t.gb_defer = value != 0;
+  else if (n == "spec") t.spec = value != 0;
   else if (n == "pack_count") t.pack_count = value != 0;
   else if (n == "pack_shift") t.pack_shift = (int)value;
   else if (n == "table_stride") t.table_stride = (int)value;
@@ -618,6 +620,11 @@ namespace pb200 {
 cudaError_t launch_scan_variant(const ScanVariant& v, size_t smem_bytes, int grid, const QueryDesc& q, const TmaTable& tt,
                                 const SegDesc* dsegs, cudaStream_t st) {
   if (v.group_by) {
+    if (v.spec) {
+      if (v.warps == 8 && v.min_blocks == 1) return launch_scan_w8_gb1_spec(smem_bytes, grid, q, tt, dsegs, st);
+      if (v.warps == 6 && v.min_blocks == 2) return launch_scan_w6_gb2_spec(smem_bytes, grid, q, tt, dsegs, st);
+      return cudaErrorInvalidValue;
+    }
     if (v.min_blocks >= 2) return v.warps == 8 ? launch_scan_w8_gb2(smem_bytes, grid, q, tt, dsegs, st) : launch_scan_w6_gb2(smem_bytes, grid, q, tt, dsegs, st);
     return v.warps == 8 ? launch_scan_w8_gb1(smem_bytes, grid, q, tt, dsegs, st) : launch_scan_w6_gb1(smem_bytes, grid, q, tt, dsegs, st);
   }

@@ -73,6 +73,7 @@ struct Tuning {
   long long dense_max = 1ll << 24;   // PB200_DENSE_MAX: dense group table up to this many raw keys, hash table beyond
   int defer = 1;                 // !PB200_NO_DEFER: software-pipelined gathers, aggregation-only kernel
   int gb_defer = 1;              // !PB200_NO_GB_DEFER: software-pipelined last queue batch, group-by kernel
+  int spec = 1;                  // !PB200_NO_SPEC: the group-by kernel specialised for the shared-table shape when it qualifies
   int pack_count = 1;            // !PB200_NO_PACK_COUNT: group-by COUNT carried inside an INT SUM's reductions (pb200_plan.cpp)
   int table_stride = 0;          // PB200_TABLE_STRIDE: dense group tables hold raw key k at k * stride (0 = auto, 1 = off)
   int pack_shift = 0;            // PB200_PACK_SHIFT: force the carrier's count shift (tests of the overflow fallback); 0 = from the doc count

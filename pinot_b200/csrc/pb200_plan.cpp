@@ -743,6 +743,29 @@ int plan_scan(const Tuning& tune, DeviceLimits lim, const pb200_query* query, pb
     return PB200_E_UNSUPPORTED;
   }
 
+  // ---- the group-by kernel specialised for the shared-table shape (pb200_scan.cuh SPEC) when the launch has it: a
+  //      conjunction of at most two dictionary range leaves (or constant leaves) in every segment, a dense key over one or
+  //      two columns, the CTA-private table, and COUNT plus at most two INT dictionary sums, all of them pipelined.  It
+  //      runs the same geometry, layouts and descriptors; only the instruction stream differs. ----
+  if (tune.spec && plan.group_by && q.smem_groups > 0 && q.conj && nleaves <= 2 && ngb <= 2 &&
+      ((cw == 8 && ctas_per_sm == 1) || (cw == 6 && ctas_per_sm == 2))) {
+    bool spec = true;
+    for (int a = 0; a < nagg && spec; a++) {
+      const int fn = q.aggs[a].function;
+      spec = fn == PB200_AGG_COUNT || ((fn == PB200_AGG_SUM || fn == PB200_AGG_AVG) && q.aggs[a].val_kind == VAL_DICT_I32 && pipelined[a]);
+    }
+    for (int r = 0; r < nres && spec; r++) spec = !plan.tables[r].hashed;
+    for (int s = 0; s < nseg && spec; s++) {
+      const SegDesc& sd = plan.segs[s];
+      spec = sd.num_agg_codes == sd.num_defer_codes && sd.num_agg_codes <= 2;
+      for (int l = 0; l < nleaves && spec; l++) {
+        const LeafDesc& lf = sd.leaves[l];
+        spec = lf.kind == LEAF_ALL || lf.kind == LEAF_NONE || (lf.kind == LEAF_RANGE && sd.slots[lf.slot].bits <= 31);
+      }
+    }
+    plan.variant.spec = spec;
+  }
+
   // ---- launch chunks of <= kMaxLaunchSegs segments (their TMA table travels in the kernel parameters) ----
   for (int c0 = 0; c0 < nseg; c0 += kMaxLaunchSegs) {
     LaunchChunk ch;

@@ -294,9 +294,17 @@ struct MinMaxLeft {
 //   [survivor queue: W x 1024 u16][group table copies: [count,] (lo, hi) per sum -- optional]   (group-by kernel)
 // acc64/accmm are the per-thread running aggregates; they live in shared memory (private slot per thread, touched once
 // per tile) instead of registers so that two CTAs fit on an SM.
-template <int W, bool GROUPBY, bool DEFER = !GROUPBY, int MINB = (GROUPBY ? 1 : 2)>
+//
+// SPEC: the shared-table GROUP BY shape (plan_scan admits it, ScanVariant::spec): a conjunction of at most two LEAF_RANGE /
+// LEAF_ALL / LEAF_NONE leaves, a dense key over one or two columns, the CTA-private table, COUNT and at most two INT
+// dictionary sums, all of them in the pipelined last batch.  Everything a tile needs about its segment -- leaf bounds and
+// shapes, column widths and stage offsets, key multipliers, dictionaries, addends and table offsets -- is decoded into
+// registers once per segment change; the tile loop then runs without descriptor loads, code decoding or branches for
+// functions the shape cannot have.  The ring, segment changes and table flushes are the generic kernel's.
+template <int W, bool GROUPBY, bool DEFER = !GROUPBY, int MINB = (GROUPBY ? 1 : 2), bool SPEC = false>
 __global__ void __launch_bounds__(W * 32, MINB)
 scan_kernel(const __grid_constant__ QueryDesc q, const __grid_constant__ TmaTable tt, const SegDesc* __restrict__ segs) {
+  static_assert(!SPEC || GROUPBY, "the specialised shape is a GROUP BY");
   extern __shared__ __align__(128) unsigned char smem_raw[];
   // The shared-window base is made opaque to the compiler once: otherwise every access through hdr-> / the accumulator
   // pointers rematerialises it as S2R SR_CgaCtaId + LEA (a variable-latency special-register read per access).
@@ -429,8 +437,67 @@ scan_kernel(const __grid_constant__ QueryDesc q, const __grid_constant__ TmaTabl
   uint32_t px[GROUPBY ? kGD : 1][GROUPBY ? kQB : 1];  // loaded word: biased / float dictionary value, or current MIN / MAX entry
   uint32_t pq[GROUPBY ? kGD : 1][GROUPBY ? kQB : 1];  // MIN / MAX: the row's order-preserving encoding
   uint32_t pend_ok = 0;                      // bit u: entry u is pending
+
+  // SPEC: the current segment in registers (loaded at every segment change)
+  constexpr int kS = SPEC ? 2 : 1;           // leaves, group-by columns and sums of the shape: at most two each
+  enum { SL_ALL = 0, SL_NONE, SL_GE, SL_LT, SL_BOTH };
+  int sl_shape[kS], sl_bits[kS], sg_bits[kS], ss_bits[kS];
+  uint32_t sl_neg[kS], sl_lo[kS], sl_span[kS], sl_off[kS];      // leaf: ~0 when negated, dictId range, stage offset
+  uint32_t sg_off[kS], sg_mult[kS];                             // group-by column: stage offset, key multiplier
+  uint32_t ss_off[kS], ss_tab[kS];                              // sum: stage offset, word offset of its lo array (lane's copy)
+  const uint32_t* ss_dict[kS];
+  unsigned long long ss_add[kS];
+  int s_ng = 0, s_ns = 0;                                       // group-by columns, sums
+  auto load_spec = [&]() {
+    if constexpr (SPEC) {
+#pragma unroll
+      for (int l = 0; l < kS; ++l) {
+        const uint32_t code = l < q.num_leaves ? sd.leaves[l].code : (uint32_t)LEAF_ALL;
+        const int kind = (int)(code & 7u), cmp = (int)((code >> 4) & 3u);
+        sl_shape[l] = kind == LEAF_NONE ? SL_NONE : kind != LEAF_RANGE ? SL_ALL : cmp == CMP_GE ? SL_GE : cmp == CMP_LT ? SL_LT : SL_BOTH;
+        sl_neg[l] = ((code >> 8) & 1u) ? 0xFFFFFFFFu : 0u;
+        sl_bits[l] = (int)((code >> 12) & 63u);
+        sl_off[l] = code >> 18;
+        sl_lo[l] = sd.leaves[l].lo;
+        sl_span[l] = sd.leaves[l].span;
+      }
+      s_ng = q.num_group_by;
+#pragma unroll
+      for (int k = 0; k < kS; ++k) {
+        const SlotDesc& sl = sd.slots[hdr->group_slot[k < s_ng ? k : 0]];
+        sg_bits[k] = sl.bits;
+        sg_off[k] = sl.stage_words;
+        sg_mult[k] = sd.group_mult[k];
+      }
+      s_ns = sd.num_agg_codes;  // every one of them is pipelined (num_defer_codes)
+#pragma unroll
+      for (int k = 0; k < kS; ++k) {
+        const uint32_t ac = sd.agg_code[k < s_ns ? k : 0];
+        const int a = (int)(ac & 7u);
+        ss_bits[k] = (int)((ac >> 12) & 63u);
+        ss_off[k] = ac >> 18;
+        ss_dict[k] = static_cast<const uint32_t*>(sd.dict[a]);
+        ss_add[k] = sd.sum_addend[a];
+        ss_tab[k] = tcopy + TA * ((uint32_t)q.smem_count + 2u * (uint32_t)q.smem_slot[a]);
+      }
+    }
+  };
+
   auto drain_gb = [&]() {
-    if constexpr (GROUPBY) {
+    if constexpr (SPEC) {
+      if (pend_ok) {
+#pragma unroll
+        for (int k = 0; k < kGD; ++k) {
+          if (k < s_ns) {
+            uint32_t* lo = tcnt + ss_tab[k];
+#pragma unroll
+            for (int u = 0; u < kQB; ++u)
+              if ((pend_ok >> u) & 1u) smem_add64(lo, lo + TA, pg[u], (unsigned long long)px[k][u] + ss_add[k]);
+          }
+        }
+        pend_ok = 0;
+      }
+    } else if constexpr (GROUPBY) {
       if (pend_ok) {
         const int n = sd.num_agg_codes, nd = sd.num_defer_codes;
 #pragma unroll
@@ -568,6 +635,7 @@ scan_kernel(const __grid_constant__ QueryDesc q, const __grid_constant__ TmaTabl
       c_first = tt.seg[ns].first_tile;
       c_end = tt.seg[ns].end_tile;
       c_docs = tt.seg[ns].num_docs;
+      load_spec();
     }
     const uint32_t row0 = (uint32_t)((T - c_first) * W + warp) * 1024u + (uint32_t)lane * kRowsPerThread;
     const int left = row0 >= c_docs ? 0 : (c_docs - row0 >= 32u ? 32 : (int)(c_docs - row0));
@@ -583,7 +651,42 @@ scan_kernel(const __grid_constant__ QueryDesc q, const __grid_constant__ TmaTabl
     // thread survive, the remaining columns are probed per surviving row straight from the shared-memory tile
     // (the GPU form of ScanBasedDocIdIterator.applyAnd on the bitmap of survivors, AndDocIdSet.java:167-169)
     // instead of unpacking all 32 values.
-    if (q.num_nodes > 0 && __any_sync(0xFFFFFFFFu, m != 0u)) {
+    if constexpr (SPEC) {
+      // the same leaf-by-leaf conjunction over range leaves, its parameters selected from registers
+      if (q.num_leaves > 0 && __any_sync(0xFFFFFFFFu, m != 0u)) {
+#pragma unroll 1
+        for (int l = 0; l < q.num_leaves; ++l) {
+          const int shape = l == 0 ? sl_shape[0] : sl_shape[1];
+          uint32_t lm = 0xFFFFFFFFu;
+          if (shape == SL_NONE) {
+            lm = 0u;
+          } else if (shape != SL_ALL) {
+            const int sbits = l == 0 ? sl_bits[0] : sl_bits[1];
+            const uint32_t* base = st + (l == 0 ? sl_off[0] : sl_off[1]);
+            const uint32_t lf_lo = l == 0 ? sl_lo[0] : sl_lo[1], lf_span = l == 0 ? sl_span[0] : sl_span[1];
+            const int wmax = l == 0 ? 32 : __reduce_max_sync(0xFFFFFFFFu, __popc(m));
+            if (wmax == 0) {
+              lm = 0u;
+            } else if (wmax <= q.sparse_max) {
+              const uint32_t* p = base + group_in_stage * sbits;
+              uint32_t keep = 0, mm = m;
+              while (mm) {
+                const int j = 31 - __clz(mm);
+                mm &= ~(1u << j);
+                keep |= ((read_one_group(p, j, sbits) - lf_lo) < lf_span ? 1u : 0u) << j;
+              }
+              lm = keep;
+            } else {
+              const int sh = 32 - sbits;
+              if (shape == SL_GE) { RangeGE f; f.LO = lf_lo << sh; dispatch_left_aligned(sbits, base, group_in_stage, f); lm = f.mask(); }
+              else if (shape == SL_LT) { RangeLT f; f.HI = (lf_lo + lf_span) << sh; dispatch_left_aligned(sbits, base, group_in_stage, f); lm = f.mask(); }
+              else { RangeBoth f; f.LO = lf_lo << sh; f.SPAN = lf_span << sh; dispatch_left_aligned(sbits, base, group_in_stage, f); lm = f.mask(); }
+            }
+          }
+          m &= lm ^ (l == 0 ? sl_neg[0] : sl_neg[1]);
+        }
+      }
+    } else if (q.num_nodes > 0 && __any_sync(0xFFFFFFFFu, m != 0u)) {
       if (q.conj) {
 #pragma unroll 1
         for (int l = 0; l < q.num_leaves; ++l) {
@@ -765,6 +868,52 @@ scan_kernel(const __grid_constant__ QueryDesc q, const __grid_constant__ TmaTabl
           bool ok[kQB];
 #pragma unroll
           for (int u = 0; u < kQB; ++u) { ok[u] = i0 + 32 * u < S; e[u] = ok[u] ? (uint32_t)wq[i0 + 32 * u] : 0u; g[u] = 0u; }
+          if constexpr (SPEC) {
+            // dense key, the CTA's shared table, COUNT and pipelined INT sums only: the generic batch below without its
+            // descriptor loads and dispatch
+#pragma unroll
+            for (int k = 0; k < kS; ++k) {
+              if (k == 0 || k < s_ng) {
+#pragma unroll
+                for (int u = 0; u < kQB; ++u)
+                  g[u] += read_one_group(st + sg_off[k] + (e[u] >> 5) * sg_bits[k], (int)(e[u] & 31u), sg_bits[k]) * sg_mult[k];
+              }
+            }
+            if (q.smem_count) {
+#pragma unroll
+              for (int u = 0; u < kQB; ++u) if (ok[u]) atomicAdd(tcnt + tcopy + g[u], 1u);
+            }
+            if (last && s_ns > 0) {   // issue the gathers; drain_gb adds them to the table one tile later
+              uint32_t okm = 0;
+#pragma unroll
+              for (int u = 0; u < kQB; ++u) { okm |= (ok[u] ? 1u : 0u) << u; pg[u] = g[u]; }
+#pragma unroll
+              for (int k = 0; k < kGD; ++k) {
+                if (k < s_ns) {
+#pragma unroll
+                  for (int u = 0; u < kQB; ++u) {
+                    const uint32_t id = read_one_group(st + ss_off[k] + (e[u] >> 5) * ss_bits[k], (int)(e[u] & 31u), ss_bits[k]);
+                    px[k][u] = (uint32_t)ldg_pred_s32(reinterpret_cast<const int*>(ss_dict[k] + id), ok[u] ? 1u : 0u);
+                  }
+                }
+              }
+              pend_ok = okm;
+            } else if (!last) {
+#pragma unroll
+              for (int k = 0; k < kGD; ++k) {
+                if (k < s_ns) {
+                  uint32_t xv[kQB];
+#pragma unroll
+                  for (int u = 0; u < kQB; ++u)
+                    xv[u] = __ldg(ss_dict[k] + read_one_group(st + ss_off[k] + (e[u] >> 5) * ss_bits[k], (int)(e[u] & 31u), ss_bits[k]));
+                  uint32_t* lo = tcnt + ss_tab[k];
+#pragma unroll
+                  for (int u = 0; u < kQB; ++u) if (ok[u]) smem_add64(lo, lo + TA, g[u], (unsigned long long)xv[u] + ss_add[k]);
+                }
+              }
+            }
+            continue;
+          }
           if (sd.h_keys) {  // hash table: 64-bit raw key -> slot
             unsigned long long key[kQB];
 #pragma unroll
@@ -903,7 +1052,7 @@ scan_kernel(const __grid_constant__ QueryDesc q, const __grid_constant__ TmaTabl
         handled = true;  // the __syncwarp() before the ring refill also orders the queue reads before the next appends
       }
     }
-    if (handled) {
+    if (handled || SPEC) {
     } else if (wmax2 > 0 && wmax2 <= q.sparse_max_agg) {
       uint32_t mm = m;
       while (mm) {

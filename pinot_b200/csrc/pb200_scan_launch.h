@@ -13,6 +13,7 @@ struct ScanVariant {
   bool group_by;
   bool defer;      // aggregation only: dictionary gathers of the deferred SUM are software-pipelined across tiles
   int min_blocks;  // __launch_bounds__ minBlocksPerMultiprocessor
+  bool spec;       // group-by: the kernel specialised for the shared-table shape (pb200_scan.cuh SPEC; 8 x 1 or 6 x 2 only)
 };
 
 // Launches the matching instantiation on `st`.  cudaErrorInvalidValue if the variant was not built.
@@ -28,5 +29,7 @@ PB200_SCAN_LAUNCHER(launch_scan_w6_gb1);        // <6, true, false, 1>
 PB200_SCAN_LAUNCHER(launch_scan_w8_gb1);        // <8, true, false, 1>
 PB200_SCAN_LAUNCHER(launch_scan_w6_gb2);        // <6, true, false, 2>
 PB200_SCAN_LAUNCHER(launch_scan_w8_gb2);        // <8, true, false, 2>
+PB200_SCAN_LAUNCHER(launch_scan_w8_gb1_spec);   // <8, true, false, 1, true>
+PB200_SCAN_LAUNCHER(launch_scan_w6_gb2_spec);   // <6, true, false, 2, true>
 
 }  // namespace pb200
