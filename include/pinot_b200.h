@@ -345,6 +345,52 @@ int32_t pb200_result_selection(const pb200_result* result, int64_t* rows, const 
 int32_t pb200_execute_distinct(pb200_ctx* ctx, const pb200_query* filter_only, const pb200_selection* distinct,
                                pb200_segment* const* segments, int32_t num_segments, int32_t flags, pb200_result** results);
 
+/* ---- derived columns: single-column transforms (DATETRUNC, date parts, time conversions, arithmetic with literals) ---- */
+/* A function of one dictionary column is a function of its dictId: the program is evaluated once per entry of the
+ * column's (device) dictionary, the distinct results sorted into a new dictionary, and the forward index re-encoded
+ * through dictId -> rank once.  The result is an ordinary dictionary column: every query route takes it unchanged.
+ * Programs are POSTFIX: leaves push a value (the column, or a literal), operations pop their operands and push one value.
+ * Semantics (DESIGN.md section 3.8):
+ *   PLUS, MINUS, TIMES, DIVIDE, MOD (x, y), FLOOR, CEIL, ABS (x)  operands as doubles, one round-to-nearest operation each,
+ *                                       MOD = C fmod (Java %), x / 0 = +-inf or NaN; result DOUBLE
+ *   DATETRUNC (x)    i = unit | inUnit << 8 | outUnit << 16 (PB200_DT_* unit, PB200_TU_* time units): ms = inUnit.toMillis(x)
+ *                    floored to the start of the UTC unit (WEEK: ISO, Monday), then outUnit.convert(ms, MILLISECONDS); LONG
+ *   YEAR .. MILLISECOND (x)  UTC calendar fields of epoch ms x (proleptic Gregorian; WEEK is the ISO week, DAYOFWEEK
+ *                    1 = Monday); INT
+ *   TIMECONVERT (x)  i = inUnit | outUnit << 8: outUnit.convert(x, inUnit) (toward 0 when coarser, saturated when finer); LONG
+ *   TOEPOCH (x), TOEPOCH_BUCKET / _ROUNDED (x, n)  i = PB200_TU_SECONDS .. DAYS: x ms in that unit (toward 0), / n,
+ *                    (/ n) * n; n a positive LONG literal; LONG
+ * Time functions take INT / LONG operands only (the column or another time function).  DATETRUNC and the calendar fields
+ * refuse a dictionary holding an instant beyond +-2^53 ms (after the input-unit conversion). */
+enum { PB200_T_COLUMN = 0, PB200_T_LONG_LITERAL = 1, PB200_T_DOUBLE_LITERAL = 2,
+       PB200_T_PLUS = 3, PB200_T_MINUS = 4, PB200_T_TIMES = 5, PB200_T_DIVIDE = 6, PB200_T_MOD = 7,
+       PB200_T_FLOOR = 8, PB200_T_CEIL = 9, PB200_T_ABS = 10, PB200_T_DATETRUNC = 11,
+       PB200_T_YEAR = 12, PB200_T_QUARTER = 13, PB200_T_MONTH = 14, PB200_T_WEEK = 15, PB200_T_DAY = 16,
+       PB200_T_DAYOFWEEK = 17, PB200_T_DAYOFYEAR = 18, PB200_T_HOUR = 19, PB200_T_MINUTE = 20, PB200_T_SECOND = 21,
+       PB200_T_MILLISECOND = 22, PB200_T_TIMECONVERT = 23, PB200_T_TOEPOCH = 24, PB200_T_TOEPOCH_BUCKET = 25,
+       PB200_T_TOEPOCH_ROUNDED = 26 };
+enum { PB200_TU_NANOSECONDS = 0, PB200_TU_MICROSECONDS = 1, PB200_TU_MILLISECONDS = 2, PB200_TU_SECONDS = 3,
+       PB200_TU_MINUTES = 4, PB200_TU_HOURS = 5, PB200_TU_DAYS = 6 };
+enum { PB200_DT_MILLISECOND = 0, PB200_DT_SECOND = 1, PB200_DT_MINUTE = 2, PB200_DT_HOUR = 3, PB200_DT_DAY = 4,
+       PB200_DT_WEEK = 5, PB200_DT_MONTH = 6, PB200_DT_QUARTER = 7, PB200_DT_YEAR = 8 };
+typedef struct {
+  int32_t op;        /* PB200_T_* */
+  int32_t reserved;  /* 0 */
+  int64_t i;         /* LONG literal, or the operation's units */
+  double d;          /* DOUBLE literal */
+} pb200_transform_op;
+#define PB200_MAX_DERIVED_COLUMNS 32 /* derived columns per segment */
+/* Adds the derived column `program(source_column)` to the segment and returns its column id (the next free id, after
+ * the registered and earlier derived columns).  The source must carry dictIds: INT / LONG / FLOAT / DOUBLE dictionaries,
+ * raw columns whose dictionary was synthesised at load, or a column bound to a domain (the program then runs over the
+ * domain's dictionary, so every bound segment derives the same dictionary, and pb200_segment_local_ids gives the derived
+ * ids this segment holds).  The new column has no inverted index, is never sorted, and counts in
+ * pb200_segment_device_bytes.  Queries already running on the segment are not disturbed: no existing column moves.
+ * PB200_E_UNSUPPORTED: STRING or raw 32-bit sources, a program outside the supported set, an instant beyond +-2^53 ms,
+ * more than PB200_MAX_DERIVED_COLUMNS derived columns.  PB200_E_INVALID: a malformed program. */
+int32_t pb200_segment_derive_column(pb200_ctx* ctx, pb200_segment* segment, int32_t source_column, int32_t num_ops,
+                                    const pb200_transform_op* ops, int32_t* new_column);
+
 /* ---- results (the data a GroupByResultsBlock / AggregationResultsBlock is built from) ---------------------------- */
 enum { PB200_REGIME_NONE = 0, PB200_REGIME_ARRAY = 1, PB200_REGIME_INT_MAP = 2, PB200_REGIME_LONG_MAP = 3,
        PB200_REGIME_ARRAY_MAP = 4 };

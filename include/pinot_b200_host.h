@@ -65,6 +65,24 @@ int32_t pb200h_segment_column_info(const pb200h_segment* segment, int32_t column
 int32_t pb200h_dictionary_get(const pb200h_segment* segment, int32_t column, int32_t dict_id, double* num, int64_t* lng,
                               char* str, int32_t str_capacity);
 
+/* ---- derived columns: single-column expressions by their canonical text (pb200_segment_derive_column) ------------- */
+/* An expression is named by the text of the reference's ExpressionContext.toString(): function names in lower case
+ * without '_', arguments separated by ',' without spaces, literals in single quotes -- datetrunc('DAY',ts),
+ * divide(ts,'1000').  Aliases (DATE_TRUNC is datetrunc, ADD is plus, DOW is dayofweek, ...), time-unit literals in any
+ * case and numeric literals by value are normalised first, so two spellings share one derived column.  That text is then
+ * the column's name wherever a column name is accepted: pb200h_execute*, selection / DISTINCT columns and order items,
+ * filter leaves, FILTER (WHERE ...) clauses, pb200h_domain_build, pb200h_explain -- each of them derives an expression it
+ * does not know yet on every segment of the call, once per segment, before planning.  A stored column whose name equals
+ * the text wins.  pb200h_segment_column_index / _column_info / pb200h_dictionary_get describe derived columns (types
+ * LONG, INT or DOUBLE); pb200h_segment_num_columns counts stored columns only.  A derived column is never answered from
+ * its dictionary alone (NonScanBasedAggregationOperator), has no inverted or sorted index, is no star-tree dimension, and
+ * is freed with its segment.  Expressions derived in different orders on different segments can land at different
+ * column ids: a call over such segments is PB200_E_UNSUPPORTED.
+ * Explicit derivation: `column` receives the derived column's id.  PB200_E_INVALID: malformed text or an unknown column;
+ * PB200_E_UNSUPPORTED: see pb200_segment_derive_column, plus two or more columns, unknown functions, wrong argument types
+ * or counts, time zones other than UTC. */
+int32_t pb200h_segment_derive(pb200_ctx* ctx, pb200h_segment* segment, const char* expression, int32_t* column);
+
 /* ---- HBM residency (what BaseTableDataManager + SegmentDataManager reference counting are to the JVM heap / page cache) ---- */
 /* Segments resident on the device, keyed by (segment name, CRC) -- SegmentMetadata.getName() / getCrc(); a new CRC under a
  * known name is a refresh (BaseTableDataManager.replaceSegment).  A byte budget (0 = 80 % of the device) with least-recently-

@@ -61,6 +61,46 @@ JNIEXPORT jint JNICALL CLS(segmentRelease)(JNIEnv* env, jclass cls, jlong ctx, j
   return pb200_segment_release((pb200_ctx*)(intptr_t)ctx, (pb200_segment*)(intptr_t)seg);
 }
 
+JNIEXPORT jint JNICALL CLS(segmentDeriveColumn)(JNIEnv* env, jclass cls, jlong ctx, jlong seg, jint source, jintArray op,
+                                                jlongArray iv, jdoubleArray dv) {
+  jsize n = (*env)->GetArrayLength(env, op);
+  if (n <= 0 || n > 64 || (*env)->GetArrayLength(env, iv) != n || (*env)->GetArrayLength(env, dv) != n) return PB200_E_INVALID;
+  pb200_transform_op prog[64];
+  jint* o = (*env)->GetIntArrayElements(env, op, NULL);
+  jlong* i = (*env)->GetLongArrayElements(env, iv, NULL);
+  jdouble* d = (*env)->GetDoubleArrayElements(env, dv, NULL);
+  for (jsize k = 0; k < n; k++) { prog[k].op = o[k]; prog[k].reserved = 0; prog[k].i = i[k]; prog[k].d = d[k]; }
+  (*env)->ReleaseIntArrayElements(env, op, o, JNI_ABORT);
+  (*env)->ReleaseLongArrayElements(env, iv, i, JNI_ABORT);
+  (*env)->ReleaseDoubleArrayElements(env, dv, d, JNI_ABORT);
+  int32_t column = -1;
+  int32_t rc = pb200_segment_derive_column((pb200_ctx*)(intptr_t)ctx, (pb200_segment*)(intptr_t)seg, source, n, prog, &column);
+  return rc ? rc : column;
+}
+
+JNIEXPORT jint JNICALL CLS(segmentColumnInfo)(JNIEnv* env, jclass cls, jlong seg, jint column, jlongArray infoOut) {
+  if ((*env)->GetArrayLength(env, infoOut) < 6) return PB200_E_INVALID;
+  int64_t info[6];
+  int32_t rc = pb200_segment_column_info((const pb200_segment*)(intptr_t)seg, column, info);
+  jlong* o = (*env)->GetLongArrayElements(env, infoOut, NULL);
+  for (int k = 0; k < 6 && rc == PB200_OK; k++) o[k] = info[k];
+  (*env)->ReleaseLongArrayElements(env, infoOut, o, 0);
+  return rc;
+}
+
+JNIEXPORT jbyteArray JNICALL CLS(segmentDictionary)(JNIEnv* env, jclass cls, jlong ctx, jlong seg, jint column) {
+  pb200_ctx* c = (pb200_ctx*)(intptr_t)ctx;
+  const pb200_segment* s = (const pb200_segment*)(intptr_t)seg;
+  int64_t n = pb200_segment_read_index(c, s, column, 1, NULL, 0);
+  if (n < 0) return NULL;
+  jbyteArray out = (*env)->NewByteArray(env, (jsize)n);
+  if (!out || n == 0) return out;
+  jbyte* b = (*env)->GetByteArrayElements(env, out, NULL);
+  int64_t r = pb200_segment_read_index(c, s, column, 1, b, (uint64_t)n);
+  (*env)->ReleaseByteArrayElements(env, out, b, 0);
+  return r < 0 ? NULL : out;
+}
+
 JNIEXPORT jint JNICALL CLS(execute)(JNIEnv* env, jclass cls, jlong ctx, jlongArray segments, jint numNodes, jintArray op,
                                     jintArray column, jintArray numChildren, jintArray lo, jintArray hi, jintArray ids,
                                     jintArray idsOffset, jintArray idsLength, jintArray groupBy, jintArray aggFn,

@@ -36,6 +36,16 @@ public final class B200Native {
   public static native long segmentRegister(long ctx, String segmentName, int numDocs, int[] fwdKind, int[] storedType,
       int[] bits, int[] cardinality, ByteBuffer[] fwd, ByteBuffer[] dict, ByteBuffer[] inv);
   public static native int segmentRelease(long ctx, long segment);
+  /**
+   * pb200_segment_derive_column: the postfix program (op[k], i[k], d[k]) of a single-column expression over
+   * sourceColumn.  Returns the new column id, or a negative PB200_E_* code (see lastError(); E_UNSUPPORTED: run the
+   * stock operator).
+   */
+  public static native int segmentDeriveColumn(long ctx, long segment, int sourceColumn, int[] op, long[] i, double[] d);
+  /** pb200_segment_column_info into infoOut[6]: {fwd_kind, stored_type, bits, cardinality, has_inverted, fwd_bytes}. */
+  public static native int segmentColumnInfo(long segment, int column, long[] infoOut);
+  /** pb200_segment_read_index(..., which = 1): the column's big-endian dictionary bytes, or null. */
+  public static native byte[] segmentDictionary(long ctx, long segment, int column);
 
   /**
    * pb200_execute for ONE query over n segments.  The filter is flattened in postfix order, one tree per segment

@@ -64,7 +64,10 @@ public class B200Operator extends BaseOperator<BaseResultsBlock> {
     _fallback = fallback;
   }
 
-  /** AND / OR / NOT of EQ / NOT_EQ / IN / NOT_IN / RANGE on dictionary-encoded single-value identifiers. */
+  /**
+   * AND / OR / NOT of EQ / NOT_EQ / IN / NOT_IN / RANGE on dictionary-encoded single-value identifiers, or on
+   * single-column transform expressions (B200Transform: answered over a derived dictionary column).
+   */
   static boolean filterIsAccelerated(FilterContext filter, IndexSegment segment) {
     if (filter == null) {
       return true;
@@ -75,11 +78,14 @@ public class B200Operator extends BaseOperator<BaseResultsBlock> {
       case PREDICATE:
         Predicate p = filter.getPredicate();
         if (p.getLhs().getType() != ExpressionContext.Type.IDENTIFIER) {
-          return false;
-        }
-        DataSource ds = segment.getDataSource(p.getLhs().getIdentifier());
-        if (ds.getDictionary() == null || !ds.getDataSourceMetadata().isSingleValue()) {
-          return false;
+          if (!B200Transform.accepted(p.getLhs(), segment)) {
+            return false;
+          }
+        } else {
+          DataSource ds = segment.getDataSource(p.getLhs().getIdentifier());
+          if (ds.getDictionary() == null || !ds.getDataSourceMetadata().isSingleValue()) {
+            return false;
+          }
         }
         switch (p.getType()) {
           case EQ: case NOT_EQ: case IN: case NOT_IN: case RANGE:
@@ -121,6 +127,24 @@ public class B200Operator extends BaseOperator<BaseResultsBlock> {
         break;
     }
     Predicate predicate = filter.getPredicate();
+    if (predicate.getLhs().getType() != ExpressionContext.Type.IDENTIFIER) {
+      // a derived column: resolved on its (sorted) dictionary; it has no inverted or sorted index, so the leaf is a scan
+      B200Transform.Derived d = derived(predicate.getLhs());
+      int[] ids = d.matchingIds(predicate);
+      if (ids == null) {
+        throw new Refused();
+      }
+      if (ids.length == 0) {
+        out.add(F_EMPTY, d._column, 0, 0, 0, null);
+      } else if (ids.length == d.cardinality()) {
+        out.add(F_MATCH_ALL, d._column, 0, 0, 0, null);
+      } else if (predicate.getType() == Predicate.Type.RANGE) {
+        out.add(F_SCAN_RANGE, d._column, 0, ids[0], ids[ids.length - 1] + 1, null);
+      } else {
+        out.add(F_SCAN_IN, d._column, 0, 0, 0, ids);
+      }
+      return;
+    }
     String column = predicate.getLhs().getIdentifier();
     DataSource ds = _segment.getDataSource(column);
     Dictionary dictionary = ds.getDictionary();
@@ -193,24 +217,67 @@ public class B200Operator extends BaseOperator<BaseResultsBlock> {
     return flat;
   }
 
+  /** The library refused a derived column (or a predicate on one): the stock operator answers the query. */
+  private static final class Refused extends RuntimeException {
+    Refused() {
+      super(null, null, false, false);
+    }
+  }
+
+  private B200SegmentCache.Resident _resident;
+
+  /** The derived column of a transform expression on this segment (derived by the first query that names it). */
+  private B200Transform.Derived derived(ExpressionContext e) {
+    B200Transform.Derived d = _resident.derive(_ctx, e);
+    if (d == null) {
+      throw new Refused();
+    }
+    return d;
+  }
+
+  private int columnOf(ExpressionContext e) {
+    return e.getType() == ExpressionContext.Type.IDENTIFIER ? _resident.columnId(e.getIdentifier()) : derived(e)._column;
+  }
+
+  /** Dictionary.getInternal(dictId) of a column or of a derived column. */
+  private java.util.function.IntFunction<Object> decoder(ExpressionContext e) {
+    if (e.getType() != ExpressionContext.Type.IDENTIFIER) {
+      return derived(e)::get;
+    }
+    Dictionary dictionary = _segment.getDataSource(e.getIdentifier()).getDictionary();
+    return dictionary::getInternal;
+  }
+
+  private BaseResultsBlock stock() {
+    Operator<? extends BaseResultsBlock> stock = _fallback.get();
+    BaseResultsBlock block = stock.nextBlock();
+    _statistics = stock.getExecutionStatistics();
+    return block;
+  }
+
   @Override
   protected BaseResultsBlock getNextBlock() {
-    B200SegmentCache.Resident resident = _cache.get(_segment);
+    _resident = _cache.get(_segment);
+    B200SegmentCache.Resident resident = _resident;
     Nodes nodes = new Nodes();
-    if (_queryContext.getFilter() != null) {
-      flatten(_queryContext.getFilter(), resident, nodes);
-    }
     AggregationFunction[] functions = _queryContext.getAggregationFunctions();
     int[] aggFunctions = new int[functions.length];
     int[] aggColumns = new int[functions.length];
-    for (int i = 0; i < functions.length; i++) {
-      aggFunctions[i] = nativeFunction(functions[i]);
-      List<ExpressionContext> inputs = functions[i].getInputExpressions();
-      aggColumns[i] = inputs.isEmpty() ? -1 : resident.columnId(inputs.get(0).getIdentifier());
-    }
     List<ExpressionContext> groupBy = _queryContext.getGroupByExpressions();
-    int[] groupByColumns = groupBy == null ? new int[0]
-        : groupBy.stream().mapToInt(e -> resident.columnId(e.getIdentifier())).toArray();
+    int[] groupByColumns;
+    try {
+      if (_queryContext.getFilter() != null) {
+        flatten(_queryContext.getFilter(), resident, nodes);
+      }
+      for (int i = 0; i < functions.length; i++) {
+        aggFunctions[i] = nativeFunction(functions[i]);
+        List<ExpressionContext> inputs = functions[i].getInputExpressions();
+        aggColumns[i] = inputs.isEmpty() ? -1 : columnOf(inputs.get(0));
+      }
+      groupByColumns = groupBy == null ? new int[0] : groupBy.stream().mapToInt(this::columnOf).toArray();
+    } catch (Refused refused) {
+      return stock();
+    }
     int n = nodes._rows.size();
     int[] op = new int[n], column = new int[n], children = new int[n], lo = new int[n], hi = new int[n],
         idsOffset = new int[n], idsLength = new int[n];
@@ -226,10 +293,7 @@ public class B200Operator extends BaseOperator<BaseResultsBlock> {
     if (rc == B200Native.E_UNSUPPORTED || rc == B200Native.E_LIMIT) {
       // outside the accelerated set (e.g. LONG_MAP / ARRAY_MAP key spaces, numGroupsLimit binding): run the stock
       // operator so results stay exactly the reference's
-      Operator<? extends BaseResultsBlock> stock = _fallback.get();
-      BaseResultsBlock block = stock.nextBlock();
-      _statistics = stock.getExecutionStatistics();
-      return block;
+      return stock();
     }
     if (rc != B200Native.OK) {
       throw new RuntimeException("pb200_execute failed for segment " + _segment.getSegmentName() + ": "
@@ -263,8 +327,10 @@ public class B200Operator extends BaseOperator<BaseResultsBlock> {
     int k = groupBy.size();
     int[] keyIds = new int[rows * k];
     B200Native.resultGroupKeys(result, keyIds);
-    Dictionary[] dictionaries = groupBy.stream().map(e -> _segment.getDataSource(e.getIdentifier()).getDictionary())
-        .toArray(Dictionary[]::new);
+    List<java.util.function.IntFunction<Object>> dictionaries = new ArrayList<>();
+    for (ExpressionContext e : groupBy) {
+      dictionaries.add(decoder(e));
+    }
     GroupKeyGenerator generator = new GroupKeyGenerator() {
       @Override public int getGlobalGroupKeyUpperBound() { return rows; }
       @Override public void generateKeysForBlock(org.apache.pinot.core.operator.blocks.ValueBlock b, int[] out) { throw new UnsupportedOperationException(); }
@@ -279,7 +345,7 @@ public class B200Operator extends BaseOperator<BaseResultsBlock> {
           @Override public GroupKey next() {
             Object[] keys = new Object[k];
             for (int j = 0; j < k; j++) {
-              keys[j] = dictionaries[j].getInternal(keyIds[_next * k + j]);
+              keys[j] = dictionaries.get(j).apply(keyIds[_next * k + j]);
             }
             _groupKey._groupId = _next++;
             _groupKey._keys = keys;
@@ -326,11 +392,10 @@ public class B200Operator extends BaseOperator<BaseResultsBlock> {
       case DISTINCTCOUNT: {
         // the reference returns the VALUE set (BaseDistinctAggregateAggregationFunction.extractAggregationResult
         // converts the dictId bitmap with convertToValueSet): do the same from the returned dictIds
-        Dictionary dictionary = _segment.getDataSource(((ExpressionContext) function.getInputExpressions().get(0))
-            .getIdentifier()).getDictionary();
+        java.util.function.IntFunction<Object> dictionary = decoder((ExpressionContext) function.getInputExpressions().get(0));
         Set<Object> values = new HashSet<>();
         for (int id : B200Native.resultDistinct(result, a, row)) {
-          values.add(dictionary.getInternal(id));
+          values.add(dictionary.apply(id));
         }
         return values;
       }
@@ -346,8 +411,9 @@ public class B200Operator extends BaseOperator<BaseResultsBlock> {
     DataSchema.ColumnDataType[] types = new DataSchema.ColumnDataType[k + functions.length];
     for (int j = 0; j < k; j++) {
       names[j] = groupBy.get(j).toString();
-      types[j] = DataSchema.ColumnDataType.fromDataTypeSV(
-          _segment.getDataSource(groupBy.get(j).getIdentifier()).getDataSourceMetadata().getDataType());
+      ExpressionContext e = groupBy.get(j);
+      types[j] = DataSchema.ColumnDataType.fromDataTypeSV(e.getType() == ExpressionContext.Type.IDENTIFIER
+          ? _segment.getDataSource(e.getIdentifier()).getDataSourceMetadata().getDataType() : derived(e)._type);
     }
     for (int a = 0; a < functions.length; a++) {
       names[k + a] = functions[a].getResultColumnName();

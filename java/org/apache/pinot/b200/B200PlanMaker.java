@@ -49,7 +49,10 @@ public class B200PlanMaker extends InstancePlanMakerImplV2 {
         () -> B200PlanMaker.super.makeSegmentPlanNode(segmentContext, queryContext).run());
   }
 
-  /** The accelerated set: identifier-only expressions, no null handling, COUNT/SUM/MIN/MAX/AVG/DISTINCTCOUNT. */
+  /**
+   * The accelerated set: identifiers and single-column transform expressions (B200Transform), no null handling,
+   * COUNT/SUM/MIN/MAX/AVG/DISTINCTCOUNT.
+   */
   static boolean isAccelerated(QueryContext queryContext, IndexSegment segment) {
     if (queryContext.isNullHandlingEnabled() || queryContext.getFilteredAggregationsIndexMap() != null
         && !queryContext.getFilteredAggregationsIndexMap().isEmpty()) {
@@ -64,8 +67,14 @@ public class B200PlanMaker extends InstancePlanMakerImplV2 {
       }
       for (Object e : function.getInputExpressions()) {
         ExpressionContext expression = (ExpressionContext) e;
-        if (expression.getType() != ExpressionContext.Type.IDENTIFIER
-            || !segment.getDataSource(expression.getIdentifier()).getDataSourceMetadata().isSingleValue()) {
+        if (expression.getType() != ExpressionContext.Type.IDENTIFIER) {
+          // a single-column transform: a derived column of the resident segment (B200Transform), numeric by construction
+          if (!B200Transform.accepted(expression, segment)) {
+            return false;
+          }
+          continue;
+        }
+        if (!segment.getDataSource(expression.getIdentifier()).getDataSourceMetadata().isSingleValue()) {
           return false;
         }
         // MIN / MAX of a STRING column come back as dictIds, which DoubleAggregationResultHolder cannot carry: stock operator
@@ -86,8 +95,11 @@ public class B200PlanMaker extends InstancePlanMakerImplV2 {
     List<ExpressionContext> groupBy = queryContext.getGroupByExpressions();
     if (groupBy != null) {
       for (ExpressionContext expression : groupBy) {
-        if (expression.getType() != ExpressionContext.Type.IDENTIFIER
-            || segment.getDataSource(expression.getIdentifier()).getDictionary() == null) {
+        if (expression.getType() != ExpressionContext.Type.IDENTIFIER) {
+          if (!B200Transform.accepted(expression, segment)) {
+            return false;
+          }
+        } else if (segment.getDataSource(expression.getIdentifier()).getDictionary() == null) {
           return false;
         }
       }

@@ -40,6 +40,45 @@ public final class B200SegmentCache {
       }
       return -1;
     }
+
+    // Derived columns by the expression's canonical text (ExpressionContext.toString()): derived once per resident
+    // segment, on the first query that names the expression; a refusal is remembered so that later queries go to the
+    // stock operator without asking the device again
+    private final Map<String, B200Transform.Derived> _derived = new java.util.HashMap<>();
+    private final Set<String> _refused = new java.util.HashSet<>();
+
+    /** The derived column of `expression`, or null when the library refuses it (the caller runs the stock operator). */
+    public synchronized B200Transform.Derived derive(long ctx, org.apache.pinot.common.request.context.ExpressionContext expression) {
+      String key = expression.toString();
+      B200Transform.Derived d = _derived.get(key);
+      if (d != null || _refused.contains(key)) {
+        return d;
+      }
+      B200Transform.Program p;
+      try {
+        p = B200Transform.compile(expression);
+      } catch (IllegalArgumentException e) {
+        _refused.add(key);
+        return null;
+      }
+      int source = columnId(p._column);
+      int n = p._op.size();
+      int column = source < 0 ? -1 : B200Native.segmentDeriveColumn(ctx, _handle, source,
+          p._op.stream().mapToInt(Integer::intValue).toArray(), p._i.stream().mapToLong(Long::longValue).toArray(),
+          p._d.stream().mapToDouble(Double::doubleValue).toArray());
+      long[] info = new long[6];
+      if (column >= 0 && B200Native.segmentColumnInfo(_handle, column, info) != 0) {
+        column = -1;
+      }
+      byte[] dictionary = column < 0 ? null : B200Native.segmentDictionary(ctx, _handle, column);
+      if (column < 0 || dictionary == null || n == 0) {
+        _refused.add(key);
+        return null;
+      }
+      d = new B200Transform.Derived(column, (int) info[1], dictionary);
+      _derived.put(key, d);
+      return d;
+    }
   }
 
   private final long _ctx;

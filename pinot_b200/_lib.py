@@ -140,6 +140,10 @@ class HSelection(C.Structure):
 MAX_SELECT_LIMIT = 1_000_000
 
 
+class TransformOp(C.Structure):
+    _fields_ = [("op", C.c_int32), ("reserved", C.c_int32), ("i", C.c_int64), ("d", C.c_double)]
+
+
 class HStarMetric(C.Structure):
     _fields_ = [("function", C.c_int32), ("reserved", C.c_int32), ("column", C.c_char_p), ("fwd", C.c_void_p),
                 ("fwd_bytes", C.c_uint64)]
@@ -164,6 +168,7 @@ EXPORTED_SYMBOLS = [
     "pb200_execute_selection", "pb200_result_selection", "pb200h_execute_selection",
     "pb200_execute_distinct", "pb200h_execute_distinct",
     "pb200_execute_args", "pb200h_execute_args", "pb200_result_histogram",
+    "pb200_segment_derive_column", "pb200h_segment_derive",
 ]
 
 _LIB = None
@@ -261,6 +266,8 @@ def load() -> C.CDLL:
     L.pb200_segment_bind_domain.argtypes = [vp, vp, vp]
     L.pb200_segment_local_ids.restype = i64
     L.pb200_segment_local_ids.argtypes = [vp, i32, vp, i64]
+    L.pb200_segment_derive_column.argtypes = [vp, vp, i32, i32, C.POINTER(TransformOp), C.POINTER(i32)]
+    L.pb200h_segment_derive.argtypes = [vp, vp, C.c_char_p, C.POINTER(i32)]
     _LIB = L
     return L
 

@@ -33,6 +33,7 @@ struct HostColumn {
   int data_type = 0, has_dictionary = 0, bits = 0, cardinality = 0, is_sorted = 0, entry_bytes = 0;
   bool has_inverted = false;
   bool synthesized_dictionary = false;    // the segment stores this column raw: `dict` was built from its values at load (raw_forward.cpp)
+  bool derived = false;                   // a transform of a stored column (transform.cpp): `name` is its canonical text
   std::vector<unsigned char> dict;        // big-endian values or padded strings (host copy): the SEGMENT's own dictionary
   std::vector<unsigned char> sorted_idx;  // (start,end) BE pairs when is_sorted
   // Bound to a table-wide dictionary domain (pb200h_segment_bind_domain): predicates are still resolved against the
@@ -130,19 +131,48 @@ struct StarTreeIndex {
 };
 }  // namespace pb200h
 
+namespace pb200h {
+// transform.cpp: canonical text of a single-column expression (function names and their aliases to the canonical name,
+// time-unit literals in upper case, numeric literals by value); false when `text` is no expression
+bool normalize_expression(const char* text, std::string* canonical);
+// the canonical text, the postfix program (pb200_transform_op) and the column of an expression; PB200_E_* with a message
+int compile_expression(const char* text, std::string* canonical, std::vector<pb200_transform_op>* ops, std::string* column);
+}  // namespace pb200h
+
 struct pb200h_segment {
   pb200_ctx* ctx = nullptr;
   pb200_segment* dev = nullptr;
   std::string name;
   int num_docs = 0;
+  // Stored columns, then derived ones in the order they were derived (the same ids as in `dev`).  Room for
+  // PB200_MAX_DERIVED_COLUMNS more is reserved at creation: a derived column is appended complete, under derive_mu,
+  // without moving a column that a running query references.
+  // Readers bound column ids by num_columns(), never by cols.size(): the count is published with release only after
+  // the appended column is complete.
   std::vector<pb200h::HostColumn> cols;
+  int num_stored = 0;
+  std::atomic<int> published{-1};  // -1: a column list that never grows (cols.size())
+  std::mutex derive_mu;
+  int num_columns() const { const int p = published.load(std::memory_order_acquire); return p < 0 ? (int)cols.size() : p; }
   std::vector<std::unique_ptr<pb200h::StarTreeIndex>> star_trees;
+  // A stored column whose name is `n`, else the derived column of the expression `n` (any spelling), else -1
   int column_index(const char* n) const {
     if (!n) return -1;
-    for (size_t i = 0; i < cols.size(); i++) if (cols[i].name == n) return (int)i;
+    const int published_now = num_columns();
+    for (int i = 0; i < published_now; i++) if (cols[i].name == n) return i;
+    std::string canonical;
+    if (published_now == num_stored || !strchr(n, '(') || !pb200h::normalize_expression(n, &canonical)) return -1;
+    for (int i = num_stored; i < published_now; i++) if (cols[i].name == canonical) return i;
     return -1;
   }
 };
+
+namespace pb200h {
+// transform.cpp: resolves every name that is no column of a segment as an expression and derives it there once
+// (pb200h_segment_derive); afterwards every name is at one position in all segments (else PB200_E_UNSUPPORTED)
+int derive_names(pb200_ctx* ctx, pb200h_segment* const* segs, int nseg, const std::vector<const char*>& names);
+int derive_query_names(pb200_ctx* ctx, const pb200h_query& q, pb200h_segment* const* segs, int nseg, const char* const* extra, int nextra);
+}  // namespace pb200h
 
 namespace pb200h {
 // raw_forward.cpp: no-dictionary fixed-width SV forward indexes at load time

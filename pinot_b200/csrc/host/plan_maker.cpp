@@ -209,6 +209,9 @@ bool non_scan_answerable(const pb200h_segment& seg, const pb200h_query& q) {
     if (ag.function != PB200_AGG_MIN && ag.function != PB200_AGG_MAX && ag.function != PB200_AGG_DISTINCTCOUNT) return false;
     int ci = seg.column_index(ag.column);
     if (ci < 0 || !seg.cols[ci].has_dictionary) return false;
+    // a derived column's dictionary may hold values absent from the segment (derived over a domain), and the reference
+    // takes this shortcut for identifiers only
+    if (seg.cols[ci].derived) return false;
     if (ag.function != PB200_AGG_DISTINCTCOUNT && seg.cols[ci].data_type == PB200_STRING) return false;
   }
   return true;
@@ -300,6 +303,8 @@ extern "C" int32_t pb200h_segment_create(pb200_ctx* ctx, const char* name, int32
   if (!ctx || !cols || !out || ncols <= 0) { set_error("invalid argument to pb200h_segment_create"); return PB200_E_INVALID; }
   std::unique_ptr<pb200h_segment> seg(new pb200h_segment());
   seg->ctx = ctx; seg->name = name ? name : ""; seg->num_docs = num_docs;
+  seg->cols.reserve((size_t)ncols + PB200_MAX_DERIVED_COLUMNS);
+  seg->num_stored = ncols;
   std::vector<pb200_col_desc> descs(ncols);
   // Raw (no-dictionary) columns: all chunks are decoded once here; a column with at most PB200_RAW_DICT_MAX (default 2^20)
   // distinct values is dictionary-encoded on the fly and is an ordinary dictionary column from here on (raw_forward.cpp)
@@ -350,6 +355,7 @@ extern "C" int32_t pb200h_segment_create(pb200_ctx* ctx, const char* name, int32
   }
   int rc = pb200_segment_register(ctx, name, num_docs, ncols, descs.data(), &seg->dev);
   if (rc) return rc;
+  seg->published.store(ncols, std::memory_order_release);
   *out = seg.release();
   return PB200_OK;
 }
@@ -359,6 +365,8 @@ extern "C" int32_t pb200h_segment_adopt(pb200_ctx* ctx, pb200_segment* dev, int3
   if (!ctx || !dev || !out || !names) { set_error("invalid argument to pb200h_segment_adopt"); return PB200_E_INVALID; }
   std::unique_ptr<pb200h_segment> seg(new pb200h_segment());
   seg->ctx = ctx; seg->dev = dev; seg->num_docs = num_docs;
+  seg->cols.reserve((size_t)ncols + PB200_MAX_DERIVED_COLUMNS);
+  seg->num_stored = ncols;
   for (int i = 0; i < ncols; i++) {
     int64_t info[6];
     int rc = pb200_segment_column_info(dev, i, info);
@@ -372,6 +380,7 @@ extern "C" int32_t pb200h_segment_adopt(pb200_ctx* ctx, pb200_segment* dev, int3
     if (n > 0) { h.dict.resize(n); pb200_segment_read_index(ctx, dev, i, 1, h.dict.data(), n); }
     seg->cols.push_back(std::move(h));
   }
+  seg->published.store(ncols, std::memory_order_release);
   *out = seg.release();
   return PB200_OK;
 }
@@ -384,13 +393,13 @@ extern "C" int32_t pb200h_segment_destroy(pb200h_segment* seg) {
 }
 extern "C" pb200_segment* pb200h_segment_device(pb200h_segment* seg) { return seg ? seg->dev : nullptr; }
 extern "C" int32_t pb200h_segment_num_docs(const pb200h_segment* seg) { return seg ? seg->num_docs : -1; }
-extern "C" int32_t pb200h_segment_num_columns(const pb200h_segment* seg) { return seg ? (int)seg->cols.size() : -1; }
+extern "C" int32_t pb200h_segment_num_columns(const pb200h_segment* seg) { return seg ? seg->num_stored : -1; }  // stored columns only
 extern "C" int32_t pb200h_segment_column_index(const pb200h_segment* seg, const char* name) { return seg ? seg->column_index(name) : -1; }
 extern "C" const char* pb200h_segment_column_name(const pb200h_segment* seg, int32_t c) {
-  return (seg && c >= 0 && c < (int)seg->cols.size()) ? seg->cols[c].name.c_str() : nullptr;
+  return (seg && c >= 0 && c < seg->num_columns()) ? seg->cols[c].name.c_str() : nullptr;
 }
 extern "C" int32_t pb200h_segment_column_info(const pb200h_segment* seg, int32_t c, int32_t out[6]) {
-  if (!seg || c < 0 || c >= (int)seg->cols.size()) { set_error("bad column"); return PB200_E_INVALID; }
+  if (!seg || c < 0 || c >= seg->num_columns()) { set_error("bad column"); return PB200_E_INVALID; }
   const HostColumn& h = seg->cols[c];
   const HostColumn& g = h.decode_column();  // bound column: the id space results come back in is the domain's
   out[0] = h.data_type; out[1] = h.has_dictionary; out[2] = g.bits; out[3] = g.cardinality; out[4] = h.is_sorted; out[5] = h.has_inverted;
@@ -398,7 +407,7 @@ extern "C" int32_t pb200h_segment_column_info(const pb200h_segment* seg, int32_t
 }
 extern "C" int32_t pb200h_dictionary_get(const pb200h_segment* seg, int32_t c, int32_t id, double* num, int64_t* lng,
                                          char* str, int32_t cap) {
-  if (!seg || c < 0 || c >= (int)seg->cols.size()) { set_error("bad column"); return PB200_E_INVALID; }
+  if (!seg || c < 0 || c >= seg->num_columns()) { set_error("bad column"); return PB200_E_INVALID; }
   const HostColumn& h = seg->cols[c].decode_column();
   if (id < 0 || id >= h.cardinality || h.dict.empty()) { set_error("dictId %d out of range", id); return PB200_E_INVALID; }
   if (h.data_type == PB200_STRING) {
@@ -417,6 +426,7 @@ extern "C" int32_t pb200h_domain_build(pb200_ctx* ctx, pb200h_segment* const* se
   if (!ctx || !segs || !names || !out || nseg <= 0 || ncols <= 0) { set_error("invalid argument to pb200h_domain_build"); return PB200_E_INVALID; }
   std::vector<int32_t> cols(ncols);
   std::vector<pb200_segment*> dev(nseg);
+  if (int rc = derive_names(ctx, segs, nseg, std::vector<const char*>(names, names + ncols))) return rc;
   for (int k = 0; k < ncols; k++) {
     cols[k] = segs[0]->column_index(names[k]);
     if (cols[k] < 0) { set_error("unknown column '%s'", names[k] ? names[k] : "(null)"); return PB200_E_INVALID; }
@@ -652,6 +662,10 @@ extern "C" int32_t pb200h_segment_load_dir(pb200_ctx* ctx, const char* path, pb2
 // ------------------------------------------------------------------------------------------------------------------
 extern "C" int32_t pb200h_explain(pb200_ctx* ctx, const pb200h_query* q, pb200h_segment* seg, char* out, int32_t cap) {
   if (!q || !seg || !out || cap <= 0) { set_error("null argument"); return PB200_E_INVALID; }
+  if (ctx) {
+    pb200h_segment* one = seg;
+    if (int rc = derive_query_names(ctx, *q, &one, 1, nullptr, 0)) return rc;
+  }
   SegmentFilter f;
   std::string text;
   int rc = build_segment_filter(*seg, *q, f, &text);
@@ -681,6 +695,7 @@ extern "C" int32_t pb200h_execute_args(pb200_ctx* ctx, const pb200h_query* q, co
   if (q->num_aggs <= 0) { set_error("selection queries are outside this path"); return PB200_E_UNSUPPORTED; }
   if (int vrc = pb200::order_validate(order, q->num_aggs, q->num_group_by)) return vrc;
   if (q->num_group_by == 0) order = nullptr;  // aggregation only: one row, nothing to order
+  if (int rc = derive_query_names(ctx, *q, segs, nseg, nullptr, 0)) return rc;  // expressions become derived columns once
   bool any_clause = false;   // some aggregation has a FILTER (WHERE ...) clause
   if (q->agg_filter_count && q->agg_filter_start && q->agg_filter_nodes)
     for (int a = 0; a < q->num_aggs; a++) any_clause |= q->agg_filter_count[a] > 0;
@@ -723,7 +738,7 @@ extern "C" int32_t pb200h_execute_args(pb200_ctx* ctx, const pb200h_query* q, co
   std::vector<SegmentFilter> filters(nseg);
   std::vector<int> kind(nseg, q->num_group_by > 0 ? PB200H_OP_GROUP_BY : PB200H_OP_AGGREGATION);
   for (int s = 0; s < nseg; s++) {
-    if (segs[s]->cols.size() != s0.cols.size()) { set_error("segments do not share a schema"); return PB200_E_INVALID; }
+    if (segs[s]->num_stored != s0.num_stored) { set_error("segments do not share a schema"); return PB200_E_INVALID; }
     // group-by / aggregation columns were resolved by name against segment 0: every segment must hold the same column
     // (name, type, dictionary-encoded or not) at that position
     auto same_column = [&](int idx) {
@@ -814,6 +829,13 @@ using RowsDeviceCall = int32_t (*)(pb200_ctx*, const pb200_query*, const pb200_s
 int32_t execute_rows(pb200_ctx* ctx, const pb200h_query* q, const pb200h_selection* sel, pb200h_segment* const* segs, int32_t nseg,
                      pb200_result** results, RowsDeviceCall device) {
   if (sel->num_columns < 0 || (sel->num_columns > 0 && !sel->columns)) { set_error("selection: bad column list"); return PB200_E_INVALID; }
+  {
+    std::vector<const char*> extra(sel->columns, sel->columns + sel->num_columns);
+    for (int k = 0; k < sel->num_order_items && k < PB200_MAX_ORDER_BY; k++) extra.push_back(sel->order[k].column);
+    pb200h_query fq = *q;  // the filter part only: the group-by and aggregation fields are ignored here
+    fq.num_group_by = 0; fq.num_aggs = 0; fq.agg_filter_count = nullptr;
+    if (int rc = derive_query_names(ctx, fq, segs, nseg, extra.data(), (int)extra.size())) return rc;
+  }
   const pb200h_segment& s0 = *segs[0];
   std::vector<int32_t> cols(sel->num_columns);
   for (int k = 0; k < sel->num_columns; k++) {
@@ -838,7 +860,7 @@ int32_t execute_rows(pb200_ctx* ctx, const pb200h_query* q, const pb200h_selecti
   std::vector<SegmentFilter> filters(nseg);
   std::vector<int> dev_idx;
   for (int s = 0; s < nseg; s++) {
-    if (segs[s]->cols.size() != s0.cols.size()) { set_error("segments do not share a schema"); return PB200_E_INVALID; }
+    if (segs[s]->num_stored != s0.num_stored) { set_error("segments do not share a schema"); return PB200_E_INVALID; }
     for (int k = 0; k < sel->num_columns; k++) {
       const HostColumn &a = s0.cols[cols[k]], &b = segs[s]->cols[cols[k]];
       if (a.name != b.name || a.data_type != b.data_type) { set_error("segment %d: column '%s' is not at the position it has in segment 0", s, sel->columns[k]); return PB200_E_INVALID; }

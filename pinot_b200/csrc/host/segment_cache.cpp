@@ -49,8 +49,17 @@ void drop(pb200h_cache* c, std::list<pb200h_cache::Entry>::iterator it) {  // ca
   pb200h_segment_destroy(it->seg);
   c->entries.erase(it);
 }
+// a segment grows when queries derive columns on it (host/transform.cpp): the resident bytes follow (caller holds mu)
+void refresh_bytes(pb200h_cache* c) {
+  for (auto& e : c->entries) {
+    const int64_t now = pb200_segment_device_bytes(pb200h_segment_device(e.seg));
+    c->resident_bytes += now - e.bytes;
+    e.bytes = now;
+  }
+}
 // frees least-recently-used unpinned segments until `need` more bytes fit the budget; false if they cannot
 bool make_room(pb200h_cache* c, int64_t need) {
+  refresh_bytes(c);
   while (c->resident_bytes + need > c->budget) {
     auto victim = c->entries.end();
     for (auto it = c->entries.begin(); it != c->entries.end(); ++it)
@@ -142,6 +151,7 @@ extern "C" int32_t pb200h_cache_evict(pb200h_cache* c, const char* name, uint64_
 extern "C" int32_t pb200h_cache_stats(pb200h_cache* c, int64_t out[6]) {
   if (!c || !out) { set_error("null argument"); return PB200_E_INVALID; }
   std::lock_guard<std::mutex> g(c->mu);
+  refresh_bytes(c);
   out[0] = (int64_t)c->entries.size(); out[1] = c->resident_bytes; out[2] = c->budget;
   out[3] = c->hits; out[4] = c->misses; out[5] = c->evictions;
   return PB200_OK;

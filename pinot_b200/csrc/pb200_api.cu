@@ -166,12 +166,6 @@ static cudaError_t fwd_words_to_native(void* p, size_t bytes, int sm_count, cuda
   return cudaGetLastError();
 }
 
-static uint64_t padded_fwd_bytes(long long num_docs, int bits) {
-  // whole tiles for ANY tile size <= kMaxTileRows: ceil(N/t)*t < N + t <= alloc rows
-  long long tiles = (num_docs + kMaxTileRows - 1) / kMaxTileRows + 1;
-  return (uint64_t)tiles * kMaxTileRows / 8 * bits + 64;
-}
-
 // ------------------------------------------------------------------------------------------------------------------
 // small kernels
 // ------------------------------------------------------------------------------------------------------------------
@@ -430,7 +424,10 @@ extern "C" int32_t pb200_segment_register(pb200_ctx* ctx, const char* name, int3
   seg->ctx = ctx;
   seg->name = name ? name : "";
   seg->num_docs = num_docs;
+  seg->cols.reserve((size_t)ncols + PB200_MAX_DERIVED_COLUMNS);  // derived columns append without moving these
   seg->cols.resize(ncols);
+  seg->num_stored = ncols;
+  seg->published.store(ncols, std::memory_order_release);
   auto fail = [&](int rc) { for (auto& c : seg->cols) free_column(ctx, c); return rc; };
   for (int i = 0; i < ncols; i++) {
     const pb200_col_desc& d = cols[i];
@@ -577,7 +574,7 @@ extern "C" int32_t pb200_segment_release(pb200_ctx* ctx, pb200_segment* seg) {
 extern "C" int64_t pb200_segment_device_bytes(const pb200_segment* seg) { return seg ? seg->device_bytes : 0; }
 
 extern "C" int32_t pb200_segment_column_info(const pb200_segment* seg, int32_t col, int64_t out[6]) {
-  if (!seg || col < 0 || col >= (int)seg->cols.size()) { set_error("bad column"); return PB200_E_INVALID; }
+  if (!seg || col < 0 || col >= seg->num_columns()) { set_error("bad column"); return PB200_E_INVALID; }
   const DeviceColumn& c = seg->cols[col];
   out[0] = c.fwd_kind; out[1] = c.stored_type; out[2] = c.bits; out[3] = c.cardinality; out[4] = c.inv != nullptr;
   out[5] = (int64_t)c.fwd_file_bytes;
@@ -586,7 +583,7 @@ extern "C" int32_t pb200_segment_column_info(const pb200_segment* seg, int32_t c
 
 extern "C" int64_t pb200_segment_read_index(pb200_ctx* ctx, const pb200_segment* seg, int32_t col, int32_t which,
                                             void* out, uint64_t cap) {
-  if (!seg || col < 0 || col >= (int)seg->cols.size()) { set_error("bad column"); return PB200_E_INVALID; }
+  if (!seg || col < 0 || col >= seg->num_columns()) { set_error("bad column"); return PB200_E_INVALID; }
   const DeviceColumn& c = seg->cols[col];
   cudaSetDevice(seg->ctx->device);
   if (which == 0) {

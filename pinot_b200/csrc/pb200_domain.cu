@@ -100,12 +100,22 @@ __global__ void reencode_kernel(const uint32_t* __restrict__ src, int sb, uint32
   }
 }
 
-uint64_t padded_bytes(long long num_docs, int bits) {  // same rule as pb200_api.cu padded_fwd_bytes
+}  // namespace
+
+uint64_t padded_fwd_bytes(long long num_docs, int bits) {
+  // whole tiles for ANY tile size <= kMaxTileRows: ceil(N/t)*t < N + t <= alloc rows
   long long tiles = (num_docs + kMaxTileRows - 1) / kMaxTileRows + 1;
   return (uint64_t)tiles * kMaxTileRows / 8 * bits + 64;
 }
 
-}  // namespace
+cudaError_t reencode_column(pb200_ctx* ctx, cudaStream_t st, const uint32_t* src, int sb, uint32_t* dst, int db,
+                            const uint32_t* remap, uint32_t card, long long num_docs) {
+  const long long groups = (num_docs + 31) / 32;
+  if (groups <= 0) return cudaSuccess;
+  const int blocks = (int)std::min<long long>((groups + 255) / 256, (long long)ctx->sm_count * 16);
+  reencode_kernel<<<blocks, 256, 0, st>>>(src, sb, dst, db, remap, card, num_docs, groups);
+  return cudaGetLastError();
+}
 }  // namespace pb200
 
 using namespace pb200;
@@ -203,7 +213,7 @@ extern "C" int32_t pb200_domain_from_segments(pb200_ctx* ctx, pb200_segment* con
   std::vector<std::vector<int32_t>> cards(ncols), widths(ncols);
   for (int k = 0; k < ncols; k++) {
     for (int s = 0; s < nseg; s++) {
-      if (!segs[s] || columns[k] < 0 || columns[k] >= (int)segs[s]->cols.size()) { set_error("segment %d has no column %d", s, columns[k]); return PB200_E_INVALID; }
+      if (!segs[s] || columns[k] < 0 || columns[k] >= segs[s]->num_columns()) { set_error("segment %d has no column %d", s, columns[k]); return PB200_E_INVALID; }
       const DeviceColumn& c = segs[s]->cols[columns[k]];
       if (c.dict_be.empty()) { set_error("segment %d column %d was registered without dictionary bytes", s, columns[k]); return PB200_E_INVALID; }
       if (c.stored_type != segs[0]->cols[columns[k]].stored_type) { set_error("column %d changes type between segments", columns[k]); return PB200_E_INVALID; }
@@ -263,7 +273,7 @@ extern "C" int32_t pb200_segment_bind_domain(pb200_ctx* ctx, pb200_segment* seg,
   struct Work { int col; const pb200_domain::Col* dc; std::vector<uint32_t> remap; };
   std::vector<Work> work;
   for (const auto& dc : dom->cols) {
-    if (dc.column >= (int)seg->cols.size()) { set_error("domain column %d is outside segment '%s'", dc.column, seg->name.c_str()); return PB200_E_INVALID; }
+    if (dc.column >= seg->num_columns()) { set_error("domain column %d is outside segment '%s'", dc.column, seg->name.c_str()); return PB200_E_INVALID; }
     const DeviceColumn& c = seg->cols[dc.column];
     if (c.fwd_kind != PB200_FWD_DICT_FIXEDBIT || c.bits > 31) { set_error("column %d is not dictionary-encoded: it cannot join a domain", dc.column); return PB200_E_INVALID; }
     if (c.dict_be.empty()) { set_error("column %d was registered without dictionary bytes", dc.column); return PB200_E_INVALID; }
@@ -302,18 +312,13 @@ extern "C" int32_t pb200_segment_bind_domain(pb200_ctx* ctx, pb200_segment* seg,
       void* nf = nullptr;
       int rc = dev_alloc(ctx, std::max<size_t>(w.remap.size() * 4, 16), &remap_dev);
       if (rc) return rc;
-      const uint64_t nbytes = padded_bytes(seg->num_docs, dc.bits);
+      const uint64_t nbytes = padded_fwd_bytes(seg->num_docs, dc.bits);
       rc = dev_alloc(ctx, nbytes, &nf);
       if (rc) { dev_free(ctx, remap_dev); return rc; }
-      const long long groups = ((long long)seg->num_docs + 31) / 32;
       cudaError_t e = cudaMemcpyAsync(remap_dev, w.remap.data(), w.remap.size() * 4, cudaMemcpyHostToDevice, st);
       if (e == cudaSuccess) e = cudaMemsetAsync(nf, 0, nbytes, st);
-      if (e == cudaSuccess && groups > 0) {
-        const int blocks = (int)std::min<long long>((groups + 255) / 256, (long long)ctx->sm_count * 16);
-        reencode_kernel<<<blocks, 256, 0, st>>>(c.fwd, c.bits, (uint32_t*)nf, dc.bits, (const uint32_t*)remap_dev,
-                                                (uint32_t)c.cardinality, seg->num_docs, groups);
-        e = cudaGetLastError();
-      }
+      if (e == cudaSuccess)
+        e = reencode_column(ctx, st, c.fwd, c.bits, (uint32_t*)nf, dc.bits, (const uint32_t*)remap_dev, (uint32_t)c.cardinality, seg->num_docs);
       if (e == cudaSuccess) e = cudaStreamSynchronize(st);
       dev_free(ctx, remap_dev);
       if (e != cudaSuccess) { dev_free(ctx, nf); set_error("re-encoding column %d failed: %s", w.col, cudaGetErrorString(e)); return PB200_E_CUDA; }
@@ -357,7 +362,7 @@ extern "C" int32_t pb200_segment_bind_domain(pb200_ctx* ctx, pb200_segment* seg,
 }
 
 extern "C" int64_t pb200_segment_local_ids(const pb200_segment* seg, int32_t column, int32_t* out, int64_t cap) {
-  if (!seg || column < 0 || column >= (int)seg->cols.size()) { set_error("bad column"); return PB200_E_INVALID; }
+  if (!seg || column < 0 || column >= seg->num_columns()) { set_error("bad column"); return PB200_E_INVALID; }
   const DeviceColumn& c = seg->cols[column];
   if (c.local_ids.empty()) {  // unbound: every id of the dictionary occurs (Pinot dictionaries hold only present values)
     if (out) for (int64_t i = 0; i < c.cardinality && i < cap; i++) out[i] = (int32_t)i;

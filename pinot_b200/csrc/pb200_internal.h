@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <atomic>
 #include <cstdint>
 #include <map>
 #include <memory>
@@ -120,10 +121,31 @@ struct pb200_segment {
   pb200_ctx* ctx = nullptr;
   std::string name;
   int num_docs = 0;
+  // Registered columns, then derived ones (pb200_transform.cu).  Registration reserves room for
+  // PB200_MAX_DERIVED_COLUMNS more, so appending a derived column (under derive_mu) never moves a column that a
+  // running query references.  Readers bound their column ids by num_columns(), never by cols.size(): the count is
+  // published with release only after the appended column is complete.
   std::vector<pb200::DeviceColumn> cols;
+  int num_stored = 0;              // registered columns: segments of one table agree on these
+  std::atomic<int> published{-1};  // columns queries may read; -1: a column list that never grows (cols.size())
+  std::mutex derive_mu;
+  int num_columns() const { const int p = published.load(std::memory_order_acquire); return p < 0 ? (int)cols.size() : p; }
   int64_t device_bytes = 0;
   pb200_domain* domain = nullptr;  // holds one reference
 };
+
+namespace pb200 {
+// Columns every segment of a submission has (derived columns may have been added to some segments only); -1 when the
+// segments do not share their registered columns
+inline int common_columns(pb200_segment* const* segments, int nseg) {
+  int n = segments[0]->num_columns();
+  for (int s = 0; s < nseg; s++) {
+    if (!segments[s] || segments[s]->num_stored != segments[0]->num_stored) return -1;
+    n = std::min(n, segments[s]->num_columns());
+  }
+  return n;
+}
+}  // namespace pb200
 
 namespace pb200 {
 // A pinned (mapped) host block shared by the results whose extracted groups live in it; goes back to the context's pinned
@@ -260,6 +282,11 @@ int roaring_decode_batch(pb200_ctx* ctx, cudaStream_t stream, const std::vector<
 // pb200_domain.cu
 uint64_t dictionary_hash(int stored_type, int entry_bytes, int cardinality, const unsigned char* be);
 int bits_for_cardinality(int card);
+uint64_t padded_fwd_bytes(long long num_docs, int bits);  // allocation of a forward index (whole max tiles + slack)
+// Launches the re-encode of a fixed-bit column on `st`: value v of `src` (sb bits, card values) becomes remap[v] in `dst`
+// (db bits, zeroed by the caller); padding rows stay 0.
+cudaError_t reencode_column(pb200_ctx* ctx, cudaStream_t st, const uint32_t* src, int sb, uint32_t* dst, int db,
+                            const uint32_t* remap, uint32_t card, long long num_docs);
 // pb200_synth.cu
 int synth_build_inverted(pb200_ctx* ctx, cudaStream_t stream, DeviceColumn& col, long long num_docs);
 }  // namespace pb200

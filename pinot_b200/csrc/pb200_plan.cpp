@@ -84,10 +84,8 @@ int plan_scan(const Tuning& tune, DeviceLimits lim, const pb200_query* query, pb
   }
   if (nagg == 0) { set_error("at least one aggregation is required on this path"); return PB200_E_INVALID; }
   if (!segments[0]) { set_error("segment %d does not belong to this context / schema", 0); return PB200_E_INVALID; }
-  const int ncols = (int)segments[0]->cols.size();
-  for (int s = 0; s < nseg; s++) {
-    if (!segments[s] || (int)segments[s]->cols.size() != ncols) { set_error("segment %d does not belong to this context / schema", s); return PB200_E_INVALID; }
-  }
+  const int ncols = common_columns(segments, nseg);
+  if (ncols < 0) { set_error("the segments do not belong to this context / schema"); return PB200_E_INVALID; }
 
   if (merge && nseg > 1) {
     for (int g = 0; g < ngb; g++) {
@@ -814,7 +812,7 @@ int plan_selection(const Tuning& tune, DeviceLimits lim, const pb200_query* filt
   p.limit = sel->limit;
 
   // ---- selected and order columns: one value kind for all segments ----
-  const int ncols = (int)segments[0]->cols.size();
+  const int ncols = common_columns(segments, nseg);
   auto kind_of = [&](int c, const char* what, int* out_kind) -> int {
     if (c < 0 || c >= ncols) { set_error("%s column %d out of range", what, c); return PB200_E_INVALID; }
     int kind = -1;

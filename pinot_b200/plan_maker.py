@@ -172,6 +172,13 @@ class IndexSegment:
         be merged with the other bound segments on the device and across GPUs, by value."""
         _lib.check(self.ctx.lib.pb200h_segment_bind_domain(self.ctx.handle, self.handle, domain.handle))
 
+    def derive(self, expression: str) -> int:
+        """Derives the column of a single-column expression (pb200h_segment_derive; a no-op when it exists) and returns
+        its column id.  Queries derive the expressions they name by themselves; this does it ahead of them."""
+        col = C.c_int32()
+        _lib.check(self.ctx.lib.pb200h_segment_derive(self.ctx.handle, self.handle, expression.encode(), C.byref(col)))
+        return col.value
+
     def local_ids(self, column: str) -> np.ndarray:
         """Ids of `column` that occur in this segment (bound: domain ids; unbound: 0..cardinality-1)."""
         L = self.ctx.lib

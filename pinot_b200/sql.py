@@ -15,6 +15,12 @@ stays Java).  This module exists so the parity tests read like the reference's
     cond  := cond AND cond | cond OR cond | NOT cond | (cond) | col op literal | col BETWEEN a AND b
              | col [NOT] IN (literal, ...)
     op    := = | != | <> | < | <= | > | >=
+    col   := a column, or a single-column expression wherever a column is accepted (select list, GROUP BY, aggregation
+             arguments, the left-hand side of predicates, ORDER BY, selection and DISTINCT lists):
+             expr := term (+|- term)* ; term := factor (*|/|% factor)* ; factor := col | number | (expr) | fn(args)
+             fn in TRANSFORMS (DATETRUNC('DAY', ts), YEAR(ts), TIMECONVERT(ts, 'MILLISECONDS', 'HOURS'), FLOOR(x / 10), ...).
+             An expression is named by its canonical text (the reference's ExpressionContext.toString()):
+             ts / 1000 -> divide(ts,'1000'), DATE_TRUNC('day', ts) -> datetrunc('DAY',ts)
 """
 from __future__ import annotations
 
@@ -24,11 +30,36 @@ from typing import List, Optional
 
 from .query import Aggregation, Filter, FilterNode, Predicate, QueryContext, optimize_filter
 
-_TOKEN = re.compile(r"\s*(?:(\d+\.\d+(?:[eE][-+]?\d+)?|-?\d+\.\d+|-?\d+)|'((?:[^']|'')*)'|(<=|>=|<>|!=|[=<>(),*])|"
+_TOKEN = re.compile(r"\s*(?:(\d+\.\d+(?:[eE][-+]?\d+)?|-?\d+\.\d+|-?\d+)|'((?:[^']|'')*)'|(<=|>=|<>|!=|[=<>(),*+/%-])|"
                     r"([A-Za-z_$][A-Za-z0-9_$]*))")
 
 _FUNCTIONS = {"COUNT", "SUM", "MIN", "MAX", "AVG", "DISTINCTCOUNT", "PERCENTILE"}
 _PERCENTILE_N = re.compile(r"PERCENTILE(\d+)")
+
+# single-column transforms (DESIGN.md section 3.8): SQL name (lower case, no '_') -> canonical name
+TRANSFORMS = {n: n for n in (
+    "plus", "minus", "times", "divide", "mod", "floor", "ceil", "abs", "datetrunc", "year", "quarter", "month", "week",
+    "day", "dayofweek", "dayofyear", "hour", "minute", "second", "millisecond", "timeconvert",
+    *(f"toepoch{u}{k}" for u in ("seconds", "minutes", "hours", "days") for k in ("", "bucket", "rounded")))}
+TRANSFORMS.update(add="plus", sub="minus", mult="times", div="divide", weekofyear="week", dayofmonth="day",
+                  dow="dayofweek", doy="dayofyear")
+_DECIMAL = re.compile(r"[-+]?(?:\d+\.?\d*|\.\d+)(?:[eE][-+]?\d+)?")
+_INFIX = {"+": "plus", "-": "minus", "*": "times", "/": "divide", "%": "mod"}
+
+
+def _transform_name(name: str) -> Optional[str]:
+    return TRANSFORMS.get(name.lower().replace("_", ""))
+
+
+def _literal_text(v) -> str:
+    """A literal of canonical text: strings (time units, time zones) in upper case, numbers by value."""
+    if isinstance(v, str):
+        if not _DECIMAL.fullmatch(v):
+            return "'" + v.upper().replace("'", "''") + "'"
+        v = float(v) if any(ch in v for ch in ".eE") else int(v)   # a quoted number: by value, like an unquoted one
+    if isinstance(v, float) and v.is_integer() and abs(v) < 9.2e18 and not (v == 0 and str(v)[0] == "-"):  # -0.0 stays
+        v = int(v)
+    return f"'{v!r}'"
 
 
 def _is_function(name: str) -> bool:
@@ -100,7 +131,7 @@ class _Parser:
 
     def percentile_call(self, name: str):
         """After `name(`: the column and percentile of PERCENTILE(col, p) or PERCENTILE<n>(col), up to the `)`."""
-        col = self.ident()
+        col = self.column()
         m = _PERCENTILE_N.fullmatch(name.upper())
         if m:
             p = _percentile_arg(int(m.group(1)))
@@ -115,6 +146,59 @@ class _Parser:
             raise SqlError(f"expected identifier, got {self.peek()}")
         self.i += 1
         return v
+
+    # ---- single-column expressions: canonical text (a plain column stays its name) ---------------------------------
+    def column(self) -> str:
+        text, is_literal = self._additive()
+        if is_literal:
+            raise SqlError(f"expected a column or an expression, got the literal {text}")
+        return text
+
+    def _additive(self):
+        left = self._multiplicative()
+        while True:
+            k, v = self.peek()
+            if k == "op" and v in ("+", "-"):
+                self.i += 1
+                right = self._multiplicative()
+            elif k == "num" and v < 0 and not left[1]:   # `x -1` is tokenized as x, -1
+                self.i += 1
+                v, right = "-", (_literal_text(-v), True)
+            else:
+                return left
+            left = (f"{_INFIX[v]}({left[0]},{right[0]})", False)
+
+    def _multiplicative(self):
+        left = self._factor()
+        while True:
+            k, v = self.peek()
+            if k != "op" or v not in ("*", "/", "%"):
+                return left
+            self.i += 1
+            right = self._factor()
+            left = (f"{_INFIX[v]}({left[0]},{right[0]})", False)
+
+    def _factor(self):
+        k, v = self.peek()
+        if k in ("num", "str"):
+            self.i += 1
+            return _literal_text(v), True
+        if self.take_op("("):
+            inner = self._additive()
+            self.expect_op(")")
+            return inner
+        name = self.ident()
+        if self.peek() != ("op", "("):
+            return name, False
+        canonical = _transform_name(name)
+        if canonical is None:
+            raise SqlError(f"{name}(...) is not a single-column transform of this path")
+        self.i += 1
+        args = [] if self.peek() == ("op", ")") else [self._additive()]
+        while self.take_op(","):
+            args.append(self._additive())
+        self.expect_op(")")
+        return f"{canonical}({','.join(a[0] for a in args)})", False
 
     def literal(self):
         k, v = self.peek()
@@ -141,14 +225,21 @@ class _Parser:
     def not_(self) -> FilterNode:
         if self.take_kw("NOT"):
             return Filter("NOT", [self.not_()])
-        if self.take_op("("):
-            c = self.cond()
-            self.expect_op(")")
-            return c
+        if self.peek() == ("op", "("):
+            start = self.i
+            try:   # (cond), unless the parenthesis opens the expression on a comparison's left: `(x + 1) * 2 > 3`
+                self.i += 1
+                c = self.cond()
+                self.expect_op(")")
+                if self.peek()[0] != "op" or self.peek()[1] == ")":
+                    return c
+            except SqlError:
+                pass
+            self.i = start
         return self.comparison()
 
     def comparison(self) -> FilterNode:
-        col = self.ident()
+        col = self.column()
         if self.take_kw("BETWEEN"):
             lo = self.literal()
             self.expect_kw("AND")
@@ -193,9 +284,9 @@ def resolve_order_by(query: QueryContext) -> List[tuple]:
         if expr in query.group_by:
             out.append(("GROUP_BY", query.group_by.index(expr), asc))
             continue
-        m = re.fullmatch(r"([A-Za-z_$][A-Za-z0-9_$]*)\((\*|[A-Za-z_$][A-Za-z0-9_$]*)(?:,(.+))?\)", expr)
+        m = re.fullmatch(r"([A-Za-z_$][A-Za-z0-9_$]*)\((.+?)(?:,([-+0-9.eE]+))?\)", expr)
         found = None
-        if m:
+        if m and _is_function(m.group(1)):
             fn, col = m.group(1).upper(), m.group(2)
             arg = None if m.group(3) is None else float(m.group(3))
             for a, agg in enumerate(query.aggregations):
@@ -215,8 +306,9 @@ def parse(sql: str, **options) -> QueryContext:
     aggs: List[Aggregation] = []
     plain: List[str] = []
     while True:
-        name = p.ident()
-        if _is_function(name) and p.take_op("("):
+        k, name = p.peek()
+        if k == "id" and _is_function(name) and p.toks[p.i + 1:p.i + 2] == [("op", "(")]:
+            p.i += 2
             fn = name.upper()
             if fn.startswith("PERCENTILE"):
                 col, pct = p.percentile_call(name)
@@ -226,7 +318,7 @@ def parse(sql: str, **options) -> QueryContext:
                     raise SqlError(f"{fn}(*) is not valid")
                 aggs.append(Aggregation("COUNT", None))
             else:
-                col = p.ident()
+                col = p.column()
                 aggs.append(Aggregation("COUNT", None) if fn == "COUNT" else Aggregation(fn, col))
             p.expect_op(")")
             if p.take_kw("FILTER"):   # SUM(x) FILTER (WHERE cond)
@@ -235,7 +327,7 @@ def parse(sql: str, **options) -> QueryContext:
                 aggs[-1].filter = optimize_filter(p.cond())
                 p.expect_op(")")
         else:
-            plain.append(name)
+            plain.append(p.column())
         if not p.take_op(","):
             break
     p.expect_kw("FROM")
@@ -246,24 +338,26 @@ def parse(sql: str, **options) -> QueryContext:
     group_by: List[str] = []
     if p.take_kw("GROUP"):
         p.expect_kw("BY")
-        group_by.append(p.ident())
+        group_by.append(p.column())
         while p.take_op(","):
-            group_by.append(p.ident())
+            group_by.append(p.column())
     order_by = []
     if p.take_kw("ORDER"):
         p.expect_kw("BY")
         while True:
-            name = p.ident()
-            expr = name
-            if p.take_op("("):
-                if _is_function(name) and name.upper().startswith("PERCENTILE"):
+            k, name = p.peek()
+            if k == "id" and _is_function(name) and p.toks[p.i + 1:p.i + 2] == [("op", "(")]:
+                p.i += 2
+                if name.upper().startswith("PERCENTILE"):
                     inner, pct = p.percentile_call(name)
                     p.expect_op(")")
                     expr = f"percentile({inner},{pct!r})"
                 else:
-                    inner = "*" if p.take_op("*") else p.ident()
+                    inner = "*" if p.take_op("*") else p.column()
                     p.expect_op(")")
                     expr = f"{name.lower()}({inner})"
+            else:
+                expr = p.column()
             asc = True
             if p.take_kw("DESC"):
                 asc = False
@@ -321,10 +415,10 @@ def parse_selection(sql: str) -> SelectionQuery:
         columns = None
     else:
         while True:
-            name = p.ident()
-            if _is_function(name) and p.peek() == ("op", "("):
+            k, name = p.peek()
+            if k == "id" and _is_function(name) and p.toks[p.i + 1:p.i + 2] == [("op", "(")]:
                 raise SqlError(f"{name}(...) in a selection query: aggregations go through parse()")
-            columns.append(name)
+            columns.append(p.column())
             if not p.take_op(","):
                 break
     p.expect_kw("FROM")
@@ -338,7 +432,7 @@ def parse_selection(sql: str) -> SelectionQuery:
     if p.take_kw("ORDER"):
         p.expect_kw("BY")
         while True:
-            name = p.ident()
+            name = p.column()
             asc = not p.take_kw("DESC")
             if asc:
                 p.take_kw("ASC")
@@ -381,10 +475,10 @@ def parse_distinct(sql: str) -> DistinctQuery:
         raise SqlError("DISTINCT * is not supported: name the columns")
     columns: List[str] = []
     while True:
-        name = p.ident()
-        if p.peek() == ("op", "("):
-            raise SqlError(f"{name}(...) in a DISTINCT select list: functions and expressions are not supported")
-        columns.append(name)
+        k, name = p.peek()
+        if k == "id" and _is_function(name) and p.toks[p.i + 1:p.i + 2] == [("op", "(")]:
+            raise SqlError(f"{name}(...) in a DISTINCT select list: aggregations are not supported")
+        columns.append(p.column())
         if not p.take_op(","):
             break
     p.expect_kw("FROM")
@@ -398,7 +492,7 @@ def parse_distinct(sql: str) -> DistinctQuery:
     if p.take_kw("ORDER"):
         p.expect_kw("BY")
         while True:
-            name = p.ident()
+            name = p.column()
             if name not in columns:
                 raise SqlError(f"ORDER BY {name}: a DISTINCT query can only order by its selected columns")
             asc = not p.take_kw("DESC")
