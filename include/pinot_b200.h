@@ -185,9 +185,11 @@ typedef struct {
 #define PB200_NODE_IDS_ON_DEVICE 1
 
 /* Aggregation functions accelerated on this path (core/query/aggregation/function/{Count,Sum,Min,Max,Avg,
- * DistinctCount,Percentile}AggregationFunction.java).  PERCENTILE takes its percentile through pb200_execute_args. */
+ * DistinctCount,Percentile,Variance}AggregationFunction.java).  PERCENTILE takes its percentile through
+ * pb200_execute_args; the four VarianceAggregationFunction types take no argument (see pb200_result_moments). */
 enum { PB200_AGG_COUNT = 0, PB200_AGG_SUM = 1, PB200_AGG_MIN = 2, PB200_AGG_MAX = 3, PB200_AGG_AVG = 4,
-       PB200_AGG_DISTINCTCOUNT = 5, PB200_AGG_PERCENTILE = 6 };
+       PB200_AGG_DISTINCTCOUNT = 5, PB200_AGG_PERCENTILE = 6, PB200_AGG_VARPOP = 7, PB200_AGG_VARSAMP = 8,
+       PB200_AGG_STDDEVPOP = 9, PB200_AGG_STDDEVSAMP = 10 };
 
 typedef struct {
   int32_t function; /* PB200_AGG_* */
@@ -278,6 +280,26 @@ int32_t pb200_execute_args(pb200_ctx* ctx, const pb200_query* query, const pb200
  * the device on the first call for a result, so a caller that reads only the final values pays nothing for them. */
 int64_t pb200_result_histogram(const pb200_result* result, int32_t agg, int32_t row, int32_t* dict_ids, int64_t* counts,
                                int64_t capacity);
+
+/* ---- VAR_POP / VAR_SAMP / STDDEV_POP / STDDEV_SAMP: exact moments over limb dictionaries ------------------------------ */
+/* PB200_AGG_VARPOP / VARSAMP / STDDEVPOP / STDDEVSAMP through pb200_execute, pb200_execute_ordered or pb200_execute_args
+ * (no argument).  Semantics (VarianceAggregationFunction): over the n values of the column in the group's matched rows,
+ * M2 = sum (v - mean)^2, VARPOP = M2 / n, VARSAMP = M2 / (n - 1), STDDEV* = sqrt of the matching variance (a correctly
+ * rounded sqrt of that double); n == 0, and *SAMP with n == 1, give -inf.  The variance is computed EXACTLY and rounded
+ * once (the reference accumulates in double): every route and knob gives the same bits.
+ * A column qualifies when every value of its dictionary is c + k * 2^e with c the smallest value and k an integer in
+ * [0, 2^32): INT always; LONG when max - min < 2^32 (e = 0); FLOAT / DOUBLE on a common dyadic grid of that size (e.g.
+ * integral values or halves; 0.1-steps do not qualify).  Several of these functions over one column share one set of
+ * sums.  Results: pb200_result_agg gives the value (double column) and n (long column); ORDER BY compares the double.
+ * PB200_E_UNSUPPORTED (the caller runs the stock operator): STRING columns, raw columns streamed as 32-bit values,
+ * columns that do not qualify, a result over 2^32 docs or more, more than 6 aggregations after the expansion (each
+ * column adds 3 internal sums), PB200_Q_DEFER_FINALIZE; a PB200_Q_MERGE_SEGMENTS submission needs the column's
+ * dictionary to be the same in every segment.  NaN, +-inf and -0.0 are out of scope, as for MIN / MAX. */
+/* The exact intermediate behind aggregation `agg` in row `row`, for merging per-segment results by value: n values
+ * v_i = c + k_i * 2^e with c = c_mant * 2^c_exp exactly, s1 = sum k_i and s2 = s2_hi * 2^64 + s2_lo = sum k_i^2.
+ * Any output may be NULL.  PB200_E_INVALID when the aggregation is not one of the four functions. */
+int32_t pb200_result_moments(const pb200_result* result, int32_t agg, int32_t row, int64_t* n, int64_t* c_mant,
+                             int32_t* c_exp, int32_t* e, uint64_t* s1, uint64_t* s2_lo, uint64_t* s2_hi);
 
 /* ---- selection: SELECT columns WHERE ... [ORDER BY columns] LIMIT n (SelectionOnlyOperator, SelectionOrderByOperator) -- */
 /* Without order items: per segment, the first `limit` matching docs in doc-id order with the values of the selected

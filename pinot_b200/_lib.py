@@ -16,7 +16,9 @@ E_INVALID, E_UNSUPPORTED, E_CUDA, E_NOMEM, E_LIMIT = -1, -2, -3, -4, -5
 
 INT, LONG, FLOAT, DOUBLE, STRING = 0, 1, 2, 3, 4
 FWD_DICT_FIXEDBIT, FWD_DICT_SORTED, FWD_RAW_FIXEDBYTE = 0, 1, 2
-AGG_CODES = {"COUNT": 0, "SUM": 1, "MIN": 2, "MAX": 3, "AVG": 4, "DISTINCTCOUNT": 5, "PERCENTILE": 6}
+AGG_CODES = {"COUNT": 0, "SUM": 1, "MIN": 2, "MAX": 3, "AVG": 4, "DISTINCTCOUNT": 5, "PERCENTILE": 6,
+             "VARPOP": 7, "VARSAMP": 8, "STDDEVPOP": 9, "STDDEVSAMP": 10}
+MOMENT_FUNCTIONS = ("VARPOP", "VARSAMP", "STDDEVPOP", "STDDEVSAMP")
 FILTER_CODES = {"AND": 0, "OR": 1, "NOT": 2, "EQ": 3, "NEQ": 4, "IN": 5, "NOT_IN": 6, "RANGE": 7}
 REGIMES = {0: "NONE", 1: "ARRAY", 2: "INT_MAP", 3: "LONG_MAP", 4: "ARRAY_MAP"}
 OPERATOR_KINDS = {0: "AGGREGATION", 1: "GROUP_BY", 2: "NON_SCAN_AGGREGATION", 3: "EMPTY", 4: "STAR_TREE"}
@@ -167,7 +169,7 @@ EXPORTED_SYMBOLS = [
     "pb200_last_phases", "pb200_result_columns", "pb200_doc_mask_upload", "pb200_doc_mask_free", "pb200_roaring_validate", "pb200_comm_unique_id", "pb200_comm_init", "pb200_comm_shutdown", "pb200_result_combine",
     "pb200_execute_selection", "pb200_result_selection", "pb200h_execute_selection",
     "pb200_execute_distinct", "pb200h_execute_distinct",
-    "pb200_execute_args", "pb200h_execute_args", "pb200_result_histogram",
+    "pb200_execute_args", "pb200h_execute_args", "pb200_result_histogram", "pb200_result_moments",
     "pb200_segment_derive_column", "pb200h_segment_derive",
 ]
 
@@ -198,6 +200,7 @@ def load() -> C.CDLL:
                                      C.POINTER(vp)]
     L.pb200_result_histogram.restype = i64
     L.pb200_result_histogram.argtypes = [vp, i32, i32, vp, vp, i64]
+    L.pb200_result_moments.argtypes = [vp, i32, i32, vp, vp, vp, vp, vp, vp, vp]
     L.pb200_result_meta_get.argtypes = [vp, C.POINTER(ResultMeta)]
     L.pb200_result_group_keys.argtypes = [vp, vp]
     L.pb200_result_agg.argtypes = [vp, i32, vp, vp]

@@ -23,7 +23,10 @@ from typing import Dict, List
 def merge_blocks(query, segments, blocks) -> Dict[tuple, list]:
     """{key values: [intermediate per aggregation]} over all blocks: COUNT -> int, SUM / MIN / MAX -> float,
     AVG -> (sum, count), DISTINCTCOUNT -> set of values, PERCENTILE -> (p, {value: count}) from the per-segment
-    histograms, or its final float for a block merged on the device (GroupByCombineOperator / AggregationFunction.merge)."""
+    histograms, or its final float for a block merged on the device, VAR / STDDEV -> exact (n, sum v, sum v^2) from the
+    blocks' moments, each shifted from its own grid (c, e) to values, or the final float of a block merged on the device
+    (GroupByCombineOperator / AggregationFunction.merge)."""
+    from .query import MOMENT_FUNCTIONS, merge_moments
     out: Dict[tuple, list] = {}
     for seg, b in zip(segments, blocks):
         rows = 1 if b.num_groups < 0 else b.num_groups
@@ -45,6 +48,8 @@ def merge_blocks(query, segments, blocks) -> Dict[tuple, list]:
                         v = float(seg.dictionary_value(agg.column, int(d)))
                         hist[v] = hist.get(v, 0) + int(c)
                     vals.append((agg.arg, hist))
+                elif fn in MOMENT_FUNCTIONS and (a, g) in b.moments:
+                    vals.append(merge_moments([b.moments[(a, g)]]))
                 else:
                     vals.append(float(b.doubles[a][g]))
             cur = out.get(key)
@@ -64,6 +69,8 @@ def merge_blocks(query, segments, blocks) -> Dict[tuple, list]:
                 elif fn == "PERCENTILE" and isinstance(cur[a], tuple):
                     for v, c in vals[a][1].items():
                         cur[a][1][v] = cur[a][1].get(v, 0) + c
+                elif fn in MOMENT_FUNCTIONS and isinstance(cur[a], tuple):
+                    cur[a] = tuple(x + y for x, y in zip(cur[a], vals[a]))
                 else:
                     cur[a] |= vals[a]
     return out
@@ -82,7 +89,7 @@ def final_rows(query, table: Dict[tuple, list]) -> List[list]:
     DISTINCTCOUNT = set size) and breaks ties by the key values ascending, in GROUP BY column order -- the library's order.
     Without ORDER BY Pinot returns an arbitrary LIMIT-sized subset; here the rows are sorted by key to make the output
     stable."""
-    from .query import percentile_of_counts
+    from .query import MOMENT_FUNCTIONS, moments_final, percentile_of_counts
     from .sql import resolve_order_by
     items = resolve_order_by(query) if query.is_group_by else []
     rows = []
@@ -96,6 +103,8 @@ def final_rows(query, table: Dict[tuple, list]) -> List[list]:
                 vals.append(len(v))
             elif agg.function == "PERCENTILE" and isinstance(v, tuple):
                 vals.append(percentile_of_counts(v))
+            elif agg.function in MOMENT_FUNCTIONS and isinstance(v, tuple):
+                vals.append(moments_final(agg.function, v))
             else:
                 vals.append(v)
         rows.append(list(key) + vals)
@@ -134,7 +143,8 @@ def main(argv=None) -> int:
         try:
             if args.merge_on_device and len(segments) > 1:
                 cols = list(dict.fromkeys(list(query.group_by) + [a.column for a in query.aggregations
-                                                                  if a.column and a.function in ("MIN", "MAX", "DISTINCTCOUNT", "PERCENTILE")]))
+                                                                  if a.column and a.function in ("MIN", "MAX", "DISTINCTCOUNT", "PERCENTILE",
+                                                                                 "VARPOP", "VARSAMP", "STDDEVPOP", "STDDEVSAMP")]))
                 if cols:
                     domain = DictionaryDomain.build(ctx, segments, cols)
                     for s in segments:

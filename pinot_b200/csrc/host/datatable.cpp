@@ -80,6 +80,11 @@ extern "C" int64_t pb200h_result_to_datatable(const pb200h_query* q, const pb200
       set_error("PERCENTILE intermediates are not written as DataTable objects");
       return PB200_E_UNSUPPORTED;
     }
+  for (int a = 0; a < nagg; a++)
+    if (pb200::is_moments_fn(q->aggs[a].function)) {   // the reference's intermediate is a VarianceTuple
+      set_error("VAR/STDDEV intermediates are not written as DataTable objects");
+      return PB200_E_UNSUPPORTED;
+    }
   const size_t rows = meta.num_groups < 0 ? 1 : (size_t)meta.num_groups;
   // ---- intermediates through the C-ABI accessors ----
   std::vector<int32_t> keys(rows * (size_t)std::max(ngb, 1));

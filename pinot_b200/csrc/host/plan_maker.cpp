@@ -237,6 +237,8 @@ pb200_result* host_result(const pb200h_segment& seg, const pb200h_query& q, bool
       case PB200_AGG_MIN: if (empty) d = INFINITY; else { id = c->to_device_id(0); d = c->as_double(0); } break;
       case PB200_AGG_MAX: if (empty) d = -INFINITY; else { id = c->to_device_id(c->cardinality - 1); d = c->as_double(c->cardinality - 1); } break;
       case PB200_AGG_PERCENTILE: d = -INFINITY; break;   // only reached for an empty match (never answered without a scan)
+      case PB200_AGG_VARPOP: case PB200_AGG_VARSAMP: case PB200_AGG_STDDEVPOP: case PB200_AGG_STDDEVSAMP:
+        d = -INFINITY; R->mom.on[a] = true; break;       // likewise: n = 0, zero moments
       case PB200_AGG_DISTINCTCOUNT: {
         std::vector<int32_t> ids;
         if (!empty) for (int i = 0; i < c->cardinality; i++) ids.push_back(c->to_device_id(i));
@@ -711,6 +713,11 @@ extern "C" int32_t pb200h_execute_args(pb200_ctx* ctx, const pb200h_query* q, co
       return PB200_E_UNSUPPORTED;
     }
   }
+  for (int a = 0; a < q->num_aggs; a++)
+    if (pb200::is_moments_fn(q->aggs[a].function) && any_clause) {   // the per-clause submissions carry no moments
+      set_error("VAR/STDDEV in a query with FILTER (WHERE ...) clauses is not accelerated");
+      return PB200_E_UNSUPPORTED;
+    }
   if (q->agg_filter_count && q->agg_filter_start && q->agg_filter_nodes)
     for (int a = 0; a < q->num_aggs; a++)
       if (q->agg_filter_count[a] > 0) return execute_filtered(ctx, *q, order, segs, nseg, results, kinds);  // host/filtered_agg.cpp
@@ -732,6 +739,10 @@ extern "C" int32_t pb200h_execute_args(pb200_ctx* ctx, const pb200h_query* q, co
       if (aggs[a].column < 0) { set_error("unknown aggregation column '%s'", q->aggs[a].column ? q->aggs[a].column : "(null)"); return PB200_E_INVALID; }
       const HostColumn& c = s0.cols[aggs[a].column];
       if (c.data_type == PB200_STRING && q->aggs[a].function != PB200_AGG_DISTINCTCOUNT) { set_error("%s over STRING column", "aggregation"); return PB200_E_UNSUPPORTED; }
+      if (pb200::is_moments_fn(q->aggs[a].function) && !c.has_dictionary) {
+        set_error("VAR/STDDEV over raw column '%s' is not accelerated", q->aggs[a].column);
+        return PB200_E_UNSUPPORTED;
+      }
     }
   }
   // per-segment filters + plan shortcuts

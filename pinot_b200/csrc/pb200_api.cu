@@ -729,13 +729,15 @@ static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment*
 
   // ---- plan: every decision about the launch (pb200_plan.cpp) ----
   const Tuning tune = [&]() { std::lock_guard<std::mutex> g(ctx->mu); return ctx->tune; }();
+  if (int rc = moments_prepare(ctx, query, segments, nseg)) return rc;   // VAR / STDDEV limb dictionaries (pb200_moments.cu)
   ScanPlan plan;
   {
     const int rc = plan_scan(tune, DeviceLimits{ctx->sm_count, ctx->max_smem_optin}, query, segments, nseg, allow_count_carrier, &plan, agg_args);
     if (rc) return rc;
   }
   const QueryDesc& q = plan.q;
-  const int nagg = q.num_aggs, ngb = q.num_group_by, nres = plan.nres;
+  // nagg: the launch's aggregations, the internal VAR / STDDEV limb sums included; nuser: the caller's (the result's columns)
+  const int nagg = q.num_aggs, nuser = plan.num_user_aggs, ngb = q.num_group_by, nres = plan.nres;
   const bool merge = plan.merge;
 
   cudaStream_t st = take_stream(ctx);
@@ -834,7 +836,11 @@ static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment*
       d.stride = t.stride;
       d.live = true;
       d.num_groups_limit = query->num_groups_limit;
-      for (int a = 0; a < nagg; a++) { d.aggs.push_back(query->aggs[a]); d.val_kind.push_back(q.aggs[a].val_kind); d.agg_cols.push_back(q.aggs[a].slot < 0 ? nullptr : &seg->cols[query->aggs[a].column]); }
+      for (int a = 0; a < nuser; a++) { d.aggs.push_back(query->aggs[a]); d.val_kind.push_back(q.aggs[a].val_kind); d.agg_cols.push_back(q.aggs[a].slot < 0 ? nullptr : &seg->cols[query->aggs[a].column]); }
+      for (int a = 0; a < nuser; a++) {
+        d.mom_first[a] = plan.mom_first[a];
+        if (plan.mom_first[a] >= 0) d.mom_e[a] = seg->cols[query->aggs[a].column].moments->grid.e;
+      }
       d.pack_agg = t.carrier.agg; d.pack_shift = t.carrier.shift; d.pack_vmin = t.carrier.vmin;
       d.reduce_world = t.reduce_world;
       d.flag_slot = t.flag_slot;
@@ -1003,20 +1009,22 @@ static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment*
     long long total_docs = 0;
     if (merge) for (int s = 0; s < nseg; s++) total_docs += segments[s]->num_docs; else total_docs = segments[r]->num_docs;
     R.meta.num_group_by = ngb;
-    R.meta.num_aggs = nagg;
-    R.agg_functions.resize(nagg);
-    for (int a = 0; a < nagg; a++) R.agg_functions[a] = q.aggs[a].function;
+    R.meta.num_aggs = nuser;
+    R.agg_functions.resize(nuser);
+    for (int a = 0; a < nuser; a++) R.agg_functions[a] = q.aggs[a].function;
+    for (int a = 0; a < nuser; a++)
+      if (plan.mom_first[a] >= 0) { R.mom.on[a] = true; R.mom.grid[a] = segments[merge ? 0 : r]->cols[query->aggs[a].column].moments->grid; }
     R.meta.num_docs_scanned = (int64_t)acc.count;
     R.meta.num_entries_scanned_in_filter = plan.in_filter[r];
     R.meta.num_entries_scanned_post_filter = (int64_t)acc.count * plan.projected;
     R.meta.num_total_docs = total_docs;
     R.meta.device_ms = ms;
-    R.dbl.resize(nagg); R.lng.resize(nagg); R.ids.resize(nagg); R.distinct.resize(nagg);
+    R.dbl.resize(nuser); R.lng.resize(nuser); R.ids.resize(nuser); R.distinct.resize(nuser);
     if (!plan.group_by) {
       R.meta.num_groups = -1;
       R.meta.regime = PB200_REGIME_NONE;
       const pb200_segment* seg = segments[merge ? 0 : r];
-      for (int a = 0; a < nagg; a++) {
+      for (int a = 0; a < nuser; a++) {
         const int fn = q.aggs[a].function, vk = q.aggs[a].val_kind;
         double d = 0; int64_t l = 0; int32_t id = -1;
         const DeviceColumn* c = q.aggs[a].slot < 0 ? nullptr : &seg->cols[query->aggs[a].column];
@@ -1031,6 +1039,13 @@ static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment*
           }
         };
         if (fn == PB200_AGG_COUNT) { l = (int64_t)acc.count; d = (double)l; }
+        else if (is_moments_fn(fn)) {   // the exact moments from the limb sums (pb200_moments.h), rounded once
+          const int k0 = plan.mom_first[a];
+          const Moments m = moments_from_sums(acc.count, acc.isum[k0], acc.isum[k0 + 1], acc.isum[k0 + 2]);
+          d = moments_final(fn, m, R.mom.grid[a].e);
+          l = (int64_t)acc.count;
+          R.mom.one[a][0] = m.s1; R.mom.one[a][1] = (unsigned long long)m.s2; R.mom.one[a][2] = (unsigned long long)(m.s2 >> 64);
+        }
         else if (fn == PB200_AGG_SUM || fn == PB200_AGG_AVG) {
           d = sum_in_double(vk) ? acc.dsum[a] : (double)acc.isum[a];
           l = (int64_t)acc.count;
@@ -1064,7 +1079,7 @@ static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment*
   if (plan.group_by && order) for (int r = 0; r < nres; r++) res[r]->order = *order;  // a deferred result keeps it for its extraction
   const double t_results = now_ms();
   if (plan.group_by && plan.defer_finalize) {
-    for (int r = 0; r < nres; r++) { res[r]->meta.num_groups = 0; res[r]->dbl.assign(nagg, {}); res[r]->lng.assign(nagg, {}); res[r]->ids.assign(nagg, {}); res[r]->distinct.assign(nagg, {}); }
+    for (int r = 0; r < nres; r++) { res[r]->meta.num_groups = 0; res[r]->dbl.assign(nuser, {}); res[r]->lng.assign(nuser, {}); res[r]->ids.assign(nuser, {}); res[r]->distinct.assign(nuser, {}); }
   } else if (plan.group_by) {  // all results of the submission are extracted together (two device round trips in total)
     std::vector<pb200_result*> rs;
     for (int r = 0; r < nres; r++) rs.push_back(res[r].get());
@@ -1111,6 +1126,8 @@ extern "C" int32_t pb200_result_device_buffers(pb200_result* R, int32_t kind, vo
   if (!R || !p || !n) { set_error("null argument"); return PB200_E_INVALID; }
   pb200_result::Dense& d = R->dense;
   if (d.hkeys) { set_error("hash group tables of different GPUs are not element-wise reducible"); return PB200_E_UNSUPPORTED; }
+  for (int a = 0; a < kMaxAggs; a++)
+    if (R->mom.on[a]) { set_error("VAR/STDDEV moments are not combined across GPUs"); return PB200_E_UNSUPPORTED; }
   for (int a = 0; a < kMaxAggs; a++)
     if (R->pct.hist[a]) {
       set_error("PERCENTILE keeps dictId histograms on the device: a cross-GPU reduce of the tables would drop the other ranks' values");

@@ -136,6 +136,8 @@ static int combine_scalars(NcclApi* api, pb200_ctx* ctx, pb200_result* R, int ro
     if ((int)R->distinct.size() > a && !R->distinct[a].empty()) { set_error("DISTINCTCOUNT sets are merged on the host"); return PB200_E_UNSUPPORTED; }
   for (int a = 0; a < nagg; a++)
     if (R->pct.rep[a] >= 0) { set_error("PERCENTILE histograms are merged on the host"); return PB200_E_UNSUPPORTED; }
+  for (int a = 0; a < nagg; a++)
+    if (R->mom.on[a]) { set_error("VAR/STDDEV moments are merged on the host"); return PB200_E_UNSUPPORTED; }
   PB200_CUDA(cudaSetDevice(ctx->device));
   ncclComm_t comm = static_cast<ncclComm_t>(ctx->nccl_comm);
   cudaStream_t st = take_stream(ctx);

@@ -346,6 +346,8 @@ extern "C" int32_t pb200_segment_bind_domain(pb200_ctx* ctx, pb200_segment* seg,
     }
     // adopt the domain's dictionary (device copy shared by all bound segments)
     if (c.dict_native && !c.dict_shared) { seg->device_bytes -= (int64_t)c.dict_host.size(); dev_free(ctx, c.dict_native); }
+    if (!c.dict_shared && c.moments->limbs) seg->device_bytes -= 12ll * c.moments->entries;
+    c.moments = dc.moments;   // VAR / STDDEV limb dictionaries: one set per domain dictionary
     c.dict_native = dc.dict_native;
     c.dict_shared = true;
     c.dict_host = dc.dict_host;

@@ -65,6 +65,9 @@ struct ExtractDesc {
   const uint32_t* dbits[kMaxAggs];   // DISTINCTCOUNT per-group bitsets (an ORDER BY key is the popcount of a row)
   uint32_t dwords[kMaxAggs];
   const uint32_t* pct_n[kMaxAggs];   // PERCENTILE: values per table entry (src[a] holds the selected dictIds)
+  const long long* mom[kMaxAggs][3]; // VAR / STDDEV: the K, H, L limb sum tables (pb200_moments.h)
+  int32_t mom_e[kMaxAggs];           // ... and the grid exponent of the column
+  unsigned long long off_mom[kMaxAggs];  // ... {s1, s2 low, s2 high} per row, for pb200_result_moments
 };
 
 __device__ __forceinline__ bool non_empty(const ExtractDesc& d, long long i) {
@@ -166,6 +169,9 @@ __device__ __forceinline__ void agg_values(const ExtractDesc& d, int a, long lon
     lv = d.pct_n[a][g];
     if (x == ~0u) dv = -INFINITY;
     else { id = (int32_t)x; dv = dict_value(d, a, x); }
+  } else if (is_moments_fn(fn)) {  // exact moments from the group's limb sums and count, rounded once
+    dv = moments_final(fn, moments_from_sums(cnt, d.mom[a][0][g], d.mom[a][1][g], d.mom[a][2][g]), d.mom_e[a]);
+    lv = (long long)cnt;
   }
 }
 
@@ -191,6 +197,11 @@ __device__ __forceinline__ void write_row(const ExtractDesc& d, unsigned long lo
     if (d.off_dbl[a] != kNoCol) reinterpret_cast<double*>(out + d.off_dbl[a])[row] = dv;
     if (d.off_lng[a] != kNoCol) reinterpret_cast<long long*>(out + d.off_lng[a])[row] = lv;
     if (d.off_ids[a] != kNoCol) reinterpret_cast<int32_t*>(out + d.off_ids[a])[row] = id;
+    if (d.off_mom[a] != kNoCol) {
+      const Moments m = moments_from_sums(cnt, d.mom[a][0][g], d.mom[a][1][g], d.mom[a][2][g]);
+      unsigned long long* mp = reinterpret_cast<unsigned long long*>(out + d.off_mom[a]) + 3 * row;
+      mp[0] = m.s1; mp[1] = (unsigned long long)m.s2; mp[2] = (unsigned long long)(m.s2 >> 64);
+    }
   }
 }
 
@@ -307,8 +318,9 @@ static size_t layout_result(const pb200_result::Dense& d, ExtractDesc& e, size_t
     const int fn = e.fn[a];
     e.off_dbl[a] = take(8, rows);
     e.off_lng[a] = (fn == PB200_AGG_COUNT || fn == PB200_AGG_AVG || fn == PB200_AGG_SUM || fn == PB200_AGG_DISTINCTCOUNT ||
-                    fn == PB200_AGG_PERCENTILE) ? take(8, rows) : kNoCol;
+                    fn == PB200_AGG_PERCENTILE || is_moments_fn(fn)) ? take(8, rows) : kNoCol;
     e.off_ids[a] = (fn == PB200_AGG_MIN || fn == PB200_AGG_MAX || fn == PB200_AGG_PERCENTILE) ? take(4, rows) : kNoCol;
+    e.off_mom[a] = is_moments_fn(fn) ? take(24, rows) : kNoCol;
   }
   return off;
 }
@@ -378,6 +390,10 @@ int extract_groups(pb200_ctx* ctx, pb200_result* const* Rs, int nres, cudaStream
       else if (fn == PB200_AGG_MIN) e.src[a] = d.gmin[a];
       else if (fn == PB200_AGG_MAX) e.src[a] = d.gmax[a];
       else if (fn == PB200_AGG_PERCENTILE) { e.src[a] = Rs[r]->pct.ids[a]; e.pct_n[a] = Rs[r]->pct.n[Rs[r]->pct.rep[a]]; }
+      else if (is_moments_fn(fn)) {
+        for (int j = 0; j < 3; j++) e.mom[a][j] = d.isum[d.mom_first[a] + j];
+        e.mom_e[a] = d.mom_e[a];
+      }
       const DeviceColumn* c = d.agg_cols[a];
       e.dict[a] = (c && vk != VAL_RAW_I32 && !c->dict_host.empty()) ? c->dict_native : nullptr;
     }
@@ -510,6 +526,7 @@ int extract_groups(pb200_ctx* ctx, pb200_result* const* Rs, int nres, cudaStream
       v.dbl[a] = e.off_dbl[a] == kNoCol ? nullptr : reinterpret_cast<const double*>(out + e.off_dbl[a]);
       v.lng[a] = e.off_lng[a] == kNoCol ? nullptr : reinterpret_cast<const int64_t*>(out + e.off_lng[a]);
       v.ids[a] = e.off_ids[a] == kNoCol ? nullptr : reinterpret_cast<const int32_t*>(out + e.off_ids[a]);
+      R->mom.rows[a] = e.off_mom[a] == kNoCol ? nullptr : reinterpret_cast<const unsigned long long*>(out + e.off_mom[a]);
     }
     // DISTINCTCOUNT with GROUP BY: the groups' bitset rows are gathered on the device and decoded here into dictId lists
     // (what extractGroupByResult's value-set conversion starts from, BaseDistinctAggregateAggregationFunction :306-321)

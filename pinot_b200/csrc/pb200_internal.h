@@ -13,6 +13,7 @@
 
 #include "../../include/pinot_b200.h"
 #include "pb200_desc.h"
+#include "pb200_moments.h"
 
 namespace pb200 {
 
@@ -35,8 +36,23 @@ constexpr int kMaxTileRows = 8192;
 // words a device doc mask needs: whole tiles + one spare tile (the kernel reads masks tile-wise) + a tail
 inline size_t doc_mask_words(long long num_docs) { return (((size_t)num_docs + kMaxTileRows - 1) / kMaxTileRows + 1) * (kMaxTileRows / 32) + 8; }
 
+// Limb dictionaries of one device dictionary for VAR / STDDEV (pb200_moments.h, pb200_moments.cu): built on the first
+// query that needs them, under `mu`, and published with `ready` (release) before any launch reads them.  Shared by the
+// columns that share the dictionary (a domain's bound segments); freed with the last of them.
+struct MomentDict {
+  std::mutex mu;
+  std::atomic<bool> ready{false};  // evaluated: `eligible`, `grid` and (eligible) `limbs` are final
+  bool eligible = false;
+  MomentGrid grid{};
+  pb200_ctx* ctx = nullptr;
+  uint32_t* limbs = nullptr;       // device: K, H, L arrays of `entries` u32 each, one allocation
+  int entries = 0;
+  ~MomentDict();                   // pb200_moments.cu
+};
+
 struct DeviceColumn {
   int fwd_kind = 0, stored_type = 0, bits = 0, cardinality = 0;
+  std::shared_ptr<MomentDict> moments = std::make_shared<MomentDict>();  // replaced by the domain's when bound
   uint32_t* fwd = nullptr;        // packed words, padded to whole max tiles (+ slack)
   uint64_t fwd_file_bytes = 0;    // length of the original index file: ceil(N*bits/8)
   uint64_t fwd_alloc_bytes = 0;
@@ -112,6 +128,7 @@ struct pb200_domain {
     std::vector<unsigned char> dict_host;  // native little-endian values (numeric types)
     void* dict_native = nullptr;           // device copy (INT: biased), shared by every bound segment
     uint64_t hash = 0;
+    std::shared_ptr<pb200::MomentDict> moments = std::make_shared<pb200::MomentDict>();  // shared by every bound segment
   };
   std::vector<Col> cols;
   int refs = 1;  // the creator + one per bound segment (guarded by ctx->mu)
@@ -191,7 +208,14 @@ struct pb200_result {
     const uint32_t* row_entry = nullptr;         // group-by: table entry of each extracted row (inside view.block)
     std::vector<uint32_t> host[pb200::kMaxAggs]; // owners: histogram rows of the result's rows, copied on first use
   } pct;
-  pb200_order_by order{};                        // ORDER BY spec of a group-by result (num_items 0: none), applied at extraction
+  // VAR / STDDEV (pb200_moments.h): the grid of each such aggregation's dictionary and its exact moments per row
+  struct Mom {
+    bool on[pb200::kMaxAggs] = {};
+    pb200::MomentGrid grid[pb200::kMaxAggs] = {};
+    const unsigned long long* rows[pb200::kMaxAggs] = {};  // group-by: {s1, s2 low, s2 high} per row (inside view.block)
+    unsigned long long one[pb200::kMaxAggs][3] = {};        // aggregation only: the same for the one row
+  } mom;
+  pb200_order_by order{};                      // ORDER BY spec of a group-by result (num_items 0: none), applied at extraction
   std::vector<int32_t> agg_functions;            // PB200_AGG_* per aggregation (set by pb200_execute)
   std::vector<int32_t> keys;                     // [G x k]
   std::vector<std::vector<double>> dbl;          // per agg [rows]
@@ -222,6 +246,9 @@ struct pb200_result {
     uint32_t* gmax[pb200::kMaxAggs] = {};
     std::vector<uint32_t> mult;
     std::vector<unsigned long long> mult64;
+    int mom_first[pb200::kMaxAggs];             // VAR / STDDEV: the first of the three limb sums (isum) of aggregation a, -1 if none
+    int mom_e[pb200::kMaxAggs] = {};            // ... and the grid exponent of its column
+    Dense() { std::fill(mom_first, mom_first + pb200::kMaxAggs, -1); }
     uint32_t* dbits[pb200::kMaxAggs] = {};      // DISTINCTCOUNT with GROUP BY: per-group dictId bitsets, dwords[a] words each
     uint32_t dwords[pb200::kMaxAggs] = {};
     unsigned long long* hkeys = nullptr;        // hash table keys (NULL: dense table indexed by raw key)
@@ -287,6 +314,9 @@ uint64_t padded_fwd_bytes(long long num_docs, int bits);  // allocation of a for
 // (db bits, zeroed by the caller); padding rows stay 0.
 cudaError_t reencode_column(pb200_ctx* ctx, cudaStream_t st, const uint32_t* src, int sb, uint32_t* dst, int db,
                             const uint32_t* remap, uint32_t card, long long num_docs);
+// pb200_moments.cu: builds (once per device dictionary) the limb dictionaries of every VAR / STDDEV column of the query
+// that has dictIds, before it is planned; columns the planner refuses are skipped
+int moments_prepare(pb200_ctx* ctx, const pb200_query* query, pb200_segment* const* segments, int nseg);
 // pb200_synth.cu
 int synth_build_inverted(pb200_ctx* ctx, cudaStream_t stream, DeviceColumn& col, long long num_docs);
 }  // namespace pb200

@@ -77,12 +77,12 @@ int plan_scan(const Tuning& tune, DeviceLimits lim, const pb200_query* query, pb
   if (!query || !segments || !out || nseg <= 0) { set_error("invalid argument to pb200_execute"); return PB200_E_INVALID; }
   const bool per_seg_filter = query->flags & PB200_Q_PER_SEGMENT_FILTER;
   const bool merge = query->flags & PB200_Q_MERGE_SEGMENTS;
-  const int nnodes = query->num_filter_nodes, nagg = query->num_aggs, ngb = query->num_group_by;
-  if (nagg < 0 || nagg > kMaxAggs || ngb < 0 || ngb > kMaxGroupBy || nnodes < 0 || nnodes > kMaxNodes) {
-    set_error("query exceeds device limits (aggs %d/%d, group-by %d/%d, filter nodes %d/%d)", nagg, kMaxAggs, ngb, kMaxGroupBy, nnodes, kMaxNodes);
+  const int nnodes = query->num_filter_nodes, nuser = query->num_aggs, ngb = query->num_group_by;
+  if (nuser < 0 || nuser > kMaxAggs || ngb < 0 || ngb > kMaxGroupBy || nnodes < 0 || nnodes > kMaxNodes) {
+    set_error("query exceeds device limits (aggs %d/%d, group-by %d/%d, filter nodes %d/%d)", nuser, kMaxAggs, ngb, kMaxGroupBy, nnodes, kMaxNodes);
     return PB200_E_UNSUPPORTED;
   }
-  if (nagg == 0) { set_error("at least one aggregation is required on this path"); return PB200_E_INVALID; }
+  if (nuser == 0) { set_error("at least one aggregation is required on this path"); return PB200_E_INVALID; }
   if (!segments[0]) { set_error("segment %d does not belong to this context / schema", 0); return PB200_E_INVALID; }
   const int ncols = common_columns(segments, nseg);
   if (ncols < 0) { set_error("the segments do not belong to this context / schema"); return PB200_E_INVALID; }
@@ -92,19 +92,62 @@ int plan_scan(const Tuning& tune, DeviceLimits lim, const pb200_query* query, pb
       const int c = query->group_by_columns[g];
       if (c >= 0 && c < ncols && !same_dictionary(segments, nseg, c, "group-by")) return PB200_E_UNSUPPORTED;
     }
-    for (int a = 0; a < nagg; a++) {
+    for (int a = 0; a < nuser; a++) {
       const pb200_agg& ag = query->aggs[a];
       if (ag.function != PB200_AGG_MIN && ag.function != PB200_AGG_MAX && ag.function != PB200_AGG_DISTINCTCOUNT &&
-          ag.function != PB200_AGG_PERCENTILE) continue;
+          ag.function != PB200_AGG_PERCENTILE && !is_moments_fn(ag.function)) continue;
       if (ag.column < 0 || ag.column >= ncols) continue;
       if (segments[0]->cols[ag.column].bits == 32 && !segments[0]->cols[ag.column].dict_native) continue;  // raw values, no ids
-      const char* what = ag.function == PB200_AGG_DISTINCTCOUNT ? "DISTINCTCOUNT" : ag.function == PB200_AGG_PERCENTILE ? "PERCENTILE" : "MIN/MAX";
+      const char* what = ag.function == PB200_AGG_DISTINCTCOUNT ? "DISTINCTCOUNT" : ag.function == PB200_AGG_PERCENTILE ? "PERCENTILE"
+                         : is_moments_fn(ag.function) ? "VAR/STDDEV" : "MIN/MAX";
       if (!same_dictionary(segments, nseg, ag.column, what)) return PB200_E_UNSUPPORTED;
     }
   }
 
   ScanPlan& plan = *out;
   plan = ScanPlan();
+  // ---- VAR / STDDEV: each column's moments are three internal INT-dictionary SUMs over its limb dictionaries
+  //      (pb200_moments.h), appended behind the caller's aggregations; functions of one column share them ----
+  plan.num_user_aggs = nuser;
+  plan.aggs.assign(query->aggs, query->aggs + nuser);
+  plan.mom_first.assign(nuser, -1);
+  for (int a = 0; a < nuser; a++) {
+    const pb200_agg& ag = query->aggs[a];
+    if (!is_moments_fn(ag.function)) continue;
+    if (ag.column < 0 || ag.column >= ncols) { set_error("aggregation column %d out of range", ag.column); return PB200_E_INVALID; }
+    if (merge && (query->flags & PB200_Q_DEFER_FINALIZE)) { set_error("VAR/STDDEV moments are not reducible across GPUs (PB200_Q_DEFER_FINALIZE)"); return PB200_E_UNSUPPORTED; }
+    for (int t = 0; t < nseg; t++) {
+      const DeviceColumn& mc = segments[t]->cols[ag.column];
+      if (mc.stored_type == PB200_STRING) { set_error("VAR/STDDEV over STRING column %d", ag.column); return PB200_E_UNSUPPORTED; }
+      if (mc.bits > 31 || !mc.dict_native || mc.cardinality <= 0) {
+        set_error("VAR/STDDEV over column %d: no dictIds in segment %d (raw values): not accelerated", ag.column, t);
+        return PB200_E_UNSUPPORTED;
+      }
+      const MomentDict& md = *mc.moments;
+      if (!md.ready.load(std::memory_order_acquire)) { set_error("internal: limb dictionaries of column %d not prepared", ag.column); return PB200_E_INVALID; }
+      if (!md.eligible) {
+        set_error("VAR/STDDEV over column %d: its values in segment %d are not on a grid of 2^32 steps (c + k * 2^e): not accelerated", ag.column, t);
+        return PB200_E_UNSUPPORTED;
+      }
+    }
+    for (int b = 0; b < a && plan.mom_first[a] < 0; b++)
+      if (plan.mom_first[b] >= 0 && query->aggs[b].column == ag.column) plan.mom_first[a] = plan.mom_first[b];
+    if (plan.mom_first[a] >= 0) continue;
+    plan.mom_first[a] = (int)plan.aggs.size();
+    for (int j = 0; j < 3; j++) plan.aggs.push_back(pb200_agg{PB200_AGG_SUM, ag.column});
+  }
+  const int nagg = (int)plan.aggs.size();
+  if (nagg > kMaxAggs) {
+    set_error("VAR/STDDEV: %d aggregations with the internal moment sums (3 per column), at most %d", nagg, kMaxAggs);
+    return PB200_E_UNSUPPORTED;
+  }
+  plan.limb.assign(nagg, -1);
+  for (int a = 0; a < nuser; a++)
+    if (plan.mom_first[a] >= 0) for (int j = 0; j < 3; j++) plan.limb[plan.mom_first[a] + j] = j;
+  pb200_query expanded = *query;
+  expanded.aggs = plan.aggs.data();
+  expanded.num_aggs = nagg;
+  query = &expanded;
   QueryDesc& q = plan.q;
   plan.group_by = ngb > 0;
   plan.merge = merge;
@@ -150,7 +193,7 @@ int plan_scan(const Tuning& tune, DeviceLimits lim, const pb200_query* query, pb
     q.aggs[a].function = ag.function;
     q.aggs[a].slot = -1;
     q.aggs[a].val_kind = VAL_NONE;
-    if (ag.function == PB200_AGG_COUNT) continue;
+    if (ag.function == PB200_AGG_COUNT || is_moments_fn(ag.function)) continue;   // VAR / STDDEV: read their limb sums
     if (ag.function < 0 || ag.function > PB200_AGG_PERCENTILE) { set_error("unknown aggregation function %d", ag.function); return PB200_E_INVALID; }
     if (ag.column < 0 || ag.column >= ncols) { set_error("aggregation column %d out of range", ag.column); return PB200_E_INVALID; }
     if (ag.function == PB200_AGG_PERCENTILE) {
@@ -195,6 +238,7 @@ int plan_scan(const Tuning& tune, DeviceLimits lim, const pb200_query* query, pb
           vk = VAL_DICT_I32;
       }
     }
+    if (plan.limb[a] >= 0) vk = VAL_DICT_I32;   // limb words are read as biased INT dictionary values
     q.aggs[a].val_kind = vk;
   }
   q.num_slots = (int)plan.slot_cols.size();
@@ -260,6 +304,7 @@ int plan_scan(const Tuning& tune, DeviceLimits lim, const pb200_query* query, pb
       for (int a = 0; a < nagg; a++) {
         const int fn = q.aggs[a].function;
         if ((fn != PB200_AGG_SUM && fn != PB200_AGG_AVG) || q.aggs[a].val_kind != VAL_DICT_I32) continue;
+        if (plan.limb[a] >= 0) continue;   // the moments read limb sums as they are: never a carrier
         long long vmin = std::numeric_limits<long long>::max(), vmax = std::numeric_limits<long long>::min();
         bool ok = true;
         for (int s = 0; s < nseg && ok; s++) {
@@ -324,7 +369,7 @@ int plan_scan(const Tuning& tune, DeviceLimits lim, const pb200_query* query, pb
     int nsum = 0;
     for (int a = 0; a < nagg && ok; a++) {
       const int fn = q.aggs[a].function, vk = q.aggs[a].val_kind;
-      if (fn == PB200_AGG_COUNT) continue;
+      if (fn == PB200_AGG_COUNT || is_moments_fn(fn)) continue;   // VAR / STDDEV: the count and their limb sums
       if ((fn == PB200_AGG_SUM || fn == PB200_AGG_AVG) && (vk == VAL_DICT_I32 || vk == VAL_RAW_I32)) q.smem_slot[a] = (int8_t)nsum++;
       else ok = false;
     }
@@ -580,6 +625,11 @@ int plan_scan(const Tuning& tune, DeviceLimits lim, const pb200_query* query, pb
       if (q.aggs[a].slot < 0) continue;
       const DeviceColumn& c = segments[s]->cols[query->aggs[a].column];
       sd.dict[a] = c.dict_native;
+      if (plan.limb[a] >= 0) {   // K, H or L of the column's limb dictionaries (checked ready above)
+        const MomentDict& md = *c.moments;
+        sd.dict[a] = md.limbs + (size_t)plan.limb[a] * md.entries;
+        continue;
+      }
       if ((q.aggs[a].function == PB200_AGG_SUM || q.aggs[a].function == PB200_AGG_AVG) && q.aggs[a].val_kind != VAL_RAW_I32 && !c.dict_native) {
         set_error("SUM/AVG over column %d needs its dictionary on the device", query->aggs[a].column);
         return PB200_E_INVALID;
@@ -587,14 +637,18 @@ int plan_scan(const Tuning& tune, DeviceLimits lim, const pb200_query* query, pb
     }
   }
 
-  bool any_pct = false;
+  bool any_pct = false, any_mom = false;
   for (int a = 0; a < nagg; a++) any_pct |= plan.pct_rep[a] >= 0;
-  if (any_pct) {
-    // histogram bins are u32: a result over 2^32 docs could wrap one
+  for (int a = 0; a < nuser; a++) any_mom |= plan.mom_first[a] >= 0;
+  if (any_pct || any_mom) {
+    // histogram bins are u32; the moments' limb sums are exact for n < 2^32: a result over 2^32 docs is refused
     for (int r = 0; r < nres; r++) {
       unsigned long long docs = 0;
       for (int s = 0; s < nseg; s++) if (merge || s == r) docs += (unsigned long long)segments[s]->num_docs;
-      if (docs >= (1ull << 32)) { set_error("PERCENTILE over %llu docs in one result: histogram bins are 32-bit", docs); return PB200_E_UNSUPPORTED; }
+      if (docs >= (1ull << 32)) {
+        set_error("%s over %llu docs in one result: at most 2^32 - 1", any_pct ? "PERCENTILE" : "VAR/STDDEV", docs);
+        return PB200_E_UNSUPPORTED;
+      }
     }
   }
   if (!plan.group_by) {
@@ -677,7 +731,7 @@ int plan_scan(const Tuning& tune, DeviceLimits lim, const pb200_query* query, pb
       };
       bool has_marker = false;
       for (int a = 0; a < nagg; a++) {
-        need_count |= q.aggs[a].function == PB200_AGG_COUNT || q.aggs[a].function == PB200_AGG_AVG;
+        need_count |= q.aggs[a].function == PB200_AGG_COUNT || q.aggs[a].function == PB200_AGG_AVG || is_moments_fn(q.aggs[a].function);
         has_marker |= marks_groups(a);
       }
       bool need_seen = !need_count && !has_marker && !t.hashed;  // a hash table's keys mark the groups that exist

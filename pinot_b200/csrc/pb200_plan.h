@@ -79,6 +79,12 @@ struct ScanPlan {
   // first PERCENTILE of its column, the only one with an agg code (-1: not a PERCENTILE)
   std::vector<double> pct_p;
   std::vector<int> pct_rep;
+  // VAR / STDDEV (pb200_moments.h): the caller's aggregations come first, then three internal INT-dictionary SUMs per
+  // column (K, H, L limbs) -- q.num_aggs and every per-aggregation array count them all
+  int num_user_aggs = 0;
+  std::vector<pb200_agg> aggs;                        // the launch's aggregations, internal ones included
+  std::vector<int> mom_first;                         // [user agg] the first of its column's limb sums (-1: not VAR / STDDEV)
+  std::vector<int> limb;                              // [agg] 0 / 1 / 2 for the K / H / L limb sums, else -1
   std::vector<std::vector<size_t>> hist_entries;      // aggregation only: [result][agg] histogram entries of an owner (0: none)
   long long hist_total = 0;                           // histogram entries of all results of the call
   std::vector<long long> in_filter;                   // per result: num_entries_scanned_in_filter

@@ -196,6 +196,10 @@ def execute_and_combine(plan_maker_or_backend, segments: Sequence, query, dist, 
         # per-GPU histograms are not reduced across GPUs: the caller runs the query per GPU and merges by value
         from ._lib import E_UNSUPPORTED, UnsupportedQueryError
         raise UnsupportedQueryError(E_UNSUPPORTED, "PERCENTILE is not combined across GPUs")
+    if any(a.function in ("VARPOP", "VARSAMP", "STDDEVPOP", "STDDEVSAMP") for a in query.aggregations):
+        # per-GPU moments are not reduced across GPUs: the caller runs the query per GPU and merges them by value
+        from ._lib import E_UNSUPPORTED, UnsupportedQueryError
+        raise UnsupportedQueryError(E_UNSUPPORTED, "VAR/STDDEV is not combined across GPUs")
     backend = plan_maker_or_backend if hasattr(plan_maker_or_backend, "finish") else DeviceBackend(plan_maker_or_backend)
     world = dist.get_world_size()
     if any(a.function == "DISTINCTCOUNT" for a in query.aggregations):

@@ -24,7 +24,7 @@ import numpy as np
 
 from . import _lib
 from ._lib import UnsupportedQueryError  # noqa: F401  (re-export)
-from .query import Filter, QueryContext, postfix
+from .query import MOMENT_FUNCTIONS, Filter, Moments, QueryContext, postfix
 
 
 class B200Context:
@@ -321,6 +321,8 @@ class ResultsBlock:
     # PERCENTILE of per-segment results: (agg, row) -> (dictIds ascending, counts) of the row's non-zero histogram bins,
     # the intermediate a by-value merge adds up (cli.merge_blocks)
     histograms: Dict[Tuple[int, int], Tuple[np.ndarray, np.ndarray]] = field(default_factory=dict)
+    # VAR / STDDEV: (agg, row) -> the row's exact Moments (pb200_result_moments), what a by-value merge adds up
+    moments: Dict[Tuple[int, int], Moments] = field(default_factory=dict)
 
     def release(self, ctx: "B200Context") -> None:
         """Frees the native result of a block executed with keep_handle=True (or views=True: the arrays die with it)."""
@@ -502,7 +504,7 @@ def _read_result(ctx: B200Context, handle, q: QueryContext, kind: int, keep_hand
     g = meta.num_groups
     rows = 1 if g < 0 else g
     k = len(q.group_by)
-    if views and not any(a.function in ("DISTINCTCOUNT", "PERCENTILE") for a in q.aggregations):
+    if views and not any(a.function in ("DISTINCTCOUNT", "PERCENTILE") + MOMENT_FUNCTIONS for a in q.aggregations):
         keys, doubles, longs, ids = _read_views(ctx, handle, q, meta)
         stats = ExecutionStatistics(meta.num_docs_scanned, meta.num_entries_scanned_in_filter,
                                     meta.num_entries_scanned_post_filter, meta.num_total_docs)
@@ -541,11 +543,21 @@ def _read_result(ctx: B200Context, handle, q: QueryContext, kind: int, keep_hand
                 hid, hcnt = np.zeros(int(n), dtype=np.int32), np.zeros(int(n), dtype=np.int64)
                 _lib.check(min(0, int(L.pb200_result_histogram(handle, a, row, _ptr(hid), _ptr(hcnt), int(n)))))
                 hists[(a, row)] = (hid, hcnt)
+    moments = {}
+    for a, agg in enumerate(q.aggregations):
+        if agg.function in MOMENT_FUNCTIONS and histograms:   # per-segment blocks: what a by-value merge adds up
+            n, cm, s1, lo, hi = C.c_int64(), C.c_int64(), C.c_uint64(), C.c_uint64(), C.c_uint64()
+            cx, e = C.c_int32(), C.c_int32()
+            for row in range(rows):
+                _lib.check(L.pb200_result_moments(handle, a, row, C.byref(n), C.byref(cm), C.byref(cx), C.byref(e),
+                                                  C.byref(s1), C.byref(lo), C.byref(hi)))
+                moments[(a, row)] = Moments(n.value, cm.value, cx.value, e.value, s1.value, (hi.value << 64) | lo.value)
     stats = ExecutionStatistics(meta.num_docs_scanned, meta.num_entries_scanned_in_filter,
                                 meta.num_entries_scanned_post_filter, meta.num_total_docs)
     block = ResultsBlock(g, _lib.REGIMES[meta.regime], bool(meta.groups_limit_reached), stats, keys, doubles, longs,
                          ids, distinct, meta.device_ms, _lib.OPERATOR_KINDS.get(kind, "AGGREGATION"))
     block.histograms = hists
+    block.moments = moments
     block.count_carrier = bool(meta.reserved & 1)
     block.carrier_unsafe = bool(meta.reserved & 2)
     block.flag_slot = bool(meta.reserved & 4)

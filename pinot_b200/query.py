@@ -45,7 +45,7 @@ FilterNode = Union[Filter, Predicate]
 
 @dataclass
 class Aggregation:
-    function: str  # COUNT | SUM | MIN | MAX | AVG | DISTINCTCOUNT | PERCENTILE
+    function: str  # COUNT | SUM | MIN | MAX | AVG | DISTINCTCOUNT | PERCENTILE | VARPOP | VARSAMP | STDDEVPOP | STDDEVSAMP
     column: Optional[str] = None  # None for COUNT(*)
     # FILTER (WHERE ...) clause of this function (QueryContext.getFilteredAggregationFunctions: Pair<function, FilterContext>);
     # evaluated together with the query's own filter (AggregationFunctionUtils.buildFilteredAggregationInfos)
@@ -79,6 +79,52 @@ def percentile_of_counts(counts) -> float:
         if k < 0:
             return float(v)
     raise AssertionError("unreachable")
+
+
+MOMENT_FUNCTIONS = ("VARPOP", "VARSAMP", "STDDEVPOP", "STDDEVSAMP")
+
+
+@dataclass(frozen=True)
+class Moments:
+    """Exact moments of n values v_i = c + k_i * 2^e (c = c_mant * 2^c_exp): s1 = sum k_i, s2 = sum k_i^2 -- the
+    intermediate of VAR / STDDEV that per-segment results are merged by (pb200_result_moments)."""
+    n: int
+    c_mant: int
+    c_exp: int
+    e: int
+    s1: int
+    s2: int
+
+    def value_sums(self):
+        """(n, sum v, sum v^2) as exact Fractions."""
+        from fractions import Fraction
+        c = Fraction(self.c_mant) * Fraction(2) ** self.c_exp
+        u = Fraction(2) ** self.e
+        return self.n, self.n * c + self.s1 * u, self.n * c * c + 2 * c * self.s1 * u + self.s2 * u * u
+
+
+def merge_moments(parts) -> tuple:
+    """By-value merge of Moments: (n, sum v, sum v^2), exact."""
+    from fractions import Fraction
+    n, s1, s2 = 0, Fraction(0), Fraction(0)
+    for m in parts:
+        a, b, c = m.value_sums()
+        n, s1, s2 = n + a, s1 + b, s2 + c
+    return n, s1, s2
+
+
+def moments_final(function: str, sums) -> float:
+    """VarianceAggregationFunction's final value from exact (n, sum v, sum v^2), rounded once: -inf for n == 0, and for
+    the *SAMP functions at n == 1; STDDEV is the sqrt of the rounded variance."""
+    import math
+    from fractions import Fraction
+    n, s1, s2 = sums
+    samp = function in ("VARSAMP", "STDDEVSAMP")
+    if n == 0 or (samp and n == 1):
+        return float("-inf")
+    m2 = Fraction(s2) - Fraction(s1) * Fraction(s1) / n   # sum (v - mean)^2
+    var = float(m2 / (n - 1 if samp else n))              # Fraction -> float rounds to nearest
+    return math.sqrt(var) if function.startswith("STDDEV") else var
 
 
 @dataclass

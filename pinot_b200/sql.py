@@ -8,6 +8,7 @@ stays Java).  This module exists so the parity tests read like the reference's
 
     SELECT item[, item...] FROM table [WHERE cond] [GROUP BY col[, col...]] [ORDER BY expr [ASC|DESC], ...] [LIMIT n]
     item  := COUNT(*) | FN(col) | PERCENTILE(col, p) | PERCENTILE<n>(col) | col
+             (FN also VAR_POP / VARPOP, VAR_SAMP / VARSAMP, STDDEV_POP / STDDEVPOP, STDDEV_SAMP / STDDEVSAMP)
              (plain columns are allowed only when they are group-by keys; 0 <= p <= 100, fractions allowed)
     selection (parse_selection): SELECT * | col[, col...] FROM table [WHERE cond] [ORDER BY col [ASC|DESC], ...] [LIMIT n]
     distinct (parse_distinct): SELECT DISTINCT col[, col...] FROM table [WHERE cond] [ORDER BY col [ASC|DESC], ...] [LIMIT n]
@@ -33,7 +34,10 @@ from .query import Aggregation, Filter, FilterNode, Predicate, QueryContext, opt
 _TOKEN = re.compile(r"\s*(?:(\d+\.\d+(?:[eE][-+]?\d+)?|-?\d+\.\d+|-?\d+)|'((?:[^']|'')*)'|(<=|>=|<>|!=|[=<>(),*+/%-])|"
                     r"([A-Za-z_$][A-Za-z0-9_$]*))")
 
-_FUNCTIONS = {"COUNT", "SUM", "MIN", "MAX", "AVG", "DISTINCTCOUNT", "PERCENTILE"}
+# VarianceAggregationFunction: both spellings of each function, the underscore one canonicalised to the other
+_ALIASES = {"VAR_POP": "VARPOP", "VAR_SAMP": "VARSAMP", "STDDEV_POP": "STDDEVPOP", "STDDEV_SAMP": "STDDEVSAMP"}
+_FUNCTIONS = {"COUNT", "SUM", "MIN", "MAX", "AVG", "DISTINCTCOUNT", "PERCENTILE", "VARPOP", "VARSAMP", "STDDEVPOP",
+              "STDDEVSAMP"} | set(_ALIASES)
 _PERCENTILE_N = re.compile(r"PERCENTILE(\d+)")
 
 # single-column transforms (DESIGN.md section 3.8): SQL name (lower case, no '_') -> canonical name
@@ -287,7 +291,7 @@ def resolve_order_by(query: QueryContext) -> List[tuple]:
         m = re.fullmatch(r"([A-Za-z_$][A-Za-z0-9_$]*)\((.+?)(?:,([-+0-9.eE]+))?\)", expr)
         found = None
         if m and _is_function(m.group(1)):
-            fn, col = m.group(1).upper(), m.group(2)
+            fn, col = _ALIASES.get(m.group(1).upper(), m.group(1).upper()), m.group(2)
             arg = None if m.group(3) is None else float(m.group(3))
             for a, agg in enumerate(query.aggregations):
                 if agg.function == fn and (fn == "COUNT" or agg.column == col) and (fn != "PERCENTILE" or agg.arg == arg):
@@ -309,7 +313,7 @@ def parse(sql: str, **options) -> QueryContext:
         k, name = p.peek()
         if k == "id" and _is_function(name) and p.toks[p.i + 1:p.i + 2] == [("op", "(")]:
             p.i += 2
-            fn = name.upper()
+            fn = _ALIASES.get(name.upper(), name.upper())
             if fn.startswith("PERCENTILE"):
                 col, pct = p.percentile_call(name)
                 aggs.append(Aggregation("PERCENTILE", col, arg=pct))
