@@ -15,7 +15,6 @@ from __future__ import annotations
 
 import argparse
 import json
-import struct
 import sys
 from typing import Dict, List
 
@@ -25,13 +24,15 @@ def merge_blocks(query, segments, blocks) -> Dict[tuple, list]:
     AVG -> (sum, count), DISTINCTCOUNT -> set of values, PERCENTILE -> (p, {value: count}) from the per-segment
     histograms, or its final float for a block merged on the device, VAR / STDDEV -> exact (n, sum v, sum v^2) from the
     blocks' moments, each shifted from its own grid (c, e) to values, or the final float of a block merged on the device
-    (GroupByCombineOperator / AggregationFunction.merge)."""
-    from .query import MOMENT_FUNCTIONS, merge_moments
+    (GroupByCombineOperator / AggregationFunction.merge).  Float keys, set members and histogram values are compared by
+    identity (query.ValueKey: one NaN, -0.0 apart from 0.0) and MIN / MAX merge in Double.compare order, as the reference's
+    Double.equals / doubleToLongBits keyed tables and its dictionary order do."""
+    from .query import MOMENT_FUNCTIONS, merge_moments, value_key, value_order
     out: Dict[tuple, list] = {}
     for seg, b in zip(segments, blocks):
         rows = 1 if b.num_groups < 0 else b.num_groups
         for g in range(rows):
-            key = () if b.num_groups < 0 else tuple(seg.dictionary_value(c, int(b.keys[g, j])) for j, c in enumerate(query.group_by))
+            key = () if b.num_groups < 0 else tuple(value_key(seg.dictionary_value(c, int(b.keys[g, j]))) for j, c in enumerate(query.group_by))
             vals = []
             for a, agg in enumerate(query.aggregations):
                 fn = agg.function
@@ -40,12 +41,12 @@ def merge_blocks(query, segments, blocks) -> Dict[tuple, list]:
                 elif fn == "AVG":
                     vals.append((float(b.doubles[a][g]), int(b.longs[a][g])))
                 elif fn == "DISTINCTCOUNT":
-                    vals.append({seg.dictionary_value(agg.column, int(d)) for d in b.distinct[(a, g)]})
+                    vals.append({value_key(seg.dictionary_value(agg.column, int(d))) for d in b.distinct[(a, g)]})
                 elif fn == "PERCENTILE" and (a, g) in b.histograms:
                     ids, counts = b.histograms[(a, g)]
                     hist: Dict[float, int] = {}
                     for d, c in zip(ids, counts):
-                        v = float(seg.dictionary_value(agg.column, int(d)))
+                        v = value_key(float(seg.dictionary_value(agg.column, int(d))))
                         hist[v] = hist.get(v, 0) + int(c)
                     vals.append((agg.arg, hist))
                 elif fn in MOMENT_FUNCTIONS and (a, g) in b.moments:
@@ -61,9 +62,9 @@ def merge_blocks(query, segments, blocks) -> Dict[tuple, list]:
                 if fn in ("COUNT", "SUM"):
                     cur[a] += vals[a]
                 elif fn == "MIN":
-                    cur[a] = min(cur[a], vals[a])
+                    cur[a] = min(cur[a], vals[a], key=value_order)
                 elif fn == "MAX":
-                    cur[a] = max(cur[a], vals[a])
+                    cur[a] = max(cur[a], vals[a], key=value_order)
                 elif fn == "AVG":
                     cur[a] = (cur[a][0] + vals[a][0], cur[a][1] + vals[a][1])
                 elif fn == "PERCENTILE" and isinstance(cur[a], tuple):
@@ -76,24 +77,16 @@ def merge_blocks(query, segments, blocks) -> Dict[tuple, list]:
     return out
 
 
-def _order_value(v):
-    """Sort key of a final value: doubles in Double.compare order (-0.0 before 0.0), other values as they are."""
-    if isinstance(v, float):
-        u = struct.unpack("<Q", struct.pack("<d", v))[0]
-        return u ^ 0xFFFFFFFFFFFFFFFF if u >> 63 else u | (1 << 63)
-    return v
-
-
 def final_rows(query, table: Dict[tuple, list]) -> List[list]:
     """Broker-side extraction of final results + ORDER BY + LIMIT.  ORDER BY compares final values (AVG = sum / count,
     DISTINCTCOUNT = set size) and breaks ties by the key values ascending, in GROUP BY column order -- the library's order.
     Without ORDER BY Pinot returns an arbitrary LIMIT-sized subset; here the rows are sorted by key to make the output
     stable."""
-    from .query import MOMENT_FUNCTIONS, moments_final, percentile_of_counts
+    from .query import MOMENT_FUNCTIONS, moments_final, percentile_of_counts, value_order
     from .sql import resolve_order_by
     items = resolve_order_by(query) if query.is_group_by else []
     rows = []
-    keys = sorted(table) if items else sorted(table, key=lambda k: tuple(str(x) for x in k))
+    keys = sorted(table, key=lambda k: tuple(value_order(x) for x in k)) if items else sorted(table, key=lambda k: tuple(str(x) for x in k))
     for key in keys:
         vals = []
         for agg, v in zip(query.aggregations, table[key]):
@@ -111,7 +104,7 @@ def final_rows(query, table: Dict[tuple, list]) -> List[list]:
     k = len(query.group_by)
     for kind, index, asc in reversed(items):  # stable passes, last item first
         col = index if kind == "GROUP_BY" else k + index
-        rows.sort(key=lambda r: _order_value(r[col]), reverse=not asc)
+        rows.sort(key=lambda r: value_order(r[col]), reverse=not asc)
     return rows[: query.limit]
 
 

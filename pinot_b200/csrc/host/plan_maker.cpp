@@ -35,10 +35,47 @@ struct Evaluated {
   std::vector<int32_t> ids;     // EQ/IN matching ids; NEQ/NOT_IN NON-matching ids (sorted)
 };
 
+// A FLOAT / DOUBLE column the segment stores raw, with a dictionary synthesised at load: the reference evaluates its
+// predicates per value with Java's <, > and == (the *RawValueBased*PredicateEvaluators), not by a dictionary search.  So
+// NaN matches only NEQ / NOT_IN, and 0 matches both zeros.  The matching entries are found by one pass over the
+// dictionary (at most raw_dict_max entries); in Double.compare order they are contiguous for a RANGE (the zeros are
+// neighbours and NaN, which no range matches, is last).
+bool raw_value_matches(const HostColumn& c, int id, const pb200h_filter_node& n, const pb200h_literal* v) {
+  const bool fl = c.data_type == PB200_FLOAT;
+  const double x = c.as_double(id);
+  auto lt = [&](const pb200h_literal& l) { return fl ? (float)x < (float)l.d : x < l.d; };
+  auto gt = [&](const pb200h_literal& l) { return fl ? (float)x > (float)l.d : x > l.d; };
+  auto eq = [&](const pb200h_literal& l) { return fl ? (float)x == (float)l.d : x == l.d; };
+  if (n.type == PB200H_RANGE) {
+    if (!n.lower_unbounded && !(n.lower_inclusive ? gt(v[0]) || eq(v[0]) : gt(v[0]))) return false;
+    if (!n.upper_unbounded && !(n.upper_inclusive ? lt(v[1]) || eq(v[1]) : lt(v[1]))) return false;
+    return x == x;  // an unbounded range matches no NaN either
+  }
+  for (int i = 0; i < n.num_values; i++) if (eq(v[i])) return true;  // EQ / IN match; NEQ / NOT_IN: the excluded values
+  return false;
+}
+
 Evaluated evaluate(const HostColumn& c, const pb200h_filter_node& n, const pb200h_literal* lits) {
   Evaluated e;
   const pb200h_literal* v = lits + n.values_offset;
   const int card = c.cardinality;
+  if (c.synthesized_dictionary && (c.data_type == PB200_FLOAT || c.data_type == PB200_DOUBLE)) {
+    e.is_range = n.type == PB200H_RANGE;
+    e.exclusive = n.type == PB200H_NEQ || n.type == PB200H_NOT_IN;
+    for (int id = 0; id < card; id++) if (raw_value_matches(c, id, n, v)) e.ids.push_back(id);
+    const int k = (int)e.ids.size();
+    if (e.is_range) {
+      e.start = k ? e.ids.front() : 0;
+      e.end = k ? e.ids.back() + 1 : 0;
+      e.ids.clear();
+      if (k == 0) e.always_false = true; else if (k == card) e.always_true = true;
+    } else if (!e.exclusive) {
+      if (k == 0) e.always_false = true; else if (k == card) e.always_true = true;
+    } else {
+      if (k == 0) e.always_true = true; else if (k == card) e.always_false = true;
+    }
+    return e;
+  }
   if (n.type == PB200H_RANGE) {  // SortedDictionaryBasedRangePredicateEvaluator :126-168
     e.is_range = true;
     if (n.lower_unbounded) e.start = 0;

@@ -120,13 +120,24 @@ bool lz4_block_decode(const unsigned char* ip, size_t n, unsigned char* dst, siz
   return true;
 }
 
-// order-preserving 64-bit key of a stored value (Pinot dictionaries are sorted by Integer / Long / Float / Double.compare)
+// order-preserving 64-bit key of a stored value (Pinot dictionaries are sorted by Integer / Long / Float / Double.compare).
+// Equal keys are one dictionary entry: every NaN bit pattern becomes the canonical NaN first (Float.floatToIntBits /
+// Double.doubleToLongBits), so all NaNs are one value, sorted after +inf; -0.0 and 0.0 stay two values.
 inline uint64_t sort_key(const unsigned char* p, int data_type) {
   switch (data_type) {
     case PB200_INT: return (uint64_t)((int64_t)(int32_t)rd_be32(p)) ^ 0x8000000000000000ull;
     case PB200_LONG: return rd_be64(p) ^ 0x8000000000000000ull;
-    case PB200_FLOAT: { uint32_t u = rd_be32(p); u = (u & 0x80000000u) ? ~u : (u | 0x80000000u); return u; }
-    default: { uint64_t u = rd_be64(p); return (u & 0x8000000000000000ull) ? ~u : (u | 0x8000000000000000ull); }
+    case PB200_FLOAT: {
+      uint32_t u = rd_be32(p);
+      if ((u & 0x7FFFFFFFu) > 0x7F800000u) u = 0x7FC00000u;
+      u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+      return u;
+    }
+    default: {
+      uint64_t u = rd_be64(p);
+      if ((u & 0x7FFFFFFFFFFFFFFFull) > 0x7FF0000000000000ull) u = 0x7FF8000000000000ull;
+      return (u & 0x8000000000000000ull) ? ~u : (u | 0x8000000000000000ull);
+    }
   }
 }
 inline void store_key(uint64_t k, int data_type, unsigned char* p) {
@@ -218,7 +229,7 @@ bool synthesize_dictionary(const std::vector<unsigned char>& values_be, int data
   // pass 1: distinct keys in an open-addressing set that gives up once the column is wider than max_cardinality
   size_t cap = 1;
   while (cap < (size_t)max_cardinality * 2 + 2) cap <<= 1;
-  const uint64_t kEmpty = ~0ull;  // not a valid key after the sign transform only for NaN payload all-ones: handled below
+  const uint64_t kEmpty = ~0ull;  // also the key of LONG Long.MAX_VALUE: handled below
   std::vector<uint64_t> slots(cap, kEmpty);
   std::vector<uint64_t> distinct;
   bool has_all_ones = false;

@@ -20,6 +20,7 @@
 #include <vector>
 
 #include "host_internal.h"
+#include "../pb200_order.h"
 
 using pb200::set_error;
 
@@ -225,13 +226,17 @@ extern "C" int32_t pb200h_startree_attach(pb200_ctx* ctx, pb200h_segment* seg, c
       dict.resize(8ull * card);
       for (int i = 0; i < card; i++) { uint64_t x = (uint64_t)u[i]; for (int b = 0; b < 8; b++) dict[8ull * i + b] = (unsigned char)(x >> (56 - 8 * b)); }
     } else {
-      std::vector<double> v(num_star_docs), u;
-      for (int i = 0; i < num_star_docs; i++) memcpy(&v[i], &raw[i], 8);
+      // sorted and made unique by Double.compare order keys: a pre-aggregated SUM may be NaN (one value, last) or -0.0
+      std::vector<uint64_t> v(num_star_docs), u;
+      for (int i = 0; i < num_star_docs; i++) { double d; memcpy(&d, &raw[i], 8); v[i] = pb200::double_order_bits(d); }
       u = v; std::sort(u.begin(), u.end()); u.erase(std::unique(u.begin(), u.end()), u.end());
       card = (int)u.size();
       for (int i = 0; i < num_star_docs; i++) ids[i] = (int32_t)(std::lower_bound(u.begin(), u.end(), v[i]) - u.begin());
       dict.resize(8ull * card);
-      for (int i = 0; i < card; i++) { uint64_t x; memcpy(&x, &u[i], 8); for (int b = 0; b < 8; b++) dict[8ull * i + b] = (unsigned char)(x >> (56 - 8 * b)); }
+      for (int i = 0; i < card; i++) {
+        const uint64_t x = (u[i] >> 63) ? (u[i] & 0x7FFFFFFFFFFFFFFFull) : ~u[i];   // the key back to the double's bits
+        for (int b = 0; b < 8; b++) dict[8ull * i + b] = (unsigned char)(x >> (56 - 8 * b));
+      }
     }
     int bits = 1;
     while (bits < 31 && (1ll << bits) < card) bits++;

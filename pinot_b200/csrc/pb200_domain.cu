@@ -63,13 +63,23 @@ inline uint32_t rd32(const unsigned char* p) { return (uint32_t)p[0] << 24 | (ui
 inline uint64_t rd64(const unsigned char* p) { return (uint64_t)rd32(p) << 32 | rd32(p + 4); }
 
 // Order key of a fixed-width dictionary entry: comparing keys as unsigned integers == the order Pinot sorted the
-// dictionary in (Integer / Long natural order; Float.compare / Double.compare order incl. -0.0 < 0.0).
+// dictionary in (Integer / Long natural order; Float.compare / Double.compare order incl. -0.0 < 0.0).  Every NaN bit
+// pattern gets the canonical NaN's key (floatToIntBits / doubleToLongBits): one value, after +inf.  A dictionary written
+// by Java stores the raw bits of the first NaN it saw, so its last entry may be a NaN with the sign bit set.
 inline uint64_t order_key(int type, const unsigned char* e) {
   switch (type) {
     case PB200_INT: return (uint64_t)(rd32(e) ^ 0x80000000u);
     case PB200_LONG: return rd64(e) ^ 0x8000000000000000ull;
-    case PB200_FLOAT: { uint32_t u = rd32(e); return (uint64_t)((u & 0x80000000u) ? ~u : (u | 0x80000000u)); }
-    default: { uint64_t u = rd64(e); return (u & 0x8000000000000000ull) ? ~u : (u | 0x8000000000000000ull); }
+    case PB200_FLOAT: {
+      uint32_t u = rd32(e);
+      if ((u & 0x7FFFFFFFu) > 0x7F800000u) u = 0x7FC00000u;
+      return (uint64_t)((u & 0x80000000u) ? ~u : (u | 0x80000000u));
+    }
+    default: {
+      uint64_t u = rd64(e);
+      if ((u & 0x7FFFFFFFFFFFFFFFull) > 0x7FF0000000000000ull) u = 0x7FF8000000000000ull;
+      return (u & 0x8000000000000000ull) ? ~u : (u | 0x8000000000000000ull);
+    }
   }
 }
 inline std::string unpadded(const unsigned char* e, int width) {
@@ -150,7 +160,8 @@ extern "C" int32_t pb200_domain_create(pb200_ctx* ctx, int32_t ncols, const pb20
           all.emplace_back(key, b + (size_t)i * fixed);
         }
       }
-      std::sort(all.begin(), all.end(), [](const auto& a, const auto& b) { return a.first < b.first; });
+      // stable: of entries with one key (NaNs with different bits), the first part's is the domain's entry
+      std::stable_sort(all.begin(), all.end(), [](const auto& a, const auto& b) { return a.first < b.first; });
       all.erase(std::unique(all.begin(), all.end(), [](const auto& a, const auto& b) { return a.first == b.first; }), all.end());
       c.entry_bytes = fixed;
       c.cardinality = (int)all.size();

@@ -6,7 +6,8 @@
 //   SUM, MIN, MAX             the double (MIN / MAX of a group without rows: +inf / -inf)
 //   AVG                       sum / count, -inf when the count is 0
 //   group-by column           its dictId (dictId order is value order within one dictionary / domain)
-// Doubles compare like Java's Double.compare (-0.0 before 0.0; NaN is not produced on this path).  Each item becomes an
+// Doubles compare like Java's Double.compare: -0.0 before 0.0, and every NaN (a SUM over +inf and -inf rows, a MAX over a
+// NaN entry, whichever NaN bits the hardware or the dictionary produced) is one value after +inf.  Each item becomes an
 // unsigned key whose ascending order is the item's order; rows equal on every item are ordered by their group-key
 // values, ascending, in GROUP BY column order.  Plain C++ when not compiled by nvcc (CPU tests compile it with g++).
 #pragma once
@@ -31,10 +32,12 @@ PB200_HD int order_cmp_of(int fn) {
   return fn == PB200_AGG_AVG ? ORDER_CMP_AVG : (fn == PB200_AGG_COUNT || fn == PB200_AGG_DISTINCTCOUNT) ? ORDER_CMP_LONG : ORDER_CMP_DOUBLE;
 }
 
-// Double.compare order as unsigned order: negative values have all bits flipped, the others only the sign bit
+// Double.compare order as unsigned order: a NaN is the canonical NaN (doubleToLongBits), then negative values have all
+// bits flipped, the others only the sign bit
 PB200_HD uint64_t double_order_bits(double v) {
   uint64_t u;
   memcpy(&u, &v, 8);
+  if ((u & 0x7FFFFFFFFFFFFFFFull) > 0x7FF0000000000000ull) u = 0x7FF8000000000000ull;
   return (u >> 63) ? ~u : (u | (1ull << 63));
 }
 

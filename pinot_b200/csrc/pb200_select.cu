@@ -38,6 +38,7 @@
 #include "pb200_internal.h"
 #include "pb200_plan.h"
 #include "pb200_scan_launch.h"
+#include "pb200_order.h"
 #include "pb200_select.cuh"
 
 namespace pb200 {
@@ -63,7 +64,10 @@ __device__ __forceinline__ uint32_t order_key(const SelCol& c, int32_t doc) {
   const uint32_t x = read_at(c, doc);
   uint32_t k;
   if (c.kind == SEL_RAW_I32) k = x ^ 0x80000000u;
-  else if (c.kind == SEL_RAW_F32) k = (x & 0x80000000u) ? ~x : (x | 0x80000000u);
+  else if (c.kind == SEL_RAW_F32) {   // Float.compare order: every NaN is the canonical one, after +inf
+    const uint32_t f = (x & 0x7FFFFFFFu) > 0x7F800000u ? 0x7FC00000u : x;
+    k = (f & 0x80000000u) ? ~f : (f | 0x80000000u);
+  }
   else k = c.bits >= 32 ? x : x << (32 - c.bits);
   return c.desc ? ~k : k;
 }
@@ -231,10 +235,11 @@ int compare_item(const pb200_segment* const* segments, int col, int kind, bool d
       const int x = i < wa ? pa[i] : 0, y = i < wb ? pb[i] : 0;
       c = x < y ? -1 : x > y;
     }
-  } else if (selection_kind_is_double(kind)) {
+  } else if (selection_kind_is_double(kind)) {   // Double.compare: -0.0 before 0.0, one NaN after +inf (a total order)
     double x, y;
     memcpy(&x, &v[ia], 8); memcpy(&y, &v[ib], 8);
-    c = x < y ? -1 : x > y;
+    const uint64_t kx = double_order_bits(x), ky = double_order_bits(y);
+    c = kx < ky ? -1 : kx > ky;
   } else {
     const long long x = (long long)v[ia], y = (long long)v[ib];
     c = x < y ? -1 : x > y;

@@ -754,19 +754,21 @@ def merge_distinct_blocks(blocks: Sequence[SelectionResultsBlock], order_by=(), 
     """By-value merge of per-segment DISTINCT blocks of one submission (segment_index refers to that submission): the
     union of their tuples, each with its earliest (segment, doc) occurrence, ordered by first occurrence or by `order_by`
     ([(column, ascending)], ties by first occurrence), then the first `limit`.  Exact, because each segment's block holds
-    its own first (or top) `limit` tuples."""
+    its own first (or top) `limit` tuples.  Floats are tuples' members by identity (one NaN, -0.0 apart from 0.0) and
+    order by Double.compare (query.value_key / value_order), as in the reference's DISTINCT table."""
+    from .query import value_key, value_order
     names = list(blocks[0].names)
     first: Dict[tuple, tuple] = {}
     for b in blocks:
         for i in range(b.num_rows):
-            key = tuple(c[i].item() if hasattr(c[i], "item") else c[i] for c in b.columns)
+            key = tuple(value_key(c[i].item() if hasattr(c[i], "item") else c[i]) for c in b.columns)
             occ = (int(b.segment_index[i]), int(b.doc_ids[i]))
             if key not in first or occ < first[key]:
                 first[key] = occ
     rows = sorted(first.items(), key=lambda kv: kv[1])
     for col, asc in reversed(list(order_by)):   # stable passes, last item first
         k = names.index(col)
-        rows.sort(key=lambda kv: kv[0][k], reverse=not asc)
+        rows.sort(key=lambda kv: value_order(kv[0][k]), reverse=not asc)
     rows = rows[:limit]
     columns = []
     for k, c in enumerate(blocks[0].columns):

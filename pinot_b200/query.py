@@ -11,6 +11,7 @@ Predicates are in VALUE space here (as the broker sends them); turning them into
 """
 from __future__ import annotations
 
+import struct
 from dataclasses import dataclass, field
 from typing import List, Optional, Sequence, Union
 
@@ -66,15 +67,46 @@ def percentile_index(n: int, p: float) -> int:
     return min(int(float(n) * float(p) / 100.0), n - 1)
 
 
+def value_order(v):
+    """Sort key of a value in the reference's total order: a float in Double.compare order (-0.0 before 0.0, every NaN
+    one value after +inf), any other value as it is."""
+    if isinstance(v, float):
+        u = struct.unpack("<Q", struct.pack("<d", v))[0]
+        if u & 0x7FFFFFFFFFFFFFFF > 0x7FF0000000000000:
+            u = 0x7FF8000000000000
+        return u ^ 0xFFFFFFFFFFFFFFFF if u >> 63 else u | (1 << 63)
+    return v
+
+
+class ValueKey(float):
+    """A float compared by identity, as the reference's group keys, DISTINCTCOUNT sets and histograms are
+    (Double.equals / doubleToLongBits): all NaNs are one value, -0.0 and 0.0 are two.  Prints and sums as the float."""
+    __slots__ = ()
+
+    def __eq__(self, other):
+        return isinstance(other, float) and value_order(float(self)) == value_order(float(other))
+
+    def __ne__(self, other):
+        return not self == other
+
+    def __hash__(self):
+        return hash(value_order(float(self)))
+
+
+def value_key(v):
+    """`v` as a key of a by-value merge: floats by identity (ValueKey), other values as they are."""
+    return ValueKey(v) if isinstance(v, float) else v
+
+
 def percentile_of_counts(counts) -> float:
     """PERCENTILE over a {value: count} multiset (the by-value merge of per-segment histograms); -inf when empty.
-    `counts` is (p, {value: count})."""
+    `counts` is (p, {value: count}); values rank in Double.compare order."""
     p, hist = counts
     n = sum(hist.values())
     if n == 0:
         return float("-inf")
     k = percentile_index(n, p)
-    for v in sorted(hist):
+    for v in sorted(hist, key=value_order):
         k -= hist[v]
         if k < 0:
             return float(v)

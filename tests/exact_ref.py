@@ -22,9 +22,8 @@ columns, and the arithmetic is exact:
 
 Merged results: the reference runs over the union of the segments' rows, keyed by value (not a sum of per-segment floats).
 
-Out of scope: NaN and -0.0 in FLOAT / DOUBLE columns.  np.unique (the test segment builder) merges -0.0 with +0.0 and
-sorts NaN last, while the reference's Math.min / Math.max propagate NaN and its group-by `<` keeps whichever zero came
-first; which one the product follows is not settled here, so no test feeds those values.
+NaN and -0.0 in FLOAT / DOUBLE columns are held by tests/float_edges_ref.py: np.unique (the test segment builder) merges
+-0.0 with +0.0, so this reference is fed columns without them, and sum_within_bound takes finite sums only.
 """
 from __future__ import annotations
 

@@ -9,7 +9,7 @@ predicate's literal exactly, in the column's own type; it never calls the oracle
 * FLOAT: np.float32 against (float)literal; DOUBLE: float.
 * STRING: unpadded UTF-8 bytes, ordered bytewise.
 
-NaN and -0.0 are out of scope (see exact_ref)."""
+NaN and -0.0 are held by tests/float_edges_ref.py."""
 from __future__ import annotations
 
 import math

@@ -5,7 +5,7 @@ histograms or dictIds.
 
 Values are sorted in the column's own type and converted to double afterwards: the conversion is monotone, so this is the
 reference's "convert, then sort" order, and the selected stored value also names the dictId a dictionary column must
-return (a LONG beyond 2^53 is then checked exactly).  NaN and -0.0 are out of scope."""
+return (a LONG beyond 2^53 is then checked exactly).  NaN and -0.0 are held by tests/float_edges_ref.py."""
 from __future__ import annotations
 
 from typing import Dict, List, Sequence

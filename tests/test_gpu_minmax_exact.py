@@ -5,7 +5,7 @@ values at the extremes of their types:
   stays a raw 32-bit stream, VAL_RAW_I32).  Groups k % 4 == 0 hold INT_MAX only, k % 4 == 1 INT_MIN only: a raw MAX at
   INT_MAX and a raw MIN at INT_MAX sit on the u32 values that mean "no row" for a dictionary entry.
 * LONG at INT64_MIN / INT64_MAX and 2^53 - 1, 2^53, 2^53 + 1 (rounded to double to nearest); FLOAT / DOUBLE at +-inf,
-  +-max and the smallest subnormals.  NaN and -0.0 are left out (see exact_ref).
+  +-max and the smallest subnormals.  NaN and -0.0: tests/test_gpu_float_edges.py.
 * DISTINCTCOUNT columns of cardinality exactly 2^5 and 2^5 + 1 (dictIds 0 and card - 1 present) over INT, LONG, FLOAT,
   DOUBLE and STRING: the group-by bitset has 1 and 2 words per group.
 * "e" with "k": `k = 0 AND e = 1` matches rows of the large segments only.  The host cannot prove it empty (each leaf
