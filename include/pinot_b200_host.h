@@ -248,6 +248,48 @@ int64_t pb200h_result_to_datatable(const pb200h_query* query, const pb200h_segme
 int32_t pb200h_explain(pb200_ctx* ctx, const pb200h_query* query, pb200h_segment* segment, char* out,
                        int32_t capacity);
 
+/* ---- star-tree built on the device (MultipleTreesBuilder at segment load) ------------------------------------- */
+/* One tree of a table's StarTreeIndexConfig. */
+typedef struct {
+  int32_t num_dimensions;
+  const char* const* dimensions;    /* dimensionsSplitOrder */
+  int32_t num_skip_star;
+  const char* const* skip_star;     /* skipStarNodeCreationForDimensions (NULL when none) */
+  int32_t num_pairs;
+  const pb200h_agg* pairs;          /* functionColumnPairs: COUNT (column NULL or "*"), SUM, MIN, MAX */
+  int32_t max_leaf_records;         /* maxLeafRecords (Pinot's default: 10000) */
+} pb200h_startree_config;
+
+enum { PB200H_STAR_PHASE_BASE = 0,      /* rows sorted by the split order, identical tuples merged */
+       PB200H_STAR_PHASE_CONSTRUCT = 1, /* nodes and STAR children, level by level */
+       PB200H_STAR_PHASE_AGGREGATE = 2, /* aggregated docs, bottom up */
+       PB200H_STAR_PHASE_ENCODE = 3 };  /* star docs -> device segment (metric dictionaries) */
+
+typedef struct {
+  int64_t num_star_docs;
+  int64_t num_base_docs;             /* docs of distinct dimension tuples: star docs [0, num_base_docs) */
+  int32_t num_nodes;
+  int32_t reserved;
+  double phase_ms[4];                /* host wall clock per PB200H_STAR_PHASE_* */
+} pb200h_startree_build_info;
+
+/* Builds one star-tree from the segment's resident columns on the device (MultipleTreesBuilder at segment load) and
+ * attaches it as pb200h_startree_attach would: the same tree as the reference's BaseSingleTreeBuilder up to how star
+ * docs are numbered, the star docs a device segment with the same columns (dimensions, then count__* / sum__m / ...).
+ * MIN / MAX follow Double.compare order; SUM over INT accumulates exactly and is rounded once, other SUMs accumulate in
+ * double.  A load-time step like attach: not to be run concurrently with queries on that segment.  info may be NULL.
+ * PB200_E_INVALID: unknown columns, an empty or repeated split order, a skip dimension outside it, maxLeafRecords < 1,
+ * no pairs.  PB200_E_UNSUPPORTED: a dimension without dictIds, a derived column, a STRING metric, a function other
+ * than COUNT / SUM / MIN / MAX, a domain-bound segment, more than 30 dimensions, a segment without docs, 2^31 or more
+ * star docs.  A failure attaches nothing. */
+int32_t pb200h_startree_build(pb200_ctx* ctx, pb200h_segment* segment, const pb200h_startree_config* config,
+                              pb200h_startree_build_info* info);
+
+/* The index-th star-tree of the segment, built or attached: its OffHeapStarTree buffer and the segment of its star
+ * docs (owned by the segment; read it with the column accessors).  PB200_E_INVALID when there is no such tree. */
+int32_t pb200h_startree_get(const pb200h_segment* segment, int32_t index, const void** tree, uint64_t* tree_bytes,
+                            pb200h_segment** star_docs);
+
 #ifdef __cplusplus
 }
 #endif

@@ -151,6 +151,20 @@ class HStarMetric(C.Structure):
                 ("fwd_bytes", C.c_uint64)]
 
 
+class HStarTreeConfig(C.Structure):
+    _fields_ = [("num_dimensions", C.c_int32), ("dimensions", C.POINTER(C.c_char_p)), ("num_skip_star", C.c_int32),
+                ("skip_star", C.POINTER(C.c_char_p)), ("num_pairs", C.c_int32), ("pairs", C.POINTER(HAgg)),
+                ("max_leaf_records", C.c_int32)]
+
+
+class HStarTreeBuildInfo(C.Structure):
+    _fields_ = [("num_star_docs", C.c_int64), ("num_base_docs", C.c_int64), ("num_nodes", C.c_int32),
+                ("reserved", C.c_int32), ("phase_ms", C.c_double * 4)]
+
+
+STAR_BUILD_PHASES = ("base", "construct", "aggregate", "encode")
+
+
 # every symbol include/pinot_b200.h and include/pinot_b200_host.h declare (checked by tests/test_abi.py)
 EXPORTED_SYMBOLS = [
     "pb200_init", "pb200_shutdown", "pb200_last_error", "pb200_abi_version", "pb200_device_info", "pb200_tuning_set",
@@ -171,6 +185,7 @@ EXPORTED_SYMBOLS = [
     "pb200_execute_distinct", "pb200h_execute_distinct",
     "pb200_execute_args", "pb200h_execute_args", "pb200_result_histogram", "pb200_result_moments",
     "pb200_segment_derive_column", "pb200h_segment_derive",
+    "pb200h_startree_build", "pb200h_startree_get",
 ]
 
 _LIB = None
@@ -271,6 +286,8 @@ def load() -> C.CDLL:
     L.pb200_segment_local_ids.argtypes = [vp, i32, vp, i64]
     L.pb200_segment_derive_column.argtypes = [vp, vp, i32, i32, C.POINTER(TransformOp), C.POINTER(i32)]
     L.pb200h_segment_derive.argtypes = [vp, vp, C.c_char_p, C.POINTER(i32)]
+    L.pb200h_startree_build.argtypes = [vp, vp, C.POINTER(HStarTreeConfig), C.POINTER(HStarTreeBuildInfo)]
+    L.pb200h_startree_get.argtypes = [vp, i32, C.POINTER(vp), C.POINTER(C.c_uint64), C.POINTER(vp)]
     _LIB = L
     return L
 

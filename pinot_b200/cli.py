@@ -116,11 +116,19 @@ def main(argv=None) -> int:
     ap.add_argument("--merge-on-device", action="store_true", help="bind the segments to one dictionary domain and combine on the GPU")
     ap.add_argument("--num-groups-limit", type=int, default=100_000)
     ap.add_argument("--json", action="store_true", help="print one JSON object instead of a table")
+    ap.add_argument("--star-tree", action="append", default=[], metavar="JSON",
+                    help="a StarTreeIndexConfig (an entry of the table config's starTreeIndexConfigs): build that tree on "
+                         "the device on every loaded segment (repeatable)")
     args = ap.parse_args(argv)
+    from .plan_maker import parse_star_tree_config
+    try:
+        args.star_tree = [parse_star_tree_config(c) for c in args.star_tree]
+    except ValueError as e:
+        ap.error(str(e))
 
     from . import sql
     from ._lib import Pb200Error
-    from .plan_maker import B200Context, B200PlanMaker, DictionaryDomain, IndexSegment
+    from .plan_maker import B200Context, B200PlanMaker, DictionaryDomain
 
     if sql.is_distinct(args.sql):
         return _distinct(args, sql.parse_distinct(args.sql))
@@ -131,7 +139,7 @@ def main(argv=None) -> int:
     segments, domain = [], None
     try:
         for d in args.segment_dir:
-            segments.append(IndexSegment.load(ctx, d))
+            segments.append(_load(ctx, d, args.star_tree))
         pm = B200PlanMaker(ctx)
         try:
             if args.merge_on_device and len(segments) > 1:
@@ -172,17 +180,30 @@ def main(argv=None) -> int:
         ctx.close()
 
 
+def _load(ctx, index_dir, star_trees):
+    """A segment directory in HBM, with the configured star-trees built on the device."""
+    from .plan_maker import IndexSegment
+    seg = IndexSegment.load(ctx, index_dir)
+    try:
+        for cfg in star_trees:
+            seg.build_star_tree(**cfg)
+    except BaseException:
+        seg.destroy()
+        raise
+    return seg
+
+
 def _selection(args, query) -> int:
     """SELECT columns ... LIMIT n: one device submission, segments taken in the order given (their dictionaries may
     differ: values are decoded per row's segment)."""
     from ._lib import Pb200Error
-    from .plan_maker import B200Context, B200PlanMaker, IndexSegment
+    from .plan_maker import B200Context, B200PlanMaker
 
     ctx = B200Context(args.device)
     segments = []
     try:
         for d in args.segment_dir:
-            segments.append(IndexSegment.load(ctx, d))
+            segments.append(_load(ctx, d, args.star_tree))
         try:
             block = B200PlanMaker(ctx).execute_selection(segments, query, merge=True)
         except Pb200Error as e:
@@ -209,13 +230,13 @@ def _distinct(args, query) -> int:
     """SELECT DISTINCT columns ... LIMIT n.  --merge-on-device: the segments are bound to one domain over the DISTINCT
     columns and answered in one merged call; otherwise one per-segment call, merged by value (merge_distinct_blocks)."""
     from ._lib import Pb200Error
-    from .plan_maker import B200Context, B200PlanMaker, DictionaryDomain, IndexSegment, merge_distinct_blocks
+    from .plan_maker import B200Context, B200PlanMaker, DictionaryDomain, merge_distinct_blocks
 
     ctx = B200Context(args.device)
     segments, domain = [], None
     try:
         for d in args.segment_dir:
-            segments.append(IndexSegment.load(ctx, d))
+            segments.append(_load(ctx, d, args.star_tree))
         pm = B200PlanMaker(ctx)
         try:
             if args.merge_on_device and len(segments) > 1:

@@ -21,6 +21,7 @@
 
 #include "host_internal.h"
 #include "../pb200_order.h"
+#include "../pb200_startree_build.h"
 
 using pb200::set_error;
 
@@ -262,6 +263,129 @@ extern "C" int32_t pb200h_startree_attach(pb200_ctx* ctx, pb200h_segment* seg, c
   if (rc) return rc;
   st->star_segment = star;
   seg->star_trees.push_back(std::move(st));
+  return PB200_OK;
+}
+
+extern "C" int32_t pb200h_startree_build(pb200_ctx* ctx, pb200h_segment* seg, const pb200h_startree_config* cfg,
+                                         pb200h_startree_build_info* info) {
+  // the configuration first: these refusals need no segment
+  if (!cfg || cfg->num_dimensions < 1 || !cfg->dimensions) { set_error("star-tree config: empty dimensionsSplitOrder"); return PB200_E_INVALID; }
+  const int D = cfg->num_dimensions, M = cfg->num_pairs;
+  if (D > 30) { set_error("star-tree config: %d dimensions, at most 30 are supported", D); return PB200_E_UNSUPPORTED; }
+  std::set<std::string> split;
+  for (int j = 0; j < D; j++) {
+    if (!cfg->dimensions[j]) { set_error("star-tree config: dimension %d has no name", j); return PB200_E_INVALID; }
+    if (!split.insert(cfg->dimensions[j]).second) { set_error("star-tree config: dimension '%s' repeated in the split order", cfg->dimensions[j]); return PB200_E_INVALID; }
+  }
+  std::vector<char> skip(D, 0);
+  if (cfg->num_skip_star < 0 || (cfg->num_skip_star > 0 && !cfg->skip_star)) { set_error("star-tree config: bad skipStarNodeCreationForDimensions"); return PB200_E_INVALID; }
+  for (int s = 0; s < cfg->num_skip_star; s++) {
+    int j = 0;
+    while (j < D && !(cfg->skip_star[s] && strcmp(cfg->skip_star[s], cfg->dimensions[j]) == 0)) j++;
+    if (j == D) { set_error("star-tree config: skip-star dimension '%s' is not in the split order", cfg->skip_star[s] ? cfg->skip_star[s] : "(null)"); return PB200_E_INVALID; }
+    skip[j] = 1;
+  }
+  if (cfg->max_leaf_records < 1) { set_error("star-tree config: maxLeafRecords %d < 1", cfg->max_leaf_records); return PB200_E_INVALID; }
+  if (M < 1 || !cfg->pairs) { set_error("star-tree config: no function-column pairs"); return PB200_E_INVALID; }
+  for (int m = 0; m < M; m++) {
+    const pb200h_agg& p = cfg->pairs[m];
+    if (p.function != PB200_AGG_COUNT && p.function != PB200_AGG_SUM && p.function != PB200_AGG_MIN && p.function != PB200_AGG_MAX) {
+      set_error("function-column pair %d: function %d has no star-tree metric here (COUNT, SUM, MIN, MAX)", m, p.function); return PB200_E_UNSUPPORTED;
+    }
+    if (p.function == PB200_AGG_COUNT ? (p.column && strcmp(p.column, "*") != 0) : !p.column) {
+      set_error("function-column pair %d: COUNT takes '*', SUM / MIN / MAX a column", m); return PB200_E_INVALID;
+    }
+  }
+  if (!ctx || !seg || !seg->dev) { set_error("invalid argument to pb200h_startree_build"); return PB200_E_INVALID; }
+  if (seg->dev->domain) { set_error("segment is bound to a dictionary domain: star-tree dimension ids would not match"); return PB200_E_UNSUPPORTED; }
+  if (seg->num_docs <= 0) { set_error("segment '%s' has no docs", seg->name.c_str()); return PB200_E_UNSUPPORTED; }
+  pb200::StarBuildSpec spec;
+  spec.skip_star = skip;
+  spec.max_leaf_records = cfg->max_leaf_records;
+  std::unique_ptr<StarTreeIndex> st(new StarTreeIndex());
+  for (int j = 0; j < D; j++) {
+    const int bc = seg->column_index(cfg->dimensions[j]);
+    if (bc < 0) { set_error("star-tree dimension '%s': no such column", cfg->dimensions[j]); return PB200_E_INVALID; }
+    if (seg->cols[bc].derived) { set_error("star-tree dimension '%s' is a derived column", cfg->dimensions[j]); return PB200_E_UNSUPPORTED; }
+    const pb200::DeviceColumn& dc = seg->dev->cols[bc];
+    if (!seg->cols[bc].has_dictionary || dc.fwd_kind != PB200_FWD_DICT_FIXEDBIT || dc.bits > 31) {
+      set_error("star-tree dimension '%s' has no dictIds (a raw column streamed as 32-bit values)", cfg->dimensions[j]); return PB200_E_UNSUPPORTED;
+    }
+    spec.dim_cols.push_back(bc);
+    st->dim_base_col.push_back(bc);
+  }
+  std::vector<std::string> metric_names;
+  for (int m = 0; m < M; m++) {
+    const pb200h_agg& p = cfg->pairs[m];
+    int bc = -1;
+    if (p.function != PB200_AGG_COUNT) {
+      bc = seg->column_index(p.column);
+      if (bc < 0) { set_error("function-column pair %d: no column '%s'", m, p.column); return PB200_E_INVALID; }
+      if (seg->cols[bc].derived) { set_error("function-column pair %d: '%s' is a derived column", m, p.column); return PB200_E_UNSUPPORTED; }
+      if (seg->cols[bc].data_type == PB200_STRING) { set_error("function-column pair %d: '%s' is a STRING column", m, p.column); return PB200_E_UNSUPPORTED; }
+    }
+    spec.metric_fn.push_back(p.function);
+    spec.metric_col.push_back(bc);
+    st->metric_fn.push_back(p.function);
+    st->metric_base_col.push_back(bc);
+    const char* fn = p.function == PB200_AGG_COUNT ? "count" : p.function == PB200_AGG_SUM ? "sum" : p.function == PB200_AGG_MIN ? "min" : "max";
+    metric_names.push_back(std::string(fn) + "__" + (bc < 0 ? "*" : p.column));
+  }
+  pb200::StarBuildResult res;
+  if (int rc = pb200::startree_build(ctx, seg->dev, spec, &res)) return rc;
+  // the star docs: the host side of their segment (dimensions keep the base columns' dictionaries)
+  std::unique_ptr<pb200h_segment> docs(new pb200h_segment());
+  docs->ctx = ctx; docs->dev = res.docs; docs->name = seg->name + "$startree"; docs->num_docs = res.docs->num_docs;
+  docs->cols.reserve((size_t)D + M + PB200_MAX_DERIVED_COLUMNS);
+  for (int j = 0; j < D; j++) {
+    HostColumn h = seg->cols[spec.dim_cols[j]];
+    h.bits = res.docs->cols[j].bits; h.is_sorted = 0; h.has_inverted = false; h.sorted_idx.clear();
+    docs->cols.push_back(std::move(h));
+  }
+  for (int m = 0; m < M; m++) {
+    const pb200::DeviceColumn& dc = res.docs->cols[D + m];
+    HostColumn h;
+    h.name = metric_names[m];
+    h.data_type = dc.stored_type; h.has_dictionary = 1; h.bits = dc.bits; h.cardinality = dc.cardinality; h.entry_bytes = 8;
+    h.dict = dc.dict_be;
+    docs->cols.push_back(std::move(h));
+  }
+  docs->num_stored = D + M;
+  docs->published.store(D + M, std::memory_order_release);
+  st->star_segment = docs.release();
+  st->num_docs = st->star_segment->num_docs;
+  // the tree: OffHeapStarTree layout, read back by the same parser as an attached tree
+  std::vector<unsigned char> b(20);
+  auto put32 = [&](size_t at, uint32_t v) { for (int k = 0; k < 4; k++) b[at + k] = (unsigned char)(v >> (8 * k)); };
+  auto app32 = [&](uint32_t v) { b.resize(b.size() + 4); put32(b.size() - 4, v); };
+  const uint64_t magic = 0xBADDA55B00DAD00Dull;
+  put32(0, (uint32_t)magic); put32(4, (uint32_t)(magic >> 32)); put32(8, 1); put32(16, (uint32_t)D);
+  for (int j = 0; j < D; j++) {
+    const size_t len = strlen(cfg->dimensions[j]);
+    app32((uint32_t)j); app32((uint32_t)len);
+    b.insert(b.end(), cfg->dimensions[j], cfg->dimensions[j] + len);
+  }
+  const int num_nodes = (int)(res.nodes.size() / 7);
+  app32((uint32_t)num_nodes);
+  put32(12, (uint32_t)b.size());
+  for (int32_t v : res.nodes) app32((uint32_t)v);
+  if (!st->tree.parse(b.data(), b.size())) { set_error("star-tree build produced a tree the reader refuses"); return PB200_E_INVALID; }
+  if (info) {
+    memset(info, 0, sizeof *info);
+    info->num_star_docs = st->num_docs; info->num_base_docs = res.num_base_docs; info->num_nodes = num_nodes;
+    for (int p = 0; p < 4; p++) info->phase_ms[p] = res.ms[p];
+  }
+  seg->star_trees.push_back(std::move(st));
+  return PB200_OK;
+}
+
+extern "C" int32_t pb200h_startree_get(const pb200h_segment* seg, int32_t index, const void** tree, uint64_t* tree_bytes,
+                                       pb200h_segment** star_docs) {
+  if (!seg || index < 0 || index >= (int)seg->star_trees.size()) { set_error("segment has no star-tree %d", index); return PB200_E_INVALID; }
+  const StarTreeIndex& st = *seg->star_trees[index];
+  if (tree) *tree = st.tree.bytes.data();
+  if (tree_bytes) *tree_bytes = st.tree.bytes.size();
+  if (star_docs) *star_docs = st.star_segment;
   return PB200_OK;
 }
 

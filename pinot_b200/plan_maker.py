@@ -16,6 +16,7 @@ marshals.  There is no CPU fallback: queries outside the accelerated set raise `
 from __future__ import annotations
 
 import ctypes as C
+import json
 import math
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional, Sequence, Tuple
@@ -60,6 +61,60 @@ class B200Context:
 
 def _ptr(a: Optional[np.ndarray]):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
+
+
+def star_tree_config(dimensions: Sequence[str], function_pairs: Sequence[tuple], max_leaf_records: int = 10000,
+                     skip_star_for: Sequence[str] = ()):
+    """(pb200h_startree_config, the objects it points into).  Functions are upper-cased; one the library has no code
+    for is passed as -1, which the library refuses as unsupported."""
+    dims = [d.encode() for d in dimensions]
+    skip = [d.encode() for d in skip_star_for]
+    pairs = (_lib.HAgg * max(len(function_pairs), 1))()
+    names = []
+    for i, (fn, col) in enumerate(function_pairs):
+        names.append(None if col is None else str(col).encode())
+        pairs[i] = _lib.HAgg(_lib.AGG_CODES.get(str(fn).upper(), -1), names[-1])
+    dim_arr = (C.c_char_p * max(len(dims), 1))(*dims)
+    skip_arr = (C.c_char_p * max(len(skip), 1))(*skip)
+    cfg = _lib.HStarTreeConfig(len(dims), dim_arr, len(skip), skip_arr if skip else None, len(function_pairs), pairs,
+                               int(max_leaf_records))
+    return cfg, (dims, skip, names, pairs, dim_arr, skip_arr)
+
+
+def parse_star_tree_config(config) -> Dict[str, object]:
+    """One StarTreeIndexConfig of a table config (JSON text or a dict) -> the keyword arguments of
+    IndexSegment.build_star_tree.  Pairs come from "functionColumnPairs" ("SUM__m", "COUNT__*") and
+    "aggregationConfigs" ([{"columnName": "m", "aggregationFunction": "SUM"}]); "maxLeafRecords" defaults to 10000."""
+    if isinstance(config, str):
+        try:
+            config = json.loads(config)
+        except json.JSONDecodeError as e:
+            raise ValueError(f"star-tree config is not JSON: {e}") from None
+    if not isinstance(config, dict):
+        raise ValueError("star-tree config must be a JSON object")
+    dims = config.get("dimensionsSplitOrder")
+    if not isinstance(dims, list) or not dims or not all(isinstance(d, str) for d in dims):
+        raise ValueError("star-tree config: dimensionsSplitOrder must be a non-empty list of column names")
+    skip = config.get("skipStarNodeCreationForDimensions") or []
+    if not isinstance(skip, list) or not all(isinstance(d, str) for d in skip):
+        raise ValueError("star-tree config: skipStarNodeCreationForDimensions must be a list of column names")
+    pairs = []
+    for p in config.get("functionColumnPairs") or []:
+        if not isinstance(p, str) or "__" not in p:
+            raise ValueError(f"star-tree config: function-column pair {p!r} is not FUNCTION__column")
+        fn, col = p.split("__", 1)
+        pairs.append((fn.upper(), None if col == "*" else col))
+    for a in config.get("aggregationConfigs") or []:
+        if not isinstance(a, dict) or "aggregationFunction" not in a or "columnName" not in a:
+            raise ValueError(f"star-tree config: aggregation config {a!r} needs columnName and aggregationFunction")
+        pairs.append((str(a["aggregationFunction"]).upper(), None if a["columnName"] == "*" else a["columnName"]))
+    if not pairs:
+        raise ValueError("star-tree config: no functionColumnPairs / aggregationConfigs")
+    leaf = config.get("maxLeafRecords", 10000)
+    if not isinstance(leaf, int) or isinstance(leaf, bool):
+        raise ValueError("star-tree config: maxLeafRecords must be an integer")
+    return {"dimensions": dims, "function_pairs": list(dict.fromkeys(pairs)), "max_leaf_records": leaf,
+            "skip_star_for": skip}
 
 
 class IndexSegment:
@@ -130,6 +185,48 @@ class IndexSegment:
             arr[i] = _lib.HStarMetric(_lib.AGG_CODES[fn], 0, nm, buf.ctypes.data, len(buf))
         _lib.check(self.ctx.lib.pb200h_startree_attach(self.ctx.handle, self.handle, _ptr(tree), len(tree), num_star_docs,
                                                        len(dimensions), names, fwd, sizes, len(metrics), arr))
+
+    def build_star_tree(self, dimensions: Sequence[str], function_pairs: Sequence[tuple], max_leaf_records: int = 10000,
+                        skip_star_for: Sequence[str] = ()) -> Dict[str, object]:
+        """Builds one star-tree of this segment on the device (pb200h_startree_build) and attaches it: `dimensions` =
+        dimensionsSplitOrder, `function_pairs` = [(function, column)] with COUNT's column None or "*".  Returns the star
+        docs, base docs and nodes of the tree and the milliseconds of each build phase."""
+        cfg, _keep = star_tree_config(dimensions, function_pairs, max_leaf_records, skip_star_for)
+        info = _lib.HStarTreeBuildInfo()
+        _lib.check(self.ctx.lib.pb200h_startree_build(self.ctx.handle, self.handle, C.byref(cfg), C.byref(info)))
+        return {"num_star_docs": int(info.num_star_docs), "num_base_docs": int(info.num_base_docs),
+                "num_nodes": int(info.num_nodes), "phase_ms": dict(zip(_lib.STAR_BUILD_PHASES, list(info.phase_ms)))}
+
+    def num_star_trees(self) -> int:
+        """Star-trees of this segment, built or attached."""
+        n = 0
+        while self.ctx.lib.pb200h_startree_get(self.handle, n, None, None, None) == _lib.PB200_OK:
+            n += 1
+        return n
+
+    def read_star_tree(self, index: int) -> Dict[str, object]:
+        """The index-th star-tree, built or attached, read back: the OffHeapStarTree bytes, and per column of its star
+        docs (dimensions: dictIds of the base dictionaries; count__*: int64; sum__m / min__m / max__m: float64) the
+        values of every star doc."""
+        L = self.ctx.lib
+        tree, size, docs = C.c_void_p(), C.c_uint64(), C.c_void_p()
+        _lib.check(L.pb200h_startree_get(self.handle, index, C.byref(tree), C.byref(size), C.byref(docs)))
+        out = {"tree": np.ctypeslib.as_array(C.cast(tree, C.POINTER(C.c_uint8)), shape=(size.value,)).copy(), "columns": {}}
+        seg = IndexSegment(self.ctx, docs, self.name + "$startree")  # owned by this segment: never destroyed here
+        out["num_docs"] = seg.num_docs
+        num_dims = int(np.frombuffer(out["tree"][16:20].tobytes(), dtype="<i4")[0])  # columns: dimensions, then metrics
+        for i, name in enumerate(seg.column_names):
+            info = seg.column_info(name)
+            fwd = seg.read_index(name, "fwd")
+            n, bits = seg.num_docs, info["bits"]
+            bitstream = np.unpackbits(fwd)[: n * bits].reshape(n, bits).astype(np.int64)
+            ids = bitstream @ (1 << np.arange(bits - 1, -1, -1, dtype=np.int64))
+            if i >= num_dims:
+                dtype = ">i8" if info["data_type"] == _lib.LONG else ">f8"
+                out["columns"][name] = np.frombuffer(seg.read_index(name, "dict").tobytes(), dtype=dtype).astype(dtype[1:])[ids]
+            else:
+                out["columns"][name] = ids.astype(np.int32)
+        return out
 
     # ---- accessors ----------------------------------------------------------------------------------------------
     def column_index(self, name: str) -> int:
