@@ -115,6 +115,8 @@ struct StarTreeIndex {
   std::vector<int> dim_base_col;     // star dimension -> column index in the base segment
   std::vector<int> metric_fn;        // function of each function-column pair
   std::vector<int> metric_base_col;  // its column in the base segment (-1 for count__*)
+  std::vector<int> metric_limb_col;  // built trees, SUM over INT: the first of its three limb columns in the star segment
+                                     // (pb200_startree_build.h StarBuildResult::limb_col); -1 otherwise
   int num_docs = 0;
   pb200h_segment* star_segment = nullptr;  // columns: dimensions..., metrics...
   // Traversal results by (predicate dictId sets per dimension, group-by mask): the BFS over a tree with 10^5..10^6 nodes

@@ -354,6 +354,7 @@ extern "C" int32_t pb200h_startree_build(pb200_ctx* ctx, pb200h_segment* seg, co
   docs->published.store(D + M, std::memory_order_release);
   st->star_segment = docs.release();
   st->num_docs = st->star_segment->num_docs;
+  st->metric_limb_col = res.limb_col;
   // the tree: OffHeapStarTree layout, read back by the same parser as an attached tree
   std::vector<unsigned char> b(20);
   auto put32 = [&](size_t at, uint32_t v) { for (int k = 0; k < 4; k++) b[at + k] = (unsigned char)(v >> (8 * k)); };
@@ -433,31 +434,54 @@ int try_star_tree(pb200_ctx* ctx, const pb200h_segment& seg, const StarTreeIndex
     gb_cols.push_back(d);  // star segment column index == dimension index
   }
   // ---- aggregations -> function-column pairs ----
-  auto metric_col = [&](int fn, int base_col) { for (size_t m = 0; m < st.metric_fn.size(); m++) if (st.metric_fn[m] == fn && st.metric_base_col[m] == base_col) return ndims + (int)m; return -1; };
+  auto metric_of = [&](int fn, int base_col) { for (size_t m = 0; m < st.metric_fn.size(); m++) if (st.metric_fn[m] == fn && st.metric_base_col[m] == base_col) return (int)m; return -1; };
+  // internal aggregations over star segment columns, each once however many of the query's aggregations read it
   std::vector<pb200_agg> star_aggs;
-  struct Map { int fn; int a0, a1; };
+  auto internal = [&](int fn, int col) {
+    for (size_t i = 0; i < star_aggs.size(); i++) if (star_aggs[i].function == fn && star_aggs[i].column == col) return (int)i;
+    star_aggs.push_back({fn, col});
+    return (int)star_aggs.size() - 1;
+  };
+  // a0: the value (MIN / MAX / a SUM of the metric's column), a1: AVG's count, limb: the first of three consecutive
+  // limb sums that replace a0 for a built tree's INT SUM (the exact sum, rounded once)
+  struct Map { int fn; int a0, a1, limb; };
   std::vector<Map> mapping;
   for (int a = 0; a < q.num_aggs; a++) {
     const int fn = q.aggs[a].function;
-    Map m{fn, -1, -1};
+    Map m{fn, -1, -1, -1};
     if (fn == PB200_AGG_COUNT) {
-      int c = metric_col(PB200_AGG_COUNT, -1);
+      const int c = metric_of(PB200_AGG_COUNT, -1);
       if (c < 0) return 0;
-      m.a0 = (int)star_aggs.size(); star_aggs.push_back({PB200_AGG_SUM, c});
+      m.a0 = internal(PB200_AGG_SUM, ndims + c);
     } else if (fn == PB200_AGG_SUM || fn == PB200_AGG_MIN || fn == PB200_AGG_MAX || fn == PB200_AGG_AVG) {
       const int bc = seg.column_index(q.aggs[a].column);
-      int c = metric_col(fn == PB200_AGG_AVG ? PB200_AGG_SUM : fn, bc);
-      if (bc < 0 || c < 0) return 0;
-      m.a0 = (int)star_aggs.size(); star_aggs.push_back({fn == PB200_AGG_AVG ? PB200_AGG_SUM : fn, c});
+      const int sfn = fn == PB200_AGG_AVG ? PB200_AGG_SUM : fn;
+      const int c = bc < 0 ? -1 : metric_of(sfn, bc);
+      if (c < 0) return 0;
+      const int limb = sfn == PB200_AGG_SUM && c < (int)st.metric_limb_col.size() ? st.metric_limb_col[c] : -1;
+      if (limb >= 0) {   // the three are only ever added together, so they stay consecutive
+        m.limb = internal(PB200_AGG_SUM, limb);
+        internal(PB200_AGG_SUM, limb + 1);
+        internal(PB200_AGG_SUM, limb + 2);
+      } else {
+        m.a0 = internal(sfn, ndims + c);
+      }
       if (fn == PB200_AGG_AVG) {
-        int cc = metric_col(PB200_AGG_COUNT, -1);
+        const int cc = metric_of(PB200_AGG_COUNT, -1);
         if (cc < 0) return 0;
-        m.a1 = (int)star_aggs.size(); star_aggs.push_back({PB200_AGG_SUM, cc});
+        m.a1 = internal(PB200_AGG_SUM, ndims + cc);
       }
     } else return 0;
     mapping.push_back(m);
   }
   if ((int)star_aggs.size() > 6) return 0;
+  // a limb-summed INT SUM: l2 * 2^42 + l1 * 2^21 + l0 in 128 bits (each limb sum is an integer below 2^52, exact in
+  // double).  The total is the rows' exact sum, |S| <= 2^31 rows x 2^31, so it fits int64 and is rounded to double
+  // once: float(exact sum), as the scan returns it
+  auto limb_sum = [](const double* l0, const double* l1, const double* l2, size_t r) {
+    const __int128 s = (__int128)(long long)l2[r] * ((__int128)1 << 42) + (__int128)(long long)l1[r] * (1 << 21) + (long long)l0[r];
+    return (double)(long long)s;
+  };
 
   // ---- traversal -> doc mask (cached per predicate set) ----
   const int sdocs = st.num_docs;
@@ -530,6 +554,7 @@ int try_star_tree(pb200_ctx* ctx, const pb200h_segment& seg, const StarTreeIndex
   pb200_segment* dev = st.star_segment->dev;
   pb200_result* sr = nullptr;
   int rc = pb200_execute(ctx, &dq, &dev, 1, &sr);
+  if (rc == PB200_E_UNSUPPORTED) return 0;   // the star docs' row is too wide for the scan (limb columns): scan the base
   if (rc) return rc;
   // ---- back to the query's own aggregation list ----
   std::unique_ptr<pb200_result> R(new pb200_result());
@@ -545,9 +570,21 @@ int try_star_tree(pb200_ctx* ctx, const pb200h_segment& seg, const StarTreeIndex
     const pb200_result::View& sv = sr->view;
     pb200_result::View& v = R->view;
     v.block = sv.block; v.rows = sv.rows; v.keys = sv.keys;
+    std::vector<double> zeros;
     for (int a = 0; a < q.num_aggs; a++) {
       const Map& m = mapping[a];
-      v.dbl[a] = sv.dbl[m.a0];
+      if (m.limb >= 0) {   // a column of its own, owned by the result
+        const double* l[3];
+        for (int k = 0; k < 3; k++) {
+          l[k] = sv.dbl[m.limb + k];
+          if (!l[k]) { zeros.assign(rows, 0.0); l[k] = zeros.data(); }
+        }
+        R->dbl[a].resize(rows);
+        for (size_t r = 0; r < rows; r++) R->dbl[a][r] = limb_sum(l[0], l[1], l[2], r);
+        v.dbl[a] = R->dbl[a].data();
+      } else {
+        v.dbl[a] = sv.dbl[m.a0];
+      }
       v.ids[a] = nullptr;   // all -1: star-tree metrics are raw values
       const int src = m.fn == PB200_AGG_COUNT ? m.a0 : m.fn == PB200_AGG_AVG ? m.a1 : -1;
       if (src >= 0 && sv.dbl[src]) {
@@ -564,7 +601,12 @@ int try_star_tree(pb200_ctx* ctx, const pb200h_segment& seg, const StarTreeIndex
     R->keys = sr->keys;
     for (int a = 0; a < q.num_aggs; a++) {
       const Map& m = mapping[a];
-      R->dbl[a] = sr->dbl[m.a0];
+      if (m.limb >= 0) {
+        R->dbl[a].resize(rows);
+        for (size_t r = 0; r < rows; r++) R->dbl[a][r] = limb_sum(sr->dbl[m.limb].data(), sr->dbl[m.limb + 1].data(), sr->dbl[m.limb + 2].data(), r);
+      } else {
+        R->dbl[a] = sr->dbl[m.a0];
+      }
       R->lng[a].assign(rows, 0);
       R->ids[a].assign(rows, -1);
       for (size_t r = 0; r < rows; r++) {

@@ -185,6 +185,14 @@ __global__ void metric_key_kernel(const uint64_t* __restrict__ acc, int kind, lo
   }
 }
 
+// limb k of an exact INT sum x (|x| < 2^62): x = l2 * 2^42 + l1 * 2^21 + l0, l0 and l1 in [0, 2^21), l2 signed
+__global__ void limb_kernel(const uint64_t* __restrict__ acc, int k, long long n, uint32_t* __restrict__ out) {
+  PB200_GRID_LOOP(i, n) {
+    const long long x = (long long)acc[i];
+    out[i] = k == 2 ? (uint32_t)(int32_t)(x >> 42) : (uint32_t)((x >> (21 * k)) & 0x1FFFFF);
+  }
+}
+
 __global__ void key_flag_kernel(const uint64_t* __restrict__ key, long long n, uint32_t* __restrict__ flags) {
   PB200_GRID_LOOP(i, n) flags[i] = i > 0 && key[i] != key[i - 1];
 }
@@ -395,7 +403,7 @@ inline void put_be(unsigned char* p, uint64_t v, int w) { for (int b = 0; b < w;
 // star docs -> device segment columns: dimensions packed at their base bits sharing the base dictionaries, metrics
 // dictionary-encoded (sort -> flags -> scan -> rank, as derived columns are)
 int encode_segment(pb200_ctx* ctx, cudaStream_t st, const pb200_segment* seg, const StarBuildSpec& spec, Builder& b,
-                   pb200_segment** out) {
+                   pb200_segment** out, std::vector<int>* limb_col) {
   const long long T = b.total;
   const int blocks = ctx->sm_count * 8;
   std::unique_ptr<pb200_segment> s(new pb200_segment());
@@ -403,8 +411,7 @@ int encode_segment(pb200_ctx* ctx, cudaStream_t st, const pb200_segment* seg, co
   s->ctx = ctx;
   s->name = seg->name + "$startree";
   s->num_docs = (int)T;
-  s->cols.reserve((size_t)D + M + PB200_MAX_DERIVED_COLUMNS);
-  s->num_stored = D + M;
+  s->cols.reserve((size_t)D + 4 * M + PB200_MAX_DERIVED_COLUMNS);
   struct FreeOnFail {
     pb200_ctx* ctx; cudaStream_t st; pb200_segment* s; bool armed = true;
     ~FreeOnFail() {
@@ -490,8 +497,25 @@ int encode_segment(pb200_ctx* ctx, cudaStream_t st, const pb200_segment* seg, co
     c.dict_hash = dictionary_hash(c.stored_type, 8, card, c.dict_be.data());
     s->device_bytes += (int64_t)c.dict_host.size();
   }
+  // an INT SUM's exact sums, also as three raw INT limb columns (see StarBuildResult::limb_col)
+  limb_col->assign(M, -1);
+  for (int m = 0; m < M; m++) {
+    if (spec.metric_fn[m] != PB200_AGG_SUM || b.acc_[m] != ACC_I64) continue;
+    (*limb_col)[m] = (int)s->cols.size();
+    for (int k = 0; k < 3; k++) {
+      limb_kernel<<<grid, kThreads, 0, st>>>(b.met[m], k, T, (uint32_t*)ids.p);
+      PB200_CUDA(cudaGetLastError());
+      s->cols.emplace_back();
+      DeviceColumn& c = s->cols.back();
+      c.stored_type = PB200_INT;
+      if (int r2 = pack((const uint32_t*)ids.p, 32, c)) return r2;
+      c.fwd_kind = PB200_FWD_RAW_FIXEDBYTE;   // bits 32 and no dictionary: the scan reads signed words (VAL_RAW_I32)
+    }
+  }
+  const int ncols = (int)s->cols.size();
+  s->num_stored = ncols;
   PB200_CUDA(cudaStreamSynchronize(st));
-  s->published.store(D + M, std::memory_order_release);
+  s->published.store(ncols, std::memory_order_release);
   guard.armed = false;
   *out = s.release();
   return PB200_OK;
@@ -635,7 +659,7 @@ int startree_build(pb200_ctx* ctx, const pb200_segment* seg, const StarBuildSpec
 
   // ---- 4. the star docs as a device segment --------------------------------------------------------------------
   pb200_segment* docs = nullptr;
-  if (int rc = encode_segment(ctx, st, seg, spec, b, &docs)) return rc;
+  if (int rc = encode_segment(ctx, st, seg, spec, b, &docs, &out->limb_col)) return rc;
   out->ms[STAR_PHASE_ENCODE] = host_ms() - t3;
   out->nodes.resize(7 * nodes.size());
   for (size_t i = 0; i < nodes.size(); i++) {

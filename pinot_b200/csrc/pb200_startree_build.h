@@ -23,7 +23,12 @@ struct StarBuildResult {
   std::vector<int32_t> nodes;       // 7 ints per node, breadth first: dim, value, start, end, agg, first child, last child
   long long num_base_docs = 0;
   pb200_segment* docs = nullptr;    // the star docs: dimensions (dictIds of the base dictionaries), then the metrics
-                                    // (count__* LONG, the others DOUBLE, dictionary encoded)
+                                    // (count__* LONG, the others DOUBLE, dictionary encoded), then hidden limb columns
+  // Per metric: -1, or for SUM over an INT column the first of three raw INT columns of `docs` that hold each star doc's
+  // exact sum x as limbs, x = l2 * 2^42 + l1 * 2^21 + l0 (l0, l1 in [0, 2^21)).  A query's limb sums stay below 2^52
+  // in magnitude for any number of star docs, so they come back from the scan exact in double; the DOUBLE sum__ column
+  // holds x rounded, and a sum of those would round once per star doc.
+  std::vector<int> limb_col;
   double ms[STAR_PHASES] = {};
 };
 
