@@ -133,6 +133,10 @@ int plan_selection(const Tuning& tune, DeviceLimits lim, const pb200_query* filt
 // Segments a prefix pass must scan again over all their docs: prefix shorter than the segment and fewer than `limit`
 // matches in it (matches[s] = matched docs of segment s in the prefix).
 std::vector<int> selection_rescan(const SelectionPlan& p, pb200_segment* const* segments, const std::vector<long long>& matches);
+// A full pass over segments `rescan` (selection or DISTINCT): the filter-only query `q` with a per-segment filter cut
+// down to those segments' trees (held in `filter`), and the segments in the same order.
+struct Rescan { pb200_query query; std::vector<pb200_segment*> segs; std::vector<pb200_filter_node> filter; };
+Rescan rescan_query(const pb200_query& q, pb200_segment* const* segments, const std::vector<int>& rescan);
 
 // ---- DISTINCT (pb200_execute_distinct): a selection scan, then a dense first-occurrence table per result ----
 constexpr int kMaxDistinctColumns = 8;                 // the group-by limit

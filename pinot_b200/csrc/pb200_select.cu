@@ -282,18 +282,9 @@ extern "C" int32_t pb200_execute_selection(pb200_ctx* ctx, const pb200_query* fi
   }
   const std::vector<int> rescan = selection_rescan(p1, segments, m1);
   if (!rescan.empty()) {
-    std::vector<pb200_segment*> rsegs;
-    std::vector<pb200_filter_node> rfilter;
-    pb200_query rq = *filter_only;
-    for (int s : rescan) {
-      rsegs.push_back(segments[s]);
-      if (filter_only->flags & PB200_Q_PER_SEGMENT_FILTER)
-        rfilter.insert(rfilter.end(), filter_only->filter + (size_t)s * filter_only->num_filter_nodes,
-                       filter_only->filter + (size_t)(s + 1) * filter_only->num_filter_nodes);
-    }
-    if (filter_only->flags & PB200_Q_PER_SEGMENT_FILTER) rq.filter = rfilter.data();
+    const Rescan rs = rescan_query(*filter_only, segments, rescan);
     SelectionPlan p2;
-    if (int rc = plan_selection(tune, lim, &rq, sel, rsegs.data(), (int)rsegs.size(), false, &p2)) return rc;
+    if (int rc = plan_selection(tune, lim, &rs.query, sel, rs.segs.data(), (int)rs.segs.size(), false, &p2)) return rc;
     std::vector<long long> m2;
     if (int rc = run_selection_scan(ctx, st, p2, mask2, m2, &ms)) return rc;
     for (size_t i = 0; i < rescan.size(); i++) {

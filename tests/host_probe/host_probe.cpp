@@ -3,9 +3,14 @@
 //   * pb200h::StarTree::parse / traverse   (StarTreeFilterOperator's traversal as the product runs it)
 //   * pb200h::matching_dict_ids             (PredicateEvaluator resolution: value-space predicate -> dictIds)
 //   * pb200::plan_scan                       (every decision about a scan launch, on segments built from metadata)
+//   * probe_plan_dump                        (every field of a scan, selection or DISTINCT plan as text: plan_diff.py)
 // Built by tests/test_host_logic_cpu.py with g++ against the in-tree library; nothing here ships.
+#include <algorithm>
+#include <cstdarg>
 #include <cstdint>
+#include <cstdio>
 #include <cstring>
+#include <string>
 #include <vector>
 
 #include "../../pinot_b200/csrc/host/host_internal.h"
@@ -126,7 +131,7 @@ typedef struct {
   int32_t dict_native;        // 1: the column has a device dictionary (a sentinel pointer, never dereferenced)
   int32_t dict_shared;        // dictionary of a bound domain
   int32_t has_inv;            // an inverted index whose every dictId has a non-empty posting list
-  int32_t reserved;
+  int32_t eligible;           // VAR / STDDEV limb dictionaries: -1 not prepared, 0 off the grid, 1 built (fake limbs)
   uint64_t dict_hash;
   const void* dict_host;      // native little-endian dictionary values (INT: 4 bytes each), or NULL
   uint64_t dict_host_bytes;
@@ -152,6 +157,59 @@ typedef struct {  // every field int64: tests/test_scan_plan_cpu.py mirrors this
 
 int64_t probe_plan_size(void) { return (int64_t)sizeof(probe_plan); }
 
+}  // extern "C"
+
+namespace {
+
+// Limb dictionaries are never read on the host: column k of segment s gets the fake device range
+// [kLimbBase + (s ncols + k) kLimbStride, + 3 x 2^31 u32)
+constexpr uintptr_t kLimbBase = (uintptr_t)1 << 44, kLimbStride = (uintptr_t)1 << 36;
+
+// Segments made of column metadata (cols: nseg x ncols).  Resident pointers are never dereferenced: the forward index,
+// device dictionary and inverted index of column k in segment s are words 3 (s ncols + k) + 0 / 1 / 2 of `sentinels`.
+struct ProbeSegments {
+  std::vector<uint32_t> sentinels;
+  std::vector<pb200_segment> segs;
+  std::vector<pb200_segment*> ptrs;
+  ProbeSegments(const probe_col* cols, int ncols, const int32_t* num_docs, int nseg)
+      : sentinels((size_t)3 * nseg * ncols), segs(nseg), ptrs(nseg) {
+    using namespace pb200;
+    for (int s = 0; s < nseg; s++) {
+      segs[s].num_docs = num_docs[s];
+      segs[s].cols.resize(ncols);
+      for (int k = 0; k < ncols; k++) {
+        const probe_col& p = cols[(size_t)s * ncols + k];
+        DeviceColumn& c = segs[s].cols[k];
+        uint32_t* sent = &sentinels[3 * ((size_t)s * ncols + k)];
+        c.fwd_kind = p.fwd_kind; c.stored_type = p.stored_type; c.bits = p.bits; c.cardinality = p.cardinality;
+        c.fwd = sent;
+        c.dict_native = p.dict_native ? sent + 1 : nullptr;
+        c.dict_shared = p.dict_shared != 0;
+        c.dict_hash = p.dict_hash;
+        if (p.dict_host) c.dict_host.assign((const unsigned char*)p.dict_host, (const unsigned char*)p.dict_host + p.dict_host_bytes);
+        if (p.has_inv) {
+          c.inv = (unsigned char*)(sent + 2);
+          for (int id = 0; id <= c.cardinality; id++) c.inv_offsets.push_back(4u * (c.cardinality + 1) + 8u * id);
+        }
+        if (p.eligible >= 0) {
+          c.moments->eligible = p.eligible != 0;
+          if (p.eligible) {
+            c.moments->limbs = reinterpret_cast<uint32_t*>(kLimbBase + ((size_t)s * ncols + k) * kLimbStride);
+            c.moments->entries = p.cardinality;
+          }
+          c.moments->ready.store(true);
+        }
+      }
+      ptrs[s] = &segs[s];
+    }
+  }
+  ~ProbeSegments() { for (auto& s : segs) for (auto& c : s.cols) c.moments->limbs = nullptr; }  // fake: never freed
+};
+
+}  // namespace
+
+extern "C" {
+
 // cols: nseg x ncols; knobs: nknobs pb200_tuning_set (name, value) pairs.  Returns plan_scan's status.
 int32_t probe_plan_scan(int32_t sm_count, int32_t max_smem_optin, const char* const* knob_names, const int64_t* knob_values,
                         int32_t nknobs, const pb200_query* query, const probe_col* cols, int32_t ncols, const int32_t* num_docs,
@@ -159,30 +217,9 @@ int32_t probe_plan_scan(int32_t sm_count, int32_t max_smem_optin, const char* co
   using namespace pb200;
   pb200_ctx ctx;
   for (int i = 0; i < nknobs; i++) if (int rc = pb200_tuning_set(&ctx, knob_names[i], knob_values[i])) return rc;
-  static uint32_t sentinel[4];
-  std::vector<pb200_segment> segs(nseg);
-  std::vector<pb200_segment*> ptrs(nseg);
-  for (int s = 0; s < nseg; s++) {
-    segs[s].num_docs = num_docs[s];
-    segs[s].cols.resize(ncols);
-    for (int k = 0; k < ncols; k++) {
-      const probe_col& p = cols[(size_t)s * ncols + k];
-      DeviceColumn& c = segs[s].cols[k];
-      c.fwd_kind = p.fwd_kind; c.stored_type = p.stored_type; c.bits = p.bits; c.cardinality = p.cardinality;
-      c.fwd = sentinel;
-      c.dict_native = p.dict_native ? sentinel : nullptr;
-      c.dict_shared = p.dict_shared != 0;
-      c.dict_hash = p.dict_hash;
-      if (p.dict_host) c.dict_host.assign((const unsigned char*)p.dict_host, (const unsigned char*)p.dict_host + p.dict_host_bytes);
-      if (p.has_inv) {
-        c.inv = (unsigned char*)sentinel;
-        for (int id = 0; id <= c.cardinality; id++) c.inv_offsets.push_back(4u * (c.cardinality + 1) + 8u * id);
-      }
-    }
-    ptrs[s] = &segs[s];
-  }
+  ProbeSegments ps(cols, ncols, num_docs, nseg);
   ScanPlan plan;
-  const int rc = plan_scan(ctx.tune, DeviceLimits{sm_count, max_smem_optin}, query, ptrs.data(), nseg, allow_count_carrier != 0, &plan);
+  const int rc = plan_scan(ctx.tune, DeviceLimits{sm_count, max_smem_optin}, query, ps.ptrs.data(), nseg, allow_count_carrier != 0, &plan);
   memset(out, 0, sizeof *out);
   if (rc) return rc;
   const QueryDesc& q = plan.q;
@@ -227,6 +264,165 @@ int32_t probe_plan_scan(int32_t sm_count, int32_t max_smem_optin, const char* co
     }
   }
   return PB200_OK;
+}
+
+}  // extern "C"
+
+namespace {
+
+// Text form of a plan.  A pointer is written as (range, byte offset): range 1 is the sentinels, 2 the fake limb
+// dictionaries, 3 + i the ids of filter node i of the query; so dumps taken by two processes compare byte for byte.
+struct PlanDump {
+  const ProbeSegments& ps;
+  const pb200_query* query;
+  int nnodes_total;
+  std::string out;
+
+  uint64_t token(const void* p) const {
+    const uintptr_t a = (uintptr_t)p;
+    if (!p) return 0;
+    const uintptr_t s0 = (uintptr_t)ps.sentinels.data();
+    if (a >= s0 && a < s0 + ps.sentinels.size() * 4) return 1ull << 48 | (a - s0);
+    if (a >= kLimbBase && a < kLimbBase + ps.ptrs.size() * ps.segs[0].cols.size() * kLimbStride) return 2ull << 48 | (a - kLimbBase);
+    for (int i = 0; i < nnodes_total; i++) {
+      const pb200_filter_node& n = query->filter[i];
+      const uintptr_t b = (uintptr_t)n.ids;
+      if (n.ids && a >= b && a < b + (size_t)std::max(n.num_ids, 1) * 4) return (3ull + i) << 48 | (a - b);
+    }
+    return ~0ull;   // a pointer the plan should not hold
+  }
+  void line(const char* fmt, ...) __attribute__((format(printf, 2, 3))) {
+    char buf[512];
+    va_list ap;
+    va_start(ap, fmt);
+    vsnprintf(buf, sizeof buf, fmt, ap);
+    va_end(ap);
+    out += buf;
+    out += '\n';
+  }
+  void bytes(const char* name, const void* p, size_t n) {
+    static const char* hex = "0123456789abcdef";
+    out += name;
+    out += ' ';
+    for (size_t i = 0; i < n; i++) { const unsigned char b = ((const unsigned char*)p)[i]; out += hex[b >> 4]; out += hex[b & 15]; }
+    out += '\n';
+  }
+  template <class T> void vec(const char* name, const std::vector<T>& v) {
+    out += name;
+    for (const T& x : v) { out += ' '; out += std::to_string(x); }
+    out += '\n';
+  }
+  void vec(const char* name, const std::vector<double>& v) {
+    out += name;
+    for (double x : v) { uint64_t u; memcpy(&u, &x, 8); out += ' '; out += std::to_string(u); }
+    out += '\n';
+  }
+  void vec(const char* name, const std::vector<bool>& v) { vec(name, std::vector<int>(v.begin(), v.end())); }
+
+  void scan(const pb200::ScanPlan& p) {
+    using namespace pb200;
+    bytes("q", &p.q, sizeof p.q);   // QueryDesc: integers only, no padding
+    for (size_t s = 0; s < p.segs.size(); s++) {
+      SegDesc d;                    // memset by the planner: padding included, every byte is defined
+      memcpy(&d, &p.segs[s], sizeof d);
+      for (auto& sl : d.slots) sl.data = (const uint32_t*)token(sl.data);
+      for (auto& lf : d.leaves) { lf.bits = (const uint32_t*)token(lf.bits); lf.ranges = (const int32_t*)token(lf.ranges); }
+      for (int a = 0; a < kMaxAggs; a++) {
+        d.dict[a] = (const void*)token(d.dict[a]); d.distinct_bits[a] = (uint32_t*)token(d.distinct_bits[a]);
+        d.g_isum[a] = (long long*)token(d.g_isum[a]); d.g_dsum[a] = (double*)token(d.g_dsum[a]);
+        d.g_min[a] = (uint32_t*)token(d.g_min[a]); d.g_max[a] = (uint32_t*)token(d.g_max[a]);
+      }
+      d.accum = (AggAccum*)token(d.accum); d.g_count = (unsigned long long*)token(d.g_count); d.g_seen = (uint32_t*)token(d.g_seen);
+      d.h_keys = (unsigned long long*)token(d.h_keys); d.h_ctl = (uint32_t*)token(d.h_ctl);
+      line("seg %zu", s);
+      bytes("segdesc", &d, sizeof d);
+    }
+    vec("slot_cols", p.slot_cols);
+    vec("leaf_node", p.leaf_node);
+    line("flags %d %d %d nres %d warps %d ctas %d skip %d smem %zu", p.group_by, p.merge, p.defer_finalize, p.nres, p.warps,
+         p.ctas_per_sm, p.skip_masks, p.smem_bytes);
+    line("variant %d %d %d %d %d", p.variant.warps, p.variant.group_by, p.variant.defer, p.variant.min_blocks, p.variant.spec);
+    for (const LaunchChunk& c : p.chunks) line("chunk %d %d %d %d", c.first_seg, c.num_segs, c.total_tiles, c.grid);
+    for (const LeafBuffer& b : p.leaf_buffers) {
+      uint64_t h = 1469598103934665603ull;   // FNV-1a over the LUT words
+      for (uint32_t w : b.lut) { h ^= w; h *= 1099511628211ull; }
+      line("leafbuf %d %d %d %zu lut %zu %llx src %llx %zu jobs %zu", (int)b.kind, b.seg, b.leaf, b.words, b.lut.size(),
+           (unsigned long long)h, (unsigned long long)token(b.src), b.src_words, b.jobs.size());
+      for (const DecodeJob& j : b.jobs)
+        line("job %llx %llu %llu %llx %lld", (unsigned long long)token(j.inv), j.offset, j.length, (unsigned long long)token(j.mask), j.num_docs);
+    }
+    for (const TableLayout& t : p.tables) {
+      vec("cards", t.cards); vec("mult", t.mult); vec("mult64", t.mult64);
+      line("table %d %lld %d %d %d %d %d carrier %d %d %lld rw %d flag %d tail %d elems %lld %lld %lld %lld", t.hashed, t.groups,
+           t.stride, t.need_count, t.need_seen, t.exists_min, t.exists_max, t.carrier.agg, t.carrier.shift, t.carrier.vmin,
+           t.reduce_world, t.flag_slot, t.tail_slots, t.i64_elems, t.f64_elems, t.u32max_elems, t.u32min_elems);
+      vec("index", std::vector<int>(t.index, t.index + kMaxAggs));
+      vec("dwords", std::vector<uint32_t>(t.dwords, t.dwords + kMaxAggs));
+      vec("hist_per_group", std::vector<uint32_t>(t.hist_per_group, t.hist_per_group + kMaxAggs));
+    }
+    for (const auto& v : p.distinct_words) vec("distinct_words", v);
+    vec("pct_p", p.pct_p);
+    vec("pct_rep", p.pct_rep);
+    line("num_user_aggs %d", p.num_user_aggs);
+    for (const pb200_agg& a : p.aggs) line("agg %d %d", a.function, a.column);
+    vec("mom_first", p.mom_first);
+    vec("limb", p.limb);
+    for (const auto& v : p.hist_entries) vec("hist_entries", v);
+    line("hist_total %lld", p.hist_total);
+    vec("in_filter", p.in_filter);
+    line("projected %d", p.projected);
+  }
+  void selection(const pb200::SelectionPlan& p) {
+    scan(p.scan);
+    vec("columns", p.columns); vec("kinds", p.kinds); vec("order_cols", p.order_cols); vec("order_kinds", p.order_kinds);
+    vec("order_desc", p.order_desc);
+    line("limit %lld mask_words %lld prefix %d", p.limit, p.mask_words, p.prefix);
+    vec("mask_word_off", p.mask_word_off); vec("chunk_word_off", p.chunk_word_off); vec("scan_docs", p.scan_docs);
+  }
+  void distinct(const pb200::DistinctPlan& p) {
+    selection(p.sel);
+    line("nres %d table_entries %lld", p.nres, p.table_entries);
+    for (const auto& v : p.cards) vec("cards", v);
+    for (const auto& v : p.mult) vec("mult", v);
+    vec("table_off", p.table_off); vec("table_size", p.table_size); vec("order_key", p.order_key); vec("order_desc", p.order_desc);
+  }
+};
+
+}  // namespace
+
+extern "C" {
+
+// The whole plan of one input as text into out (cap bytes); returns its length (not truncated when < cap), or a
+// negative pb200_tuning_set status.  kind 0: plan_scan (agg_args as for pb200_execute_args, may be NULL), 1:
+// plan_selection, 2: plan_distinct (sel: the selection / DISTINCT columns).  A refusal dumps its status and message.
+int64_t probe_plan_dump(int32_t kind, int32_t sm_count, int32_t max_smem_optin, const char* const* knob_names,
+                        const int64_t* knob_values, int32_t nknobs, const pb200_query* query, const double* agg_args,
+                        const pb200_selection* sel, const probe_col* cols, int32_t ncols, const int32_t* num_docs, int32_t nseg,
+                        int32_t allow_count_carrier, int32_t merge, int32_t prefix, char* out, int64_t cap) {
+  using namespace pb200;
+  pb200_ctx ctx;
+  for (int i = 0; i < nknobs; i++) if (int rc = pb200_tuning_set(&ctx, knob_names[i], knob_values[i])) return rc;
+  ProbeSegments ps(cols, ncols, num_docs, nseg);
+  const DeviceLimits lim{sm_count, max_smem_optin};
+  const int nnodes_total = query->num_filter_nodes * ((query->flags & PB200_Q_PER_SEGMENT_FILTER) ? nseg : 1);
+  PlanDump d{ps, query, nnodes_total, {}};
+  int rc;
+  if (kind == 0) {
+    ScanPlan p;
+    rc = plan_scan(ctx.tune, lim, query, ps.ptrs.data(), nseg, allow_count_carrier != 0, &p, agg_args);
+    if (!rc) d.scan(p);
+  } else if (kind == 1) {
+    SelectionPlan p;
+    rc = plan_selection(ctx.tune, lim, query, sel, ps.ptrs.data(), nseg, prefix != 0, &p);
+    if (!rc) d.selection(p);
+  } else {
+    DistinctPlan p;
+    rc = plan_distinct(ctx.tune, lim, query, sel, ps.ptrs.data(), nseg, merge != 0, prefix != 0, &p);
+    if (!rc) d.distinct(p);
+  }
+  if (rc) d.line("refused %d %s", rc, pb200_last_error());
+  memcpy(out, d.out.data(), std::min<size_t>(d.out.size(), (size_t)cap));
+  return (int64_t)d.out.size();
 }
 
 }  // extern "C"

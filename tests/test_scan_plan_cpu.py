@@ -49,7 +49,7 @@ class ProbePlan(C.Structure):
 
 class ProbeCol(C.Structure):
     _fields_ = [("fwd_kind", C.c_int32), ("stored_type", C.c_int32), ("bits", C.c_int32), ("cardinality", C.c_int32),
-                ("dict_native", C.c_int32), ("dict_shared", C.c_int32), ("has_inv", C.c_int32), ("reserved", C.c_int32),
+                ("dict_native", C.c_int32), ("dict_shared", C.c_int32), ("has_inv", C.c_int32), ("eligible", C.c_int32),
                 ("dict_hash", C.c_uint64), ("dict_host", C.c_void_p), ("dict_host_bytes", C.c_uint64)]
 
 
@@ -128,7 +128,7 @@ def plan(probe, seg_cols, num_docs, q, knobs=None, carrier=True, limits=H100):
         for k, c in enumerate(cs):
             host = c.get("cbuf")
             cols[s * ncols + k] = ProbeCol(c["kind"], c["stored"], c["bits"], c["card"], int(c["native"]), int(c["shared"]),
-                                           int(c["inv"]), 0, c["hash"], C.cast(host, C.c_void_p) if host else None,
+                                           int(c["inv"]), -1, c["hash"], C.cast(host, C.c_void_p) if host else None,
                                            len(c["host"]) if host else 0)
     names = (C.c_char_p * max(len(knobs), 1))(*[k.encode() for k in knobs])
     values = (C.c_int64 * max(len(knobs), 1))(*knobs.values())
