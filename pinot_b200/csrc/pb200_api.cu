@@ -14,6 +14,7 @@
 #include <cstring>
 #include <limits>
 #include <memory>
+#include <optional>
 
 #include "pb200_internal.h"
 #include "pb200_percentile.h"
@@ -628,9 +629,7 @@ cudaError_t launch_scan_variant(const ScanVariant& v, size_t smem_bytes, int gri
   if (v.warps == 8) return v.defer ? launch_scan_w8_agg(smem_bytes, grid, q, tt, dsegs, st) : launch_scan_w8_agg_nodefer(smem_bytes, grid, q, tt, dsegs, st);
   return launch_scan_w6_agg(smem_bytes, grid, q, tt, dsegs, st);
 }
-}  // namespace pb200
 
-namespace pb200 {
 // Device buffers of the plan's filter leaves: LUTs, doc masks, range lists, and every posting list decoded by ONE launch;
 // the leaf descriptors in plan.segs point at them.  They live in `temps` until the caller is done with the launch.
 int bind_leaf_buffers(pb200_ctx* ctx, ScanPlan& plan, cudaStream_t st, std::vector<std::unique_ptr<DevBufRaw>>& temps) {
@@ -674,10 +673,32 @@ int bind_leaf_buffers(pb200_ctx* ctx, ScanPlan& plan, cudaStream_t st, std::vect
   }
   return PB200_OK;
 }
+
+int launch_chunks(pb200_ctx* ctx, cudaStream_t st, const ScanPlan& plan, DevBufRaw& dsegs, EventPair& ev, const char* what,
+                  uint32_t* mask, const long long* chunk_word_off, double* t_launch) {
+  const size_t bytes = sizeof(SegDesc) * plan.segs.size();
+  if (int rc = dsegs.alloc(bytes)) return rc;
+  if (int rc = ev.take()) return rc;
+  PB200_CUDA(cudaMemcpyAsync(dsegs.p, plan.segs.data(), bytes, cudaMemcpyHostToDevice, st));
+  if (t_launch) *t_launch = now_ms();
+  PB200_CUDA(cudaEventRecord(ev.a, st));
+  for (size_t c = 0; c < plan.chunks.size(); c++) {
+    const LaunchChunk& ch = plan.chunks[c];
+    QueryDesc cq = plan.q;
+    cq.num_segments = ch.num_segs;
+    cq.total_tiles = ch.total_tiles;
+    if (mask) set_selection_mask(cq, mask + chunk_word_off[c]);
+    const cudaError_t le = launch_scan_variant(plan.variant, plan.smem_bytes, ch.grid, cq, tma_table(plan, ch),
+                                               static_cast<const SegDesc*>(dsegs.p) + ch.first_seg, st);
+    if (le != cudaSuccess) { set_error("%s launch failed: %s (smem %zu B, grid %d)", what, cudaGetErrorString(le), plan.smem_bytes, ch.grid); return PB200_E_CUDA; }
+  }
+  PB200_CUDA(cudaEventRecord(ev.b, st));
+  return PB200_OK;
+}
 }  // namespace pb200
 
-// Internal return code of execute_impl: a count-carrying sum overflowed its field (detected exactly, see the verification
-// after the launch) -- the caller runs the submission again with separate COUNT reductions.
+// Internal return code of execute_impl: a count-carrying sum overflowed its field (detected exactly, see
+// ScanCall::read_back_and_verify) -- the caller runs the submission again with separate COUNT reductions.
 constexpr int kRetryWithoutCountCarrier = 1;
 static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment* const* segments, int32_t nseg,
                         pb200_result** results, bool allow_count_carrier, const pb200_order_by* order, const double* agg_args);
@@ -719,100 +740,132 @@ __global__ void carrier_verify_kernel(const unsigned long long* __restrict__ tab
   if ((threadIdx.x & 31) == 0) { if (c) atomicAdd(out, c); if (mx) atomicMax(out + 1, mx); if (mc) atomicMax(out + 2, mc); }
 }
 
-static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment* const* segments, int32_t nseg,
-                        pb200_result** results, bool allow_count_carrier, const pb200_order_by* order, const double* agg_args) {
-  if (!ctx || !query || !segments || !results || nseg <= 0) { set_error("invalid argument to pb200_execute"); return PB200_E_INVALID; }
-  const double t_enter = now_ms();
-  PB200_CUDA(cudaSetDevice(ctx->device));
-  for (int s = 0; s < nseg; s++)
-    if (segments[s] && segments[s]->ctx != ctx) { set_error("segment %d does not belong to this context / schema", s); return PB200_E_INVALID; }
+namespace {
+// The accumulator block of one call: on the device, and in each half of a pooled pinned block (initial values go up and
+// results come back through it, both asynchronously on the call's stream: a pageable cudaMemcpy would synchronise the
+// device twice per query).  nres AggAccum records, then 4 words per result for the count-carrier verification {sum of
+// carried counts, largest sum field, largest carried count, unused}, then (aggregation-only PERCENTILE) per result
+// kMaxAggs selected dictIds and kMaxAggs value counts, u32 each.
+struct AccumLayout {
+  size_t verify_off = 0, pct_off = 0, bytes = 0;
+  AccumLayout() = default;
+  AccumLayout(int nres, bool pct)
+      : verify_off(sizeof(AggAccum) * nres), pct_off(verify_off + 32ull * nres), bytes(pct_off + (pct ? 8ull * kMaxAggs * nres : 0)) {}
+  static AggAccum* records(void* b) { return static_cast<AggAccum*>(b); }
+  unsigned long long* verify(void* b) const { return reinterpret_cast<unsigned long long*>(static_cast<unsigned char*>(b) + verify_off); }
+  uint32_t* pct(void* b) const { return reinterpret_cast<uint32_t*>(static_cast<unsigned char*>(b) + pct_off); }
+};
 
-  // ---- plan: every decision about the launch (pb200_plan.cpp) ----
-  const Tuning tune = [&]() { std::lock_guard<std::mutex> g(ctx->mu); return ctx->tune; }();
-  if (int rc = moments_prepare(ctx, query, segments, nseg)) return rc;   // VAR / STDDEV limb dictionaries (pb200_moments.cu)
+// Frees a result's group tables and PERCENTILE selections; its histograms too unless keep_hist (pb200_result_histogram).
+void release_tables(pb200_result& R, bool keep_hist) {
+  pb200_result::Dense& d = R.dense;
+  if (d.ctx) {
+    dev_free(d.ctx, d.i64_block); dev_free(d.ctx, d.f64_block); dev_free(d.ctx, d.u32max_block); dev_free(d.ctx, d.u32min_block);
+    dev_free(d.ctx, d.hkeys); dev_free(d.ctx, d.hctl);
+    for (int a = 0; a < kMaxAggs; a++) { dev_free(d.ctx, d.dbits[a]); d.dbits[a] = nullptr; }
+    d.i64_block = d.f64_block = d.u32max_block = d.u32min_block = nullptr;
+    d.hkeys = nullptr; d.hctl = nullptr;
+    d.live = false;
+  }
+  pb200_result::Pct& p = R.pct;
+  if (p.ctx)
+    for (int a = 0; a < kMaxAggs; a++) {
+      if (!keep_hist) { dev_free(p.ctx, p.hist[a]); p.hist[a] = nullptr; }
+      dev_free(p.ctx, p.ids[a]); dev_free(p.ctx, p.n[a]); p.ids[a] = p.n[a] = nullptr;
+    }
+}
+
+// One attempt of pb200_execute; execute_impl runs its stages in order.  Members are only the state that crosses stages.
+struct ScanCall {
+  pb200_ctx* const ctx;
+  const pb200_query* const query;
+  pb200_segment* const* const segments;
+  const int nseg;
+  double t_enter = 0, t_launch = 0, t_queued = 0, t_synced = 0, t_results = 0;
+  Tuning tune;
   ScanPlan plan;
-  {
-    const int rc = plan_scan(tune, DeviceLimits{ctx->sm_count, ctx->max_smem_optin}, query, segments, nseg, allow_count_carrier, &plan, agg_args);
-    if (rc) return rc;
-  }
-  const QueryDesc& q = plan.q;
-  // nagg: the launch's aggregations, the internal VAR / STDDEV limb sums included; nuser: the caller's (the result's columns)
-  const int nagg = q.num_aggs, nuser = plan.num_user_aggs, ngb = q.num_group_by, nres = plan.nres;
-  const bool merge = plan.merge;
-
-  cudaStream_t st = take_stream(ctx);
-  struct StreamReturn { pb200_ctx* c; cudaStream_t s; ~StreamReturn() { give_stream(c, s); } } stream_return{ctx, st};
-  std::vector<std::unique_ptr<pb200_result>> res;
-  for (int r = 0; r < nres; r++) {
-    res.emplace_back(new pb200_result());
-    res.back()->pct.ctx = ctx;
-    for (int a = 0; a < nagg; a++) res.back()->pct.rep[a] = plan.pct_rep[a];
-  }
-  bool any_pct = false;
-  for (int a = 0; a < nagg; a++) any_pct |= plan.pct_rep[a] >= 0;
-  struct ResultCleanup {  // frees dense device state if we fail midway
-    std::vector<std::unique_ptr<pb200_result>>* r;
-    bool armed = true;
-    ~ResultCleanup() { if (armed) for (auto& x : *r) if (x) pb200_result_free(x.release()); }
-  } cleanup{&res};
-
-  std::vector<std::unique_ptr<DevBufRaw>> temps;  // freed after the launch
-  if (int rc = bind_leaf_buffers(ctx, plan, st, temps)) return rc;
-
-  // ---- bind the outputs ----
-  AggAccum init_acc;
-  memset(&init_acc, 0, sizeof init_acc);
-  for (int a = 0; a < kMaxAggs; a++) init_acc.min_id[a] = 0xFFFFFFFFu;
-  // initial values go up and results come back through ONE pooled pinned block, both asynchronously on the query's stream
-  // (a pageable cudaMemcpy would synchronise the device twice per query)
+  std::optional<StreamLease> lease;                  // taken once the plan stands
+  cudaStream_t st = nullptr;
+  std::vector<std::unique_ptr<pb200_result>> res;    // freed with their device state unless handed out
+  std::vector<std::unique_ptr<DevBufRaw>> temps;     // leaf buffers and PERCENTILE scratch, needed until the call returns
   struct PinnedScratch {
     pb200_ctx* c; void* p = nullptr; size_t bytes = 0;
     ~PinnedScratch() { pinned_free(c, p, bytes); }
-  } pacc{ctx};
-  {
-    int rc = pinned_alloc(ctx, 2 * (sizeof(AggAccum) + 32 + (any_pct && !plan.group_by ? 8 * kMaxAggs : 0)) * nres, &pacc.p, &pacc.bytes);
-    if (rc) return rc;
+  } pin{ctx};
+  AccumLayout acc;
+  DevBufRaw accum{ctx};
+  unsigned char* back = nullptr;                     // the pinned half the accumulator block is read back into
+  std::vector<std::vector<std::unique_ptr<DevBufRaw>>> distinct_bufs;  // aggregation only: DISTINCTCOUNT bitsets
+  DevBufRaw dsegs{ctx};
+  EventPair ev{ctx};                                 // around the scan launches
+
+  ~ScanCall() { for (auto& r : res) if (r) pb200_result_free(r.release()); }
+
+  // 1. the call's arguments and device, and the tuning snapshot the planner reads
+  int check_call(pb200_result** results) {
+    if (!ctx || !query || !segments || !results || nseg <= 0) { set_error("invalid argument to pb200_execute"); return PB200_E_INVALID; }
+    t_enter = now_ms();
+    PB200_CUDA(cudaSetDevice(ctx->device));
+    for (int s = 0; s < nseg; s++)
+      if (segments[s] && segments[s]->ctx != ctx) { set_error("segment %d does not belong to this context / schema", s); return PB200_E_INVALID; }
+    std::lock_guard<std::mutex> g(ctx->mu);
+    tune = ctx->tune;
+    return PB200_OK;
   }
-  // block layout (device and both pinned halves): nres AggAccum records, then 4 words per result for the count-carrier
-  // verification {sum of carried counts, largest sum field, largest carried count, unused}, then (aggregation-only
-  // PERCENTILE) per result kMaxAggs selected dictIds and kMaxAggs value counts, u32 each -- read back with the accumulators
-  const size_t pct_bytes = any_pct && !plan.group_by ? 8ull * kMaxAggs * nres : 0;
-  const size_t acc_bytes = (sizeof(AggAccum) + 32) * nres + pct_bytes;
-  unsigned char* const pin_init = static_cast<unsigned char*>(pacc.p);
-  unsigned char* const pin_back = pin_init + acc_bytes;
-  AggAccum* host_acc = reinterpret_cast<AggAccum*>(pin_back);
-  const unsigned long long* host_verify = reinterpret_cast<const unsigned long long*>(pin_back + sizeof(AggAccum) * nres);
-  DevBufRaw accum_buf(ctx);  // nres AggAccum records, initialised and read back with ONE copy each
-  {
-    memset(pin_init, 0, acc_bytes);
-    AggAccum* init = reinterpret_cast<AggAccum*>(pin_init);
-    for (int r = 0; r < nres; r++) init[r] = init_acc;
-    int rc = accum_buf.alloc(acc_bytes);
-    if (rc) return rc;
-    PB200_CUDA(cudaMemcpyAsync(accum_buf.p, pin_init, acc_bytes, cudaMemcpyHostToDevice, st));
+
+  // 2. VAR / STDDEV limb dictionaries (pb200_moments.cu), then every decision about the launch (pb200_plan.cpp)
+  int prepare_and_plan(bool allow_count_carrier, const double* agg_args) {
+    if (int rc = moments_prepare(ctx, query, segments, nseg)) return rc;
+    return plan_scan(tune, DeviceLimits{ctx->sm_count, ctx->max_smem_optin}, query, segments, nseg, allow_count_carrier, &plan, agg_args);
   }
-  unsigned long long* const dev_verify = reinterpret_cast<unsigned long long*>(static_cast<unsigned char*>(accum_buf.p) + sizeof(AggAccum) * nres);
-  uint32_t* const dev_pct = reinterpret_cast<uint32_t*>(static_cast<unsigned char*>(accum_buf.p) + (sizeof(AggAccum) + 32) * nres);
-  const uint32_t* const host_pct = reinterpret_cast<const uint32_t*>(pin_back + (sizeof(AggAccum) + 32) * nres);
-  for (int s = 0; s < nseg; s++) plan.segs[s].accum = (AggAccum*)accum_buf.p + (merge ? 0 : s);
-  std::vector<std::vector<std::unique_ptr<DevBufRaw>>> distinct_bufs(nres);  // aggregation only: DISTINCTCOUNT bitsets
-  if (!plan.group_by) {
-    for (int r = 0; r < nres; r++) {
+
+  // 3. the stream, the results, and the device buffers of the filter leaves
+  int alloc_results() {
+    lease.emplace(ctx);
+    st = *lease;
+    for (int r = 0; r < plan.nres; r++) {
+      res.emplace_back(new pb200_result());
+      res.back()->pct.ctx = ctx;
+      for (int a = 0; a < plan.q.num_aggs; a++) res.back()->pct.rep[a] = plan.pct_rep[a];
+    }
+    return bind_leaf_buffers(ctx, plan, st, temps);
+  }
+
+  // 4. the accumulator block, initialised with one copy from the pinned block's first half
+  int bind_accumulators() {
+    bool any_pct = false;
+    for (int a = 0; a < plan.q.num_aggs; a++) any_pct |= plan.pct_rep[a] >= 0;
+    acc = AccumLayout(plan.nres, any_pct && !plan.group_by);
+    if (int rc = pinned_alloc(ctx, 2 * acc.bytes, &pin.p, &pin.bytes)) return rc;
+    unsigned char* const init = static_cast<unsigned char*>(pin.p);
+    back = init + acc.bytes;
+    AggAccum init_acc;
+    memset(&init_acc, 0, sizeof init_acc);
+    for (int a = 0; a < kMaxAggs; a++) init_acc.min_id[a] = 0xFFFFFFFFu;
+    memset(init, 0, acc.bytes);
+    for (int r = 0; r < plan.nres; r++) AccumLayout::records(init)[r] = init_acc;
+    if (int rc = accum.alloc(acc.bytes)) return rc;
+    PB200_CUDA(cudaMemcpyAsync(accum.p, init, acc.bytes, cudaMemcpyHostToDevice, st));
+    for (int s = 0; s < nseg; s++) plan.segs[s].accum = AccumLayout::records(accum.p) + (plan.merge ? 0 : s);
+    return PB200_OK;
+  }
+
+  // 5. aggregation only: DISTINCTCOUNT bitsets, and PERCENTILE dictId histograms (one per result and column, owned by the
+  //    result from here on)
+  int bind_agg_outputs() {
+    const int nagg = plan.q.num_aggs;
+    distinct_bufs.resize(plan.nres);
+    for (int r = 0; r < plan.nres; r++) {
       distinct_bufs[r].resize(nagg);
       for (int a = 0; a < nagg; a++) {
         const size_t words = plan.distinct_words[r][a];
         if (!words) continue;
         distinct_bufs[r][a].reset(new DevBufRaw(ctx));
-        int rc = distinct_bufs[r][a]->alloc(words * 4);
-        if (rc) return rc;
+        if (int rc = distinct_bufs[r][a]->alloc(words * 4)) return rc;
         PB200_CUDA(cudaMemsetAsync(distinct_bufs[r][a]->p, 0, words * 4, st));
       }
     }
-    for (int s = 0; s < nseg; s++)
-      for (int a = 0; a < nagg; a++)
-        if (distinct_bufs[merge ? 0 : s][a]) plan.segs[s].distinct_bits[a] = (uint32_t*)distinct_bufs[merge ? 0 : s][a]->p;
-    // PERCENTILE: one dictId histogram per result and column, owned by the result from here on
-    for (int r = 0; r < nres; r++)
+    for (int r = 0; r < plan.nres; r++)
       for (int a = 0; a < nagg; a++) {
         const size_t entries = plan.hist_entries[r][a];
         if (!entries) continue;
@@ -821,172 +874,163 @@ static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment*
         PB200_CUDA(cudaMemsetAsync(p.hist[a], 0, entries * 4, st));
         p.entries[a] = (uint32_t)entries;
       }
-    for (int s = 0; s < nseg; s++)
-      for (int a = 0; a < nagg; a++)
-        if (res[merge ? 0 : s]->pct.hist[a]) plan.segs[s].distinct_bits[a] = res[merge ? 0 : s]->pct.hist[a];
-  } else {
-    // group tables to the plan's layout; they belong to the results from here on
-    for (int r = 0; r < nres; r++) {
-      const pb200_segment* seg = segments[merge ? 0 : r];
-      const TableLayout& t = plan.tables[r];
-      pb200_result::Dense& d = res[r]->dense;
-      d.ctx = ctx;
-      d.cards = t.cards; d.mult = t.mult; d.mult64 = t.mult64;
-      d.groups = t.groups;
-      d.stride = t.stride;
-      d.live = true;
-      d.num_groups_limit = query->num_groups_limit;
-      for (int a = 0; a < nuser; a++) { d.aggs.push_back(query->aggs[a]); d.val_kind.push_back(q.aggs[a].val_kind); d.agg_cols.push_back(q.aggs[a].slot < 0 ? nullptr : &seg->cols[query->aggs[a].column]); }
-      for (int a = 0; a < nuser; a++) {
-        d.mom_first[a] = plan.mom_first[a];
-        if (plan.mom_first[a] >= 0) d.mom_e[a] = seg->cols[query->aggs[a].column].moments->grid.e;
-      }
-      d.pack_agg = t.carrier.agg; d.pack_shift = t.carrier.shift; d.pack_vmin = t.carrier.vmin;
-      d.reduce_world = t.reduce_world;
-      d.flag_slot = t.flag_slot;
-      d.tail_slots = t.tail_slots;
-      d.i64_elems = t.i64_elems; d.f64_elems = t.f64_elems; d.u32max_elems = t.u32max_elems; d.u32min_elems = t.u32min_elems;
-      auto alloc_block = [&](void** p, long long elems, size_t esz, int fill) -> int {
-        if (!elems) return PB200_OK;
-        int rc = dev_alloc(ctx, (size_t)elems * esz, p);
-        if (rc) return rc;
-        PB200_CUDA(cudaMemsetAsync(*p, fill, (size_t)elems * esz, st));
-        return PB200_OK;
-      };
-      int rc;
-      if (t.hashed) {
-        if ((rc = alloc_block((void**)&d.hkeys, t.groups, 8, 0xFF))) return rc;
-        if ((rc = alloc_block((void**)&d.hctl, 2, 4, 0))) return rc;
-      }
-      if ((rc = alloc_block(&d.i64_block, d.i64_elems, 8, 0))) return rc;
-      if ((rc = alloc_block(&d.f64_block, d.f64_elems, 8, 0))) return rc;
-      if ((rc = alloc_block(&d.u32max_block, d.u32max_elems, 4, 0))) return rc;
-      if ((rc = alloc_block(&d.u32min_block, d.u32min_elems, 4, 0xFF))) return rc;
-      d.count = t.need_count ? (unsigned long long*)d.i64_block : nullptr;
-      d.seen = t.need_seen ? (uint32_t*)d.u32max_block : nullptr;
+    for (int s = 0; s < nseg; s++) {
+      const int r = plan.merge ? 0 : s;
       for (int a = 0; a < nagg; a++) {
-        const int fn = q.aggs[a].function;
-        const long long off = (long long)t.index[a] * t.groups;
-        if (fn == PB200_AGG_SUM || fn == PB200_AGG_AVG) {
-          if (sum_in_double(q.aggs[a].val_kind)) d.dsum[a] = (double*)d.f64_block + off;
-          else d.isum[a] = (long long*)d.i64_block + off;
-        } else if (fn == PB200_AGG_MIN) d.gmin[a] = (uint32_t*)d.u32min_block + off;
-        else if (fn == PB200_AGG_MAX) d.gmax[a] = (uint32_t*)d.u32max_block + off;
-        else if (fn == PB200_AGG_DISTINCTCOUNT) {  // one dictId bitset per group / slot
-          const size_t bytes = (size_t)t.dwords[a] * t.groups * 4;
-          if ((rc = dev_alloc(ctx, bytes, (void**)&d.dbits[a]))) return rc;
-          PB200_CUDA(cudaMemsetAsync(d.dbits[a], 0, bytes, st));
-          d.dwords[a] = t.dwords[a];
-        } else if (fn == PB200_AGG_PERCENTILE) {  // one dictId histogram per group / slot (owner), a dictId per entry (each)
-          pb200_result::Pct& p = res[r]->pct;
-          if (t.hist_per_group[a]) {
-            const size_t entries = (size_t)t.hist_per_group[a] * t.groups;
-            if ((rc = dev_alloc(ctx, entries * 4, (void**)&p.hist[a]))) return rc;
-            PB200_CUDA(cudaMemsetAsync(p.hist[a], 0, entries * 4, st));
-            p.entries[a] = t.hist_per_group[a];
-            if ((rc = dev_alloc(ctx, (size_t)t.groups * 4, (void**)&p.n[a]))) return rc;
-          }
-          if ((rc = dev_alloc(ctx, (size_t)t.groups * 4, (void**)&p.ids[a]))) return rc;
-        }
+        if (distinct_bufs[r][a]) plan.segs[s].distinct_bits[a] = (uint32_t*)distinct_bufs[r][a]->p;
+        if (res[r]->pct.hist[a]) plan.segs[s].distinct_bits[a] = res[r]->pct.hist[a];
       }
-      if (d.pack_agg >= 0) d.exists_packed = (const unsigned long long*)d.isum[d.pack_agg];
-      if (t.exists_min >= 0) d.exists_min = d.gmin[t.exists_min];
-      if (t.exists_max >= 0) d.exists_max = d.gmax[t.exists_max];
     }
+    return PB200_OK;
+  }
+
+  // 6. group-by: each result's tables to the plan's layout (owned by the result from here on), then the segments'
+  //    descriptors pointed at them
+  int bind_group_tables() {
+    for (int r = 0; r < plan.nres; r++)
+      if (int rc = build_dense(r)) return rc;
     for (int s = 0; s < nseg; s++) {
       SegDesc& sd = plan.segs[s];
-      const pb200_result::Dense& d = res[merge ? 0 : s]->dense;
+      const pb200_result& R = *res[plan.merge ? 0 : s];
+      const pb200_result::Dense& d = R.dense;
       sd.g_count = d.count;
       sd.g_seen = d.seen;
-      for (int a = 0; a < nagg; a++) { sd.g_isum[a] = d.isum[a]; sd.g_dsum[a] = d.dsum[a]; sd.g_min[a] = d.gmin[a]; sd.g_max[a] = d.gmax[a]; sd.distinct_bits[a] = d.dbits[a]; }
-      for (int a = 0; a < nagg; a++) if (res[merge ? 0 : s]->pct.hist[a]) sd.distinct_bits[a] = res[merge ? 0 : s]->pct.hist[a];
       sd.h_keys = d.hkeys;
       sd.h_ctl = d.hctl;
+      for (int a = 0; a < plan.q.num_aggs; a++) {
+        sd.g_isum[a] = d.isum[a]; sd.g_dsum[a] = d.dsum[a]; sd.g_min[a] = d.gmin[a]; sd.g_max[a] = d.gmax[a];
+        sd.distinct_bits[a] = R.pct.hist[a] ? R.pct.hist[a] : d.dbits[a];
+      }
     }
+    return PB200_OK;
+  }
+  int build_dense(int r) {
+    const pb200_segment* seg = segments[plan.merge ? 0 : r];
+    const TableLayout& t = plan.tables[r];
+    const QueryDesc& q = plan.q;
+    pb200_result::Dense& d = res[r]->dense;
+    pb200_result::Pct& p = res[r]->pct;
+    d.ctx = ctx;
+    d.cards = t.cards; d.mult = t.mult; d.mult64 = t.mult64;
+    d.groups = t.groups;
+    d.stride = t.stride;
+    d.live = true;
+    d.num_groups_limit = query->num_groups_limit;
+    for (int a = 0; a < plan.num_user_aggs; a++) {
+      d.aggs.push_back(query->aggs[a]);
+      d.val_kind.push_back(q.aggs[a].val_kind);
+      d.agg_cols.push_back(q.aggs[a].slot < 0 ? nullptr : &seg->cols[query->aggs[a].column]);
+      d.mom_first[a] = plan.mom_first[a];
+      if (plan.mom_first[a] >= 0) d.mom_e[a] = seg->cols[query->aggs[a].column].moments->grid.e;
+    }
+    d.pack_agg = t.carrier.agg; d.pack_shift = t.carrier.shift; d.pack_vmin = t.carrier.vmin;
+    d.reduce_world = t.reduce_world;
+    d.flag_slot = t.flag_slot;
+    d.tail_slots = t.tail_slots;
+    d.i64_elems = t.i64_elems; d.f64_elems = t.f64_elems; d.u32max_elems = t.u32max_elems; d.u32min_elems = t.u32min_elems;
+    auto alloc_block = [&](void** out, long long elems, size_t esz, int fill) -> int {
+      if (!elems) return PB200_OK;
+      if (int rc = dev_alloc(ctx, (size_t)elems * esz, out)) return rc;
+      PB200_CUDA(cudaMemsetAsync(*out, fill, (size_t)elems * esz, st));
+      return PB200_OK;
+    };
+    int rc;
+    if (t.hashed) {
+      if ((rc = alloc_block((void**)&d.hkeys, t.groups, 8, 0xFF))) return rc;
+      if ((rc = alloc_block((void**)&d.hctl, 2, 4, 0))) return rc;
+    }
+    if ((rc = alloc_block(&d.i64_block, d.i64_elems, 8, 0))) return rc;
+    if ((rc = alloc_block(&d.f64_block, d.f64_elems, 8, 0))) return rc;
+    if ((rc = alloc_block(&d.u32max_block, d.u32max_elems, 4, 0))) return rc;
+    if ((rc = alloc_block(&d.u32min_block, d.u32min_elems, 4, 0xFF))) return rc;
+    d.count = t.need_count ? (unsigned long long*)d.i64_block : nullptr;
+    d.seen = t.need_seen ? (uint32_t*)d.u32max_block : nullptr;
+    for (int a = 0; a < q.num_aggs; a++) {
+      const int fn = q.aggs[a].function;
+      const long long off = (long long)t.index[a] * t.groups;
+      if (fn == PB200_AGG_SUM || fn == PB200_AGG_AVG) {
+        if (sum_in_double(q.aggs[a].val_kind)) d.dsum[a] = (double*)d.f64_block + off;
+        else d.isum[a] = (long long*)d.i64_block + off;
+      } else if (fn == PB200_AGG_MIN) d.gmin[a] = (uint32_t*)d.u32min_block + off;
+      else if (fn == PB200_AGG_MAX) d.gmax[a] = (uint32_t*)d.u32max_block + off;
+      else if (fn == PB200_AGG_DISTINCTCOUNT) {  // one dictId bitset per group / slot
+        const size_t bytes = (size_t)t.dwords[a] * t.groups * 4;
+        if ((rc = dev_alloc(ctx, bytes, (void**)&d.dbits[a]))) return rc;
+        PB200_CUDA(cudaMemsetAsync(d.dbits[a], 0, bytes, st));
+        d.dwords[a] = t.dwords[a];
+      } else if (fn == PB200_AGG_PERCENTILE) {  // one dictId histogram per group / slot (owner), a dictId per entry (each)
+        if (t.hist_per_group[a]) {
+          const size_t entries = (size_t)t.hist_per_group[a] * t.groups;
+          if ((rc = dev_alloc(ctx, entries * 4, (void**)&p.hist[a]))) return rc;
+          PB200_CUDA(cudaMemsetAsync(p.hist[a], 0, entries * 4, st));
+          p.entries[a] = t.hist_per_group[a];
+          if ((rc = dev_alloc(ctx, (size_t)t.groups * 4, (void**)&p.n[a]))) return rc;
+        }
+        if ((rc = dev_alloc(ctx, (size_t)t.groups * 4, (void**)&p.ids[a]))) return rc;
+      }
+    }
+    if (d.pack_agg >= 0) d.exists_packed = (const unsigned long long*)d.isum[d.pack_agg];
+    if (t.exists_min >= 0) d.exists_min = d.gmin[t.exists_min];
+    if (t.exists_max >= 0) d.exists_max = d.gmax[t.exists_max];
+    return PB200_OK;
   }
 
-  // ---- launch the chunks ----
-  DevBufRaw dsegs(ctx);
-  int rc = dsegs.alloc(sizeof(SegDesc) * nseg);
-  if (rc) return rc;
-  struct Events {  // pooled per context (creating / destroying two events per query costs more than the launch itself)
-    pb200_ctx* c; cudaEvent_t a = nullptr, b = nullptr;
-    ~Events() { give_event(c, a); give_event(c, b); }
-  } ev{ctx};
-  ev.a = take_event(ctx);
-  ev.b = take_event(ctx);
-  if (!ev.a || !ev.b) { set_error("cudaEventCreate failed"); return PB200_E_CUDA; }
-  cudaEvent_t e0 = ev.a, e1 = ev.b;
-  PB200_CUDA(cudaMemcpyAsync(dsegs.p, plan.segs.data(), sizeof(SegDesc) * nseg, cudaMemcpyHostToDevice, st));
-  const double t_launch = now_ms();
-  PB200_CUDA(cudaEventRecord(e0, st));
-  cudaError_t le = cudaSuccess;
-  int grid = 0;
-  for (size_t c = 0; c < plan.chunks.size() && le == cudaSuccess; c++) {
-    const LaunchChunk& ch = plan.chunks[c];
-    QueryDesc cq = q;
-    cq.num_segments = ch.num_segs;
-    cq.total_tiles = ch.total_tiles;
-    grid = ch.grid;
-    le = launch_scan_variant(plan.variant, plan.smem_bytes, grid, cq, tma_table(plan, ch), (const SegDesc*)dsegs.p + ch.first_seg, st);
+  // 7. the descriptors and every chunk's scan, between the call's two events
+  int launch() { return launch_chunks(ctx, st, plan, dsegs, ev, "scan kernel", nullptr, nullptr, &t_launch); }
+
+  // 8. PERCENTILE: histograms -> selected dictIds, queued behind the scan (aggregation only: into the accumulator block;
+  //    group-by: per table entry, read by the extraction)
+  int finalize_percentiles() {
+    uint32_t* const dev_pct = acc.pct(accum.p);
+    for (int r = 0; r < plan.nres; r++)
+      for (int a = 0; a < plan.q.num_aggs; a++) {
+        pb200_result::Pct& p = res[r]->pct;
+        if (!p.hist[a]) continue;
+        PercentileJob job;
+        job.hist = p.hist[a];
+        job.E = p.entries[a];
+        job.rows = plan.group_by ? plan.tables[r].groups : 1;
+        job.n_out = plan.group_by ? p.n[a] : dev_pct + (size_t)r * 2 * kMaxAggs + kMaxAggs + a;
+        for (int b = 0; b < plan.q.num_aggs; b++) {
+          if (plan.pct_rep[b] != a) continue;
+          job.p[job.np] = plan.pct_p[b];
+          job.ids[job.np++] = plan.group_by ? p.ids[b] : dev_pct + (size_t)r * 2 * kMaxAggs + b;
+        }
+        if (int rc = percentile_finalize(ctx, st, job, temps)) return rc;
+      }
+    return PB200_OK;
   }
-  if (le != cudaSuccess) { set_error("scan kernel launch failed: %s (smem %zu B, grid %d)", cudaGetErrorString(le), plan.smem_bytes, grid); return PB200_E_CUDA; }
-  PB200_CUDA(cudaEventRecord(e1, st));
 
-  // ---- PERCENTILE finalize: histograms -> selected dictIds, queued behind the scan (aggregation only: into the block
-  //      that is read back with the accumulators; group-by: per table entry, read by the extraction) ----
-  std::vector<std::unique_ptr<DevBufRaw>> pct_temps;
-  for (int r = 0; r < nres && any_pct; r++)
-    for (int a = 0; a < nagg; a++) {
-      pb200_result::Pct& p = res[r]->pct;
-      if (!p.hist[a]) continue;
-      PercentileJob job;
-      job.hist = p.hist[a];
-      job.E = p.entries[a];
-      if (plan.group_by) {
-        job.rows = plan.tables[r].groups;
-        job.n_out = p.n[a];
-      } else {
-        job.rows = 1;
-        job.n_out = dev_pct + (size_t)r * 2 * kMaxAggs + kMaxAggs + a;
+  // 9. the count carriers' check queued behind the scan, the accumulator block read back, the wait for both, and the
+  //    carriers' verdict: kRetryWithoutCountCarrier when a carried sum overflowed its field
+  int read_back_and_verify() {
+    if (plan.group_by)
+      for (int r = 0; r < plan.nres; r++) {
+        const pb200_result::Dense& d = res[r]->dense;
+        if (d.pack_agg < 0) continue;
+        const int vb = (int)std::max<long long>(1, std::min<long long>((d.groups + 1023) / 1024, (long long)ctx->sm_count * 4));
+        carrier_verify_kernel<<<vb, 256, 0, st>>>((const unsigned long long*)d.isum[d.pack_agg], d.groups, d.pack_shift, acc.verify(accum.p) + 4 * r);
       }
-      for (int b = 0; b < nagg; b++) {
-        if (plan.pct_rep[b] != a) continue;
-        job.p[job.np] = plan.pct_p[b];
-        job.ids[job.np++] = plan.group_by ? p.ids[b] : dev_pct + (size_t)r * 2 * kMaxAggs + b;
-      }
-      if (int prc = percentile_finalize(ctx, st, job, pct_temps)) return prc;
-    }
-
-  // ---- verify the count carriers ----
-  if (plan.group_by)
-    for (int r = 0; r < nres; r++) {
-      const pb200_result::Dense& d = res[r]->dense;
+    PB200_CUDA(cudaMemcpyAsync(back, accum.p, acc.bytes, cudaMemcpyDeviceToHost, st));
+    t_queued = now_ms();
+    const cudaError_t se = cudaStreamSynchronize(st);
+    if (se != cudaSuccess) { set_error("scan kernel failed: %s", cudaGetErrorString(se)); return PB200_E_CUDA; }
+    t_synced = now_ms();
+    for (int r = 0; r < plan.nres && plan.group_by; r++) {
+      pb200_result::Dense& d = res[r]->dense;
       if (d.pack_agg < 0) continue;
-      const int vb = (int)std::max<long long>(1, std::min<long long>((d.groups + 1023) / 1024, (long long)ctx->sm_count * 4));
-      carrier_verify_kernel<<<vb, 256, 0, st>>>((const unsigned long long*)d.isum[d.pack_agg], d.groups, d.pack_shift, dev_verify + 4 * r);
-    }
-  PB200_CUDA(cudaMemcpyAsync(pin_back, accum_buf.p, acc_bytes, cudaMemcpyDeviceToHost, st));
-  const double t_queued = now_ms();
-  cudaError_t se = cudaStreamSynchronize(st);
-  if (se != cudaSuccess) { set_error("scan kernel failed: %s", cudaGetErrorString(se)); return PB200_E_CUDA; }
-  const double t_synced = now_ms();
-  if (plan.group_by)
-    for (int r = 0; r < nres; r++) {
-      const pb200_result::Dense& d = res[r]->dense;
-      if (d.pack_agg < 0) continue;
-      const unsigned long long* vw = host_verify + 4 * r;   // {sum of counts, largest sum field, largest count}
-      const bool exact = vw[0] == host_acc[r].count;
+      const unsigned long long* vw = acc.verify(back) + 4 * r;   // {sum of counts, largest sum field, largest count}
+      const bool exact = vw[0] == AccumLayout::records(back)[r].count;
       if (d.reduce_world > 1) {
         // cross-GPU: the reduce adds `reduce_world` fields of each kind; neither can overflow if every rank's largest one
         // stays below its capacity / reduce_world.  A rank cannot rerun on its own (its peers' tables would have another
         // layout): it marks the result and the combine layer reruns the query on all ranks (PB200_Q_NO_COUNT_CARRIER).
         const unsigned long long w = (unsigned long long)d.reduce_world;
         const unsigned long long sum_lim = ((1ull << d.pack_shift) - 1ull) / w, cnt_lim = ((1ull << (64 - d.pack_shift)) - 1ull) / w;
-        res[r]->dense.carrier_unsafe = !exact || vw[1] > sum_lim || vw[2] > cnt_lim;
+        d.carrier_unsafe = !exact || vw[1] > sum_lim || vw[2] > cnt_lim;
         if (d.flag_slot) {   // the stream is idle (synchronised above): a blocking 8-byte copy, done before the call returns
           // (callers that bring their own collective read it from the block; pb200_result_combine rewrites the whole tail)
-          const long long verdict = res[r]->dense.carrier_unsafe ? 1 : 0;
+          const long long verdict = d.carrier_unsafe ? 1 : 0;
           PB200_CUDA(cudaMemcpy((long long*)d.i64_block + (d.i64_elems - 1), &verdict, 8, cudaMemcpyHostToDevice));
         }
         continue;
@@ -997,117 +1041,136 @@ static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment*
         PB200_CUDA(cudaMemcpy(ctl, d.hctl, 8, cudaMemcpyDeviceToHost));
         if (ctl[1]) continue;
       }
-      return kRetryWithoutCountCarrier;  // ResultCleanup frees the tables
+      return kRetryWithoutCountCarrier;
     }
-  float ms = 0.f;
-  cudaEventElapsedTime(&ms, e0, e1);
+    return PB200_OK;
+  }
 
-  // ---- results ----
-  for (int r = 0; r < nres; r++) {
+  // 10. aggregation only: aggregation a of result r's one row, {double, long, dictId}
+  struct AggValue { double d = 0; int64_t l = 0; int32_t id = -1; };
+  int agg_value(int r, int a, AggValue* v) {
     pb200_result& R = *res[r];
-    const AggAccum acc = host_acc[r];
-    long long total_docs = 0;
-    if (merge) for (int s = 0; s < nseg; s++) total_docs += segments[s]->num_docs; else total_docs = segments[r]->num_docs;
-    R.meta.num_group_by = ngb;
-    R.meta.num_aggs = nuser;
-    R.agg_functions.resize(nuser);
-    for (int a = 0; a < nuser; a++) R.agg_functions[a] = q.aggs[a].function;
-    for (int a = 0; a < nuser; a++)
-      if (plan.mom_first[a] >= 0) { R.mom.on[a] = true; R.mom.grid[a] = segments[merge ? 0 : r]->cols[query->aggs[a].column].moments->grid; }
-    R.meta.num_docs_scanned = (int64_t)acc.count;
-    R.meta.num_entries_scanned_in_filter = plan.in_filter[r];
-    R.meta.num_entries_scanned_post_filter = (int64_t)acc.count * plan.projected;
-    R.meta.num_total_docs = total_docs;
-    R.meta.device_ms = ms;
-    R.dbl.resize(nuser); R.lng.resize(nuser); R.ids.resize(nuser); R.distinct.resize(nuser);
-    if (!plan.group_by) {
+    const AggAccum& acc_r = AccumLayout::records(back)[r];
+    const uint32_t* host_pct = acc.pct(back) + (size_t)r * 2 * kMaxAggs;
+    const int fn = plan.q.aggs[a].function, vk = plan.q.aggs[a].val_kind;
+    const DeviceColumn* c = plan.q.aggs[a].slot < 0 ? nullptr : &segments[plan.merge ? 0 : r]->cols[query->aggs[a].column];
+    auto value_of = [&](uint32_t x) -> double {
+      if (vk == VAL_RAW_I32) return (double)(int32_t)(x ^ 0x80000000u);
+      const unsigned char* h = c->dict_host.data();
+      switch (vk) {
+        case VAL_DICT_I32: { int32_t y; memcpy(&y, h + 4ull * x, 4); return (double)y; }
+        case VAL_DICT_I64: { int64_t y; memcpy(&y, h + 8ull * x, 8); return (double)y; }
+        case VAL_DICT_F32: { float y; memcpy(&y, h + 4ull * x, 4); return (double)y; }
+        default: { double y; memcpy(&y, h + 8ull * x, 8); return y; }
+      }
+    };
+    if (fn == PB200_AGG_COUNT) { v->l = (int64_t)acc_r.count; v->d = (double)v->l; }
+    else if (is_moments_fn(fn)) {   // the exact moments from the limb sums (pb200_moments.h), rounded once
+      const int k0 = plan.mom_first[a];
+      const Moments m = moments_from_sums(acc_r.count, acc_r.isum[k0], acc_r.isum[k0 + 1], acc_r.isum[k0 + 2]);
+      v->d = moments_final(fn, m, R.mom.grid[a].e);
+      v->l = (int64_t)acc_r.count;
+      R.mom.one[a][0] = m.s1; R.mom.one[a][1] = (unsigned long long)m.s2; R.mom.one[a][2] = (unsigned long long)(m.s2 >> 64);
+    } else if (fn == PB200_AGG_SUM || fn == PB200_AGG_AVG) {
+      v->d = sum_in_double(vk) ? acc_r.dsum[a] : (double)acc_r.isum[a];
+      v->l = (int64_t)acc_r.count;
+    } else if (fn == PB200_AGG_MIN || fn == PB200_AGG_MAX) {
+      // raw INT: 0xFFFFFFFF / 0 are INT_MAX / INT_MIN as well as "no row" (max_offset): only the count tells
+      const bool mn = fn == PB200_AGG_MIN;
+      const uint32_t x = mn ? acc_r.min_id[a] : acc_r.max_id_plus1[a] - max_offset(vk);
+      const bool empty = acc_r.count == 0 || (vk != VAL_RAW_I32 && (mn ? acc_r.min_id[a] == 0xFFFFFFFFu : acc_r.max_id_plus1[a] == 0));
+      if (empty) v->d = mn ? INFINITY : -INFINITY;
+      else { v->id = (int32_t)x; v->d = c->dict_host.empty() && vk != VAL_RAW_I32 ? (double)v->id : value_of(x); }
+    } else if (fn == PB200_AGG_PERCENTILE) {
+      const uint32_t x = host_pct[a];
+      if (x == ~0u) v->d = -INFINITY;   // no matched row
+      else { v->id = (int32_t)x; v->d = value_of(x); v->l = host_pct[kMaxAggs + plan.pct_rep[a]]; }
+    } else if (fn == PB200_AGG_DISTINCTCOUNT) {
+      std::vector<uint32_t> bits(plan.distinct_words[r][a]);
+      PB200_CUDA(cudaMemcpy(bits.data(), distinct_bufs[r][a]->p, bits.size() * 4, cudaMemcpyDeviceToHost));
+      R.distinct[a].push_back(bitset_ids(bits.data(), bits.size()));
+      v->l = (int64_t)R.distinct[a].back().size(); v->d = (double)v->l;
+    }
+    return PB200_OK;
+  }
+
+  // 11. every result's metadata and (aggregation only) its row, then the group-by rows extracted, or left for
+  //     pb200_result_finalize (deferred); per-segment results release their tables
+  int fill_results_and_extract(const pb200_order_by* order) {
+    const int nuser = plan.num_user_aggs;
+    const float ms = ev.ms();
+    for (int r = 0; r < plan.nres; r++) {
+      pb200_result& R = *res[r];
+      const unsigned long long count = AccumLayout::records(back)[r].count;
+      long long total_docs = 0;
+      if (plan.merge) for (int s = 0; s < nseg; s++) total_docs += segments[s]->num_docs; else total_docs = segments[r]->num_docs;
+      R.meta.num_group_by = plan.q.num_group_by;
+      R.meta.num_aggs = nuser;
+      R.agg_functions.resize(nuser);
+      for (int a = 0; a < nuser; a++) R.agg_functions[a] = plan.q.aggs[a].function;
+      for (int a = 0; a < nuser; a++)
+        if (plan.mom_first[a] >= 0) { R.mom.on[a] = true; R.mom.grid[a] = segments[plan.merge ? 0 : r]->cols[query->aggs[a].column].moments->grid; }
+      R.meta.num_docs_scanned = (int64_t)count;
+      R.meta.num_entries_scanned_in_filter = plan.in_filter[r];
+      R.meta.num_entries_scanned_post_filter = (int64_t)count * plan.projected;
+      R.meta.num_total_docs = total_docs;
+      R.meta.device_ms = ms;
+      R.dbl.resize(nuser); R.lng.resize(nuser); R.ids.resize(nuser); R.distinct.resize(nuser);
+      if (plan.group_by) {
+        R.meta.regime = regime_of(R.dense.cards, query->max_initial_result_holder_capacity);
+        R.meta.reserved = (R.dense.pack_agg >= 0 ? 1 : 0) | (R.dense.carrier_unsafe ? 2 : 0) | (R.dense.flag_slot ? 4 : 0);  // include/pinot_b200.h
+        if (order) R.order = *order;   // a deferred result keeps it for its extraction
+        continue;
+      }
       R.meta.num_groups = -1;
       R.meta.regime = PB200_REGIME_NONE;
-      const pb200_segment* seg = segments[merge ? 0 : r];
       for (int a = 0; a < nuser; a++) {
-        const int fn = q.aggs[a].function, vk = q.aggs[a].val_kind;
-        double d = 0; int64_t l = 0; int32_t id = -1;
-        const DeviceColumn* c = q.aggs[a].slot < 0 ? nullptr : &seg->cols[query->aggs[a].column];
-        auto value_of = [&](uint32_t x) -> double {
-          if (vk == VAL_RAW_I32) return (double)(int32_t)(x ^ 0x80000000u);
-          const unsigned char* h = c->dict_host.data();
-          switch (vk) {
-            case VAL_DICT_I32: { int32_t v; memcpy(&v, h + 4ull * x, 4); return (double)v; }
-            case VAL_DICT_I64: { int64_t v; memcpy(&v, h + 8ull * x, 8); return (double)v; }
-            case VAL_DICT_F32: { float v; memcpy(&v, h + 4ull * x, 4); return (double)v; }
-            default: { double v; memcpy(&v, h + 8ull * x, 8); return v; }
-          }
-        };
-        if (fn == PB200_AGG_COUNT) { l = (int64_t)acc.count; d = (double)l; }
-        else if (is_moments_fn(fn)) {   // the exact moments from the limb sums (pb200_moments.h), rounded once
-          const int k0 = plan.mom_first[a];
-          const Moments m = moments_from_sums(acc.count, acc.isum[k0], acc.isum[k0 + 1], acc.isum[k0 + 2]);
-          d = moments_final(fn, m, R.mom.grid[a].e);
-          l = (int64_t)acc.count;
-          R.mom.one[a][0] = m.s1; R.mom.one[a][1] = (unsigned long long)m.s2; R.mom.one[a][2] = (unsigned long long)(m.s2 >> 64);
-        }
-        else if (fn == PB200_AGG_SUM || fn == PB200_AGG_AVG) {
-          d = sum_in_double(vk) ? acc.dsum[a] : (double)acc.isum[a];
-          l = (int64_t)acc.count;
-        } else if (fn == PB200_AGG_MIN || fn == PB200_AGG_MAX) {
-          // raw INT: 0xFFFFFFFF / 0 are INT_MAX / INT_MIN as well as "no row" (max_offset): only the count tells
-          const bool mn = fn == PB200_AGG_MIN;
-          const uint32_t x = mn ? acc.min_id[a] : acc.max_id_plus1[a] - max_offset(vk);
-          const bool empty = acc.count == 0 || (vk != VAL_RAW_I32 && (mn ? acc.min_id[a] == 0xFFFFFFFFu : acc.max_id_plus1[a] == 0));
-          if (empty) d = mn ? INFINITY : -INFINITY;
-          else { id = (int32_t)x; d = c->dict_host.empty() && vk != VAL_RAW_I32 ? (double)id : value_of(x); }
-        } else if (fn == PB200_AGG_PERCENTILE) {
-          const uint32_t x = host_pct[(size_t)r * 2 * kMaxAggs + a];
-          if (x == ~0u) d = -INFINITY;   // no matched row
-          else { id = (int32_t)x; d = value_of(x); l = host_pct[(size_t)r * 2 * kMaxAggs + kMaxAggs + plan.pct_rep[a]]; }
-        } else if (fn == PB200_AGG_DISTINCTCOUNT) {
-          const size_t words = plan.distinct_words[r][a];
-          std::vector<uint32_t> bits(words);
-          PB200_CUDA(cudaMemcpy(bits.data(), distinct_bufs[r][a]->p, words * 4, cudaMemcpyDeviceToHost));
-          std::vector<int32_t> idsv;
-          for (size_t w = 0; w < words; w++) { uint32_t x = bits[w]; while (x) { idsv.push_back((int32_t)(w * 32 + __builtin_ctz(x))); x &= x - 1; } }
-          l = (int64_t)idsv.size(); d = (double)l;
-          R.distinct[a].push_back(std::move(idsv));
-        }
-        R.dbl[a].push_back(d); R.lng[a].push_back(l); R.ids[a].push_back(id);
-      }
-    } else {
-      R.meta.regime = regime_of(R.dense.cards, query->max_initial_result_holder_capacity);
-      R.meta.reserved = (R.dense.pack_agg >= 0 ? 1 : 0) | (R.dense.carrier_unsafe ? 2 : 0) | (R.dense.flag_slot ? 4 : 0);  // include/pinot_b200.h
-    }
-  }
-  if (plan.group_by && order) for (int r = 0; r < nres; r++) res[r]->order = *order;  // a deferred result keeps it for its extraction
-  const double t_results = now_ms();
-  if (plan.group_by && plan.defer_finalize) {
-    for (int r = 0; r < nres; r++) { res[r]->meta.num_groups = 0; res[r]->dbl.assign(nuser, {}); res[r]->lng.assign(nuser, {}); res[r]->ids.assign(nuser, {}); res[r]->distinct.assign(nuser, {}); }
-  } else if (plan.group_by) {  // all results of the submission are extracted together (two device round trips in total)
-    std::vector<pb200_result*> rs;
-    for (int r = 0; r < nres; r++) rs.push_back(res[r].get());
-    int frc = extract_groups(ctx, rs.data(), nres, st);
-    if (frc) return frc;
-    if (!merge) {  // per-segment results do not need the dense state any more
-      for (int r = 0; r < nres; r++) {
-        pb200_result::Dense& d = res[r]->dense;
-        dev_free(ctx, d.i64_block); dev_free(ctx, d.f64_block); dev_free(ctx, d.u32max_block); dev_free(ctx, d.u32min_block);
-        dev_free(ctx, d.hkeys); dev_free(ctx, d.hctl);
-        d.hkeys = nullptr; d.hctl = nullptr;
-        for (int a = 0; a < kMaxAggs; a++) { dev_free(ctx, d.dbits[a]); d.dbits[a] = nullptr; }
-        pb200_result::Pct& p = res[r]->pct;   // the histograms stay for pb200_result_histogram
-        for (int a = 0; a < kMaxAggs; a++) { dev_free(ctx, p.ids[a]); dev_free(ctx, p.n[a]); p.ids[a] = p.n[a] = nullptr; }
-        d.i64_block = d.f64_block = d.u32max_block = d.u32min_block = nullptr;
-        d.live = false;
+        AggValue v;
+        if (int rc = agg_value(r, a, &v)) return rc;
+        R.dbl[a].push_back(v.d); R.lng[a].push_back(v.l); R.ids[a].push_back(v.id);
       }
     }
+    t_results = now_ms();
+    if (!plan.group_by) return PB200_OK;
+    if (plan.defer_finalize) {
+      for (auto& R : res) { R->meta.num_groups = 0; R->dbl.assign(nuser, {}); R->lng.assign(nuser, {}); R->ids.assign(nuser, {}); R->distinct.assign(nuser, {}); }
+      return PB200_OK;
+    }
+    std::vector<pb200_result*> rs;   // all results of the submission are extracted together (two device round trips in total)
+    for (auto& R : res) rs.push_back(R.get());
+    if (int rc = extract_groups(ctx, rs.data(), plan.nres, st)) return rc;
+    if (!plan.merge)   // per-segment results do not need the dense state any more
+      for (auto& R : res) release_tables(*R, true);
+    return PB200_OK;
   }
-  cleanup.armed = false;
-  for (int r = 0; r < nres; r++) results[r] = res[r].release();
-  const double t_exit = now_ms();
-  g_phase_ms[PB200_PHASE_PLAN] = t_launch - t_enter;       // validation, plan, table allocation + memsets queued, descriptors
-  g_phase_ms[PB200_PHASE_LAUNCH] = t_queued - t_launch;    // kernel launches queued
-  g_phase_ms[PB200_PHASE_DEVICE_WAIT] = t_synced - t_queued;
-  g_phase_ms[PB200_PHASE_RESULTS] = t_results - t_synced;  // carrier verdict, metadata, scalar results
-  g_phase_ms[PB200_PHASE_EXTRACT] = t_exit - t_results;    // group extraction (device kernels + their sync) and table release
-  g_phase_ms[PB200_PHASE_TOTAL] = t_exit - t_enter;
+
+  // 12. the results handed out, and the phases of the call (pb200_last_phases)
+  void hand_out(pb200_result** results) {
+    for (int r = 0; r < plan.nres; r++) results[r] = res[r].release();
+    const double t_exit = now_ms();
+    g_phase_ms[PB200_PHASE_PLAN] = t_launch - t_enter;       // validation, plan, table allocation + memsets queued, descriptors
+    g_phase_ms[PB200_PHASE_LAUNCH] = t_queued - t_launch;    // kernel launches queued
+    g_phase_ms[PB200_PHASE_DEVICE_WAIT] = t_synced - t_queued;
+    g_phase_ms[PB200_PHASE_RESULTS] = t_results - t_synced;  // carrier verdict, metadata, scalar results
+    g_phase_ms[PB200_PHASE_EXTRACT] = t_exit - t_results;    // group extraction (device kernels + their sync) and table release
+    g_phase_ms[PB200_PHASE_TOTAL] = t_exit - t_enter;
+  }
+};
+}  // namespace
+
+static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment* const* segments, int32_t nseg,
+                        pb200_result** results, bool allow_count_carrier, const pb200_order_by* order, const double* agg_args) {
+  ScanCall c{ctx, query, segments, nseg};
+  if (int rc = c.check_call(results)) return rc;
+  if (int rc = c.prepare_and_plan(allow_count_carrier, agg_args)) return rc;
+  if (int rc = c.alloc_results()) return rc;
+  if (int rc = c.bind_accumulators()) return rc;
+  if (int rc = c.plan.group_by ? c.bind_group_tables() : c.bind_agg_outputs()) return rc;
+  if (int rc = c.launch()) return rc;
+  if (int rc = c.finalize_percentiles()) return rc;
+  if (int rc = c.read_back_and_verify()) return rc;   // kRetryWithoutCountCarrier: ~ScanCall frees this attempt's tables
+  if (int rc = c.fill_results_and_extract(order)) return rc;
+  c.hand_out(results);
   return PB200_OK;
 }
 
@@ -1116,8 +1179,7 @@ extern "C" int32_t pb200_result_finalize(pb200_ctx* ctx, pb200_result* R) {
   pb200_result::Dense& d = R->dense;
   if (!d.ctx || d.groups <= 0 || !d.live) { set_error("result has no dense device state"); return PB200_E_INVALID; }
   PB200_CUDA(cudaSetDevice(ctx->device));
-  cudaStream_t st = take_stream(ctx);
-  struct StreamReturn { pb200_ctx* c; cudaStream_t s; ~StreamReturn() { give_stream(c, s); } } stream_return{ctx, st};
+  StreamLease st(ctx);
   pb200_result* one[1] = {R};
   return extract_groups(ctx, one, 1, st);
 }
@@ -1241,9 +1303,7 @@ extern "C" int64_t pb200_result_distinct(const pb200_result* R, int32_t a, int32
 }
 extern "C" int32_t pb200_result_free(pb200_result* R) {
   if (!R) return PB200_OK;
-  pb200_result::Dense& d = R->dense;
-  if (d.ctx) { dev_free(d.ctx, d.i64_block); dev_free(d.ctx, d.f64_block); dev_free(d.ctx, d.u32max_block); dev_free(d.ctx, d.u32min_block); dev_free(d.ctx, d.hkeys); dev_free(d.ctx, d.hctl); for (int a = 0; a < kMaxAggs; a++) dev_free(d.ctx, d.dbits[a]); }
-  if (R->pct.ctx) for (int a = 0; a < kMaxAggs; a++) { dev_free(R->pct.ctx, R->pct.hist[a]); dev_free(R->pct.ctx, R->pct.ids[a]); dev_free(R->pct.ctx, R->pct.n[a]); }
+  release_tables(*R, false);
   delete R;
   return PB200_OK;
 }

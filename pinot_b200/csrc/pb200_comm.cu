@@ -140,8 +140,7 @@ static int combine_scalars(NcclApi* api, pb200_ctx* ctx, pb200_result* R, int ro
     if (R->mom.on[a]) { set_error("VAR/STDDEV moments are merged on the host"); return PB200_E_UNSUPPORTED; }
   PB200_CUDA(cudaSetDevice(ctx->device));
   ncclComm_t comm = static_cast<ncclComm_t>(ctx->nccl_comm);
-  cudaStream_t st = take_stream(ctx);
-  struct StreamReturn { pb200_ctx* c; cudaStream_t s; ~StreamReturn() { give_stream(c, s); } } stream_return{ctx, st};
+  StreamLease st(ctx);
   std::lock_guard<std::mutex> g(ctx->comm_mu);
   // pinned / device scratch (8-byte slots): [0,4) statistics | [8,16) double sums | [16,24) long counts | [24,32) double mins | [32,40) double maxs; outputs at +64
   long long* pin = ctx->comm_pinned;
@@ -201,8 +200,7 @@ extern "C" int32_t pb200_result_combine(pb200_ctx* ctx, pb200_result* R, int32_t
   }
   PB200_CUDA(cudaSetDevice(ctx->device));
   ncclComm_t comm = static_cast<ncclComm_t>(ctx->nccl_comm);
-  cudaStream_t st = take_stream(ctx);
-  struct StreamReturn { pb200_ctx* c; cudaStream_t s; ~StreamReturn() { give_stream(c, s); } } stream_return{ctx, st};
+  StreamLease st(ctx);
   long long verdict = 0;
   {
     std::lock_guard<std::mutex> g(ctx->comm_mu);  // one communicator: collectives of concurrent queries must not interleave

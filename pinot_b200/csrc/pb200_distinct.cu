@@ -179,15 +179,6 @@ __global__ void dist_gather_kernel(const int32_t* __restrict__ pick, const unsig
   }
 }
 
-int grid_for(pb200_ctx* ctx, long long items) {
-  return (int)std::max<long long>(1, std::min<long long>((items + kThreads - 1) / kThreads, (long long)ctx->sm_count * 8));
-}
-
-struct EventPair {
-  pb200_ctx* c; cudaEvent_t a = nullptr, b = nullptr;
-  ~EventPair() { give_event(c, a); give_event(c, b); }
-};
-
 // Builds the tables from the masks of segments `ds` (one scan's worth); adds the kernels' event time to *ms.
 int build_tables(pb200_ctx* ctx, cudaStream_t st, const std::vector<DistSeg>& ds, float* ms) {
   if (ds.empty()) return PB200_OK;
@@ -196,20 +187,16 @@ int build_tables(pb200_ctx* ctx, cudaStream_t st, const std::vector<DistSeg>& ds
   DevBufRaw dd(ctx);
   if (int rc = dd.alloc(sizeof(DistSeg) * ds.size())) return rc;
   PB200_CUDA(cudaMemcpyAsync(dd.p, ds.data(), sizeof(DistSeg) * ds.size(), cudaMemcpyHostToDevice, st));
-  EventPair ev{ctx};
-  ev.a = take_event(ctx);
-  ev.b = take_event(ctx);
-  if (!ev.a || !ev.b) { set_error("cudaEventCreate failed"); return PB200_E_CUDA; }
+  EventPair ev(ctx);
+  if (int rc = ev.take()) return rc;
   PB200_CUDA(cudaEventRecord(ev.a, st));
-  const dim3 grid((unsigned)grid_for(ctx, max_words), (unsigned)ds.size());
+  const dim3 grid((unsigned)grid_for(ctx, max_words, kThreads), (unsigned)ds.size());
   dist_build_kernel<<<grid, kThreads, 0, st>>>(static_cast<const DistSeg*>(dd.p));
   PB200_CUDA(cudaGetLastError());
   PB200_CUDA(cudaEventRecord(ev.b, st));
   const cudaError_t se = cudaStreamSynchronize(st);   // the descriptors live until the build is done
   if (se != cudaSuccess) { set_error("DISTINCT table build failed: %s", cudaGetErrorString(se)); return PB200_E_CUDA; }
-  float t = 0.f;
-  cudaEventElapsedTime(&t, ev.a, ev.b);
-  *ms += t;
+  *ms += ev.ms();
   return PB200_OK;
 }
 
@@ -220,29 +207,21 @@ using namespace pb200;
 
 extern "C" int32_t pb200_execute_distinct(pb200_ctx* ctx, const pb200_query* filter_only, const pb200_selection* distinct,
                                           pb200_segment* const* segments, int32_t nseg, int32_t flags, pb200_result** results) {
-  if (!ctx || !filter_only || !distinct || !segments || !results || nseg <= 0) { set_error("invalid argument to pb200_execute_distinct"); return PB200_E_INVALID; }
-  if (flags & ~PB200_Q_MERGE_SEGMENTS) { set_error("pb200_execute_distinct: flags other than PB200_Q_MERGE_SEGMENTS"); return PB200_E_INVALID; }
-  for (int s = 0; s < nseg; s++)
-    if (!segments[s] || segments[s]->ctx != ctx) { set_error("segment %d does not belong to this context / schema", s); return PB200_E_INVALID; }
-  const double t_enter = host_ms();
-  PB200_CUDA(cudaSetDevice(ctx->device));
-  const Tuning tune = [&]() { std::lock_guard<std::mutex> g(ctx->mu); return ctx->tune; }();
-  const DeviceLimits lim{ctx->sm_count, ctx->max_smem_optin};
-  const bool merge = flags & PB200_Q_MERGE_SEGMENTS;
+  RowsCall call;
+  if (int rc = rows_call_enter(ctx, filter_only && distinct && results, segments, nseg, flags, "distinct", &call)) return rc;
+  const bool merge = call.merge;
   DistinctPlan p;
-  if (int rc = plan_distinct(tune, lim, filter_only, distinct, segments, nseg, merge, true, &p)) return rc;
-  const double t_planned = host_ms();
+  if (int rc = plan_distinct(call.tune, call.lim, filter_only, distinct, segments, nseg, merge, true, &p)) return rc;
+  call.t_planned = host_ms();
 
-  cudaStream_t st = take_stream(ctx);
-  struct StreamReturn { pb200_ctx* c; cudaStream_t s; ~StreamReturn() { give_stream(c, s); } } stream_return{ctx, st};
+  StreamLease st(ctx);
   const int nres = p.nres, nkeys = (int)p.sel.columns.size();
-  float ms = 0.f;
   DevBufRaw tables(ctx), mask1(ctx), mask2(ctx);
   if (int rc = tables.alloc(std::max<long long>(p.table_entries, 1) * 8)) return rc;
   unsigned long long* tb = static_cast<unsigned long long*>(tables.p);
   PB200_CUDA(cudaMemsetAsync(tb, 0xFF, (size_t)p.table_entries * 8, st));
   std::vector<long long> m1;
-  if (int rc = run_selection_scan(ctx, st, p.sel, mask1, m1, &ms)) return rc;
+  if (int rc = run_selection_scan(ctx, st, p.sel, mask1, m1, &call.ms)) return rc;
   auto dist_seg = [&](int s, const uint32_t* mask, long long docs) {
     DistSeg d;
     memset(&d, 0, sizeof d);
@@ -257,12 +236,13 @@ extern "C" int32_t pb200_execute_distinct(pb200_ctx* ctx, const pb200_query* fil
     }
     return d;
   };
-  std::vector<long long> matches(m1), in_filter(p.sel.scan.in_filter);
+  call.matches = m1;
+  call.in_filter = p.sel.scan.in_filter;
   {
     std::vector<DistSeg> ds;
     for (int s = 0; s < nseg; s++)
       if (m1[s] > 0) ds.push_back(dist_seg(s, static_cast<const uint32_t*>(mask1.p) + p.sel.mask_word_off[s], p.sel.scan_docs[s]));
-    if (int rc = build_tables(ctx, st, ds, &ms)) return rc;
+    if (int rc = build_tables(ctx, st, ds, &call.ms)) return rc;
   }
   if (p.sel.prefix) {
     // ---- the prefix-final rule: count the entries below each result's bound ----
@@ -280,7 +260,7 @@ extern "C" int32_t pb200_execute_distinct(pb200_ctx* ctx, const pb200_query* fil
     PB200_CUDA(cudaMemsetAsync(dbelow, 0, (size_t)nres * 8, st));
     long long max_size = 0;
     for (long long z : p.table_size) max_size = std::max(max_size, z);
-    dist_below_kernel<<<dim3((unsigned)grid_for(ctx, max_size), (unsigned)nres), kThreads, 0, st>>>(tb, doff, dsize, dbound, dbelow);
+    dist_below_kernel<<<dim3((unsigned)grid_for(ctx, max_size, kThreads), (unsigned)nres), kThreads, 0, st>>>(tb, doff, dsize, dbound, dbelow);
     PB200_CUDA(cudaGetLastError());
     std::vector<long long> below(nres);
     PB200_CUDA(cudaMemcpyAsync(below.data(), dbelow, (size_t)nres * 8, cudaMemcpyDeviceToHost, st));
@@ -289,19 +269,19 @@ extern "C" int32_t pb200_execute_distinct(pb200_ctx* ctx, const pb200_query* fil
     if (!rescan.empty()) {
       const Rescan rs = rescan_query(*filter_only, segments, rescan);
       SelectionPlan p2;
-      if (int rc = plan_selection(tune, lim, &rs.query, distinct, rs.segs.data(), (int)rs.segs.size(), false, &p2)) return rc;
+      if (int rc = plan_selection(call.tune, call.lim, &rs.query, distinct, rs.segs.data(), (int)rs.segs.size(), false, &p2)) return rc;
       std::vector<long long> m2;
-      if (int rc = run_selection_scan(ctx, st, p2, mask2, m2, &ms)) return rc;
+      if (int rc = run_selection_scan(ctx, st, p2, mask2, m2, &call.ms)) return rc;
       std::vector<DistSeg> ds;
       for (size_t i = 0; i < rescan.size(); i++) {
         const int s = rescan[i];
-        matches[s] = m2[i]; in_filter[s] = p2.scan.in_filter[i];
+        call.matches[s] = m2[i]; call.in_filter[s] = p2.scan.in_filter[i];
         if (m2[i] > 0) ds.push_back(dist_seg(s, static_cast<const uint32_t*>(mask2.p) + p2.mask_word_off[i], p2.scan_docs[i]));
       }
-      if (int rc = build_tables(ctx, st, ds, &ms)) return rc;
+      if (int rc = build_tables(ctx, st, ds, &call.ms)) return rc;
     }
   }
-  const double t_scanned = host_ms();
+  call.t_scanned = host_ms();
 
   // ---- extraction: compact, count per result ----
   const long long nent = p.table_entries;
@@ -372,7 +352,7 @@ extern "C" int32_t pb200_execute_distinct(pb200_ctx* ctx, const pb200_query* fil
     int32_t* v0 = reinterpret_cast<int32_t*>(k1 + n);
     int32_t* v1 = v0 + n;
     int32_t* pick = v1 + n;
-    const int cgrid = grid_for(ctx, n);
+    const int cgrid = grid_for(ctx, n, kThreads);
     dist_fill_kernel<<<cgrid, kThreads, 0, st>>>(tb, static_cast<const int32_t*>(pos.p), n, doff, merge, occ0, raw, v0);
     PB200_CUDA(cudaGetLastError());
     size_t sort_bytes = 0, key_bytes = 0;
@@ -400,57 +380,21 @@ extern "C" int32_t pb200_execute_distinct(pb200_ctx* ctx, const pb200_query* fil
         PB200_CUDA(cub::DeviceRadixSort::SortPairs(stmp.p, key_bytes, kb, vb, (int)n, 0, bits, st));
       }
     }
-    dist_pick_kernel<<<dim3((unsigned)grid_for(ctx, p.sel.limit), (unsigned)nres), kThreads, 0, st>>>(static_cast<const DistRes*>(dres.p), vb.Current(), pick);
+    dist_pick_kernel<<<dim3((unsigned)grid_for(ctx, p.sel.limit, kThreads), (unsigned)nres), kThreads, 0, st>>>(static_cast<const DistRes*>(dres.p), vb.Current(), pick);
     PB200_CUDA(cudaGetLastError());
     unsigned char* dst = nullptr;
-    const bool mapped = out_bytes <= kSelMappedBytes;
-    if (mapped) {
-      void* dp = nullptr;
-      PB200_CUDA(cudaHostGetDevicePointer(&dp, block->p, 0));
-      dst = static_cast<unsigned char*>(dp);
-    } else {
-      if (int rc = staging.alloc(out_bytes)) return rc;
-      dst = static_cast<unsigned char*>(staging.p);
-    }
-    dist_gather_kernel<<<grid_for(ctx, total_rows), kThreads, 0, st>>>(pick, occ, raw, total_rows, static_cast<const SelCol*>(dcols.p),
+    if (int rc = rows_output(*block, out_bytes, staging, &dst)) return rc;
+    dist_gather_kernel<<<grid_for(ctx, total_rows, kThreads), kThreads, 0, st>>>(pick, occ, raw, total_rows, static_cast<const SelCol*>(dcols.p),
                                                                        static_cast<const DistKey*>(dkeys.p), nkeys, dst);
     PB200_CUDA(cudaGetLastError());
-    if (!mapped) PB200_CUDA(cudaMemcpyAsync(block->p, staging.p, out_bytes, cudaMemcpyDeviceToHost, st));
+    if (staging.p) PB200_CUDA(cudaMemcpyAsync(block->p, staging.p, out_bytes, cudaMemcpyDeviceToHost, st));
     const cudaError_t se = cudaStreamSynchronize(st);
     if (se != cudaSuccess) { set_error("DISTINCT extraction failed: %s", cudaGetErrorString(se)); return PB200_E_CUDA; }
   }
 
   // ---- results: row ranges of the one block ----
-  unsigned char* base = static_cast<unsigned char*>(block->p);
-  int32_t* all_docs = reinterpret_cast<int32_t*>(base);
-  int32_t* all_segs = all_docs + total_rows;
-  const unsigned long long* all_cols = reinterpret_cast<const unsigned long long*>(base + 8 * total_rows);
-  for (int r = 0; r < nres; r++) {
-    const int s0 = merge ? 0 : r, s1 = merge ? nseg : r + 1;
-    std::unique_ptr<pb200_result> R(new pb200_result());
-    pb200_result::Selection& v = R->selection;
-    v.present = true;
-    v.block = block;
-    long long docs_scanned = 0, entries = 0, total_docs = 0;
-    for (int s = s0; s < s1; s++) { docs_scanned += matches[s]; entries += in_filter[s]; total_docs += segments[s]->num_docs; }
-    v.rows = res[r].rows;
-    v.doc_ids = all_docs + res[r].row_off;
-    v.segment_index = all_segs + res[r].row_off;
-    for (int k = 0; k < nkeys; k++) v.columns.push_back(all_cols + (size_t)k * total_rows + res[r].row_off);
-    R->meta.num_groups = (int32_t)v.rows;
-    R->meta.regime = PB200_REGIME_NONE;
-    R->meta.num_docs_scanned = docs_scanned;
-    R->meta.num_entries_scanned_in_filter = entries;
-    R->meta.num_entries_scanned_post_filter = docs_scanned * nkeys;
-    R->meta.num_total_docs = total_docs;
-    R->meta.device_ms = ms;
-    results[r] = R.release();
-  }
-  const double t_exit = host_ms();
-  for (int ph = 0; ph < PB200_NUM_PHASES; ph++) set_phase_ms(ph, 0.0);
-  set_phase_ms(PB200_PHASE_PLAN, t_planned - t_enter);
-  set_phase_ms(PB200_PHASE_DEVICE_WAIT, t_scanned - t_planned);
-  set_phase_ms(PB200_PHASE_EXTRACT, t_exit - t_scanned);
-  set_phase_ms(PB200_PHASE_TOTAL, t_exit - t_enter);
+  std::vector<std::pair<long long, long long>> ranges;
+  for (const DistRes& g : res) ranges.emplace_back(g.row_off, g.rows);
+  rows_results(call, block, total_rows, nkeys, ranges, false, results);
   return PB200_OK;
 }

@@ -312,8 +312,7 @@ extern "C" int32_t pb200_segment_bind_domain(pb200_ctx* ctx, pb200_segment* seg,
     work.push_back(std::move(w));
   }
   // ---- pass 2: re-encode ----
-  cudaStream_t st = take_stream(ctx);
-  struct StreamReturn { pb200_ctx* c; cudaStream_t s; ~StreamReturn() { give_stream(c, s); } } stream_return{ctx, st};
+  StreamLease st(ctx);
   for (auto& w : work) {
     DeviceColumn& c = seg->cols[w.col];
     const pb200_domain::Col& dc = *w.dc;

@@ -454,7 +454,7 @@ int extract_groups(pb200_ctx* ctx, pb200_result* const* Rs, int nres, cudaStream
     extract_write_kernel<<<chunks, kExtractThreads, 0, st>>>(ddescs, nres, (const uint32_t*)dcount.p, totals, out, true);
     for (int r = 0; r < nres; r++) {
       const size_t cap = descs[r].idx_cap;
-      const int grid = (int)std::max<size_t>(1, std::min<size_t>((cap + kExtractThreads - 1) / kExtractThreads, (size_t)ctx->sm_count * 8));
+      const int grid = grid_for(ctx, (long long)cap, kExtractThreads);
       for (size_t p = 0; p < passes[r].size(); p++) {
         const OrderPass& op = passes[r][p];
         order_key_kernel<<<grid, kExtractThreads, 0, st>>>(ddescs, r, op, totals, sb[r].v[p % 2], sb[r].k[0]);
@@ -537,8 +537,7 @@ int extract_groups(pb200_ctx* ctx, pb200_result* const* Rs, int nres, cudaStream
       if (rows) {
         DevBufRaw g(ctx);
         if ((rc = g.alloc(rows * wpg * 4))) return rc;
-        const int gb2 = (int)std::max<size_t>(1, std::min<size_t>((rows * wpg + 255) / 256, (size_t)ctx->sm_count * 8));
-        gather_bitset_rows_kernel<<<gb2, 256, 0, st>>>(d.dbits[a], reinterpret_cast<const uint32_t*>(out + e.off_idx), (long long)rows, (int)wpg, (uint32_t*)g.p);
+        gather_bitset_rows_kernel<<<grid_for(ctx, (long long)(rows * wpg), 256), 256, 0, st>>>(d.dbits[a], reinterpret_cast<const uint32_t*>(out + e.off_idx), (long long)rows, (int)wpg, (uint32_t*)g.p);
         PB200_CUDA(cudaMemcpyAsync(bits.data(), g.p, rows * wpg * 4, cudaMemcpyDeviceToHost, st));
         PB200_CUDA(cudaStreamSynchronize(st));
       }
@@ -546,13 +545,18 @@ int extract_groups(pb200_ctx* ctx, pb200_result* const* Rs, int nres, cudaStream
       int64_t* sizes = const_cast<int64_t*>(v.lng[a]);   // the kernel left zeros: the set sizes go here
       double* dsz = const_cast<double*>(v.dbl[a]);
       for (size_t i = 0; i < rows; i++) {
-        std::vector<int32_t>& ids = R->distinct[a][i];
-        for (size_t w = 0; w < wpg; w++) { uint32_t x = bits[i * wpg + w]; while (x) { ids.push_back((int32_t)(w * 32 + __builtin_ctz(x))); x &= x - 1; } }
-        sizes[i] = (int64_t)ids.size(); dsz[i] = (double)ids.size();
+        R->distinct[a][i] = bitset_ids(bits.data() + i * wpg, wpg);
+        sizes[i] = (int64_t)R->distinct[a][i].size(); dsz[i] = (double)sizes[i];
       }
     }
   }
   return PB200_OK;
+}
+
+std::vector<int32_t> bitset_ids(const uint32_t* bits, size_t words) {
+  std::vector<int32_t> ids;
+  for (size_t w = 0; w < words; w++) for (uint32_t x = bits[w]; x; x &= x - 1) ids.push_back((int32_t)(w * 32 + __builtin_ctz(x)));
+  return ids;
 }
 
 // Copies a view-backed result into the std::vector fields (host-side consumers that re-map results: star-tree).

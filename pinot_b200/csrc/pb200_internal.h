@@ -286,6 +286,36 @@ struct DevBufRaw {  // RAII pooled device buffer
   ~DevBufRaw() { dev_free(ctx, p); }
   int alloc(size_t bytes) { return dev_alloc(ctx, bytes, &p); }
 };
+struct StreamLease {  // RAII stream of the context's pool; converts to the stream
+  pb200_ctx* ctx;
+  cudaStream_t s;
+  explicit StreamLease(pb200_ctx* c) : ctx(c), s(take_stream(c)) {}
+  StreamLease(const StreamLease&) = delete;
+  StreamLease& operator=(const StreamLease&) = delete;
+  ~StreamLease() { give_stream(ctx, s); }
+  operator cudaStream_t() const { return s; }
+};
+struct EventPair {  // two pooled events around queued work (creating / destroying them per query costs more than a launch)
+  pb200_ctx* ctx;
+  cudaEvent_t a = nullptr, b = nullptr;
+  explicit EventPair(pb200_ctx* c) : ctx(c) {}
+  EventPair(const EventPair&) = delete;
+  EventPair& operator=(const EventPair&) = delete;
+  ~EventPair() { give_event(ctx, a); give_event(ctx, b); }
+  int take() {
+    a = take_event(ctx);
+    b = take_event(ctx);
+    if (!a || !b) { set_error("cudaEventCreate failed"); return PB200_E_CUDA; }
+    return PB200_OK;
+  }
+  float ms() const { float t = 0.f; cudaEventElapsedTime(&t, a, b); return t; }
+};
+// grid of a grid-stride kernel over `items`: one thread per item, at most 8 blocks per SM
+inline int grid_for(const pb200_ctx* ctx, long long items, int threads) {
+  return (int)std::max<long long>(1, std::min<long long>((items + threads - 1) / threads, (long long)ctx->sm_count * 8));
+}
+// dictIds of the set bits of a DISTINCTCOUNT bitset (bit j of word w = dictId 32w + j), ascending
+std::vector<int32_t> bitset_ids(const uint32_t* bits, size_t words);
 // pb200_extract.cu: non-empty groups of the results' device tables -> final layout in pinned memory (all results at once)
 int extract_groups(pb200_ctx* ctx, pb200_result* const* results, int nres, cudaStream_t st);
 void result_materialize(pb200_result* R);  // view -> the std::vector fields

@@ -48,8 +48,7 @@ static int ensure_limbs(pb200_ctx* ctx, pb200_segment* seg, DeviceColumn& c) {
     void* p = nullptr;
     if (int rc = dev_alloc(ctx, bytes, &p)) return rc;
     cudaStream_t st = take_stream(ctx);
-    const int grid_dim = (int)std::max<long long>(1, std::min<long long>((c.cardinality + 255) / 256, (long long)ctx->sm_count * 8));
-    limb_build_kernel<<<grid_dim, 256, 0, st>>>(c.dict_native, grid, c.cardinality, (uint32_t*)p);
+    limb_build_kernel<<<grid_for(ctx, c.cardinality, 256), 256, 0, st>>>(c.dict_native, grid, c.cardinality, (uint32_t*)p);
     cudaError_t e = cudaGetLastError();
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     give_stream(ctx, st);

@@ -101,11 +101,8 @@ int percentile_finalize(pb200_ctx* ctx, cudaStream_t st, const PercentileJob& jo
   if (int rc = temps.back()->alloc(4ull * (size_t)j.rows * j.nchunks)) return rc;
   uint32_t* sums = static_cast<uint32_t*>(temps.back()->p);
   const long long warps1 = j.rows * (long long)j.nchunks;
-  const int cap = ctx->sm_count * 8;
-  const int g1 = (int)std::max<long long>(1, std::min<long long>((warps1 * 32 + kHistThreads - 1) / kHistThreads, cap));
-  hist_chunk_sum_kernel<<<g1, kHistThreads, 0, st>>>(j.hist, j.rows, j.E, j.nchunks, sums);
-  const int g2 = (int)std::max<long long>(1, std::min<long long>((j.rows * 32 + kHistThreads - 1) / kHistThreads, cap));
-  hist_select_kernel<<<g2, kHistThreads, 0, st>>>(j, sums);
+  hist_chunk_sum_kernel<<<grid_for(ctx, warps1 * 32, kHistThreads), kHistThreads, 0, st>>>(j.hist, j.rows, j.E, j.nchunks, sums);
+  hist_select_kernel<<<grid_for(ctx, j.rows * 32, kHistThreads), kHistThreads, 0, st>>>(j, sums);
   PB200_CUDA(cudaGetLastError());
   return PB200_OK;
 }
@@ -115,16 +112,14 @@ int percentile_read_rows(pb200_ctx* ctx, const uint32_t* hist, const uint32_t* i
   out.assign((size_t)rows * E, 0u);
   if (!rows || !E) return PB200_OK;
   PB200_CUDA(cudaSetDevice(ctx->device));
-  cudaStream_t st = take_stream(ctx);
-  struct StreamReturn { pb200_ctx* c; cudaStream_t s; ~StreamReturn() { give_stream(c, s); } } stream_return{ctx, st};
+  StreamLease st(ctx);
   DevBufRaw rows_dev(ctx), g(ctx);
   const uint32_t* src = hist;
   if (idx) {   // group-by: the histogram rows of the result's rows, in row order
     if (int rc = rows_dev.alloc(4ull * rows)) return rc;
     if (int rc = g.alloc(4ull * rows * E)) return rc;
     PB200_CUDA(cudaMemcpyAsync(rows_dev.p, idx, 4ull * rows, cudaMemcpyHostToDevice, st));
-    const int gb = (int)std::max<long long>(1, std::min<long long>((rows * (long long)E + 255) / 256, (long long)ctx->sm_count * 8));
-    hist_gather_rows_kernel<<<gb, 256, 0, st>>>(hist, (const uint32_t*)rows_dev.p, rows, E, (uint32_t*)g.p);
+    hist_gather_rows_kernel<<<grid_for(ctx, rows * (long long)E, 256), 256, 0, st>>>(hist, (const uint32_t*)rows_dev.p, rows, E, (uint32_t*)g.p);
     PB200_CUDA(cudaGetLastError());
     src = (const uint32_t*)g.p;
   }

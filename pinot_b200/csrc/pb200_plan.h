@@ -181,6 +181,11 @@ TmaTable tma_table(const ScanPlan& plan, const LaunchChunk& c);
 // pb200_api.cu: allocates and fills the device buffers plan.leaf_buffers lists on `st` and points the leaf descriptors of
 // plan.segs at them; the buffers stay in `temps` until the launch that reads them is done.
 int bind_leaf_buffers(pb200_ctx* ctx, ScanPlan& plan, cudaStream_t st, std::vector<std::unique_ptr<DevBufRaw>>& temps);
+// pb200_api.cu: copies plan.segs into `dsegs` (allocated here) and launches every chunk on `st` between the events of `ev`
+// (taken here).  mask: a selection scan's match mask, chunk c writing from word chunk_word_off[c] (NULL: none).  t_launch
+// (if set): the host clock once the descriptors are queued.  A launch that fails is reported as "<what> launch failed".
+int launch_chunks(pb200_ctx* ctx, cudaStream_t st, const ScanPlan& plan, DevBufRaw& dsegs, EventPair& ev, const char* what,
+                  uint32_t* mask, const long long* chunk_word_off, double* t_launch);
 
 // pb200_select.cu: one scan launch of a selection plan on `st`: fills `mask` (p.mask_words words) and the matched docs of
 // each segment, adds the scan's CUDA-event time to *ms; ends in a stream synchronisation.

@@ -169,11 +169,6 @@ __global__ void sel_gather_kernel(const int32_t* __restrict__ docs, const int32_
   }
 }
 
-struct EventPair {
-  pb200_ctx* c; cudaEvent_t a = nullptr, b = nullptr;
-  ~EventPair() { give_event(c, a); give_event(c, b); }
-};
-
 }  // namespace
 
 int run_selection_scan(pb200_ctx* ctx, cudaStream_t st, SelectionPlan& p, DevBufRaw& mask, std::vector<long long>& matches,
@@ -184,38 +179,81 @@ int run_selection_scan(pb200_ctx* ctx, cudaStream_t st, SelectionPlan& p, DevBuf
   if (int rc = bind_leaf_buffers(ctx, plan, st, temps)) return rc;
   const size_t acc_bytes = sizeof(AggAccum) * nseg;
   DevBufRaw accum(ctx), dsegs(ctx);
+  EventPair ev(ctx);
   if (int rc = accum.alloc(acc_bytes)) return rc;
-  if (int rc = dsegs.alloc(sizeof(SegDesc) * nseg)) return rc;
   if (int rc = mask.alloc(std::max<long long>(p.mask_words, 1) * 4)) return rc;  // every word is written by the launch
   PB200_CUDA(cudaMemsetAsync(accum.p, 0, acc_bytes, st));
   for (int s = 0; s < nseg; s++) plan.segs[s].accum = static_cast<AggAccum*>(accum.p) + s;
-  PB200_CUDA(cudaMemcpyAsync(dsegs.p, plan.segs.data(), sizeof(SegDesc) * nseg, cudaMemcpyHostToDevice, st));
-  EventPair ev{ctx};
-  ev.a = take_event(ctx);
-  ev.b = take_event(ctx);
-  if (!ev.a || !ev.b) { set_error("cudaEventCreate failed"); return PB200_E_CUDA; }
-  PB200_CUDA(cudaEventRecord(ev.a, st));
-  for (size_t c = 0; c < plan.chunks.size(); c++) {
-    const LaunchChunk& ch = plan.chunks[c];
-    QueryDesc cq = plan.q;
-    cq.num_segments = ch.num_segs;
-    cq.total_tiles = ch.total_tiles;
-    set_selection_mask(cq, static_cast<uint32_t*>(mask.p) + p.chunk_word_off[c]);
-    const cudaError_t le = launch_scan_variant(plan.variant, plan.smem_bytes, ch.grid, cq, tma_table(plan, ch),
-                                               static_cast<const SegDesc*>(dsegs.p) + ch.first_seg, st);
-    if (le != cudaSuccess) { set_error("selection scan launch failed: %s (smem %zu B, grid %d)", cudaGetErrorString(le), plan.smem_bytes, ch.grid); return PB200_E_CUDA; }
-  }
-  PB200_CUDA(cudaEventRecord(ev.b, st));
+  if (int rc = launch_chunks(ctx, st, plan, dsegs, ev, "selection scan", static_cast<uint32_t*>(mask.p), p.chunk_word_off.data(), nullptr)) return rc;
   std::vector<AggAccum> acc(nseg);
   PB200_CUDA(cudaMemcpyAsync(acc.data(), accum.p, acc_bytes, cudaMemcpyDeviceToHost, st));
   const cudaError_t se = cudaStreamSynchronize(st);
   if (se != cudaSuccess) { set_error("selection scan failed: %s", cudaGetErrorString(se)); return PB200_E_CUDA; }
   matches.resize(nseg);
   for (int s = 0; s < nseg; s++) matches[s] = (long long)acc[s].count;
-  float t = 0.f;
-  cudaEventElapsedTime(&t, ev.a, ev.b);
-  *ms += t;
+  *ms += ev.ms();
   return PB200_OK;
+}
+
+int rows_call_enter(pb200_ctx* ctx, bool args_ok, pb200_segment* const* segments, int nseg, int32_t flags, const char* fn,
+                    RowsCall* c) {
+  if (!ctx || !args_ok || !segments || nseg <= 0) { set_error("invalid argument to pb200_execute_%s", fn); return PB200_E_INVALID; }
+  if (flags & ~PB200_Q_MERGE_SEGMENTS) { set_error("pb200_execute_%s: flags other than PB200_Q_MERGE_SEGMENTS", fn); return PB200_E_INVALID; }
+  for (int s = 0; s < nseg; s++)
+    if (!segments[s] || segments[s]->ctx != ctx) { set_error("segment %d does not belong to this context / schema", s); return PB200_E_INVALID; }
+  c->segments = segments;
+  c->nseg = nseg;
+  c->merge = flags & PB200_Q_MERGE_SEGMENTS;
+  c->t_enter = host_ms();
+  PB200_CUDA(cudaSetDevice(ctx->device));
+  std::lock_guard<std::mutex> g(ctx->mu);
+  c->tune = ctx->tune;
+  c->lim = DeviceLimits{ctx->sm_count, ctx->max_smem_optin};
+  return PB200_OK;
+}
+
+int rows_output(const PinnedBlock& block, size_t bytes, DevBufRaw& staging, unsigned char** dst) {
+  void* p = nullptr;
+  if (bytes > kSelMappedBytes) { if (int rc = staging.alloc(bytes)) return rc; p = staging.p; }
+  else PB200_CUDA(cudaHostGetDevicePointer(&p, block.p, 0));
+  *dst = static_cast<unsigned char*>(p);
+  return PB200_OK;
+}
+
+void rows_results(const RowsCall& c, const std::shared_ptr<PinnedBlock>& block, long long total_rows, int ncols,
+                  const std::vector<std::pair<long long, long long>>& ranges, bool per_row, pb200_result** results) {
+  unsigned char* base = static_cast<unsigned char*>(block->p);
+  int32_t* all_docs = reinterpret_cast<int32_t*>(base);
+  int32_t* all_segs = all_docs + total_rows;
+  const unsigned long long* all_cols = reinterpret_cast<const unsigned long long*>(base + 8 * total_rows);
+  for (int r = 0; r < (int)ranges.size(); r++) {
+    const int s0 = c.merge ? 0 : r, s1 = c.merge ? c.nseg : r + 1;
+    const long long off = ranges[r].first;
+    std::unique_ptr<pb200_result> R(new pb200_result());
+    pb200_result::Selection& v = R->selection;
+    v.present = true;
+    v.block = block;
+    long long docs_scanned = 0, entries = 0, total_docs = 0;
+    for (int s = s0; s < s1; s++) { docs_scanned += c.matches[s]; entries += c.in_filter[s]; total_docs += c.segments[s]->num_docs; }
+    v.rows = ranges[r].second;
+    v.doc_ids = all_docs + off;
+    v.segment_index = all_segs + off;
+    for (int k = 0; k < ncols; k++) v.columns.push_back(all_cols + (size_t)k * total_rows + off);
+    R->meta.num_groups = (int32_t)v.rows;
+    R->meta.regime = PB200_REGIME_NONE;
+    R->meta.num_docs_scanned = docs_scanned;
+    R->meta.num_entries_scanned_in_filter = entries;
+    R->meta.num_entries_scanned_post_filter = (per_row ? v.rows : docs_scanned) * ncols;
+    R->meta.num_total_docs = total_docs;
+    R->meta.device_ms = c.ms;
+    results[r] = R.release();
+  }
+  const double t_exit = host_ms();
+  for (int ph = 0; ph < PB200_NUM_PHASES; ph++) set_phase_ms(ph, 0.0);
+  set_phase_ms(PB200_PHASE_PLAN, c.t_planned - c.t_enter);
+  set_phase_ms(PB200_PHASE_DEVICE_WAIT, c.t_scanned - c.t_planned);
+  set_phase_ms(PB200_PHASE_EXTRACT, t_exit - c.t_scanned);
+  set_phase_ms(PB200_PHASE_TOTAL, t_exit - c.t_enter);
 }
 
 namespace {
@@ -254,51 +292,42 @@ using namespace pb200;
 
 extern "C" int32_t pb200_execute_selection(pb200_ctx* ctx, const pb200_query* filter_only, const pb200_selection* sel,
                                            pb200_segment* const* segments, int32_t nseg, int32_t flags, pb200_result** results) {
-  if (!ctx || !filter_only || !sel || !segments || !results || nseg <= 0) { set_error("invalid argument to pb200_execute_selection"); return PB200_E_INVALID; }
-  if (flags & ~PB200_Q_MERGE_SEGMENTS) { set_error("pb200_execute_selection: flags other than PB200_Q_MERGE_SEGMENTS"); return PB200_E_INVALID; }
-  for (int s = 0; s < nseg; s++)
-    if (!segments[s] || segments[s]->ctx != ctx) { set_error("segment %d does not belong to this context / schema", s); return PB200_E_INVALID; }
-  const double t_enter = host_ms();
-  PB200_CUDA(cudaSetDevice(ctx->device));
-  const Tuning tune = [&]() { std::lock_guard<std::mutex> g(ctx->mu); return ctx->tune; }();
-  const DeviceLimits lim{ctx->sm_count, ctx->max_smem_optin};
+  RowsCall call;
+  if (int rc = rows_call_enter(ctx, filter_only && sel && results, segments, nseg, flags, "selection", &call)) return rc;
   SelectionPlan p1;
-  if (int rc = plan_selection(tune, lim, filter_only, sel, segments, nseg, true, &p1)) return rc;
-  const double t_planned = host_ms();
+  if (int rc = plan_selection(call.tune, call.lim, filter_only, sel, segments, nseg, true, &p1)) return rc;
+  call.t_planned = host_ms();
 
-  cudaStream_t st = take_stream(ctx);
-  struct StreamReturn { pb200_ctx* c; cudaStream_t s; ~StreamReturn() { give_stream(c, s); } } stream_return{ctx, st};
-  float ms = 0.f;
+  StreamLease st(ctx);
   DevBufRaw mask1(ctx), mask2(ctx);
   std::vector<long long> m1;
-  if (int rc = run_selection_scan(ctx, st, p1, mask1, m1, &ms)) return rc;
+  if (int rc = run_selection_scan(ctx, st, p1, mask1, m1, &call.ms)) return rc;
 
   // where each segment's rows come from: the prefix pass, or the full rescan
   std::vector<const uint32_t*> smask(nseg);
-  std::vector<long long> sdocs(nseg), matches(nseg), in_filter(nseg);
-  for (int s = 0; s < nseg; s++) {
-    smask[s] = static_cast<const uint32_t*>(mask1.p) + p1.mask_word_off[s];
-    sdocs[s] = p1.scan_docs[s]; matches[s] = m1[s]; in_filter[s] = p1.scan.in_filter[s];
-  }
+  std::vector<long long> sdocs(p1.scan_docs);
+  call.matches = m1;
+  call.in_filter = p1.scan.in_filter;
+  for (int s = 0; s < nseg; s++) smask[s] = static_cast<const uint32_t*>(mask1.p) + p1.mask_word_off[s];
   const std::vector<int> rescan = selection_rescan(p1, segments, m1);
   if (!rescan.empty()) {
     const Rescan rs = rescan_query(*filter_only, segments, rescan);
     SelectionPlan p2;
-    if (int rc = plan_selection(tune, lim, &rs.query, sel, rs.segs.data(), (int)rs.segs.size(), false, &p2)) return rc;
+    if (int rc = plan_selection(call.tune, call.lim, &rs.query, sel, rs.segs.data(), (int)rs.segs.size(), false, &p2)) return rc;
     std::vector<long long> m2;
-    if (int rc = run_selection_scan(ctx, st, p2, mask2, m2, &ms)) return rc;
+    if (int rc = run_selection_scan(ctx, st, p2, mask2, m2, &call.ms)) return rc;
     for (size_t i = 0; i < rescan.size(); i++) {
       const int s = rescan[i];
       smask[s] = static_cast<const uint32_t*>(mask2.p) + p2.mask_word_off[i];
-      sdocs[s] = p2.scan_docs[i]; matches[s] = m2[i]; in_filter[s] = p2.scan.in_filter[i];
+      sdocs[s] = p2.scan_docs[i]; call.matches[s] = m2[i]; call.in_filter[s] = p2.scan.in_filter[i];
     }
   }
-  const double t_scanned = host_ms();
+  call.t_scanned = host_ms();
 
   // ---- rows.  Selection only: per segment its first min(limit, matches) matches, merged: segments in submission order
   //      up to `limit`.  ORDER BY: per segment its top min(limit, matches) rows; merged, the tops are merged by value below.
-  const bool merge = flags & PB200_Q_MERGE_SEGMENTS;
-  const int nres = merge ? 1 : nseg;
+  const bool merge = call.merge;
+  const std::vector<long long>& matches = call.matches;
   const int ncols = (int)p1.columns.size();
   const int nitems = (int)p1.order_cols.size();
   const bool ordered = nitems > 0;
@@ -345,7 +374,7 @@ extern "C" int32_t pb200_execute_selection(pb200_ctx* ctx, const pb200_query* fi
     PB200_CUDA(cudaMemcpyAsync(dsc.p, sc.data(), sizeof(SelCol) * sc.size(), cudaMemcpyHostToDevice, st));
     PB200_CUDA(cudaMemcpyAsync(dsk.p, sk.data(), sizeof(SelCol) * sk.size(), cudaMemcpyHostToDevice, st));
     const SelCol* keys = ordered ? static_cast<const SelCol*>(dsk.p) : nullptr;
-    const dim3 wgrid((unsigned)std::max<long long>(1, std::min<long long>((max_words + kSelThreads - 1) / kSelThreads, (long long)ctx->sm_count * 8)), (unsigned)nseg);
+    const dim3 wgrid((unsigned)grid_for(ctx, max_words, kSelThreads), (unsigned)nseg);
     if (ordered) {
       // ---- threshold bucket per segment: the better buckets plus it hold at least `rows` matches ----
       if (int rc = hist.alloc((size_t)nseg * kHistBins * 4)) return rc;
@@ -399,7 +428,7 @@ extern "C" int32_t pb200_execute_selection(pb200_ctx* ctx, const pb200_query* fi
       int32_t* v0 = reinterpret_cast<int32_t*>(k1 + ncand);
       int32_t* v1 = v0 + ncand;
       int32_t* pk = v1 + ncand;
-      const int cgrid = (int)std::max<long long>(1, std::min<long long>((ncand + kSelThreads - 1) / kSelThreads, (long long)ctx->sm_count * 8));
+      const int cgrid = grid_for(ctx, ncand, kSelThreads);
       sel_iota_kernel<<<cgrid, kSelThreads, 0, st>>>(v0, ncand);
       cub::DoubleBuffer<uint32_t> kb(k0, k1);
       cub::DoubleBuffer<int32_t> vb(v0, v1);
@@ -417,27 +446,18 @@ extern "C" int32_t pb200_execute_selection(pb200_ctx* ctx, const pb200_query* fi
       pick = pk;
     }
     unsigned char* dst = nullptr;
-    const bool mapped = out_bytes <= kSelMappedBytes;
-    if (mapped) {
-      void* dp = nullptr;
-      PB200_CUDA(cudaHostGetDevicePointer(&dp, block->p, 0));
-      dst = static_cast<unsigned char*>(dp);
-    } else {
-      if (int rc = staging.alloc(out_bytes)) return rc;
-      dst = static_cast<unsigned char*>(staging.p);
-    }
-    const int ggrid = (int)std::max<long long>(1, std::min<long long>((total_rows + kSelThreads - 1) / kSelThreads, (long long)ctx->sm_count * 8));
-    sel_gather_kernel<<<ggrid, kSelThreads, 0, st>>>(cdoc, cseg, pick, total_rows, static_cast<const SelCol*>(dsc.p), gcols, dst);
+    if (int rc = rows_output(*block, out_bytes, staging, &dst)) return rc;
+    sel_gather_kernel<<<grid_for(ctx, total_rows, kSelThreads), kSelThreads, 0, st>>>(cdoc, cseg, pick, total_rows, static_cast<const SelCol*>(dsc.p), gcols, dst);
     PB200_CUDA(cudaGetLastError());
-    if (!mapped) PB200_CUDA(cudaMemcpyAsync(block->p, staging.p, out_bytes, cudaMemcpyDeviceToHost, st));
+    if (staging.p) PB200_CUDA(cudaMemcpyAsync(block->p, staging.p, out_bytes, cudaMemcpyDeviceToHost, st));
     const cudaError_t se = cudaStreamSynchronize(st);
     if (se != cudaSuccess) { set_error("selection select phase failed: %s", cudaGetErrorString(se)); return PB200_E_CUDA; }
   }
 
   // ---- merged ORDER BY: the segments' tops by value, ties by (segment, doc id), first `limit` into a block of their own ----
-  unsigned char* base = static_cast<unsigned char*>(block->p);
   long long out_rows = total_rows;
   if (ordered && merge && total_rows > 0) {
+    const unsigned char* base = static_cast<const unsigned char*>(block->p);
     const int32_t* docs = reinterpret_cast<const int32_t*>(base);
     const int32_t* segi = docs + total_rows;
     const unsigned long long* vals = reinterpret_cast<const unsigned long long*>(base + 8 * total_rows);
@@ -466,41 +486,13 @@ extern "C" int32_t pb200_execute_selection(pb200_ctx* ctx, const pb200_query* fi
       for (int k = 0; k < ncols; k++) mvals[(size_t)k * out_rows + r] = vals[(size_t)k * total_rows + i];
     }
     block = merged;
-    base = mb;
   }
 
   // ---- results: row ranges of the one block ----
-  int32_t* all_docs = reinterpret_cast<int32_t*>(base);
-  int32_t* all_segs = all_docs + out_rows;
-  const unsigned long long* all_cols = reinterpret_cast<const unsigned long long*>(base + 8 * out_rows);
-  for (int r = 0; r < nres; r++) {
-    const int s0 = merge ? 0 : r, s1 = merge ? nseg : r + 1;
-    std::unique_ptr<pb200_result> R(new pb200_result());
-    pb200_result::Selection& v = R->selection;
-    v.present = true;
-    v.block = block;
-    const long long off = merge ? 0 : ss[s0].row_off;
-    long long docs_scanned = 0, entries = 0, total_docs = 0;
-    for (int s = s0; s < s1; s++) { docs_scanned += matches[s]; entries += in_filter[s]; total_docs += segments[s]->num_docs; }
-    v.rows = merge ? out_rows : ss[r].rows;
-    v.doc_ids = all_docs + off;
-    v.segment_index = all_segs + off;
-    for (int k = 0; k < ncols; k++) v.columns.push_back(all_cols + (size_t)k * out_rows + off);
-    R->meta.num_groups = (int32_t)v.rows;
-    R->meta.regime = PB200_REGIME_NONE;
-    R->meta.num_docs_scanned = docs_scanned;
-    R->meta.num_entries_scanned_in_filter = entries;
-    R->meta.num_entries_scanned_post_filter = v.rows * ncols;
-    R->meta.num_total_docs = total_docs;
-    R->meta.device_ms = ms;
-    results[r] = R.release();
-  }
-  const double t_exit = host_ms();
-  for (int ph = 0; ph < PB200_NUM_PHASES; ph++) set_phase_ms(ph, 0.0);
-  set_phase_ms(PB200_PHASE_PLAN, t_planned - t_enter);
-  set_phase_ms(PB200_PHASE_DEVICE_WAIT, t_scanned - t_planned);
-  set_phase_ms(PB200_PHASE_EXTRACT, t_exit - t_scanned);
-  set_phase_ms(PB200_PHASE_TOTAL, t_exit - t_enter);
+  std::vector<std::pair<long long, long long>> ranges;
+  if (merge) ranges.emplace_back(0, out_rows);
+  else for (const SelSeg& g : ss) ranges.emplace_back(g.row_off, g.rows);
+  rows_results(call, block, out_rows, ncols, ranges, true, results);
   return PB200_OK;
 }
 

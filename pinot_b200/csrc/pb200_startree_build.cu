@@ -528,8 +528,7 @@ int startree_build(pb200_ctx* ctx, const pb200_segment* seg, const StarBuildSpec
   const long long N = seg->num_docs;
   if (D < 1 || D > kMaxDims || M < 1) { set_error("star-tree build: %d dimensions, %d metrics", D, M); return PB200_E_UNSUPPORTED; }
   PB200_CUDA(cudaSetDevice(ctx->device));
-  cudaStream_t st = take_stream(ctx);
-  struct StreamReturn { pb200_ctx* c; cudaStream_t s; ~StreamReturn() { give_stream(c, s); } } stream_return{ctx, st};
+  StreamLease st(ctx);
   std::vector<int> acc(M);
   for (int m = 0; m < M; m++) {
     const int fn = spec.metric_fn[m];

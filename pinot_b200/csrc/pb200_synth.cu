@@ -206,8 +206,7 @@ extern "C" int32_t pb200_synth_segment(pb200_ctx* ctx, const char* name, int32_t
                                        const pb200_synth_col* cols, pb200_segment** out) {
   if (!ctx || !cols || !out || num_docs <= 0 || ncols <= 0) { set_error("invalid argument to pb200_synth_segment"); return PB200_E_INVALID; }
   PB200_CUDA(cudaSetDevice(ctx->device));
-  cudaStream_t st = take_stream(ctx);
-  struct StreamReturn { pb200_ctx* c; cudaStream_t s; ~StreamReturn() { give_stream(c, s); } } stream_return{ctx, st};
+  StreamLease st(ctx);
   std::vector<pb200_col_desc> descs(ncols);
   std::vector<void*> tmp_dicts;
   std::vector<void*> fwds;

@@ -104,8 +104,7 @@ extern "C" int32_t pb200_segment_derive_column(pb200_ctx* ctx, pb200_segment* se
 
   const uint32_t n = (uint32_t)src.cardinality;
   const int width = kind == TK_INT ? 4 : 8;
-  cudaStream_t st = take_stream(ctx);
-  struct StreamReturn { pb200_ctx* c; cudaStream_t s; ~StreamReturn() { give_stream(c, s); } } stream_return{ctx, st};
+  StreamLease st(ctx);
   // scratch: keys and ids in and out of the sort, flags / ranks, the sort's temporary storage
   size_t sort_bytes = 0, scan_bytes = 0;
   cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (const uint64_t*)nullptr, (uint64_t*)nullptr, (const uint32_t*)nullptr,
