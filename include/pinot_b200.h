@@ -37,7 +37,8 @@ extern "C" {
 #define PB200_ABI_VERSION 3 /* 2: pb200_query.reduce_world / merged_docs_bound, domains, tuning, pb200_result_meta.reserved bits;
                               3: pb200_comm_*, pb200_result_columns, doc masks, pb200h_query.agg_filter_* (the host query struct grew);
                                  pb200_order_by / pb200_execute_ordered / pb200h_execute_ordered were added later without a
-                                 version change: they are new symbols and structs, no existing one changed */
+                                 version change: they are new symbols and structs, no existing one changed; so were
+                                 pb200_having / pb200_execute_having / pb200h_execute_having */
 
 enum {
   PB200_OK = 0,
@@ -274,6 +275,38 @@ int32_t pb200_execute_ordered(pb200_ctx* ctx, const pb200_query* query, const pb
  * needs the column's dictionary to be the same in every segment.  NaN and -0.0 are out of scope, as for MIN / MAX. */
 int32_t pb200_execute_args(pb200_ctx* ctx, const pb200_query* query, const pb200_order_by* order, const double* agg_args,
                            pb200_segment* const* segments, int32_t num_segments, pb200_result** results);
+
+/* ---- HAVING of group-by results (the broker's GroupByDataTableReducer filter, applied to a FINAL result) ----------- */
+/* A POSTFIX tree (children before parent, root last) of at most PB200_MAX_HAVING_NODES nodes.  A leaf compares the FINAL
+ * value of aggregation `agg` (index into pb200_query.aggs) as a double: COUNT / DISTINCTCOUNT the count, AVG sum / count
+ * (-inf at count 0), the other functions their double column.  Comparisons are Java's <, <=, ==: a NaN value matches only
+ * NEQ, -0.0 equals 0.0, +-inf compare as usual (NOT the Double.compare order of ORDER BY).  The caller expands IN into an
+ * OR of EQ leaves and NOT IN into an AND of NEQ leaves. */
+#define PB200_MAX_HAVING_NODES 32
+enum { PB200_HAVING_AND = 0, PB200_HAVING_OR = 1, PB200_HAVING_NOT = 2, PB200_HAVING_RANGE = 3, PB200_HAVING_EQ = 4,
+       PB200_HAVING_NEQ = 5 };
+typedef struct {
+  int32_t op;           /* PB200_HAVING_* */
+  int32_t num_children; /* AND / OR: operands (>= 1); NOT: 1 */
+  int32_t agg;          /* leaves: index into pb200_query.aggs */
+  int32_t flags;        /* RANGE: as pb200_filter_node.raw_flags (bit0 lower unbounded, bit1 upper unbounded, bit2 lower
+                           exclusive, bit3 upper exclusive); at least one side bounded */
+  double lo, hi;        /* RANGE: bounds; EQ / NEQ: the literal in lo.  Never NaN */
+} pb200_having_node;
+typedef struct {
+  int32_t num_nodes;    /* 1 .. PB200_MAX_HAVING_NODES */
+  int32_t reserved;
+  pb200_having_node nodes[PB200_MAX_HAVING_NODES];
+} pb200_having;
+/* pb200_execute_args with the group-by rows filtered by `having` on the device, before the ORDER BY and its trim
+ * (having == NULL: exactly pb200_execute_args).  The numGroupsLimit check applies to the group count before HAVING;
+ * num_groups is the number of rows kept; the execution statistics do not change.  HAVING needs a final result: a group-by
+ * query that writes ONE result (PB200_Q_MERGE_SEGMENTS, or one segment).
+ * PB200_E_INVALID: a malformed tree, an aggregation index out of range, a NaN bound, no group-by, more than one result.
+ * PB200_E_UNSUPPORTED: PB200_Q_DEFER_FINALIZE or reduce_world > 1 (HAVING across GPUs is not offered). */
+int32_t pb200_execute_having(pb200_ctx* ctx, const pb200_query* query, const pb200_order_by* order, const double* agg_args,
+                             const pb200_having* having, pb200_segment* const* segments, int32_t num_segments,
+                             pb200_result** results);
 /* The histogram behind PERCENTILE aggregation `agg` in row `row`: its non-zero bins ascending by dictId (counts > 0), the
  * intermediate for merging per-segment results by value (the analogue of pb200_result_distinct).  Returns the number of
  * bins (or < 0 on error) and writes at most `capacity` of them; either output may be NULL.  The histograms are copied from

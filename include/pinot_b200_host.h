@@ -210,6 +210,14 @@ int32_t pb200h_execute_ordered(pb200_ctx* ctx, const pb200h_query* query, const 
 int32_t pb200h_execute_args(pb200_ctx* ctx, const pb200h_query* query, const pb200_order_by* order, const double* agg_args,
                             pb200h_segment* const* segments, int32_t num_segments, pb200_result** results,
                             int32_t* operator_kinds);
+/* pb200h_execute_args with the group-by rows filtered by HAVING (pb200_execute_having of include/pinot_b200.h; leaves index
+ * query->aggs) before the ORDER BY and its trim.  having == NULL: exactly pb200h_execute_args.  Device results are filtered
+ * on the device; results built on the host (star-tree, FILTER clauses) are filtered on the host by the same predicate,
+ * after the FILTER clauses' submissions are aligned.  The same errors as pb200_execute_having (more than one result:
+ * merge_segments == 0 with several segments; merge_segments == 2 is PB200_E_UNSUPPORTED). */
+int32_t pb200h_execute_having(pb200_ctx* ctx, const pb200h_query* query, const pb200_order_by* order, const double* agg_args,
+                              const pb200_having* having, pb200h_segment* const* segments, int32_t num_segments,
+                              pb200_result** results, int32_t* operator_kinds);
 /* ---- selection (SELECT columns WHERE ... LIMIT n; pb200_execute_selection of include/pinot_b200.h) --------------- */
 typedef struct {
   const char* column;
@@ -240,7 +248,8 @@ int32_t pb200h_execute_distinct(pb200_ctx* ctx, const pb200h_query* query, const
  * (GroupByResultsBlock.java:186-236): typed group-key values (STRING keys through the DataTable's own string dictionary),
  * COUNT as LONG, SUM / MIN / MAX as DOUBLE, AVG as OBJECT AvgPair, DISTINCTCOUNT as OBJECT value set, + the execution
  * statistics as metadata.  `segment` supplies the dictionaries the result's ids refer to (any segment of a merged
- * result: they share dictionaries).  Returns the size (or the size needed when out == NULL), < 0 on error. */
+ * result: they share dictionaries).  Returns the size (or the size needed when out == NULL), < 0 on error.
+ * A result filtered by HAVING is PB200_E_UNSUPPORTED: a server's DataTable never carries rows HAVING removed. */
 int64_t pb200h_result_to_datatable(const pb200h_query* query, const pb200h_segment* segment, const pb200_result* result,
                                    void* out, uint64_t capacity);
 

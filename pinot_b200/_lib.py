@@ -121,6 +121,20 @@ class OrderBy(C.Structure):
     _fields_ = [("num_items", C.c_int32), ("trim_size", C.c_int32), ("items", OrderItem * MAX_ORDER_BY)]
 
 
+MAX_HAVING_NODES = 32
+HAVING_CODES = {"AND": 0, "OR": 1, "NOT": 2, "RANGE": 3, "EQ": 4, "NEQ": 5}
+HAVING_LO_UNBOUNDED, HAVING_HI_UNBOUNDED, HAVING_LO_EXCLUSIVE, HAVING_HI_EXCLUSIVE = 1, 2, 4, 8
+
+
+class HavingNode(C.Structure):
+    _fields_ = [("op", C.c_int32), ("num_children", C.c_int32), ("agg", C.c_int32), ("flags", C.c_int32),
+                ("lo", C.c_double), ("hi", C.c_double)]
+
+
+class Having(C.Structure):
+    _fields_ = [("num_nodes", C.c_int32), ("reserved", C.c_int32), ("nodes", HavingNode * MAX_HAVING_NODES)]
+
+
 class SelectOrder(C.Structure):
     _fields_ = [("column", C.c_int32), ("descending", C.c_int32)]
 
@@ -186,6 +200,7 @@ EXPORTED_SYMBOLS = [
     "pb200_execute_args", "pb200h_execute_args", "pb200_result_histogram", "pb200_result_moments",
     "pb200_segment_derive_column", "pb200h_segment_derive",
     "pb200h_startree_build", "pb200h_startree_get",
+    "pb200_execute_having", "pb200h_execute_having",
 ]
 
 _LIB = None
@@ -213,6 +228,8 @@ def load() -> C.CDLL:
     L.pb200_execute_ordered.argtypes = [vp, C.POINTER(Query), C.POINTER(OrderBy), C.POINTER(vp), i32, C.POINTER(vp)]
     L.pb200_execute_args.argtypes = [vp, C.POINTER(Query), C.POINTER(OrderBy), C.POINTER(C.c_double), C.POINTER(vp), i32,
                                      C.POINTER(vp)]
+    L.pb200_execute_having.argtypes = [vp, C.POINTER(Query), C.POINTER(OrderBy), C.POINTER(C.c_double), C.POINTER(Having),
+                                       C.POINTER(vp), i32, C.POINTER(vp)]
     L.pb200_result_histogram.restype = i64
     L.pb200_result_histogram.argtypes = [vp, i32, i32, vp, vp, i64]
     L.pb200_result_moments.argtypes = [vp, i32, i32, vp, vp, vp, vp, vp, vp, vp]
@@ -248,6 +265,8 @@ def load() -> C.CDLL:
                                          C.POINTER(i32)]
     L.pb200h_execute_args.argtypes = [vp, C.POINTER(HQuery), C.POINTER(OrderBy), C.POINTER(C.c_double), C.POINTER(vp), i32,
                                       C.POINTER(vp), C.POINTER(i32)]
+    L.pb200h_execute_having.argtypes = [vp, C.POINTER(HQuery), C.POINTER(OrderBy), C.POINTER(C.c_double), C.POINTER(Having),
+                                        C.POINTER(vp), i32, C.POINTER(vp), C.POINTER(i32)]
     L.pb200h_explain.argtypes = [vp, C.POINTER(HQuery), vp, C.c_char_p, i32]
     L.pb200h_startree_attach.argtypes = [vp, vp, vp, C.c_uint64, i32, i32, C.POINTER(C.c_char_p), C.POINTER(vp),
                                          C.POINTER(C.c_uint64), i32, C.POINTER(HStarMetric)]

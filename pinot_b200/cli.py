@@ -6,8 +6,9 @@
 What happens: ``pb200h_segment_load_dir`` per directory (v1 file-per-index or v3 columns.psf + index_map, raw columns decoded
 and dictionary-encoded at load, star-trees attached), ``pb200h_execute`` over all segments in one submission, then -- what the
 reference's combine + broker reduce do, in a few lines of Python -- the per-segment results blocks are merged by key VALUES
-(``AggregationFunction.merge``), final results extracted (AVG = sum / count, DISTINCTCOUNT = set size) and the first LIMIT rows
-printed.  With ``--merge-on-device`` the segments are first bound to one dictionary domain and combined on the GPU.
+(``AggregationFunction.merge``), final results extracted (AVG = sum / count, DISTINCTCOUNT = set size), filtered by HAVING,
+ordered, and the first LIMIT rows printed.  With ``--merge-on-device`` the segments are first bound to one dictionary domain
+and combined on the GPU, where HAVING, ORDER BY and the trim run too.
 
 Needs a GPU: the product has no CPU fallback.  Queries outside the accelerated set exit with the library's message (a Pinot
 server would run the stock operator for them)."""
@@ -78,13 +79,15 @@ def merge_blocks(query, segments, blocks) -> Dict[tuple, list]:
 
 
 def final_rows(query, table: Dict[tuple, list]) -> List[list]:
-    """Broker-side extraction of final results + ORDER BY + LIMIT.  ORDER BY compares final values (AVG = sum / count,
-    DISTINCTCOUNT = set size) and breaks ties by the key values ascending, in GROUP BY column order -- the library's order.
-    Without ORDER BY Pinot returns an arbitrary LIMIT-sized subset; here the rows are sorted by key to make the output
-    stable."""
-    from .query import MOMENT_FUNCTIONS, moments_final, percentile_of_counts, value_order
-    from .sql import resolve_order_by
+    """Broker-side extraction of final results + HAVING + ORDER BY + LIMIT.  HAVING keeps the rows whose final values pass
+    it (Java's comparisons: query.having_eval).  ORDER BY compares final values (AVG = sum / count, DISTINCTCOUNT = set
+    size) and breaks ties by the key values ascending, in GROUP BY column order -- the library's order.  Without ORDER BY
+    Pinot returns an arbitrary LIMIT-sized subset; here the rows are sorted by key to make the output stable.  Hidden
+    aggregations (named only in HAVING) are left out of the rows."""
+    from .query import MOMENT_FUNCTIONS, having_eval, moments_final, percentile_of_counts, value_order
+    from .sql import resolve_having, resolve_order_by
     items = resolve_order_by(query) if query.is_group_by else []
+    having = resolve_having(query)
     rows = []
     keys = sorted(table, key=lambda k: tuple(value_order(x) for x in k)) if items else sorted(table, key=lambda k: tuple(str(x) for x in k))
     for key in keys:
@@ -100,12 +103,15 @@ def final_rows(query, table: Dict[tuple, list]) -> List[list]:
                 vals.append(moments_final(agg.function, v))
             else:
                 vals.append(v)
+        if having and not having_eval(having, [float(x) for x in vals]):
+            continue
         rows.append(list(key) + vals)
     k = len(query.group_by)
     for kind, index, asc in reversed(items):  # stable passes, last item first
         col = index if kind == "GROUP_BY" else k + index
         rows.sort(key=lambda r: value_order(r[col]), reverse=not asc)
-    return rows[: query.limit]
+    shown = list(range(k)) + [k + a for a, agg in enumerate(query.aggregations) if not agg.hidden]
+    return [[r[c] for c in shown] for r in rows[: query.limit]]
 
 
 def main(argv=None) -> int:
@@ -159,7 +165,7 @@ def main(argv=None) -> int:
             sys.stderr.write(f"{e}\n")
             return 2
         rows = final_rows(query, table)
-        names = list(query.group_by) + [str(a) for a in query.aggregations]
+        names = list(query.group_by) + [str(a) for a in query.aggregations if not a.hidden]
         stats = {"numDocsScanned": sum(b.stats.num_docs_scanned for b in blocks), "totalDocs": sum(s.num_docs for s in segments),
                  "numSegments": len(segments), "deviceMs": round(sum(b.device_ms for b in blocks[:1]), 4),
                  "operators": sorted({b.operator_kind for b in blocks})}

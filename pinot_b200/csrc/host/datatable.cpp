@@ -75,6 +75,10 @@ extern "C" int64_t pb200h_result_to_datatable(const pb200h_query* q, const pb200
   if (pb200_result_meta_get(R, &meta)) return PB200_E_INVALID;
   const int ngb = q->num_group_by, nagg = q->num_aggs;
   if (meta.num_group_by != ngb || meta.num_aggs != nagg) { set_error("result does not belong to this query"); return PB200_E_INVALID; }
+  if (R->having.num_nodes > 0) {   // HAVING is the broker's: a server never sends rows it removed
+    set_error("a result filtered by HAVING is final: it is not written as a server DataTable");
+    return PB200_E_UNSUPPORTED;
+  }
   for (int a = 0; a < nagg; a++)
     if (q->aggs[a].function == PB200_AGG_PERCENTILE) {  // its intermediate is the reference's DoubleArrayList of values
       set_error("PERCENTILE intermediates are not written as DataTable objects");

@@ -42,8 +42,8 @@ struct ResultGuard {
 
 }  // namespace
 
-int execute_filtered(pb200_ctx* ctx, const pb200h_query& q, const pb200_order_by* order, pb200h_segment* const* segs, int nseg,
-                     pb200_result** results, int32_t* kinds) {
+int execute_filtered(pb200_ctx* ctx, const pb200h_query& q, const pb200_order_by* order, const pb200_having* having,
+                     pb200h_segment* const* segs, int nseg, pb200_result** results, int32_t* kinds) {
   if (q.merge_segments == 2) { set_error("FILTER clauses with a deferred (cross-GPU) combine are not accelerated"); return PB200_E_UNSUPPORTED; }
   const int nagg = q.num_aggs, ngb = q.num_group_by;
   const int nres = q.merge_segments ? 1 : nseg;
@@ -171,8 +171,9 @@ int execute_filtered(pb200_ctx* ctx, const pb200h_query& q, const pb200_order_by
         }
       }
     }
-    // ORDER BY: the infos ran unordered (a trimmed info could miss a group of the main filter); the aligned rows are
-    // ordered and trimmed here, by the same keys as the device sort
+    // HAVING and ORDER BY: the infos ran unfiltered and unordered (each holds partial columns, and a trimmed info could miss
+    // a group of the main filter); the aligned rows are filtered, ordered and trimmed here, by the device's rules
+    if (having && ngb > 0) pb200::having_rows_host(R.get(), *having, R->agg_functions.data());
     if (order && ngb > 0) pb200::order_rows_host(R.get(), *order, R->agg_functions.data());
     aligned[r] = std::move(R);
   }

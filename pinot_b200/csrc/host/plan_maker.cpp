@@ -730,9 +730,18 @@ extern "C" int32_t pb200h_execute_ordered(pb200_ctx* ctx, const pb200h_query* q,
 
 extern "C" int32_t pb200h_execute_args(pb200_ctx* ctx, const pb200h_query* q, const pb200_order_by* order, const double* agg_args,
                                        pb200h_segment* const* segs, int32_t nseg, pb200_result** results, int32_t* kinds) {
+  return pb200h_execute_having(ctx, q, order, agg_args, nullptr, segs, nseg, results, kinds);
+}
+
+extern "C" int32_t pb200h_execute_having(pb200_ctx* ctx, const pb200h_query* q, const pb200_order_by* order, const double* agg_args,
+                                         const pb200_having* having, pb200h_segment* const* segs, int32_t nseg,
+                                         pb200_result** results, int32_t* kinds) {
   if (!ctx || !q || !segs || !results || nseg <= 0) { set_error("invalid argument to pb200h_execute"); return PB200_E_INVALID; }
   if (q->num_aggs <= 0) { set_error("selection queries are outside this path"); return PB200_E_UNSUPPORTED; }
   if (int vrc = pb200::order_validate(order, q->num_aggs, q->num_group_by)) return vrc;
+  if (int hrc = pb200::having_check(having, q->num_aggs, q->num_group_by, q->merge_segments ? 1 : nseg,
+                                    q->merge_segments == 2 || q->reduce_world > 1))
+    return hrc;
   if (q->num_group_by == 0) order = nullptr;  // aggregation only: one row, nothing to order
   if (int rc = derive_query_names(ctx, *q, segs, nseg, nullptr, 0)) return rc;  // expressions become derived columns once
   bool any_clause = false;   // some aggregation has a FILTER (WHERE ...) clause
@@ -757,7 +766,7 @@ extern "C" int32_t pb200h_execute_args(pb200_ctx* ctx, const pb200h_query* q, co
     }
   if (q->agg_filter_count && q->agg_filter_start && q->agg_filter_nodes)
     for (int a = 0; a < q->num_aggs; a++)
-      if (q->agg_filter_count[a] > 0) return execute_filtered(ctx, *q, order, segs, nseg, results, kinds);  // host/filtered_agg.cpp
+      if (q->agg_filter_count[a] > 0) return execute_filtered(ctx, *q, order, having, segs, nseg, results, kinds);  // host/filtered_agg.cpp
   const bool merge = q->merge_segments != 0;
   // resolve columns by name against segment 0 (all segments of a table share the schema)
   const pb200h_segment& s0 = *segs[0];
@@ -812,11 +821,11 @@ extern "C" int32_t pb200h_execute_args(pb200_ctx* ctx, const pb200h_query* q, co
         if (rc < 0) { for (auto r : star_results) if (r) pb200_result_free(r); return rc; }
         if (rc == 1) {
           kind[s] = PB200H_OP_STAR_TREE;
-          if (order) {  // the star-tree's own submission computes other functions: order by the query's, on the host
-            std::vector<int32_t> fns(q->num_aggs);
-            for (int a = 0; a < q->num_aggs; a++) fns[a] = q->aggs[a].function;
-            pb200::order_rows_host(star_results[s], *order, fns.data());
-          }
+          // the star-tree's own submission computes other functions: filter and order by the query's, on the host
+          std::vector<int32_t> fns(q->num_aggs);
+          for (int a = 0; a < q->num_aggs; a++) fns[a] = q->aggs[a].function;
+          if (having) pb200::having_rows_host(star_results[s], *having, fns.data());
+          if (order) pb200::order_rows_host(star_results[s], *order, fns.data());
           break;
         }
       }
@@ -845,14 +854,17 @@ extern "C" int32_t pb200h_execute_args(pb200_ctx* ctx, const pb200h_query* q, co
     dq.filter = flat.data();
     dq.group_by_columns = gb.data();
     dq.aggs = aggs.data();
-    int rc = pb200_execute_args(ctx, &dq, order, agg_args, dsegs.data(), (int)dsegs.size(), dev_results.data());
+    int rc = pb200_execute_having(ctx, &dq, order, agg_args, having, dsegs.data(), (int)dsegs.size(), dev_results.data());
     if (rc) { for (auto r : star_results) if (r) pb200_result_free(r); return rc; }
   }
   if (merge) { results[0] = dev_results[0]; return PB200_OK; }
   size_t di = 0;
   for (int s = 0; s < nseg; s++) {
     if (kind[s] == PB200H_OP_STAR_TREE) results[s] = star_results[s];
-    else if (kind[s] == PB200H_OP_EMPTY) results[s] = host_result(*segs[s], *q, true);
+    else if (kind[s] == PB200H_OP_EMPTY) {
+      results[s] = host_result(*segs[s], *q, true);
+      if (having) results[s]->having = *having;   // no rows to filter, but the result is as final as a filtered one
+    }
     else if (kind[s] == PB200H_OP_NON_SCAN_AGGREGATION) results[s] = host_result(*segs[s], *q, false);
     else results[s] = dev_results[di++];
   }

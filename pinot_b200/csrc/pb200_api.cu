@@ -701,14 +701,26 @@ int launch_chunks(pb200_ctx* ctx, cudaStream_t st, const ScanPlan& plan, DevBufR
 // ScanCall::read_back_and_verify) -- the caller runs the submission again with separate COUNT reductions.
 constexpr int kRetryWithoutCountCarrier = 1;
 static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment* const* segments, int32_t nseg,
-                        pb200_result** results, bool allow_count_carrier, const pb200_order_by* order, const double* agg_args);
+                        pb200_result** results, bool allow_count_carrier, const pb200_order_by* order, const double* agg_args,
+                        const pb200_having* having);
+
+extern "C" int32_t pb200_execute_having(pb200_ctx* ctx, const pb200_query* query, const pb200_order_by* order, const double* agg_args,
+                                        const pb200_having* having, pb200_segment* const* segments, int32_t nseg,
+                                        pb200_result** results) {
+  if (query) {
+    if (const int vrc = order_validate(order, query->num_aggs, query->num_group_by)) return vrc;
+    const int nres = (query->flags & PB200_Q_MERGE_SEGMENTS) ? 1 : nseg;
+    const bool deferred = (query->flags & PB200_Q_DEFER_FINALIZE) || query->reduce_world > 1;
+    if (const int hrc = having_check(having, query->num_aggs, query->num_group_by, nres, deferred)) return hrc;
+  }
+  int rc = execute_impl(ctx, query, segments, nseg, results, true, order, agg_args, having);
+  if (rc == kRetryWithoutCountCarrier) rc = execute_impl(ctx, query, segments, nseg, results, false, order, agg_args, having);
+  return rc;
+}
 
 extern "C" int32_t pb200_execute_args(pb200_ctx* ctx, const pb200_query* query, const pb200_order_by* order, const double* agg_args,
                                       pb200_segment* const* segments, int32_t nseg, pb200_result** results) {
-  if (query) { const int vrc = order_validate(order, query->num_aggs, query->num_group_by); if (vrc) return vrc; }
-  int rc = execute_impl(ctx, query, segments, nseg, results, true, order, agg_args);
-  if (rc == kRetryWithoutCountCarrier) rc = execute_impl(ctx, query, segments, nseg, results, false, order, agg_args);
-  return rc;
+  return pb200_execute_having(ctx, query, order, agg_args, nullptr, segments, nseg, results);
 }
 
 extern "C" int32_t pb200_execute_ordered(pb200_ctx* ctx, const pb200_query* query, const pb200_order_by* order,
@@ -1096,7 +1108,7 @@ struct ScanCall {
 
   // 11. every result's metadata and (aggregation only) its row, then the group-by rows extracted, or left for
   //     pb200_result_finalize (deferred); per-segment results release their tables
-  int fill_results_and_extract(const pb200_order_by* order) {
+  int fill_results_and_extract(const pb200_order_by* order, const pb200_having* having) {
     const int nuser = plan.num_user_aggs;
     const float ms = ev.ms();
     for (int r = 0; r < plan.nres; r++) {
@@ -1120,6 +1132,7 @@ struct ScanCall {
         R.meta.regime = regime_of(R.dense.cards, query->max_initial_result_holder_capacity);
         R.meta.reserved = (R.dense.pack_agg >= 0 ? 1 : 0) | (R.dense.carrier_unsafe ? 2 : 0) | (R.dense.flag_slot ? 4 : 0);  // include/pinot_b200.h
         if (order) R.order = *order;   // a deferred result keeps it for its extraction
+        if (having) R.having = *having;
         continue;
       }
       R.meta.num_groups = -1;
@@ -1159,7 +1172,8 @@ struct ScanCall {
 }  // namespace
 
 static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment* const* segments, int32_t nseg,
-                        pb200_result** results, bool allow_count_carrier, const pb200_order_by* order, const double* agg_args) {
+                        pb200_result** results, bool allow_count_carrier, const pb200_order_by* order, const double* agg_args,
+                        const pb200_having* having) {
   ScanCall c{ctx, query, segments, nseg};
   if (int rc = c.check_call(results)) return rc;
   if (int rc = c.prepare_and_plan(allow_count_carrier, agg_args)) return rc;
@@ -1169,7 +1183,7 @@ static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment*
   if (int rc = c.launch()) return rc;
   if (int rc = c.finalize_percentiles()) return rc;
   if (int rc = c.read_back_and_verify()) return rc;   // kRetryWithoutCountCarrier: ~ScanCall frees this attempt's tables
-  if (int rc = c.fill_results_and_extract(order)) return rc;
+  if (int rc = c.fill_results_and_extract(order, having)) return rc;
   c.hand_out(results);
   return PB200_OK;
 }

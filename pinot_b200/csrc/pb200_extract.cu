@@ -20,6 +20,10 @@
 // pass, stable LSD radix sorts order the index by the group-key tie key first and then by the items from last to first, and
 // the write kernel writes row r from entry idx[r] for r < min(groups, trim_size).  The block is sized for the trimmed rows,
 // so a trimmed result stays on the one-synchronisation path.
+// A result with a HAVING tree (pb200_having, pb200_having.h) takes one step before count: a keep kernel evaluates the tree
+// on every existing entry's final values and writes a keep bitmap (1 bit per entry, one byte per 8 consecutive entries)
+// plus the number of existing entries, which the numGroupsLimit check uses.  Count and write (also index-only) then test
+// the keep bit instead of non_empty(), so HAVING runs before the ORDER BY and its trim, and only removes rows.
 #include <cuda_runtime.h>
 #include <cub/device/device_radix_sort.cuh>
 
@@ -28,6 +32,7 @@
 #include <cstring>
 
 #include "pb200_internal.h"
+#include "pb200_having.h"
 #include "pb200_order.h"
 
 namespace pb200 {
@@ -68,12 +73,21 @@ struct ExtractDesc {
   const long long* mom[kMaxAggs][3]; // VAR / STDDEV: the K, H, L limb sum tables (pb200_moments.h)
   int32_t mom_e[kMaxAggs];           // ... and the grid exponent of the column
   unsigned long long off_mom[kMaxAggs];  // ... {s1, s2 low, s2 high} per row, for pb200_result_moments
+  const uint8_t* keep;               // HAVING only: bit j of byte i = entry 8i + j is a row (NULL: every non_empty() entry is)
 };
 
 __device__ __forceinline__ bool non_empty(const ExtractDesc& d, long long i) {
   if (d.hkeys) return d.hkeys[i] != ~0ull;
   if (d.packed) return d.packed[i] != 0ull;
   return (d.count && d.count[i] != 0ull) || (d.seen && d.seen[i] != 0u) || (d.maxk && d.maxk[i] != 0u) || (d.mink && d.mink[i] != 0xFFFFFFFFu);
+}
+// bit j = entry base + j is a row of the result (base: a multiple of 8)
+__device__ __forceinline__ uint32_t entry_flags(const ExtractDesc& d, long long base) {
+  if (d.keep) return d.keep[base >> 3];
+  uint32_t flags = 0;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) flags |= ((base + j < d.groups && non_empty(d, base + j)) ? 1u : 0u) << j;
+  return flags;
 }
 __device__ __forceinline__ int find_result(const ExtractDesc* descs, int nres, uint32_t chunk) {
   int r = 0;
@@ -87,9 +101,7 @@ __global__ void __launch_bounds__(kExtractThreads) extract_count_kernel(const Ex
   const int r = find_result(descs, nres, blockIdx.x);
   const ExtractDesc& d = descs[r];
   const long long base = (long long)(blockIdx.x - d.first_chunk) * kChunk + threadIdx.x * 8;
-  uint32_t c = 0;
-#pragma unroll
-  for (int j = 0; j < 8; ++j) c += (base + j < d.groups && non_empty(d, base + j)) ? 1u : 0u;
+  uint32_t c = __popc(entry_flags(d, base));
   c = __reduce_add_sync(0xFFFFFFFFu, c);
   if ((threadIdx.x & 31) == 0) wsum[threadIdx.x >> 5] = c;
   __syncthreads();
@@ -175,6 +187,14 @@ __device__ __forceinline__ void agg_values(const ExtractDesc& d, int a, long lon
   }
 }
 
+// set size of DISTINCTCOUNT aggregation a in entry g: the popcount of its bitset row
+__device__ __forceinline__ long long distinct_size(const ExtractDesc& d, int a, long long g) {
+  const uint32_t* row = d.dbits[a] + (size_t)g * d.dwords[a];
+  long long n = 0;
+  for (uint32_t w = 0; w < d.dwords[a]; ++w) n += __popc(row[w]);
+  return n;
+}
+
 __device__ __forceinline__ unsigned long long raw_key_of(const ExtractDesc& d, long long g) {
   return d.hkeys ? d.hkeys[g] : (unsigned long long)g / (unsigned)d.stride;
 }
@@ -222,9 +242,7 @@ __global__ void __launch_bounds__(kExtractThreads) extract_write_kernel(const Ex
     return;
   }
   if (!d.order_idx && index_only) return;
-  uint32_t flags = 0;
-#pragma unroll
-  for (int j = 0; j < 8; ++j) flags |= ((base + j < d.groups && non_empty(d, base + j)) ? 1u : 0u) << j;
+  const uint32_t flags = entry_flags(d, base);
   const uint32_t mine = __popc(flags);
   // CTA-wide exclusive scan of the per-thread counts (entries stay in raw-key order)
   uint32_t incl = mine;
@@ -273,9 +291,7 @@ __global__ void __launch_bounds__(kExtractThreads) order_key_kernel(const Extrac
       long long lv;
       int32_t id;
       if (d.fn[p.index] == PB200_AGG_DISTINCTCOUNT) {
-        const uint32_t* row = d.dbits[p.index] + (size_t)g * d.dwords[p.index];
-        lv = 0;
-        for (uint32_t w = 0; w < d.dwords[p.index]; ++w) lv += __popc(row[w]);
+        lv = distinct_size(d, p.index, g);
         dv = (double)lv;
       } else {
         agg_values(d, p.index, g, group_count(d, g), dv, lv, id);
@@ -295,6 +311,40 @@ __global__ void __launch_bounds__(kExtractThreads) order_key_kernel(const Extrac
       k = p.what == PASS_TIE ? tie : order_key(ORDER_CMP_LONG, p.descending != 0, p.mask, 0.0, (long long)id);
     }
     keys[i] = k;
+  }
+}
+
+// keep[i] = the HAVING outcome of entries 8i .. 8i + 7 of result r (bit j: entry 8i + j exists and passes), for every
+// entry of the result's chunks; exists[r] += the result's existing entries (the count numGroupsLimit is checked on)
+__global__ void __launch_bounds__(kExtractThreads) having_kernel(const ExtractDesc* __restrict__ descs, int r, const pb200_having h,
+                                                                 uint8_t* __restrict__ keep, unsigned long long* __restrict__ exists) {
+  __shared__ uint32_t wsum[kExtractThreads / 32];
+  const ExtractDesc& d = descs[r];
+  const long long base = (long long)blockIdx.x * kChunk + threadIdx.x * 8;
+  uint32_t flags = 0, c = 0;
+  for (int j = 0; j < 8; ++j) {
+    const long long g = base + j;
+    if (g >= d.groups || !non_empty(d, g)) continue;
+    ++c;
+    const unsigned long long cnt = group_count(d, g);
+    const bool pass = having_eval(h, [&](int a) -> double {
+      if (d.fn[a] == PB200_AGG_DISTINCTCOUNT) return (double)distinct_size(d, a, g);
+      double dv;
+      long long lv;
+      int32_t id;
+      agg_values(d, a, g, cnt, dv, lv, id);
+      return having_value(d.fn[a], dv, lv);
+    });
+    flags |= (pass ? 1u : 0u) << j;
+  }
+  keep[base >> 3] = (uint8_t)flags;
+  c = __reduce_add_sync(0xFFFFFFFFu, c);
+  if ((threadIdx.x & 31) == 0) wsum[threadIdx.x >> 5] = c;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    unsigned long long t = 0;
+    for (int w = 0; w < kExtractThreads / 32; ++w) t += wsum[w];
+    if (t) atomicAdd(exists + r, t);
   }
 }
 
@@ -371,7 +421,11 @@ int extract_groups(pb200_ctx* ctx, pb200_result* const* Rs, int nres, cudaStream
   size_t order_bytes = 0;  // per ordered result: 2 index buffers [idx_cap] u32 + 2 key buffers [idx_cap] u64
   std::vector<ExtractDesc> descs(nres);
   uint32_t chunks = 0;
-  size_t worst = 64 + 8ull * nres;  // header: totals
+  bool any_having = false;
+  for (int r = 0; r < nres; r++) any_having |= Rs[r]->having.num_nodes > 0;
+  // header: totals (rows), then with HAVING the existing entries per result (what numGroupsLimit is checked on)
+  const size_t head = 64 + 8ull * nres * (any_having ? 2 : 1);
+  size_t worst = head;
   for (int r = 0; r < nres; r++) {
     const pb200_result::Dense& d = Rs[r]->dense;
     ExtractDesc& e = descs[r];
@@ -403,8 +457,17 @@ int extract_groups(pb200_ctx* ctx, pb200_result* const* Rs, int nres, cudaStream
     const unsigned long long cap = (unsigned long long)std::min<long long>(d.groups, (long long)d.num_groups_limit + 1);
     e.idx_cap = cap;
     worst = layout_result(d, e, worst, kept_rows(Rs[r], cap));
-    if (Rs[r]->order.num_items > 0) {
+    if (Rs[r]->order.num_items > 0 || Rs[r]->having.num_nodes > 0) {
       for (int a = 0; a < e.nagg; a++) { e.dbits[a] = d.dbits[a]; e.dwords[a] = d.dwords[a]; }
+      for (int i = 0; i < Rs[r]->having.num_nodes; i++) {
+        const pb200_having_node& hn = Rs[r]->having.nodes[i];
+        const bool leaf = hn.op == PB200_HAVING_RANGE || hn.op == PB200_HAVING_EQ || hn.op == PB200_HAVING_NEQ;
+        if (leaf && e.fn[hn.agg] == PB200_AGG_DISTINCTCOUNT && !d.dbits[hn.agg]) {
+          set_error("HAVING on a DISTINCTCOUNT without per-group sets"); return PB200_E_UNSUPPORTED;
+        }
+      }
+    }
+    if (Rs[r]->order.num_items > 0) {
       for (int i = 0; i < Rs[r]->order.num_items; i++) {
         const pb200_order_item& it = Rs[r]->order.items[i];
         if (it.kind == PB200_ORDER_AGG && e.fn[it.index] == PB200_AGG_DISTINCTCOUNT && !d.dbits[it.index]) {
@@ -421,7 +484,7 @@ int extract_groups(pb200_ctx* ctx, pb200_result* const* Rs, int nres, cudaStream
   if ((rc = dcount.alloc(4ull * std::max<uint32_t>(chunks, 1)))) return rc;
   auto pin = std::make_shared<PinnedBlock>();
   pin->ctx = ctx;
-  if ((rc = pinned_alloc(ctx, speculative ? worst : 64 + 8ull * nres, &pin->p, &pin->bytes))) return rc;
+  if ((rc = pinned_alloc(ctx, speculative ? worst : head, &pin->p, &pin->bytes))) return rc;
   unsigned char* out = static_cast<unsigned char*>(pin->p);
   unsigned long long* totals = reinterpret_cast<unsigned long long*>(out);  // header of the block (written by the scan kernel)
   // ---- ORDER BY buffers: v[0] takes the compaction, pass p sorts (k0, v[p % 2]) -> (k1, v[(p + 1) % 2]) ----
@@ -446,8 +509,24 @@ int extract_groups(pb200_ctx* ctx, pb200_result* const* Rs, int nres, cudaStream
     }
     if ((rc = otemp.alloc(std::max<size_t>(temp_bytes, 256)))) return rc;
   }
+  // ---- HAVING: one keep byte per 8 entries of each filtered result, and its existing-entry counter ----
+  DevBufRaw dkeep(ctx), dexist(ctx);
+  if (any_having) {
+    if ((rc = dkeep.alloc(256ull * std::max<uint32_t>(chunks, 1)))) return rc;   // kChunk / 8 bytes per chunk
+    if ((rc = dexist.alloc(8ull * nres))) return rc;
+    for (int r = 0; r < nres; r++)
+      if (Rs[r]->having.num_nodes > 0) descs[r].keep = static_cast<const uint8_t*>(dkeep.p) + 256ull * descs[r].first_chunk;
+  }
   const ExtractDesc* ddescs = (const ExtractDesc*)ddesc.p;
   PB200_CUDA(cudaMemcpyAsync(ddesc.p, descs.data(), sizeof(ExtractDesc) * nres, cudaMemcpyHostToDevice, st));
+  if (any_having) {
+    PB200_CUDA(cudaMemsetAsync(dexist.p, 0, 8ull * nres, st));
+    for (int r = 0; r < nres; r++)
+      if (descs[r].keep && descs[r].num_chunks)
+        having_kernel<<<descs[r].num_chunks, kExtractThreads, 0, st>>>(ddescs, r, Rs[r]->having, const_cast<uint8_t*>(descs[r].keep),
+                                                                       static_cast<unsigned long long*>(dexist.p));
+    PB200_CUDA(cudaMemcpyAsync(totals + nres, dexist.p, 8ull * nres, cudaMemcpyDeviceToHost, st));
+  }
   if (chunks) extract_count_kernel<<<chunks, kExtractThreads, 0, st>>>(ddescs, nres, (uint32_t*)dcount.p);
   extract_scan_kernel<<<nres, kExtractThreads, 0, st>>>(ddescs, (uint32_t*)dcount.p, totals);
   if (order_bytes && chunks) {
@@ -468,8 +547,8 @@ int extract_groups(pb200_ctx* ctx, pb200_result* const* Rs, int nres, cudaStream
   PB200_CUDA(cudaGetLastError());
   PB200_CUDA(cudaStreamSynchronize(st));  // descs may be rewritten below: the copy above has completed
   // ---- group counts, limits ----
-  std::vector<unsigned long long> n(nres);
-  for (int r = 0; r < nres; r++) n[r] = totals[r];
+  std::vector<unsigned long long> n(nres), groups(nres);  // rows kept, existing groups (before HAVING)
+  for (int r = 0; r < nres; r++) { n[r] = totals[r]; groups[r] = Rs[r]->having.num_nodes > 0 ? totals[nres + r] : n[r]; }
   for (int r = 0; r < nres; r++) {
     pb200_result* R = Rs[r];
     const pb200_result::Dense& d = R->dense;
@@ -482,16 +561,16 @@ int extract_groups(pb200_ctx* ctx, pb200_result* const* Rs, int nres, cudaStream
       }
     }
     R->meta.num_groups = (int32_t)kept_rows(R, n[r]);
-    R->meta.groups_limit_reached = (long long)n[r] >= d.num_groups_limit;
-    if ((long long)n[r] > d.num_groups_limit) {
+    R->meta.groups_limit_reached = (long long)groups[r] >= d.num_groups_limit;
+    if ((long long)groups[r] > d.num_groups_limit) {
       // the reference admits groups in doc order until the limit binds (IntGroupIdMap.getGroupId :1022-1047); that order
       // is not reproducible by a parallel scan -> the caller must run the Java operator for this segment
-      set_error("numGroupsLimit %d would bind (%llu groups): fall back to the reference operator", d.num_groups_limit, n[r]);
+      set_error("numGroupsLimit %d would bind (%llu groups): fall back to the reference operator", d.num_groups_limit, groups[r]);
       return PB200_E_LIMIT;
     }
   }
   if (!speculative) {  // exact-size block, second pass
-    size_t off = 64 + 8ull * nres;
+    size_t off = head;
     for (int r = 0; r < nres; r++) off = layout_result(Rs[r]->dense, descs[r], off, kept_rows(Rs[r], n[r]));
     auto pin2 = std::make_shared<PinnedBlock>();
     pin2->ctx = ctx;
@@ -504,7 +583,7 @@ int extract_groups(pb200_ctx* ctx, pb200_result* const* Rs, int nres, cudaStream
     PB200_CUDA(cudaMemcpyAsync(ddesc.p, descs.data(), sizeof(ExtractDesc) * nres, cudaMemcpyHostToDevice, st));
     if (chunks) extract_write_kernel<<<chunks, kExtractThreads, 0, st>>>(ddescs, nres, (const uint32_t*)dcount.p, totals, (unsigned char*)staging.p, false);
     PB200_CUDA(cudaGetLastError());
-    const size_t head = 64 + 8ull * nres;  // the block's header is not written by the kernel
+    // the block's header is not written by the kernel
     if (off > head) PB200_CUDA(cudaMemcpyAsync(out + head, (unsigned char*)staging.p + head, off - head, cudaMemcpyDeviceToHost, st));
     PB200_CUDA(cudaStreamSynchronize(st));
   }
@@ -638,6 +717,38 @@ void order_rows_host(pb200_result* R, const pb200_order_by& o, const int32_t* fn
   }
   R->distinct = std::move(distinct);
   R->view = pb200_result::View();
+  R->meta.num_groups = (int32_t)kept;
+}
+
+int having_check(const pb200_having* h, int num_aggs, int num_group_by, int nres, bool deferred) {
+  if (!h) return PB200_OK;
+  if (const char* why = having_validate(h, num_aggs)) { set_error("%s", why); return PB200_E_INVALID; }
+  if (num_group_by <= 0) { set_error("HAVING needs a GROUP BY"); return PB200_E_INVALID; }
+  if (nres != 1) {
+    set_error("HAVING needs a final result: merge the segments or pass one (a call writing %d per-segment results is not final)", nres);
+    return PB200_E_INVALID;
+  }
+  if (deferred) { set_error("HAVING across GPUs (PB200_Q_DEFER_FINALIZE, reduce_world > 1) is not accelerated"); return PB200_E_UNSUPPORTED; }
+  return PB200_OK;
+}
+
+void having_rows_host(pb200_result* R, const pb200_having& h, const int32_t* fns) {
+  R->having = h;
+  if (R->meta.num_groups < 0) return;
+  result_materialize(R);
+  const size_t rows = (size_t)R->meta.num_groups, ngb = (size_t)R->meta.num_group_by, nagg = (size_t)R->meta.num_aggs;
+  size_t kept = 0;
+  for (size_t r = 0; r < rows; r++) {
+    if (!having_eval(h, [&](int a) { return having_value(fns[a], R->dbl[a][r], R->lng[a][r]); })) continue;
+    for (size_t k = 0; k < ngb; k++) R->keys[kept * ngb + k] = R->keys[r * ngb + k];
+    for (size_t a = 0; a < nagg; a++) { R->dbl[a][kept] = R->dbl[a][r]; R->lng[a][kept] = R->lng[a][r]; R->ids[a][kept] = R->ids[a][r]; }
+    if (kept != r)
+      for (auto& d : R->distinct) if (d.size() == rows) d[kept] = std::move(d[r]);
+    ++kept;
+  }
+  R->keys.resize(kept * ngb);
+  for (size_t a = 0; a < nagg; a++) { R->dbl[a].resize(kept); R->lng[a].resize(kept); R->ids[a].resize(kept); }
+  for (auto& d : R->distinct) if (d.size() == rows) d.resize(kept);
   R->meta.num_groups = (int32_t)kept;
 }
 

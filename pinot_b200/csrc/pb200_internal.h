@@ -216,6 +216,8 @@ struct pb200_result {
     unsigned long long one[pb200::kMaxAggs][3] = {};        // aggregation only: the same for the one row
   } mom;
   pb200_order_by order{};                      // ORDER BY spec of a group-by result (num_items 0: none), applied at extraction
+  pb200_having having{};                       // HAVING of a group-by result (num_nodes 0: none), applied at extraction before
+                                               // the order; set on every result whose rows it filtered
   std::vector<int32_t> agg_functions;            // PB200_AGG_* per aggregation (set by pb200_execute)
   std::vector<int32_t> keys;                     // [G x k]
   std::vector<std::vector<double>> dbl;          // per agg [rows]
@@ -324,6 +326,12 @@ int order_validate(const pb200_order_by* order, int num_aggs, int num_group_by);
 // Orders and trims a host-built group-by result (rows in its std::vector fields or view) by `order`; fns = PB200_AGG_* per
 // aggregation.  Same keys as the device sort (pb200_order.h); the result's rows end up in its std::vector fields.
 void order_rows_host(pb200_result* R, const pb200_order_by& order, const int32_t* fns);
+// pb200_having checks of the device and host entry points (having may be NULL): PB200_OK, or PB200_E_INVALID /
+// PB200_E_UNSUPPORTED (message set).  nres = results the call writes, deferred = PB200_Q_DEFER_FINALIZE or reduce_world > 1.
+int having_check(const pb200_having* having, int num_aggs, int num_group_by, int nres, bool deferred);
+// Keeps the rows of a host-built group-by result that pass `having` (pb200_having.h, fns = PB200_AGG_* per aggregation)
+// and marks the result as filtered; the kept rows end up in its std::vector fields, in their order.
+void having_rows_host(pb200_result* R, const pb200_having& having, const int32_t* fns);
 
 // pb200_roaring.cu
 // One serialized RoaringBitmap (posting list of one dictId) to be OR-ed into `mask` (1 bit per doc, bit j of 32-bit

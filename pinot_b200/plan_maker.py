@@ -553,6 +553,29 @@ def order_spec(q: QueryContext, merge: bool):
     return spec
 
 
+def having_spec(q: QueryContext):
+    """pb200_having of a query with HAVING (None otherwise): sql.resolve_having's postfix nodes as the C struct."""
+    from .sql import resolve_having
+    nodes = resolve_having(q)
+    if not nodes:
+        return None
+    spec = _lib.Having(len(nodes), 0)
+    for i, n in enumerate(nodes):
+        op = _lib.HAVING_CODES[n[0]]
+        if n[0] in ("AND", "OR"):
+            spec.nodes[i] = _lib.HavingNode(op, n[1], 0, 0, 0.0, 0.0)
+        elif n[0] == "NOT":
+            spec.nodes[i] = _lib.HavingNode(op, 1, 0, 0, 0.0, 0.0)
+        elif n[0] in ("EQ", "NEQ"):
+            spec.nodes[i] = _lib.HavingNode(op, 0, n[1], 0, n[2], 0.0)
+        else:
+            _, a, lo, hi, lo_inc, hi_inc = n
+            flags = ((_lib.HAVING_LO_UNBOUNDED if lo is None else 0) | (_lib.HAVING_HI_UNBOUNDED if hi is None else 0) |
+                     (0 if lo_inc else _lib.HAVING_LO_EXCLUSIVE) | (0 if hi_inc else _lib.HAVING_HI_EXCLUSIVE))
+            spec.nodes[i] = _lib.HavingNode(op, 0, a, flags, 0.0 if lo is None else lo, 0.0 if hi is None else hi)
+    return spec
+
+
 class _NativeResult:
     """Owner of a native pb200_result whose columns numpy arrays alias (views=True): freed with the block (or release())."""
 
@@ -738,7 +761,9 @@ class B200PlanMaker:
         well, a group-by block comes back WITHOUT its groups extracted (PB200_Q_DEFER_FINALIZE): its dense device tables
         are meant to be reduced across GPUs (pinot_b200.distributed.combine_across_ranks), which extracts on the root.
         A GROUP BY query with an ORDER BY gets its rows ordered and trimmed by the library (order_spec; a deferred block
-        when it is extracted); ordered=False returns every group in the library's row order."""
+        when it is extracted); ordered=False returns every group in the library's row order.  A query with HAVING gets
+        its rows filtered by the library before that order when the call's result is final (merge=True, or one segment,
+        and ordered); per-segment blocks of several segments come back unfiltered, for the caller's merge to filter."""
         # merge + keep_handle: the caller reduces the dense tables across GPUs first; groups are extracted afterwards
         # defer=False with keep_handle=True: extracted blocks that keep their native handle (to_datatable); release() them
         if defer is None:
@@ -756,8 +781,13 @@ class B200PlanMaker:
         res = (C.c_void_p * nres)()
         kinds = (C.c_int32 * n)()
         spec = order_spec(query, merge) if ordered else None
+        having = having_spec(query) if ordered and (merge or n == 1) else None
         pct = [a.function == "PERCENTILE" for a in query.aggregations]
-        if any(pct):
+        if having is not None:
+            args = (C.c_double * max(1, len(pct)))(*[float(a.arg) if is_p else 0.0 for a, is_p in zip(query.aggregations, pct)])
+            _lib.check(self.ctx.lib.pb200h_execute_having(self.ctx.handle, C.byref(hq), C.byref(spec) if spec is not None else None,
+                                                          args, C.byref(having), segs, n, res, kinds))
+        elif any(pct):
             # one argument per aggregation: the percentile of each PERCENTILE (pb200h_execute_args)
             args = (C.c_double * len(pct))(*[float(a.arg) if is_p else 0.0 for a, is_p in zip(query.aggregations, pct)])
             _lib.check(self.ctx.lib.pb200h_execute_args(self.ctx.handle, C.byref(hq), C.byref(spec) if spec is not None else None,

@@ -52,6 +52,8 @@ class Aggregation:
     # evaluated together with the query's own filter (AggregationFunctionUtils.buildFilteredAggregationInfos)
     filter: Optional["FilterNode"] = None
     arg: Optional[float] = None  # PERCENTILE: the percentile, 0 <= p <= 100
+    # named only in HAVING: computed like the others, never an output column (Pinot's QueryContext adds such functions too)
+    hidden: bool = False
 
     def __str__(self):
         if self.function == "PERCENTILE":
@@ -175,10 +177,37 @@ class QueryContext:
     # (query options minServerGroupTrimSize, default 5000) and per-segment results (minSegmentGroupTrimSize, default off)
     min_server_group_trim_size: int = 5000
     min_segment_group_trim_size: int = -1
+    # HAVING: a filter tree whose leaves name aggregations by sql.having_name and compare them with numeric literals
+    # (sql.resolve_having gives the library's postfix form); applied to final rows, before ORDER BY and LIMIT
+    having: Optional[FilterNode] = None
 
     @property
     def is_group_by(self) -> bool:
         return len(self.group_by) > 0
+
+
+def having_eval(nodes, values) -> bool:
+    """The outcome of a HAVING postfix tree (sql.resolve_having) for one row; values[a] = the final value of aggregation a
+    as a float.  Python's float comparisons are Java's: a NaN matches only NEQ, -0.0 == 0.0 (pinot_b200/csrc/pb200_having.h
+    is the library's copy of this rule)."""
+    stack = []
+    for n in nodes:
+        op = n[0]
+        if op in ("AND", "OR"):
+            args = stack[len(stack) - n[1]:]
+            del stack[len(stack) - n[1]:]
+            stack.append(all(args) if op == "AND" else any(args))
+        elif op == "NOT":
+            stack.append(not stack.pop())
+        elif op == "EQ":
+            stack.append(values[n[1]] == n[2])
+        elif op == "NEQ":
+            stack.append(not values[n[1]] == n[2])
+        else:  # RANGE: (agg, lo or None, hi or None, lo inclusive, hi inclusive)
+            _, a, lo, hi, lo_inc, hi_inc = n
+            v = values[a]
+            stack.append((lo is None or (v >= lo if lo_inc else v > lo)) and (hi is None or (v <= hi if hi_inc else v < hi)))
+    return stack[0]
 
 
 # ----------------------------------------------------------------------------------------------------------------------

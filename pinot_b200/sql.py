@@ -6,7 +6,8 @@ stays Java).  This module exists so the parity tests read like the reference's
 (``getOperator("SELECT COUNT(*), SUM(column1) FROM testTable WHERE ... GROUP BY column9")``,
 ``pinot-core/src/test/java/org/apache/pinot/queries/BaseQueriesTest.java:97-102``).  Grammar:
 
-    SELECT item[, item...] FROM table [WHERE cond] [GROUP BY col[, col...]] [ORDER BY expr [ASC|DESC], ...] [LIMIT n]
+    SELECT item[, item...] FROM table [WHERE cond] [GROUP BY col[, col...] [HAVING hcond]] [ORDER BY expr [ASC|DESC], ...]
+           [LIMIT n]
     item  := COUNT(*) | FN(col) | PERCENTILE(col, p) | PERCENTILE<n>(col) | col
              (FN also VAR_POP / VARPOP, VAR_SAMP / VARSAMP, STDDEV_POP / STDDEVPOP, STDDEV_SAMP / STDDEVSAMP)
              (plain columns are allowed only when they are group-by keys; 0 <= p <= 100, fractions allowed)
@@ -16,6 +17,9 @@ stays Java).  This module exists so the parity tests read like the reference's
     cond  := cond AND cond | cond OR cond | NOT cond | (cond) | col op literal | col BETWEEN a AND b
              | col [NOT] IN (literal, ...)
     op    := = | != | <> | < | <= | > | >=
+    hcond := cond whose left-hand sides are aggregation calls (COUNT(*), FN(col), PERCENTILE(col, p), ...) and whose
+             literals are numbers.  An aggregation named only in HAVING is computed as a hidden one (Aggregation.hidden):
+             ORDER BY may name it, it is never an output column.  HAVING on a column belongs in WHERE and is refused.
     col   := a column, or a single-column expression wherever a column is accepted (select list, GROUP BY, aggregation
              arguments, the left-hand side of predicates, ORDER BY, selection and DISTINCT lists):
              expr := term (+|- term)* ; term := factor (*|/|% factor)* ; factor := col | number | (expr) | fn(args)
@@ -29,7 +33,7 @@ import re
 from dataclasses import dataclass, field
 from typing import List, Optional
 
-from .query import Aggregation, Filter, FilterNode, Predicate, QueryContext, optimize_filter
+from .query import Aggregation, Filter, FilterNode, Predicate, QueryContext, flatten, optimize_filter
 
 _TOKEN = re.compile(r"\s*(?:(\d+\.\d+(?:[eE][-+]?\d+)?|-?\d+\.\d+|-?\d+)|'((?:[^']|'')*)'|(<=|>=|<>|!=|[=<>(),*+/%-])|"
                     r"([A-Za-z_$][A-Za-z0-9_$]*))")
@@ -84,6 +88,16 @@ class SqlError(ValueError):
     pass
 
 
+def having_name(agg: Aggregation) -> str:
+    """How a HAVING leaf names an aggregation (QueryContext.having)."""
+    if agg.function == "PERCENTILE":
+        return f"percentile({agg.column},{agg.arg!r})"
+    return f"{agg.function.lower()}({agg.column or '*'})"
+
+
+MAX_HAVING_NODES = 32
+
+
 class _Parser:
     def __init__(self, text: str):
         self.toks = []
@@ -104,6 +118,7 @@ class _Parser:
                 self.toks.append(("id", ident))
             pos = m.end()
         self.i = 0
+        self.having: Optional[List[Aggregation]] = None   # inside HAVING: the aggregations its leaves name
 
     def peek(self):
         return self.toks[self.i] if self.i < len(self.toks) else (None, None)
@@ -208,8 +223,40 @@ class _Parser:
         k, v = self.peek()
         if k not in ("num", "str"):
             raise SqlError(f"expected literal, got {self.peek()}")
+        if k == "str" and self.having is not None:
+            raise SqlError(f"HAVING compares aggregations with numbers, got the string literal {v!r}")
         self.i += 1
         return v
+
+    def aggregation_call(self) -> Aggregation:
+        """An aggregation call after its name, e.g. `SUM(` + `m)`: the name token is at self.i - 2."""
+        name = self.toks[self.i - 2][1]
+        fn = _ALIASES.get(name.upper(), name.upper())
+        if fn.startswith("PERCENTILE"):
+            col, pct = self.percentile_call(name)
+            agg = Aggregation("PERCENTILE", col, arg=pct)
+        elif self.take_op("*"):
+            if fn != "COUNT":
+                raise SqlError(f"{fn}(*) is not valid")
+            agg = Aggregation("COUNT", None)
+        else:
+            col = self.column()
+            agg = Aggregation("COUNT", None) if fn == "COUNT" else Aggregation(fn, col)
+        self.expect_op(")")
+        return agg
+
+    def having_operand(self) -> str:
+        """Left-hand side of a HAVING comparison: an aggregation call, named by having_name."""
+        k, v = self.peek()
+        if k in ("num", "str"):
+            raise SqlError(f"HAVING: the literal {v!r} is on the left-hand side; write the aggregation first")
+        if k == "id" and _is_function(v) and self.toks[self.i + 1:self.i + 2] == [("op", "(")]:
+            self.i += 2
+            agg = self.aggregation_call()
+            self.having.append(agg)
+            return having_name(agg)
+        col = self.column()
+        raise SqlError(f"HAVING on the column {col}: HAVING filters aggregations, move the condition to WHERE")
 
     # cond := or
     def cond(self) -> FilterNode:
@@ -243,7 +290,7 @@ class _Parser:
         return self.comparison()
 
     def comparison(self) -> FilterNode:
-        col = self.column()
+        col = self.having_operand() if self.having is not None else self.column()
         if self.take_kw("BETWEEN"):
             lo = self.literal()
             self.expect_kw("AND")
@@ -303,6 +350,50 @@ def resolve_order_by(query: QueryContext) -> List[tuple]:
     return out
 
 
+def _same_aggregation(a: Aggregation, b: Aggregation) -> bool:
+    """a computes what the HAVING leaf b names (a FILTER clause makes it another aggregation)."""
+    return a.filter is None and having_name(a) == having_name(b)
+
+
+def resolve_having(query: QueryContext) -> List[tuple]:
+    """HAVING -> the library's postfix form (pb200_having), root last: ("AND" | "OR", operands), ("NOT",),
+    ("EQ" | "NEQ", agg, value), ("RANGE", agg, lo or None, hi or None, lo inclusive, hi inclusive), where agg indexes
+    query.aggregations and values are floats.  IN becomes an OR of EQ leaves, NOT IN an AND of NEQ leaves.  [] without
+    HAVING; more than MAX_HAVING_NODES nodes is refused."""
+    if query.having is None:
+        return []
+    out: List[tuple] = []
+
+    def index(name):
+        for a, agg in enumerate(query.aggregations):
+            if agg.filter is None and having_name(agg) == name:
+                return a
+        raise SqlError(f"HAVING {name}: no aggregation of the query computes it")
+
+    def walk(n):
+        if isinstance(n, Filter):
+            for c in n.children:
+                walk(c)
+            out.append(("NOT",) if n.type == "NOT" else (n.type, len(n.children)))
+            return
+        a = index(n.column)
+        if n.type in ("EQ", "NEQ"):
+            out.append((n.type, a, float(n.values[0])))
+        elif n.type in ("IN", "NOT_IN"):
+            leaf = "EQ" if n.type == "IN" else "NEQ"
+            out.extend((leaf, a, float(v)) for v in n.values)
+            if len(n.values) > 1:
+                out.append(("OR" if n.type == "IN" else "AND", len(n.values)))
+        else:
+            out.append(("RANGE", a, None if n.lower is None else float(n.lower), None if n.upper is None else float(n.upper),
+                        n.lower_inclusive, n.upper_inclusive))
+
+    walk(query.having)
+    if len(out) > MAX_HAVING_NODES:
+        raise SqlError(f"HAVING needs {len(out)} nodes, at most {MAX_HAVING_NODES} are supported")
+    return out
+
+
 def parse(sql: str, **options) -> QueryContext:
     """SQL text -> QueryContext (filter already run through the broker-side filter optimizers)."""
     p = _Parser(sql)
@@ -313,18 +404,7 @@ def parse(sql: str, **options) -> QueryContext:
         k, name = p.peek()
         if k == "id" and _is_function(name) and p.toks[p.i + 1:p.i + 2] == [("op", "(")]:
             p.i += 2
-            fn = _ALIASES.get(name.upper(), name.upper())
-            if fn.startswith("PERCENTILE"):
-                col, pct = p.percentile_call(name)
-                aggs.append(Aggregation("PERCENTILE", col, arg=pct))
-            elif p.take_op("*"):
-                if fn != "COUNT":
-                    raise SqlError(f"{fn}(*) is not valid")
-                aggs.append(Aggregation("COUNT", None))
-            else:
-                col = p.column()
-                aggs.append(Aggregation("COUNT", None) if fn == "COUNT" else Aggregation(fn, col))
-            p.expect_op(")")
+            aggs.append(p.aggregation_call())
             if p.take_kw("FILTER"):   # SUM(x) FILTER (WHERE cond)
                 p.expect_op("(")
                 p.expect_kw("WHERE")
@@ -345,6 +425,17 @@ def parse(sql: str, **options) -> QueryContext:
         group_by.append(p.column())
         while p.take_op(","):
             group_by.append(p.column())
+    having: Optional[FilterNode] = None
+    if p.take_kw("HAVING"):
+        if not group_by:
+            raise SqlError("HAVING needs a GROUP BY (HAVING on an aggregation-only query is not supported)")
+        p.having = []
+        having = flatten(p.cond())
+        for agg in p.having:   # aggregations named only in HAVING: hidden extra aggregations
+            if not any(_same_aggregation(a, agg) for a in aggs):
+                agg.hidden = True
+                aggs.append(agg)
+        p.having = None
     order_by = []
     if p.take_kw("ORDER"):
         p.expect_kw("BY")
@@ -381,8 +472,9 @@ def parse(sql: str, **options) -> QueryContext:
     if not aggs:
         raise SqlError("only aggregation / group-by queries are on this path")
     query = QueryContext(aggregations=aggs, filter=optimize_filter(flt), group_by=group_by, table=table, limit=limit,
-                         order_by=order_by, **options)
+                         order_by=order_by, having=having, **options)
     resolve_order_by(query)
+    resolve_having(query)
     return query
 
 
