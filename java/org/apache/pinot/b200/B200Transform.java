@@ -260,6 +260,9 @@ final class B200Transform {
      */
     int[] matchingIds(Predicate predicate) {
       int n = cardinality();
+      if (_doubles != null) {
+        return valueMatches(predicate);
+      }
       switch (predicate.getType()) {
         case RANGE: {
           RangePredicate r = (RangePredicate) predicate;
@@ -278,6 +281,67 @@ final class B200Transform {
         default:
           return null;
       }
+    }
+
+    /**
+     * A DOUBLE expression has no dictionary in the reference: ExpressionFilterOperator evaluates it per row and compares
+     * each value with Java's <, > and == (the raw-value predicate evaluators).  So NaN matches only NOT_EQ / NOT_IN, and
+     * 0 matches both zeros.  In Double.compare order the entries a RANGE matches are contiguous (the zeros are
+     * neighbours, NaN is last and matches no range), so a scan of [first, last] selects exactly them.
+     */
+    private int[] valueMatches(Predicate predicate) {
+      List<String> values;
+      boolean negate = false;
+      switch (predicate.getType()) {
+        case RANGE: {
+          RangePredicate r = (RangePredicate) predicate;
+          boolean lowerOpen = r.getLowerBound().equals(RangePredicate.UNBOUNDED);
+          boolean upperOpen = r.getUpperBound().equals(RangePredicate.UNBOUNDED);
+          double lower = lowerOpen ? 0.0 : Double.parseDouble(r.getLowerBound());
+          double upper = upperOpen ? 0.0 : Double.parseDouble(r.getUpperBound());
+          List<Integer> out = new ArrayList<>();
+          for (int k = 0; k < _doubles.length; k++) {
+            double x = _doubles[k];
+            boolean above = lowerOpen || (r.isLowerInclusive() ? x >= lower : x > lower);
+            boolean below = upperOpen || (r.isUpperInclusive() ? x <= upper : x < upper);
+            if (above && below && x == x) {  // an unbounded range matches no NaN either
+              out.add(k);
+            }
+          }
+          return out.stream().mapToInt(Integer::intValue).toArray();
+        }
+        case EQ:
+          values = List.of(((EqPredicate) predicate).getValue());
+          break;
+        case NOT_EQ:
+          values = List.of(((NotEqPredicate) predicate).getValue());
+          negate = true;
+          break;
+        case IN:
+          values = ((InPredicate) predicate).getValues();
+          break;
+        case NOT_IN:
+          values = ((NotInPredicate) predicate).getValues();
+          negate = true;
+          break;
+        default:
+          return null;
+      }
+      double[] literals = new double[values.size()];
+      for (int k = 0; k < literals.length; k++) {
+        literals[k] = Double.parseDouble(values.get(k));
+      }
+      List<Integer> out = new ArrayList<>();
+      for (int k = 0; k < _doubles.length; k++) {
+        boolean hit = false;
+        for (double l : literals) {
+          hit |= _doubles[k] == l;
+        }
+        if (hit != negate) {
+          out.add(k);
+        }
+      }
+      return out.stream().mapToInt(Integer::intValue).toArray();
     }
 
     private static int[] range(int start, int end) {

@@ -35,11 +35,16 @@ struct Evaluated {
   std::vector<int32_t> ids;     // EQ/IN matching ids; NEQ/NOT_IN NON-matching ids (sorted)
 };
 
-// A FLOAT / DOUBLE column the segment stores raw, with a dictionary synthesised at load: the reference evaluates its
-// predicates per value with Java's <, > and == (the *RawValueBased*PredicateEvaluators), not by a dictionary search.  So
-// NaN matches only NEQ / NOT_IN, and 0 matches both zeros.  The matching entries are found by one pass over the
-// dictionary (at most raw_dict_max entries); in Double.compare order they are contiguous for a RANGE (the zeros are
-// neighbours and NaN, which no range matches, is last).
+// The FLOAT / DOUBLE columns the reference has no dictionary for, so it evaluates their predicates per value with Java's
+// <, > and == (the *RawValueBased*PredicateEvaluators), not by a dictionary search: a column the segment stores raw, with
+// a dictionary synthesised at load, and a DOUBLE expression (ExpressionFilterOperator evaluates it per row), whose
+// dictionary the derivation built.  So NaN matches only NEQ / NOT_IN, and 0 matches both zeros.  The matching entries are
+// found by one pass over the dictionary; both dictionaries are in Double.compare order with one NaN entry, last, so for a
+// RANGE they are contiguous (the zeros are neighbours and NaN, which no range matches, is last).
+bool compared_by_value(const HostColumn& c) {
+  return (c.synthesized_dictionary || c.derived) && (c.data_type == PB200_FLOAT || c.data_type == PB200_DOUBLE);
+}
+
 bool raw_value_matches(const HostColumn& c, int id, const pb200h_filter_node& n, const pb200h_literal* v) {
   const bool fl = c.data_type == PB200_FLOAT;
   const double x = c.as_double(id);
@@ -59,7 +64,7 @@ Evaluated evaluate(const HostColumn& c, const pb200h_filter_node& n, const pb200
   Evaluated e;
   const pb200h_literal* v = lits + n.values_offset;
   const int card = c.cardinality;
-  if (c.synthesized_dictionary && (c.data_type == PB200_FLOAT || c.data_type == PB200_DOUBLE)) {
+  if (compared_by_value(c)) {
     e.is_range = n.type == PB200H_RANGE;
     e.exclusive = n.type == PB200H_NEQ || n.type == PB200H_NOT_IN;
     for (int id = 0; id < card; id++) if (raw_value_matches(c, id, n, v)) e.ids.push_back(id);

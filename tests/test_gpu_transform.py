@@ -10,8 +10,8 @@ with the product), written by the oracle's segment writer without an inverted in
     nothing, 12 threads deriving at once leave one column per segment; every refusal;
   * a source bound to a domain wider than the segment, DataTable bytes (the expression's name and result type), a
     star-tree segment answering an expression by the raw scan, and destroyed segments giving their derived memory back.
-Predicates on DOUBLE expressions whose results include -0.0 or NaN keep the open status of DOUBLE columns (DESIGN.md
-section 5): the expressions and data here produce neither."""
+The expressions and data here produce no NaN and no -0.0: tests/test_gpu_transform_edges.py holds expressions that do
+to a per-row reference."""
 import threading
 
 import numpy as np
