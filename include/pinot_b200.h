@@ -111,6 +111,19 @@ int32_t pb200_segment_release(pb200_ctx* ctx, pb200_segment* segment);
 /* Bytes of HBM held by the segment. */
 int64_t pb200_segment_device_bytes(const pb200_segment* segment);
 
+/* ---- REGEXP_LIKE on STRING dictionaries (RegexpLikePredicateEvaluatorFactory: a pattern -> matching dictIds) --------- */
+/* Matches `pattern` (UTF-8, NUL terminated; Java's Pattern.compile(pattern).matcher(value).find() over the subset of
+ * DESIGN.md section 3.12) against every entry of column columns[s] of segments[s], for all segments in one launch, and
+ * sets bit j of match_bits[s] (bit j % 32 of word j / 32) iff entry j of the segment's OWN dictionary matches: for a
+ * column bound to a domain, ids are the segment's local dictIds, not the domain's.  match_bits[s] holds
+ * ceil(cardinality / 32) words of that dictionary; the bits after the last entry of its last word are 0.  A value is
+ * its dictionary entry up to the first NUL.  The first call on a column uploads a compact copy of its dictionary (counted
+ * in pb200_segment_device_bytes, freed with the segment).  PB200_E_INVALID: a pattern that is not valid UTF-8, bad
+ * arguments.  PB200_E_UNSUPPORTED: a pattern outside the subset, a column that is not a STRING dictionary column of the
+ * segment (raw, derived). */
+int32_t pb200_match_pattern(pb200_ctx* ctx, const char* pattern, int32_t num_segments, pb200_segment* const* segments,
+                            const int32_t* columns, uint32_t* const* match_bits);
+
 /* ---- table-wide dictionaries ("domains") ------------------------------------------------------------------------- */
 /* dictIds are segment local in Pinot; the reference merges per-segment results BY VALUE
  * (GroupByCombineOperator.java:130-146 -> IndexedTable.upsert, AggregationFunction.merge).  A device-side or cross-GPU

@@ -131,7 +131,13 @@ int32_t pb200h_startree_attach(pb200_ctx* ctx, pb200h_segment* segment, const vo
 
 /* ---- QueryContext ---------------------------------------------------------------------------------------------- */
 enum { PB200H_AND = 0, PB200H_OR = 1, PB200H_NOT = 2, PB200H_EQ = 3, PB200H_NEQ = 4, PB200H_IN = 5, PB200H_NOT_IN = 6,
-       PB200H_RANGE = 7 };
+       PB200H_RANGE = 7, PB200H_REGEXP_LIKE = 8 };
+/* PB200H_REGEXP_LIKE: one literal, `s` = the pattern (pb200_match_pattern), on a STRING dictionary column.  Every pattern
+ * leaf of a call -- filter and FILTER (WHERE ...) clauses -- is resolved on the device before planning, one
+ * pb200_match_pattern per distinct (pattern, column) over all segments of the call; the leaf is then planned as an IN
+ * over the matching dictIds (EMPTY / MATCH_ALL when none / all match; sorted, inverted or scan leaf as for IN).
+ * PB200_E_UNSUPPORTED: a column that is not a STRING dictionary column, a derived column, a pattern outside the subset;
+ * PB200_E_INVALID: a pattern that is not valid UTF-8. */
 
 typedef struct {
   /* `d`: every numeric literal rounded to double (FLOAT columns compare (float)d).  `i`: the literal when it is an

@@ -36,6 +36,7 @@ import org.apache.pinot.core.query.aggregation.groupby.ObjectGroupByResultHolder
 import org.apache.pinot.core.query.request.context.QueryContext;
 import org.apache.pinot.segment.local.customobject.AvgPair;
 import org.apache.pinot.segment.spi.IndexSegment;
+import org.apache.pinot.spi.data.FieldSpec;
 import org.apache.pinot.segment.spi.SegmentContext;
 import org.apache.pinot.segment.spi.datasource.DataSource;
 import org.apache.pinot.segment.spi.index.reader.Dictionary;
@@ -90,6 +91,12 @@ public class B200Operator extends BaseOperator<BaseResultsBlock> {
         switch (p.getType()) {
           case EQ: case NOT_EQ: case IN: case NOT_IN: case RANGE:
             return true;
+          case REGEXP_LIKE:
+            // a pattern on a dictionary STRING column resolves to dictIds like an IN (flatten() asks Pinot's own
+            // PredicateEvaluator for them, so Java's regex semantics hold exactly)
+            return p.getLhs().getType() == ExpressionContext.Type.IDENTIFIER
+                && segment.getDataSource(p.getLhs().getIdentifier()).getDataSourceMetadata().getDataType().getStoredType()
+                == FieldSpec.DataType.STRING;
           default:
             return false;
         }

@@ -19,7 +19,7 @@ FWD_DICT_FIXEDBIT, FWD_DICT_SORTED, FWD_RAW_FIXEDBYTE = 0, 1, 2
 AGG_CODES = {"COUNT": 0, "SUM": 1, "MIN": 2, "MAX": 3, "AVG": 4, "DISTINCTCOUNT": 5, "PERCENTILE": 6,
              "VARPOP": 7, "VARSAMP": 8, "STDDEVPOP": 9, "STDDEVSAMP": 10}
 MOMENT_FUNCTIONS = ("VARPOP", "VARSAMP", "STDDEVPOP", "STDDEVSAMP")
-FILTER_CODES = {"AND": 0, "OR": 1, "NOT": 2, "EQ": 3, "NEQ": 4, "IN": 5, "NOT_IN": 6, "RANGE": 7}
+FILTER_CODES = {"AND": 0, "OR": 1, "NOT": 2, "EQ": 3, "NEQ": 4, "IN": 5, "NOT_IN": 6, "RANGE": 7, "REGEXP_LIKE": 8}
 REGIMES = {0: "NONE", 1: "ARRAY", 2: "INT_MAP", 3: "LONG_MAP", 4: "ARRAY_MAP"}
 OPERATOR_KINDS = {0: "AGGREGATION", 1: "GROUP_BY", 2: "NON_SCAN_AGGREGATION", 3: "EMPTY", 4: "STAR_TREE"}
 
@@ -201,6 +201,7 @@ EXPORTED_SYMBOLS = [
     "pb200_segment_derive_column", "pb200h_segment_derive",
     "pb200h_startree_build", "pb200h_startree_get",
     "pb200_execute_having", "pb200h_execute_having",
+    "pb200_match_pattern",
 ]
 
 _LIB = None
@@ -279,6 +280,7 @@ def load() -> C.CDLL:
     L.pb200_roaring_validate.argtypes = [vp, C.c_uint64, C.c_int64]
     L.pb200_doc_mask_upload.argtypes = [vp, i32, vp, C.c_int64, C.POINTER(vp)]
     L.pb200_doc_mask_free.argtypes = [vp, vp]
+    L.pb200_match_pattern.argtypes = [vp, C.c_char_p, i32, C.POINTER(vp), C.POINTER(i32), C.POINTER(vp)]
     L.pb200_last_phases.argtypes = [C.POINTER(C.c_double)]
     L.pb200_comm_unique_id.argtypes = [vp]
     L.pb200_comm_init.argtypes = [vp, vp, i32, i32]

@@ -195,4 +195,24 @@ int leaf_to_device(const pb200h_segment& seg, int column, const pb200h_filter_no
                    SegmentFilterStore& store, pb200_filter_node& out);
 int try_star_tree(pb200_ctx* ctx, const pb200h_segment& seg, const StarTreeIndex& st, const pb200h_query& q,
                   pb200_result** out);
+
+// patterns.cpp: the matching dictIds of the REGEXP_LIKE leaves of one call.  An entry point declares one PatternScope
+// (it becomes the calling thread's innermost scope until it goes out of scope) and fills it with resolve_patterns before
+// planning; evaluate() then finds a leaf's ids with pattern_ids, which searches the thread's scopes innermost first, so
+// a nested call (a FILTER clause's submission) reuses what its caller resolved.
+struct PatternScope {
+  std::vector<std::pair<std::pair<const HostColumn*, std::string>, std::vector<int32_t>>> ids;  // local dictIds, ascending
+  PatternScope* outer;
+  PatternScope();
+  ~PatternScope();
+  PatternScope(const PatternScope&) = delete;
+  PatternScope& operator=(const PatternScope&) = delete;
+};
+// One pb200_match_pattern per distinct (pattern, column) of the query's filter and FILTER clauses not resolved yet, over
+// all segments; PB200_E_UNSUPPORTED for a column that is not a STRING dictionary column or is derived
+int resolve_patterns(pb200_ctx* ctx, const pb200h_query& q, pb200h_segment* const* segs, int nseg, PatternScope& scope);
+// The matching ids of `pattern` on column c, or NULL when no scope of the thread resolved it
+const std::vector<int32_t>* pattern_ids(const HostColumn& c, const char* pattern);
+// Makes `to` (a star-tree dimension, sharing `from`'s dictionary) resolve `pattern` as `from` does, when `from` does
+void pattern_alias(const HostColumn& from, const HostColumn& to, const char* pattern);
 }  // namespace pb200h

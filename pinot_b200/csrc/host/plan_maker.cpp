@@ -64,6 +64,12 @@ Evaluated evaluate(const HostColumn& c, const pb200h_filter_node& n, const pb200
   Evaluated e;
   const pb200h_literal* v = lits + n.values_offset;
   const int card = c.cardinality;
+  if (n.type == PB200H_REGEXP_LIKE) {   // resolved before planning (patterns.cpp): an IN over the matching ids
+    if (const std::vector<int32_t>* m = pattern_ids(c, v[0].s)) e.ids = *m;
+    const int k = (int)e.ids.size();
+    if (k == 0) e.always_false = true; else if (k == card) e.always_true = true;
+    return e;
+  }
   if (compared_by_value(c)) {
     e.is_range = n.type == PB200H_RANGE;
     e.exclusive = n.type == PB200H_NEQ || n.type == PB200H_NOT_IN;
@@ -119,6 +125,13 @@ bool raw_leaf(const HostColumn& c, const pb200h_filter_node& n, const pb200h_lit
   // EQ with a fractional literal: [ceil, floor] is empty
   if (n.type == PB200H_EQ) { d.op = PB200_F_RAW_RANGE; d.raw_lo = d.raw_hi = v[0].d; d.raw_flags = 0; return true; }
   return false;
+}
+
+// A pattern leaf is planned from the ids its call resolved (resolve_patterns); one that was not is a caller's error
+int check_resolved(const HostColumn& c, const pb200h_filter_node& n, const pb200h_literal* lits) {
+  if (n.type != PB200H_REGEXP_LIKE || pattern_ids(c, lits[n.values_offset].s)) return PB200_OK;
+  set_error("REGEXP_LIKE leaf on '%s' was not resolved before planning", c.name.c_str());
+  return PB200_E_INVALID;
 }
 
 // One segment's device filter tree + the arrays its nodes point to.
@@ -203,6 +216,7 @@ int build_segment_filter(const pb200h_segment& seg, const pb200h_query& q, Segme
       text.push_back(std::string("FILTER_FULL_SCAN(") + (n.type == PB200H_RANGE ? "RANGE," : "EQ,") + c.name + ")");
       continue;
     }
+    if (int rc = check_resolved(c, n, q.literals)) return rc;
     Evaluated e = evaluate(c, n, q.literals);
     d.column = ci;
     if (e.always_false) { d.op = PB200_F_EMPTY; constant.push_back(2); text.push_back("FILTER_EMPTY"); continue; }
@@ -213,7 +227,7 @@ int build_segment_filter(const pb200h_segment& seg, const pb200h_query& q, Segme
       d.ids = out.id_store.back()->data();
       d.num_ids = (int)out.id_store.back()->size();
     };
-    const char* pname = n.type == PB200H_RANGE ? "RANGE" : n.type == PB200H_EQ ? "EQ" : n.type == PB200H_NEQ ? "NOT_EQ" : n.type == PB200H_IN ? "IN" : "NOT_IN";
+    const char* pname = n.type == PB200H_RANGE ? "RANGE" : n.type == PB200H_EQ ? "EQ" : n.type == PB200H_NEQ ? "NOT_EQ" : n.type == PB200H_IN ? "IN" : n.type == PB200H_NOT_IN ? "NOT_IN" : "REGEXP_LIKE";
     if (c.is_sorted) {  // FilterOperatorUtils :98-101,117-120
       store(sorted_doc_ranges(c, e, seg.num_docs));
       d.op = PB200_F_DOC_RANGES;
@@ -320,6 +334,7 @@ int leaf_to_device(const pb200h_segment& seg, int column, const pb200h_filter_no
     if (!raw_leaf(c, n, lits, d)) { set_error("this predicate on raw column '%s' is not accelerated", c.name.c_str()); return PB200_E_UNSUPPORTED; }
     return PB200_OK;
   }
+  if (int rc = check_resolved(c, n, lits)) return rc;
   Evaluated e = evaluate(c, n, lits);
   d.column = column;
   if (e.always_false) { d.op = PB200_F_EMPTY; return PB200_OK; }
@@ -706,9 +721,11 @@ extern "C" int32_t pb200h_segment_load_dir(pb200_ctx* ctx, const char* path, pb2
 // ------------------------------------------------------------------------------------------------------------------
 extern "C" int32_t pb200h_explain(pb200_ctx* ctx, const pb200h_query* q, pb200h_segment* seg, char* out, int32_t cap) {
   if (!q || !seg || !out || cap <= 0) { set_error("null argument"); return PB200_E_INVALID; }
+  PatternScope patterns;
   if (ctx) {
     pb200h_segment* one = seg;
     if (int rc = derive_query_names(ctx, *q, &one, 1, nullptr, 0)) return rc;
+    if (int rc = resolve_patterns(ctx, *q, &one, 1, patterns)) return rc;
   }
   SegmentFilter f;
   std::string text;
@@ -749,6 +766,8 @@ extern "C" int32_t pb200h_execute_having(pb200_ctx* ctx, const pb200h_query* q, 
     return hrc;
   if (q->num_group_by == 0) order = nullptr;  // aggregation only: one row, nothing to order
   if (int rc = derive_query_names(ctx, *q, segs, nseg, nullptr, 0)) return rc;  // expressions become derived columns once
+  PatternScope patterns;
+  if (int rc = resolve_patterns(ctx, *q, segs, nseg, patterns)) return rc;      // pattern leaves become dictId sets once
   bool any_clause = false;   // some aggregation has a FILTER (WHERE ...) clause
   if (q->agg_filter_count && q->agg_filter_start && q->agg_filter_nodes)
     for (int a = 0; a < q->num_aggs; a++) any_clause |= q->agg_filter_count[a] > 0;
@@ -901,6 +920,8 @@ int32_t execute_rows(pb200_ctx* ctx, const pb200h_query* q, const pb200h_selecti
     fq.num_group_by = 0; fq.num_aggs = 0; fq.agg_filter_count = nullptr;
     if (int rc = derive_query_names(ctx, fq, segs, nseg, extra.data(), (int)extra.size())) return rc;
   }
+  PatternScope patterns;
+  if (int rc = resolve_patterns(ctx, *q, segs, nseg, patterns)) return rc;
   const pb200h_segment& s0 = *segs[0];
   std::vector<int32_t> cols(sel->num_columns);
   for (int k = 0; k < sel->num_columns; k++) {

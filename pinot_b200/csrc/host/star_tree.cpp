@@ -537,6 +537,8 @@ int try_star_tree(pb200_ctx* ctx, const pb200h_segment& seg, const StarTreeIndex
     const int d = star_dim_of(seg.column_index(n.column));
     if (!((remaining >> d) & 1)) continue;
     pb200_filter_node dn;
+    if (n.type == PB200H_REGEXP_LIKE)   // the star docs' dimension shares the base column's dictionary, so its ids
+      pattern_alias(seg.cols[seg.column_index(n.column)], st.star_segment->cols[d], q.literals[n.values_offset].s);
     int rc = leaf_to_device(*st.star_segment, d, n, q.literals, store, dn);
     if (rc) return rc;
     nodes.push_back(dn);

@@ -50,9 +50,24 @@ struct MomentDict {
   ~MomentDict();                   // pb200_moments.cu
 };
 
+// Compact device copy of a STRING dictionary for REGEXP_LIKE (pb200_pattern.cu): the entries of the segment's OWN
+// dictionary (also once the column is bound to a domain) without their zero padding, `entries + 1` u32 offsets followed by
+// the bytes, in one allocation.  Built on the first pattern query, under `mu`, and published with `ready` (release).
+struct StringDict {
+  std::mutex mu;
+  std::atomic<bool> ready{false};
+  pb200_ctx* ctx = nullptr;
+  void* block = nullptr;
+  const uint32_t* offsets = nullptr;
+  const unsigned char* bytes = nullptr;
+  uint32_t entries = 0;
+  ~StringDict();                   // pb200_pattern.cu
+};
+
 struct DeviceColumn {
   int fwd_kind = 0, stored_type = 0, bits = 0, cardinality = 0;
   std::shared_ptr<MomentDict> moments = std::make_shared<MomentDict>();  // replaced by the domain's when bound
+  std::shared_ptr<StringDict> strings = std::make_shared<StringDict>();  // STRING columns; stays the segment's when bound
   uint32_t* fwd = nullptr;        // packed words, padded to whole max tiles (+ slack)
   uint64_t fwd_file_bytes = 0;    // length of the original index file: ceil(N*bits/8)
   uint64_t fwd_alloc_bytes = 0;

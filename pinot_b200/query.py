@@ -24,10 +24,10 @@ Literal = Union[int, float, str]
 
 @dataclass
 class Predicate:
-    """Leaf of the filter tree: ``Predicate.Type`` EQ / NOT_EQ / IN / NOT_IN / RANGE on an identifier."""
-    type: str  # "EQ" | "NEQ" | "IN" | "NOT_IN" | "RANGE"
+    """Leaf of the filter tree: ``Predicate.Type`` EQ / NOT_EQ / IN / NOT_IN / RANGE / REGEXP_LIKE on an identifier."""
+    type: str  # "EQ" | "NEQ" | "IN" | "NOT_IN" | "RANGE" | "REGEXP_LIKE"
     column: str
-    values: List[Literal] = field(default_factory=list)  # EQ/NEQ: [v]; IN/NOT_IN: [v...]
+    values: List[Literal] = field(default_factory=list)  # EQ/NEQ: [v]; IN/NOT_IN: [v...]; REGEXP_LIKE: [pattern]
     lower: Optional[Literal] = None  # RANGE; None = unbounded ("*")
     upper: Optional[Literal] = None
     lower_inclusive: bool = True

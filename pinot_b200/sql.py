@@ -15,7 +15,9 @@ stays Java).  This module exists so the parity tests read like the reference's
     distinct (parse_distinct): SELECT DISTINCT col[, col...] FROM table [WHERE cond] [ORDER BY col [ASC|DESC], ...] [LIMIT n]
                   (every ORDER BY column must be a DISTINCT column)
     cond  := cond AND cond | cond OR cond | NOT cond | (cond) | col op literal | col BETWEEN a AND b
-             | col [NOT] IN (literal, ...)
+             | col [NOT] IN (literal, ...) | col [NOT] LIKE 'pattern' | REGEXP_LIKE(col, 'regex')
+             (LIKE is rewritten into REGEXP_LIKE by like_to_regexp; both only on STRING dictionary columns, never in
+             HAVING)
     op    := = | != | <> | < | <= | > | >=
     hcond := cond whose left-hand sides are aggregation calls (COUNT(*), FN(col), PERCENTILE(col, p), ...) and whose
              literals are numbers.  An aggregation named only in HAVING is computed as a hidden one (Aggregation.hidden):
@@ -96,6 +98,27 @@ def having_name(agg: Aggregation) -> str:
 
 
 MAX_HAVING_NODES = 32
+
+_REGEX_META = set("\\.^$|?*+()[]{}")
+
+
+def like_to_regexp(like: str) -> str:
+    """The REGEXP_LIKE pattern of `col LIKE like` (Pinot's RegexpPatternConverterUtils.likeToRegexpLike): a leading run
+    of % drops the ^ anchor and a trailing run the $ anchor, % becomes .* and _ becomes ., every regex metacharacter is
+    escaped; a pattern of only % is '' (every value) and '' is ^$.  A backslash is refused: Pinot's LIKE escapes are not
+    restated here."""
+    if "\\" in like:
+        raise SqlError(f"LIKE pattern {like!r} contains a backslash: LIKE escapes are not supported")
+    if like == "":
+        return "^$"
+    if set(like) == {"%"}:
+        return ""
+    lead = len(like) - len(like.lstrip("%"))
+    trail = len(like) - len(like.rstrip("%"))
+    body = "".join(".*" if ch == "%" else "." if ch == "_" else "\\" + ch if ch in _REGEX_META else ch
+                   for ch in like[lead:len(like) - trail])
+    return ("" if lead else "^") + body + ("" if trail else "$")
+
 
 
 class _Parser:
@@ -289,7 +312,26 @@ class _Parser:
             self.i = start
         return self.comparison()
 
+    def pattern(self) -> str:
+        k, v = self.peek()
+        if k != "str":
+            raise SqlError(f"expected a string pattern, got {self.peek()}")
+        self.i += 1
+        return v
+
     def comparison(self) -> FilterNode:
+        k, v = self.peek()
+        if k == "id" and v.upper() == "REGEXP_LIKE" and self.toks[self.i + 1:self.i + 2] == [("op", "(")]:
+            if self.having is not None:
+                raise SqlError("REGEXP_LIKE in HAVING: HAVING filters aggregations, move the condition to WHERE")
+            self.i += 2
+            col = self.column()
+            self.expect_op(",")
+            pat = self.pattern()
+            if self.peek() == ("op", ","):
+                raise SqlError("REGEXP_LIKE with match flags is not supported")
+            self.expect_op(")")
+            return Predicate("REGEXP_LIKE", col, [pat])
         col = self.having_operand() if self.having is not None else self.column()
         if self.take_kw("BETWEEN"):
             lo = self.literal()
@@ -297,6 +339,11 @@ class _Parser:
             hi = self.literal()
             return Predicate("RANGE", col, [], lo, hi, True, True)
         negate = self.take_kw("NOT")
+        if self.take_kw("LIKE"):
+            if self.having is not None:
+                raise SqlError("LIKE in HAVING: HAVING compares aggregations with numbers")
+            leaf = Predicate("REGEXP_LIKE", col, [like_to_regexp(self.pattern())])
+            return Filter("NOT", [leaf]) if negate else leaf
         if self.take_kw("IN"):
             self.expect_op("(")
             vals = [self.literal()]
@@ -305,7 +352,7 @@ class _Parser:
             self.expect_op(")")
             return Predicate("NOT_IN" if negate else "IN", col, vals)
         if negate:
-            raise SqlError("NOT must be followed by IN here")
+            raise SqlError("NOT must be followed by IN or LIKE here")
         k, op = self.peek()
         if k != "op":
             raise SqlError(f"expected comparison operator, got {self.peek()}")
