@@ -38,7 +38,8 @@ extern "C" {
                               3: pb200_comm_*, pb200_result_columns, doc masks, pb200h_query.agg_filter_* (the host query struct grew);
                                  pb200_order_by / pb200_execute_ordered / pb200h_execute_ordered were added later without a
                                  version change: they are new symbols and structs, no existing one changed; so were
-                                 pb200_having / pb200_execute_having / pb200h_execute_having */
+                                 pb200_having / pb200_execute_having / pb200h_execute_having, and pb200_agg_arg /
+                                 pb200_execute_agg_args / pb200h_execute_agg_args */
 
 enum {
   PB200_OK = 0,
@@ -199,11 +200,12 @@ typedef struct {
 #define PB200_NODE_IDS_ON_DEVICE 1
 
 /* Aggregation functions accelerated on this path (core/query/aggregation/function/{Count,Sum,Min,Max,Avg,
- * DistinctCount,Percentile,Variance}AggregationFunction.java).  PERCENTILE takes its percentile through
- * pb200_execute_args; the four VarianceAggregationFunction types take no argument (see pb200_result_moments). */
+ * DistinctCount,Percentile,Variance,FirstWithTime,LastWithTime}AggregationFunction.java).  PERCENTILE takes its
+ * percentile through pb200_execute_args; the four VarianceAggregationFunction types take no argument (see
+ * pb200_result_moments); FIRSTWITHTIME / LASTWITHTIME take their time column through pb200_execute_agg_args. */
 enum { PB200_AGG_COUNT = 0, PB200_AGG_SUM = 1, PB200_AGG_MIN = 2, PB200_AGG_MAX = 3, PB200_AGG_AVG = 4,
        PB200_AGG_DISTINCTCOUNT = 5, PB200_AGG_PERCENTILE = 6, PB200_AGG_VARPOP = 7, PB200_AGG_VARSAMP = 8,
-       PB200_AGG_STDDEVPOP = 9, PB200_AGG_STDDEVSAMP = 10 };
+       PB200_AGG_STDDEVPOP = 9, PB200_AGG_STDDEVSAMP = 10, PB200_AGG_FIRSTWITHTIME = 11, PB200_AGG_LASTWITHTIME = 12 };
 
 typedef struct {
   int32_t function; /* PB200_AGG_* */
@@ -320,6 +322,37 @@ typedef struct {
 int32_t pb200_execute_having(pb200_ctx* ctx, const pb200_query* query, const pb200_order_by* order, const double* agg_args,
                              const pb200_having* having, pb200_segment* const* segments, int32_t num_segments,
                              pb200_result** results);
+
+/* ---- FIRSTWITHTIME / LASTWITHTIME(v, t, 'T'): the value of v in the first / last matched row by time ---------------- */
+/* One argument per aggregation that may name a second column.  p: the percentile of a PERCENTILE (as agg_args of
+ * pb200_execute_args).  time_column, value_type: the time column t (column id) and the type literal 'T' (PB200_INT ...
+ * PB200_STRING; BOOLEAN names PB200_INT) of a FIRSTWITHTIME / LASTWITHTIME, whose pb200_agg.column is the data column v.
+ * The other functions ignore the fields. */
+typedef struct {
+  double p;
+  int32_t time_column;
+  int32_t value_type;
+} pb200_agg_arg;
+/* pb200_execute_having with a pb200_agg_arg per aggregation (args == NULL: PERCENTILE and the *WITHTIME functions are
+ * PB200_E_INVALID; pb200_execute, pb200_execute_ordered, pb200_execute_args and pb200_execute_having refuse the
+ * *WITHTIME functions the same way).
+ * Semantics (DESIGN.md section 3.13): LASTWITHTIME is the value of v in the matched row of the group with the largest t,
+ * FIRSTWITHTIME with the smallest t.  Ties on t: LAST takes the tied row that comes last in the call's row order, FIRST
+ * the one that comes first; that order is segments in submission order, then doc id.  t must be an INT or LONG column
+ * with dictIds (a stored dictionary, a raw column whose dictionary was synthesised at load, a derived column): a
+ * dictionary is sorted, so dictId order is time order.  v must be an INT, LONG, FLOAT, DOUBLE or STRING column with
+ * dictIds, and value_type its stored type (the library never casts).
+ * Results: pb200_result_agg gives the value of v as a double (STRING: its dictId, as for MIN / MAX; -inf when the group
+ * has no matched row) and the winning row's time value, exact, in the long column; pb200_result_agg_dict_ids the dictId
+ * of v (-1 when empty), so that STRING values and LONG values beyond 2^53 are looked up exactly.  ORDER BY and HAVING
+ * compare the double.
+ * PB200_E_UNSUPPORTED (the caller runs the stock operator): a time column that is not INT / LONG or has no dictIds, a
+ * data column without dictIds (raw 32-bit values), a value_type that is not the data column's stored type, a call over
+ * 2^32 docs or more, PB200_Q_DEFER_FINALIZE or reduce_world > 1, ORDER BY or HAVING on a STRING-typed *WITHTIME; a
+ * PB200_Q_MERGE_SEGMENTS submission needs the same dictionary for v and for t in every segment. */
+int32_t pb200_execute_agg_args(pb200_ctx* ctx, const pb200_query* query, const pb200_order_by* order, const pb200_agg_arg* args,
+                               const pb200_having* having, pb200_segment* const* segments, int32_t num_segments,
+                               pb200_result** results);
 /* The histogram behind PERCENTILE aggregation `agg` in row `row`: its non-zero bins ascending by dictId (counts > 0), the
  * intermediate for merging per-segment results by value (the analogue of pb200_result_distinct).  Returns the number of
  * bins (or < 0 on error) and writes at most `capacity` of them; either output may be NULL.  The histograms are copied from

@@ -224,6 +224,20 @@ int32_t pb200h_execute_args(pb200_ctx* ctx, const pb200h_query* query, const pb2
 int32_t pb200h_execute_having(pb200_ctx* ctx, const pb200h_query* query, const pb200_order_by* order, const double* agg_args,
                               const pb200_having* having, pb200h_segment* const* segments, int32_t num_segments,
                               pb200_result** results, int32_t* operator_kinds);
+/* One argument per aggregation (pb200_agg_arg of include/pinot_b200.h, the time column by name): p is the percentile of a
+ * PERCENTILE; time_column (a column or an expression such as "datetrunc('HOUR',ts)", derived like any other name) and
+ * value_type (PB200_INT ... PB200_STRING) belong to a FIRSTWITHTIME / LASTWITHTIME over pb200h_agg.column. */
+typedef struct {
+  double p;
+  const char* time_column;
+  int32_t value_type;
+} pb200h_agg_arg;
+/* pb200h_execute_having with a pb200h_agg_arg per aggregation (pb200_execute_agg_args).  args == NULL is
+ * pb200h_execute_having without percentiles; the other entry points refuse FIRST/LASTWITHTIME with PB200_E_INVALID.
+ * FIRST/LASTWITHTIME in a query with any FILTER (WHERE ...) clause is PB200_E_UNSUPPORTED. */
+int32_t pb200h_execute_agg_args(pb200_ctx* ctx, const pb200h_query* query, const pb200_order_by* order, const pb200h_agg_arg* args,
+                                const pb200_having* having, pb200h_segment* const* segments, int32_t num_segments,
+                                pb200_result** results, int32_t* operator_kinds);
 /* ---- selection (SELECT columns WHERE ... LIMIT n; pb200_execute_selection of include/pinot_b200.h) --------------- */
 typedef struct {
   const char* column;

@@ -17,7 +17,8 @@ E_INVALID, E_UNSUPPORTED, E_CUDA, E_NOMEM, E_LIMIT = -1, -2, -3, -4, -5
 INT, LONG, FLOAT, DOUBLE, STRING = 0, 1, 2, 3, 4
 FWD_DICT_FIXEDBIT, FWD_DICT_SORTED, FWD_RAW_FIXEDBYTE = 0, 1, 2
 AGG_CODES = {"COUNT": 0, "SUM": 1, "MIN": 2, "MAX": 3, "AVG": 4, "DISTINCTCOUNT": 5, "PERCENTILE": 6,
-             "VARPOP": 7, "VARSAMP": 8, "STDDEVPOP": 9, "STDDEVSAMP": 10}
+             "VARPOP": 7, "VARSAMP": 8, "STDDEVPOP": 9, "STDDEVSAMP": 10, "FIRSTWITHTIME": 11, "LASTWITHTIME": 12}
+WITHTIME_FUNCTIONS = ("FIRSTWITHTIME", "LASTWITHTIME")
 MOMENT_FUNCTIONS = ("VARPOP", "VARSAMP", "STDDEVPOP", "STDDEVSAMP")
 FILTER_CODES = {"AND": 0, "OR": 1, "NOT": 2, "EQ": 3, "NEQ": 4, "IN": 5, "NOT_IN": 6, "RANGE": 7, "REGEXP_LIKE": 8}
 REGIMES = {0: "NONE", 1: "ARRAY", 2: "INT_MAP", 3: "LONG_MAP", 4: "ARRAY_MAP"}
@@ -97,6 +98,14 @@ class HFilterNode(C.Structure):
 
 class HAgg(C.Structure):
     _fields_ = [("function", C.c_int32), ("column", C.c_char_p)]
+
+
+class AggArg(C.Structure):  # pb200_agg_arg
+    _fields_ = [("p", C.c_double), ("time_column", C.c_int32), ("value_type", C.c_int32)]
+
+
+class HAggArg(C.Structure):  # pb200h_agg_arg
+    _fields_ = [("p", C.c_double), ("time_column", C.c_char_p), ("value_type", C.c_int32)]
 
 
 class HQuery(C.Structure):
@@ -200,7 +209,7 @@ EXPORTED_SYMBOLS = [
     "pb200_execute_args", "pb200h_execute_args", "pb200_result_histogram", "pb200_result_moments",
     "pb200_segment_derive_column", "pb200h_segment_derive",
     "pb200h_startree_build", "pb200h_startree_get",
-    "pb200_execute_having", "pb200h_execute_having",
+    "pb200_execute_having", "pb200h_execute_having", "pb200_execute_agg_args", "pb200h_execute_agg_args",
     "pb200_match_pattern",
 ]
 
@@ -231,6 +240,8 @@ def load() -> C.CDLL:
                                      C.POINTER(vp)]
     L.pb200_execute_having.argtypes = [vp, C.POINTER(Query), C.POINTER(OrderBy), C.POINTER(C.c_double), C.POINTER(Having),
                                        C.POINTER(vp), i32, C.POINTER(vp)]
+    L.pb200_execute_agg_args.argtypes = [vp, C.POINTER(Query), C.POINTER(OrderBy), C.POINTER(AggArg), C.POINTER(Having),
+                                         C.POINTER(vp), i32, C.POINTER(vp)]
     L.pb200_result_histogram.restype = i64
     L.pb200_result_histogram.argtypes = [vp, i32, i32, vp, vp, i64]
     L.pb200_result_moments.argtypes = [vp, i32, i32, vp, vp, vp, vp, vp, vp, vp]
@@ -268,6 +279,8 @@ def load() -> C.CDLL:
                                       C.POINTER(vp), C.POINTER(i32)]
     L.pb200h_execute_having.argtypes = [vp, C.POINTER(HQuery), C.POINTER(OrderBy), C.POINTER(C.c_double), C.POINTER(Having),
                                         C.POINTER(vp), i32, C.POINTER(vp), C.POINTER(i32)]
+    L.pb200h_execute_agg_args.argtypes = [vp, C.POINTER(HQuery), C.POINTER(OrderBy), C.POINTER(HAggArg), C.POINTER(Having),
+                                          C.POINTER(vp), i32, C.POINTER(vp), C.POINTER(i32)]
     L.pb200h_explain.argtypes = [vp, C.POINTER(HQuery), vp, C.c_char_p, i32]
     L.pb200h_startree_attach.argtypes = [vp, vp, vp, C.c_uint64, i32, i32, C.POINTER(C.c_char_p), C.POINTER(vp),
                                          C.POINTER(C.c_uint64), i32, C.POINTER(HStarMetric)]

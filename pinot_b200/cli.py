@@ -24,11 +24,13 @@ def merge_blocks(query, segments, blocks) -> Dict[tuple, list]:
     """{key values: [intermediate per aggregation]} over all blocks: COUNT -> int, SUM / MIN / MAX -> float,
     AVG -> (sum, count), DISTINCTCOUNT -> set of values, PERCENTILE -> (p, {value: count}) from the per-segment
     histograms, or its final float for a block merged on the device, VAR / STDDEV -> exact (n, sum v, sum v^2) from the
-    blocks' moments, each shifted from its own grid (c, e) to values, or the final float of a block merged on the device
+    blocks' moments, each shifted from its own grid (c, e) to values, or the final float of a block merged on the device,
+    FIRST/LASTWITHTIME -> (time value, data value) of the winning row or None for an empty block (query.withtime_pick: ties
+    go to the later segment for LAST, to the earlier one for FIRST)
     (GroupByCombineOperator / AggregationFunction.merge).  Float keys, set members and histogram values are compared by
     identity (query.ValueKey: one NaN, -0.0 apart from 0.0) and MIN / MAX merge in Double.compare order, as the reference's
     Double.equals / doubleToLongBits keyed tables and its dictionary order do."""
-    from .query import MOMENT_FUNCTIONS, merge_moments, value_key, value_order
+    from .query import MOMENT_FUNCTIONS, WITHTIME_FUNCTIONS, merge_moments, value_key, value_order, withtime_pick
     out: Dict[tuple, list] = {}
     for seg, b in zip(segments, blocks):
         rows = 1 if b.num_groups < 0 else b.num_groups
@@ -52,6 +54,8 @@ def merge_blocks(query, segments, blocks) -> Dict[tuple, list]:
                     vals.append((agg.arg, hist))
                 elif fn in MOMENT_FUNCTIONS and (a, g) in b.moments:
                     vals.append(merge_moments([b.moments[(a, g)]]))
+                elif fn in WITHTIME_FUNCTIONS:
+                    vals.append(b.withtime(a, g, seg, agg.column))
                 else:
                     vals.append(float(b.doubles[a][g]))
             cur = out.get(key)
@@ -73,6 +77,8 @@ def merge_blocks(query, segments, blocks) -> Dict[tuple, list]:
                         cur[a][1][v] = cur[a][1].get(v, 0) + c
                 elif fn in MOMENT_FUNCTIONS and isinstance(cur[a], tuple):
                     cur[a] = tuple(x + y for x, y in zip(cur[a], vals[a]))
+                elif fn in WITHTIME_FUNCTIONS:
+                    cur[a] = withtime_pick(fn, cur[a], vals[a])
                 else:
                     cur[a] |= vals[a]
     return out
@@ -101,9 +107,13 @@ def final_rows(query, table: Dict[tuple, list]) -> List[list]:
                 vals.append(percentile_of_counts(v))
             elif agg.function in MOMENT_FUNCTIONS and isinstance(v, tuple):
                 vals.append(moments_final(agg.function, v))
+            elif agg.function in ("FIRSTWITHTIME", "LASTWITHTIME"):
+                vals.append(float("-inf") if v is None else v[1])
             else:
                 vals.append(v)
-        if having and not having_eval(having, [float(x) for x in vals]):
+        # HAVING compares numbers; a STRING FIRST/LASTWITHTIME value is never one of its operands (sql.resolve_having
+        # refuses that), so it stands in as -inf, the value the device compares for it when empty
+        if having and not having_eval(having, [float("-inf") if isinstance(x, (bytes, str)) else float(x) for x in vals]):
             continue
         rows.append(list(key) + vals)
     k = len(query.group_by)
@@ -151,7 +161,9 @@ def main(argv=None) -> int:
             if args.merge_on_device and len(segments) > 1:
                 cols = list(dict.fromkeys(list(query.group_by) + [a.column for a in query.aggregations
                                                                   if a.column and a.function in ("MIN", "MAX", "DISTINCTCOUNT", "PERCENTILE",
-                                                                                 "VARPOP", "VARSAMP", "STDDEVPOP", "STDDEVSAMP")]))
+                                                                                 "VARPOP", "VARSAMP", "STDDEVPOP", "STDDEVSAMP",
+                                                                                 "FIRSTWITHTIME", "LASTWITHTIME")]
+                                           + [a.time_column for a in query.aggregations if a.time_column and "(" not in a.time_column]))
                 if cols:
                     domain = DictionaryDomain.build(ctx, segments, cols)
                     for s in segments:

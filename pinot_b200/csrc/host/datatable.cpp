@@ -85,6 +85,12 @@ extern "C" int64_t pb200h_result_to_datatable(const pb200h_query* q, const pb200
       return PB200_E_UNSUPPORTED;
     }
   for (int a = 0; a < nagg; a++)
+    if (q->aggs[a].function == PB200_AGG_FIRSTWITHTIME || q->aggs[a].function == PB200_AGG_LASTWITHTIME) {
+      // the reference's intermediate is a (value, time) pair object
+      set_error("FIRST/LASTWITHTIME intermediates are not written as DataTable objects");
+      return PB200_E_UNSUPPORTED;
+    }
+  for (int a = 0; a < nagg; a++)
     if (pb200::is_moments_fn(q->aggs[a].function)) {   // the reference's intermediate is a VarianceTuple
       set_error("VAR/STDDEV intermediates are not written as DataTable objects");
       return PB200_E_UNSUPPORTED;

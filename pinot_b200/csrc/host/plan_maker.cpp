@@ -293,6 +293,7 @@ pb200_result* host_result(const pb200h_segment& seg, const pb200h_query& q, bool
       case PB200_AGG_MIN: if (empty) d = INFINITY; else { id = c->to_device_id(0); d = c->as_double(0); } break;
       case PB200_AGG_MAX: if (empty) d = -INFINITY; else { id = c->to_device_id(c->cardinality - 1); d = c->as_double(c->cardinality - 1); } break;
       case PB200_AGG_PERCENTILE: d = -INFINITY; break;   // only reached for an empty match (never answered without a scan)
+      case PB200_AGG_FIRSTWITHTIME: case PB200_AGG_LASTWITHTIME: d = -INFINITY; break;   // likewise: no row, dictId -1
       case PB200_AGG_VARPOP: case PB200_AGG_VARSAMP: case PB200_AGG_STDDEVPOP: case PB200_AGG_STDDEVSAMP:
         d = -INFINITY; R->mom.on[a] = true; break;       // likewise: n = 0, zero moments
       case PB200_AGG_DISTINCTCOUNT: {
@@ -758,6 +759,16 @@ extern "C" int32_t pb200h_execute_args(pb200_ctx* ctx, const pb200h_query* q, co
 extern "C" int32_t pb200h_execute_having(pb200_ctx* ctx, const pb200h_query* q, const pb200_order_by* order, const double* agg_args,
                                          const pb200_having* having, pb200h_segment* const* segs, int32_t nseg,
                                          pb200_result** results, int32_t* kinds) {
+  if (!q || q->num_aggs < 0 || q->num_aggs > pb200::kMaxAggs || !agg_args)
+    return pb200h_execute_agg_args(ctx, q, order, nullptr, having, segs, nseg, results, kinds);
+  std::vector<pb200h_agg_arg> args(q->num_aggs);
+  for (int a = 0; a < q->num_aggs; a++) args[a] = pb200h_agg_arg{agg_args[a], nullptr, 0};
+  return pb200h_execute_agg_args(ctx, q, order, args.data(), having, segs, nseg, results, kinds);
+}
+
+extern "C" int32_t pb200h_execute_agg_args(pb200_ctx* ctx, const pb200h_query* q, const pb200_order_by* order, const pb200h_agg_arg* args,
+                                           const pb200_having* having, pb200h_segment* const* segs, int32_t nseg,
+                                           pb200_result** results, int32_t* kinds) {
   if (!ctx || !q || !segs || !results || nseg <= 0) { set_error("invalid argument to pb200h_execute"); return PB200_E_INVALID; }
   if (q->num_aggs <= 0) { set_error("selection queries are outside this path"); return PB200_E_UNSUPPORTED; }
   if (int vrc = pb200::order_validate(order, q->num_aggs, q->num_group_by)) return vrc;
@@ -765,17 +776,31 @@ extern "C" int32_t pb200h_execute_having(pb200_ctx* ctx, const pb200h_query* q, 
                                     q->merge_segments == 2 || q->reduce_world > 1))
     return hrc;
   if (q->num_group_by == 0) order = nullptr;  // aggregation only: one row, nothing to order
-  if (int rc = derive_query_names(ctx, *q, segs, nseg, nullptr, 0)) return rc;  // expressions become derived columns once
+  std::vector<const char*> time_names;   // FIRST/LASTWITHTIME time columns: derived like every other name of the query
+  for (int a = 0; a < q->num_aggs; a++) {
+    const int fn = q->aggs[a].function;
+    if (fn != PB200_AGG_FIRSTWITHTIME && fn != PB200_AGG_LASTWITHTIME) continue;
+    if (!args || !args[a].time_column) { set_error("FIRST/LASTWITHTIME (aggregation %d) needs its time column: call pb200h_execute_agg_args", a); return PB200_E_INVALID; }
+    time_names.push_back(args[a].time_column);
+  }
+  if (int rc = derive_query_names(ctx, *q, segs, nseg, time_names.data(), (int)time_names.size())) return rc;  // expressions become derived columns once
   PatternScope patterns;
   if (int rc = resolve_patterns(ctx, *q, segs, nseg, patterns)) return rc;      // pattern leaves become dictId sets once
   bool any_clause = false;   // some aggregation has a FILTER (WHERE ...) clause
   if (q->agg_filter_count && q->agg_filter_start && q->agg_filter_nodes)
     for (int a = 0; a < q->num_aggs; a++) any_clause |= q->agg_filter_count[a] > 0;
   for (int a = 0; a < q->num_aggs; a++) {
+    const int fn = q->aggs[a].function;
+    if ((fn == PB200_AGG_FIRSTWITHTIME || fn == PB200_AGG_LASTWITHTIME) && any_clause) {   // the per-clause submissions carry no time columns
+      set_error("FIRST/LASTWITHTIME in a query with FILTER (WHERE ...) clauses is not accelerated");
+      return PB200_E_UNSUPPORTED;
+    }
+  }
+  for (int a = 0; a < q->num_aggs; a++) {
     if (q->aggs[a].function != PB200_AGG_PERCENTILE) continue;
     // the same checks as the device path, made before any segment can be answered on the host
-    if (!agg_args) { set_error("PERCENTILE (aggregation %d) needs its percentile: call pb200h_execute_args", a); return PB200_E_INVALID; }
-    if (!(agg_args[a] >= 0.0 && agg_args[a] <= 100.0)) { set_error("PERCENTILE (aggregation %d): percentile %g outside [0, 100]", a, agg_args[a]); return PB200_E_INVALID; }
+    if (!args) { set_error("PERCENTILE (aggregation %d) needs its percentile: call pb200h_execute_args", a); return PB200_E_INVALID; }
+    if (!(args[a].p >= 0.0 && args[a].p <= 100.0)) { set_error("PERCENTILE (aggregation %d): percentile %g outside [0, 100]", a, args[a].p); return PB200_E_INVALID; }
     // FILTER clauses run as one submission per clause (host/filtered_agg.cpp), which carries no percentiles: a PERCENTILE
     // anywhere in such a query -- with its own clause or next to another function's -- goes to the stock operator
     if (any_clause) {
@@ -801,6 +826,7 @@ extern "C" int32_t pb200h_execute_having(pb200_ctx* ctx, const pb200h_query* q, 
     if (!s0.cols[gb[g]].has_dictionary) { set_error("group-by on raw column '%s' is not accelerated", q->group_by[g]); return PB200_E_UNSUPPORTED; }
   }
   std::vector<pb200_agg> aggs(q->num_aggs);
+  std::vector<pb200_agg_arg> dev_args(q->num_aggs, pb200_agg_arg{0.0, -1, 0});
   for (int a = 0; a < q->num_aggs; a++) {
     aggs[a].function = q->aggs[a].function;
     aggs[a].column = -1;
@@ -808,7 +834,14 @@ extern "C" int32_t pb200h_execute_having(pb200_ctx* ctx, const pb200h_query* q, 
       aggs[a].column = s0.column_index(q->aggs[a].column);
       if (aggs[a].column < 0) { set_error("unknown aggregation column '%s'", q->aggs[a].column ? q->aggs[a].column : "(null)"); return PB200_E_INVALID; }
       const HostColumn& c = s0.cols[aggs[a].column];
-      if (c.data_type == PB200_STRING && q->aggs[a].function != PB200_AGG_DISTINCTCOUNT) { set_error("%s over STRING column", "aggregation"); return PB200_E_UNSUPPORTED; }
+      const bool wt = q->aggs[a].function == PB200_AGG_FIRSTWITHTIME || q->aggs[a].function == PB200_AGG_LASTWITHTIME;
+      if (c.data_type == PB200_STRING && q->aggs[a].function != PB200_AGG_DISTINCTCOUNT && !wt) { set_error("%s over STRING column", "aggregation"); return PB200_E_UNSUPPORTED; }
+      if (args) dev_args[a].p = args[a].p;
+      if (wt) {
+        dev_args[a].time_column = s0.column_index(args[a].time_column);
+        if (dev_args[a].time_column < 0) { set_error("unknown time column '%s'", args[a].time_column); return PB200_E_INVALID; }
+        dev_args[a].value_type = args[a].value_type;
+      }
       if (pb200::is_moments_fn(q->aggs[a].function) && !c.has_dictionary) {
         set_error("VAR/STDDEV over raw column '%s' is not accelerated", q->aggs[a].column);
         return PB200_E_UNSUPPORTED;
@@ -828,6 +861,7 @@ extern "C" int32_t pb200h_execute_having(pb200_ctx* ctx, const pb200h_query* q, 
     };
     for (int g = 0; g < q->num_group_by; g++) if (!same_column(gb[g])) { set_error("segment %d: column '%s' is not at the position it has in segment 0", s, q->group_by[g]); return PB200_E_INVALID; }
     for (int a = 0; a < q->num_aggs; a++) if (aggs[a].column >= 0 && !same_column(aggs[a].column)) { set_error("segment %d: column '%s' is not at the position it has in segment 0", s, q->aggs[a].column); return PB200_E_INVALID; }
+    for (int a = 0; a < q->num_aggs; a++) if (dev_args[a].time_column >= 0 && !same_column(dev_args[a].time_column)) { set_error("segment %d: column '%s' is not at the position it has in segment 0", s, args[a].time_column); return PB200_E_INVALID; }
     int rc = build_segment_filter(*segs[s], *q, filters[s], nullptr);
     if (rc) return rc;
     if (!merge) {
@@ -878,7 +912,7 @@ extern "C" int32_t pb200h_execute_having(pb200_ctx* ctx, const pb200h_query* q, 
     dq.filter = flat.data();
     dq.group_by_columns = gb.data();
     dq.aggs = aggs.data();
-    int rc = pb200_execute_having(ctx, &dq, order, agg_args, having, dsegs.data(), (int)dsegs.size(), dev_results.data());
+    int rc = pb200_execute_agg_args(ctx, &dq, order, args ? dev_args.data() : nullptr, having, dsegs.data(), (int)dsegs.size(), dev_results.data());
     if (rc) { for (auto r : star_results) if (r) pb200_result_free(r); return rc; }
   }
   if (merge) { results[0] = dev_results[0]; return PB200_OK; }

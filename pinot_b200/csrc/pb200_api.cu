@@ -18,6 +18,7 @@
 
 #include "pb200_internal.h"
 #include "pb200_percentile.h"
+#include "pb200_withtime.h"
 #include "pb200_plan.h"
 #include "pb200_scan_launch.h"
 #include "pb200_unpack.cuh"
@@ -702,7 +703,7 @@ int launch_chunks(pb200_ctx* ctx, cudaStream_t st, const ScanPlan& plan, DevBufR
 constexpr int kRetryWithoutCountCarrier = 1;
 static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment* const* segments, int32_t nseg,
                         pb200_result** results, bool allow_count_carrier, const pb200_order_by* order, const double* agg_args,
-                        const pb200_having* having);
+                        const pb200_having* having, const pb200_agg_arg* wt_args);
 
 extern "C" int32_t pb200_execute_having(pb200_ctx* ctx, const pb200_query* query, const pb200_order_by* order, const double* agg_args,
                                         const pb200_having* having, pb200_segment* const* segments, int32_t nseg,
@@ -713,8 +714,42 @@ extern "C" int32_t pb200_execute_having(pb200_ctx* ctx, const pb200_query* query
     const bool deferred = (query->flags & PB200_Q_DEFER_FINALIZE) || query->reduce_world > 1;
     if (const int hrc = having_check(having, query->num_aggs, query->num_group_by, nres, deferred)) return hrc;
   }
-  int rc = execute_impl(ctx, query, segments, nseg, results, true, order, agg_args, having);
-  if (rc == kRetryWithoutCountCarrier) rc = execute_impl(ctx, query, segments, nseg, results, false, order, agg_args, having);
+  int rc = execute_impl(ctx, query, segments, nseg, results, true, order, agg_args, having, nullptr);
+  if (rc == kRetryWithoutCountCarrier) rc = execute_impl(ctx, query, segments, nseg, results, false, order, agg_args, having, nullptr);
+  return rc;
+}
+
+extern "C" int32_t pb200_execute_agg_args(pb200_ctx* ctx, const pb200_query* query, const pb200_order_by* order, const pb200_agg_arg* args,
+                                          const pb200_having* having, pb200_segment* const* segments, int32_t nseg,
+                                          pb200_result** results) {
+  if (!query || !args || query->num_aggs < 0 || query->num_aggs > kMaxAggs || (query->num_aggs > 0 && !query->aggs))
+    return pb200_execute_having(ctx, query, order, nullptr, having, segments, nseg, results);
+  if (const int vrc = order_validate(order, query->num_aggs, query->num_group_by)) return vrc;
+  const int nres = (query->flags & PB200_Q_MERGE_SEGMENTS) ? 1 : nseg;
+  const bool deferred = (query->flags & PB200_Q_DEFER_FINALIZE) || query->reduce_world > 1;
+  if (const int hrc = having_check(having, query->num_aggs, query->num_group_by, nres, deferred)) return hrc;
+  // ORDER BY / HAVING compare the double column: for a STRING-typed *WITHTIME that is a dictId, not a value
+  if (segments && nseg > 0 && segments[0] && query->num_group_by > 0) {
+    auto string_wt = [&](int a) {
+      const pb200_agg& ag = query->aggs[a];
+      return is_withtime_fn(ag.function) && ag.column >= 0 && ag.column < (int)segments[0]->cols.size() &&
+             segments[0]->cols[ag.column].stored_type == PB200_STRING;
+    };
+    for (int i = 0; order && i < order->num_items; i++)
+      if (order->items[i].kind == PB200_ORDER_AGG && string_wt(order->items[i].index)) {
+        set_error("ORDER BY a STRING FIRST/LASTWITHTIME is not accelerated"); return PB200_E_UNSUPPORTED;
+      }
+    for (int i = 0; having && i < having->num_nodes; i++) {
+      const pb200_having_node& hn = having->nodes[i];
+      if ((hn.op == PB200_HAVING_RANGE || hn.op == PB200_HAVING_EQ || hn.op == PB200_HAVING_NEQ) && string_wt(hn.agg)) {
+        set_error("HAVING on a STRING FIRST/LASTWITHTIME is not accelerated"); return PB200_E_UNSUPPORTED;
+      }
+    }
+  }
+  double p[kMaxAggs] = {};
+  for (int a = 0; a < query->num_aggs; a++) p[a] = args[a].p;
+  int rc = execute_impl(ctx, query, segments, nseg, results, true, order, p, having, args);
+  if (rc == kRetryWithoutCountCarrier) rc = execute_impl(ctx, query, segments, nseg, results, false, order, p, having, args);
   return rc;
 }
 
@@ -758,14 +793,21 @@ namespace {
 // device twice per query).  nres AggAccum records, then 4 words per result for the count-carrier verification {sum of
 // carried counts, largest sum field, largest carried count, unused}, then (aggregation-only PERCENTILE) per result
 // kMaxAggs selected dictIds and kMaxAggs value counts, u32 each.
+// Then (aggregation-only FIRST/LASTWITHTIME) per result kMaxAggs winning keys and kMaxAggs time values, u64 each, and
+// kMaxAggs data dictIds, u32 each.
 struct AccumLayout {
-  size_t verify_off = 0, pct_off = 0, bytes = 0;
+  size_t verify_off = 0, pct_off = 0, wt_off = 0, bytes = 0;
+  int nres = 0;
   AccumLayout() = default;
-  AccumLayout(int nres, bool pct)
-      : verify_off(sizeof(AggAccum) * nres), pct_off(verify_off + 32ull * nres), bytes(pct_off + (pct ? 8ull * kMaxAggs * nres : 0)) {}
+  AccumLayout(int nres, bool pct, bool wt)
+      : verify_off(sizeof(AggAccum) * nres), pct_off(verify_off + 32ull * nres), wt_off(pct_off + (pct ? 8ull * kMaxAggs * nres : 0)),
+        bytes(wt_off + (wt ? 20ull * kMaxAggs * nres : 0)), nres(nres) {}
   static AggAccum* records(void* b) { return static_cast<AggAccum*>(b); }
   unsigned long long* verify(void* b) const { return reinterpret_cast<unsigned long long*>(static_cast<unsigned char*>(b) + verify_off); }
   uint32_t* pct(void* b) const { return reinterpret_cast<uint32_t*>(static_cast<unsigned char*>(b) + pct_off); }
+  unsigned long long* wt_key(void* b, int r) const { return reinterpret_cast<unsigned long long*>(static_cast<unsigned char*>(b) + wt_off) + (size_t)r * kMaxAggs; }
+  long long* wt_time(void* b, int r) const { return reinterpret_cast<long long*>(wt_key(b, nres)) + (size_t)r * kMaxAggs; }
+  uint32_t* wt_ids(void* b, int r) const { return reinterpret_cast<uint32_t*>(wt_time(b, nres)) + (size_t)r * kMaxAggs; }
 };
 
 // Frees a result's group tables and PERCENTILE selections; its histograms too unless keep_hist (pb200_result_histogram).
@@ -784,6 +826,12 @@ void release_tables(pb200_result& R, bool keep_hist) {
     for (int a = 0; a < kMaxAggs; a++) {
       if (!keep_hist) { dev_free(p.ctx, p.hist[a]); p.hist[a] = nullptr; }
       dev_free(p.ctx, p.ids[a]); dev_free(p.ctx, p.n[a]); p.ids[a] = p.n[a] = nullptr;
+    }
+  pb200_result::Wt& w = R.wt;
+  if (d.ctx)
+    for (int a = 0; a < kMaxAggs; a++) {
+      dev_free(d.ctx, w.key[a]); dev_free(d.ctx, w.ids[a]); dev_free(d.ctx, w.time[a]);
+      w.key[a] = nullptr; w.ids[a] = nullptr; w.time[a] = nullptr;
     }
 }
 
@@ -826,9 +874,9 @@ struct ScanCall {
   }
 
   // 2. VAR / STDDEV limb dictionaries (pb200_moments.cu), then every decision about the launch (pb200_plan.cpp)
-  int prepare_and_plan(bool allow_count_carrier, const double* agg_args) {
+  int prepare_and_plan(bool allow_count_carrier, const double* agg_args, const pb200_agg_arg* wt_args) {
     if (int rc = moments_prepare(ctx, query, segments, nseg)) return rc;
-    return plan_scan(tune, DeviceLimits{ctx->sm_count, ctx->max_smem_optin}, query, segments, nseg, allow_count_carrier, &plan, agg_args);
+    return plan_scan(tune, DeviceLimits{ctx->sm_count, ctx->max_smem_optin}, query, segments, nseg, allow_count_carrier, &plan, agg_args, wt_args);
   }
 
   // 3. the stream, the results, and the device buffers of the filter leaves
@@ -847,7 +895,7 @@ struct ScanCall {
   int bind_accumulators() {
     bool any_pct = false;
     for (int a = 0; a < plan.q.num_aggs; a++) any_pct |= plan.pct_rep[a] >= 0;
-    acc = AccumLayout(plan.nres, any_pct && !plan.group_by);
+    acc = AccumLayout(plan.nres, any_pct && !plan.group_by, plan.any_wt && !plan.group_by);
     if (int rc = pinned_alloc(ctx, 2 * acc.bytes, &pin.p, &pin.bytes)) return rc;
     unsigned char* const init = static_cast<unsigned char*>(pin.p);
     back = init + acc.bytes;
@@ -856,6 +904,10 @@ struct ScanCall {
     for (int a = 0; a < kMaxAggs; a++) init_acc.min_id[a] = 0xFFFFFFFFu;
     memset(init, 0, acc.bytes);
     for (int r = 0; r < plan.nres; r++) AccumLayout::records(init)[r] = init_acc;
+    if (plan.any_wt && !plan.group_by)   // FIRSTWITHTIME keys start at u64 max (a u64 min reduction), LASTWITHTIME at 0
+      for (int r = 0; r < plan.nres; r++)
+        for (int a = 0; a < plan.q.num_aggs; a++)
+          if (plan.q.aggs[a].function == PB200_AGG_FIRSTWITHTIME) acc.wt_key(init, r)[a] = ~0ull;
     if (int rc = accum.alloc(acc.bytes)) return rc;
     PB200_CUDA(cudaMemcpyAsync(accum.p, init, acc.bytes, cudaMemcpyHostToDevice, st));
     for (int s = 0; s < nseg; s++) plan.segs[s].accum = AccumLayout::records(accum.p) + (plan.merge ? 0 : s);
@@ -891,6 +943,7 @@ struct ScanCall {
       for (int a = 0; a < nagg; a++) {
         if (distinct_bufs[r][a]) plan.segs[s].distinct_bits[a] = (uint32_t*)distinct_bufs[r][a]->p;
         if (res[r]->pct.hist[a]) plan.segs[s].distinct_bits[a] = res[r]->pct.hist[a];
+        if (plan.wt_time[a] >= 0) plan.segs[s].distinct_bits[a] = reinterpret_cast<uint32_t*>(acc.wt_key(accum.p, r) + a);
       }
     }
     return PB200_OK;
@@ -911,7 +964,7 @@ struct ScanCall {
       sd.h_ctl = d.hctl;
       for (int a = 0; a < plan.q.num_aggs; a++) {
         sd.g_isum[a] = d.isum[a]; sd.g_dsum[a] = d.dsum[a]; sd.g_min[a] = d.gmin[a]; sd.g_max[a] = d.gmax[a];
-        sd.distinct_bits[a] = R.pct.hist[a] ? R.pct.hist[a] : d.dbits[a];
+        sd.distinct_bits[a] = R.pct.hist[a] ? R.pct.hist[a] : R.wt.key[a] ? reinterpret_cast<uint32_t*>(R.wt.key[a]) : d.dbits[a];
       }
     }
     return PB200_OK;
@@ -979,6 +1032,11 @@ struct ScanCall {
           if ((rc = dev_alloc(ctx, (size_t)t.groups * 4, (void**)&p.n[a]))) return rc;
         }
         if ((rc = dev_alloc(ctx, (size_t)t.groups * 4, (void**)&p.ids[a]))) return rc;
+      } else if (is_withtime_fn(fn)) {  // one key per group / slot: u64 min (FIRST) starts at ~0, u64 max (LAST) at 0
+        pb200_result::Wt& w = res[r]->wt;
+        if ((rc = alloc_block((void**)&w.key[a], t.groups, 8, fn == PB200_AGG_FIRSTWITHTIME ? 0xFF : 0))) return rc;
+        if ((rc = dev_alloc(ctx, (size_t)t.groups * 4, (void**)&w.ids[a]))) return rc;
+        if ((rc = dev_alloc(ctx, (size_t)t.groups * 8, (void**)&w.time[a]))) return rc;
       }
     }
     if (d.pack_agg >= 0) d.exists_packed = (const unsigned long long*)d.isum[d.pack_agg];
@@ -1010,6 +1068,28 @@ struct ScanCall {
         }
         if (int rc = percentile_finalize(ctx, st, job, temps)) return rc;
       }
+    return PB200_OK;
+  }
+
+  // 8b. FIRST/LASTWITHTIME: winning keys -> data dictIds and time values, queued behind the scan (aggregation only: in the
+  //     accumulator block; group-by: per table entry, read by the extraction)
+  int finalize_withtime() {
+    if (!plan.any_wt) return PB200_OK;
+    for (int a = 0; a < plan.q.num_aggs; a++) {
+      if (plan.wt_time[a] < 0) continue;
+      const WtSeg* wsegs = nullptr;
+      if (int rc = withtime_segments(ctx, st, segments, nseg, query->aggs[a].column, plan.wt_time[a], plan.wt_base, temps, &wsegs)) return rc;
+      for (int r = 0; r < plan.nres; r++) {
+        WithTimeJob job;
+        if (plan.group_by) {
+          const pb200_result::Wt& w = res[r]->wt;
+          job = WithTimeJob{w.key[a], plan.tables[r].groups, w.ids[a], w.time[a]};
+        } else {
+          job = WithTimeJob{acc.wt_key(accum.p, r) + a, 1, acc.wt_ids(accum.p, r) + a, acc.wt_time(accum.p, r) + a};
+        }
+        if (int rc = withtime_finalize(ctx, st, job, wsegs, nseg)) return rc;
+      }
+    }
     return PB200_OK;
   }
 
@@ -1097,6 +1177,10 @@ struct ScanCall {
       const uint32_t x = host_pct[a];
       if (x == ~0u) v->d = -INFINITY;   // no matched row
       else { v->id = (int32_t)x; v->d = value_of(x); v->l = host_pct[kMaxAggs + plan.pct_rep[a]]; }
+    } else if (is_withtime_fn(fn)) {   // the finalize's data dictId and time value; an empty result has no row
+      const uint32_t x = acc.wt_ids(back, r)[a];
+      if (acc_r.count == 0 || x == ~0u) v->d = -INFINITY;
+      else { v->id = (int32_t)x; v->d = c->dict_host.empty() ? (double)v->id : value_of(x); v->l = acc.wt_time(back, r)[a]; }
     } else if (fn == PB200_AGG_DISTINCTCOUNT) {
       std::vector<uint32_t> bits(plan.distinct_words[r][a]);
       PB200_CUDA(cudaMemcpy(bits.data(), distinct_bufs[r][a]->p, bits.size() * 4, cudaMemcpyDeviceToHost));
@@ -1173,15 +1257,16 @@ struct ScanCall {
 
 static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment* const* segments, int32_t nseg,
                         pb200_result** results, bool allow_count_carrier, const pb200_order_by* order, const double* agg_args,
-                        const pb200_having* having) {
+                        const pb200_having* having, const pb200_agg_arg* wt_args) {
   ScanCall c{ctx, query, segments, nseg};
   if (int rc = c.check_call(results)) return rc;
-  if (int rc = c.prepare_and_plan(allow_count_carrier, agg_args)) return rc;
+  if (int rc = c.prepare_and_plan(allow_count_carrier, agg_args, wt_args)) return rc;
   if (int rc = c.alloc_results()) return rc;
   if (int rc = c.bind_accumulators()) return rc;
   if (int rc = c.plan.group_by ? c.bind_group_tables() : c.bind_agg_outputs()) return rc;
   if (int rc = c.launch()) return rc;
   if (int rc = c.finalize_percentiles()) return rc;
+  if (int rc = c.finalize_withtime()) return rc;
   if (int rc = c.read_back_and_verify()) return rc;   // kRetryWithoutCountCarrier: ~ScanCall frees this attempt's tables
   if (int rc = c.fill_results_and_extract(order, having)) return rc;
   c.hand_out(results);
@@ -1204,6 +1289,8 @@ extern "C" int32_t pb200_result_device_buffers(pb200_result* R, int32_t kind, vo
   if (d.hkeys) { set_error("hash group tables of different GPUs are not element-wise reducible"); return PB200_E_UNSUPPORTED; }
   for (int a = 0; a < kMaxAggs; a++)
     if (R->mom.on[a]) { set_error("VAR/STDDEV moments are not combined across GPUs"); return PB200_E_UNSUPPORTED; }
+  for (int a = 0; a < kMaxAggs; a++)
+    if (R->wt.key[a]) { set_error("FIRST/LASTWITHTIME results are not combined across GPUs"); return PB200_E_UNSUPPORTED; }
   for (int a = 0; a < kMaxAggs; a++)
     if (R->pct.hist[a]) {
       set_error("PERCENTILE keeps dictId histograms on the device: a cross-GPU reduce of the tables would drop the other ranks' values");

@@ -49,6 +49,17 @@ __host__ __device__ inline long long percentile_index(long long n, double p) {
   return k < n - 1 ? k : n - 1;
 }
 
+// FIRSTWITHTIME / LASTWITHTIME (DESIGN.md section 3.13) in SegDesc.agg_code: function field kFnWithTime over the TIME
+// column's slot, the value-kind field says which end wins.  A row's key is (time dictId << 32) | row ordinal, the
+// ordinal being the segment's doc base in the call plus the doc id: u64 max is the last row by (time, call order), u64
+// min the first.  The key table is SegDesc.distinct_bits[a] (as u64: one per result, or one per group / slot) and the
+// segment's doc base is SegDesc.distinct_words[a].
+constexpr int kFnWithTime = 7;
+enum : int32_t { WT_MAX = 0, WT_MIN = 1 };
+__host__ __device__ constexpr unsigned long long withtime_key(uint32_t time_id, uint32_t ordinal) {
+  return (unsigned long long)time_id << 32 | ordinal;
+}
+
 struct SlotDesc {
   const uint32_t* data;  // device: packed words, padded to whole tiles
   int32_t bits;          // 1..32 (32 = raw big-endian 32-bit values)
@@ -107,6 +118,7 @@ struct SegDesc {
   //   PERCENTILE:    u32 histogram of dictId counts, distinct_words[a] = entries per group (the column's cardinality);
   //                  aggregation only: 1 when the warps count into private shared-memory histograms first (at most
   //                  64 dictIds, in the aggregation's accumulator slots), else 0
+  //   FIRST/LASTWITHTIME: u64 key table (kFnWithTime above), distinct_words[a] = the segment's doc base in the call
   uint32_t* distinct_bits[kMaxAggs];
   uint32_t distinct_words[kMaxAggs];
   AggAccum* accum;                     // aggregation-only output

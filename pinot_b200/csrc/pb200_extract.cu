@@ -70,6 +70,7 @@ struct ExtractDesc {
   const uint32_t* dbits[kMaxAggs];   // DISTINCTCOUNT per-group bitsets (an ORDER BY key is the popcount of a row)
   uint32_t dwords[kMaxAggs];
   const uint32_t* pct_n[kMaxAggs];   // PERCENTILE: values per table entry (src[a] holds the selected dictIds)
+  const long long* wt_time[kMaxAggs];  // FIRST/LASTWITHTIME: the winning row's time value per table entry (src[a]: data dictIds)
   const long long* mom[kMaxAggs][3]; // VAR / STDDEV: the K, H, L limb sum tables (pb200_moments.h)
   int32_t mom_e[kMaxAggs];           // ... and the grid exponent of the column
   unsigned long long off_mom[kMaxAggs];  // ... {s1, s2 low, s2 high} per row, for pb200_result_moments
@@ -181,6 +182,10 @@ __device__ __forceinline__ void agg_values(const ExtractDesc& d, int a, long lon
     lv = d.pct_n[a][g];
     if (x == ~0u) dv = -INFINITY;
     else { id = (int32_t)x; dv = dict_value(d, a, x); }
+  } else if (fn == PB200_AGG_FIRSTWITHTIME || fn == PB200_AGG_LASTWITHTIME) {  // finalized (pb200_withtime.cu): ~0 = no row
+    const uint32_t x = static_cast<const uint32_t*>(d.src[a])[g];
+    if (x == ~0u) dv = -INFINITY;
+    else { id = (int32_t)x; dv = dict_value(d, a, x); lv = d.wt_time[a][g]; }
   } else if (is_moments_fn(fn)) {  // exact moments from the group's limb sums and count, rounded once
     dv = moments_final(fn, moments_from_sums(cnt, d.mom[a][0][g], d.mom[a][1][g], d.mom[a][2][g]), d.mom_e[a]);
     lv = (long long)cnt;
@@ -367,9 +372,10 @@ static size_t layout_result(const pb200_result::Dense& d, ExtractDesc& e, size_t
   for (int a = 0; a < e.nagg; a++) {
     const int fn = e.fn[a];
     e.off_dbl[a] = take(8, rows);
+    const bool wt = fn == PB200_AGG_FIRSTWITHTIME || fn == PB200_AGG_LASTWITHTIME;
     e.off_lng[a] = (fn == PB200_AGG_COUNT || fn == PB200_AGG_AVG || fn == PB200_AGG_SUM || fn == PB200_AGG_DISTINCTCOUNT ||
-                    fn == PB200_AGG_PERCENTILE || is_moments_fn(fn)) ? take(8, rows) : kNoCol;
-    e.off_ids[a] = (fn == PB200_AGG_MIN || fn == PB200_AGG_MAX || fn == PB200_AGG_PERCENTILE) ? take(4, rows) : kNoCol;
+                    fn == PB200_AGG_PERCENTILE || is_moments_fn(fn) || wt) ? take(8, rows) : kNoCol;
+    e.off_ids[a] = (fn == PB200_AGG_MIN || fn == PB200_AGG_MAX || fn == PB200_AGG_PERCENTILE || wt) ? take(4, rows) : kNoCol;
     e.off_mom[a] = is_moments_fn(fn) ? take(24, rows) : kNoCol;
   }
   return off;
@@ -444,6 +450,7 @@ int extract_groups(pb200_ctx* ctx, pb200_result* const* Rs, int nres, cudaStream
       else if (fn == PB200_AGG_MIN) e.src[a] = d.gmin[a];
       else if (fn == PB200_AGG_MAX) e.src[a] = d.gmax[a];
       else if (fn == PB200_AGG_PERCENTILE) { e.src[a] = Rs[r]->pct.ids[a]; e.pct_n[a] = Rs[r]->pct.n[Rs[r]->pct.rep[a]]; }
+      else if (fn == PB200_AGG_FIRSTWITHTIME || fn == PB200_AGG_LASTWITHTIME) { e.src[a] = Rs[r]->wt.ids[a]; e.wt_time[a] = Rs[r]->wt.time[a]; }
       else if (is_moments_fn(fn)) {
         for (int j = 0; j < 3; j++) e.mom[a][j] = d.isum[d.mom_first[a] + j];
         e.mom_e[a] = d.mom_e[a];

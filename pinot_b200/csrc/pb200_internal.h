@@ -223,6 +223,13 @@ struct pb200_result {
     const uint32_t* row_entry = nullptr;         // group-by: table entry of each extracted row (inside view.block)
     std::vector<uint32_t> host[pb200::kMaxAggs]; // owners: histogram rows of the result's rows, copied on first use
   } pct;
+  // FIRST/LASTWITHTIME with GROUP BY (pb200_withtime.cu): per table entry the winning key, then the data dictId (~0: no
+  // row) and the time value the finalize decoded from it; allocated with the dense tables and freed with them
+  struct Wt {
+    unsigned long long* key[pb200::kMaxAggs] = {};
+    uint32_t* ids[pb200::kMaxAggs] = {};
+    long long* time[pb200::kMaxAggs] = {};
+  } wt;
   // VAR / STDDEV (pb200_moments.h): the grid of each such aggregation's dictionary and its exact moments per row
   struct Mom {
     bool on[pb200::kMaxAggs] = {};

@@ -162,10 +162,38 @@ struct ScanPlanner {
     q.num_segments = nseg; q.num_aggs = nagg; q.num_group_by = ngb;
     plan.pct_p.assign(nagg, std::numeric_limits<double>::quiet_NaN());
     plan.pct_rep.assign(nagg, -1);
+    plan.wt_time.assign(nagg, -1);
+    return PB200_OK;
+  }
+  // FIRST/LASTWITHTIME: the time column t (INT / LONG with dictIds), the data column v (dictIds) and the type literal
+  int check_withtime(int a, const pb200_agg_arg* wt_args) {
+    const pb200_agg& ag = plan.aggs[a];
+    const char* name = ag.function == PB200_AGG_FIRSTWITHTIME ? "FIRSTWITHTIME" : "LASTWITHTIME";
+    if (!wt_args) { set_error("unknown aggregation function %d without arguments: %s (aggregation %d) takes its time column through pb200_execute_agg_args", ag.function, name, a); return PB200_E_INVALID; }
+    const int tc = wt_args[a].time_column;
+    if (tc < 0 || tc >= ncols) { set_error("%s (aggregation %d): time column %d out of range", name, a, tc); return PB200_E_INVALID; }
+    if (plan.defer_finalize || query->reduce_world > 1) { set_error("%s is not combined across GPUs (PB200_Q_DEFER_FINALIZE / reduce_world)", name); return PB200_E_UNSUPPORTED; }
+    for (int t = 0; t < nseg; t++) {
+      const DeviceColumn &c = segments[t]->cols[tc], &v = segments[t]->cols[ag.column];
+      if ((c.stored_type != PB200_INT && c.stored_type != PB200_LONG) || c.bits > 31 || !c.dict_native || c.cardinality <= 0) {
+        set_error("%s over time column %d: not an INT / LONG column with dictIds in segment %d: not accelerated", name, tc, t);
+        return PB200_E_UNSUPPORTED;
+      }
+      if (v.bits > 31 || v.cardinality <= 0 || (v.stored_type != PB200_STRING && !v.dict_native)) {
+        set_error("%s over data column %d: no dictIds in segment %d (raw values): not accelerated", name, ag.column, t);
+        return PB200_E_UNSUPPORTED;
+      }
+      if (v.stored_type != wt_args[a].value_type) {
+        set_error("%s (aggregation %d): type literal %d is not the stored type %d of column %d: not accelerated", name, a, wt_args[a].value_type, v.stored_type, ag.column);
+        return PB200_E_UNSUPPORTED;
+      }
+    }
+    plan.wt_time[a] = tc;
+    plan.any_wt = true;
     return PB200_OK;
   }
   // ---- slots: filter scan columns, then group-by keys, then aggregation arguments ----
-  int assign_slots(const double* agg_args) {
+  int assign_slots(const double* agg_args, const pb200_agg_arg* wt_args) {
     const pb200_filter_node* f0 = query->filter;
     for (int s = 0; s < (per_seg_filter ? nseg : 1); s++) {
       for (int i = 0; i < nnodes; i++) {
@@ -195,8 +223,16 @@ struct ScanPlanner {
       const pb200_agg& ag = plan.aggs[a];
       q.aggs[a] = AggDesc{ag.function, -1, VAL_NONE, 0};
       if (ag.function == PB200_AGG_COUNT || is_moments_fn(ag.function)) continue;   // VAR / STDDEV: read their limb sums
-      if (ag.function < 0 || ag.function > PB200_AGG_PERCENTILE) { set_error("unknown aggregation function %d", ag.function); return PB200_E_INVALID; }
+      if (ag.function < 0 || (ag.function > PB200_AGG_PERCENTILE && !is_withtime_fn(ag.function))) { set_error("unknown aggregation function %d", ag.function); return PB200_E_INVALID; }
       if (ag.column < 0 || ag.column >= ncols) { set_error("aggregation column %d out of range", ag.column); return PB200_E_INVALID; }
+      if (is_withtime_fn(ag.function)) {
+        // the scan streams the time column; the data column is read once per result or group by the finalize
+        if (int rc = check_withtime(a, wt_args)) return rc;
+        if ((q.aggs[a].slot = slot_of(plan, plan.wt_time[a], ROLE_AGG)) < 0) return PB200_E_UNSUPPORTED;
+        const int vt = segments[0]->cols[ag.column].stored_type;
+        q.aggs[a].val_kind = vt == PB200_LONG ? VAL_DICT_I64 : vt == PB200_FLOAT ? VAL_DICT_F32 : vt == PB200_DOUBLE ? VAL_DICT_F64 : VAL_DICT_I32;
+        continue;
+      }
       if (ag.function == PB200_AGG_PERCENTILE) {
         // the percentile travels beside the query (pb200_execute_args); PercentileAggregationFunction takes 0 <= p <= 100
         if (!agg_args) {   // pb200_execute / pb200_execute_ordered carry no percentile
@@ -591,7 +627,10 @@ struct ScanPlanner {
           if (q.aggs[a].slot < 0 || pipelined[a] != (pass == 1)) continue;
           if (plan.pct_rep[a] >= 0 && plan.pct_rep[a] != a) continue;   // reads another PERCENTILE's histogram
           const SlotDesc& sl = sd.slots[q.aggs[a].slot];
-          sd.agg_code[n++] = agg_code(a, q.aggs[a].function, q.aggs[a].val_kind, sl.bits, sl.stage_words);
+          if (plan.wt_time[a] >= 0)   // the value-kind field says which end of the key order wins
+            sd.agg_code[n++] = agg_code(a, kFnWithTime, q.aggs[a].function == PB200_AGG_LASTWITHTIME ? WT_MAX : WT_MIN, sl.bits, sl.stage_words);
+          else
+            sd.agg_code[n++] = agg_code(a, q.aggs[a].function, q.aggs[a].val_kind, sl.bits, sl.stage_words);
         }
       sd.num_agg_codes = n;
       sd.num_defer_codes = plan.group_by ? npipe : 0;
@@ -624,6 +663,16 @@ struct ScanPlanner {
         set_error("%s over %llu docs in one result: at most 2^32 - 1", any_pct ? "PERCENTILE" : "VAR/STDDEV", result_docs(r));
         return PB200_E_UNSUPPORTED;
       }
+    if (plan.any_wt) {
+      // row ordinals are 32-bit: the call's docs must stay below 2^32
+      unsigned long long base = 0;
+      plan.wt_base.assign(nseg, 0);
+      for (int s = 0; s < nseg; s++) { plan.wt_base[s] = base; base += (unsigned long long)segments[s]->num_docs; }
+      if (base >= (1ull << 32)) { set_error("FIRST/LASTWITHTIME over %llu docs in one call: at most 2^32 - 1", base); return PB200_E_UNSUPPORTED; }
+      for (int s = 0; s < nseg; s++)
+        for (int a = 0; a < q.num_aggs; a++)
+          if (plan.wt_time[a] >= 0) plan.segs[s].distinct_words[a] = (uint32_t)plan.wt_base[s];
+    }
     if (!plan.group_by) {
       // PERCENTILE: one histogram of 2^bits u32 entries per result and column (every representable dictId is addressable)
       plan.hist_entries.assign(plan.nres, std::vector<size_t>(q.num_aggs, 0));
@@ -654,7 +703,7 @@ struct ScanPlanner {
         for (int a = 0; a < q.num_aggs; a++) {
           sd.sum_addend[a] = 0ull - (1ull << 31);  // plain INT-dictionary sum: remove the device copy's bias
           if (a == t.carrier.agg) sd.sum_addend[a] = (1ull << t.carrier.shift) - (unsigned long long)((uint32_t)(int32_t)t.carrier.vmin ^ 0x80000000u);
-          sd.distinct_words[a] = plan.pct_rep[a] >= 0 ? t.hist_per_group[a] : t.dwords[a];
+          sd.distinct_words[a] = plan.wt_time[a] >= 0 ? (uint32_t)plan.wt_base[s] : plan.pct_rep[a] >= 0 ? t.hist_per_group[a] : t.dwords[a];
         }
         for (int g = 0; g < ngb; g++) { sd.group_mult[g] = t.mult[g] * (uint32_t)t.stride; sd.group_mult64[g] = t.mult64[g]; }  // hash tables: stride 1
         sd.h_mask = t.hashed ? (uint32_t)(t.groups - 1) : 0u;
@@ -809,7 +858,7 @@ struct ScanPlanner {
 }  // namespace
 
 int plan_scan(const Tuning& tune, DeviceLimits lim, const pb200_query* query, pb200_segment* const* segments, int nseg,
-              bool allow_count_carrier, ScanPlan* out, const double* agg_args) {
+              bool allow_count_carrier, ScanPlan* out, const double* agg_args, const pb200_agg_arg* wt_args) {
   if (!query || !segments || !out || nseg <= 0) { set_error("invalid argument to pb200_execute"); return PB200_E_INVALID; }
   const bool merge = query->flags & PB200_Q_MERGE_SEGMENTS;
   const int nnodes = query->num_filter_nodes, nuser = query->num_aggs, ngb = query->num_group_by;
@@ -837,11 +886,18 @@ int plan_scan(const Tuning& tune, DeviceLimits lim, const pb200_query* query, pb
                          : is_moments_fn(ag.function) ? "VAR/STDDEV" : "MIN/MAX";
       if (!same_dictionary(segments, nseg, ag.column, what)) return PB200_E_UNSUPPORTED;
     }
+    for (int a = 0; a < nuser && wt_args; a++) {   // FIRST/LASTWITHTIME: one dictionary for the data and the time column
+      const pb200_agg& ag = query->aggs[a];
+      if (!is_withtime_fn(ag.function)) continue;
+      const int tc = wt_args[a].time_column;
+      for (int c : {ag.column, tc})
+        if (c >= 0 && c < ncols && !same_dictionary(segments, nseg, c, "FIRST/LASTWITHTIME")) return PB200_E_UNSUPPORTED;
+    }
   }
   *out = ScanPlan();
   ScanPlanner p{tune, lim, query, segments, nseg, ncols, *out};
   if (int rc = p.expand_moments()) return rc;
-  if (int rc = p.assign_slots(agg_args)) return rc;
+  if (int rc = p.assign_slots(agg_args, wt_args)) return rc;
   if (int rc = p.compile_filter()) return rc;
   p.choose_carriers(allow_count_carrier);
   if (int rc = p.choose_geometry()) return rc;

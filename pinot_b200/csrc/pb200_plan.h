@@ -85,6 +85,11 @@ struct ScanPlan {
   std::vector<pb200_agg> aggs;                        // the launch's aggregations, internal ones included
   std::vector<int> mom_first;                         // [user agg] the first of its column's limb sums (-1: not VAR / STDDEV)
   std::vector<int> limb;                              // [agg] 0 / 1 / 2 for the K / H / L limb sums, else -1
+  // FIRST/LASTWITHTIME (DESIGN.md section 3.13): the time column of aggregation a (-1: not one of them; its slot streams
+  // the time column, its column is the data column), and each segment's doc base in the call (row ordinal = base + doc)
+  std::vector<int> wt_time;
+  std::vector<unsigned long long> wt_base;
+  bool any_wt = false;
   std::vector<std::vector<size_t>> hist_entries;      // aggregation only: [result][agg] histogram entries of an owner (0: none)
   long long hist_total = 0;                           // histogram entries of all results of the call
   std::vector<long long> in_filter;                   // per result: num_entries_scanned_in_filter
@@ -98,8 +103,11 @@ constexpr long long kMaxHistogramEntries = 1ll << 28;  // PERCENTILE histogram e
 // accumulator slots in shared memory (32 threads x 8 bytes = 64 u32 bins), flushed once per segment, instead of one
 // same-address L2 reduction per row (DESIGN.md section 3.7 has the measurements)
 constexpr int kHistWarpPrivateMaxCard = 64;
+// wt_args: one per aggregation, the time column and type literal of a FIRST/LASTWITHTIME (NULL: they are refused, as
+// every entry point but pb200_execute_agg_args does).
 int plan_scan(const Tuning& tune, DeviceLimits lim, const pb200_query* query, pb200_segment* const* segments, int nseg,
-              bool allow_count_carrier, ScanPlan* out, const double* agg_args = nullptr);
+              bool allow_count_carrier, ScanPlan* out, const double* agg_args = nullptr, const pb200_agg_arg* wt_args = nullptr);
+inline bool is_withtime_fn(int fn) { return fn == PB200_AGG_FIRSTWITHTIME || fn == PB200_AGG_LASTWITHTIME; }
 
 // ---- selection (pb200_execute_selection): plan_scan with COUNT(*) as the only aggregation, plus the match mask ----
 constexpr long long kSelectPrefixRows = 1ll << 20;  // first pass of a selection without ORDER BY: at least this many docs

@@ -276,6 +276,17 @@ struct MinMaxLeft {
   __device__ __forceinline__ void operator()(int j, uint32_t xl) {
     if ((m >> j) & 1u) { mn = min(mn, xl); mx = max(mx, xl); }
   }
+};// FIRST/LASTWITHTIME: the largest (last) or smallest time dictId of the surviving rows on the left-aligned form and the
+// row holding it -- rows arrive ascending, so LAST keeps the later of equal times and FIRST the earlier one.  The low
+// bits of a left-aligned value belong to the next rows: `keep` clears them so that equal times compare equal.
+struct BestTimeLeft {
+  uint32_t m, keep;
+  bool last;
+  uint32_t bt, bj;
+  __device__ __forceinline__ void operator()(int j, uint32_t xl) {
+    const uint32_t x = xl & keep;
+    if (((m >> j) & 1u) && (last ? x >= bt : x < bt)) { bt = x; bj = (uint32_t)j; }
+  }
 };
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -831,6 +842,12 @@ scan_kernel(const __grid_constant__ QueryDesc q, const __grid_constant__ TmaTabl
         } else if (fn == 6) {  // PERCENTILE: the result's dictId histogram (the sorted value list of the reference)
           if (!GROUPBY && sd.distinct_words[a]) atomicAdd(reinterpret_cast<uint32_t*>(acc64 + a * kConsumers + warp * 32) + id, 1u);
           else red_add_u32(sd.distinct_bits[a] + id, 1u);
+        } else if (!GROUPBY && fn == kFnWithTime) {
+          // FIRST/LASTWITHTIME, few survivors: the row's key straight into the result's, when it can win
+          unsigned long long* const kp = reinterpret_cast<unsigned long long*>(sd.distinct_bits[a]);
+          const unsigned long long key = withtime_key(id, sd.distinct_words[a] + row0 + (uint32_t)j);
+          if (vk == WT_MAX) { if (key > __ldcg(kp)) atomicMax(kp, key); }
+          else if (key < __ldcg(kp)) atomicMin(kp, key);
         }
       }
     };
@@ -1031,6 +1048,16 @@ scan_kernel(const __grid_constant__ QueryDesc q, const __grid_constant__ TmaTabl
               const size_t epg = sd.distinct_words[a];
 #pragma unroll
               for (int u = 0; u < kQB; ++u) if (ok[u]) red_add_u32(hist + (size_t)g[u] * epg + id[u], 1u);
+            } else if (fn == kFnWithTime) {  // FIRST/LASTWITHTIME: the group's best (time dictId, row ordinal) key
+              unsigned long long* const kt = reinterpret_cast<unsigned long long*>(sd.distinct_bits[a]);
+              const uint32_t ord0 = sd.distinct_words[a] + (row0 & ~1023u);  // the slice's first row (queue entries are slice rows)
+              if (vk == WT_MAX) {
+#pragma unroll
+                for (int u = 0; u < kQB; ++u) if (ok[u]) atomicMax(kt + g[u], withtime_key(id[u], ord0 + e[u]));
+              } else {
+#pragma unroll
+                for (int u = 0; u < kQB; ++u) if (ok[u]) atomicMin(kt + g[u], withtime_key(id[u], ord0 + e[u]));
+              }
             } else if (fn == 2 || fn == 3) {
               // MIN / MAX tables change for only O(log n) of a group's rows: read the current entries first, then issue
               // a reduction only where the row can win (a stale read costs a redundant reduction, never a wrong result)
@@ -1092,6 +1119,23 @@ scan_kernel(const __grid_constant__ QueryDesc q, const __grid_constant__ TmaTabl
               mmx.x = min(mmx.x, f.mn >> sh);
               mmx.y = max(mmx.y, (f.mx >> sh) + 1u);
               accmm[a * kConsumers + group] = mmx;
+            }
+          } else if (fn == kFnWithTime) {
+            // FIRST/LASTWITHTIME: the thread's best (time dictId, row) over its surviving rows, each read straight from
+            // the tile, then the warp's best with two 32-bit warp reductions (time, then the row among the lanes holding
+            // that time) and one 64-bit atomic per warp and tile.  No unpack switch and no 64-bit shuffles: either would
+            // cost registers next to the deferred gathers.
+            const bool last = vk == WT_MAX;
+            BestTimeLeft f{m, 0xFFFFFFFFu << (32 - abits), last, last ? 0u : 0xFFFFFFFFu, 0u};
+            dispatch_left_aligned(abits, base, group_in_stage, f);
+            const uint32_t bt = f.bt >> (32 - abits), bj = f.bj;
+            const uint32_t wt = last ? __reduce_max_sync(0xFFFFFFFFu, pc ? bt : 0u) : __reduce_min_sync(0xFFFFFFFFu, pc ? bt : 0xFFFFFFFFu);
+            const bool mine = pc && bt == wt;
+            const uint32_t ord = sd.distinct_words[a] + row0 + bj;
+            const uint32_t wo = last ? __reduce_max_sync(0xFFFFFFFFu, mine ? ord : 0u) : __reduce_min_sync(0xFFFFFFFFu, mine ? ord : 0xFFFFFFFFu);
+            if (__any_sync(0xFFFFFFFFu, pc != 0) && lane == 0) {
+              unsigned long long* const kp = reinterpret_cast<unsigned long long*>(sd.distinct_bits[a]);
+              if (last) atomicMax(kp, withtime_key(wt, wo)); else atomicMin(kp, withtime_key(wt, wo));
             }
           } else {
             uint32_t v[32];

@@ -192,6 +192,10 @@ def combine_tables(backend, block, query, dist, dst: int = 0):
 def execute_and_combine(plan_maker_or_backend, segments: Sequence, query, dist, dst: int = 0, merged_docs_bound: int = 0):
     """One query over the whole table: every rank scans its segments with the device-side combine, the per-GPU group tables
     are reduced ONCE to rank `dst`, which gets the results block of the whole table (others get None)."""
+    if any(a.function in ("FIRSTWITHTIME", "LASTWITHTIME") for a in query.aggregations):
+        # the winning rows of different GPUs are compared by time value on the host: the caller merges per-GPU results
+        from ._lib import E_UNSUPPORTED, UnsupportedQueryError
+        raise UnsupportedQueryError(E_UNSUPPORTED, "FIRSTWITHTIME / LASTWITHTIME are not combined across GPUs")
     if any(a.function == "PERCENTILE" for a in query.aggregations):
         # per-GPU histograms are not reduced across GPUs: the caller runs the query per GPU and merges by value
         from ._lib import E_UNSUPPORTED, UnsupportedQueryError

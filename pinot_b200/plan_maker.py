@@ -25,7 +25,7 @@ import numpy as np
 
 from . import _lib
 from ._lib import UnsupportedQueryError  # noqa: F401  (re-export)
-from .query import MOMENT_FUNCTIONS, Filter, Moments, QueryContext, postfix
+from .query import MOMENT_FUNCTIONS, WITHTIME_FUNCTIONS, WITHTIME_TYPES, Filter, Moments, QueryContext, postfix
 
 
 class B200Context:
@@ -432,12 +432,25 @@ class ResultsBlock:
             ctx.lib.pb200_result_free(self.handle)
             self.handle = None
 
-    def get_results(self, query: QueryContext) -> List[object]:
+    def withtime(self, a: int, row: int, segment: "IndexSegment", column: str):
+        """FIRST/LASTWITHTIME aggregation `a` in row `row`: (time value, data value) of the winning row, or None when the
+        row has no matched doc.  The data value is looked up exactly through its dictId in `segment`'s dictionary of
+        `column` (the block's segment; for a merged block any of its bound segments): STRING values and LONG values
+        beyond 2^53 come back as stored."""
+        d = int(self.dict_ids[a][row])
+        return None if d < 0 else (int(self.longs[a][row]), segment.dictionary_value(column, d))
+
+    def get_results(self, query: QueryContext, segment: Optional["IndexSegment"] = None) -> List[object]:
         """AggregationResultsBlock.getResults(): Long for COUNT, Double for SUM/MIN/MAX/PERCENTILE, (sum, count) for AVG,
-        set size for DISTINCTCOUNT -- row 0 (aggregation only)."""
+        set size for DISTINCTCOUNT -- row 0 (aggregation only).  FIRST/LASTWITHTIME: with `segment` (the block's), the
+        data value as stored (STRING included), -inf without a matched doc; without it the double column, which holds
+        the dictId for a STRING column."""
         out = []
         for a, agg in enumerate(query.aggregations):
-            if agg.function == "COUNT":
+            if agg.function in WITHTIME_FUNCTIONS and segment is not None:
+                v = self.withtime(a, 0, segment, agg.column)
+                out.append(float("-inf") if v is None else v[1])
+            elif agg.function == "COUNT":
                 out.append(int(self.longs[a][0]))
             elif agg.function == "AVG":
                 out.append((float(self.doubles[a][0]), int(self.longs[a][0])))
@@ -783,7 +796,16 @@ class B200PlanMaker:
         spec = order_spec(query, merge) if ordered else None
         having = having_spec(query) if ordered and (merge or n == 1) else None
         pct = [a.function == "PERCENTILE" for a in query.aggregations]
-        if having is not None:
+        if any(a.function in WITHTIME_FUNCTIONS for a in query.aggregations):
+            # FIRST/LASTWITHTIME: the time column and the type literal travel beside the query (pb200h_execute_agg_args)
+            args = (_lib.HAggArg * len(pct))(*[
+                _lib.HAggArg(float(a.arg) if is_p else 0.0,
+                             a.time_column.encode() if a.function in WITHTIME_FUNCTIONS else None,
+                             WITHTIME_TYPES[a.value_type] if a.function in WITHTIME_FUNCTIONS else 0)
+                for a, is_p in zip(query.aggregations, pct)])
+            _lib.check(self.ctx.lib.pb200h_execute_agg_args(self.ctx.handle, C.byref(hq), C.byref(spec) if spec is not None else None,
+                                                            args, C.byref(having) if having is not None else None, segs, n, res, kinds))
+        elif having is not None:
             args = (C.c_double * max(1, len(pct)))(*[float(a.arg) if is_p else 0.0 for a, is_p in zip(query.aggregations, pct)])
             _lib.check(self.ctx.lib.pb200h_execute_having(self.ctx.handle, C.byref(hq), C.byref(spec) if spec is not None else None,
                                                           args, C.byref(having), segs, n, res, kinds))

@@ -47,18 +47,41 @@ FilterNode = Union[Filter, Predicate]
 @dataclass
 class Aggregation:
     function: str  # COUNT | SUM | MIN | MAX | AVG | DISTINCTCOUNT | PERCENTILE | VARPOP | VARSAMP | STDDEVPOP | STDDEVSAMP
+    #                | FIRSTWITHTIME | LASTWITHTIME
     column: Optional[str] = None  # None for COUNT(*)
     # FILTER (WHERE ...) clause of this function (QueryContext.getFilteredAggregationFunctions: Pair<function, FilterContext>);
     # evaluated together with the query's own filter (AggregationFunctionUtils.buildFilteredAggregationInfos)
     filter: Optional["FilterNode"] = None
     arg: Optional[float] = None  # PERCENTILE: the percentile, 0 <= p <= 100
+    # FIRSTWITHTIME / LASTWITHTIME(column, time_column, 'value_type'): the time column and the type literal (upper case)
+    time_column: Optional[str] = None
+    value_type: Optional[str] = None
     # named only in HAVING: computed like the others, never an output column (Pinot's QueryContext adds such functions too)
     hidden: bool = False
 
     def __str__(self):
         if self.function == "PERCENTILE":
             return f"percentile({self.column}, {self.arg:g})"
+        if self.function in WITHTIME_FUNCTIONS:
+            return f"{self.function.lower()}({self.column},{self.time_column},'{self.value_type}')"
         return f"{self.function.lower()}({self.column or '*'})"
+
+
+WITHTIME_FUNCTIONS = ("FIRSTWITHTIME", "LASTWITHTIME")
+# the type literal of FIRST/LASTWITHTIME -> the stored type it names (BOOLEAN is stored as INT)
+WITHTIME_TYPES = {"INT": 0, "BOOLEAN": 0, "LONG": 1, "FLOAT": 2, "DOUBLE": 3, "STRING": 4}
+
+
+def withtime_pick(function: str, cur, new):
+    """By-value merge of two FIRST/LASTWITHTIME intermediates (time value, data value); None is an empty one.  `new`
+    comes later in the call's row order: LAST keeps it on a tie, FIRST keeps `cur`."""
+    if cur is None:
+        return new
+    if new is None:
+        return cur
+    if function == "LASTWITHTIME":
+        return new if new[0] >= cur[0] else cur
+    return new if new[0] < cur[0] else cur
 
 
 def percentile_index(n: int, p: float) -> int:

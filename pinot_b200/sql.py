@@ -8,8 +8,11 @@ stays Java).  This module exists so the parity tests read like the reference's
 
     SELECT item[, item...] FROM table [WHERE cond] [GROUP BY col[, col...] [HAVING hcond]] [ORDER BY expr [ASC|DESC], ...]
            [LIMIT n]
-    item  := COUNT(*) | FN(col) | PERCENTILE(col, p) | PERCENTILE<n>(col) | col
-             (FN also VAR_POP / VARPOP, VAR_SAMP / VARSAMP, STDDEV_POP / STDDEVPOP, STDDEV_SAMP / STDDEVSAMP)
+    item  := COUNT(*) | FN(col) | PERCENTILE(col, p) | PERCENTILE<n>(col) | FIRSTWITHTIME(col, col, 'T')
+             | LASTWITHTIME(col, col, 'T') | col
+             (FN also VAR_POP / VARPOP, VAR_SAMP / VARSAMP, STDDEV_POP / STDDEVPOP, STDDEV_SAMP / STDDEVSAMP; T is the
+             data column's type, INT | LONG | FLOAT | DOUBLE | STRING | BOOLEAN, any case; the canonical text is
+             lastwithtime(v,t,'INT'))
              (plain columns are allowed only when they are group-by keys; 0 <= p <= 100, fractions allowed)
     selection (parse_selection): SELECT * | col[, col...] FROM table [WHERE cond] [ORDER BY col [ASC|DESC], ...] [LIMIT n]
     distinct (parse_distinct): SELECT DISTINCT col[, col...] FROM table [WHERE cond] [ORDER BY col [ASC|DESC], ...] [LIMIT n]
@@ -35,7 +38,7 @@ import re
 from dataclasses import dataclass, field
 from typing import List, Optional
 
-from .query import Aggregation, Filter, FilterNode, Predicate, QueryContext, flatten, optimize_filter
+from .query import WITHTIME_FUNCTIONS, WITHTIME_TYPES, Aggregation, Filter, FilterNode, Predicate, QueryContext, flatten, optimize_filter
 
 _TOKEN = re.compile(r"\s*(?:(\d+\.\d+(?:[eE][-+]?\d+)?|-?\d+\.\d+|-?\d+)|'((?:[^']|'')*)'|(<=|>=|<>|!=|[=<>(),*+/%-])|"
                     r"([A-Za-z_$][A-Za-z0-9_$]*))")
@@ -43,7 +46,7 @@ _TOKEN = re.compile(r"\s*(?:(\d+\.\d+(?:[eE][-+]?\d+)?|-?\d+\.\d+|-?\d+)|'((?:[^
 # VarianceAggregationFunction: both spellings of each function, the underscore one canonicalised to the other
 _ALIASES = {"VAR_POP": "VARPOP", "VAR_SAMP": "VARSAMP", "STDDEV_POP": "STDDEVPOP", "STDDEV_SAMP": "STDDEVSAMP"}
 _FUNCTIONS = {"COUNT", "SUM", "MIN", "MAX", "AVG", "DISTINCTCOUNT", "PERCENTILE", "VARPOP", "VARSAMP", "STDDEVPOP",
-              "STDDEVSAMP"} | set(_ALIASES)
+              "STDDEVSAMP", *WITHTIME_FUNCTIONS} | set(_ALIASES)
 _PERCENTILE_N = re.compile(r"PERCENTILE(\d+)")
 
 # single-column transforms (DESIGN.md section 3.8): SQL name (lower case, no '_') -> canonical name
@@ -94,6 +97,8 @@ def having_name(agg: Aggregation) -> str:
     """How a HAVING leaf names an aggregation (QueryContext.having)."""
     if agg.function == "PERCENTILE":
         return f"percentile({agg.column},{agg.arg!r})"
+    if agg.function in WITHTIME_FUNCTIONS:
+        return str(agg)
     return f"{agg.function.lower()}({agg.column or '*'})"
 
 
@@ -182,6 +187,18 @@ class _Parser:
             p = _percentile_arg(self.literal())
         return col, p
 
+    def withtime_call(self, fn: str) -> Aggregation:
+        """After `FIRSTWITHTIME(` / `LASTWITHTIME(`: data column, time column and type literal, up to the `)`."""
+        col = self.column()
+        self.expect_op(",")
+        time_col = self.column()
+        self.expect_op(",")
+        k, v = self.peek()
+        if k != "str" or v.upper() not in WITHTIME_TYPES:
+            raise SqlError(f"{fn} needs the data column's type as a string literal ({', '.join(WITHTIME_TYPES)}), got {self.peek()}")
+        self.i += 1
+        return Aggregation(fn, col, time_column=time_col, value_type=v.upper())
+
     def ident(self) -> str:
         k, v = self.peek()
         if k != "id":
@@ -258,6 +275,8 @@ class _Parser:
         if fn.startswith("PERCENTILE"):
             col, pct = self.percentile_call(name)
             agg = Aggregation("PERCENTILE", col, arg=pct)
+        elif fn in WITHTIME_FUNCTIONS:
+            agg = self.withtime_call(fn)
         elif self.take_op("*"):
             if fn != "COUNT":
                 raise SqlError(f"{fn}(*) is not valid")
@@ -384,7 +403,11 @@ def resolve_order_by(query: QueryContext) -> List[tuple]:
             continue
         m = re.fullmatch(r"([A-Za-z_$][A-Za-z0-9_$]*)\((.+?)(?:,([-+0-9.eE]+))?\)", expr)
         found = None
-        if m and _is_function(m.group(1)):
+        for a, agg in enumerate(query.aggregations):
+            if agg.function in WITHTIME_FUNCTIONS and having_name(agg) == expr:
+                found = a
+                break
+        if found is None and m and _is_function(m.group(1)):
             fn, col = _ALIASES.get(m.group(1).upper(), m.group(1).upper()), m.group(2)
             arg = None if m.group(3) is None else float(m.group(3))
             for a, agg in enumerate(query.aggregations):
@@ -393,6 +416,8 @@ def resolve_order_by(query: QueryContext) -> List[tuple]:
                     break
         if found is None:
             raise SqlError(f"ORDER BY {expr}: neither a GROUP BY column nor an aggregation of the SELECT list")
+        if query.aggregations[found].value_type == "STRING":
+            raise SqlError(f"ORDER BY {expr}: a STRING FIRST/LASTWITHTIME is not ordered on this path")
         out.append(("AGG", found, asc))
     return out
 
@@ -414,6 +439,8 @@ def resolve_having(query: QueryContext) -> List[tuple]:
     def index(name):
         for a, agg in enumerate(query.aggregations):
             if agg.filter is None and having_name(agg) == name:
+                if agg.value_type == "STRING":
+                    raise SqlError(f"HAVING {name}: a STRING FIRST/LASTWITHTIME is not compared on this path")
                 return a
         raise SqlError(f"HAVING {name}: no aggregation of the query computes it")
 
@@ -494,6 +521,9 @@ def parse(sql: str, **options) -> QueryContext:
                     inner, pct = p.percentile_call(name)
                     p.expect_op(")")
                     expr = f"percentile({inner},{pct!r})"
+                elif name.upper() in WITHTIME_FUNCTIONS:
+                    expr = having_name(p.withtime_call(name.upper()))
+                    p.expect_op(")")
                 else:
                     inner = "*" if p.take_op("*") else p.column()
                     p.expect_op(")")
