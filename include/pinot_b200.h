@@ -576,8 +576,14 @@ int32_t pb200_comm_shutdown(pb200_ctx* ctx);
  * *retry = 1 on EVERY rank when a count-carrying sum was not provably safe for the reduce: all ranks free the result and
  * execute again with PB200_Q_NO_COUNT_CARRIER.  It is a COLLECTIVE: all ranks must call it for the same queries in the same
  * order (calls of one context are serialised internally; concurrent queries need an agreed order across ranks, e.g. the
- * broker's request id).  Aggregation-only results (num_groups < 0) are combined too (sums / counts add, MIN / MAX by value). */
+ * broker's request id).  Aggregation-only results (num_groups < 0) are combined too (sums / counts add, MIN / MAX by value;
+ * an INT SUM / AVG adds the ranks' exact int64 sums and rounds the total once, as the group-by tables do). */
 int32_t pb200_result_combine(pb200_ctx* ctx, pb200_result* result, int32_t root, int32_t* retry);
+/* Aggregation-only result, SUM / AVG over an INT column: *out = the exact int64 sum the double column holds rounded
+ * (after pb200_result_combine on the root: the whole table's).  Returns 1 when written, 0 when aggregation `agg` has no
+ * exact sum (another function, a sum accumulated in double, a star-tree answer, a group-by result), < 0 on error.  A
+ * caller that adds results across processes adds these and rounds once: rounded sums beyond 2^53 do not add exactly. */
+int32_t pb200_result_exact_sum(const pb200_result* result, int32_t agg, int64_t* out);
 
 /* ---- synthetic segments (SegmentIndexCreationDriverImpl stand-in for benchmarks; bytes are Pinot's formats) ---- */
 typedef struct {

@@ -210,7 +210,7 @@ EXPORTED_SYMBOLS = [
     "pb200_segment_derive_column", "pb200h_segment_derive",
     "pb200h_startree_build", "pb200h_startree_get",
     "pb200_execute_having", "pb200h_execute_having", "pb200_execute_agg_args", "pb200h_execute_agg_args",
-    "pb200_match_pattern",
+    "pb200_match_pattern", "pb200_result_exact_sum",
 ]
 
 _LIB = None
@@ -249,6 +249,7 @@ def load() -> C.CDLL:
     L.pb200_result_group_keys.argtypes = [vp, vp]
     L.pb200_result_agg.argtypes = [vp, i32, vp, vp]
     L.pb200_result_agg_dict_ids.argtypes = [vp, i32, vp]
+    L.pb200_result_exact_sum.argtypes = [vp, i32, C.POINTER(i64)]
     L.pb200_result_distinct.restype = i64
     L.pb200_result_distinct.argtypes = [vp, i32, i32, vp, i64]
     L.pb200_result_fetch.argtypes = [vp, vp, vp, vp, vp]

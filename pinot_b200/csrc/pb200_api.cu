@@ -1166,6 +1166,7 @@ struct ScanCall {
     } else if (fn == PB200_AGG_SUM || fn == PB200_AGG_AVG) {
       v->d = sum_in_double(vk) ? acc_r.dsum[a] : (double)acc_r.isum[a];
       v->l = (int64_t)acc_r.count;
+      if (!sum_in_double(vk)) { R.exact.on[a] = true; R.exact.sum[a] = acc_r.isum[a]; }
     } else if (fn == PB200_AGG_MIN || fn == PB200_AGG_MAX) {
       // raw INT: 0xFFFFFFFF / 0 are INT_MAX / INT_MIN as well as "no row" (max_offset): only the count tells
       const bool mn = fn == PB200_AGG_MIN;
@@ -1345,6 +1346,12 @@ extern "C" int32_t pb200_result_agg(const pb200_result* R, int32_t a, double* od
   if (od && !R->dbl[a].empty()) memcpy(od, R->dbl[a].data(), R->dbl[a].size() * 8);
   if (ol && !R->lng[a].empty()) memcpy(ol, R->lng[a].data(), R->lng[a].size() * 8);
   return PB200_OK;
+}
+extern "C" int32_t pb200_result_exact_sum(const pb200_result* R, int32_t a, int64_t* out) {
+  if (!R || a < 0 || a >= R->meta.num_aggs || !out) { set_error("bad aggregation index"); return PB200_E_INVALID; }
+  if (R->meta.num_groups >= 0 || a >= kMaxAggs || !R->exact.on[a]) return 0;
+  *out = R->exact.sum[a];
+  return 1;
 }
 extern "C" int32_t pb200_result_agg_dict_ids(const pb200_result* R, int32_t a, int32_t* out) {
   if (!R || a < 0 || a >= R->meta.num_aggs || !out) { set_error("bad aggregation index"); return PB200_E_INVALID; }

@@ -142,28 +142,32 @@ static int combine_scalars(NcclApi* api, pb200_ctx* ctx, pb200_result* R, int ro
   ncclComm_t comm = static_cast<ncclComm_t>(ctx->nccl_comm);
   StreamLease st(ctx);
   std::lock_guard<std::mutex> g(ctx->comm_mu);
-  // pinned / device scratch (8-byte slots): [0,4) statistics | [8,16) double sums | [16,24) long counts | [24,32) double mins | [32,40) double maxs; outputs at +64
+  // pinned / device scratch (8-byte slots): [0,4) statistics | [8,16) double sums | [16,24) long counts | [24,32) double mins |
+  // [32,40) double maxs | [40,48) exact int64 sums of INT SUM / AVG; outputs at +64
+  static_assert(64 + 48 <= 128, "comm scratch holds 128 slots");
   long long* pin = ctx->comm_pinned;
   double* pd = reinterpret_cast<double*>(pin);
   pin[0] = R->meta.num_docs_scanned; pin[1] = R->meta.num_entries_scanned_in_filter;
   pin[2] = R->meta.num_entries_scanned_post_filter; pin[3] = R->meta.num_total_docs;
-  for (int a = 0; a < kMaxAggs; a++) { pd[8 + a] = 0.0; pin[16 + a] = 0; pd[24 + a] = INFINITY; pd[32 + a] = -INFINITY; }
+  for (int a = 0; a < kMaxAggs; a++) { pd[8 + a] = 0.0; pin[16 + a] = 0; pd[24 + a] = INFINITY; pd[32 + a] = -INFINITY; pin[40 + a] = 0; }
   for (int a = 0; a < nagg; a++) {
     const double dv = R->dbl[a].empty() ? 0.0 : R->dbl[a][0];
     const long long lv = R->lng[a].empty() ? 0 : R->lng[a][0];
     pd[8 + a] = dv; pin[16 + a] = lv; pd[24 + a] = dv; pd[32 + a] = dv;
+    if (R->exact.on[a]) pin[40 + a] = R->exact.sum[a];
   }
   long long* dev = ctx->comm_scratch;
-  PB200_CUDA(cudaMemcpyAsync(dev, pin, 40 * sizeof(long long), cudaMemcpyHostToDevice, st));
+  PB200_CUDA(cudaMemcpyAsync(dev, pin, 48 * sizeof(long long), cudaMemcpyHostToDevice, st));
   PB200_NCCL(api, api->GroupStart());
   ncclResult_t r = api->Reduce(dev, dev + 64, 4, ncclInt64, ncclSum, root, comm, st);
   if (r == ncclSuccess) r = api->Reduce(dev + 8, dev + 64 + 8, 8, ncclFloat64, ncclSum, root, comm, st);
   if (r == ncclSuccess) r = api->Reduce(dev + 16, dev + 64 + 16, 8, ncclInt64, ncclSum, root, comm, st);
   if (r == ncclSuccess) r = api->Reduce(dev + 24, dev + 64 + 24, 8, ncclFloat64, ncclMin, root, comm, st);
   if (r == ncclSuccess) r = api->Reduce(dev + 32, dev + 64 + 32, 8, ncclFloat64, ncclMax, root, comm, st);
+  if (r == ncclSuccess) r = api->Reduce(dev + 40, dev + 64 + 40, 8, ncclInt64, ncclSum, root, comm, st);
   ncclResult_t e = api->GroupEnd();
   if (r != ncclSuccess || e != ncclSuccess) { set_error("NCCL reduce of the aggregation scalars failed"); return PB200_E_CUDA; }
-  PB200_CUDA(cudaMemcpyAsync(pin + 64, dev + 64, 40 * sizeof(long long), cudaMemcpyDeviceToHost, st));
+  PB200_CUDA(cudaMemcpyAsync(pin + 64, dev + 64, 48 * sizeof(long long), cudaMemcpyDeviceToHost, st));
   PB200_CUDA(cudaStreamSynchronize(st));
   if (ctx->comm_rank != root) return PB200_OK;
   R->meta.num_docs_scanned = pin[64]; R->meta.num_entries_scanned_in_filter = pin[65];
@@ -175,7 +179,10 @@ static int combine_scalars(NcclApi* api, pb200_ctx* ctx, pb200_result* R, int ro
     if (fn == PB200_AGG_MIN) R->dbl[a][0] = pd[64 + 24 + a];
     else if (fn == PB200_AGG_MAX) R->dbl[a][0] = pd[64 + 32 + a];
     else if (fn == PB200_AGG_COUNT) { R->lng[a][0] = pin[64 + 16 + a]; R->dbl[a][0] = (double)pin[64 + 16 + a]; }
-    else { R->dbl[a][0] = pd[64 + 8 + a]; R->lng[a][0] = pin[64 + 16 + a]; }
+    else if (R->exact.on[a]) {   // INT SUM / AVG: the exact total, rounded once (the ranks' doubles are rounded already)
+      R->exact.sum[a] = pin[64 + 40 + a];
+      R->dbl[a][0] = (double)pin[64 + 40 + a]; R->lng[a][0] = pin[64 + 16 + a];
+    } else { R->dbl[a][0] = pd[64 + 8 + a]; R->lng[a][0] = pin[64 + 16 + a]; }
     if ((fn == PB200_AGG_MIN || fn == PB200_AGG_MAX) && a < (int)R->ids.size() && !R->ids[a].empty()) R->ids[a][0] = -1;
   }
   return PB200_OK;

@@ -237,6 +237,12 @@ struct pb200_result {
     const unsigned long long* rows[pb200::kMaxAggs] = {};  // group-by: {s1, s2 low, s2 high} per row (inside view.block)
     unsigned long long one[pb200::kMaxAggs][3] = {};        // aggregation only: the same for the one row
   } mom;
+  // aggregation only: the exact int64 sum behind an INT SUM / AVG (the double column holds it rounded), so that a
+  // cross-GPU combine adds exact sums and rounds once (pb200_result_exact_sum, pb200_comm.cu: combine_scalars)
+  struct ExactSum {
+    bool on[pb200::kMaxAggs] = {};
+    long long sum[pb200::kMaxAggs] = {};
+  } exact;
   pb200_order_by order{};                      // ORDER BY spec of a group-by result (num_items 0: none), applied at extraction
   pb200_having having{};                       // HAVING of a group-by result (num_nodes 0: none), applied at extraction before
                                                // the order; set on every result whose rows it filtered

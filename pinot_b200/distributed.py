@@ -24,8 +24,9 @@ device buffers (``pb200_result_device_buffers``), nothing is copied.  The tables
 exchange is latency-bound (C4: 100 000 groups x (8+8+4) B = 2 MB per rank).
 
 The control flow (``execute_and_combine``) talks to the tables through a small backend interface so that the SAME code is
-exercised by the world_size-2 gloo test on CPU (tests/test_distributed_cpu.py, tables built from the oracle) and by the
-NCCL test on GPUs (tests/test_gpu_multi.py, ``DeviceBackend``).
+exercised by the world_size-2 gloo test on CPU (tests/test_distributed_cpu.py, tables built from the oracle), by 2 and 3
+simulated ranks on one GPU (tests/test_gpu_combine_loopback.py, ``DeviceBackend`` over an in-process collective) and by
+the NCCL test on two GPUs (tests/test_gpu_multi.py).
 """
 from __future__ import annotations
 
@@ -135,6 +136,11 @@ class DeviceBackend:
         import torch
         return torch.tensor([value], dtype=torch.int32, device=f"cuda:{self.ctx.device}")
 
+    def stats_tensor(self, block):
+        """The block's four execution statistics as an int64 tensor on the device, for a SUM reduce."""
+        import torch
+        return torch.tensor(_stats_list(block.stats), dtype=torch.int64, device=f"cuda:{self.ctx.device}")
+
     def synchronize(self):
         import torch
         torch.cuda.synchronize(self.ctx.device)  # the extraction runs on the library's own stream
@@ -167,6 +173,10 @@ def combine_tables(backend, block, query, dist, dst: int = 0):
     said unsafe -- then all ranks must run the query again without the carrier (the tables of all ranks must share one
     layout, so the fallback is collective)."""
     bufs = backend.buffers(block)
+    # the execution statistics of the whole table (the broker sums them over servers), as the in-library combine does
+    stats = backend.stats_tensor(block) if hasattr(backend, "stats_tensor") else None
+    if stats is not None:
+        dist.reduce(stats, dst=dst, op=dist.ReduceOp.SUM)
     flag = None
     if block.count_carrier and getattr(block, "flag_slot", False):
         # the verdict rides as the last element of the int64 block: one SUM all-reduce moves tables and verdicts together
@@ -186,12 +196,31 @@ def combine_tables(backend, block, query, dist, dst: int = 0):
             return None, True
     else:
         backend.synchronize()
-    return backend.finish(block, query, dist.get_rank() == dst), False
+    out = backend.finish(block, query, dist.get_rank() == dst)
+    if out is not None and stats is not None:
+        _set_stats(out, stats.tolist())
+    return out, False
+
+
+def _stats_list(stats) -> List[int]:
+    return [stats.num_docs_scanned, stats.num_entries_scanned_in_filter, stats.num_entries_scanned_post_filter,
+            stats.num_total_docs]
+
+
+def _set_stats(block, values: Sequence[int]) -> None:
+    (block.stats.num_docs_scanned, block.stats.num_entries_scanned_in_filter, block.stats.num_entries_scanned_post_filter,
+     block.stats.num_total_docs) = (int(v) for v in values)
 
 
 def execute_and_combine(plan_maker_or_backend, segments: Sequence, query, dist, dst: int = 0, merged_docs_bound: int = 0):
     """One query over the whole table: every rank scans its segments with the device-side combine, the per-GPU group tables
-    are reduced ONCE to rank `dst`, which gets the results block of the whole table (others get None)."""
+    are reduced ONCE to rank `dst`, which gets the results block of the whole table (others get None).  Every refusal
+    below is raised on every rank before any collective is issued."""
+    if getattr(query, "having", None) is not None:
+        # HAVING filters final rows: no route here applies it to the whole table's rows (the dense tables are filtered at
+        # extraction only on one GPU, the host merge would drop it): the caller filters the combined rows
+        from ._lib import E_UNSUPPORTED, UnsupportedQueryError
+        raise UnsupportedQueryError(E_UNSUPPORTED, "HAVING is not combined across GPUs")
     if any(a.function in ("FIRSTWITHTIME", "LASTWITHTIME") for a in query.aggregations):
         # the winning rows of different GPUs are compared by time value on the host: the caller merges per-GPU results
         from ._lib import E_UNSUPPORTED, UnsupportedQueryError
@@ -271,6 +300,8 @@ def _combine_with_sets(backend, segments, query, dist, dst):
                 else:
                     cur[a] = max(cur[a], vals[a], key=lambda t: t[0])
     keys_sorted = sorted(merged)   # raw-key order is not defined across tables: ascending ids, column 0 most significant
+    if query.is_group_by and query.order_by:
+        keys_sorted = _order_and_trim(query, fns, keys_sorted, merged)
     n, k = len(keys_sorted), len(query.group_by)
     out_keys = np.asarray(keys_sorted, dtype=np.int32).reshape(n, k) if query.is_group_by else np.zeros((0, 0), dtype=np.int32)
     doubles, longs, ids, distinct = [], [], [], {}
@@ -293,35 +324,90 @@ def _combine_with_sets(backend, segments, query, dist, dst):
     return block
 
 
+def _order_and_trim(query, fns, keys, merged):
+    """The merged rows (`keys` ascending, column 0 most significant) in ORDER BY order, trimmed as the dense route trims a
+    merged result (plan_maker.order_spec): one stable sort per item, last item first, so rows equal on every item keep
+    the key order -- the library's tie rule.  Values compare in the reference's order (query.value_order); a key column
+    compares by domain id, which is its value order."""
+    from .plan_maker import order_spec
+    from .query import value_order
+    from .sql import resolve_order_by
+
+    def final(a, v):
+        f = fns[a]
+        if f == "DISTINCTCOUNT":
+            return float(len(v))
+        if f == "COUNT":
+            return float(v[1])
+        if f == "AVG":
+            return v[0] / v[1] if v[1] else float("-inf")
+        return v[0]
+    rows = list(keys)
+    for kind, index, asc in reversed(resolve_order_by(query)):
+        if kind == "GROUP_BY":
+            rows.sort(key=lambda key: key[index], reverse=not asc)
+        else:
+            rows.sort(key=lambda key: value_order(float(final(index, merged[key][index]))), reverse=not asc)
+    trim = order_spec(query, merge=True).trim_size
+    return rows[:trim] if trim > 0 else rows
+
+
+def _exact_sums(ctx, block, n: int) -> List[Optional[int]]:
+    """Per aggregation of an aggregation-only block: the exact int64 sum behind an INT SUM / AVG, else None."""
+    out = []
+    for a in range(n):
+        v = C.c_int64()
+        rc = ctx.lib.pb200_result_exact_sum(block.handle, a, C.byref(v))
+        if rc < 0:
+            from . import _lib
+            _lib.check(rc)
+        out.append(v.value if rc == 1 else None)
+    return out
+
+
 def _combine_scalars(backend, segments, query, dist, dst):
     """Aggregation-only queries: a handful of scalars per rank (AggregationResultsBlockMerger.java:34-44)."""
     if getattr(backend, "native", False):   # the scalars meet inside the library too (pb200_comm.cu: combine_scalars)
         block = backend.pm.execute_segments(segments, query, merge=True, keep_handle=True, defer=False)[0]
         return backend.combine_native(block, query, dst)[0]
     import torch
-    block = backend.pm.execute_segments(segments, query, merge=True)[0]
+    block = backend.pm.execute_segments(segments, query, merge=True, keep_handle=True, defer=False)[0]
     fns = [a.function for a in query.aggregations]
+    n = len(fns)
+    exact = _exact_sums(backend.ctx, block, n)
+    block.release(backend.ctx)
     dev = f"cuda:{backend.ctx.device}"
-    sums = torch.tensor([float(block.doubles[a][0]) if f in ("SUM", "AVG") else 0.0 for a, f in enumerate(fns)] +
-                        [float(block.longs[a][0]) for a in range(len(fns))] + [float(block.stats.num_docs_scanned)],
-                        dtype=torch.float64, device=dev)          # counts < 2^53: exact in float64
+    sums = torch.tensor([float(block.doubles[a][0]) if f in ("SUM", "AVG") else 0.0 for a, f in enumerate(fns)],
+                        dtype=torch.float64, device=dev)
+    # INT SUM / AVG add exactly and round once on the root: the ranks' doubles are rounded already, and rounded sums beyond
+    # 2^53 do not add to the rounded total.  [exact sums | ranks that had one | counts | the four statistics]
+    ints = torch.tensor([e or 0 for e in exact] + [int(e is not None) for e in exact] +
+                        [int(block.longs[a][0]) for a in range(n)] + _stats_list(block.stats), dtype=torch.int64, device=dev)
     mins = torch.tensor([float(block.doubles[a][0]) if f == "MIN" else float("inf") for a, f in enumerate(fns)], dtype=torch.float64, device=dev)
     maxs = torch.tensor([float(block.doubles[a][0]) if f == "MAX" else float("-inf") for a, f in enumerate(fns)], dtype=torch.float64, device=dev)
     dist.reduce(sums, dst=dst, op=dist.ReduceOp.SUM)
+    dist.reduce(ints, dst=dst, op=dist.ReduceOp.SUM)
     if "MIN" in fns:
         dist.reduce(mins, dst=dst, op=dist.ReduceOp.MIN)
     if "MAX" in fns:
         dist.reduce(maxs, dst=dst, op=dist.ReduceOp.MAX)
     if dist.get_rank() != dst:
         return None
-    n = len(fns)
-    sums, mins, maxs = sums.cpu().numpy(), mins.cpu().numpy(), maxs.cpu().numpy()
+    world = dist.get_world_size()
+    sums, mins, maxs, ints = sums.cpu().numpy(), mins.cpu().numpy(), maxs.cpu().numpy(), [int(x) for x in ints.tolist()]
     for a, f in enumerate(fns):
-        block.longs[a][0] = int(sums[n + a])
-        block.doubles[a][0] = mins[a] if f == "MIN" else maxs[a] if f == "MAX" else sums[a] if f in ("SUM", "AVG") else float(sums[n + a])
+        block.longs[a][0] = ints[2 * n + a]
+        if f == "MIN":
+            block.doubles[a][0] = mins[a]
+        elif f == "MAX":
+            block.doubles[a][0] = maxs[a]
+        elif f in ("SUM", "AVG"):
+            block.doubles[a][0] = float(ints[a]) if ints[n + a] == world else sums[a]
+        else:
+            block.doubles[a][0] = float(ints[2 * n + a])
         if f in ("MIN", "MAX"):
             block.dict_ids[a][0] = -1   # ids are rank local unless the segments are bound to one domain
-    block.stats.num_docs_scanned = int(sums[2 * n])
+    _set_stats(block, ints[3 * n:3 * n + 4])
     return block
 
 
