@@ -200,12 +200,14 @@ typedef struct {
 #define PB200_NODE_IDS_ON_DEVICE 1
 
 /* Aggregation functions accelerated on this path (core/query/aggregation/function/{Count,Sum,Min,Max,Avg,
- * DistinctCount,Percentile,Variance,FirstWithTime,LastWithTime}AggregationFunction.java).  PERCENTILE takes its
- * percentile through pb200_execute_args; the four VarianceAggregationFunction types take no argument (see
- * pb200_result_moments); FIRSTWITHTIME / LASTWITHTIME take their time column through pb200_execute_agg_args. */
+ * DistinctCount,Percentile,Variance,FirstWithTime,LastWithTime,DistinctSum,DistinctAvg}AggregationFunction.java).
+ * PERCENTILE takes its percentile through pb200_execute_args; the four VarianceAggregationFunction types and
+ * DISTINCTSUM / DISTINCTAVG take no argument (see pb200_result_moments and the DISTINCTSUM section below);
+ * FIRSTWITHTIME / LASTWITHTIME take their time column through pb200_execute_agg_args. */
 enum { PB200_AGG_COUNT = 0, PB200_AGG_SUM = 1, PB200_AGG_MIN = 2, PB200_AGG_MAX = 3, PB200_AGG_AVG = 4,
        PB200_AGG_DISTINCTCOUNT = 5, PB200_AGG_PERCENTILE = 6, PB200_AGG_VARPOP = 7, PB200_AGG_VARSAMP = 8,
-       PB200_AGG_STDDEVPOP = 9, PB200_AGG_STDDEVSAMP = 10, PB200_AGG_FIRSTWITHTIME = 11, PB200_AGG_LASTWITHTIME = 12 };
+       PB200_AGG_STDDEVPOP = 9, PB200_AGG_STDDEVSAMP = 10, PB200_AGG_FIRSTWITHTIME = 11, PB200_AGG_LASTWITHTIME = 12,
+       PB200_AGG_DISTINCTSUM = 13, PB200_AGG_DISTINCTAVG = 14 };
 
 typedef struct {
   int32_t function; /* PB200_AGG_* */
@@ -380,6 +382,20 @@ int64_t pb200_result_histogram(const pb200_result* result, int32_t agg, int32_t 
 int32_t pb200_result_moments(const pb200_result* result, int32_t agg, int32_t row, int64_t* n, int64_t* c_mant,
                              int32_t* c_exp, int32_t* e, uint64_t* s1, uint64_t* s2_lo, uint64_t* s2_hi);
 
+/* ---- DISTINCTSUM / DISTINCTAVG: exact sums over DISTINCTCOUNT's value sets (DESIGN.md section 3.14) ------------------ */
+/* PB200_AGG_DISTINCTSUM / DISTINCTAVG through any pb200_execute* entry point (no argument).  Over S, the set of distinct
+ * values of the column in the group's matched rows (the set DISTINCTCOUNT counts; -0.0 and 0.0 are two members, all NaNs
+ * one): DISTINCTSUM is the exact sum of S rounded once to the nearest double (0.0 for an empty S), DISTINCTAVG that sum
+ * divided by |S| rounded once (-inf for an empty S).  NaN in S, or both infinities, give NaN; otherwise an infinity in S
+ * gives that infinity.  A column qualifies when it carries dictIds and its dictionary is INT or LONG, or FLOAT / DOUBLE
+ * with every finite value j * 2^e for one exponent e and an integer |j| < 2^63 (integral values, halves: yes; 0.01-steps:
+ * no).  Several of these functions and DISTINCTCOUNT over one column share one bitset.
+ * Results: pb200_result_agg gives the value (double column) and |S| (long column); pb200_result_distinct the dictId set,
+ * as for DISTINCTCOUNT; ORDER BY and HAVING compare the double.
+ * PB200_E_UNSUPPORTED (the caller runs the stock operator): STRING columns, raw columns streamed as 32-bit values, FLOAT /
+ * DOUBLE dictionaries off such a grid, the DISTINCTCOUNT bitset budget; a PB200_Q_MERGE_SEGMENTS submission needs the
+ * column's dictionary to be the same in every segment.  Like DISTINCTCOUNT they are not reduced across GPUs on the device. */
+
 /* ---- selection: SELECT columns WHERE ... [ORDER BY columns] LIMIT n (SelectionOnlyOperator, SelectionOrderByOperator) -- */
 /* Without order items: per segment, the first `limit` matching docs in doc-id order with the values of the selected
  * columns.  With PB200_Q_MERGE_SEGMENTS one result: the segments are taken in submission order and each contributes a
@@ -524,7 +540,8 @@ int32_t pb200_result_group_keys(const pb200_result* result, int32_t* out);
 int32_t pb200_result_agg(const pb200_result* result, int32_t agg, double* out_double, int64_t* out_long);
 /* MIN/MAX as dictIds (dict-encoded columns; -1 when empty), for exact value lookup on the caller's side */
 int32_t pb200_result_agg_dict_ids(const pb200_result* result, int32_t agg, int32_t* out);
-/* DISTINCTCOUNT: the dictId set of row `row` (ascending); returns the count (or < 0 on error), writes <= capacity */
+/* DISTINCTCOUNT, DISTINCTSUM, DISTINCTAVG: the dictId set of row `row` (ascending); returns the count (or < 0 on error),
+ * writes <= capacity */
 int64_t pb200_result_distinct(const pb200_result* result, int32_t agg, int32_t row, int32_t* out, int64_t capacity);
 /* Everything of a result in ONE call (a JNI / ctypes round trip per accessor adds up when many small per-segment results
  * are read): keys [rows x num_group_by] (may be NULL), doubles / longs / dict_ids [num_aggs x rows] each (row-major by

@@ -172,7 +172,7 @@ typedef struct {
   const pb200h_agg* aggs;
   int32_t num_groups_limit;
   int32_t max_initial_result_holder_capacity;
-  int32_t merge_segments; /* 1: device-side combine (group-by / MIN / MAX / DISTINCTCOUNT columns must have identical
+  int32_t merge_segments; /* 1: device-side combine (group-by / MIN / MAX / DISTINCT* columns must have identical
                              dictionaries in all segments -- bind them to a domain -- else PB200_E_UNSUPPORTED);
                              2: combine and defer the group extraction (PB200_Q_DEFER_FINALIZE) */
   int32_t skip_star_tree; /* query option useStarTree=false */
@@ -266,7 +266,7 @@ int32_t pb200h_execute_distinct(pb200_ctx* ctx, const pb200h_query* query, const
 /* The result as the server -> broker wire format: DataTableImplV4 bytes (pinot-common/.../datatable/DataTableImplV4.java:49-81)
  * exactly as GroupByResultsBlock.getDataTable() / AggregationResultsBlock.getDataTable() build them for the same rows
  * (GroupByResultsBlock.java:186-236): typed group-key values (STRING keys through the DataTable's own string dictionary),
- * COUNT as LONG, SUM / MIN / MAX as DOUBLE, AVG as OBJECT AvgPair, DISTINCTCOUNT as OBJECT value set, + the execution
+ * COUNT as LONG, SUM / MIN / MAX as DOUBLE, AVG as OBJECT AvgPair, DISTINCTCOUNT / DISTINCTSUM / DISTINCTAVG as OBJECT value set, + the execution
  * statistics as metadata.  `segment` supplies the dictionaries the result's ids refer to (any segment of a merged
  * result: they share dictionaries).  Returns the size (or the size needed when out == NULL), < 0 on error.
  * A result filtered by HAVING is PB200_E_UNSUPPORTED: a server's DataTable never carries rows HAVING removed. */

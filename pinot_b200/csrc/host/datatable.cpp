@@ -21,7 +21,8 @@
 //
 // The rows come from a pb200_result (merged over the server's segments by the device-side combine): group keys are
 // decoded through the (domain) dictionaries of the segment, intermediates are COUNT -> LONG, SUM / MIN / MAX -> DOUBLE,
-// AVG -> OBJECT(AvgPair), DISTINCTCOUNT -> OBJECT(value set) -- AggregationFunction.getIntermediateResultColumnType().
+// AVG -> OBJECT(AvgPair), DISTINCTCOUNT / DISTINCTSUM / DISTINCTAVG -> OBJECT(value set) --
+// AggregationFunction.getIntermediateResultColumnType().
 // A JVM wraps these bytes with DataTableFactory.getDataTable(ByteBuffer) instead of building Key / Record objects.
 #include <algorithm>
 #include <cstring>
@@ -53,6 +54,8 @@ const char* fn_name(int fn) {
     case PB200_AGG_MIN: return "min";
     case PB200_AGG_MAX: return "max";
     case PB200_AGG_AVG: return "avg";
+    case PB200_AGG_DISTINCTSUM: return "distinctsum";
+    case PB200_AGG_DISTINCTAVG: return "distinctavg";
     default: return "distinctcount";
   }
 }
@@ -121,7 +124,7 @@ extern "C" int64_t pb200h_result_to_datatable(const pb200h_query* q, const pb200
       agg_cols[a] = &seg->cols[ci].decode_column();
     }
     names.push_back(std::string(fn_name(fn)) + "(" + (q->aggs[a].column ? q->aggs[a].column : "*") + ")");
-    types.push_back(fn == PB200_AGG_COUNT ? "LONG" : (fn == PB200_AGG_AVG || fn == PB200_AGG_DISTINCTCOUNT) ? "OBJECT" : "DOUBLE");
+    types.push_back(fn == PB200_AGG_COUNT ? "LONG" : (fn == PB200_AGG_AVG || fn == PB200_AGG_DISTINCTCOUNT || pb200::is_distinct_value_fn(fn)) ? "OBJECT" : "DOUBLE");
     width.push_back(8);
   }
   // ---- rows ----

@@ -296,6 +296,10 @@ pb200_result* host_result(const pb200h_segment& seg, const pb200h_query& q, bool
       case PB200_AGG_FIRSTWITHTIME: case PB200_AGG_LASTWITHTIME: d = -INFINITY; break;   // likewise: no row, dictId -1
       case PB200_AGG_VARPOP: case PB200_AGG_VARSAMP: case PB200_AGG_STDDEVPOP: case PB200_AGG_STDDEVSAMP:
         d = -INFINITY; R->mom.on[a] = true; break;       // likewise: n = 0, zero moments
+      case PB200_AGG_DISTINCTSUM: case PB200_AGG_DISTINCTAVG:   // only reached for an empty match: S is empty
+        d = ag.function == PB200_AGG_DISTINCTSUM ? 0.0 : -INFINITY;
+        R->distinct[a].push_back({});
+        break;
       case PB200_AGG_DISTINCTCOUNT: {
         std::vector<int32_t> ids;
         if (!empty) for (int i = 0; i < c->cardinality; i++) ids.push_back(c->to_device_id(i));
@@ -811,6 +815,11 @@ extern "C" int32_t pb200h_execute_agg_args(pb200_ctx* ctx, const pb200h_query* q
   for (int a = 0; a < q->num_aggs; a++)
     if (pb200::is_moments_fn(q->aggs[a].function) && any_clause) {   // the per-clause submissions carry no moments
       set_error("VAR/STDDEV in a query with FILTER (WHERE ...) clauses is not accelerated");
+      return PB200_E_UNSUPPORTED;
+    }
+  for (int a = 0; a < q->num_aggs; a++)
+    if (pb200::is_distinct_value_fn(q->aggs[a].function) && any_clause) {   // nor the finalized sums of value sets
+      set_error("DISTINCTSUM/DISTINCTAVG in a query with FILTER (WHERE ...) clauses is not accelerated");
       return PB200_E_UNSUPPORTED;
     }
   if (q->agg_filter_count && q->agg_filter_start && q->agg_filter_nodes)

@@ -795,13 +795,17 @@ namespace {
 // kMaxAggs selected dictIds and kMaxAggs value counts, u32 each.
 // Then (aggregation-only FIRST/LASTWITHTIME) per result kMaxAggs winning keys and kMaxAggs time values, u64 each, and
 // kMaxAggs data dictIds, u32 each.
+// Then (aggregation-only DISTINCTSUM / DISTINCTAVG) per result and aggregation the finalized state, kDsWords u64 each.
 struct AccumLayout {
-  size_t verify_off = 0, pct_off = 0, wt_off = 0, bytes = 0;
+  size_t verify_off = 0, pct_off = 0, wt_off = 0, ds_off = 0, bytes = 0;
   int nres = 0;
   AccumLayout() = default;
-  AccumLayout(int nres, bool pct, bool wt)
+  AccumLayout(int nres, bool pct, bool wt, bool ds)
       : verify_off(sizeof(AggAccum) * nres), pct_off(verify_off + 32ull * nres), wt_off(pct_off + (pct ? 8ull * kMaxAggs * nres : 0)),
-        bytes(wt_off + (wt ? 20ull * kMaxAggs * nres : 0)), nres(nres) {}
+        ds_off(wt_off + (wt ? 20ull * kMaxAggs * nres : 0)), bytes(ds_off + (ds ? 8ull * kDsWords * kMaxAggs * nres : 0)), nres(nres) {}
+  unsigned long long* ds(void* b, int r, int a) const {
+    return reinterpret_cast<unsigned long long*>(static_cast<unsigned char*>(b) + ds_off) + ((size_t)r * kMaxAggs + a) * kDsWords;
+  }
   static AggAccum* records(void* b) { return static_cast<AggAccum*>(b); }
   unsigned long long* verify(void* b) const { return reinterpret_cast<unsigned long long*>(static_cast<unsigned char*>(b) + verify_off); }
   uint32_t* pct(void* b) const { return reinterpret_cast<uint32_t*>(static_cast<unsigned char*>(b) + pct_off); }
@@ -816,7 +820,7 @@ void release_tables(pb200_result& R, bool keep_hist) {
   if (d.ctx) {
     dev_free(d.ctx, d.i64_block); dev_free(d.ctx, d.f64_block); dev_free(d.ctx, d.u32max_block); dev_free(d.ctx, d.u32min_block);
     dev_free(d.ctx, d.hkeys); dev_free(d.ctx, d.hctl);
-    for (int a = 0; a < kMaxAggs; a++) { dev_free(d.ctx, d.dbits[a]); d.dbits[a] = nullptr; }
+    for (int a = 0; a < kMaxAggs; a++) { dev_free(d.ctx, d.dbits[a]); d.dbits[a] = nullptr; dev_free(d.ctx, d.ds_state[a]); d.ds_state[a] = nullptr; }
     d.i64_block = d.f64_block = d.u32max_block = d.u32min_block = nullptr;
     d.hkeys = nullptr; d.hctl = nullptr;
     d.live = false;
@@ -895,7 +899,9 @@ struct ScanCall {
   int bind_accumulators() {
     bool any_pct = false;
     for (int a = 0; a < plan.q.num_aggs; a++) any_pct |= plan.pct_rep[a] >= 0;
-    acc = AccumLayout(plan.nres, any_pct && !plan.group_by, plan.any_wt && !plan.group_by);
+    bool any_ds = false;
+    for (int a = 0; a < plan.q.num_aggs; a++) any_ds |= plan.ds_rep[a] >= 0;
+    acc = AccumLayout(plan.nres, any_pct && !plan.group_by, plan.any_wt && !plan.group_by, any_ds && !plan.group_by);
     if (int rc = pinned_alloc(ctx, 2 * acc.bytes, &pin.p, &pin.bytes)) return rc;
     unsigned char* const init = static_cast<unsigned char*>(pin.p);
     back = init + acc.bytes;
@@ -987,6 +993,8 @@ struct ScanCall {
       d.agg_cols.push_back(q.aggs[a].slot < 0 ? nullptr : &seg->cols[query->aggs[a].column]);
       d.mom_first[a] = plan.mom_first[a];
       if (plan.mom_first[a] >= 0) d.mom_e[a] = seg->cols[query->aggs[a].column].moments->grid.e;
+      d.ds_rep[a] = plan.ds_rep[a];
+      if (plan.ds_rep[a] >= 0) d.ds_e[plan.ds_rep[a]] = seg->cols[query->aggs[a].column].moments->ds_e;
     }
     d.pack_agg = t.carrier.agg; d.pack_shift = t.carrier.shift; d.pack_vmin = t.carrier.vmin;
     d.reduce_world = t.reduce_world;
@@ -1018,11 +1026,15 @@ struct ScanCall {
         else d.isum[a] = (long long*)d.i64_block + off;
       } else if (fn == PB200_AGG_MIN) d.gmin[a] = (uint32_t*)d.u32min_block + off;
       else if (fn == PB200_AGG_MAX) d.gmax[a] = (uint32_t*)d.u32max_block + off;
-      else if (fn == PB200_AGG_DISTINCTCOUNT) {  // one dictId bitset per group / slot
+      else if (owns_bitset(plan, a)) {  // one dictId bitset per group / slot
         const size_t bytes = (size_t)t.dwords[a] * t.groups * 4;
         if ((rc = dev_alloc(ctx, bytes, (void**)&d.dbits[a]))) return rc;
         PB200_CUDA(cudaMemsetAsync(d.dbits[a], 0, bytes, st));
         d.dwords[a] = t.dwords[a];
+      }
+      if (is_distinct_value_fn(fn)) {   // the set's finalized state per group / slot (pb200_extract.cu runs the finalize)
+        unsigned long long*& state = d.ds_state[plan.ds_rep[a]];
+        if (!state && (rc = dev_alloc(ctx, (size_t)t.groups * kDsWords * 8, (void**)&state))) return rc;
       } else if (fn == PB200_AGG_PERCENTILE) {  // one dictId histogram per group / slot (owner), a dictId per entry (each)
         if (t.hist_per_group[a]) {
           const size_t entries = (size_t)t.hist_per_group[a] * t.groups;
@@ -1090,6 +1102,24 @@ struct ScanCall {
         if (int rc = withtime_finalize(ctx, st, job, wsegs, nseg)) return rc;
       }
     }
+    return PB200_OK;
+  }
+
+  // 8c. DISTINCTSUM / DISTINCTAVG, aggregation only: each result's set -> its state in the accumulator block (slot of the
+  //     aggregation b whose bitset holds it, once per set), queued behind the scan (group-by: the extraction finalizes)
+  int finalize_distinct_sums() {
+    if (plan.group_by) return PB200_OK;
+    for (int r = 0; r < plan.nres; r++)
+      for (int a = 0; a < plan.q.num_aggs; a++) {
+        const int b = plan.ds_rep[a];
+        bool done = false;
+        for (int x = 0; x < a && !done; x++) done = plan.ds_rep[x] == b;
+        if (b < 0 || done) continue;
+        const DeviceColumn& c = segments[plan.merge ? 0 : r]->cols[query->aggs[a].column];
+        const DistinctSumJob job{static_cast<const uint32_t*>(distinct_bufs[r][b]->p), plan.distinct_words[r][b], 1, true,
+                                 c.dict_native, c.stored_type, c.moments->ds_e, acc.ds(accum.p, r, b)};
+        if (int rc = distinct_sum_finalize(ctx, st, job, temps)) return rc;
+      }
     return PB200_OK;
   }
 
@@ -1182,11 +1212,16 @@ struct ScanCall {
       const uint32_t x = acc.wt_ids(back, r)[a];
       if (acc_r.count == 0 || x == ~0u) v->d = -INFINITY;
       else { v->id = (int32_t)x; v->d = c->dict_host.empty() ? (double)v->id : value_of(x); v->l = acc.wt_time(back, r)[a]; }
-    } else if (fn == PB200_AGG_DISTINCTCOUNT) {
-      std::vector<uint32_t> bits(plan.distinct_words[r][a]);
-      PB200_CUDA(cudaMemcpy(bits.data(), distinct_bufs[r][a]->p, bits.size() * 4, cudaMemcpyDeviceToHost));
+    } else if (fn == PB200_AGG_DISTINCTCOUNT || is_distinct_value_fn(fn)) {
+      const int b = fn == PB200_AGG_DISTINCTCOUNT ? a : plan.ds_rep[a];   // the aggregation whose bitset holds the set
+      std::vector<uint32_t> bits(plan.distinct_words[r][b]);
+      PB200_CUDA(cudaMemcpy(bits.data(), distinct_bufs[r][b]->p, bits.size() * 4, cudaMemcpyDeviceToHost));
       R.distinct[a].push_back(bitset_ids(bits.data(), bits.size()));
       v->l = (int64_t)R.distinct[a].back().size(); v->d = (double)v->l;
+      if (is_distinct_value_fn(fn)) {
+        const unsigned long long* ds = acc.ds(back, r, b);
+        memcpy(&v->d, ds + ds_final_word(fn), 8);   // rounded once by the finalize
+      }
     }
     return PB200_OK;
   }
@@ -1268,6 +1303,7 @@ static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment*
   if (int rc = c.launch()) return rc;
   if (int rc = c.finalize_percentiles()) return rc;
   if (int rc = c.finalize_withtime()) return rc;
+  if (int rc = c.finalize_distinct_sums()) return rc;
   if (int rc = c.read_back_and_verify()) return rc;   // kRetryWithoutCountCarrier: ~ScanCall frees this attempt's tables
   if (int rc = c.fill_results_and_extract(order, having)) return rc;
   c.hand_out(results);

@@ -74,6 +74,7 @@ struct ExtractDesc {
   const long long* mom[kMaxAggs][3]; // VAR / STDDEV: the K, H, L limb sum tables (pb200_moments.h)
   int32_t mom_e[kMaxAggs];           // ... and the grid exponent of the column
   unsigned long long off_mom[kMaxAggs];  // ... {s1, s2 low, s2 high} per row, for pb200_result_moments
+  const unsigned long long* ds[kMaxAggs];  // DISTINCTSUM / DISTINCTAVG: the finalized state per table entry (kDsWords u64)
   const uint8_t* keep;               // HAVING only: bit j of byte i = entry 8i + j is a row (NULL: every non_empty() entry is)
 };
 
@@ -189,6 +190,10 @@ __device__ __forceinline__ void agg_values(const ExtractDesc& d, int a, long lon
   } else if (is_moments_fn(fn)) {  // exact moments from the group's limb sums and count, rounded once
     dv = moments_final(fn, moments_from_sums(cnt, d.mom[a][0][g], d.mom[a][1][g], d.mom[a][2][g]), d.mom_e[a]);
     lv = (long long)cnt;
+  } else if (is_distinct_value_fn(fn)) {  // rounded once by the finalize (pb200_distinct_sum.cu); no rounding here keeps the
+    const unsigned long long* st = d.ds[a] + (size_t)g * kDsWords;   // registers of the kernels every group-by query runs
+    dv = __longlong_as_double((long long)st[ds_final_word(fn)]);
+    lv = (long long)st[2];
   }
 }
 
@@ -374,7 +379,7 @@ static size_t layout_result(const pb200_result::Dense& d, ExtractDesc& e, size_t
     e.off_dbl[a] = take(8, rows);
     const bool wt = fn == PB200_AGG_FIRSTWITHTIME || fn == PB200_AGG_LASTWITHTIME;
     e.off_lng[a] = (fn == PB200_AGG_COUNT || fn == PB200_AGG_AVG || fn == PB200_AGG_SUM || fn == PB200_AGG_DISTINCTCOUNT ||
-                    fn == PB200_AGG_PERCENTILE || is_moments_fn(fn) || wt) ? take(8, rows) : kNoCol;
+                    fn == PB200_AGG_PERCENTILE || is_moments_fn(fn) || is_distinct_value_fn(fn) || wt) ? take(8, rows) : kNoCol;
     e.off_ids[a] = (fn == PB200_AGG_MIN || fn == PB200_AGG_MAX || fn == PB200_AGG_PERCENTILE || wt) ? take(4, rows) : kNoCol;
     e.off_mom[a] = is_moments_fn(fn) ? take(24, rows) : kNoCol;
   }
@@ -454,7 +459,7 @@ int extract_groups(pb200_ctx* ctx, pb200_result* const* Rs, int nres, cudaStream
       else if (is_moments_fn(fn)) {
         for (int j = 0; j < 3; j++) e.mom[a][j] = d.isum[d.mom_first[a] + j];
         e.mom_e[a] = d.mom_e[a];
-      }
+      } else if (is_distinct_value_fn(fn)) e.ds[a] = d.ds_state[d.ds_rep[a]];
       const DeviceColumn* c = d.agg_cols[a];
       e.dict[a] = (c && vk != VAL_RAW_I32 && !c->dict_host.empty()) ? c->dict_native : nullptr;
     }
@@ -523,6 +528,18 @@ int extract_groups(pb200_ctx* ctx, pb200_result* const* Rs, int nres, cudaStream
     if ((rc = dexist.alloc(8ull * nres))) return rc;
     for (int r = 0; r < nres; r++)
       if (Rs[r]->having.num_nodes > 0) descs[r].keep = static_cast<const uint8_t*>(dkeep.p) + 256ull * descs[r].first_chunk;
+  }
+  // ---- DISTINCTSUM / DISTINCTAVG: every table entry's bitset row -> its state, before HAVING, the order keys and the rows
+  //      read it (entries without rows have an empty row and finalize to the empty state) ----
+  std::vector<std::unique_ptr<DevBufRaw>> ds_temps;
+  for (int r = 0; r < nres; r++) {
+    const pb200_result::Dense& d = Rs[r]->dense;
+    for (int b = 0; b < descs[r].nagg; b++) {   // one state per set: indexed by the aggregation whose bitset holds it
+      if (!d.ds_state[b]) continue;
+      const DeviceColumn& c = *d.agg_cols[b];
+      const DistinctSumJob job{d.dbits[b], d.dwords[b], d.groups, false, c.dict_native, c.stored_type, d.ds_e[b], d.ds_state[b]};
+      if ((rc = distinct_sum_finalize(ctx, st, job, ds_temps))) return rc;
+    }
   }
   const ExtractDesc* ddescs = (const ExtractDesc*)ddesc.p;
   PB200_CUDA(cudaMemcpyAsync(ddesc.p, descs.data(), sizeof(ExtractDesc) * nres, cudaMemcpyHostToDevice, st));
@@ -616,14 +633,22 @@ int extract_groups(pb200_ctx* ctx, pb200_result* const* Rs, int nres, cudaStream
     }
     // DISTINCTCOUNT with GROUP BY: the groups' bitset rows are gathered on the device and decoded here into dictId lists
     // (what extractGroupByResult's value-set conversion starts from, BaseDistinctAggregateAggregationFunction :306-321)
+    // (DISTINCTSUM / DISTINCTAVG: the same from the bitset that holds their set, decoded once per bitset; their columns
+    // already hold value and size)
+    std::vector<int> decoded(nagg, -1);   // the bitset aggregation a's set was decoded from
     for (int a = 0; a < nagg; a++) {
-      if (d.aggs[a].function != PB200_AGG_DISTINCTCOUNT || !d.dbits[a]) continue;
-      const size_t wpg = d.dwords[a], rows = v.rows;
+      const bool value_fn = is_distinct_value_fn(d.aggs[a].function);
+      const int b = value_fn ? d.ds_rep[a] : a;
+      if ((d.aggs[a].function != PB200_AGG_DISTINCTCOUNT && !value_fn) || b < 0 || !d.dbits[b]) continue;
+      decoded[a] = b;
+      const int same = (int)(std::find(decoded.begin(), decoded.begin() + a, b) - decoded.begin());
+      if (same < a) { R->distinct[a] = R->distinct[same]; continue; }
+      const size_t wpg = d.dwords[b], rows = v.rows;
       std::vector<uint32_t> bits(rows * wpg);
       if (rows) {
         DevBufRaw g(ctx);
         if ((rc = g.alloc(rows * wpg * 4))) return rc;
-        gather_bitset_rows_kernel<<<grid_for(ctx, (long long)(rows * wpg), 256), 256, 0, st>>>(d.dbits[a], reinterpret_cast<const uint32_t*>(out + e.off_idx), (long long)rows, (int)wpg, (uint32_t*)g.p);
+        gather_bitset_rows_kernel<<<grid_for(ctx, (long long)(rows * wpg), 256), 256, 0, st>>>(d.dbits[b], reinterpret_cast<const uint32_t*>(out + e.off_idx), (long long)rows, (int)wpg, (uint32_t*)g.p);
         PB200_CUDA(cudaMemcpyAsync(bits.data(), g.p, rows * wpg * 4, cudaMemcpyDeviceToHost, st));
         PB200_CUDA(cudaStreamSynchronize(st));
       }
@@ -632,7 +657,7 @@ int extract_groups(pb200_ctx* ctx, pb200_result* const* Rs, int nres, cudaStream
       double* dsz = const_cast<double*>(v.dbl[a]);
       for (size_t i = 0; i < rows; i++) {
         R->distinct[a][i] = bitset_ids(bits.data() + i * wpg, wpg);
-        sizes[i] = (int64_t)R->distinct[a][i].size(); dsz[i] = (double)sizes[i];
+        if (!value_fn) { sizes[i] = (int64_t)R->distinct[a][i].size(); dsz[i] = (double)sizes[i]; }
       }
     }
   }

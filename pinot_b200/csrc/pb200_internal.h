@@ -13,6 +13,7 @@
 
 #include "../../include/pinot_b200.h"
 #include "pb200_desc.h"
+#include "pb200_distinct_sum.h"
 #include "pb200_moments.h"
 
 namespace pb200 {
@@ -36,7 +37,8 @@ constexpr int kMaxTileRows = 8192;
 // words a device doc mask needs: whole tiles + one spare tile (the kernel reads masks tile-wise) + a tail
 inline size_t doc_mask_words(long long num_docs) { return (((size_t)num_docs + kMaxTileRows - 1) / kMaxTileRows + 1) * (kMaxTileRows / 32) + 8; }
 
-// Limb dictionaries of one device dictionary for VAR / STDDEV (pb200_moments.h, pb200_moments.cu): built on the first
+// Facts of one device dictionary that queries derive once: the DISTINCTSUM / DISTINCTAVG grid (ds_state below), and
+// the limb dictionaries for VAR / STDDEV (pb200_moments.h, pb200_moments.cu): built on the first
 // query that needs them, under `mu`, and published with `ready` (release) before any launch reads them.  Shared by the
 // columns that share the dictionary (a domain's bound segments); freed with the last of them.
 struct MomentDict {
@@ -47,6 +49,10 @@ struct MomentDict {
   pb200_ctx* ctx = nullptr;
   uint32_t* limbs = nullptr;       // device: K, H, L arrays of `entries` u32 each, one allocation
   int entries = 0;
+  // DISTINCTSUM / DISTINCTAVG eligibility of the same dictionary (pb200_distinct_sum.h distinct_grid): evaluated on the
+  // host copy by the first query that needs it, under `mu`; 0 not yet, 1 eligible with exponent ds_e, -1 not eligible
+  std::atomic<int> ds_state{0};
+  int ds_e = 0;
   ~MomentDict();                   // pb200_moments.cu
 };
 
@@ -278,9 +284,15 @@ struct pb200_result {
     std::vector<unsigned long long> mult64;
     int mom_first[pb200::kMaxAggs];             // VAR / STDDEV: the first of the three limb sums (isum) of aggregation a, -1 if none
     int mom_e[pb200::kMaxAggs] = {};            // ... and the grid exponent of its column
-    Dense() { std::fill(mom_first, mom_first + pb200::kMaxAggs, -1); }
+    Dense() { std::fill(mom_first, mom_first + pb200::kMaxAggs, -1); std::fill(ds_rep, ds_rep + pb200::kMaxAggs, -1); }
     uint32_t* dbits[pb200::kMaxAggs] = {};      // DISTINCTCOUNT with GROUP BY: per-group dictId bitsets, dwords[a] words each
     uint32_t dwords[pb200::kMaxAggs] = {};
+    // DISTINCTSUM / DISTINCTAVG (pb200_distinct_sum.h): the aggregation b whose bitset holds the set (-1: neither
+    // function); indexed by b, the grid exponent and the set's finalized state per table entry (kDsWords u64 each,
+    // device), shared by every function that reads the set
+    int ds_rep[pb200::kMaxAggs];
+    int ds_e[pb200::kMaxAggs] = {};
+    unsigned long long* ds_state[pb200::kMaxAggs] = {};
     unsigned long long* hkeys = nullptr;        // hash table keys (NULL: dense table indexed by raw key)
     uint32_t* hctl = nullptr;                   // [0] inserted, [1] overflow
     std::vector<int> cards;
@@ -383,6 +395,19 @@ cudaError_t reencode_column(pb200_ctx* ctx, cudaStream_t st, const uint32_t* src
 // pb200_moments.cu: builds (once per device dictionary) the limb dictionaries of every VAR / STDDEV column of the query
 // that has dictIds, before it is planned; columns the planner refuses are skipped
 int moments_prepare(pb200_ctx* ctx, const pb200_query* query, pb200_segment* const* segments, int nseg);
+// pb200_distinct_sum.cu: DISTINCTSUM / DISTINCTAVG states (kDsWords u64 per row, pb200_distinct_sum.h) of `rows` bitset
+// rows of `words` words each, queued on `st`.  single: one row of an aggregation-only result (a grid-wide pass; its
+// scratch goes to `temps`).
+struct DistinctSumJob {
+  const uint32_t* bits;
+  size_t words;
+  long long rows;
+  bool single;
+  const void* dict;           // the column's device dictionary (INT: biased)
+  int stored_type, e;
+  unsigned long long* out;
+};
+int distinct_sum_finalize(pb200_ctx* ctx, cudaStream_t st, const DistinctSumJob& job, std::vector<std::unique_ptr<DevBufRaw>>& temps);
 // pb200_synth.cu
 int synth_build_inverted(pb200_ctx* ctx, cudaStream_t stream, DeviceColumn& col, long long num_docs);
 }  // namespace pb200

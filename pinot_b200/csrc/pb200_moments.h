@@ -68,30 +68,43 @@ PB200_MHD int bitlen128(u128 x) {
 #endif
 }
 
-// round-to-nearest-even of num / den * 2^scale (num > 0, 0 < den < 2^64) by long division: the quotient is developed bit by
-// bit until it holds at least 55 significant bits; the remainder is the sticky bit
-PB200_MHD double div_round(u128 num, unsigned long long den, int scale) {
+// round-to-nearest-even of (neg ? -1 : 1) * num / den * 2^scale (0 < num < 2^128, 0 < den < 2^64), correctly rounded into
+// the subnormal range and to +-inf on overflow.  The quotient is developed bit by bit until it holds at least 55
+// significant bits (the remainder is the sticky bit); then exactly the bits the result can hold are kept -- 53, or fewer
+// where the result is subnormal -- and rounded once.
+PB200_MHD double round_dyadic(bool neg, u128 num, unsigned long long den, int scale) {
   u128 q = 0, r = 0;
   for (int i = 127; i >= 0; --i) {
     r = (r << 1) | ((num >> i) & 1u);
     q <<= 1;
     if (r >= den) { r -= den; q |= 1u; }
   }
-  int len = bitlen128(q), exp = 0;
-  while (len < 55) {  // fractional quotient bits
+  int len = bitlen128(q), lsb = scale;   // value = (q + r / den) * 2^lsb
+  while (len < 55) {
     r <<= 1;
     q <<= 1;
     if (r >= den) { r -= den; q |= 1u; }
-    --exp;
+    --lsb;
     len = bitlen128(q);
   }
-  int sh = len - 53;  // >= 2
-  unsigned long long keep = (unsigned long long)(q >> sh);
-  const u128 low = q & (((u128)1 << sh) - 1u), half = (u128)1 << (sh - 1);
-  if (low > half || (low == half && (r != 0 || (keep & 1ull)))) ++keep;
-  if (keep == (1ull << 53)) { keep >>= 1; ++sh; }
-  return ldexp((double)keep, sh + exp + scale);
+  int sh = len - 53;                           // bits dropped from q
+  if (lsb + sh < -1074) sh = -1074 - lsb;      // subnormal: the last kept bit weighs 2^-1074
+  double out;
+  if (sh > len) {
+    out = 0.0;                                 // below half the smallest subnormal
+  } else {
+    const unsigned long long keep0 = sh >= 128 ? 0ull : (unsigned long long)(q >> sh);
+    const u128 low = sh >= 128 ? q : (q & (((u128)1 << sh) - 1u)), half = (u128)1 << (sh - 1);
+    unsigned long long keep = keep0;
+    if (low > half || (low == half && (r != 0 || (keep & 1ull)))) ++keep;
+    if (keep == (1ull << 53)) { keep >>= 1; ++sh; }
+    out = ldexp((double)keep, lsb + sh);       // exact, or +inf beyond the largest double
+  }
+  return neg ? -out : out;
 }
+
+// the positive case (VAR / STDDEV)
+PB200_MHD double div_round(u128 num, unsigned long long den, int scale) { return round_dyadic(false, num, den, scale); }
 
 // The final value of function fn (PB200_AGG_VARPOP .. STDDEVSAMP) over moments m of values on grid exponent e
 PB200_MHD double moments_final(int fn, const Moments& m, int e) {

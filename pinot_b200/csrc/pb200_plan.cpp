@@ -162,6 +162,7 @@ struct ScanPlanner {
     q.num_segments = nseg; q.num_aggs = nagg; q.num_group_by = ngb;
     plan.pct_p.assign(nagg, std::numeric_limits<double>::quiet_NaN());
     plan.pct_rep.assign(nagg, -1);
+    plan.ds_rep.assign(nagg, -1);
     plan.wt_time.assign(nagg, -1);
     return PB200_OK;
   }
@@ -190,6 +191,40 @@ struct ScanPlanner {
     }
     plan.wt_time[a] = tc;
     plan.any_wt = true;
+    return PB200_OK;
+  }
+  // DISTINCTSUM / DISTINCTAVG: a column with dictIds whose dictionary is on one grid j * 2^e (pb200_distinct_sum.h) in
+  // every segment (evaluated once per device dictionary and cached with it), and the bitset it reads
+  int check_distinct_value(int a) {
+    const pb200_agg& ag = plan.aggs[a];
+    const char* name = ag.function == PB200_AGG_DISTINCTSUM ? "DISTINCTSUM" : "DISTINCTAVG";
+    for (int t = 0; t < nseg; t++) {
+      DeviceColumn& c = segments[t]->cols[ag.column];
+      if (c.stored_type == PB200_STRING) { set_error("%s over STRING column %d", name, ag.column); return PB200_E_UNSUPPORTED; }
+      if (c.bits > 31 || !c.dict_native || c.cardinality <= 0) { set_error("%s on raw column not accelerated", name); return PB200_E_UNSUPPORTED; }
+      MomentDict& md = *c.moments;
+      if (md.ds_state.load(std::memory_order_acquire) == 0) {
+        std::lock_guard<std::mutex> lock(md.mu);
+        if (md.ds_state.load(std::memory_order_relaxed) == 0) {
+          int e = 0;
+          const bool ok = c.dict_host.size() >= (size_t)c.cardinality * c.dict_width() &&
+                          distinct_grid(c.stored_type, c.dict_host.data(), c.cardinality, &e);
+          md.ds_e = e;
+          md.ds_state.store(ok ? 1 : -1, std::memory_order_release);
+        }
+      }
+      if (md.ds_state.load(std::memory_order_acquire) < 0) {
+        set_error("%s over column %d: its values in segment %d are not on one grid j * 2^e with |j| < 2^63: not accelerated", name, ag.column, t);
+        return PB200_E_UNSUPPORTED;
+      }
+    }
+    plan.ds_rep[a] = a;
+    for (int b = 0; b < a; b++) {   // share the bitset of an earlier DISTINCTCOUNT / DISTINCTSUM / DISTINCTAVG of the column
+      const int fb = plan.aggs[b].function;
+      if (plan.aggs[b].column != ag.column || (fb != PB200_AGG_DISTINCTCOUNT && !is_distinct_value_fn(fb))) continue;
+      plan.ds_rep[a] = fb == PB200_AGG_DISTINCTCOUNT ? b : plan.ds_rep[b];
+      break;
+    }
     return PB200_OK;
   }
   // ---- slots: filter scan columns, then group-by keys, then aggregation arguments ----
@@ -223,8 +258,12 @@ struct ScanPlanner {
       const pb200_agg& ag = plan.aggs[a];
       q.aggs[a] = AggDesc{ag.function, -1, VAL_NONE, 0};
       if (ag.function == PB200_AGG_COUNT || is_moments_fn(ag.function)) continue;   // VAR / STDDEV: read their limb sums
-      if (ag.function < 0 || (ag.function > PB200_AGG_PERCENTILE && !is_withtime_fn(ag.function))) { set_error("unknown aggregation function %d", ag.function); return PB200_E_INVALID; }
+      if (ag.function < 0 || (ag.function > PB200_AGG_PERCENTILE && !is_withtime_fn(ag.function) && !is_distinct_value_fn(ag.function))) { set_error("unknown aggregation function %d", ag.function); return PB200_E_INVALID; }
       if (ag.column < 0 || ag.column >= ncols) { set_error("aggregation column %d out of range", ag.column); return PB200_E_INVALID; }
+      if (is_distinct_value_fn(ag.function)) {
+        if (int rc = check_distinct_value(a)) return rc;
+        if (plan.ds_rep[a] != a) continue;   // reads another aggregation's bitset: no slot, no agg code
+      }
       if (is_withtime_fn(ag.function)) {
         // the scan streams the time column; the data column is read once per result or group by the finalize
         if (int rc = check_withtime(a, wt_args)) return rc;
@@ -629,6 +668,8 @@ struct ScanPlanner {
           const SlotDesc& sl = sd.slots[q.aggs[a].slot];
           if (plan.wt_time[a] >= 0)   // the value-kind field says which end of the key order wins
             sd.agg_code[n++] = agg_code(a, kFnWithTime, q.aggs[a].function == PB200_AGG_LASTWITHTIME ? WT_MAX : WT_MIN, sl.bits, sl.stage_words);
+          else if (plan.ds_rep[a] == a)   // DISTINCTSUM / DISTINCTAVG owning its set: the scan builds a DISTINCTCOUNT bitset
+            sd.agg_code[n++] = agg_code(a, PB200_AGG_DISTINCTCOUNT, q.aggs[a].val_kind, sl.bits, sl.stage_words);
           else
             sd.agg_code[n++] = agg_code(a, q.aggs[a].function, q.aggs[a].val_kind, sl.bits, sl.stage_words);
         }
@@ -691,7 +732,7 @@ struct ScanPlanner {
       plan.distinct_words.assign(plan.nres, std::vector<size_t>(q.num_aggs, 0));
       for (int r = 0; r < plan.nres; r++)
         for (int a = 0; a < q.num_aggs; a++)
-          if (q.aggs[a].function == PB200_AGG_DISTINCTCOUNT) plan.distinct_words[r][a] = ((size_t)1 << result_max_bits(r, plan.aggs[a].column)) / 32 + 1;
+          if (owns_bitset(plan, a)) plan.distinct_words[r][a] = ((size_t)1 << result_max_bits(r, plan.aggs[a].column)) / 32 + 1;
     } else {
       plan.tables.resize(plan.nres);
       for (int r = 0; r < plan.nres; r++)
@@ -750,7 +791,7 @@ struct ScanPlanner {
       // With one entry per 128 bytes the same reductions spread over >= 4096 chunks.  Costs table bytes (<= 2 MB each,
       // memset + extraction scan), no instruction in the kernel: the stride is folded into the key multipliers.
       bool any_bitset = false;
-      for (int a = 0; a < q.num_aggs; a++) any_bitset |= q.aggs[a].function == PB200_AGG_DISTINCTCOUNT || q.aggs[a].function == PB200_AGG_PERCENTILE;
+      for (int a = 0; a < q.num_aggs; a++) any_bitset |= owns_bitset(plan, a) || q.aggs[a].function == PB200_AGG_PERCENTILE;
       if (q.smem_groups == 0 && !any_bitset && tune.table_stride != 1) {
         long long s = 1;
         if (tune.table_stride > 1) s = tune.table_stride;
@@ -789,11 +830,12 @@ struct ScanPlanner {
       if (fn == PB200_AGG_SUM || fn == PB200_AGG_AVG) t.index[a] = (int)(sum_in_double(vk) ? fi++ : ii++);
       else if (fn == PB200_AGG_MIN) { t.index[a] = (int)ni++; if (!need_count && marks_groups(a) && t.exists_max < 0 && t.exists_min < 0) t.exists_min = a; }
       else if (fn == PB200_AGG_MAX) { t.index[a] = (int)xi++; if (!need_count && marks_groups(a) && t.exists_max < 0 && t.exists_min < 0) t.exists_max = a; }
-      else if (fn == PB200_AGG_DISTINCTCOUNT) {  // one dictId bitset per group / slot
+      else if (owns_bitset(plan, a)) {  // one dictId bitset per group / slot
         const DeviceColumn& c = seg->cols[plan.aggs[a].column];
         const unsigned long long words = ((unsigned long long)c.cardinality + 31) / 32;
         if (words * (unsigned long long)t.groups > (1ull << 28)) {
-          set_error("DISTINCTCOUNT with GROUP BY: %lld groups x %d dictIds exceed the device bitset budget", t.groups, c.cardinality);
+          set_error("%s with GROUP BY: %lld groups x %d dictIds exceed the device bitset budget",
+                    fn == PB200_AGG_DISTINCTCOUNT ? "DISTINCTCOUNT" : fn == PB200_AGG_DISTINCTSUM ? "DISTINCTSUM" : "DISTINCTAVG", t.groups, c.cardinality);
           return PB200_E_UNSUPPORTED;
         }
         t.dwords[a] = (uint32_t)words;
@@ -879,11 +921,11 @@ int plan_scan(const Tuning& tune, DeviceLimits lim, const pb200_query* query, pb
     for (int a = 0; a < nuser; a++) {
       const pb200_agg& ag = query->aggs[a];
       if (ag.function != PB200_AGG_MIN && ag.function != PB200_AGG_MAX && ag.function != PB200_AGG_DISTINCTCOUNT &&
-          ag.function != PB200_AGG_PERCENTILE && !is_moments_fn(ag.function)) continue;
+          ag.function != PB200_AGG_PERCENTILE && !is_moments_fn(ag.function) && !is_distinct_value_fn(ag.function)) continue;
       if (ag.column < 0 || ag.column >= ncols) continue;
       if (segments[0]->cols[ag.column].bits == 32 && !segments[0]->cols[ag.column].dict_native) continue;  // raw values, no ids
       const char* what = ag.function == PB200_AGG_DISTINCTCOUNT ? "DISTINCTCOUNT" : ag.function == PB200_AGG_PERCENTILE ? "PERCENTILE"
-                         : is_moments_fn(ag.function) ? "VAR/STDDEV" : "MIN/MAX";
+                         : is_moments_fn(ag.function) ? "VAR/STDDEV" : is_distinct_value_fn(ag.function) ? "DISTINCTSUM/DISTINCTAVG" : "MIN/MAX";
       if (!same_dictionary(segments, nseg, ag.column, what)) return PB200_E_UNSUPPORTED;
     }
     for (int a = 0; a < nuser && wt_args; a++) {   // FIRST/LASTWITHTIME: one dictionary for the data and the time column

@@ -79,6 +79,11 @@ struct ScanPlan {
   // first PERCENTILE of its column, the only one with an agg code (-1: not a PERCENTILE)
   std::vector<double> pct_p;
   std::vector<int> pct_rep;
+  // DISTINCTSUM / DISTINCTAVG (pb200_distinct_sum.h): the aggregation whose DISTINCTCOUNT bitset holds the set -- an
+  // earlier DISTINCTCOUNT / DISTINCTSUM / DISTINCTAVG of the column, or itself, the only one of them then with an agg code
+  // (the DISTINCTCOUNT code: the scan cannot tell them apart); -1: neither function.  The grid exponent of each result's
+  // dictionary is cached with it (MomentDict::ds_e)
+  std::vector<int> ds_rep;
   // VAR / STDDEV (pb200_moments.h): the caller's aggregations come first, then three internal INT-dictionary SUMs per
   // column (K, H, L limbs) -- q.num_aggs and every per-aggregation array count them all
   int num_user_aggs = 0;
@@ -108,6 +113,11 @@ constexpr int kHistWarpPrivateMaxCard = 64;
 int plan_scan(const Tuning& tune, DeviceLimits lim, const pb200_query* query, pb200_segment* const* segments, int nseg,
               bool allow_count_carrier, ScanPlan* out, const double* agg_args = nullptr, const pb200_agg_arg* wt_args = nullptr);
 inline bool is_withtime_fn(int fn) { return fn == PB200_AGG_FIRSTWITHTIME || fn == PB200_AGG_LASTWITHTIME; }
+// aggregation a of the plan sets bits in a DISTINCTCOUNT bitset of its own: a DISTINCTCOUNT, or the owner of a
+// DISTINCTSUM / DISTINCTAVG set
+inline bool owns_bitset(const ScanPlan& p, int a) {
+  return p.q.aggs[a].function == PB200_AGG_DISTINCTCOUNT || (p.ds_rep[a] == a);
+}
 
 // ---- selection (pb200_execute_selection): plan_scan with COUNT(*) as the only aggregation, plus the match mask ----
 constexpr long long kSelectPrefixRows = 1ll << 20;  // first pass of a selection without ORDER BY: at least this many docs

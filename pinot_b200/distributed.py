@@ -33,6 +33,8 @@ from __future__ import annotations
 import ctypes as C
 from typing import Dict, List, Optional, Sequence
 
+from .query import DISTINCT_SET_FUNCTIONS, distinct_final
+
 
 KINDS = {"i64": 0, "f64": 1, "u32max": 2, "u32min": 3}
 _TORCH_DTYPES = {"i64": "int64", "f64": "float64", "u32max": "int32", "u32min": "int32"}
@@ -235,7 +237,7 @@ def execute_and_combine(plan_maker_or_backend, segments: Sequence, query, dist, 
         raise UnsupportedQueryError(E_UNSUPPORTED, "VAR/STDDEV is not combined across GPUs")
     backend = plan_maker_or_backend if hasattr(plan_maker_or_backend, "finish") else DeviceBackend(plan_maker_or_backend)
     world = dist.get_world_size()
-    if any(a.function == "DISTINCTCOUNT" for a in query.aggregations):
+    if any(a.function in DISTINCT_SET_FUNCTIONS for a in query.aggregations):
         return _combine_with_sets(backend, segments, query, dist, dst)
     if not query.is_group_by:
         return _combine_scalars(backend, segments, query, dist, dst)
@@ -275,7 +277,7 @@ def _combine_with_sets(backend, segments, query, dist, dst):
     mine = {}
     for g in range(rows):
         key = () if block.num_groups < 0 else tuple(int(x) for x in block.keys[g])
-        mine[key] = [frozenset(int(d) for d in block.distinct[(a, g)]) if f == "DISTINCTCOUNT"
+        mine[key] = [frozenset(int(d) for d in block.distinct[(a, g)]) if f in DISTINCT_SET_FUNCTIONS
                      else (float(block.doubles[a][g]), int(block.longs[a][g]), int(block.dict_ids[a][g])) for a, f in enumerate(fns)]
     stats = (block.stats.num_docs_scanned, block.stats.num_entries_scanned_in_filter, block.stats.num_entries_scanned_post_filter,
              block.stats.num_total_docs)
@@ -291,7 +293,7 @@ def _combine_with_sets(backend, segments, query, dist, dst):
                 merged[key] = list(vals)
                 continue
             for a, f in enumerate(fns):
-                if f == "DISTINCTCOUNT":
+                if f in DISTINCT_SET_FUNCTIONS:
                     cur[a] = cur[a] | vals[a]
                 elif f in ("COUNT", "SUM", "AVG"):
                     cur[a] = (cur[a][0] + vals[a][0], cur[a][1] + vals[a][1], -1)
@@ -300,8 +302,12 @@ def _combine_with_sets(backend, segments, query, dist, dst):
                 else:
                     cur[a] = max(cur[a], vals[a], key=lambda t: t[0])
     keys_sorted = sorted(merged)   # raw-key order is not defined across tables: ascending ids, column 0 most significant
+    def set_final(a, id_set):   # DISTINCTCOUNT / DISTINCTSUM / DISTINCTAVG of a merged set of domain ids, exact
+        if fns[a] == "DISTINCTCOUNT":
+            return float(len(id_set))
+        return float(distinct_final(fns[a], [segments[0].dictionary_value(query.aggregations[a].column, d) for d in id_set]))
     if query.is_group_by and query.order_by:
-        keys_sorted = _order_and_trim(query, fns, keys_sorted, merged)
+        keys_sorted = _order_and_trim(query, fns, keys_sorted, merged, set_final)
     n, k = len(keys_sorted), len(query.group_by)
     out_keys = np.asarray(keys_sorted, dtype=np.int32).reshape(n, k) if query.is_group_by else np.zeros((0, 0), dtype=np.int32)
     doubles, longs, ids, distinct = [], [], [], {}
@@ -309,9 +315,9 @@ def _combine_with_sets(backend, segments, query, dist, dst):
         d, l, i = np.zeros(max(n, 1)), np.zeros(max(n, 1), dtype=np.int64), np.full(max(n, 1), -1, dtype=np.int32)
         for g, key in enumerate(keys_sorted):
             v = merged[key][a]
-            if f == "DISTINCTCOUNT":
+            if f in DISTINCT_SET_FUNCTIONS:
                 distinct[(a, g)] = np.asarray(sorted(v), dtype=np.int32)
-                d[g], l[g] = float(len(v)), len(v)
+                d[g], l[g] = set_final(a, v), len(v)
             else:
                 d[g], l[g], i[g] = v
         doubles.append(d[:n] if query.is_group_by else d); longs.append(l[:n] if query.is_group_by else l); ids.append(i[:n] if query.is_group_by else i)
@@ -324,7 +330,7 @@ def _combine_with_sets(backend, segments, query, dist, dst):
     return block
 
 
-def _order_and_trim(query, fns, keys, merged):
+def _order_and_trim(query, fns, keys, merged, set_final):
     """The merged rows (`keys` ascending, column 0 most significant) in ORDER BY order, trimmed as the dense route trims a
     merged result (plan_maker.order_spec): one stable sort per item, last item first, so rows equal on every item keep
     the key order -- the library's tie rule.  Values compare in the reference's order (query.value_order); a key column
@@ -335,8 +341,8 @@ def _order_and_trim(query, fns, keys, merged):
 
     def final(a, v):
         f = fns[a]
-        if f == "DISTINCTCOUNT":
-            return float(len(v))
+        if f in DISTINCT_SET_FUNCTIONS:
+            return set_final(a, v)
         if f == "COUNT":
             return float(v[1])
         if f == "AVG":

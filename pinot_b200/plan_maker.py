@@ -25,7 +25,7 @@ import numpy as np
 
 from . import _lib
 from ._lib import UnsupportedQueryError  # noqa: F401  (re-export)
-from .query import MOMENT_FUNCTIONS, WITHTIME_FUNCTIONS, WITHTIME_TYPES, Filter, Moments, QueryContext, postfix
+from .query import DISTINCT_SET_FUNCTIONS, MOMENT_FUNCTIONS, WITHTIME_FUNCTIONS, WITHTIME_TYPES, Filter, Moments, QueryContext, postfix
 
 
 class B200Context:
@@ -637,7 +637,7 @@ def _read_result(ctx: B200Context, handle, q: QueryContext, kind: int, keep_hand
     g = meta.num_groups
     rows = 1 if g < 0 else g
     k = len(q.group_by)
-    if views and not any(a.function in ("DISTINCTCOUNT", "PERCENTILE") + MOMENT_FUNCTIONS for a in q.aggregations):
+    if views and not any(a.function in DISTINCT_SET_FUNCTIONS + ("PERCENTILE",) + MOMENT_FUNCTIONS for a in q.aggregations):
         keys, doubles, longs, ids = _read_views(ctx, handle, q, meta)
         stats = ExecutionStatistics(meta.num_docs_scanned, meta.num_entries_scanned_in_filter,
                                     meta.num_entries_scanned_post_filter, meta.num_total_docs)
@@ -659,7 +659,7 @@ def _read_result(ctx: B200Context, handle, q: QueryContext, kind: int, keep_hand
         _lib.check(L.pb200_result_fetch(handle, _ptr(keys) if (g > 0 and k > 0) else None, _ptr(d_all), _ptr(l_all), _ptr(i_all)))
     doubles, longs, ids, distinct = list(d_all), list(l_all), list(i_all), {}
     for a, agg in enumerate(q.aggregations):
-        if agg.function == "DISTINCTCOUNT":
+        if agg.function in DISTINCT_SET_FUNCTIONS:
             for row in range(rows):
                 buf = np.zeros(int(l_all[a][row]), dtype=np.int32)
                 n = L.pb200_result_distinct(handle, a, row, _ptr(buf), len(buf))

@@ -11,8 +11,10 @@ Predicates are in VALUE space here (as the broker sends them); turning them into
 """
 from __future__ import annotations
 
+import math
 import struct
 from dataclasses import dataclass, field
+from fractions import Fraction
 from typing import List, Optional, Sequence, Union
 
 # InstancePlanMakerImplV2 defaults (core/plan/maker/InstancePlanMakerImplV2.java:68-82)
@@ -47,7 +49,7 @@ FilterNode = Union[Filter, Predicate]
 @dataclass
 class Aggregation:
     function: str  # COUNT | SUM | MIN | MAX | AVG | DISTINCTCOUNT | PERCENTILE | VARPOP | VARSAMP | STDDEVPOP | STDDEVSAMP
-    #                | FIRSTWITHTIME | LASTWITHTIME
+    #                | FIRSTWITHTIME | LASTWITHTIME | DISTINCTSUM | DISTINCTAVG
     column: Optional[str] = None  # None for COUNT(*)
     # FILTER (WHERE ...) clause of this function (QueryContext.getFilteredAggregationFunctions: Pair<function, FilterContext>);
     # evaluated together with the query's own filter (AggregationFunctionUtils.buildFilteredAggregationInfos)
@@ -136,6 +138,34 @@ def percentile_of_counts(counts) -> float:
         if k < 0:
             return float(v)
     raise AssertionError("unreachable")
+
+
+# functions whose intermediate is the set of distinct values (merged by union)
+DISTINCT_SET_FUNCTIONS = ("DISTINCTCOUNT", "DISTINCTSUM", "DISTINCTAVG")
+
+
+def distinct_final(function: str, values) -> float:
+    """The final DISTINCTCOUNT / DISTINCTSUM / DISTINCTAVG of a set of distinct values (DESIGN.md section 3.14):
+    the set size, or the exact sum (divided by the size) rounded once to the nearest double.  Empty: 0.0 / -inf.  NaN
+    in the set, or both infinities: NaN; otherwise an infinity in the set wins.  Integer members (INT / LONG values) stay
+    Python integers: a LONG beyond 2^53 is summed exactly, not rounded to a double first."""
+    if function == "DISTINCTCOUNT":
+        return len(values)
+    values = [v.item() if hasattr(v, "item") else v for v in values]
+    floats = [float(v) for v in values if isinstance(v, float)]
+    if any(math.isnan(v) for v in floats) or (math.inf in floats and -math.inf in floats):
+        return math.nan
+    if math.inf in floats or -math.inf in floats:
+        return math.inf if math.inf in floats else -math.inf
+    if not values:
+        return 0.0 if function == "DISTINCTSUM" else -math.inf
+    exact = sum((Fraction(v) for v in values), Fraction(0))
+    if function == "DISTINCTAVG":
+        exact /= len(values)
+    try:
+        return float(exact)   # numerator / denominator of ints: correctly rounded, subnormals included
+    except OverflowError:
+        return math.inf if exact > 0 else -math.inf
 
 
 MOMENT_FUNCTIONS = ("VARPOP", "VARSAMP", "STDDEVPOP", "STDDEVSAMP")

@@ -9,7 +9,9 @@ stays Java).  This module exists so the parity tests read like the reference's
     SELECT item[, item...] FROM table [WHERE cond] [GROUP BY col[, col...] [HAVING hcond]] [ORDER BY expr [ASC|DESC], ...]
            [LIMIT n]
     item  := COUNT(*) | FN(col) | PERCENTILE(col, p) | PERCENTILE<n>(col) | FIRSTWITHTIME(col, col, 'T')
-             | LASTWITHTIME(col, col, 'T') | col
+             | LASTWITHTIME(col, col, 'T') | COUNT(DISTINCT col) | SUM(DISTINCT col) | AVG(DISTINCT col) | col
+             (COUNT / SUM / AVG(DISTINCT col) are DISTINCTCOUNT / DISTINCTSUM / DISTINCTAVG(col), named
+             distinctcount(col) ...; MIN / MAX(DISTINCT col), COUNT(DISTINCT *) and COUNT(DISTINCT a, b) are refused)
              (FN also VAR_POP / VARPOP, VAR_SAMP / VARSAMP, STDDEV_POP / STDDEVPOP, STDDEV_SAMP / STDDEVSAMP; T is the
              data column's type, INT | LONG | FLOAT | DOUBLE | STRING | BOOLEAN, any case; the canonical text is
              lastwithtime(v,t,'INT'))
@@ -45,8 +47,10 @@ _TOKEN = re.compile(r"\s*(?:(\d+\.\d+(?:[eE][-+]?\d+)?|-?\d+\.\d+|-?\d+)|'((?:[^
 
 # VarianceAggregationFunction: both spellings of each function, the underscore one canonicalised to the other
 _ALIASES = {"VAR_POP": "VARPOP", "VAR_SAMP": "VARSAMP", "STDDEV_POP": "STDDEVPOP", "STDDEV_SAMP": "STDDEVSAMP"}
-_FUNCTIONS = {"COUNT", "SUM", "MIN", "MAX", "AVG", "DISTINCTCOUNT", "PERCENTILE", "VARPOP", "VARSAMP", "STDDEVPOP",
-              "STDDEVSAMP", *WITHTIME_FUNCTIONS} | set(_ALIASES)
+_FUNCTIONS = {"COUNT", "SUM", "MIN", "MAX", "AVG", "DISTINCTCOUNT", "DISTINCTSUM", "DISTINCTAVG", "PERCENTILE", "VARPOP",
+              "VARSAMP", "STDDEVPOP", "STDDEVSAMP", *WITHTIME_FUNCTIONS} | set(_ALIASES)
+# FN(DISTINCT col): the function Pinot's query compiler rewrites it into
+_DISTINCT_OF = {"COUNT": "DISTINCTCOUNT", "SUM": "DISTINCTSUM", "AVG": "DISTINCTAVG"}
 _PERCENTILE_N = re.compile(r"PERCENTILE(\d+)")
 
 # single-column transforms (DESIGN.md section 3.8): SQL name (lower case, no '_') -> canonical name
@@ -268,11 +272,24 @@ class _Parser:
         self.i += 1
         return v
 
+    def distinct_call(self, fn: str) -> str:
+        """After `FN(DISTINCT`: the column of COUNT / SUM / AVG(DISTINCT col), up to the `)`."""
+        if fn not in _DISTINCT_OF:
+            raise SqlError(f"{fn}(DISTINCT ...) is not supported (COUNT, SUM and AVG take DISTINCT)")
+        if self.take_op("*"):
+            raise SqlError(f"{fn}(DISTINCT *) is not valid")
+        col = self.column()
+        if self.take_op(","):
+            raise SqlError(f"{fn}(DISTINCT ...) over more than one column is not supported")
+        return col
+
     def aggregation_call(self) -> Aggregation:
         """An aggregation call after its name, e.g. `SUM(` + `m)`: the name token is at self.i - 2."""
         name = self.toks[self.i - 2][1]
         fn = _ALIASES.get(name.upper(), name.upper())
-        if fn.startswith("PERCENTILE"):
+        if self.take_kw("DISTINCT"):
+            agg = Aggregation(_DISTINCT_OF.get(fn, fn), self.distinct_call(fn))
+        elif fn.startswith("PERCENTILE"):
             col, pct = self.percentile_call(name)
             agg = Aggregation("PERCENTILE", col, arg=pct)
         elif fn in WITHTIME_FUNCTIONS:
@@ -524,6 +541,10 @@ def parse(sql: str, **options) -> QueryContext:
                 elif name.upper() in WITHTIME_FUNCTIONS:
                     expr = having_name(p.withtime_call(name.upper()))
                     p.expect_op(")")
+                elif p.take_kw("DISTINCT"):
+                    inner = p.distinct_call(name.upper())
+                    p.expect_op(")")
+                    expr = f"{_DISTINCT_OF[name.upper()].lower()}({inner})"
                 else:
                     inner = "*" if p.take_op("*") else p.column()
                     p.expect_op(")")
