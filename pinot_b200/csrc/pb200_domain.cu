@@ -316,7 +316,8 @@ extern "C" int32_t pb200_segment_bind_domain(pb200_ctx* ctx, pb200_segment* seg,
   for (auto& w : work) {
     DeviceColumn& c = seg->cols[w.col];
     const pb200_domain::Col& dc = *w.dc;
-    const bool identity = c.cardinality == dc.cardinality;  // a subset of equal size is the same dictionary
+    // a subset of equal size is the same dictionary; a stream registered wider than the domain's width is still repacked
+    const bool identity = c.cardinality == dc.cardinality && c.bits == dc.bits;
     if (!identity) {
       void* remap_dev = nullptr;
       void* nf = nullptr;
