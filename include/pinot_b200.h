@@ -497,6 +497,34 @@ typedef struct {
   double d;          /* DOUBLE literal */
 } pb200_transform_op;
 #define PB200_MAX_DERIVED_COLUMNS 32 /* derived columns per segment */
+
+/* ---- aggregations over expressions of two or more columns: SUM / AVG / MIN / MAX(a * b) (DESIGN.md section 3.15) ---- */
+/* One program per aggregation.  num_ops == 0: the aggregation reads its pb200_agg.column as usual.  Otherwise `ops` is a
+ * POSTFIX program of the arithmetic operations above (PLUS, MINUS, TIMES, DIVIDE, MOD, FLOOR, CEIL, ABS, LONG / DOUBLE
+ * literals; at most 16 operations) with 2 .. 8 PB200_T_COLUMN leaves whose `i` is a column id (the same column may
+ * appear twice), and pb200_agg.column is ignored. */
+typedef struct {
+  int32_t num_ops;
+  int32_t reserved;                 /* 0 */
+  const pb200_transform_op* ops;
+} pb200_expr_program;
+/* pb200_execute_agg_args with a pb200_expr_program per aggregation (exprs == NULL: exactly pb200_execute_agg_args).
+ * Semantics per matched row: every leaf value becomes a double (INT / LONG converted, LONG beyond 2^53 rounded to
+ * nearest), every operation is one IEEE-754 round-to-nearest step without FMA, MOD is fmod, x / 0 is +-inf or NaN.
+ * SUM adds the row values in IEEE arithmetic in any order (NaN when a row is NaN or both infinities occur; an exact zero
+ * is +0.0); AVG is that sum over the group's COUNT(*); MIN / MAX are the first / last row value in Double.compare order
+ * (-0.0 before 0.0, NaN after +inf), +inf / -inf without rows.  COUNT over a program is COUNT(*).  Leaves are INT, LONG,
+ * FLOAT or DOUBLE columns with a device dictionary or raw INT / FLOAT 32-bit values; each segment reads them through its
+ * own dictionary, so PB200_Q_MERGE_SEGMENTS needs no shared dictionary for them.
+ * Results: pb200_result_agg gives the value in the double column (SUM / AVG: the sum, with the count in the long column;
+ * MIN / MAX dictId -1); ORDER BY and HAVING compare it like a DOUBLE column's.
+ * PB200_E_INVALID: a malformed program or a column id out of range.  PB200_E_UNSUPPORTED (the caller runs the stock
+ * operator): a STRING leaf or one without dictIds or raw 32-bit values, a time function in the program, fewer than two
+ * or more than 8 column leaves, a function other than SUM / AVG / MIN / MAX / COUNT over a program, and with GROUP BY
+ * PB200_Q_DEFER_FINALIZE or reduce_world > 1. */
+int32_t pb200_execute_exprs(pb200_ctx* ctx, const pb200_query* query, const pb200_order_by* order, const pb200_agg_arg* args,
+                            const pb200_having* having, const pb200_expr_program* exprs, pb200_segment* const* segments,
+                            int32_t num_segments, pb200_result** results);
 /* Adds the derived column `program(source_column)` to the segment and returns its column id (the next free id, after
  * the registered and earlier derived columns).  The source must carry dictIds: INT / LONG / FLOAT / DOUBLE dictionaries,
  * raw columns whose dictionary was synthesised at load, or a column bound to a domain (the program then runs over the

@@ -170,6 +170,10 @@ class TransformOp(C.Structure):
     _fields_ = [("op", C.c_int32), ("reserved", C.c_int32), ("i", C.c_int64), ("d", C.c_double)]
 
 
+class ExprProgram(C.Structure):  # pb200_expr_program
+    _fields_ = [("num_ops", C.c_int32), ("reserved", C.c_int32), ("ops", C.POINTER(TransformOp))]
+
+
 class HStarMetric(C.Structure):
     _fields_ = [("function", C.c_int32), ("reserved", C.c_int32), ("column", C.c_char_p), ("fwd", C.c_void_p),
                 ("fwd_bytes", C.c_uint64)]
@@ -211,7 +215,7 @@ EXPORTED_SYMBOLS = [
     "pb200_segment_derive_column", "pb200h_segment_derive",
     "pb200h_startree_build", "pb200h_startree_get",
     "pb200_execute_having", "pb200h_execute_having", "pb200_execute_agg_args", "pb200h_execute_agg_args",
-    "pb200_match_pattern", "pb200_result_exact_sum",
+    "pb200_match_pattern", "pb200_result_exact_sum", "pb200_execute_exprs",
 ]
 
 _LIB = None
@@ -243,6 +247,8 @@ def load() -> C.CDLL:
                                        C.POINTER(vp), i32, C.POINTER(vp)]
     L.pb200_execute_agg_args.argtypes = [vp, C.POINTER(Query), C.POINTER(OrderBy), C.POINTER(AggArg), C.POINTER(Having),
                                          C.POINTER(vp), i32, C.POINTER(vp)]
+    L.pb200_execute_exprs.argtypes = [vp, C.POINTER(Query), C.POINTER(OrderBy), C.POINTER(AggArg), C.POINTER(Having),
+                                      C.POINTER(ExprProgram), C.POINTER(vp), i32, C.POINTER(vp)]
     L.pb200_result_histogram.restype = i64
     L.pb200_result_histogram.argtypes = [vp, i32, i32, vp, vp, i64]
     L.pb200_result_moments.argtypes = [vp, i32, i32, vp, vp, vp, vp, vp, vp, vp]

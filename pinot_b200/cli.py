@@ -146,6 +146,7 @@ def main(argv=None) -> int:
     from . import sql
     from ._lib import Pb200Error
     from .plan_maker import B200Context, B200PlanMaker, DictionaryDomain
+    from .query import is_multi_column_expression
 
     if sql.is_distinct(args.sql):
         return _distinct(args, sql.parse_distinct(args.sql))
@@ -161,7 +162,8 @@ def main(argv=None) -> int:
         try:
             if args.merge_on_device and len(segments) > 1:
                 cols = list(dict.fromkeys(list(query.group_by) + [a.column for a in query.aggregations
-                                                                  if a.column and a.function in ("MIN", "MAX", "DISTINCTCOUNT", "PERCENTILE",
+                                                                  if a.column and not is_multi_column_expression(a.function, a.column)
+                                                                  and a.function in ("MIN", "MAX", "DISTINCTCOUNT", "PERCENTILE",
                                                                                  "DISTINCTSUM", "DISTINCTAVG",
                                                                                  "VARPOP", "VARSAMP", "STDDEVPOP", "STDDEVSAMP",
                                                                                  "FIRSTWITHTIME", "LASTWITHTIME")]

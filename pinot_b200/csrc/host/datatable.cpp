@@ -118,12 +118,20 @@ extern "C" int64_t pb200h_result_to_datatable(const pb200h_query* q, const pb200
   }
   for (int a = 0; a < nagg; a++) {
     const int fn = q->aggs[a].function;
+    std::string arg = q->aggs[a].column ? q->aggs[a].column : "*";
     if (q->aggs[a].column) {
       const int ci = seg->column_index(q->aggs[a].column);
-      if (ci < 0) { set_error("unknown aggregation column '%s'", q->aggs[a].column); return PB200_E_INVALID; }
-      agg_cols[a] = &seg->cols[ci].decode_column();
+      std::vector<pb200_transform_op> ops;
+      std::vector<std::string> leaves;
+      // an expression over several columns: written like the function over a DOUBLE column, named by its canonical text
+      if (ci < 0 && expression_function(fn) && is_multi_column_expression(q->aggs[a].column)) {
+        if (int rc = compile_multi_expression(q->aggs[a].column, &arg, &ops, &leaves)) return rc;
+      } else {
+        if (ci < 0) { set_error("unknown aggregation column '%s'", q->aggs[a].column); return PB200_E_INVALID; }
+        agg_cols[a] = &seg->cols[ci].decode_column();
+      }
     }
-    names.push_back(std::string(fn_name(fn)) + "(" + (q->aggs[a].column ? q->aggs[a].column : "*") + ")");
+    names.push_back(std::string(fn_name(fn)) + "(" + arg + ")");
     types.push_back(fn == PB200_AGG_COUNT ? "LONG" : (fn == PB200_AGG_AVG || fn == PB200_AGG_DISTINCTCOUNT || pb200::is_distinct_value_fn(fn)) ? "OBJECT" : "DOUBLE");
     width.push_back(8);
   }

@@ -173,6 +173,15 @@ namespace pb200h {
 // transform.cpp: resolves every name that is no column of a segment as an expression and derives it there once
 // (pb200h_segment_derive); afterwards every name is at one position in all segments (else PB200_E_UNSUPPORTED)
 int derive_names(pb200_ctx* ctx, pb200h_segment* const* segs, int nseg, const std::vector<const char*>& names);
+// Multi-column expressions (DESIGN.md section 3.15): `text` in the grammar of compile_expression with two or more column
+// leaves, compiled to a program whose PB200_T_COLUMN leaf k (i = k) reads column leaves[k].  PB200_E_INVALID (malformed)
+// or PB200_E_UNSUPPORTED (fewer than two or more than 8 leaves, a time function, outside the grammar), message set.
+int compile_multi_expression(const char* text, std::string* canonical, std::vector<pb200_transform_op>* ops,
+                             std::vector<std::string>* leaves);
+// `text` compiles as a multi-column expression (the last error is left as it was)
+bool is_multi_column_expression(const char* text);
+// the functions that take a multi-column expression as their argument
+inline bool expression_function(int fn) { return fn == PB200_AGG_SUM || fn == PB200_AGG_AVG || fn == PB200_AGG_MIN || fn == PB200_AGG_MAX; }
 int derive_query_names(pb200_ctx* ctx, const pb200h_query& q, pb200h_segment* const* segs, int nseg, const char* const* extra, int nextra);
 }  // namespace pb200h
 

@@ -286,12 +286,15 @@ pb200_result* host_result(const pb200h_segment& seg, const pb200h_query& q, bool
   for (int a = 0; a < nagg; a++) {
     const pb200h_agg& ag = q.aggs[a];
     double d = 0; int64_t l = 0; int32_t id = -1;
-    const HostColumn* c = ag.column ? &seg.cols[seg.column_index(ag.column)] : nullptr;
+    // MIN / MAX read the column's dictionary; an expression argument has no column here (its aggregation is never
+    // answered without a scan, so only an empty match reaches this)
+    const int ci = ag.column ? seg.column_index(ag.column) : -1;
+    const HostColumn* c = ci >= 0 ? &seg.cols[ci] : nullptr;
     switch (ag.function) {
       case PB200_AGG_COUNT: l = empty ? 0 : seg.num_docs; d = (double)l; break;
       case PB200_AGG_SUM: case PB200_AGG_AVG: d = 0; l = 0; break;
-      case PB200_AGG_MIN: if (empty) d = INFINITY; else { id = c->to_device_id(0); d = c->as_double(0); } break;
-      case PB200_AGG_MAX: if (empty) d = -INFINITY; else { id = c->to_device_id(c->cardinality - 1); d = c->as_double(c->cardinality - 1); } break;
+      case PB200_AGG_MIN: if (empty || !c) d = INFINITY; else { id = c->to_device_id(0); d = c->as_double(0); } break;
+      case PB200_AGG_MAX: if (empty || !c) d = -INFINITY; else { id = c->to_device_id(c->cardinality - 1); d = c->as_double(c->cardinality - 1); } break;
       case PB200_AGG_PERCENTILE: d = -INFINITY; break;   // only reached for an empty match (never answered without a scan)
       case PB200_AGG_FIRSTWITHTIME: case PB200_AGG_LASTWITHTIME: d = -INFINITY; break;   // likewise: no row, dictId -1
       case PB200_AGG_VARPOP: case PB200_AGG_VARSAMP: case PB200_AGG_STDDEVPOP: case PB200_AGG_STDDEVSAMP:
@@ -836,10 +839,32 @@ extern "C" int32_t pb200h_execute_agg_args(pb200_ctx* ctx, const pb200h_query* q
   }
   std::vector<pb200_agg> aggs(q->num_aggs);
   std::vector<pb200_agg_arg> dev_args(q->num_aggs, pb200_agg_arg{0.0, -1, 0});
+  // SUM / AVG / MIN / MAX over an expression of two or more columns: a program over column ids, evaluated per row
+  std::vector<std::vector<pb200_transform_op>> expr_ops(q->num_aggs);
+  std::vector<pb200_expr_program> programs(q->num_aggs, pb200_expr_program{0, 0, nullptr});
+  std::vector<int> leaf_cols;
+  bool any_expr = false;
+  for (int a = 0; a < q->num_aggs; a++) {
+    if (!expression_function(q->aggs[a].function) || !is_multi_column_expression(q->aggs[a].column)) continue;
+    std::string canonical;
+    std::vector<std::string> leaves;
+    if (int rc = compile_multi_expression(q->aggs[a].column, &canonical, &expr_ops[a], &leaves)) return rc;
+    for (pb200_transform_op& o : expr_ops[a]) {
+      if (o.op != PB200_T_COLUMN) continue;
+      const char* name = leaves[(size_t)o.i].c_str();
+      const int ci = s0.column_index(name);
+      if (ci < 0 || ci >= s0.num_stored) { set_error("expression '%s': unknown column '%s'", q->aggs[a].column, name); return PB200_E_INVALID; }
+      if (s0.cols[ci].data_type == PB200_STRING) { set_error("expression '%s': STRING column '%s' in arithmetic", q->aggs[a].column, name); return PB200_E_UNSUPPORTED; }
+      o.i = ci;
+      leaf_cols.push_back(ci);
+    }
+    programs[a] = pb200_expr_program{(int32_t)expr_ops[a].size(), 0, expr_ops[a].data()};
+    any_expr = true;
+  }
   for (int a = 0; a < q->num_aggs; a++) {
     aggs[a].function = q->aggs[a].function;
     aggs[a].column = -1;
-    if (q->aggs[a].function != PB200_AGG_COUNT) {
+    if (q->aggs[a].function != PB200_AGG_COUNT && !programs[a].num_ops) {
       aggs[a].column = s0.column_index(q->aggs[a].column);
       if (aggs[a].column < 0) { set_error("unknown aggregation column '%s'", q->aggs[a].column ? q->aggs[a].column : "(null)"); return PB200_E_INVALID; }
       const HostColumn& c = s0.cols[aggs[a].column];
@@ -871,16 +896,17 @@ extern "C" int32_t pb200h_execute_agg_args(pb200_ctx* ctx, const pb200h_query* q
     for (int g = 0; g < q->num_group_by; g++) if (!same_column(gb[g])) { set_error("segment %d: column '%s' is not at the position it has in segment 0", s, q->group_by[g]); return PB200_E_INVALID; }
     for (int a = 0; a < q->num_aggs; a++) if (aggs[a].column >= 0 && !same_column(aggs[a].column)) { set_error("segment %d: column '%s' is not at the position it has in segment 0", s, q->aggs[a].column); return PB200_E_INVALID; }
     for (int a = 0; a < q->num_aggs; a++) if (dev_args[a].time_column >= 0 && !same_column(dev_args[a].time_column)) { set_error("segment %d: column '%s' is not at the position it has in segment 0", s, args[a].time_column); return PB200_E_INVALID; }
+    for (int c : leaf_cols) if (!same_column(c)) { set_error("segment %d: column '%s' is not at the position it has in segment 0", s, s0.cols[c].name.c_str()); return PB200_E_INVALID; }
     int rc = build_segment_filter(*segs[s], *q, filters[s], nullptr);
     if (rc) return rc;
     if (!merge) {
       if (filters[s].root_empty) kind[s] = PB200H_OP_EMPTY;
-      else if (filters[s].root_all && non_scan_answerable(*segs[s], *q)) kind[s] = PB200H_OP_NON_SCAN_AGGREGATION;
+      else if (filters[s].root_all && !any_expr && non_scan_answerable(*segs[s], *q)) kind[s] = PB200H_OP_NON_SCAN_AGGREGATION;
     }
   }
   // star-tree substitution (AggregationFunctionUtils.buildAggregationInfo :285-310): first star-tree that fits wins
   std::vector<pb200_result*> star_results(nseg, nullptr);
-  if (!merge && !q->skip_star_tree) {
+  if (!merge && !q->skip_star_tree && !any_expr) {   // expressions are computed per row: the raw scan runs
     for (int s = 0; s < nseg; s++) {
       if (kind[s] != PB200H_OP_AGGREGATION && kind[s] != PB200H_OP_GROUP_BY) continue;
       for (auto& st : segs[s]->star_trees) {
@@ -921,7 +947,8 @@ extern "C" int32_t pb200h_execute_agg_args(pb200_ctx* ctx, const pb200h_query* q
     dq.filter = flat.data();
     dq.group_by_columns = gb.data();
     dq.aggs = aggs.data();
-    int rc = pb200_execute_agg_args(ctx, &dq, order, args ? dev_args.data() : nullptr, having, dsegs.data(), (int)dsegs.size(), dev_results.data());
+    int rc = any_expr ? pb200_execute_exprs(ctx, &dq, order, args ? dev_args.data() : nullptr, having, programs.data(), dsegs.data(), (int)dsegs.size(), dev_results.data())
+                      : pb200_execute_agg_args(ctx, &dq, order, args ? dev_args.data() : nullptr, having, dsegs.data(), (int)dsegs.size(), dev_results.data());
     if (rc) { for (auto r : star_results) if (r) pb200_result_free(r); return rc; }
   }
   if (merge) { results[0] = dev_results[0]; return PB200_OK; }

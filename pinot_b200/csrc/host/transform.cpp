@@ -13,7 +13,7 @@
 #include <vector>
 
 #include "host_internal.h"
-#include "../pb200_transform.h"
+#include "../pb200_expr.h"
 
 using pb200::set_error;
 using namespace pb200h;
@@ -166,6 +166,8 @@ struct Compiled {
   std::vector<pb200_transform_op> ops;
   std::string column;
   int columns = 0;
+  bool multi = false;                  // any number of columns: leaf k (PB200_T_COLUMN i = k) reads column leaves[k]
+  std::vector<std::string> leaves;
 };
 
 int compile(const Node& n, Compiled& c) {
@@ -177,6 +179,12 @@ int compile(const Node& n, Compiled& c) {
     o.op = is_int ? PB200_T_LONG_LITERAL : PB200_T_DOUBLE_LITERAL; o.i = i; o.d = d;
     c.ops.push_back(o);
     c.text += "'" + number_text(is_int, i, d) + "'";
+    return PB200_OK;
+  }
+  if (!n.call && c.multi) {
+    op(PB200_T_COLUMN, (int64_t)c.leaves.size());
+    c.leaves.push_back(n.text);
+    c.text += n.text;
     return PB200_OK;
   }
   if (!n.call) {
@@ -234,7 +242,8 @@ int compile(const Node& n, Compiled& c) {
   return PB200_OK;
 }
 
-int compile_text(const char* text, Compiled& c) {
+int compile_text(const char* text, Compiled& c, bool multi = false) {
+  c.multi = multi;
   Parser ps{text};
   auto root = ps.parse();
   if (root) { ps.ws(); if (*ps.p) { ps.err = "trailing characters"; root.reset(); } }
@@ -294,6 +303,36 @@ int compile_expression(const char* text, std::string* canonical, std::vector<pb2
   return rc;
 }
 
+int compile_multi_expression(const char* text, std::string* canonical, std::vector<pb200_transform_op>* ops,
+                             std::vector<std::string>* leaves) {
+  Compiled c;
+  int rc = compile_text(text, c, true);
+  if (rc == PB200_OK && c.leaves.size() < 2) { set_error("'%s' has fewer than two column leaves", text); rc = PB200_E_UNSUPPORTED; }
+  if (rc == PB200_OK)
+    for (const auto& o : c.ops)
+      if (!pb200::expr_op_ok(o.op)) {
+        set_error("'%s': time functions are not accelerated inside an expression over two or more columns", text);
+        rc = PB200_E_UNSUPPORTED;
+        break;
+      }
+  if (rc == PB200_OK && (int)c.leaves.size() > pb200::kExprMaxLeaves) {
+    set_error("'%s' has %zu column leaves (at most %d)", text, c.leaves.size(), pb200::kExprMaxLeaves);
+    rc = PB200_E_UNSUPPORTED;
+  }
+  if (rc == PB200_OK) { *canonical = c.text; *ops = c.ops; *leaves = c.leaves; }
+  return rc;
+}
+
+bool is_multi_column_expression(const char* text) {
+  if (!text || !strchr(text, '(')) return false;
+  Compiled c;
+  char saved[1024];
+  memcpy(saved, pb200_last_error(), sizeof saved);  // a failed test leaves the caller's last error alone
+  const bool multi = compile_text(text, c, true) == PB200_OK && c.leaves.size() >= 2;
+  set_error("%s", saved);
+  return multi;
+}
+
 bool normalize_expression(const char* text, std::string* canonical) {
   Compiled c;
   char saved[1024];
@@ -328,7 +367,9 @@ int derive_query_names(pb200_ctx* ctx, const pb200h_query& q, pb200h_segment* co
   std::vector<const char*> names;
   for (int i = 0; i < q.num_filter_nodes; i++) if (q.filter[i].type >= PB200H_EQ) names.push_back(q.filter[i].column);
   for (int g = 0; g < q.num_group_by; g++) names.push_back(q.group_by[g]);
-  for (int a = 0; a < q.num_aggs; a++) if (q.aggs && q.aggs[a].function != PB200_AGG_COUNT) names.push_back(q.aggs[a].column);
+  for (int a = 0; a < q.num_aggs; a++)   // an expression over several columns is computed per row, not derived
+    if (q.aggs && q.aggs[a].function != PB200_AGG_COUNT && !(expression_function(q.aggs[a].function) && is_multi_column_expression(q.aggs[a].column)))
+      names.push_back(q.aggs[a].column);
   if (q.agg_filter_count && q.agg_filter_start && q.agg_filter_nodes)
     for (int a = 0; a < q.num_aggs; a++)
       for (int k = 0; k < q.agg_filter_count[a]; k++) {

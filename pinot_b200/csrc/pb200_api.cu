@@ -17,6 +17,7 @@
 #include <optional>
 
 #include "pb200_internal.h"
+#include "pb200_expr.h"
 #include "pb200_percentile.h"
 #include "pb200_withtime.h"
 #include "pb200_plan.h"
@@ -703,7 +704,10 @@ int launch_chunks(pb200_ctx* ctx, cudaStream_t st, const ScanPlan& plan, DevBufR
 constexpr int kRetryWithoutCountCarrier = 1;
 static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment* const* segments, int32_t nseg,
                         pb200_result** results, bool allow_count_carrier, const pb200_order_by* order, const double* agg_args,
-                        const pb200_having* having, const pb200_agg_arg* wt_args);
+                        const pb200_having* having, const pb200_agg_arg* wt_args, const ExprCall* ex = nullptr);
+static int execute_checked(pb200_ctx* ctx, const pb200_query* query, const pb200_order_by* order, const pb200_agg_arg* args,
+                           const pb200_having* having, pb200_segment* const* segments, int32_t nseg, pb200_result** results,
+                           const ExprCall* ex);
 
 extern "C" int32_t pb200_execute_having(pb200_ctx* ctx, const pb200_query* query, const pb200_order_by* order, const double* agg_args,
                                         const pb200_having* having, pb200_segment* const* segments, int32_t nseg,
@@ -724,12 +728,36 @@ extern "C" int32_t pb200_execute_agg_args(pb200_ctx* ctx, const pb200_query* que
                                           pb200_result** results) {
   if (!query || !args || query->num_aggs < 0 || query->num_aggs > kMaxAggs || (query->num_aggs > 0 && !query->aggs))
     return pb200_execute_having(ctx, query, order, nullptr, having, segments, nseg, results);
+  return execute_checked(ctx, query, order, args, having, segments, nseg, results, nullptr);
+}
+
+extern "C" int32_t pb200_execute_exprs(pb200_ctx* ctx, const pb200_query* query, const pb200_order_by* order, const pb200_agg_arg* args,
+                                       const pb200_having* having, const pb200_expr_program* exprs, pb200_segment* const* segments,
+                                       int32_t nseg, pb200_result** results) {
+  if (!exprs) return pb200_execute_agg_args(ctx, query, order, args, having, segments, nseg, results);
+  if (!ctx || !results) { set_error("invalid argument to pb200_execute_exprs"); return PB200_E_INVALID; }
+  ExprCall ex;
+  if (const int rc = expr_prepare(query, exprs, segments, nseg, &ex)) return rc;
+  if (!ex.count) return pb200_execute_agg_args(ctx, query, order, args, having, segments, nseg, results);
+  // the scan runs every expression aggregation as COUNT(*): its group tables and counts are what the expressions need
+  pb200_query q = *query;
+  pb200_agg aggs[kMaxAggs];
+  for (int a = 0; a < q.num_aggs; a++) aggs[a] = ex.fn_of[a] >= 0 ? pb200_agg{PB200_AGG_COUNT, -1} : query->aggs[a];
+  q.aggs = aggs;
+  return execute_checked(ctx, &q, order, args, having, segments, nseg, results, &ex);
+}
+
+// pb200_execute_agg_args past its argument check (args NULL: no percentiles and no *WITHTIME), with the expression
+// aggregations of pb200_execute_exprs (ex NULL: none)
+static int execute_checked(pb200_ctx* ctx, const pb200_query* query, const pb200_order_by* order, const pb200_agg_arg* args,
+                           const pb200_having* having, pb200_segment* const* segments, int32_t nseg, pb200_result** results,
+                           const ExprCall* ex) {
   if (const int vrc = order_validate(order, query->num_aggs, query->num_group_by)) return vrc;
   const int nres = (query->flags & PB200_Q_MERGE_SEGMENTS) ? 1 : nseg;
   const bool deferred = (query->flags & PB200_Q_DEFER_FINALIZE) || query->reduce_world > 1;
   if (const int hrc = having_check(having, query->num_aggs, query->num_group_by, nres, deferred)) return hrc;
   // ORDER BY / HAVING compare the double column: for a STRING-typed *WITHTIME that is a dictId, not a value
-  if (segments && nseg > 0 && segments[0] && query->num_group_by > 0) {
+  if (args && segments && nseg > 0 && segments[0] && query->num_group_by > 0) {
     auto string_wt = [&](int a) {
       const pb200_agg& ag = query->aggs[a];
       return is_withtime_fn(ag.function) && ag.column >= 0 && ag.column < (int)segments[0]->cols.size() &&
@@ -747,9 +775,11 @@ extern "C" int32_t pb200_execute_agg_args(pb200_ctx* ctx, const pb200_query* que
     }
   }
   double p[kMaxAggs] = {};
-  for (int a = 0; a < query->num_aggs; a++) p[a] = args[a].p;
-  int rc = execute_impl(ctx, query, segments, nseg, results, true, order, p, having, args);
-  if (rc == kRetryWithoutCountCarrier) rc = execute_impl(ctx, query, segments, nseg, results, false, order, p, having, args);
+  for (int a = 0; args && a < query->num_aggs; a++) p[a] = args[a].p;
+  const double* agg_args = args ? p : nullptr;
+  // a retry rebuilds every table of the attempt, the expression tables included
+  int rc = execute_impl(ctx, query, segments, nseg, results, true, order, agg_args, having, args, ex);
+  if (rc == kRetryWithoutCountCarrier) rc = execute_impl(ctx, query, segments, nseg, results, false, order, agg_args, having, args, ex);
   return rc;
 }
 
@@ -796,13 +826,19 @@ namespace {
 // Then (aggregation-only FIRST/LASTWITHTIME) per result kMaxAggs winning keys and kMaxAggs time values, u64 each, and
 // kMaxAggs data dictIds, u32 each.
 // Then (aggregation-only DISTINCTSUM / DISTINCTAVG) per result and aggregation the finalized state, kDsWords u64 each.
+// Then (aggregation-only expression aggregations, pb200_expr.cu) per result and aggregation one u64: the f64 sum, or the
+// Double.compare key of a MIN / MAX.
 struct AccumLayout {
-  size_t verify_off = 0, pct_off = 0, wt_off = 0, ds_off = 0, bytes = 0;
+  size_t verify_off = 0, pct_off = 0, wt_off = 0, ds_off = 0, ex_off = 0, bytes = 0;
   int nres = 0;
   AccumLayout() = default;
-  AccumLayout(int nres, bool pct, bool wt, bool ds)
+  AccumLayout(int nres, bool pct, bool wt, bool ds, bool ex)
       : verify_off(sizeof(AggAccum) * nres), pct_off(verify_off + 32ull * nres), wt_off(pct_off + (pct ? 8ull * kMaxAggs * nres : 0)),
-        ds_off(wt_off + (wt ? 20ull * kMaxAggs * nres : 0)), bytes(ds_off + (ds ? 8ull * kDsWords * kMaxAggs * nres : 0)), nres(nres) {}
+        ds_off(wt_off + (wt ? 20ull * kMaxAggs * nres : 0)), ex_off(ds_off + (ds ? 8ull * kDsWords * kMaxAggs * nres : 0)),
+        bytes(ex_off + (ex ? 8ull * kMaxAggs * nres : 0)), nres(nres) {}
+  unsigned long long* ex(void* b, int r) const {
+    return reinterpret_cast<unsigned long long*>(static_cast<unsigned char*>(b) + ex_off) + (size_t)r * kMaxAggs;
+  }
   unsigned long long* ds(void* b, int r, int a) const {
     return reinterpret_cast<unsigned long long*>(static_cast<unsigned char*>(b) + ds_off) + ((size_t)r * kMaxAggs + a) * kDsWords;
   }
@@ -821,6 +857,7 @@ void release_tables(pb200_result& R, bool keep_hist) {
     dev_free(d.ctx, d.i64_block); dev_free(d.ctx, d.f64_block); dev_free(d.ctx, d.u32max_block); dev_free(d.ctx, d.u32min_block);
     dev_free(d.ctx, d.hkeys); dev_free(d.ctx, d.hctl);
     for (int a = 0; a < kMaxAggs; a++) { dev_free(d.ctx, d.dbits[a]); d.dbits[a] = nullptr; dev_free(d.ctx, d.ds_state[a]); d.ds_state[a] = nullptr; }
+    for (int a = 0; a < kMaxAggs; a++) { dev_free(d.ctx, d.expr_tab[a]); d.expr_tab[a] = nullptr; }
     d.i64_block = d.f64_block = d.u32max_block = d.u32min_block = nullptr;
     d.hkeys = nullptr; d.hctl = nullptr;
     d.live = false;
@@ -862,6 +899,8 @@ struct ScanCall {
   std::vector<std::vector<std::unique_ptr<DevBufRaw>>> distinct_bufs;  // aggregation only: DISTINCTCOUNT bitsets
   DevBufRaw dsegs{ctx};
   EventPair ev{ctx};                                 // around the scan launches
+  const ExprCall* ex = nullptr;                      // expression aggregations (pb200_execute_exprs), run as COUNT(*) by the scan
+  int expr_fn(int a) const { return ex ? ex->fn_of[a] : -1; }
 
   ~ScanCall() { for (auto& r : res) if (r) pb200_result_free(r.release()); }
 
@@ -901,7 +940,7 @@ struct ScanCall {
     for (int a = 0; a < plan.q.num_aggs; a++) any_pct |= plan.pct_rep[a] >= 0;
     bool any_ds = false;
     for (int a = 0; a < plan.q.num_aggs; a++) any_ds |= plan.ds_rep[a] >= 0;
-    acc = AccumLayout(plan.nres, any_pct && !plan.group_by, plan.any_wt && !plan.group_by, any_ds && !plan.group_by);
+    acc = AccumLayout(plan.nres, any_pct && !plan.group_by, plan.any_wt && !plan.group_by, any_ds && !plan.group_by, ex && !plan.group_by);
     if (int rc = pinned_alloc(ctx, 2 * acc.bytes, &pin.p, &pin.bytes)) return rc;
     unsigned char* const init = static_cast<unsigned char*>(pin.p);
     back = init + acc.bytes;
@@ -914,6 +953,10 @@ struct ScanCall {
       for (int r = 0; r < plan.nres; r++)
         for (int a = 0; a < plan.q.num_aggs; a++)
           if (plan.q.aggs[a].function == PB200_AGG_FIRSTWITHTIME) acc.wt_key(init, r)[a] = ~0ull;
+    if (ex && !plan.group_by)   // expression MIN keys start at u64 max, MAX keys at 0, sums at +0.0
+      for (int r = 0; r < plan.nres; r++)
+        for (int a = 0; a < plan.q.num_aggs; a++)
+          if (expr_fn(a) == PB200_AGG_MIN) acc.ex(init, r)[a] = kExprMinEmpty;
     if (int rc = accum.alloc(acc.bytes)) return rc;
     PB200_CUDA(cudaMemcpyAsync(accum.p, init, acc.bytes, cudaMemcpyHostToDevice, st));
     for (int s = 0; s < nseg; s++) plan.segs[s].accum = AccumLayout::records(accum.p) + (plan.merge ? 0 : s);
@@ -960,6 +1003,8 @@ struct ScanCall {
   int bind_group_tables() {
     for (int r = 0; r < plan.nres; r++)
       if (int rc = build_dense(r)) return rc;
+    for (int r = 0; r < plan.nres && ex; r++)
+      if (int rc = build_expr_tables(r)) return rc;
     for (int s = 0; s < nseg; s++) {
       SegDesc& sd = plan.segs[s];
       const pb200_result& R = *res[plan.merge ? 0 : s];
@@ -972,6 +1017,22 @@ struct ScanCall {
         sd.g_isum[a] = d.isum[a]; sd.g_dsum[a] = d.dsum[a]; sd.g_min[a] = d.gmin[a]; sd.g_max[a] = d.gmax[a];
         sd.distinct_bits[a] = R.pct.hist[a] ? R.pct.hist[a] : R.wt.key[a] ? reinterpret_cast<uint32_t*>(R.wt.key[a]) : d.dbits[a];
       }
+    }
+    return PB200_OK;
+  }
+  // expression aggregations: each one's table, and the result's view of the aggregation as the function the caller asked
+  // for over a DOUBLE value (the scan ran it as COUNT(*))
+  int build_expr_tables(int r) {
+    pb200_result::Dense& d = res[r]->dense;
+    for (int a = 0; a < plan.num_user_aggs; a++) {
+      const int fn = expr_fn(a);
+      if (fn < 0) continue;
+      const size_t bytes = (size_t)d.groups * 8;
+      if (int rc = dev_alloc(ctx, bytes, &d.expr_tab[a])) return rc;
+      PB200_CUDA(cudaMemsetAsync(d.expr_tab[a], fn == PB200_AGG_MIN ? 0xFF : 0, bytes, st));
+      d.aggs[a].function = fn;
+      d.val_kind[a] = VAL_DICT_F64;
+      if (fn == PB200_AGG_SUM || fn == PB200_AGG_AVG) d.dsum[a] = static_cast<double*>(d.expr_tab[a]);
     }
     return PB200_OK;
   }
@@ -1123,6 +1184,20 @@ struct ScanCall {
     return PB200_OK;
   }
 
+  // 8d. expression aggregations: the mask scan and the expression pass (pb200_expr.cu), queued behind the scan into the
+  //     expression tables (group-by) or the accumulator block (aggregation only)
+  int finalize_exprs() {
+    if (!ex) return PB200_OK;
+    std::vector<ExprOut> outs(plan.nres);
+    for (int r = 0; r < plan.nres; r++)
+      for (int a = 0; a < plan.num_user_aggs; a++) {
+        if (expr_fn(a) < 0) continue;
+        outs[r].out[a] = plan.group_by ? res[r]->dense.expr_tab[a] : static_cast<void*>(acc.ex(accum.p, r) + a);
+        outs[r].hkeys = res[r]->dense.hkeys;
+      }
+    return expr_launch(ctx, st, tune, query, segments, nseg, plan, *ex, outs, temps);
+  }
+
   // 9. the count carriers' check queued behind the scan, the accumulator block read back, the wait for both, and the
   //    carriers' verdict: kRetryWithoutCountCarrier when a carried sum overflowed its field
   int read_back_and_verify() {
@@ -1186,7 +1261,11 @@ struct ScanCall {
         default: { double y; memcpy(&y, h + 8ull * x, 8); return y; }
       }
     };
-    if (fn == PB200_AGG_COUNT) { v->l = (int64_t)acc_r.count; v->d = (double)v->l; }
+    if (expr_fn(a) >= 0) {   // the expression pass's sum, or the decoded MIN / MAX key
+      const unsigned long long w = acc.ex(back, r)[a];
+      if (expr_fn(a) == PB200_AGG_SUM || expr_fn(a) == PB200_AGG_AVG) { memcpy(&v->d, &w, 8); v->l = (int64_t)acc_r.count; }
+      else v->d = expr_key_value(expr_fn(a), w);
+    } else if (fn == PB200_AGG_COUNT) { v->l = (int64_t)acc_r.count; v->d = (double)v->l; }
     else if (is_moments_fn(fn)) {   // the exact moments from the limb sums (pb200_moments.h), rounded once
       const int k0 = plan.mom_first[a];
       const Moments m = moments_from_sums(acc_r.count, acc_r.isum[k0], acc_r.isum[k0 + 1], acc_r.isum[k0 + 2]);
@@ -1239,12 +1318,12 @@ struct ScanCall {
       R.meta.num_group_by = plan.q.num_group_by;
       R.meta.num_aggs = nuser;
       R.agg_functions.resize(nuser);
-      for (int a = 0; a < nuser; a++) R.agg_functions[a] = plan.q.aggs[a].function;
+      for (int a = 0; a < nuser; a++) R.agg_functions[a] = expr_fn(a) >= 0 ? expr_fn(a) : plan.q.aggs[a].function;
       for (int a = 0; a < nuser; a++)
         if (plan.mom_first[a] >= 0) { R.mom.on[a] = true; R.mom.grid[a] = segments[plan.merge ? 0 : r]->cols[query->aggs[a].column].moments->grid; }
       R.meta.num_docs_scanned = (int64_t)count;
       R.meta.num_entries_scanned_in_filter = plan.in_filter[r];
-      R.meta.num_entries_scanned_post_filter = (int64_t)count * plan.projected;
+      R.meta.num_entries_scanned_post_filter = (int64_t)count * projected();
       R.meta.num_total_docs = total_docs;
       R.meta.device_ms = ms;
       R.dbl.resize(nuser); R.lng.resize(nuser); R.ids.resize(nuser); R.distinct.resize(nuser);
@@ -1277,6 +1356,16 @@ struct ScanCall {
     return PB200_OK;
   }
 
+  // columns read after the filter: the scan's group-by and aggregation columns, and every expression leaf, each once
+  int projected() const {
+    if (!ex) return plan.projected;
+    std::vector<int> cols = ex->cols;
+    for (int k = 0; k < plan.q.num_slots; k++)
+      if ((plan.q.slot_roles[k] & (ROLE_GROUP | ROLE_AGG)) && std::find(cols.begin(), cols.end(), plan.slot_cols[k]) == cols.end())
+        cols.push_back(plan.slot_cols[k]);
+    return (int)cols.size();
+  }
+
   // 12. the results handed out, and the phases of the call (pb200_last_phases)
   void hand_out(pb200_result** results) {
     for (int r = 0; r < plan.nres; r++) results[r] = res[r].release();
@@ -1293,8 +1382,9 @@ struct ScanCall {
 
 static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment* const* segments, int32_t nseg,
                         pb200_result** results, bool allow_count_carrier, const pb200_order_by* order, const double* agg_args,
-                        const pb200_having* having, const pb200_agg_arg* wt_args) {
+                        const pb200_having* having, const pb200_agg_arg* wt_args, const ExprCall* ex) {
   ScanCall c{ctx, query, segments, nseg};
+  c.ex = ex;
   if (int rc = c.check_call(results)) return rc;
   if (int rc = c.prepare_and_plan(allow_count_carrier, agg_args, wt_args)) return rc;
   if (int rc = c.alloc_results()) return rc;
@@ -1304,6 +1394,7 @@ static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment*
   if (int rc = c.finalize_percentiles()) return rc;
   if (int rc = c.finalize_withtime()) return rc;
   if (int rc = c.finalize_distinct_sums()) return rc;
+  if (int rc = c.finalize_exprs()) return rc;
   if (int rc = c.read_back_and_verify()) return rc;   // kRetryWithoutCountCarrier: ~ScanCall frees this attempt's tables
   if (int rc = c.fill_results_and_extract(order, having)) return rc;
   c.hand_out(results);
@@ -1328,6 +1419,11 @@ extern "C" int32_t pb200_result_device_buffers(pb200_result* R, int32_t kind, vo
     if (R->mom.on[a]) { set_error("VAR/STDDEV moments are not combined across GPUs"); return PB200_E_UNSUPPORTED; }
   for (int a = 0; a < kMaxAggs; a++)
     if (R->wt.key[a]) { set_error("FIRST/LASTWITHTIME results are not combined across GPUs"); return PB200_E_UNSUPPORTED; }
+  for (int a = 0; a < kMaxAggs; a++)
+    if (d.expr_tab[a]) {   // not in the four reducible blocks: a reduce of those would keep only this rank's expression values
+      set_error("group-by expression aggregations keep their tables outside the reducible blocks: they are not combined across GPUs");
+      return PB200_E_UNSUPPORTED;
+    }
   for (int a = 0; a < kMaxAggs; a++)
     if (R->pct.hist[a]) {
       set_error("PERCENTILE keeps dictId histograms on the device: a cross-GPU reduce of the tables would drop the other ranks' values");

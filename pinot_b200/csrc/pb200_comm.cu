@@ -198,8 +198,10 @@ extern "C" int32_t pb200_result_combine(pb200_ctx* ctx, pb200_result* R, int32_t
   pb200_result::Dense& d = R->dense;
   if (!d.ctx || !d.live || d.groups <= 0) { set_error("result has no device tables (execute with PB200_Q_MERGE_SEGMENTS | PB200_Q_DEFER_FINALIZE)"); return PB200_E_INVALID; }
   if (d.hkeys) { set_error("hash group tables of different GPUs are not element-wise reducible"); return PB200_E_UNSUPPORTED; }
-  for (int a = 0; a < kMaxAggs; a++)
+  for (int a = 0; a < kMaxAggs; a++) {
     if (d.dbits[a]) { set_error("group-by DISTINCTCOUNT bitsets are not reducible by NCCL (no bitwise OR): merge on the host"); return PB200_E_UNSUPPORTED; }
+    if (d.expr_tab[a]) { set_error("group-by expression aggregations are not combined across GPUs: merge on the host"); return PB200_E_UNSUPPORTED; }
+  }
   (void)root;
   if (d.pack_agg >= 0 && ctx->comm_world > 1 && !d.flag_slot) {
     set_error("count-carrying table was not sized for a reduce: execute with pb200_query.reduce_world = world size");

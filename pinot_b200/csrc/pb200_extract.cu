@@ -32,6 +32,7 @@
 #include <cstring>
 
 #include "pb200_internal.h"
+#include "pb200_expr.h"
 #include "pb200_having.h"
 #include "pb200_order.h"
 
@@ -75,6 +76,7 @@ struct ExtractDesc {
   int32_t mom_e[kMaxAggs];           // ... and the grid exponent of the column
   unsigned long long off_mom[kMaxAggs];  // ... {s1, s2 low, s2 high} per row, for pb200_result_moments
   const unsigned long long* ds[kMaxAggs];  // DISTINCTSUM / DISTINCTAVG: the finalized state per table entry (kDsWords u64)
+  const unsigned long long* xkey[kMaxAggs];  // expression MIN / MAX (pb200_expr.cu): Double.compare key per table entry
   const uint8_t* keep;               // HAVING only: bit j of byte i = entry 8i + j is a row (NULL: every non_empty() entry is)
 };
 
@@ -167,6 +169,8 @@ __device__ __forceinline__ void agg_values(const ExtractDesc& d, int a, long lon
       dv = sum_in_double(vk) ? static_cast<const double*>(d.src[a])[g] : (double)static_cast<const long long*>(d.src[a])[g];
     }
     lv = (long long)cnt;
+  } else if (d.xkey[a]) {
+    dv = expr_key_value(fn, d.xkey[a][g]);
   } else if (fn == PB200_AGG_MIN || fn == PB200_AGG_MAX) {
     const uint32_t t = static_cast<const uint32_t*>(d.src[a])[g];
     // every row of a submission reaches each of its functions, so a group that exists has a MIN / MAX.  Raw INT entries
@@ -452,6 +456,7 @@ int extract_groups(pb200_ctx* ctx, pb200_result* const* Rs, int nres, cudaStream
       const int fn = d.aggs[a].function, vk = d.val_kind[a];
       e.fn[a] = fn; e.vk[a] = vk;
       if (fn == PB200_AGG_SUM || fn == PB200_AGG_AVG) e.src[a] = sum_in_double(vk) ? (const void*)d.dsum[a] : (const void*)d.isum[a];
+      else if (d.expr_tab[a]) e.xkey[a] = static_cast<const unsigned long long*>(d.expr_tab[a]);   // MIN / MAX of an expression
       else if (fn == PB200_AGG_MIN) e.src[a] = d.gmin[a];
       else if (fn == PB200_AGG_MAX) e.src[a] = d.gmax[a];
       else if (fn == PB200_AGG_PERCENTILE) { e.src[a] = Rs[r]->pct.ids[a]; e.pct_n[a] = Rs[r]->pct.n[Rs[r]->pct.rep[a]]; }

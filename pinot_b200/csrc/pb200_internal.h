@@ -293,6 +293,9 @@ struct pb200_result {
     int ds_rep[pb200::kMaxAggs];
     int ds_e[pb200::kMaxAggs] = {};
     unsigned long long* ds_state[pb200::kMaxAggs] = {};
+    // expression aggregations (pb200_expr.cu): per aggregation its own table, f64 sums (also pointed to by dsum) or u64
+    // Double.compare keys of MIN / MAX; NULL: not an expression
+    void* expr_tab[pb200::kMaxAggs] = {};
     unsigned long long* hkeys = nullptr;        // hash table keys (NULL: dense table indexed by raw key)
     uint32_t* hctl = nullptr;                   // [0] inserted, [1] overflow
     std::vector<int> cards;

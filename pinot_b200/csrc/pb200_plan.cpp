@@ -982,13 +982,7 @@ int plan_selection(const Tuning& tune, DeviceLimits lim, const pb200_query* filt
     int kind = -1;
     for (int s = 0; s < nseg; s++) {
       const DeviceColumn& dc = segments[s]->cols[c];
-      int ks;
-      if (dc.fwd_kind != PB200_FWD_DICT_FIXEDBIT && dc.fwd_kind != PB200_FWD_RAW_FIXEDBYTE) ks = -1;
-      else if (dc.bits == 32 && !dc.dict_native) ks = dc.stored_type == PB200_INT ? SEL_RAW_I32 : dc.stored_type == PB200_FLOAT ? SEL_RAW_F32 : -1;
-      else if (dc.stored_type == PB200_STRING) ks = SEL_DICT_ID;
-      else if (!dc.dict_native) ks = -1;
-      else ks = dc.stored_type == PB200_INT ? SEL_DICT_I32 : dc.stored_type == PB200_LONG ? SEL_DICT_I64
-              : dc.stored_type == PB200_FLOAT ? SEL_DICT_F32 : SEL_DICT_F64;
+      const int ks = selection_kind(dc);
       if (ks < 0) { set_error("%s column %d of segment %d has no device dictionary or raw 32-bit values: not accelerated", what, c, s); return PB200_E_UNSUPPORTED; }
       if (kind >= 0 && ks != kind) { set_error("%s column %d is stored differently in segment %d than in segment 0", what, c, s); return PB200_E_UNSUPPORTED; }
       kind = ks;

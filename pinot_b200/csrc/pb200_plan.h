@@ -126,6 +126,15 @@ constexpr int kMaxSelectSegments = 65535;           // segments of one selection
 enum : int32_t { SEL_DICT_I32 = 0, SEL_DICT_I64 = 1, SEL_DICT_F32 = 2, SEL_DICT_F64 = 3, SEL_DICT_ID = 4, SEL_RAW_I32 = 5,
                  SEL_RAW_F32 = 6 };
 inline bool selection_kind_is_double(int k) { return k == SEL_DICT_F32 || k == SEL_DICT_F64 || k == SEL_RAW_F32; }
+// how a column's value is read at a doc (SEL_*): its device dictionary, or raw 32-bit INT / FLOAT values; -1 when neither
+inline int selection_kind(const DeviceColumn& dc) {
+  if (dc.fwd_kind != PB200_FWD_DICT_FIXEDBIT && dc.fwd_kind != PB200_FWD_RAW_FIXEDBYTE) return -1;
+  if (dc.bits == 32 && !dc.dict_native) return dc.stored_type == PB200_INT ? SEL_RAW_I32 : dc.stored_type == PB200_FLOAT ? SEL_RAW_F32 : -1;
+  if (dc.stored_type == PB200_STRING) return SEL_DICT_ID;
+  if (!dc.dict_native) return -1;
+  return dc.stored_type == PB200_INT ? SEL_DICT_I32 : dc.stored_type == PB200_LONG ? SEL_DICT_I64
+       : dc.stored_type == PB200_FLOAT ? SEL_DICT_F32 : SEL_DICT_F64;
+}
 
 struct SelectionPlan {
   ScanPlan scan;                          // the launch; segments keep their submission order and results are per segment
@@ -204,6 +213,26 @@ int bind_leaf_buffers(pb200_ctx* ctx, ScanPlan& plan, cudaStream_t st, std::vect
 // (if set): the host clock once the descriptors are queued.  A launch that fails is reported as "<what> launch failed".
 int launch_chunks(pb200_ctx* ctx, cudaStream_t st, const ScanPlan& plan, DevBufRaw& dsegs, EventPair& ev, const char* what,
                   uint32_t* mask, const long long* chunk_word_off, double* t_launch);
+
+// ---- expression aggregations (pb200_execute_exprs, pb200_expr.cu) ----
+// The expression aggregations of one call: the scan runs each as COUNT(*), pb200_expr.cu computes its value.
+struct ExprCall {
+  ExprCall() { std::fill(fn_of, fn_of + kMaxAggs, -1); }
+  int count = 0;                                 // expression aggregations
+  int fn_of[kMaxAggs];                           // aggregation -> PB200_AGG_SUM / AVG / MIN / MAX (-1: not an expression)
+  std::vector<pb200_transform_op> ops[kMaxAggs]; // device programs: PB200_T_COLUMN i = index into cols
+  std::vector<int> cols;                         // the distinct leaf column ids
+};
+// where one result's expression values go: per aggregation a table of `groups` entries (group-by) or one word
+// (aggregation only) -- f64 sums, or u64 Double.compare keys for MIN / MAX -- and the hash table keys (NULL: dense)
+struct ExprOut { void* out[kMaxAggs] = {}; const unsigned long long* hkeys = nullptr; };
+// Validates the programs against the segments and fills `out`; PB200_OK or the code of pb200_execute_exprs (no CUDA call).
+int expr_prepare(const pb200_query* query, const pb200_expr_program* exprs, pb200_segment* const* segments, int nseg, ExprCall* out);
+// Queues the mask scan (none when the filter matches every doc) and the expression pass on `st`, behind the scan of
+// `plan`; filter_query = the query the scan ran.  Device scratch stays in `temps` until the caller's synchronisation.
+int expr_launch(pb200_ctx* ctx, cudaStream_t st, const Tuning& tune, const pb200_query* filter_query, pb200_segment* const* segments,
+                int nseg, const ScanPlan& plan, const ExprCall& x, const std::vector<ExprOut>& outs,
+                std::vector<std::unique_ptr<DevBufRaw>>& temps);
 
 // pb200_select.cu: one scan launch of a selection plan on `st`: fills `mask` (p.mask_words words) and the matched docs of
 // each segment, adds the scan's CUDA-event time to *ms; ends in a stream synchronisation.

@@ -33,7 +33,7 @@ from __future__ import annotations
 import ctypes as C
 from typing import Dict, List, Optional, Sequence
 
-from .query import DISTINCT_SET_FUNCTIONS, distinct_final
+from .query import DISTINCT_SET_FUNCTIONS, distinct_final, is_multi_column_expression
 
 
 KINDS = {"i64": 0, "f64": 1, "u32max": 2, "u32min": 3}
@@ -235,6 +235,10 @@ def execute_and_combine(plan_maker_or_backend, segments: Sequence, query, dist, 
         # per-GPU moments are not reduced across GPUs: the caller runs the query per GPU and merges them by value
         from ._lib import E_UNSUPPORTED, UnsupportedQueryError
         raise UnsupportedQueryError(E_UNSUPPORTED, "VAR/STDDEV is not combined across GPUs")
+    if query.is_group_by and any(is_multi_column_expression(a.function, a.column) for a in query.aggregations):
+        # the expression tables are not among the reduced table blocks: the caller runs the query per GPU and merges by key
+        from ._lib import E_UNSUPPORTED, UnsupportedQueryError
+        raise UnsupportedQueryError(E_UNSUPPORTED, "expression aggregations with GROUP BY are not combined across GPUs")
     backend = plan_maker_or_backend if hasattr(plan_maker_or_backend, "finish") else DeviceBackend(plan_maker_or_backend)
     world = dist.get_world_size()
     if any(a.function in DISTINCT_SET_FUNCTIONS for a in query.aggregations):

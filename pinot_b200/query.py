@@ -12,6 +12,7 @@ Predicates are in VALUE space here (as the broker sends them); turning them into
 from __future__ import annotations
 
 import math
+import re
 import struct
 from dataclasses import dataclass, field
 from fractions import Fraction
@@ -378,3 +379,20 @@ def postfix(node: Optional[FilterNode]) -> Sequence[FilterNode]:
     if node is not None:
         walk(node)
     return out
+
+
+_EXPR_TOKEN = re.compile(r"'(?:[^']|'')*'|[A-Za-z_$][\w$.]*|[0-9.][0-9.]*(?:[eE][+-]?[0-9]+)?|\S")
+
+
+def is_multi_column_expression(function: str, column) -> bool:
+    """SUM / AVG / MIN / MAX over an expression with two or more column leaves (DESIGN.md section 3.15): computed per row
+    on the device, not derived; the same test as the library's (a name followed by '(' is a function, a quoted or numeric
+    token a literal, any other name a column)."""
+    if function not in ("SUM", "AVG", "MIN", "MAX") or not column or "(" not in column:
+        return False
+    tokens = _EXPR_TOKEN.findall(column)
+    leaves = 0
+    for k, t in enumerate(tokens):
+        if (t[0].isalpha() or t[0] in "_$") and not (k + 1 < len(tokens) and tokens[k + 1] == "("):
+            leaves += 1
+    return leaves >= 2
