@@ -525,6 +525,35 @@ typedef struct {
 int32_t pb200_execute_exprs(pb200_ctx* ctx, const pb200_query* query, const pb200_order_by* order, const pb200_agg_arg* args,
                             const pb200_having* having, const pb200_expr_program* exprs, pb200_segment* const* segments,
                             int32_t num_segments, pb200_result** results);
+
+/* ---- predicates on expressions of two or more columns: WHERE a > b, WHERE price * qty > 1000 (DESIGN.md section 3.16) -- */
+/* One predicate on the value of a pb200_expr_program (the rules of pb200_execute_exprs: 2 .. 8 column leaves by column
+ * id, every leaf a double, every operation one IEEE-754 step without FMA).  The value is compared as a DOUBLE with Java's
+ * <, > and ==: NaN matches only NEQ and NOT_IN, 0.0 matches both zeros.  RANGE takes lo / hi with `flags` as
+ * pb200_filter_node.raw_flags (bit0 lower unbounded, bit1 upper unbounded, bit2 lower exclusive, bit3 upper exclusive);
+ * EQ / NEQ compare values[0], IN / NOT_IN values[0 .. num_values). */
+enum { PB200_EXPR_EQ = 0, PB200_EXPR_NEQ = 1, PB200_EXPR_IN = 2, PB200_EXPR_NOT_IN = 3, PB200_EXPR_RANGE = 4 };
+#define PB200_MAX_EXPR_VALUES 1024 /* values of one EQ / NEQ / IN / NOT_IN predicate */
+typedef struct {
+  pb200_expr_program program;
+  int32_t op;                 /* PB200_EXPR_* */
+  int32_t flags;              /* RANGE: raw_flags bits; 0 otherwise */
+  double lo, hi;              /* RANGE bounds */
+  int32_t num_values;         /* EQ / NEQ: 1; IN / NOT_IN: 1 .. PB200_MAX_EXPR_VALUES; RANGE: 0 */
+  int32_t reserved;           /* 0 */
+  const double* values;       /* host pointer */
+} pb200_expr_predicate;
+/* The doc set of each predicate on each segment, as device masks for PB200_F_DOC_MASK | PB200_NODE_IDS_ON_DEVICE leaves:
+ * masks[p * num_segments + s] is predicate p on segment s, bit j of word w = doc 32 * w + j, words past the segment's
+ * docs zero, in the padded layout pb200_doc_mask_upload makes.  Every doc of every segment is evaluated, in one launch;
+ * the call synchronises once before it returns, so the masks can be read from any stream.  Each segment reads the leaves
+ * through its own dictionary (a bound segment through the domain's, which holds the same values), so merged submissions
+ * need no shared dictionary for them.  Release every mask with pb200_doc_mask_free.  On an error no mask is returned.
+ * PB200_E_INVALID: a malformed program, an unknown op, a column id out of range, bad value counts or flags.
+ * PB200_E_UNSUPPORTED (the caller runs the stock operator): a STRING leaf or one without dictIds or raw 32-bit values, a
+ * time function in the program, fewer than two or more than 8 column leaves, more than PB200_MAX_EXPR_VALUES values. */
+int32_t pb200_expr_doc_masks(pb200_ctx* ctx, int32_t num_predicates, const pb200_expr_predicate* predicates,
+                             pb200_segment* const* segments, int32_t num_segments, uint32_t** masks);
 /* Adds the derived column `program(source_column)` to the segment and returns its column id (the next free id, after
  * the registered and earlier derived columns).  The source must carry dictIds: INT / LONG / FLOAT / DOUBLE dictionaries,
  * raw columns whose dictionary was synthesised at load, or a column bound to a domain (the program then runs over the

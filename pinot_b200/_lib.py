@@ -174,6 +174,14 @@ class ExprProgram(C.Structure):  # pb200_expr_program
     _fields_ = [("num_ops", C.c_int32), ("reserved", C.c_int32), ("ops", C.POINTER(TransformOp))]
 
 
+EXPR_OPS = {"EQ": 0, "NEQ": 1, "IN": 2, "NOT_IN": 3, "RANGE": 4}   # PB200_EXPR_*
+
+
+class ExprPredicate(C.Structure):  # pb200_expr_predicate
+    _fields_ = [("program", ExprProgram), ("op", C.c_int32), ("flags", C.c_int32), ("lo", C.c_double), ("hi", C.c_double),
+                ("num_values", C.c_int32), ("reserved", C.c_int32), ("values", C.POINTER(C.c_double))]
+
+
 class HStarMetric(C.Structure):
     _fields_ = [("function", C.c_int32), ("reserved", C.c_int32), ("column", C.c_char_p), ("fwd", C.c_void_p),
                 ("fwd_bytes", C.c_uint64)]
@@ -215,7 +223,7 @@ EXPORTED_SYMBOLS = [
     "pb200_segment_derive_column", "pb200h_segment_derive",
     "pb200h_startree_build", "pb200h_startree_get",
     "pb200_execute_having", "pb200h_execute_having", "pb200_execute_agg_args", "pb200h_execute_agg_args",
-    "pb200_match_pattern", "pb200_result_exact_sum", "pb200_execute_exprs",
+    "pb200_match_pattern", "pb200_result_exact_sum", "pb200_execute_exprs", "pb200_expr_doc_masks",
 ]
 
 _LIB = None
@@ -249,6 +257,7 @@ def load() -> C.CDLL:
                                          C.POINTER(vp), i32, C.POINTER(vp)]
     L.pb200_execute_exprs.argtypes = [vp, C.POINTER(Query), C.POINTER(OrderBy), C.POINTER(AggArg), C.POINTER(Having),
                                       C.POINTER(ExprProgram), C.POINTER(vp), i32, C.POINTER(vp)]
+    L.pb200_expr_doc_masks.argtypes = [vp, i32, C.POINTER(ExprPredicate), C.POINTER(vp), i32, C.POINTER(vp)]
     L.pb200_result_histogram.restype = i64
     L.pb200_result_histogram.argtypes = [vp, i32, i32, vp, vp, i64]
     L.pb200_result_moments.argtypes = [vp, i32, i32, vp, vp, vp, vp, vp, vp, vp]

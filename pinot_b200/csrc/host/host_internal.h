@@ -224,4 +224,36 @@ int resolve_patterns(pb200_ctx* ctx, const pb200h_query& q, pb200h_segment* cons
 const std::vector<int32_t>* pattern_ids(const HostColumn& c, const char* pattern);
 // Makes `to` (a star-tree dimension, sharing `from`'s dictionary) resolve `pattern` as `from` does, when `from` does
 void pattern_alias(const HostColumn& from, const HostColumn& to, const char* pattern);
+
+// expr_filters.cpp: predicates on expressions of two or more columns (DESIGN.md section 3.16).  Their doc sets are
+// computed on the device (pb200_expr_doc_masks) before a call is planned and kept in a scope shaped like PatternScope:
+// an entry point declares one, fills it with resolve_expr_filters, and build_segment_filter finds a leaf's mask with
+// expr_filter_mask, searching the thread's scopes innermost first, so a FILTER clause's submission reuses its caller's
+// masks.  The scope frees its masks when the entry point's frame ends.
+struct ExprFilterScope {
+  struct Mask { std::string key; const pb200h_segment* seg; uint32_t* mask; int ncols; };
+  std::vector<Mask> masks;
+  pb200_ctx* ctx = nullptr;
+  ExprFilterScope* outer;
+  ExprFilterScope();
+  ~ExprFilterScope();
+  ExprFilterScope(const ExprFilterScope&) = delete;
+  ExprFilterScope& operator=(const ExprFilterScope&) = delete;
+};
+// `text` names an expression with two or more DISTINCT column leaves: as a filter leaf it is evaluated per row, never
+// derived (an expression over one column, even used twice, stays a derived column)
+bool is_expression_filter(const char* text);
+// Every expression leaf of the query's filter and FILTER clauses: compiled, checked, and (launch) one pb200_expr_doc_masks
+// call for the distinct (expression, predicate) pairs no scope of the thread holds yet, one mask per segment.
+// PB200_E_UNSUPPORTED: REGEXP_LIKE / LIKE on an expression, a string literal, what compile_multi_expression and
+// pb200_expr_doc_masks refuse; PB200_E_INVALID: an unknown leaf column or one at different positions in the segments.
+int resolve_expr_filters(pb200_ctx* ctx, const pb200h_query& q, pb200h_segment* const* segs, int nseg, ExprFilterScope& scope,
+                         bool launch);
+// The leaf's canonical text and, when a scope of the thread resolved it on `seg`, its device mask and the number of its
+// distinct leaf columns (mask NULL otherwise); PB200_E_* when the leaf does not compile
+int expr_filter_mask(const pb200h_segment& seg, const pb200h_filter_node& n, const pb200h_literal* lits, std::string* canonical,
+                     const uint32_t** mask, int* ncols);
+// num_docs x distinct leaf columns of every expression leaf of the query's filter, on one segment (the statistics the
+// mask pass adds to num_entries_scanned_in_filter)
+long long expr_filter_entries(const pb200h_segment& seg, const pb200h_query& q);
 }  // namespace pb200h

@@ -47,6 +47,7 @@ int resolve_patterns(pb200_ctx* ctx, const pb200h_query& q, pb200h_segment* cons
   for (const pb200h_filter_node* n : leaves) {
     if (n->num_values != 1 || !q.literals || !q.literals[n->values_offset].s) { set_error("REGEXP_LIKE leaf needs one string literal (the pattern)"); return PB200_E_INVALID; }
     const char* pattern = q.literals[n->values_offset].s;
+    if (is_expression_filter(n->column)) { set_error("REGEXP_LIKE / LIKE on the expression '%s' is not accelerated", n->column); return PB200_E_UNSUPPORTED; }
     std::vector<pb200_segment*> dev(nseg);
     std::vector<int32_t> cols(nseg);
     std::vector<const HostColumn*> hcols(nseg);

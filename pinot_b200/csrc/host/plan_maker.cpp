@@ -206,6 +206,25 @@ int build_segment_filter(const pb200h_segment& seg, const pb200h_query& q, Segme
       text.back() = c == 1 ? "FILTER_EMPTY" : c == 2 ? "FILTER_MATCH_ENTIRE_SEGMENT" : "FILTER_NOT(" + text.back() + ")";
       continue;
     }
+    const char* pname = n.type == PB200H_RANGE ? "RANGE" : n.type == PB200H_EQ ? "EQ" : n.type == PB200H_NEQ ? "NOT_EQ" : n.type == PB200H_IN ? "IN" : n.type == PB200H_NOT_IN ? "NOT_IN" : "REGEXP_LIKE";
+    if (is_expression_filter(n.column)) {
+      // an expression over several columns (DESIGN.md section 3.16): the doc set its call computed on the device, the
+      // same leaf in every segment and never folded to a constant
+      std::string canonical;
+      const uint32_t* mask = nullptr;
+      int ncols = 0;
+      if (n.type == PB200H_REGEXP_LIKE) { set_error("REGEXP_LIKE / LIKE on the expression '%s' is not accelerated", n.column); return PB200_E_UNSUPPORTED; }
+      if (int rc = expr_filter_mask(seg, n, q.literals, &canonical, &mask, &ncols)) return rc;
+      if (!mask && !explain) { set_error("predicate on the expression '%s' was not resolved before planning", n.column); return PB200_E_INVALID; }
+      d.op = PB200_F_DOC_MASK;
+      d.column = -1;
+      d.ids = reinterpret_cast<const int32_t*>(mask);
+      d.num_ids = (int32_t)pb200::doc_mask_words(seg.num_docs);
+      d.reserved = PB200_NODE_IDS_ON_DEVICE;
+      constant.push_back(0);
+      text.push_back(std::string("FILTER_EXPRESSION(") + pname + "," + canonical + ")");
+      continue;
+    }
     const int ci = seg.column_index(n.column);
     if (ci < 0) { set_error("unknown column '%s'", n.column ? n.column : "(null)"); return PB200_E_INVALID; }
     const HostColumn& c = seg.cols[ci];
@@ -227,7 +246,6 @@ int build_segment_filter(const pb200h_segment& seg, const pb200h_query& q, Segme
       d.ids = out.id_store.back()->data();
       d.num_ids = (int)out.id_store.back()->size();
     };
-    const char* pname = n.type == PB200H_RANGE ? "RANGE" : n.type == PB200H_EQ ? "EQ" : n.type == PB200H_NEQ ? "NOT_EQ" : n.type == PB200H_IN ? "IN" : n.type == PB200H_NOT_IN ? "NOT_IN" : "REGEXP_LIKE";
     if (c.is_sorted) {  // FilterOperatorUtils :98-101,117-120
       store(sorted_doc_ranges(c, e, seg.num_docs));
       d.op = PB200_F_DOC_RANGES;
@@ -730,11 +748,13 @@ extern "C" int32_t pb200h_segment_load_dir(pb200_ctx* ctx, const char* path, pb2
 extern "C" int32_t pb200h_explain(pb200_ctx* ctx, const pb200h_query* q, pb200h_segment* seg, char* out, int32_t cap) {
   if (!q || !seg || !out || cap <= 0) { set_error("null argument"); return PB200_E_INVALID; }
   PatternScope patterns;
+  pb200h_segment* one = seg;
   if (ctx) {
-    pb200h_segment* one = seg;
     if (int rc = derive_query_names(ctx, *q, &one, 1, nullptr, 0)) return rc;
     if (int rc = resolve_patterns(ctx, *q, &one, 1, patterns)) return rc;
   }
+  ExprFilterScope exprs;   // checked only: explain names an expression leaf without computing its doc set
+  if (int rc = resolve_expr_filters(ctx, *q, &one, 1, exprs, false)) return rc;
   SegmentFilter f;
   std::string text;
   int rc = build_segment_filter(*seg, *q, f, &text);
@@ -825,6 +845,8 @@ extern "C" int32_t pb200h_execute_agg_args(pb200_ctx* ctx, const pb200h_query* q
       set_error("DISTINCTSUM/DISTINCTAVG in a query with FILTER (WHERE ...) clauses is not accelerated");
       return PB200_E_UNSUPPORTED;
     }
+  ExprFilterScope expr_filters;   // expression leaves become device doc sets once, also for the FILTER clauses' submissions
+  if (int rc = resolve_expr_filters(ctx, *q, segs, nseg, expr_filters, true)) return rc;
   if (q->agg_filter_count && q->agg_filter_start && q->agg_filter_nodes)
     for (int a = 0; a < q->num_aggs; a++)
       if (q->agg_filter_count[a] > 0) return execute_filtered(ctx, *q, order, having, segs, nseg, results, kinds);  // host/filtered_agg.cpp
@@ -950,6 +972,8 @@ extern "C" int32_t pb200h_execute_agg_args(pb200_ctx* ctx, const pb200h_query* q
     int rc = any_expr ? pb200_execute_exprs(ctx, &dq, order, args ? dev_args.data() : nullptr, having, programs.data(), dsegs.data(), (int)dsegs.size(), dev_results.data())
                       : pb200_execute_agg_args(ctx, &dq, order, args ? dev_args.data() : nullptr, having, dsegs.data(), (int)dsegs.size(), dev_results.data());
     if (rc) { for (auto r : star_results) if (r) pb200_result_free(r); return rc; }
+    // the mask pass of each expression leaf read its leaf columns at every doc of the segment
+    for (size_t k = 0; k < dev_idx.size(); k++) dev_results[merge ? 0 : k]->meta.num_entries_scanned_in_filter += expr_filter_entries(*segs[dev_idx[k]], *q);
   }
   if (merge) { results[0] = dev_results[0]; return PB200_OK; }
   size_t di = 0;
@@ -992,6 +1016,8 @@ int32_t execute_rows(pb200_ctx* ctx, const pb200h_query* q, const pb200h_selecti
   }
   PatternScope patterns;
   if (int rc = resolve_patterns(ctx, *q, segs, nseg, patterns)) return rc;
+  ExprFilterScope expr_filters;
+  if (int rc = resolve_expr_filters(ctx, *q, segs, nseg, expr_filters, true)) return rc;
   const pb200h_segment& s0 = *segs[0];
   std::vector<int32_t> cols(sel->num_columns);
   for (int k = 0; k < sel->num_columns; k++) {
@@ -1037,6 +1063,7 @@ int32_t execute_rows(pb200_ctx* ctx, const pb200h_query* q, const pb200h_selecti
     dq.filter = flat.data();
     int rc = device(ctx, &dq, &dsel, dsegs.data(), (int)dsegs.size(), merge ? PB200_Q_MERGE_SEGMENTS : 0, dev_results.data());
     if (rc) return rc;
+    for (size_t k = 0; k < dev_idx.size(); k++) dev_results[merge ? 0 : k]->meta.num_entries_scanned_in_filter += expr_filter_entries(*segs[dev_idx[k]], *q);
     // rows name their segment by its position in the device submission: map it back to `segs`
     for (pb200_result* R : dev_results)
       for (int64_t i = 0; i < R->selection.rows; i++) R->selection.segment_index[i] = dev_idx[R->selection.segment_index[i]];

@@ -333,6 +333,18 @@ bool is_multi_column_expression(const char* text) {
   return multi;
 }
 
+bool is_expression_filter(const char* text) {
+  if (!text || !strchr(text, '(')) return false;
+  Compiled c;
+  char saved[1024];
+  memcpy(saved, pb200_last_error(), sizeof saved);
+  bool multi = compile_text(text, c, true) == PB200_OK;
+  set_error("%s", saved);
+  if (!multi) return false;
+  for (const std::string& l : c.leaves) if (l != c.leaves[0]) return true;
+  return false;
+}
+
 bool normalize_expression(const char* text, std::string* canonical) {
   Compiled c;
   char saved[1024];
@@ -365,7 +377,9 @@ int derive_names(pb200_ctx* ctx, pb200h_segment* const* segs, int nseg, const st
 
 int derive_query_names(pb200_ctx* ctx, const pb200h_query& q, pb200h_segment* const* segs, int nseg, const char* const* extra, int nextra) {
   std::vector<const char*> names;
-  for (int i = 0; i < q.num_filter_nodes; i++) if (q.filter[i].type >= PB200H_EQ) names.push_back(q.filter[i].column);
+  // a leaf on an expression over several columns is evaluated per row (expr_filters.cpp), not derived
+  for (int i = 0; i < q.num_filter_nodes; i++)
+    if (q.filter[i].type >= PB200H_EQ && !is_expression_filter(q.filter[i].column)) names.push_back(q.filter[i].column);
   for (int g = 0; g < q.num_group_by; g++) names.push_back(q.group_by[g]);
   for (int a = 0; a < q.num_aggs; a++)   // an expression over several columns is computed per row, not derived
     if (q.aggs && q.aggs[a].function != PB200_AGG_COUNT && !(expression_function(q.aggs[a].function) && is_multi_column_expression(q.aggs[a].column)))
@@ -374,7 +388,7 @@ int derive_query_names(pb200_ctx* ctx, const pb200h_query& q, pb200h_segment* co
     for (int a = 0; a < q.num_aggs; a++)
       for (int k = 0; k < q.agg_filter_count[a]; k++) {
         const pb200h_filter_node& n = q.agg_filter_nodes[q.agg_filter_start[a] + k];
-        if (n.type >= PB200H_EQ) names.push_back(n.column);
+        if (n.type >= PB200H_EQ && !is_expression_filter(n.column)) names.push_back(n.column);
       }
   for (int k = 0; k < nextra; k++) names.push_back(extra[k]);
   return derive_names(ctx, segs, nseg, names);

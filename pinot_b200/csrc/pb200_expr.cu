@@ -12,6 +12,10 @@
 //      Lanes of a warp that hit one entry are combined first (one atomic per entry and warp word); aggregation-only
 //      results reduce in registers and once per block.
 // Both launches are queued on the call's stream behind the scan; neither synchronises.
+//
+// Predicates on such expressions (DESIGN.md section 3.16, pb200_expr_doc_masks) run before the query is planned:
+// expr_mask_kernel evaluates every doc of every segment against each predicate and writes the doc mask that the query's
+// filter tree then reads as a PB200_F_DOC_MASK leaf.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -197,6 +201,50 @@ __global__ void __launch_bounds__(kExprThreads) expr_kernel(const ExprSeg* __res
   }
 }
 
+// ---- predicates on expressions (DESIGN.md section 3.16): the doc-mask pass ----
+struct MaskJob {                    // one (predicate, segment)
+  uint32_t* mask;                   // doc_mask_words(num_docs) words
+  long long num_docs, words;
+  int32_t ncols, pad;
+  SelCol col[kExprMaxLeaves];       // the predicate's distinct leaf columns in this segment
+};
+struct MaskPred {
+  int32_t len, op, flags, nvalues;
+  long long voff;                   // first value in the call's value array
+  double lo, hi;
+  pb200_transform_op ops[kTransformMaxProgram];
+};
+
+// grid: (blocks per job, jobs); jobs are predicate-major, so block row y is predicate y / nseg.  One warp per 32-doc word:
+// each lane evaluates its doc, the ballot is the word, lane 0 stores it.  Every word of the padded mask is written.
+__global__ void __launch_bounds__(kExprThreads) expr_mask_kernel(const MaskJob* __restrict__ jobs, const MaskPred* __restrict__ preds,
+                                                                const double* __restrict__ values, int nseg) {
+  extern __shared__ double vals[];
+  __shared__ MaskPred p;
+  const MaskJob& j = jobs[blockIdx.y];
+  {
+    const uint32_t* src = reinterpret_cast<const uint32_t*>(preds + blockIdx.y / nseg);
+    uint32_t* dst = reinterpret_cast<uint32_t*>(&p);
+    for (int i = threadIdx.x; i < (int)(sizeof(MaskPred) / 4); i += blockDim.x) dst[i] = src[i];
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < p.nvalues; i += blockDim.x) vals[i] = values[p.voff + i];
+  __syncthreads();
+  const int lane = threadIdx.x & 31;
+  const long long nwarps = (long long)gridDim.x * (kExprThreads / 32);
+  double v[kExprMaxLeaves];
+  for (long long w = (long long)blockIdx.x * (kExprThreads / 32) + (threadIdx.x >> 5); w < j.words; w += nwarps) {
+    const long long doc = 32 * w + lane;
+    bool hit = false;
+    if (doc < j.num_docs) {
+      for (int c = 0; c < j.ncols; ++c) v[c] = leaf_value(j.col[c], (int32_t)doc);
+      hit = expr_matches(p.op, p.flags, p.lo, p.hi, vals, p.nvalues, expr_eval(p.ops, p.len, v));
+    }
+    const unsigned word = __ballot_sync(0xFFFFFFFFu, hit);
+    if (lane == 0) j.mask[w] = word;
+  }
+}
+
 // how the pass reads a leaf column: selection's rule, STRING excluded (-1: not readable as a number)
 int leaf_kind(const DeviceColumn& dc) { return dc.stored_type == PB200_STRING ? -1 : selection_kind(dc); }
 
@@ -359,3 +407,117 @@ int expr_launch(pb200_ctx* ctx, cudaStream_t st, const Tuning& tune, const pb200
 }
 
 }  // namespace pb200
+
+// ---- pb200_expr_doc_masks --------------------------------------------------------------------------------------------
+namespace pb200 {
+namespace {
+
+// Checks the predicates and fills the pass's descriptors (no CUDA call); PB200_OK or the code of pb200_expr_doc_masks
+int mask_prepare(const pb200_expr_predicate* preds, int n, pb200_segment* const* segments, int nseg, std::vector<MaskPred>& mp,
+                 std::vector<MaskJob>& jobs, std::vector<double>& values) {
+  const int ncols = common_columns(segments, nseg);
+  if (ncols < 0) { set_error("segments do not share their registered columns"); return PB200_E_INVALID; }
+  if ((long long)n * nseg > kMaxSelectSegments) { set_error("%d predicates over %d segments: at most %d per call", n, nseg, kMaxSelectSegments); return PB200_E_UNSUPPORTED; }
+  mp.assign(n, MaskPred());
+  jobs.assign((size_t)n * nseg, MaskJob());
+  for (int p = 0; p < n; p++) {
+    const pb200_expr_predicate& e = preds[p];
+    if (e.reserved != 0 || e.program.reserved != 0 || e.program.num_ops <= 0 || !e.program.ops) { set_error("predicate %d: malformed expression program", p); return PB200_E_INVALID; }
+    const char* why = "";
+    int leaves = 0;
+    if (int rc = expr_check(e.program.ops, e.program.num_ops, &leaves, &why)) { set_error("predicate %d: %s", p, why); return rc; }
+    if (e.op < PB200_EXPR_EQ || e.op > PB200_EXPR_RANGE) { set_error("predicate %d: unknown op %d", p, e.op); return PB200_E_INVALID; }
+    if (e.op == PB200_EXPR_RANGE ? (e.flags & ~15) != 0 || e.num_values != 0 : e.flags != 0) { set_error("predicate %d: bad flags or values for its op", p); return PB200_E_INVALID; }
+    if (e.op != PB200_EXPR_RANGE) {
+      const bool one = e.op == PB200_EXPR_EQ || e.op == PB200_EXPR_NEQ;
+      if (e.num_values < 1 || (one && e.num_values != 1) || !e.values) { set_error("predicate %d: %d values", p, e.num_values); return PB200_E_INVALID; }
+      if (e.num_values > PB200_MAX_EXPR_VALUES) { set_error("predicate %d: %d values (at most %d)", p, e.num_values, PB200_MAX_EXPR_VALUES); return PB200_E_UNSUPPORTED; }
+    }
+    MaskPred& m = mp[p];
+    memset(&m, 0, sizeof m);
+    m.len = e.program.num_ops; m.op = e.op; m.flags = e.flags; m.lo = e.lo; m.hi = e.hi;
+    m.nvalues = e.op == PB200_EXPR_RANGE ? 0 : e.num_values;
+    m.voff = (long long)values.size();
+    values.insert(values.end(), e.values, e.values + m.nvalues);
+    std::vector<int> cols;   // distinct leaf columns: program leaf i reads cols[i]
+    for (int k = 0; k < m.len; k++) {
+      pb200_transform_op o = e.program.ops[k];
+      if (o.op == PB200_T_COLUMN) {
+        if (o.i >= ncols) { set_error("predicate %d: column %lld out of range", p, (long long)o.i); return PB200_E_INVALID; }
+        const int c = (int)o.i;
+        for (int s = 0; s < nseg; s++) {
+          const DeviceColumn& dc = segments[s]->cols[c];
+          if (dc.stored_type == PB200_STRING) { set_error("predicate %d: STRING column %d in an arithmetic expression", p, c); return PB200_E_UNSUPPORTED; }
+          if (leaf_kind(dc) < 0) { set_error("predicate %d: column %d of segment %d has no device dictionary or raw 32-bit values", p, c, s); return PB200_E_UNSUPPORTED; }
+        }
+        const auto at = std::find(cols.begin(), cols.end(), c);
+        o.i = at - cols.begin();
+        if (at == cols.end()) cols.push_back(c);
+      }
+      m.ops[k] = o;
+    }
+    for (int s = 0; s < nseg; s++) {
+      MaskJob& j = jobs[(size_t)p * nseg + s];
+      memset(&j, 0, sizeof j);
+      j.num_docs = segments[s]->num_docs;
+      j.words = (long long)doc_mask_words(j.num_docs);
+      j.ncols = (int)cols.size();
+      for (int c = 0; c < j.ncols; c++) {
+        const DeviceColumn& dc = segments[s]->cols[cols[c]];
+        j.col[c] = SelCol{dc.fwd, dc.dict_native, dc.bits, leaf_kind(dc), 0, 0};
+      }
+    }
+  }
+  return PB200_OK;
+}
+
+int mask_launch(pb200_ctx* ctx, int nseg, const std::vector<MaskPred>& mp, std::vector<MaskJob>& jobs,
+                const std::vector<double>& values, std::vector<uint32_t*>& out) {
+  PB200_CUDA(cudaSetDevice(ctx->device));
+  long long max_words = 1;
+  int max_values = 0;
+  for (size_t k = 0; k < jobs.size(); k++) {
+    void* p = nullptr;
+    if (int rc = dev_alloc(ctx, (size_t)jobs[k].words * 4, &p)) return rc;
+    out[k] = jobs[k].mask = static_cast<uint32_t*>(p);
+    max_words = std::max(max_words, jobs[k].words);
+  }
+  for (const MaskPred& m : mp) max_values = std::max(max_values, m.nvalues);
+  StreamLease st(ctx);
+  DevBufRaw djobs(ctx), dpreds(ctx), dvals(ctx);
+  if (int rc = djobs.alloc(sizeof(MaskJob) * jobs.size())) return rc;
+  if (int rc = dpreds.alloc(sizeof(MaskPred) * mp.size())) return rc;
+  if (int rc = dvals.alloc(std::max<size_t>(values.size(), 1) * sizeof(double))) return rc;
+  PB200_CUDA(cudaMemcpyAsync(djobs.p, jobs.data(), sizeof(MaskJob) * jobs.size(), cudaMemcpyHostToDevice, st));
+  PB200_CUDA(cudaMemcpyAsync(dpreds.p, mp.data(), sizeof(MaskPred) * mp.size(), cudaMemcpyHostToDevice, st));
+  if (!values.empty()) PB200_CUDA(cudaMemcpyAsync(dvals.p, values.data(), values.size() * sizeof(double), cudaMemcpyHostToDevice, st));
+  const long long per_job = std::max<long long>(2, (long long)ctx->sm_count * 8 / (long long)jobs.size());
+  const dim3 grid((unsigned)std::min<long long>((max_words + kExprThreads / 32 - 1) / (kExprThreads / 32), per_job), (unsigned)jobs.size());
+  expr_mask_kernel<<<grid, kExprThreads, (size_t)max_values * sizeof(double), st>>>(
+      static_cast<const MaskJob*>(djobs.p), static_cast<const MaskPred*>(dpreds.p), static_cast<const double*>(dvals.p), nseg);
+  PB200_CUDA(cudaGetLastError());
+  PB200_CUDA(cudaStreamSynchronize(st));   // once: the masks are complete for any stream that reads them
+  return PB200_OK;
+}
+
+}  // namespace
+}  // namespace pb200
+
+extern "C" int32_t pb200_expr_doc_masks(pb200_ctx* ctx, int32_t n, const pb200_expr_predicate* preds, pb200_segment* const* segments,
+                                        int32_t nseg, uint32_t** masks) {
+  using namespace pb200;
+  if (!ctx || n < 0 || (n > 0 && !preds) || !segments || nseg <= 0 || !masks) { set_error("invalid argument to pb200_expr_doc_masks"); return PB200_E_INVALID; }
+  for (int s = 0; s < nseg; s++) if (!segments[s]) { set_error("invalid argument to pb200_expr_doc_masks"); return PB200_E_INVALID; }
+  if (n == 0) return PB200_OK;
+  std::vector<MaskPred> mp;
+  std::vector<MaskJob> jobs;
+  std::vector<double> values;
+  if (int rc = mask_prepare(preds, n, segments, nseg, mp, jobs, values)) return rc;
+  std::vector<uint32_t*> out(jobs.size(), nullptr);
+  if (int rc = mask_launch(ctx, nseg, mp, jobs, values, out)) {
+    for (uint32_t* m : out) if (m) dev_free(ctx, m);
+    return rc;
+  }
+  std::copy(out.begin(), out.end(), masks);
+  return PB200_OK;
+}

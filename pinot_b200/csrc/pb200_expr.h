@@ -76,6 +76,21 @@ PB200_HD double expr_eval(const pb200_transform_op* ops, int n, const double* le
   return D[0];
 }
 
+// A predicate on an expression's value (DESIGN.md section 3.16), the rule of the reference's raw-value predicate evaluators
+// for a DOUBLE: Java's <, > and == against the literal's double.  So NaN matches only NEQ and NOT IN (and no range, not
+// even an unbounded one), and 0.0 matches both zeros.  `flags` carries pb200_filter_node.raw_flags' bits (bit0 lower
+// unbounded, bit1 upper unbounded, bit2 lower exclusive, bit3 upper exclusive); EQ / NEQ compare values[0].
+PB200_HD bool expr_matches(int op, int flags, double lo, double hi, const double* values, int nvalues, double x) {
+  if (op == PB200_EXPR_RANGE) {
+    if (!(flags & 1) && !((flags & 4) ? x > lo : x >= lo)) return false;
+    if (!(flags & 2) && !((flags & 8) ? x < hi : x <= hi)) return false;
+    return x == x;
+  }
+  bool hit = false;
+  for (int k = 0; k < nvalues; k++) hit |= x == values[k];
+  return (op == PB200_EXPR_EQ || op == PB200_EXPR_IN) ? hit : !hit;
+}
+
 // MIN / MAX accumulate the Double.compare order key (transform_key of a DOUBLE); a MIN entry starts at ~0 and a MAX entry
 // at 0, neither of which is the key of any double (every NaN has one key), so they mean "no row".
 constexpr unsigned long long kExprMinEmpty = ~0ull, kExprMaxEmpty = 0ull;

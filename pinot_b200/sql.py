@@ -21,6 +21,11 @@ stays Java).  This module exists so the parity tests read like the reference's
                   (every ORDER BY column must be a DISTINCT column)
     cond  := cond AND cond | cond OR cond | NOT cond | (cond) | col op literal | col BETWEEN a AND b
              | col [NOT] IN (literal, ...) | col [NOT] LIKE 'pattern' | REGEXP_LIKE(col, 'regex')
+             | literal op col | col op col
+             (the reference's PredicateComparisonRewriter: `literal op col` is `col op' literal` with the operator
+             mirrored, `a op b` with a non-literal right side is `minus(a,b) op 0`, so `a > b` names the expression
+             minus(a,b), evaluated per row when it has two or more columns -- DESIGN.md section 3.16.  BETWEEN bounds
+             and IN values must be literals)
              (LIKE is rewritten into REGEXP_LIKE by like_to_regexp; both only on STRING dictionary columns, never in
              HAVING)
     op    := = | != | <> | < | <= | > | >=
@@ -368,11 +373,23 @@ class _Parser:
                 raise SqlError("REGEXP_LIKE with match flags is not supported")
             self.expect_op(")")
             return Predicate("REGEXP_LIKE", col, [pat])
-        col = self.having_operand() if self.having is not None else self.column()
+        if self.having is not None:
+            col = self.having_operand()
+        else:
+            col, left_literal, left_value = self.operand()
+            if left_literal:   # PredicateComparisonRewriter: `literal op x` is `x op' literal`
+                k, op = self.peek()
+                if k != "op" or op not in _FLIPPED:
+                    raise SqlError(f"expected a comparison operator after the literal {col}")
+                self.i += 1
+                right, right_literal, _ = self.operand()
+                if right_literal:
+                    raise SqlError(f"a comparison of two literals ({col} {op} {right}) is not supported")
+                return _comparison(right, _FLIPPED[op], left_value)
         if self.take_kw("BETWEEN"):
-            lo = self.literal()
+            lo = self.bound("BETWEEN")
             self.expect_kw("AND")
-            hi = self.literal()
+            hi = self.bound("BETWEEN")
             return Predicate("RANGE", col, [], lo, hi, True, True)
         negate = self.take_kw("NOT")
         if self.take_kw("LIKE"):
@@ -382,9 +399,9 @@ class _Parser:
             return Filter("NOT", [leaf]) if negate else leaf
         if self.take_kw("IN"):
             self.expect_op("(")
-            vals = [self.literal()]
+            vals = [self.bound("IN")]
             while self.take_op(","):
-                vals.append(self.literal())
+                vals.append(self.bound("IN"))
             self.expect_op(")")
             return Predicate("NOT_IN" if negate else "IN", col, vals)
         if negate:
@@ -393,20 +410,49 @@ class _Parser:
         if k != "op":
             raise SqlError(f"expected comparison operator, got {self.peek()}")
         self.i += 1
-        v = self.literal()
-        if op == "=":
-            return Predicate("EQ", col, [v])
-        if op in ("!=", "<>"):
-            return Predicate("NEQ", col, [v])
-        if op == ">":
-            return Predicate("RANGE", col, [], v, None, False, True)
-        if op == ">=":
-            return Predicate("RANGE", col, [], v, None, True, True)
-        if op == "<":
-            return Predicate("RANGE", col, [], None, v, True, False)
-        if op == "<=":
-            return Predicate("RANGE", col, [], None, v, True, True)
-        raise SqlError(f"unsupported operator {op}")
+        if self.having is not None:
+            return _comparison(col, op, self.literal())
+        right, right_literal, v = self.operand()
+        if not right_literal:   # PredicateComparisonRewriter: `a op b` is `minus(a,b) op 0`
+            return _comparison(f"minus({col},{right})", op, 0)
+        return _comparison(col, op, v)
+
+    def operand(self):
+        """One side of a WHERE comparison: (canonical text, is it a literal, the literal's value or None)."""
+        start = self.i
+        text, is_literal = self._additive()
+        if not is_literal:
+            return text, False, None
+        if self.i != start + 1:
+            raise SqlError(f"the constant expression {text} in a comparison is not supported")
+        return text, True, self.toks[start][1]
+
+    def bound(self, what: str):
+        """A BETWEEN bound or an IN value: a literal (a column there is refused, as the reference's compiler does)."""
+        if self.peek()[0] not in ("num", "str"):
+            raise SqlError(f"{what} with a column or an expression among its {'bounds' if what == 'BETWEEN' else 'values'} "
+                           f"is not supported, got {self.peek()}")
+        return self.literal()
+
+
+# `literal op x` written as `x op' literal`
+_FLIPPED = {"=": "=", "!=": "!=", "<>": "<>", "<": ">", "<=": ">=", ">": "<", ">=": "<="}
+
+
+def _comparison(col: str, op: str, v) -> Predicate:
+    if op == "=":
+        return Predicate("EQ", col, [v])
+    if op in ("!=", "<>"):
+        return Predicate("NEQ", col, [v])
+    if op == ">":
+        return Predicate("RANGE", col, [], v, None, False, True)
+    if op == ">=":
+        return Predicate("RANGE", col, [], v, None, True, True)
+    if op == "<":
+        return Predicate("RANGE", col, [], None, v, True, False)
+    if op == "<=":
+        return Predicate("RANGE", col, [], None, v, True, True)
+    raise SqlError(f"unsupported operator {op}")
 
 
 def resolve_order_by(query: QueryContext) -> List[tuple]:
