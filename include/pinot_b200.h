@@ -200,14 +200,15 @@ typedef struct {
 #define PB200_NODE_IDS_ON_DEVICE 1
 
 /* Aggregation functions accelerated on this path (core/query/aggregation/function/{Count,Sum,Min,Max,Avg,
- * DistinctCount,Percentile,Variance,FirstWithTime,LastWithTime,DistinctSum,DistinctAvg}AggregationFunction.java).
+ * DistinctCount,Percentile,Variance,FirstWithTime,LastWithTime,DistinctSum,DistinctAvg,DistinctCountHLL}AggregationFunction.java).
  * PERCENTILE takes its percentile through pb200_execute_args; the four VarianceAggregationFunction types and
  * DISTINCTSUM / DISTINCTAVG take no argument (see pb200_result_moments and the DISTINCTSUM section below);
- * FIRSTWITHTIME / LASTWITHTIME take their time column through pb200_execute_agg_args. */
+ * FIRSTWITHTIME / LASTWITHTIME take their time column through pb200_execute_agg_args; DISTINCTCOUNTHLL takes an optional
+ * log2m through the same per-aggregation argument (see the DISTINCTCOUNTHLL section below). */
 enum { PB200_AGG_COUNT = 0, PB200_AGG_SUM = 1, PB200_AGG_MIN = 2, PB200_AGG_MAX = 3, PB200_AGG_AVG = 4,
        PB200_AGG_DISTINCTCOUNT = 5, PB200_AGG_PERCENTILE = 6, PB200_AGG_VARPOP = 7, PB200_AGG_VARSAMP = 8,
        PB200_AGG_STDDEVPOP = 9, PB200_AGG_STDDEVSAMP = 10, PB200_AGG_FIRSTWITHTIME = 11, PB200_AGG_LASTWITHTIME = 12,
-       PB200_AGG_DISTINCTSUM = 13, PB200_AGG_DISTINCTAVG = 14 };
+       PB200_AGG_DISTINCTSUM = 13, PB200_AGG_DISTINCTAVG = 14, PB200_AGG_DISTINCTCOUNTHLL = 15 };
 
 typedef struct {
   int32_t function; /* PB200_AGG_* */
@@ -395,6 +396,23 @@ int32_t pb200_result_moments(const pb200_result* result, int32_t agg, int32_t ro
  * PB200_E_UNSUPPORTED (the caller runs the stock operator): STRING columns, raw columns streamed as 32-bit values, FLOAT /
  * DOUBLE dictionaries off such a grid, the DISTINCTCOUNT bitset budget; a PB200_Q_MERGE_SEGMENTS submission needs the
  * column's dictionary to be the same in every segment.  Like DISTINCTCOUNT they are not reduced across GPUs on the device. */
+
+/* ---- DISTINCTCOUNTHLL(col[, log2m]): HyperLogLog estimates over DISTINCTCOUNT's value sets (DESIGN.md section 3.17) --- */
+/* PB200_AGG_DISTINCTCOUNTHLL through any pb200_execute* entry point.  log2m is agg_args[a] (pb200_execute_args,
+ * pb200_execute_having) or pb200_agg_arg.p (pb200_execute_agg_args): an integral value; 0, and every entry point without
+ * arguments, mean the reference's default 8.  Over S, the set of distinct values of the column in the group's matched rows
+ * (the set DISTINCTCOUNT counts; -0.0 and 0.0 are two members, all NaNs one), the result is the estimate of a HyperLogLog
+ * with 2^log2m registers offered every member of S (stream-lib's HyperLogLog.cardinality over MurmurHash.hash(value), as
+ * DistinctCountHLLAggregationFunction computes it): the registers depend only on S, so every route, schedule and knob gives
+ * the same estimate.  An empty S gives 0.  Several DISTINCTCOUNTHLLs, DISTINCTCOUNTs, DISTINCTSUMs and DISTINCTAVGs over one
+ * column share one bitset; DISTINCTCOUNTHLLs with the same log2m share one estimate.
+ * Results: pb200_result_agg gives the estimate in the long column and the same value as a double in the double column;
+ * pb200_result_distinct the dictId set, decoded on the first call for the aggregation (a caller that reads only the
+ * estimates never pays for the sets); ORDER BY and HAVING compare the double.
+ * PB200_E_INVALID: a log2m that is not integral or is outside 0..30 (the reference's range).
+ * PB200_E_UNSUPPORTED (the caller runs the stock operator): log2m outside 4..12, raw columns streamed as 32-bit values, a
+ * STRING dictionary with an entry that is not valid UTF-8, the DISTINCTCOUNT bitset budget; a PB200_Q_MERGE_SEGMENTS
+ * submission needs the column's dictionary to be the same in every segment.  Not reduced across GPUs on the device. */
 
 /* ---- selection: SELECT columns WHERE ... [ORDER BY columns] LIMIT n (SelectionOnlyOperator, SelectionOrderByOperator) -- */
 /* Without order items: per segment, the first `limit` matching docs in doc-id order with the values of the selected
@@ -597,8 +615,8 @@ int32_t pb200_result_group_keys(const pb200_result* result, int32_t* out);
 int32_t pb200_result_agg(const pb200_result* result, int32_t agg, double* out_double, int64_t* out_long);
 /* MIN/MAX as dictIds (dict-encoded columns; -1 when empty), for exact value lookup on the caller's side */
 int32_t pb200_result_agg_dict_ids(const pb200_result* result, int32_t agg, int32_t* out);
-/* DISTINCTCOUNT, DISTINCTSUM, DISTINCTAVG: the dictId set of row `row` (ascending); returns the count (or < 0 on error),
- * writes <= capacity */
+/* DISTINCTCOUNT, DISTINCTSUM, DISTINCTAVG, DISTINCTCOUNTHLL: the dictId set of row `row` (ascending); returns the count
+ * (or < 0 on error), writes <= capacity */
 int64_t pb200_result_distinct(const pb200_result* result, int32_t agg, int32_t row, int32_t* out, int64_t capacity);
 /* Everything of a result in ONE call (a JNI / ctypes round trip per accessor adds up when many small per-segment results
  * are read): keys [rows x num_group_by] (may be NULL), doubles / longs / dict_ids [num_aggs x rows] each (row-major by

@@ -225,7 +225,7 @@ int32_t pb200h_execute_having(pb200_ctx* ctx, const pb200h_query* query, const p
                               const pb200_having* having, pb200h_segment* const* segments, int32_t num_segments,
                               pb200_result** results, int32_t* operator_kinds);
 /* One argument per aggregation (pb200_agg_arg of include/pinot_b200.h, the time column by name): p is the percentile of a
- * PERCENTILE; time_column (a column or an expression such as "datetrunc('HOUR',ts)", derived like any other name) and
+ * PERCENTILE or the log2m of a DISTINCTCOUNTHLL (0: the default 8); time_column (a column or an expression such as "datetrunc('HOUR',ts)", derived like any other name) and
  * value_type (PB200_INT ... PB200_STRING) belong to a FIRSTWITHTIME / LASTWITHTIME over pb200h_agg.column. */
 typedef struct {
   double p;
@@ -238,6 +238,12 @@ typedef struct {
 int32_t pb200h_execute_agg_args(pb200_ctx* ctx, const pb200h_query* query, const pb200_order_by* order, const pb200h_agg_arg* args,
                                 const pb200_having* having, pb200h_segment* const* segments, int32_t num_segments,
                                 pb200_result** results, int32_t* operator_kinds);
+/* DISTINCTCOUNTHLL (the DISTINCTCOUNTHLL section of include/pinot_b200.h) through every entry point above, with the same
+ * refusals.  A segment whose filter matches every doc is answered without a scan (PB200H_OP_NON_SCAN_AGGREGATION, as the
+ * reference's NonScanBasedAggregationOperator does): the estimate over the whole dictionary, computed by the device
+ * finalize.  PB200_E_UNSUPPORTED as well: a query with FILTER (WHERE ...) clauses, an argument that is an expression of
+ * two or more columns; pb200h_result_to_datatable of a result with a DISTINCTCOUNTHLL (the reference serializes its
+ * registers, which this library does not restate).  A star-tree never answers it: the raw scan runs. */
 /* ---- selection (SELECT columns WHERE ... LIMIT n; pb200_execute_selection of include/pinot_b200.h) --------------- */
 typedef struct {
   const char* column;

@@ -16,7 +16,7 @@ OBJ = os.path.join(CSRC, "_obj")
 LIB = os.path.join(HERE, "libpinot_b200.so")
 SCAN_KERNELS = ["w6_agg", "w8_agg", "w8_agg_nodefer", "w6_gb1", "w8_gb1", "w6_gb2", "w8_gb2",  # one instantiation per TU
                 "w8_gb1_spec", "w6_gb2_spec"]
-SOURCES = [f"pb200_scan_k_{k}.cu" for k in SCAN_KERNELS] + ["pb200_api.cu", "pb200_plan.cpp", "pb200_select.cu", "pb200_distinct.cu", "pb200_percentile.cu", "pb200_withtime.cu", "pb200_expr.cu", "pb200_distinct_sum.cu", "pb200_moments.cu", "pb200_transform.cu", "pb200_domain.cu", "pb200_extract.cu", "pb200_comm.cu", "pb200_roaring.cu", "pb200_synth.cu", "pb200_startree_build.cu", "pb200_pattern.cu",
+SOURCES = [f"pb200_scan_k_{k}.cu" for k in SCAN_KERNELS] + ["pb200_api.cu", "pb200_plan.cpp", "pb200_select.cu", "pb200_distinct.cu", "pb200_percentile.cu", "pb200_withtime.cu", "pb200_expr.cu", "pb200_distinct_sum.cu", "pb200_hll.cu", "pb200_moments.cu", "pb200_transform.cu", "pb200_domain.cu", "pb200_extract.cu", "pb200_comm.cu", "pb200_roaring.cu", "pb200_synth.cu", "pb200_startree_build.cu", "pb200_pattern.cu",
                                                              "host/plan_maker.cpp", "host/star_tree.cpp", "host/datatable.cpp", "host/segment_cache.cpp", "host/raw_forward.cpp", "host/filtered_agg.cpp", "host/transform.cpp", "host/patterns.cpp",
                                                              "host/expr_filters.cpp"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")

@@ -7,7 +7,7 @@ What happens: ``pb200h_segment_load_dir`` per directory (v1 file-per-index or v3
 and dictionary-encoded at load, star-trees attached), ``pb200h_execute`` over all segments in one submission, then -- what the
 reference's combine + broker reduce do, in a few lines of Python -- the per-segment results blocks are merged by key VALUES
 (``AggregationFunction.merge``), final results extracted (AVG = sum / count, DISTINCTCOUNT = set size, DISTINCTSUM /
-DISTINCTAVG = the set's exact sum / mean rounded once), filtered by HAVING,
+DISTINCTAVG = the set's exact sum / mean rounded once, DISTINCTCOUNTHLL = the set's estimate), filtered by HAVING,
 ordered, and the first LIMIT rows printed.  With ``--merge-on-device`` the segments are first bound to one dictionary domain
 and combined on the GPU, where HAVING, ORDER BY and the trim run too.
 
@@ -23,7 +23,8 @@ from typing import Dict, List
 
 def merge_blocks(query, segments, blocks) -> Dict[tuple, list]:
     """{key values: [intermediate per aggregation]} over all blocks: COUNT -> int, SUM / MIN / MAX -> float,
-    AVG -> (sum, count), DISTINCTCOUNT / DISTINCTSUM / DISTINCTAVG -> set of values, PERCENTILE -> (p, {value: count}) from the per-segment
+    AVG -> (sum, count), DISTINCTCOUNT / DISTINCTSUM / DISTINCTAVG -> set of values, DISTINCTCOUNTHLL -> query.HllSet of
+    values, or its final estimate for a block merged on the device, PERCENTILE -> (p, {value: count}) from the per-segment
     histograms, or its final float for a block merged on the device, VAR / STDDEV -> exact (n, sum v, sum v^2) from the
     blocks' moments, each shifted from its own grid (c, e) to values, or the final float of a block merged on the device,
     FIRST/LASTWITHTIME -> (time value, data value) of the winning row or None for an empty block (query.withtime_pick: ties
@@ -31,7 +32,8 @@ def merge_blocks(query, segments, blocks) -> Dict[tuple, list]:
     (GroupByCombineOperator / AggregationFunction.merge).  Float keys, set members and histogram values are compared by
     identity (query.ValueKey: one NaN, -0.0 apart from 0.0) and MIN / MAX merge in Double.compare order, as the reference's
     Double.equals / doubleToLongBits keyed tables and its dictionary order do."""
-    from .query import DISTINCT_SET_FUNCTIONS, MOMENT_FUNCTIONS, WITHTIME_FUNCTIONS, merge_moments, value_key, value_order, withtime_pick
+    from .query import (DISTINCT_SET_FUNCTIONS, MOMENT_FUNCTIONS, WITHTIME_FUNCTIONS, HllSet, merge_moments, value_key, value_order,
+                        withtime_pick)
     out: Dict[tuple, list] = {}
     for seg, b in zip(segments, blocks):
         rows = 1 if b.num_groups < 0 else b.num_groups
@@ -46,6 +48,12 @@ def merge_blocks(query, segments, blocks) -> Dict[tuple, list]:
                     vals.append((float(b.doubles[a][g]), int(b.longs[a][g])))
                 elif fn in DISTINCT_SET_FUNCTIONS:
                     vals.append({value_key(seg.dictionary_value(agg.column, int(d))) for d in b.distinct[(a, g)]})
+                elif fn == "DISTINCTCOUNTHLL":
+                    if (a, g) in b.distinct:
+                        vals.append(HllSet((value_key(seg.dictionary_value(agg.column, int(d))) for d in b.distinct[(a, g)]),
+                                           seg.column_info(agg.column)["data_type"]))
+                    else:
+                        vals.append(int(b.longs[a][g]))
                 elif fn == "PERCENTILE" and (a, g) in b.histograms:
                     ids, counts = b.histograms[(a, g)]
                     hist: Dict[float, int] = {}
@@ -91,7 +99,8 @@ def final_rows(query, table: Dict[tuple, list]) -> List[list]:
     size) and breaks ties by the key values ascending, in GROUP BY column order -- the library's order.  Without ORDER BY
     Pinot returns an arbitrary LIMIT-sized subset; here the rows are sorted by key to make the output stable.  Hidden
     aggregations (named only in HAVING) are left out of the rows."""
-    from .query import DISTINCT_SET_FUNCTIONS, MOMENT_FUNCTIONS, distinct_final, having_eval, moments_final, percentile_of_counts, value_order
+    from .query import (DISTINCT_SET_FUNCTIONS, MOMENT_FUNCTIONS, distinct_final, having_eval, hll_final, moments_final, percentile_of_counts,
+                        value_order)
     from .sql import resolve_having, resolve_order_by
     items = resolve_order_by(query) if query.is_group_by else []
     having = resolve_having(query)
@@ -104,6 +113,8 @@ def final_rows(query, table: Dict[tuple, list]) -> List[list]:
                 vals.append(v[0] / v[1] if v[1] else float("-inf"))
             elif agg.function in DISTINCT_SET_FUNCTIONS:
                 vals.append(distinct_final(agg.function, v))
+            elif agg.function == "DISTINCTCOUNTHLL":
+                vals.append(hll_final(v, agg.arg, v.data_type) if isinstance(v, set) else v)
             elif agg.function == "PERCENTILE" and isinstance(v, tuple):
                 vals.append(percentile_of_counts(v))
             elif agg.function in MOMENT_FUNCTIONS and isinstance(v, tuple):
@@ -164,7 +175,7 @@ def main(argv=None) -> int:
                 cols = list(dict.fromkeys(list(query.group_by) + [a.column for a in query.aggregations
                                                                   if a.column and not is_multi_column_expression(a.function, a.column)
                                                                   and a.function in ("MIN", "MAX", "DISTINCTCOUNT", "PERCENTILE",
-                                                                                 "DISTINCTSUM", "DISTINCTAVG",
+                                                                                 "DISTINCTSUM", "DISTINCTAVG", "DISTINCTCOUNTHLL",
                                                                                  "VARPOP", "VARSAMP", "STDDEVPOP", "STDDEVSAMP",
                                                                                  "FIRSTWITHTIME", "LASTWITHTIME")]
                                            + [a.time_column for a in query.aggregations if a.time_column and "(" not in a.time_column]))

@@ -83,6 +83,11 @@ extern "C" int64_t pb200h_result_to_datatable(const pb200h_query* q, const pb200
     return PB200_E_UNSUPPORTED;
   }
   for (int a = 0; a < nagg; a++)
+    if (q->aggs[a].function == PB200_AGG_DISTINCTCOUNTHLL) {   // its intermediate is stream-lib's serialized registers
+      set_error("DISTINCTCOUNTHLL is not written as a server DataTable (the reference's HyperLogLog bytes are not restated)");
+      return PB200_E_UNSUPPORTED;
+    }
+  for (int a = 0; a < nagg; a++)
     if (q->aggs[a].function == PB200_AGG_PERCENTILE) {  // its intermediate is the reference's DoubleArrayList of values
       set_error("PERCENTILE intermediates are not written as DataTable objects");
       return PB200_E_UNSUPPORTED;

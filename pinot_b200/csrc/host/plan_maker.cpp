@@ -280,13 +280,14 @@ bool non_scan_answerable(const pb200h_segment& seg, const pb200h_query& q) {
   for (int a = 0; a < q.num_aggs; a++) {
     const pb200h_agg& ag = q.aggs[a];
     if (ag.function == PB200_AGG_COUNT) continue;
-    if (ag.function != PB200_AGG_MIN && ag.function != PB200_AGG_MAX && ag.function != PB200_AGG_DISTINCTCOUNT) return false;
+    const bool set_fn = ag.function == PB200_AGG_DISTINCTCOUNT || ag.function == PB200_AGG_DISTINCTCOUNTHLL;
+    if (ag.function != PB200_AGG_MIN && ag.function != PB200_AGG_MAX && !set_fn) return false;
     int ci = seg.column_index(ag.column);
     if (ci < 0 || !seg.cols[ci].has_dictionary) return false;
     // a derived column's dictionary may hold values absent from the segment (derived over a domain), and the reference
     // takes this shortcut for identifiers only
     if (seg.cols[ci].derived) return false;
-    if (ag.function != PB200_AGG_DISTINCTCOUNT && seg.cols[ci].data_type == PB200_STRING) return false;
+    if (!set_fn && seg.cols[ci].data_type == PB200_STRING) return false;
   }
   return true;
 }
@@ -321,10 +322,11 @@ pb200_result* host_result(const pb200h_segment& seg, const pb200h_query& q, bool
         d = ag.function == PB200_AGG_DISTINCTSUM ? 0.0 : -INFINITY;
         R->distinct[a].push_back({});
         break;
+      case PB200_AGG_DISTINCTCOUNTHLL:   // an empty S estimates 0; the whole dictionary's estimate is set by the caller
       case PB200_AGG_DISTINCTCOUNT: {
         std::vector<int32_t> ids;
         if (!empty) for (int i = 0; i < c->cardinality; i++) ids.push_back(c->to_device_id(i));
-        l = (int64_t)ids.size(); d = (double)l;
+        if (ag.function == PB200_AGG_DISTINCTCOUNT) { l = (int64_t)ids.size(); d = (double)l; }
         R->distinct[a].push_back(std::move(ids));
         break;
       }
@@ -845,6 +847,18 @@ extern "C" int32_t pb200h_execute_agg_args(pb200_ctx* ctx, const pb200h_query* q
       set_error("DISTINCTSUM/DISTINCTAVG in a query with FILTER (WHERE ...) clauses is not accelerated");
       return PB200_E_UNSUPPORTED;
     }
+  std::vector<int> hll_log2m(q->num_aggs, 0);   // DISTINCTCOUNTHLL: the device path's checks, before any segment is answered here
+  for (int a = 0; a < q->num_aggs; a++) {
+    if (!pb200::is_hll_fn(q->aggs[a].function)) continue;
+    if (any_clause) { set_error("DISTINCTCOUNTHLL in a query with FILTER (WHERE ...) clauses is not accelerated"); return PB200_E_UNSUPPORTED; }
+    const double lv = args ? args[a].p : 0.0;
+    if (!(lv >= 0.0 && lv <= 30.0) || lv != (double)(int)lv) { set_error("DISTINCTCOUNTHLL (aggregation %d): log2m %g is not an integer in 0..30", a, lv); return PB200_E_INVALID; }
+    hll_log2m[a] = lv == 0.0 ? pb200::kHllDefaultLog2m : (int)lv;
+    if (hll_log2m[a] < pb200::kHllMinLog2m || hll_log2m[a] > pb200::kHllMaxLog2m) {
+      set_error("DISTINCTCOUNTHLL (aggregation %d): log2m %d outside %d..%d is not accelerated", a, hll_log2m[a], pb200::kHllMinLog2m, pb200::kHllMaxLog2m);
+      return PB200_E_UNSUPPORTED;
+    }
+  }
   ExprFilterScope expr_filters;   // expression leaves become device doc sets once, also for the FILTER clauses' submissions
   if (int rc = resolve_expr_filters(ctx, *q, segs, nseg, expr_filters, true)) return rc;
   if (q->agg_filter_count && q->agg_filter_start && q->agg_filter_nodes)
@@ -891,7 +905,7 @@ extern "C" int32_t pb200h_execute_agg_args(pb200_ctx* ctx, const pb200h_query* q
       if (aggs[a].column < 0) { set_error("unknown aggregation column '%s'", q->aggs[a].column ? q->aggs[a].column : "(null)"); return PB200_E_INVALID; }
       const HostColumn& c = s0.cols[aggs[a].column];
       const bool wt = q->aggs[a].function == PB200_AGG_FIRSTWITHTIME || q->aggs[a].function == PB200_AGG_LASTWITHTIME;
-      if (c.data_type == PB200_STRING && q->aggs[a].function != PB200_AGG_DISTINCTCOUNT && !wt) { set_error("%s over STRING column", "aggregation"); return PB200_E_UNSUPPORTED; }
+      if (c.data_type == PB200_STRING && q->aggs[a].function != PB200_AGG_DISTINCTCOUNT && !pb200::is_hll_fn(q->aggs[a].function) && !wt) { set_error("%s over STRING column", "aggregation"); return PB200_E_UNSUPPORTED; }
       if (args) dev_args[a].p = args[a].p;
       if (wt) {
         dev_args[a].time_column = s0.column_index(args[a].time_column);
@@ -985,6 +999,20 @@ extern "C" int32_t pb200h_execute_agg_args(pb200_ctx* ctx, const pb200h_query* q
     }
     else if (kind[s] == PB200H_OP_NON_SCAN_AGGREGATION) results[s] = host_result(*segs[s], *q, false);
     else results[s] = dev_results[di++];
+  }
+  // DISTINCTCOUNTHLL answered without a scan: the device finalize over the whole dictionary
+  for (int s = 0; s < nseg; s++) {
+    if (kind[s] != PB200H_OP_NON_SCAN_AGGREGATION) continue;
+    for (int a = 0; a < q->num_aggs; a++) {
+      if (!pb200::is_hll_fn(q->aggs[a].function)) continue;
+      long long est = 0;
+      if (int rc = pb200::hll_whole_dictionary(ctx, segs[s]->dev, aggs[a].column, hll_log2m[a], &est)) {
+        for (int k = 0; k < nseg; k++) { pb200_result_free(results[k]); results[k] = nullptr; }
+        return rc;
+      }
+      results[s]->lng[a][0] = est;
+      results[s]->dbl[a][0] = (double)est;
+    }
   }
   return PB200_OK;
 }

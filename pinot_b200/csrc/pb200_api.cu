@@ -828,14 +828,18 @@ namespace {
 // Then (aggregation-only DISTINCTSUM / DISTINCTAVG) per result and aggregation the finalized state, kDsWords u64 each.
 // Then (aggregation-only expression aggregations, pb200_expr.cu) per result and aggregation one u64: the f64 sum, or the
 // Double.compare key of a MIN / MAX.
+// Then (aggregation-only DISTINCTCOUNTHLL) per result and aggregation the estimate, int64 (slot of ScanPlan::hll_rep).
 struct AccumLayout {
-  size_t verify_off = 0, pct_off = 0, wt_off = 0, ds_off = 0, ex_off = 0, bytes = 0;
+  size_t verify_off = 0, pct_off = 0, wt_off = 0, ds_off = 0, ex_off = 0, hll_off = 0, bytes = 0;
   int nres = 0;
   AccumLayout() = default;
-  AccumLayout(int nres, bool pct, bool wt, bool ds, bool ex)
+  AccumLayout(int nres, bool pct, bool wt, bool ds, bool ex, bool hll)
       : verify_off(sizeof(AggAccum) * nres), pct_off(verify_off + 32ull * nres), wt_off(pct_off + (pct ? 8ull * kMaxAggs * nres : 0)),
         ds_off(wt_off + (wt ? 20ull * kMaxAggs * nres : 0)), ex_off(ds_off + (ds ? 8ull * kDsWords * kMaxAggs * nres : 0)),
-        bytes(ex_off + (ex ? 8ull * kMaxAggs * nres : 0)), nres(nres) {}
+        hll_off(ex_off + (ex ? 8ull * kMaxAggs * nres : 0)), bytes(hll_off + (hll ? 8ull * kMaxAggs * nres : 0)), nres(nres) {}
+  long long* hll(void* b, int r) const {
+    return reinterpret_cast<long long*>(static_cast<unsigned char*>(b) + hll_off) + (size_t)r * kMaxAggs;
+  }
   unsigned long long* ex(void* b, int r) const {
     return reinterpret_cast<unsigned long long*>(static_cast<unsigned char*>(b) + ex_off) + (size_t)r * kMaxAggs;
   }
@@ -857,6 +861,7 @@ void release_tables(pb200_result& R, bool keep_hist) {
     dev_free(d.ctx, d.i64_block); dev_free(d.ctx, d.f64_block); dev_free(d.ctx, d.u32max_block); dev_free(d.ctx, d.u32min_block);
     dev_free(d.ctx, d.hkeys); dev_free(d.ctx, d.hctl);
     for (int a = 0; a < kMaxAggs; a++) { dev_free(d.ctx, d.dbits[a]); d.dbits[a] = nullptr; dev_free(d.ctx, d.ds_state[a]); d.ds_state[a] = nullptr; }
+    for (int a = 0; a < kMaxAggs; a++) { dev_free(d.ctx, d.hll_est[a]); d.hll_est[a] = nullptr; }
     for (int a = 0; a < kMaxAggs; a++) { dev_free(d.ctx, d.expr_tab[a]); d.expr_tab[a] = nullptr; }
     d.i64_block = d.f64_block = d.u32max_block = d.u32min_block = nullptr;
     d.hkeys = nullptr; d.hctl = nullptr;
@@ -868,6 +873,9 @@ void release_tables(pb200_result& R, bool keep_hist) {
       if (!keep_hist) { dev_free(p.ctx, p.hist[a]); p.hist[a] = nullptr; }
       dev_free(p.ctx, p.ids[a]); dev_free(p.ctx, p.n[a]); p.ids[a] = p.n[a] = nullptr;
     }
+  pb200_result::LazySets& L = R.lazy;
+  if (L.ctx && !keep_hist)   // the kept DISTINCTCOUNTHLL sets go with the result, like its histograms
+    for (int b = 0; b < kMaxAggs; b++) { dev_free(L.ctx, L.bits[b]); L.bits[b] = nullptr; }
   pb200_result::Wt& w = R.wt;
   if (d.ctx)
     for (int a = 0; a < kMaxAggs; a++) {
@@ -919,6 +927,7 @@ struct ScanCall {
   // 2. VAR / STDDEV limb dictionaries (pb200_moments.cu), then every decision about the launch (pb200_plan.cpp)
   int prepare_and_plan(bool allow_count_carrier, const double* agg_args, const pb200_agg_arg* wt_args) {
     if (int rc = moments_prepare(ctx, query, segments, nseg)) return rc;
+    if (int rc = hll_prepare(ctx, query, segments, nseg)) return rc;
     return plan_scan(tune, DeviceLimits{ctx->sm_count, ctx->max_smem_optin}, query, segments, nseg, allow_count_carrier, &plan, agg_args, wt_args);
   }
 
@@ -939,8 +948,11 @@ struct ScanCall {
     bool any_pct = false;
     for (int a = 0; a < plan.q.num_aggs; a++) any_pct |= plan.pct_rep[a] >= 0;
     bool any_ds = false;
-    for (int a = 0; a < plan.q.num_aggs; a++) any_ds |= plan.ds_rep[a] >= 0;
-    acc = AccumLayout(plan.nres, any_pct && !plan.group_by, plan.any_wt && !plan.group_by, any_ds && !plan.group_by, ex && !plan.group_by);
+    for (int a = 0; a < plan.q.num_aggs; a++) any_ds |= is_distinct_value_fn(plan.q.aggs[a].function);
+    bool any_hll = false;
+    for (int a = 0; a < plan.q.num_aggs; a++) any_hll |= plan.hll_rep[a] >= 0;
+    acc = AccumLayout(plan.nres, any_pct && !plan.group_by, plan.any_wt && !plan.group_by, any_ds && !plan.group_by, ex && !plan.group_by,
+                      any_hll && !plan.group_by);
     if (int rc = pinned_alloc(ctx, 2 * acc.bytes, &pin.p, &pin.bytes)) return rc;
     unsigned char* const init = static_cast<unsigned char*>(pin.p);
     back = init + acc.bytes;
@@ -1056,6 +1068,8 @@ struct ScanCall {
       if (plan.mom_first[a] >= 0) d.mom_e[a] = seg->cols[query->aggs[a].column].moments->grid.e;
       d.ds_rep[a] = plan.ds_rep[a];
       if (plan.ds_rep[a] >= 0) d.ds_e[plan.ds_rep[a]] = seg->cols[query->aggs[a].column].moments->ds_e;
+      d.hll_log2m[a] = plan.hll_log2m[a];
+      d.hll_rep[a] = plan.hll_rep[a];
     }
     d.pack_agg = t.carrier.agg; d.pack_shift = t.carrier.shift; d.pack_vmin = t.carrier.vmin;
     d.reduce_world = t.reduce_world;
@@ -1096,6 +1110,9 @@ struct ScanCall {
       if (is_distinct_value_fn(fn)) {   // the set's finalized state per group / slot (pb200_extract.cu runs the finalize)
         unsigned long long*& state = d.ds_state[plan.ds_rep[a]];
         if (!state && (rc = dev_alloc(ctx, (size_t)t.groups * kDsWords * 8, (void**)&state))) return rc;
+      } else if (is_hll_fn(fn)) {   // the estimate per group / slot, shared by the HLLs of the column and log2m
+        long long*& est = d.hll_est[plan.hll_rep[a]];
+        if (!est && (rc = dev_alloc(ctx, (size_t)t.groups * 8, (void**)&est))) return rc;
       } else if (fn == PB200_AGG_PERCENTILE) {  // one dictId histogram per group / slot (owner), a dictId per entry (each)
         if (t.hist_per_group[a]) {
           const size_t entries = (size_t)t.hist_per_group[a] * t.groups;
@@ -1172,14 +1189,31 @@ struct ScanCall {
     if (plan.group_by) return PB200_OK;
     for (int r = 0; r < plan.nres; r++)
       for (int a = 0; a < plan.q.num_aggs; a++) {
+        if (!is_distinct_value_fn(plan.q.aggs[a].function)) continue;   // a set DISTINCTSUM / DISTINCTAVG read
         const int b = plan.ds_rep[a];
         bool done = false;
-        for (int x = 0; x < a && !done; x++) done = plan.ds_rep[x] == b;
-        if (b < 0 || done) continue;
+        for (int x = 0; x < a && !done; x++) done = is_distinct_value_fn(plan.q.aggs[x].function) && plan.ds_rep[x] == b;
+        if (done) continue;
         const DeviceColumn& c = segments[plan.merge ? 0 : r]->cols[query->aggs[a].column];
         const DistinctSumJob job{static_cast<const uint32_t*>(distinct_bufs[r][b]->p), plan.distinct_words[r][b], 1, true,
                                  c.dict_native, c.stored_type, c.moments->ds_e, acc.ds(accum.p, r, b)};
         if (int rc = distinct_sum_finalize(ctx, st, job, temps)) return rc;
+      }
+    return PB200_OK;
+  }
+
+  // 8e. DISTINCTCOUNTHLL, aggregation only: each result's set -> the estimate in the accumulator block (slot of the
+  //     first HLL of the column and log2m), queued behind the scan (group-by: the extraction finalizes)
+  int finalize_hll() {
+    if (plan.group_by) return PB200_OK;
+    for (int r = 0; r < plan.nres; r++)
+      for (int a = 0; a < plan.q.num_aggs; a++) {
+        if (plan.hll_rep[a] != a) continue;
+        const int b = plan.ds_rep[a];
+        const DeviceColumn& c = segments[plan.merge ? 0 : r]->cols[query->aggs[a].column];
+        const HllJob job{static_cast<const uint32_t*>(distinct_bufs[r][b]->p), plan.distinct_words[r][b], 1, true,
+                         c.moments->hll_hash, plan.hll_log2m[a], acc.hll(accum.p, r) + a};
+        if (int rc = hll_finalize(ctx, st, job, temps)) return rc;
       }
     return PB200_OK;
   }
@@ -1243,6 +1277,14 @@ struct ScanCall {
     return PB200_OK;
   }
 
+  // whether only DISTINCTCOUNTHLLs read the set held by aggregation b's bitset
+  bool hll_only_set(int r, int b) const {
+    if (!distinct_bufs[r][b]) return false;
+    std::vector<int> fns(plan.q.num_aggs);
+    for (int x = 0; x < plan.q.num_aggs; x++) fns[x] = plan.q.aggs[x].function;
+    return hll_only_set_of(fns.data(), plan.ds_rep.data(), plan.q.num_aggs, b);
+  }
+
   // 10. aggregation only: aggregation a of result r's one row, {double, long, dictId}
   struct AggValue { double d = 0; int64_t l = 0; int32_t id = -1; };
   int agg_value(int r, int a, AggValue* v) {
@@ -1291,7 +1333,20 @@ struct ScanCall {
       const uint32_t x = acc.wt_ids(back, r)[a];
       if (acc_r.count == 0 || x == ~0u) v->d = -INFINITY;
       else { v->id = (int32_t)x; v->d = c->dict_host.empty() ? (double)v->id : value_of(x); v->l = acc.wt_time(back, r)[a]; }
-    } else if (fn == PB200_AGG_DISTINCTCOUNT || is_distinct_value_fn(fn)) {
+    } else if (is_hll_fn(fn) && hll_only_set(r, plan.ds_rep[a])) {
+      // only DISTINCTCOUNTHLLs read this set: the bitset stays on the device until pb200_result_distinct asks for it
+      const int b = plan.ds_rep[a];
+      pb200_result::LazySets& L = R.lazy;
+      if (!L.bits[b]) {
+        L.ctx = ctx;
+        L.bits[b] = static_cast<uint32_t*>(distinct_bufs[r][b]->p);
+        distinct_bufs[r][b]->p = nullptr;
+        L.words[b] = plan.distinct_words[r][b];
+        L.rows[b] = 1;
+      }
+      L.src[a] = b;
+      v->l = acc.hll(back, r)[plan.hll_rep[a]]; v->d = (double)v->l;
+    } else if (fn == PB200_AGG_DISTINCTCOUNT || reads_distinct_set(fn)) {
       const int b = fn == PB200_AGG_DISTINCTCOUNT ? a : plan.ds_rep[a];   // the aggregation whose bitset holds the set
       std::vector<uint32_t> bits(plan.distinct_words[r][b]);
       PB200_CUDA(cudaMemcpy(bits.data(), distinct_bufs[r][b]->p, bits.size() * 4, cudaMemcpyDeviceToHost));
@@ -1300,6 +1355,8 @@ struct ScanCall {
       if (is_distinct_value_fn(fn)) {
         const unsigned long long* ds = acc.ds(back, r, b);
         memcpy(&v->d, ds + ds_final_word(fn), 8);   // rounded once by the finalize
+      } else if (is_hll_fn(fn)) {
+        v->l = acc.hll(back, r)[plan.hll_rep[a]]; v->d = (double)v->l;
       }
     }
     return PB200_OK;
@@ -1394,6 +1451,7 @@ static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment*
   if (int rc = c.finalize_percentiles()) return rc;
   if (int rc = c.finalize_withtime()) return rc;
   if (int rc = c.finalize_distinct_sums()) return rc;
+  if (int rc = c.finalize_hll()) return rc;
   if (int rc = c.finalize_exprs()) return rc;
   if (int rc = c.read_back_and_verify()) return rc;   // kRetryWithoutCountCarrier: ~ScanCall frees this attempt's tables
   if (int rc = c.fill_results_and_extract(order, having)) return rc;
@@ -1536,8 +1594,10 @@ extern "C" int32_t pb200_result_columns(const pb200_result* R, const int32_t** k
   return PB200_OK;
 }
 extern "C" int64_t pb200_result_distinct(const pb200_result* R, int32_t a, int32_t row, int32_t* out, int64_t cap) {
-  if (!R || a < 0 || a >= (int)R->distinct.size() || row < 0 || row >= (int)R->distinct[a].size()) { set_error("bad distinct index"); return PB200_E_INVALID; }
-  const auto& v = R->distinct[a][row];
+  // a DISTINCTCOUNTHLL's kept set is decoded here, once: the result is logically unchanged
+  const std::vector<std::vector<int32_t>>* sets = R ? result_sets(const_cast<pb200_result*>(R), a) : nullptr;
+  if (!sets || row < 0 || row >= (int)sets->size()) { set_error("bad distinct index"); return PB200_E_INVALID; }
+  const auto& v = (*sets)[row];
   for (int64_t i = 0; i < (int64_t)v.size() && i < cap; i++) out[i] = v[i];
   return (int64_t)v.size();
 }

@@ -133,7 +133,7 @@ static int combine_scalars(NcclApi* api, pb200_ctx* ctx, pb200_result* R, int ro
   const int nagg = R->meta.num_aggs;
   if (nagg > kMaxAggs || (int)R->dbl.size() < nagg || (int)R->lng.size() < nagg) { set_error("result is not an aggregation-only result"); return PB200_E_INVALID; }
   for (int a = 0; a < nagg; a++)
-    if ((int)R->distinct.size() > a && !R->distinct[a].empty()) { set_error("DISTINCTCOUNT sets are merged on the host"); return PB200_E_UNSUPPORTED; }
+    if (((int)R->distinct.size() > a && !R->distinct[a].empty()) || R->lazy.src[a] >= 0) { set_error("DISTINCTCOUNT sets are merged on the host"); return PB200_E_UNSUPPORTED; }
   for (int a = 0; a < nagg; a++)
     if (R->pct.rep[a] >= 0) { set_error("PERCENTILE histograms are merged on the host"); return PB200_E_UNSUPPORTED; }
   for (int a = 0; a < nagg; a++)

@@ -76,6 +76,7 @@ struct ExtractDesc {
   int32_t mom_e[kMaxAggs];           // ... and the grid exponent of the column
   unsigned long long off_mom[kMaxAggs];  // ... {s1, s2 low, s2 high} per row, for pb200_result_moments
   const unsigned long long* ds[kMaxAggs];  // DISTINCTSUM / DISTINCTAVG: the finalized state per table entry (kDsWords u64)
+  const long long* hll[kMaxAggs];    // DISTINCTCOUNTHLL: the estimate per table entry
   const unsigned long long* xkey[kMaxAggs];  // expression MIN / MAX (pb200_expr.cu): Double.compare key per table entry
   const uint8_t* keep;               // HAVING only: bit j of byte i = entry 8i + j is a row (NULL: every non_empty() entry is)
 };
@@ -198,6 +199,9 @@ __device__ __forceinline__ void agg_values(const ExtractDesc& d, int a, long lon
     const unsigned long long* st = d.ds[a] + (size_t)g * kDsWords;   // registers of the kernels every group-by query runs
     dv = __longlong_as_double((long long)st[ds_final_word(fn)]);
     lv = (long long)st[2];
+  } else if (is_hll_fn(fn)) {   // the finalize's estimate (pb200_hll.cu), in both columns
+    lv = d.hll[a][g];
+    dv = (double)lv;
   }
 }
 
@@ -383,7 +387,7 @@ static size_t layout_result(const pb200_result::Dense& d, ExtractDesc& e, size_t
     e.off_dbl[a] = take(8, rows);
     const bool wt = fn == PB200_AGG_FIRSTWITHTIME || fn == PB200_AGG_LASTWITHTIME;
     e.off_lng[a] = (fn == PB200_AGG_COUNT || fn == PB200_AGG_AVG || fn == PB200_AGG_SUM || fn == PB200_AGG_DISTINCTCOUNT ||
-                    fn == PB200_AGG_PERCENTILE || is_moments_fn(fn) || is_distinct_value_fn(fn) || wt) ? take(8, rows) : kNoCol;
+                    fn == PB200_AGG_PERCENTILE || is_moments_fn(fn) || reads_distinct_set(fn) || wt) ? take(8, rows) : kNoCol;
     e.off_ids[a] = (fn == PB200_AGG_MIN || fn == PB200_AGG_MAX || fn == PB200_AGG_PERCENTILE || wt) ? take(4, rows) : kNoCol;
     e.off_mom[a] = is_moments_fn(fn) ? take(24, rows) : kNoCol;
   }
@@ -465,6 +469,7 @@ int extract_groups(pb200_ctx* ctx, pb200_result* const* Rs, int nres, cudaStream
         for (int j = 0; j < 3; j++) e.mom[a][j] = d.isum[d.mom_first[a] + j];
         e.mom_e[a] = d.mom_e[a];
       } else if (is_distinct_value_fn(fn)) e.ds[a] = d.ds_state[d.ds_rep[a]];
+      else if (is_hll_fn(fn)) e.hll[a] = d.hll_est[d.hll_rep[a]];
       const DeviceColumn* c = d.agg_cols[a];
       e.dict[a] = (c && vk != VAL_RAW_I32 && !c->dict_host.empty()) ? c->dict_native : nullptr;
     }
@@ -545,6 +550,12 @@ int extract_groups(pb200_ctx* ctx, pb200_result* const* Rs, int nres, cudaStream
       const DistinctSumJob job{d.dbits[b], d.dwords[b], d.groups, false, c.dict_native, c.stored_type, d.ds_e[b], d.ds_state[b]};
       if ((rc = distinct_sum_finalize(ctx, st, job, ds_temps))) return rc;
     }
+    for (int a = 0; a < descs[r].nagg; a++) {   // DISTINCTCOUNTHLL: one estimate per column and log2m
+      if (d.hll_rep[a] != a || !d.hll_est[a]) continue;
+      const int b = d.ds_rep[a];
+      const HllJob job{d.dbits[b], d.dwords[b], d.groups, false, d.agg_cols[b]->moments->hll_hash, d.hll_log2m[a], d.hll_est[a]};
+      if ((rc = hll_finalize(ctx, st, job, ds_temps))) return rc;
+    }
   }
   const ExtractDesc* ddescs = (const ExtractDesc*)ddesc.p;
   PB200_CUDA(cudaMemcpyAsync(ddesc.p, descs.data(), sizeof(ExtractDesc) * nres, cudaMemcpyHostToDevice, st));
@@ -617,6 +628,7 @@ int extract_groups(pb200_ctx* ctx, pb200_result* const* Rs, int nres, cudaStream
     PB200_CUDA(cudaStreamSynchronize(st));
   }
   // ---- results point into the block ----
+  bool kept_sets = false;   // some set's rows were gathered into a result for later: wait for them before returning
   for (int r = 0; r < nres; r++) {
     pb200_result* R = Rs[r];
     const pb200_result::Dense& d = R->dense;
@@ -638,25 +650,39 @@ int extract_groups(pb200_ctx* ctx, pb200_result* const* Rs, int nres, cudaStream
     }
     // DISTINCTCOUNT with GROUP BY: the groups' bitset rows are gathered on the device and decoded here into dictId lists
     // (what extractGroupByResult's value-set conversion starts from, BaseDistinctAggregateAggregationFunction :306-321)
-    // (DISTINCTSUM / DISTINCTAVG: the same from the bitset that holds their set, decoded once per bitset; their columns
-    // already hold value and size)
+    // (DISTINCTSUM / DISTINCTAVG / DISTINCTCOUNTHLL: the same from the bitset that holds their set, decoded once per
+    // bitset; their columns already hold value and size.  A set only DISTINCTCOUNTHLLs read keeps its gathered rows on
+    // the device instead, for pb200_result_distinct to decode on first use.)
     std::vector<int> decoded(nagg, -1);   // the bitset aggregation a's set was decoded from
+    std::vector<int32_t> fns(nagg);
+    for (int a = 0; a < nagg; a++) fns[a] = d.aggs[a].function;
     for (int a = 0; a < nagg; a++) {
-      const bool value_fn = is_distinct_value_fn(d.aggs[a].function);
+      const bool value_fn = reads_distinct_set(d.aggs[a].function);
       const int b = value_fn ? d.ds_rep[a] : a;
       if ((d.aggs[a].function != PB200_AGG_DISTINCTCOUNT && !value_fn) || b < 0 || !d.dbits[b]) continue;
       decoded[a] = b;
+      const bool lazy = hll_only_set_of(fns.data(), d.ds_rep, nagg, b);
+      if (lazy) R->lazy.src[a] = b;
       const int same = (int)(std::find(decoded.begin(), decoded.begin() + a, b) - decoded.begin());
-      if (same < a) { R->distinct[a] = R->distinct[same]; continue; }
+      if (same < a) { if (!lazy) R->distinct[a] = R->distinct[same]; continue; }
       const size_t wpg = d.dwords[b], rows = v.rows;
-      std::vector<uint32_t> bits(rows * wpg);
+      std::vector<uint32_t> bits(lazy ? 0 : rows * wpg);
       if (rows) {
         DevBufRaw g(ctx);
         if ((rc = g.alloc(rows * wpg * 4))) return rc;
         gather_bitset_rows_kernel<<<grid_for(ctx, (long long)(rows * wpg), 256), 256, 0, st>>>(d.dbits[b], reinterpret_cast<const uint32_t*>(out + e.off_idx), (long long)rows, (int)wpg, (uint32_t*)g.p);
+        if (lazy) {   // owned by the result from here on; the stream orders the gather before any later copy of it
+          pb200_result::LazySets& L = R->lazy;
+          dev_free(ctx, L.bits[b]);   // a result extracted again (pb200_result_finalize) replaces its rows
+          L.ctx = ctx; L.bits[b] = static_cast<uint32_t*>(g.p); L.words[b] = wpg; L.rows[b] = rows;
+          g.p = nullptr;
+          kept_sets = true;
+          continue;
+        }
         PB200_CUDA(cudaMemcpyAsync(bits.data(), g.p, rows * wpg * 4, cudaMemcpyDeviceToHost, st));
         PB200_CUDA(cudaStreamSynchronize(st));
       }
+      if (lazy) { R->lazy.ctx = ctx; R->lazy.words[b] = wpg; R->lazy.rows[b] = 0; continue; }
       R->distinct[a].resize(rows);
       int64_t* sizes = const_cast<int64_t*>(v.lng[a]);   // the kernel left zeros: the set sizes go here
       double* dsz = const_cast<double*>(v.dbl[a]);
@@ -666,6 +692,7 @@ int extract_groups(pb200_ctx* ctx, pb200_result* const* Rs, int nres, cudaStream
       }
     }
   }
+  if (kept_sets) PB200_CUDA(cudaStreamSynchronize(st));   // the bitset tables may be freed once this returns
   return PB200_OK;
 }
 

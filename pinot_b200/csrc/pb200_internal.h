@@ -14,6 +14,7 @@
 #include "../../include/pinot_b200.h"
 #include "pb200_desc.h"
 #include "pb200_distinct_sum.h"
+#include "pb200_hll.h"
 #include "pb200_moments.h"
 
 namespace pb200 {
@@ -53,6 +54,11 @@ struct MomentDict {
   // host copy by the first query that needs it, under `mu`; 0 not yet, 1 eligible with exponent ds_e, -1 not eligible
   std::atomic<int> ds_state{0};
   int ds_e = 0;
+  // DISTINCTCOUNTHLL (pb200_hll.h): the 32-bit MurmurHash of every entry of the same dictionary (device, 4 bytes per
+  // entry), built by the first query that needs it (pb200_hll.cu hll_prepare), under `mu`; 0 not yet, 1 built, -1 a
+  // STRING entry that is not valid UTF-8 (the reference would hash U+FFFD's bytes: not accelerated)
+  std::atomic<int> hll_state{0};
+  uint32_t* hll_hash = nullptr;
   ~MomentDict();                   // pb200_moments.cu
 };
 
@@ -249,6 +255,18 @@ struct pb200_result {
     bool on[pb200::kMaxAggs] = {};
     long long sum[pb200::kMaxAggs] = {};
   } exact;
+  // DISTINCTCOUNTHLL sets that nothing else in the query reads: the result rows' bitset rows stay on the device
+  // (rows x words u32, owned per bitset b) and pb200_result_distinct decodes them into `distinct` on its first call for an
+  // aggregation a with src[a] = b -- a caller that reads only the estimates never pays for the decode
+  struct LazySets {
+    LazySets() { std::fill(src, src + pb200::kMaxAggs, -1); }
+    pb200_ctx* ctx = nullptr;
+    std::mutex mu;
+    int src[pb200::kMaxAggs];
+    uint32_t* bits[pb200::kMaxAggs] = {};
+    size_t words[pb200::kMaxAggs] = {};
+    size_t rows[pb200::kMaxAggs] = {};
+  } lazy;
   pb200_order_by order{};                      // ORDER BY spec of a group-by result (num_items 0: none), applied at extraction
   pb200_having having{};                       // HAVING of a group-by result (num_nodes 0: none), applied at extraction before
                                                // the order; set on every result whose rows it filtered
@@ -284,7 +302,11 @@ struct pb200_result {
     std::vector<unsigned long long> mult64;
     int mom_first[pb200::kMaxAggs];             // VAR / STDDEV: the first of the three limb sums (isum) of aggregation a, -1 if none
     int mom_e[pb200::kMaxAggs] = {};            // ... and the grid exponent of its column
-    Dense() { std::fill(mom_first, mom_first + pb200::kMaxAggs, -1); std::fill(ds_rep, ds_rep + pb200::kMaxAggs, -1); }
+    Dense() {
+      std::fill(mom_first, mom_first + pb200::kMaxAggs, -1);
+      std::fill(ds_rep, ds_rep + pb200::kMaxAggs, -1);
+      std::fill(hll_rep, hll_rep + pb200::kMaxAggs, -1);
+    }
     uint32_t* dbits[pb200::kMaxAggs] = {};      // DISTINCTCOUNT with GROUP BY: per-group dictId bitsets, dwords[a] words each
     uint32_t dwords[pb200::kMaxAggs] = {};
     // DISTINCTSUM / DISTINCTAVG (pb200_distinct_sum.h): the aggregation b whose bitset holds the set (-1: neither
@@ -293,6 +315,11 @@ struct pb200_result {
     int ds_rep[pb200::kMaxAggs];
     int ds_e[pb200::kMaxAggs] = {};
     unsigned long long* ds_state[pb200::kMaxAggs] = {};
+    // DISTINCTCOUNTHLL (pb200_hll.h): log2m of aggregation a (0: not one); indexed by the first HLL of a column and log2m
+    // (ScanPlan::hll_rep), the estimate per table entry (int64, device), shared by the HLLs with that column and log2m
+    int hll_log2m[pb200::kMaxAggs] = {};
+    int hll_rep[pb200::kMaxAggs];
+    long long* hll_est[pb200::kMaxAggs] = {};
     // expression aggregations (pb200_expr.cu): per aggregation its own table, f64 sums (also pointed to by dsum) or u64
     // Double.compare keys of MIN / MAX; NULL: not an expression
     void* expr_tab[pb200::kMaxAggs] = {};
@@ -411,6 +438,26 @@ struct DistinctSumJob {
   unsigned long long* out;
 };
 int distinct_sum_finalize(pb200_ctx* ctx, cudaStream_t st, const DistinctSumJob& job, std::vector<std::unique_ptr<DevBufRaw>>& temps);
+// pb200_hll.cu: builds (once per device dictionary) the hash array of every DISTINCTCOUNTHLL column of the query that has
+// dictIds, before it is planned; PB200_E_UNSUPPORTED for a STRING dictionary with an entry that is not valid UTF-8
+int hll_prepare(pb200_ctx* ctx, const pb200_query* query, pb200_segment* const* segments, int nseg);
+// DISTINCTCOUNTHLL estimates (int64 per row) of `rows` bitset rows of `words` words each, queued on `st`.  single: one row
+// of an aggregation-only result (a grid-wide pass; its scratch goes to `temps`).
+struct HllJob {
+  const uint32_t* bits;
+  size_t words;
+  long long rows;
+  bool single;
+  const uint32_t* hash;       // the column's hash array (MomentDict::hll_hash)
+  int log2m;
+  long long* out;
+};
+int hll_finalize(pb200_ctx* ctx, cudaStream_t st, const HllJob& job, std::vector<std::unique_ptr<DevBufRaw>>& temps);
+// pb200_hll.cu: the DISTINCTCOUNTHLL estimate over every value of column `column` in the segment (the host layer's answer
+// without a scan for a filter that matches every doc), computed by the finalize; synchronous
+int hll_whole_dictionary(pb200_ctx* ctx, pb200_segment* seg, int column, int log2m, long long* out);
+// pb200_hll.cu: the dictId set of pb200_result_distinct for aggregation a of R, decoding a lazily kept set first
+const std::vector<std::vector<int32_t>>* result_sets(pb200_result* R, int a);
 // pb200_synth.cu
 int synth_build_inverted(pb200_ctx* ctx, cudaStream_t stream, DeviceColumn& col, long long num_docs);
 }  // namespace pb200

@@ -14,6 +14,7 @@ namespace pb200 {
 
 MomentDict::~MomentDict() {
   if (limbs && ctx) dev_free(ctx, limbs);
+  if (hll_hash && ctx) dev_free(ctx, hll_hash);
 }
 
 // k of every dictionary entry from the device copy of the dictionary (INT: biased, value ^ 0x80000000), then its square's

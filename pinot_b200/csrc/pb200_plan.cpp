@@ -163,6 +163,8 @@ struct ScanPlanner {
     plan.pct_p.assign(nagg, std::numeric_limits<double>::quiet_NaN());
     plan.pct_rep.assign(nagg, -1);
     plan.ds_rep.assign(nagg, -1);
+    plan.hll_log2m.assign(nagg, 0);
+    plan.hll_rep.assign(nagg, -1);
     plan.wt_time.assign(nagg, -1);
     return PB200_OK;
   }
@@ -218,13 +220,42 @@ struct ScanPlanner {
         return PB200_E_UNSUPPORTED;
       }
     }
+    share_distinct_set(a);
+    return PB200_OK;
+  }
+  // a function that reads a DISTINCTCOUNT set (reads_distinct_set): the bitset of an earlier DISTINCTCOUNT or reader of
+  // the same column, else its own
+  void share_distinct_set(int a) {
+    const pb200_agg& ag = plan.aggs[a];
     plan.ds_rep[a] = a;
-    for (int b = 0; b < a; b++) {   // share the bitset of an earlier DISTINCTCOUNT / DISTINCTSUM / DISTINCTAVG of the column
+    for (int b = 0; b < a; b++) {
       const int fb = plan.aggs[b].function;
-      if (plan.aggs[b].column != ag.column || (fb != PB200_AGG_DISTINCTCOUNT && !is_distinct_value_fn(fb))) continue;
+      if (plan.aggs[b].column != ag.column || (fb != PB200_AGG_DISTINCTCOUNT && !reads_distinct_set(fb))) continue;
       plan.ds_rep[a] = fb == PB200_AGG_DISTINCTCOUNT ? b : plan.ds_rep[b];
       break;
     }
+  }
+  // DISTINCTCOUNTHLL: log2m from the aggregation's argument (none or 0: the default 8; the reference accepts 0..30, the
+  // registers fit the finalize's shared memory up to 12), a column with dictIds in every segment (STRING too: its UTF-8
+  // bytes are hashed), and the bitset it reads.  HLLs of one column and log2m share one estimate (hll_rep).
+  int check_hll(int a, const double* agg_args) {
+    const pb200_agg& ag = plan.aggs[a];
+    const double lv = agg_args ? agg_args[a] : 0.0;
+    if (!(lv >= 0.0 && lv <= 30.0) || lv != (double)(int)lv) { set_error("DISTINCTCOUNTHLL (aggregation %d): log2m %g is not an integer in 0..30", a, lv); return PB200_E_INVALID; }
+    const int p = lv == 0.0 ? kHllDefaultLog2m : (int)lv;
+    if (p < kHllMinLog2m || p > kHllMaxLog2m) { set_error("DISTINCTCOUNTHLL (aggregation %d): log2m %d outside %d..%d is not accelerated", a, p, kHllMinLog2m, kHllMaxLog2m); return PB200_E_UNSUPPORTED; }
+    for (int t = 0; t < nseg; t++) {
+      const DeviceColumn& c = segments[t]->cols[ag.column];
+      if (c.bits > 31 || c.cardinality <= 0 || (c.stored_type != PB200_STRING && !c.dict_native)) {
+        set_error("DISTINCTCOUNTHLL over column %d: no dictIds in segment %d (raw values): not accelerated", ag.column, t);
+        return PB200_E_UNSUPPORTED;
+      }
+    }
+    plan.hll_log2m[a] = p;
+    plan.hll_rep[a] = a;
+    for (int b = 0; b < a; b++)
+      if (is_hll_fn(plan.aggs[b].function) && plan.aggs[b].column == ag.column && plan.hll_log2m[b] == p) { plan.hll_rep[a] = b; break; }
+    share_distinct_set(a);
     return PB200_OK;
   }
   // ---- slots: filter scan columns, then group-by keys, then aggregation arguments ----
@@ -258,10 +289,10 @@ struct ScanPlanner {
       const pb200_agg& ag = plan.aggs[a];
       q.aggs[a] = AggDesc{ag.function, -1, VAL_NONE, 0};
       if (ag.function == PB200_AGG_COUNT || is_moments_fn(ag.function)) continue;   // VAR / STDDEV: read their limb sums
-      if (ag.function < 0 || (ag.function > PB200_AGG_PERCENTILE && !is_withtime_fn(ag.function) && !is_distinct_value_fn(ag.function))) { set_error("unknown aggregation function %d", ag.function); return PB200_E_INVALID; }
+      if (ag.function < 0 || (ag.function > PB200_AGG_PERCENTILE && !is_withtime_fn(ag.function) && !reads_distinct_set(ag.function))) { set_error("unknown aggregation function %d", ag.function); return PB200_E_INVALID; }
       if (ag.column < 0 || ag.column >= ncols) { set_error("aggregation column %d out of range", ag.column); return PB200_E_INVALID; }
-      if (is_distinct_value_fn(ag.function)) {
-        if (int rc = check_distinct_value(a)) return rc;
+      if (reads_distinct_set(ag.function)) {
+        if (int rc = is_hll_fn(ag.function) ? check_hll(a, agg_args) : check_distinct_value(a)) return rc;
         if (plan.ds_rep[a] != a) continue;   // reads another aggregation's bitset: no slot, no agg code
       }
       if (is_withtime_fn(ag.function)) {
@@ -668,7 +699,7 @@ struct ScanPlanner {
           const SlotDesc& sl = sd.slots[q.aggs[a].slot];
           if (plan.wt_time[a] >= 0)   // the value-kind field says which end of the key order wins
             sd.agg_code[n++] = agg_code(a, kFnWithTime, q.aggs[a].function == PB200_AGG_LASTWITHTIME ? WT_MAX : WT_MIN, sl.bits, sl.stage_words);
-          else if (plan.ds_rep[a] == a)   // DISTINCTSUM / DISTINCTAVG owning its set: the scan builds a DISTINCTCOUNT bitset
+          else if (plan.ds_rep[a] == a)   // a reader owning its set (DISTINCTSUM ...): the scan builds a DISTINCTCOUNT bitset
             sd.agg_code[n++] = agg_code(a, PB200_AGG_DISTINCTCOUNT, q.aggs[a].val_kind, sl.bits, sl.stage_words);
           else
             sd.agg_code[n++] = agg_code(a, q.aggs[a].function, q.aggs[a].val_kind, sl.bits, sl.stage_words);
@@ -835,7 +866,8 @@ struct ScanPlanner {
         const unsigned long long words = ((unsigned long long)c.cardinality + 31) / 32;
         if (words * (unsigned long long)t.groups > (1ull << 28)) {
           set_error("%s with GROUP BY: %lld groups x %d dictIds exceed the device bitset budget",
-                    fn == PB200_AGG_DISTINCTCOUNT ? "DISTINCTCOUNT" : fn == PB200_AGG_DISTINCTSUM ? "DISTINCTSUM" : "DISTINCTAVG", t.groups, c.cardinality);
+                    fn == PB200_AGG_DISTINCTCOUNT ? "DISTINCTCOUNT" : fn == PB200_AGG_DISTINCTSUM ? "DISTINCTSUM"
+                    : fn == PB200_AGG_DISTINCTAVG ? "DISTINCTAVG" : "DISTINCTCOUNTHLL", t.groups, c.cardinality);
           return PB200_E_UNSUPPORTED;
         }
         t.dwords[a] = (uint32_t)words;
@@ -921,11 +953,12 @@ int plan_scan(const Tuning& tune, DeviceLimits lim, const pb200_query* query, pb
     for (int a = 0; a < nuser; a++) {
       const pb200_agg& ag = query->aggs[a];
       if (ag.function != PB200_AGG_MIN && ag.function != PB200_AGG_MAX && ag.function != PB200_AGG_DISTINCTCOUNT &&
-          ag.function != PB200_AGG_PERCENTILE && !is_moments_fn(ag.function) && !is_distinct_value_fn(ag.function)) continue;
+          ag.function != PB200_AGG_PERCENTILE && !is_moments_fn(ag.function) && !reads_distinct_set(ag.function)) continue;
       if (ag.column < 0 || ag.column >= ncols) continue;
       if (segments[0]->cols[ag.column].bits == 32 && !segments[0]->cols[ag.column].dict_native) continue;  // raw values, no ids
       const char* what = ag.function == PB200_AGG_DISTINCTCOUNT ? "DISTINCTCOUNT" : ag.function == PB200_AGG_PERCENTILE ? "PERCENTILE"
-                         : is_moments_fn(ag.function) ? "VAR/STDDEV" : is_distinct_value_fn(ag.function) ? "DISTINCTSUM/DISTINCTAVG" : "MIN/MAX";
+                         : is_moments_fn(ag.function) ? "VAR/STDDEV" : is_distinct_value_fn(ag.function) ? "DISTINCTSUM/DISTINCTAVG"
+                         : is_hll_fn(ag.function) ? "DISTINCTCOUNTHLL" : "MIN/MAX";
       if (!same_dictionary(segments, nseg, ag.column, what)) return PB200_E_UNSUPPORTED;
     }
     for (int a = 0; a < nuser && wt_args; a++) {   // FIRST/LASTWITHTIME: one dictionary for the data and the time column

@@ -84,6 +84,10 @@ struct ScanPlan {
   // (the DISTINCTCOUNT code: the scan cannot tell them apart); -1: neither function.  The grid exponent of each result's
   // dictionary is cached with it (MomentDict::ds_e)
   std::vector<int> ds_rep;
+  // DISTINCTCOUNTHLL (pb200_hll.h): the log2m of aggregation a (0: not one), and the aggregation whose estimate it shares --
+  // the first DISTINCTCOUNTHLL of its column and log2m (-1: not one).  Its set is found through ds_rep like DISTINCTSUM's.
+  std::vector<int> hll_log2m;
+  std::vector<int> hll_rep;
   // VAR / STDDEV (pb200_moments.h): the caller's aggregations come first, then three internal INT-dictionary SUMs per
   // column (K, H, L limbs) -- q.num_aggs and every per-aggregation array count them all
   int num_user_aggs = 0;
@@ -102,7 +106,8 @@ struct ScanPlan {
 };
 
 // PB200_OK, or the PB200_E_* code of pb200_execute_args for this input (message set with set_error).  agg_args: one per
-// aggregation, the percentile of a PERCENTILE (NULL: PERCENTILE is refused, as pb200_execute does).
+// aggregation, the percentile of a PERCENTILE or the log2m of a DISTINCTCOUNTHLL (NULL: PERCENTILE is refused, as
+// pb200_execute does, and DISTINCTCOUNTHLL takes the default log2m).
 constexpr long long kMaxHistogramEntries = 1ll << 28;  // PERCENTILE histogram entries of one call (u32 each)
 // Aggregation-only PERCENTILE over at most this many dictIds: each warp counts into a private histogram in its own
 // accumulator slots in shared memory (32 threads x 8 bytes = 64 u32 bins), flushed once per segment, instead of one
@@ -113,8 +118,8 @@ constexpr int kHistWarpPrivateMaxCard = 64;
 int plan_scan(const Tuning& tune, DeviceLimits lim, const pb200_query* query, pb200_segment* const* segments, int nseg,
               bool allow_count_carrier, ScanPlan* out, const double* agg_args = nullptr, const pb200_agg_arg* wt_args = nullptr);
 inline bool is_withtime_fn(int fn) { return fn == PB200_AGG_FIRSTWITHTIME || fn == PB200_AGG_LASTWITHTIME; }
-// aggregation a of the plan sets bits in a DISTINCTCOUNT bitset of its own: a DISTINCTCOUNT, or the owner of a
-// DISTINCTSUM / DISTINCTAVG set
+// aggregation a of the plan sets bits in a DISTINCTCOUNT bitset of its own: a DISTINCTCOUNT, or the owner of a set that
+// DISTINCTSUM / DISTINCTAVG / DISTINCTCOUNTHLL read
 inline bool owns_bitset(const ScanPlan& p, int a) {
   return p.q.aggs[a].function == PB200_AGG_DISTINCTCOUNT || (p.ds_rep[a] == a);
 }

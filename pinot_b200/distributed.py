@@ -33,7 +33,10 @@ from __future__ import annotations
 import ctypes as C
 from typing import Dict, List, Optional, Sequence
 
-from .query import DISTINCT_SET_FUNCTIONS, distinct_final, is_multi_column_expression
+from .query import DISTINCT_SET_FUNCTIONS, HllSet, distinct_final, hll_final, is_multi_column_expression, value_key
+
+# functions whose per-rank intermediate is a set of domain ids, united on the host
+_SET_FUNCTIONS = DISTINCT_SET_FUNCTIONS + ("DISTINCTCOUNTHLL",)
 
 
 KINDS = {"i64": 0, "f64": 1, "u32max": 2, "u32min": 3}
@@ -241,7 +244,7 @@ def execute_and_combine(plan_maker_or_backend, segments: Sequence, query, dist, 
         raise UnsupportedQueryError(E_UNSUPPORTED, "expression aggregations with GROUP BY are not combined across GPUs")
     backend = plan_maker_or_backend if hasattr(plan_maker_or_backend, "finish") else DeviceBackend(plan_maker_or_backend)
     world = dist.get_world_size()
-    if any(a.function in DISTINCT_SET_FUNCTIONS for a in query.aggregations):
+    if any(a.function in _SET_FUNCTIONS for a in query.aggregations):
         return _combine_with_sets(backend, segments, query, dist, dst)
     if not query.is_group_by:
         return _combine_scalars(backend, segments, query, dist, dst)
@@ -275,13 +278,15 @@ def _combine_with_sets(backend, segments, query, dist, dst):
     import numpy as np
     from .plan_maker import ResultsBlock
     # every group of every rank: a rank-level trim before this merge by key could drop a group of the global top rows
-    block = backend.pm.execute_segments(segments, query, merge=True, ordered=False)[0]
+    # a DISTINCTCOUNTHLL's set is only read on request: the merged block's sets travel to the root
+    hll = {"sets": True} if any(a.function == "DISTINCTCOUNTHLL" for a in query.aggregations) else {}
+    block = backend.pm.execute_segments(segments, query, merge=True, ordered=False, **hll)[0]
     fns = [a.function for a in query.aggregations]
     rows = 1 if block.num_groups < 0 else block.num_groups
     mine = {}
     for g in range(rows):
         key = () if block.num_groups < 0 else tuple(int(x) for x in block.keys[g])
-        mine[key] = [frozenset(int(d) for d in block.distinct[(a, g)]) if f in DISTINCT_SET_FUNCTIONS
+        mine[key] = [frozenset(int(d) for d in block.distinct[(a, g)]) if f in _SET_FUNCTIONS
                      else (float(block.doubles[a][g]), int(block.longs[a][g]), int(block.dict_ids[a][g])) for a, f in enumerate(fns)]
     stats = (block.stats.num_docs_scanned, block.stats.num_entries_scanned_in_filter, block.stats.num_entries_scanned_post_filter,
              block.stats.num_total_docs)
@@ -297,7 +302,7 @@ def _combine_with_sets(backend, segments, query, dist, dst):
                 merged[key] = list(vals)
                 continue
             for a, f in enumerate(fns):
-                if f in DISTINCT_SET_FUNCTIONS:
+                if f in _SET_FUNCTIONS:
                     cur[a] = cur[a] | vals[a]
                 elif f in ("COUNT", "SUM", "AVG"):
                     cur[a] = (cur[a][0] + vals[a][0], cur[a][1] + vals[a][1], -1)
@@ -306,9 +311,14 @@ def _combine_with_sets(backend, segments, query, dist, dst):
                 else:
                     cur[a] = max(cur[a], vals[a], key=lambda t: t[0])
     keys_sorted = sorted(merged)   # raw-key order is not defined across tables: ascending ids, column 0 most significant
-    def set_final(a, id_set):   # DISTINCTCOUNT / DISTINCTSUM / DISTINCTAVG of a merged set of domain ids, exact
+    def set_final(a, id_set):   # DISTINCTCOUNT / DISTINCTSUM / DISTINCTAVG / DISTINCTCOUNTHLL of a merged set of domain ids, exact
         if fns[a] == "DISTINCTCOUNT":
             return float(len(id_set))
+        if fns[a] == "DISTINCTCOUNTHLL":
+            agg = query.aggregations[a]
+            members = HllSet((value_key(segments[0].dictionary_value(agg.column, d)) for d in id_set),   # -0.0 apart from 0.0
+                             segments[0].column_info(agg.column)["data_type"])
+            return hll_final(members, agg.arg, members.data_type)
         return float(distinct_final(fns[a], [segments[0].dictionary_value(query.aggregations[a].column, d) for d in id_set]))
     if query.is_group_by and query.order_by:
         keys_sorted = _order_and_trim(query, fns, keys_sorted, merged, set_final)
@@ -319,9 +329,13 @@ def _combine_with_sets(backend, segments, query, dist, dst):
         d, l, i = np.zeros(max(n, 1)), np.zeros(max(n, 1), dtype=np.int64), np.full(max(n, 1), -1, dtype=np.int32)
         for g, key in enumerate(keys_sorted):
             v = merged[key][a]
-            if f in DISTINCT_SET_FUNCTIONS:
+            if f in _SET_FUNCTIONS:
                 distinct[(a, g)] = np.asarray(sorted(v), dtype=np.int32)
-                d[g], l[g] = set_final(a, v), len(v)
+                if f == "DISTINCTCOUNTHLL":   # the estimate in both columns, as the library returns it
+                    est = set_final(a, v)
+                    d[g], l[g] = float(est), est
+                else:
+                    d[g], l[g] = set_final(a, v), len(v)
             else:
                 d[g], l[g], i[g] = v
         doubles.append(d[:n] if query.is_group_by else d); longs.append(l[:n] if query.is_group_by else l); ids.append(i[:n] if query.is_group_by else i)
@@ -345,7 +359,7 @@ def _order_and_trim(query, fns, keys, merged, set_final):
 
     def final(a, v):
         f = fns[a]
-        if f in DISTINCT_SET_FUNCTIONS:
+        if f in _SET_FUNCTIONS:
             return set_final(a, v)
         if f == "COUNT":
             return float(v[1])

@@ -631,13 +631,16 @@ def _read_views(ctx: B200Context, handle, q: QueryContext, meta):
 
 def _read_result(ctx: B200Context, handle, q: QueryContext, kind: int, keep_handle: bool, views: bool = False,
                  histograms: bool = False) -> ResultsBlock:
+    # histograms=True (per-segment blocks, the intermediates of a by-value merge): also PERCENTILE histograms, moments and
+    # DISTINCTCOUNTHLL sets; otherwise a DISTINCTCOUNTHLL's set is never read, so the library never decodes it
     L = ctx.lib
     meta = _lib.ResultMeta()
     _lib.check(L.pb200_result_meta_get(handle, C.byref(meta)))
     g = meta.num_groups
     rows = 1 if g < 0 else g
     k = len(q.group_by)
-    if views and not any(a.function in DISTINCT_SET_FUNCTIONS + ("PERCENTILE",) + MOMENT_FUNCTIONS for a in q.aggregations):
+    if views and not any(a.function in DISTINCT_SET_FUNCTIONS + ("PERCENTILE",) + MOMENT_FUNCTIONS or (a.function == "DISTINCTCOUNTHLL" and histograms)
+                         for a in q.aggregations):
         keys, doubles, longs, ids = _read_views(ctx, handle, q, meta)
         stats = ExecutionStatistics(meta.num_docs_scanned, meta.num_entries_scanned_in_filter,
                                     meta.num_entries_scanned_post_filter, meta.num_total_docs)
@@ -665,6 +668,14 @@ def _read_result(ctx: B200Context, handle, q: QueryContext, kind: int, keep_hand
                 n = L.pb200_result_distinct(handle, a, row, _ptr(buf), len(buf))
                 if n < 0:
                     _lib.check(int(n))
+                distinct[(a, row)] = buf
+        elif agg.function == "DISTINCTCOUNTHLL" and histograms:   # its long column is the estimate: ask for the size
+            for row in range(rows):
+                n = L.pb200_result_distinct(handle, a, row, None, 0)
+                if n < 0:
+                    _lib.check(int(n))
+                buf = np.zeros(int(n), dtype=np.int32)
+                _lib.check(min(0, int(L.pb200_result_distinct(handle, a, row, _ptr(buf), len(buf)))))
                 distinct[(a, row)] = buf
     hists = {}
     for a, agg in enumerate(q.aggregations):
@@ -768,7 +779,7 @@ class B200PlanMaker:
     def execute_segments(self, segments: Sequence[IndexSegment], query: QueryContext, merge: bool = False,
                          keep_handle: bool = False, reduce_world: int = 0, merged_docs_bound: int = 0,
                          no_count_carrier: bool = False, defer: Optional[bool] = None, views: bool = False,
-                         ordered: bool = True) -> List[ResultsBlock]:
+                         ordered: bool = True, sets: bool = False) -> List[ResultsBlock]:
         """All segments of one query in ONE device submission (makeInstancePlan-level batching).  With merge=True the
         segments (sharing dictionaries) are combined on the device and one block is returned; with keep_handle=True as
         well, a group-by block comes back WITHOUT its groups extracted (PB200_Q_DEFER_FINALIZE): its dense device tables
@@ -776,7 +787,9 @@ class B200PlanMaker:
         A GROUP BY query with an ORDER BY gets its rows ordered and trimmed by the library (order_spec; a deferred block
         when it is extracted); ordered=False returns every group in the library's row order.  A query with HAVING gets
         its rows filtered by the library before that order when the call's result is final (merge=True, or one segment,
-        and ordered); per-segment blocks of several segments come back unfiltered, for the caller's merge to filter."""
+        and ordered); per-segment blocks of several segments come back unfiltered, for the caller's merge to filter.
+        Per-segment blocks carry the intermediates of a by-value merge (DISTINCTCOUNTHLL sets among them); sets=True
+        reads those of a merged block too."""
         # merge + keep_handle: the caller reduces the dense tables across GPUs first; groups are extracted afterwards
         # defer=False with keep_handle=True: extracted blocks that keep their native handle (to_datatable); release() them
         if defer is None:
@@ -795,7 +808,11 @@ class B200PlanMaker:
         kinds = (C.c_int32 * n)()
         spec = order_spec(query, merge) if ordered else None
         having = having_spec(query) if ordered and (merge or n == 1) else None
-        pct = [a.function == "PERCENTILE" for a in query.aggregations]
+        for a in query.aggregations:
+            if a.function == "DISTINCTCOUNTHLL" and a.arg == 0:   # the library reads an argument of 0 as the default 8
+                raise UnsupportedQueryError(_lib.E_UNSUPPORTED, "DISTINCTCOUNTHLL with log2m 0 is not accelerated")
+        # one argument per aggregation: the percentile of a PERCENTILE, the log2m of a DISTINCTCOUNTHLL
+        pct = [a.function in ("PERCENTILE", "DISTINCTCOUNTHLL") for a in query.aggregations]
         if any(a.function in WITHTIME_FUNCTIONS for a in query.aggregations):
             # FIRST/LASTWITHTIME: the time column and the type literal travel beside the query (pb200h_execute_agg_args)
             args = (_lib.HAggArg * len(pct))(*[
@@ -821,7 +838,7 @@ class B200PlanMaker:
         # views=True: the blocks' arrays alias the native results' pinned memory (no copy); keep the block alive while you
         # use them and drop it before the context closes
         blocks = [_read_result(self.ctx, C.c_void_p(res[i]), query, kinds[i if not merge else 0], keep_handle, views,
-                               histograms=not merge) for i in range(nres)]
+                               histograms=not merge or sets) for i in range(nres)]
         self.last_device_ms = blocks[0].device_ms
         return blocks
 

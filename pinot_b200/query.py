@@ -50,12 +50,12 @@ FilterNode = Union[Filter, Predicate]
 @dataclass
 class Aggregation:
     function: str  # COUNT | SUM | MIN | MAX | AVG | DISTINCTCOUNT | PERCENTILE | VARPOP | VARSAMP | STDDEVPOP | STDDEVSAMP
-    #                | FIRSTWITHTIME | LASTWITHTIME | DISTINCTSUM | DISTINCTAVG
+    #                | FIRSTWITHTIME | LASTWITHTIME | DISTINCTSUM | DISTINCTAVG | DISTINCTCOUNTHLL
     column: Optional[str] = None  # None for COUNT(*)
     # FILTER (WHERE ...) clause of this function (QueryContext.getFilteredAggregationFunctions: Pair<function, FilterContext>);
     # evaluated together with the query's own filter (AggregationFunctionUtils.buildFilteredAggregationInfos)
     filter: Optional["FilterNode"] = None
-    arg: Optional[float] = None  # PERCENTILE: the percentile, 0 <= p <= 100
+    arg: Optional[float] = None  # PERCENTILE: the percentile, 0 <= p <= 100; DISTINCTCOUNTHLL: log2m (an int, default 8)
     # FIRSTWITHTIME / LASTWITHTIME(column, time_column, 'value_type'): the time column and the type literal (upper case)
     time_column: Optional[str] = None
     value_type: Optional[str] = None
@@ -65,6 +65,8 @@ class Aggregation:
     def __str__(self):
         if self.function == "PERCENTILE":
             return f"percentile({self.column}, {self.arg:g})"
+        if self.function == "DISTINCTCOUNTHLL" and self.arg != HLL_DEFAULT_LOG2M:
+            return f"distinctcounthll({self.column}, {self.arg})"
         if self.function in WITHTIME_FUNCTIONS:
             return f"{self.function.lower()}({self.column},{self.time_column},'{self.value_type}')"
         return f"{self.function.lower()}({self.column or '*'})"
@@ -167,6 +169,101 @@ def distinct_final(function: str, values) -> float:
         return float(exact)   # numerator / denominator of ints: correctly rounded, subnormals included
     except OverflowError:
         return math.inf if exact > 0 else -math.inf
+
+
+# DISTINCTCOUNTHLL (DESIGN.md section 3.17): its intermediate is DISTINCTCOUNT's set of distinct values too, merged by union
+HLL_DEFAULT_LOG2M = 8
+_M32 = 0xFFFFFFFF
+_MURMUR_M = 0x5BD1E995
+
+
+def _hll_hash_long(data: int) -> int:
+    """stream-lib MurmurHash.hashLong of a Java long (any Python int, taken mod 2^64)."""
+    data &= 0xFFFFFFFFFFFFFFFF
+    h = 0
+    k = ((data & _M32) * _MURMUR_M) & _M32
+    k ^= k >> 24
+    h ^= (k * _MURMUR_M) & _M32
+    k = ((data >> 32) * _MURMUR_M) & _M32
+    k ^= k >> 24
+    h = (h * _MURMUR_M) & _M32
+    h ^= (k * _MURMUR_M) & _M32
+    h ^= h >> 13
+    h = (h * _MURMUR_M) & _M32
+    return h ^ (h >> 15)
+
+
+def _hll_hash_bytes(b: bytes, seed: int = -1) -> int:
+    """stream-lib MurmurHash.hash(byte[], length, seed): the tail bytes are sign-extended, as a Java byte is."""
+    n = len(b)
+    h = (seed ^ n) & _M32
+    for i in range(n >> 2):
+        k = (int.from_bytes(b[4 * i:4 * i + 4], "little") * _MURMUR_M) & _M32
+        k ^= k >> 24
+        k = (k * _MURMUR_M) & _M32
+        h = ((h * _MURMUR_M) & _M32) ^ k
+    left = n & 3
+    if left:
+        sx = [x - 256 if x > 127 else x for x in b[n - left:]]
+        if left >= 3:
+            h ^= (sx[-3] << 16) & _M32
+        if left >= 2:
+            h ^= (sx[-2] << 8) & _M32
+        h ^= sx[-1] & _M32
+        h = (h * _MURMUR_M) & _M32
+    h ^= h >> 13
+    h = (h * _MURMUR_M) & _M32
+    return h ^ (h >> 15)
+
+
+def hll_hash(value, data_type: Optional[str] = None) -> int:
+    """MurmurHash.hash(Object) of a dictionary value: INT / LONG as a long, FLOAT through floatToRawIntBits
+    (sign-extended), DOUBLE through doubleToRawLongBits, STRING over its UTF-8 bytes.  data_type ("INT" ... "STRING")
+    tells a FLOAT from a DOUBLE; without it a float is a DOUBLE."""
+    value = value.item() if hasattr(value, "item") else value
+    if isinstance(value, str):
+        return _hll_hash_bytes(value.encode("utf-8"))
+    if isinstance(value, float):
+        if data_type == "FLOAT":
+            return _hll_hash_long(struct.unpack("<i", struct.pack("<f", value))[0])
+        return _hll_hash_long(struct.unpack("<q", struct.pack("<d", value))[0])
+    return _hll_hash_long(int(value))
+
+
+_TYPE_NAMES = {0: "INT", 1: "LONG", 2: "FLOAT", 3: "DOUBLE", 4: "STRING"}
+
+
+class HllSet(set):
+    """The distinct values of a DISTINCTCOUNTHLL intermediate and the column's stored type (a FLOAT hashes other bits
+    than the same DOUBLE); unions in place keep the type."""
+
+    def __init__(self, values=(), data_type=None):
+        super().__init__(values)
+        self.data_type = _TYPE_NAMES.get(data_type, data_type)
+
+
+def hll_final(values, log2m: int = HLL_DEFAULT_LOG2M, data_type: Optional[str] = None) -> int:
+    """DISTINCTCOUNTHLL of a set of distinct values (DESIGN.md section 3.17): the estimate of stream-lib's HyperLogLog with
+    2^log2m registers offered every member (HyperLogLog.cardinality, registerSum summed exactly, Java's Math.round).  An
+    empty set gives 0."""
+    p = int(log2m)
+    m = 1 << p
+    reg = [0] * m
+    for v in values:
+        x = hll_hash(v, data_type)
+        y = ((x << p) & _M32) | ((1 << (p - 1)) + 1)
+        j = x >> (32 - p)
+        reg[j] = max(reg[j], 33 - y.bit_length())
+    register_sum = math.ldexp(sum(1 << (33 - p - r) for r in reg), -(33 - p))   # exact: an integer below 2^34, scaled
+    zeros = reg.count(0)
+    alpha_mm = {4: 0.673 * m * m, 5: 0.697 * m * m, 6: 0.709 * m * m}.get(p, (0.7213 / (1 + 1.079 / m)) * m * m)
+    estimate = alpha_mm * (1 / register_sum)
+    if estimate <= 2.5 * m:
+        if zeros == 0:
+            return (1 << 63) - 1   # m * log(+inf): Math.round(+inf)
+        estimate = m * math.log(m / zeros)
+    f = math.floor(estimate)
+    return f + (1 if estimate - f >= 0.5 else 0)
 
 
 MOMENT_FUNCTIONS = ("VARPOP", "VARSAMP", "STDDEVPOP", "STDDEVSAMP")

@@ -45,14 +45,14 @@ import re
 from dataclasses import dataclass, field
 from typing import List, Optional
 
-from .query import WITHTIME_FUNCTIONS, WITHTIME_TYPES, Aggregation, Filter, FilterNode, Predicate, QueryContext, flatten, optimize_filter
+from .query import HLL_DEFAULT_LOG2M, WITHTIME_FUNCTIONS, WITHTIME_TYPES, Aggregation, Filter, FilterNode, Predicate, QueryContext, flatten, optimize_filter
 
 _TOKEN = re.compile(r"\s*(?:(\d+\.\d+(?:[eE][-+]?\d+)?|-?\d+\.\d+|-?\d+)|'((?:[^']|'')*)'|(<=|>=|<>|!=|[=<>(),*+/%-])|"
                     r"([A-Za-z_$][A-Za-z0-9_$]*))")
 
 # VarianceAggregationFunction: both spellings of each function, the underscore one canonicalised to the other
 _ALIASES = {"VAR_POP": "VARPOP", "VAR_SAMP": "VARSAMP", "STDDEV_POP": "STDDEVPOP", "STDDEV_SAMP": "STDDEVSAMP"}
-_FUNCTIONS = {"COUNT", "SUM", "MIN", "MAX", "AVG", "DISTINCTCOUNT", "DISTINCTSUM", "DISTINCTAVG", "PERCENTILE", "VARPOP",
+_FUNCTIONS = {"COUNT", "SUM", "MIN", "MAX", "AVG", "DISTINCTCOUNT", "DISTINCTSUM", "DISTINCTAVG", "DISTINCTCOUNTHLL", "PERCENTILE", "VARPOP",
               "VARSAMP", "STDDEVPOP", "STDDEVSAMP", *WITHTIME_FUNCTIONS} | set(_ALIASES)
 # FN(DISTINCT col): the function Pinot's query compiler rewrites it into
 _DISTINCT_OF = {"COUNT": "DISTINCTCOUNT", "SUM": "DISTINCTSUM", "AVG": "DISTINCTAVG"}
@@ -106,6 +106,8 @@ def having_name(agg: Aggregation) -> str:
     """How a HAVING leaf names an aggregation (QueryContext.having)."""
     if agg.function == "PERCENTILE":
         return f"percentile({agg.column},{agg.arg!r})"
+    if agg.function == "DISTINCTCOUNTHLL" and agg.arg != HLL_DEFAULT_LOG2M:
+        return f"distinctcounthll({agg.column},{agg.arg})"
     if agg.function in WITHTIME_FUNCTIONS:
         return str(agg)
     return f"{agg.function.lower()}({agg.column or '*'})"
@@ -195,6 +197,18 @@ class _Parser:
             self.expect_op(",")
             p = _percentile_arg(self.literal())
         return col, p
+
+    def hll_call(self):
+        """After `DISTINCTCOUNTHLL(`: the column and log2m, an integer literal in 0..30 (the reference's range; default 8),
+        up to the `)`."""
+        col = self.column()
+        log2m = HLL_DEFAULT_LOG2M
+        if self.take_op(","):
+            v = self.literal()
+            if isinstance(v, bool) or not isinstance(v, int) or not 0 <= v <= 30:
+                raise SqlError(f"DISTINCTCOUNTHLL needs an integer log2m in 0..30, got {v!r}")
+            log2m = v
+        return col, log2m
 
     def withtime_call(self, fn: str) -> Aggregation:
         """After `FIRSTWITHTIME(` / `LASTWITHTIME(`: data column, time column and type literal, up to the `)`."""
@@ -299,6 +313,9 @@ class _Parser:
             agg = Aggregation("PERCENTILE", col, arg=pct)
         elif fn in WITHTIME_FUNCTIONS:
             agg = self.withtime_call(fn)
+        elif fn == "DISTINCTCOUNTHLL" and self.peek() != ("op", "*"):
+            col, log2m = self.hll_call()
+            agg = Aggregation(fn, col, arg=log2m)
         elif self.take_op("*"):
             if fn != "COUNT":
                 raise SqlError(f"{fn}(*) is not valid")
@@ -474,7 +491,7 @@ def resolve_order_by(query: QueryContext) -> List[tuple]:
             fn, col = _ALIASES.get(m.group(1).upper(), m.group(1).upper()), m.group(2)
             arg = None if m.group(3) is None else float(m.group(3))
             for a, agg in enumerate(query.aggregations):
-                if agg.function == fn and (fn == "COUNT" or agg.column == col) and (fn != "PERCENTILE" or agg.arg == arg):
+                if agg.function == fn and (fn == "COUNT" or agg.column == col) and (fn not in ("PERCENTILE", "DISTINCTCOUNTHLL") or agg.arg == arg):
                     found = a
                     break
         if found is None:
@@ -587,6 +604,10 @@ def parse(sql: str, **options) -> QueryContext:
                 elif name.upper() in WITHTIME_FUNCTIONS:
                     expr = having_name(p.withtime_call(name.upper()))
                     p.expect_op(")")
+                elif name.upper() == "DISTINCTCOUNTHLL":
+                    inner, log2m = p.hll_call()
+                    p.expect_op(")")
+                    expr = f"distinctcounthll({inner},{log2m})"
                 elif p.take_kw("DISTINCT"):
                     inner = p.distinct_call(name.upper())
                     p.expect_op(")")
