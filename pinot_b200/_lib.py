@@ -19,8 +19,6 @@ FWD_DICT_FIXEDBIT, FWD_DICT_SORTED, FWD_RAW_FIXEDBYTE = 0, 1, 2
 AGG_CODES = {"COUNT": 0, "SUM": 1, "MIN": 2, "MAX": 3, "AVG": 4, "DISTINCTCOUNT": 5, "PERCENTILE": 6,
              "VARPOP": 7, "VARSAMP": 8, "STDDEVPOP": 9, "STDDEVSAMP": 10, "FIRSTWITHTIME": 11, "LASTWITHTIME": 12,
              "DISTINCTSUM": 13, "DISTINCTAVG": 14, "DISTINCTCOUNTHLL": 15}
-WITHTIME_FUNCTIONS = ("FIRSTWITHTIME", "LASTWITHTIME")
-MOMENT_FUNCTIONS = ("VARPOP", "VARSAMP", "STDDEVPOP", "STDDEVSAMP")
 FILTER_CODES = {"AND": 0, "OR": 1, "NOT": 2, "EQ": 3, "NEQ": 4, "IN": 5, "NOT_IN": 6, "RANGE": 7, "REGEXP_LIKE": 8}
 REGIMES = {0: "NONE", 1: "ARRAY", 2: "INT_MAP", 3: "LONG_MAP", 4: "ARRAY_MAP"}
 OPERATOR_KINDS = {0: "AGGREGATION", 1: "GROUP_BY", 2: "NON_SCAN_AGGREGATION", 3: "EMPTY", 4: "STAR_TREE"}

@@ -157,7 +157,7 @@ def main(argv=None) -> int:
     from . import sql
     from ._lib import Pb200Error
     from .plan_maker import B200Context, B200PlanMaker, DictionaryDomain
-    from .query import is_multi_column_expression
+    from .query import functions_where, is_multi_column_expression
 
     if sql.is_distinct(args.sql):
         return _distinct(args, sql.parse_distinct(args.sql))
@@ -174,10 +174,7 @@ def main(argv=None) -> int:
             if args.merge_on_device and len(segments) > 1:
                 cols = list(dict.fromkeys(list(query.group_by) + [a.column for a in query.aggregations
                                                                   if a.column and not is_multi_column_expression(a.function, a.column)
-                                                                  and a.function in ("MIN", "MAX", "DISTINCTCOUNT", "PERCENTILE",
-                                                                                 "DISTINCTSUM", "DISTINCTAVG", "DISTINCTCOUNTHLL",
-                                                                                 "VARPOP", "VARSAMP", "STDDEVPOP", "STDDEVSAMP",
-                                                                                 "FIRSTWITHTIME", "LASTWITHTIME")]
+                                                                  and a.function in functions_where(lambda f: f.dict_ids or f.arg == "time")]
                                            + [a.time_column for a in query.aggregations if a.time_column and "(" not in a.time_column]))
                 if cols:
                     domain = DictionaryDomain.build(ctx, segments, cols)

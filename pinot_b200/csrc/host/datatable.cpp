@@ -47,18 +47,6 @@ struct Out {
   void bytes(const Out& o) { b.insert(b.end(), o.b.begin(), o.b.end()); }
 };
 
-const char* fn_name(int fn) {
-  switch (fn) {
-    case PB200_AGG_COUNT: return "count";
-    case PB200_AGG_SUM: return "sum";
-    case PB200_AGG_MIN: return "min";
-    case PB200_AGG_MAX: return "max";
-    case PB200_AGG_AVG: return "avg";
-    case PB200_AGG_DISTINCTSUM: return "distinctsum";
-    case PB200_AGG_DISTINCTAVG: return "distinctavg";
-    default: return "distinctcount";
-  }
-}
 const char* type_name(int t) {
   switch (t) {
     case PB200_INT: return "INT";
@@ -82,27 +70,13 @@ extern "C" int64_t pb200h_result_to_datatable(const pb200h_query* q, const pb200
     set_error("a result filtered by HAVING is final: it is not written as a server DataTable");
     return PB200_E_UNSUPPORTED;
   }
-  for (int a = 0; a < nagg; a++)
-    if (q->aggs[a].function == PB200_AGG_DISTINCTCOUNTHLL) {   // its intermediate is stream-lib's serialized registers
-      set_error("DISTINCTCOUNTHLL is not written as a server DataTable (the reference's HyperLogLog bytes are not restated)");
-      return PB200_E_UNSUPPORTED;
-    }
-  for (int a = 0; a < nagg; a++)
-    if (q->aggs[a].function == PB200_AGG_PERCENTILE) {  // its intermediate is the reference's DoubleArrayList of values
-      set_error("PERCENTILE intermediates are not written as DataTable objects");
-      return PB200_E_UNSUPPORTED;
-    }
-  for (int a = 0; a < nagg; a++)
-    if (q->aggs[a].function == PB200_AGG_FIRSTWITHTIME || q->aggs[a].function == PB200_AGG_LASTWITHTIME) {
-      // the reference's intermediate is a (value, time) pair object
-      set_error("FIRST/LASTWITHTIME intermediates are not written as DataTable objects");
-      return PB200_E_UNSUPPORTED;
-    }
-  for (int a = 0; a < nagg; a++)
-    if (pb200::is_moments_fn(q->aggs[a].function)) {   // the reference's intermediate is a VarianceTuple
-      set_error("VAR/STDDEV intermediates are not written as DataTable objects");
-      return PB200_E_UNSUPPORTED;
-    }
+  // the reference's intermediates of the functions without a DataTable type: stream-lib's serialized HyperLogLog registers,
+  // PERCENTILE's DoubleArrayList of values, a (value, time) pair object, a VarianceTuple
+  for (int a : aggs_by_family(*q, {PB200_AGG_DISTINCTCOUNTHLL, PB200_AGG_PERCENTILE, PB200_AGG_FIRSTWITHTIME, PB200_AGG_VARPOP})) {
+    const pb200::AggFn* d = pb200::agg_fn(q->aggs[a].function);
+    if (!d) { set_error("unknown aggregation function %d", q->aggs[a].function); return PB200_E_INVALID; }
+    if (!d->datatable) { set_error("%s", d->datatable_refusal); return PB200_E_UNSUPPORTED; }
+  }
   const size_t rows = meta.num_groups < 0 ? 1 : (size_t)meta.num_groups;
   // ---- intermediates through the C-ABI accessors ----
   std::vector<int32_t> keys(rows * (size_t)std::max(ngb, 1));
@@ -136,8 +110,8 @@ extern "C" int64_t pb200h_result_to_datatable(const pb200h_query* q, const pb200
         agg_cols[a] = &seg->cols[ci].decode_column();
       }
     }
-    names.push_back(std::string(fn_name(fn)) + "(" + arg + ")");
-    types.push_back(fn == PB200_AGG_COUNT ? "LONG" : (fn == PB200_AGG_AVG || fn == PB200_AGG_DISTINCTCOUNT || pb200::is_distinct_value_fn(fn)) ? "OBJECT" : "DOUBLE");
+    names.push_back(lower_fn_name(fn) + "(" + arg + ")");
+    types.push_back(pb200::agg_fn(fn)->datatable);
     width.push_back(8);
   }
   // ---- rows ----

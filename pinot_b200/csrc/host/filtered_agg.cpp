@@ -47,11 +47,6 @@ int execute_filtered(pb200_ctx* ctx, const pb200h_query& q, const pb200_order_by
   if (q.merge_segments == 2) { set_error("FILTER clauses with a deferred (cross-GPU) combine are not accelerated"); return PB200_E_UNSUPPORTED; }
   const int nagg = q.num_aggs, ngb = q.num_group_by;
   const int nres = q.merge_segments ? 1 : nseg;
-  for (int a = 0; a < nagg; a++)   // the per-clause submissions carry no time columns
-    if (q.aggs[a].function == PB200_AGG_FIRSTWITHTIME || q.aggs[a].function == PB200_AGG_LASTWITHTIME) {
-      set_error("FIRST/LASTWITHTIME in a query with FILTER (WHERE ...) clauses is not accelerated");
-      return PB200_E_UNSUPPORTED;
-    }
   // ---- infos: distinct FILTER clauses in order of first appearance, then the main filter ----
   struct Info { int start = 0, count = 0; std::vector<int> aggs; };
   std::vector<Info> infos;

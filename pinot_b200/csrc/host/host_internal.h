@@ -183,6 +183,12 @@ bool is_multi_column_expression(const char* text);
 // the functions that take a multi-column expression as their argument
 inline bool expression_function(int fn) { return fn == PB200_AGG_SUM || fn == PB200_AGG_AVG || fn == PB200_AGG_MIN || fn == PB200_AGG_MAX; }
 int derive_query_names(pb200_ctx* ctx, const pb200h_query& q, pb200h_segment* const* segs, int nseg, const char* const* extra, int nextra);
+// the name of function fn (PB200_AGG_*) in lower case, as result column names spell it
+std::string lower_fn_name(int fn);
+// The positions of q's aggregations in the order a check that refuses some functions visits them: those of the families of
+// `first` in that order, then the others, each in query order.  So a query with several refused functions is refused
+// for the same one whatever their order in the query.
+std::vector<int> aggs_by_family(const pb200h_query& q, std::initializer_list<int> first);
 }  // namespace pb200h
 
 namespace pb200h {

@@ -7,12 +7,14 @@
 //   core/plan/AggregationPlanNode.java:90-121,159-190      NonScanBasedAggregationOperator shortcut
 // and hands dictId-space trees to the device through include/pinot_b200.h only.
 #include <algorithm>
+#include <cctype>
 #include <cmath>
 #include <cstdio>
 #include <cstring>
 #include <fstream>
 #include <map>
 #include <memory>
+#include <numeric>
 #include <sstream>
 #include <string>
 #include <vector>
@@ -339,6 +341,28 @@ pb200_result* host_result(const pb200h_segment& seg, const pb200h_query& q, bool
 }  // namespace
 
 namespace pb200h {
+
+std::string lower_fn_name(int fn) {
+  std::string s = pb200::agg_fn(fn)->name;
+  for (char& ch : s) ch = (char)std::tolower((unsigned char)ch);
+  return s;
+}
+
+std::vector<int> aggs_by_family(const pb200h_query& q, std::initializer_list<int> first) {
+  auto rank = [&](int a) {
+    const pb200::AggFn* d = pb200::agg_fn(q.aggs[a].function);
+    int r = 0;
+    for (int fn : first) {
+      if (d && strcmp(d->family, pb200::agg_fn(fn)->family) == 0) return r;
+      r++;
+    }
+    return r;
+  };
+  std::vector<int> order(q.num_aggs);
+  std::iota(order.begin(), order.end(), 0);
+  std::stable_sort(order.begin(), order.end(), [&](int x, int y) { return rank(x) < rank(y); });
+  return order;
+}
 
 std::vector<int32_t> matching_dict_ids(const HostColumn& c, const pb200h_filter_node& n, const pb200h_literal* lits) {
   Evaluated e = evaluate(c, n, lits);
@@ -807,8 +831,7 @@ extern "C" int32_t pb200h_execute_agg_args(pb200_ctx* ctx, const pb200h_query* q
   if (q->num_group_by == 0) order = nullptr;  // aggregation only: one row, nothing to order
   std::vector<const char*> time_names;   // FIRST/LASTWITHTIME time columns: derived like every other name of the query
   for (int a = 0; a < q->num_aggs; a++) {
-    const int fn = q->aggs[a].function;
-    if (fn != PB200_AGG_FIRSTWITHTIME && fn != PB200_AGG_LASTWITHTIME) continue;
+    if (!pb200::is_withtime_fn(q->aggs[a].function)) continue;
     if (!args || !args[a].time_column) { set_error("FIRST/LASTWITHTIME (aggregation %d) needs its time column: call pb200h_execute_agg_args", a); return PB200_E_INVALID; }
     time_names.push_back(args[a].time_column);
   }
@@ -818,46 +841,21 @@ extern "C" int32_t pb200h_execute_agg_args(pb200_ctx* ctx, const pb200h_query* q
   bool any_clause = false;   // some aggregation has a FILTER (WHERE ...) clause
   if (q->agg_filter_count && q->agg_filter_start && q->agg_filter_nodes)
     for (int a = 0; a < q->num_aggs; a++) any_clause |= q->agg_filter_count[a] > 0;
-  for (int a = 0; a < q->num_aggs; a++) {
-    const int fn = q->aggs[a].function;
-    if ((fn == PB200_AGG_FIRSTWITHTIME || fn == PB200_AGG_LASTWITHTIME) && any_clause) {   // the per-clause submissions carry no time columns
-      set_error("FIRST/LASTWITHTIME in a query with FILTER (WHERE ...) clauses is not accelerated");
-      return PB200_E_UNSUPPORTED;
+  // The device path's argument checks, before any segment can be answered on the host.  FILTER clauses run as one
+  // submission per clause (host/filtered_agg.cpp), which carries no percentiles, time columns, moments or finalized value
+  // sets: such a function anywhere in the query -- with its own clause or next to another function's -- goes to the
+  // stock operator.
+  std::vector<int> hll_log2m(q->num_aggs, 0);
+  for (int a : aggs_by_family(*q, {PB200_AGG_FIRSTWITHTIME, PB200_AGG_PERCENTILE, PB200_AGG_VARPOP, PB200_AGG_DISTINCTSUM, PB200_AGG_DISTINCTCOUNTHLL})) {
+    const pb200::AggFn* d = pb200::agg_fn(q->aggs[a].function);
+    if (!d) continue;
+    if (d->arg == pb200::ARG_PERCENTILE) {
+      if (!args) { set_error("PERCENTILE (aggregation %d) needs its percentile: call pb200h_execute_args", a); return PB200_E_INVALID; }
+      if (int rc = pb200::check_percentile(args[a].p, a)) return rc;
     }
-  }
-  for (int a = 0; a < q->num_aggs; a++) {
-    if (q->aggs[a].function != PB200_AGG_PERCENTILE) continue;
-    // the same checks as the device path, made before any segment can be answered on the host
-    if (!args) { set_error("PERCENTILE (aggregation %d) needs its percentile: call pb200h_execute_args", a); return PB200_E_INVALID; }
-    if (!(args[a].p >= 0.0 && args[a].p <= 100.0)) { set_error("PERCENTILE (aggregation %d): percentile %g outside [0, 100]", a, args[a].p); return PB200_E_INVALID; }
-    // FILTER clauses run as one submission per clause (host/filtered_agg.cpp), which carries no percentiles: a PERCENTILE
-    // anywhere in such a query -- with its own clause or next to another function's -- goes to the stock operator
-    if (any_clause) {
-      set_error("PERCENTILE in a query with FILTER (WHERE ...) clauses is not accelerated");
-      return PB200_E_UNSUPPORTED;
-    }
-  }
-  for (int a = 0; a < q->num_aggs; a++)
-    if (pb200::is_moments_fn(q->aggs[a].function) && any_clause) {   // the per-clause submissions carry no moments
-      set_error("VAR/STDDEV in a query with FILTER (WHERE ...) clauses is not accelerated");
-      return PB200_E_UNSUPPORTED;
-    }
-  for (int a = 0; a < q->num_aggs; a++)
-    if (pb200::is_distinct_value_fn(q->aggs[a].function) && any_clause) {   // nor the finalized sums of value sets
-      set_error("DISTINCTSUM/DISTINCTAVG in a query with FILTER (WHERE ...) clauses is not accelerated");
-      return PB200_E_UNSUPPORTED;
-    }
-  std::vector<int> hll_log2m(q->num_aggs, 0);   // DISTINCTCOUNTHLL: the device path's checks, before any segment is answered here
-  for (int a = 0; a < q->num_aggs; a++) {
-    if (!pb200::is_hll_fn(q->aggs[a].function)) continue;
-    if (any_clause) { set_error("DISTINCTCOUNTHLL in a query with FILTER (WHERE ...) clauses is not accelerated"); return PB200_E_UNSUPPORTED; }
-    const double lv = args ? args[a].p : 0.0;
-    if (!(lv >= 0.0 && lv <= 30.0) || lv != (double)(int)lv) { set_error("DISTINCTCOUNTHLL (aggregation %d): log2m %g is not an integer in 0..30", a, lv); return PB200_E_INVALID; }
-    hll_log2m[a] = lv == 0.0 ? pb200::kHllDefaultLog2m : (int)lv;
-    if (hll_log2m[a] < pb200::kHllMinLog2m || hll_log2m[a] > pb200::kHllMaxLog2m) {
-      set_error("DISTINCTCOUNTHLL (aggregation %d): log2m %d outside %d..%d is not accelerated", a, hll_log2m[a], pb200::kHllMinLog2m, pb200::kHllMaxLog2m);
-      return PB200_E_UNSUPPORTED;
-    }
+    if (!d->filter_clause && any_clause) { set_error("%s in a query with FILTER (WHERE ...) clauses is not accelerated", d->family); return PB200_E_UNSUPPORTED; }
+    if (d->arg == pb200::ARG_LOG2M)
+      if (int rc = pb200::hll_log2m(args ? args[a].p : 0.0, a, &hll_log2m[a])) return rc;
   }
   ExprFilterScope expr_filters;   // expression leaves become device doc sets once, also for the FILTER clauses' submissions
   if (int rc = resolve_expr_filters(ctx, *q, segs, nseg, expr_filters, true)) return rc;
@@ -904,7 +902,7 @@ extern "C" int32_t pb200h_execute_agg_args(pb200_ctx* ctx, const pb200h_query* q
       aggs[a].column = s0.column_index(q->aggs[a].column);
       if (aggs[a].column < 0) { set_error("unknown aggregation column '%s'", q->aggs[a].column ? q->aggs[a].column : "(null)"); return PB200_E_INVALID; }
       const HostColumn& c = s0.cols[aggs[a].column];
-      const bool wt = q->aggs[a].function == PB200_AGG_FIRSTWITHTIME || q->aggs[a].function == PB200_AGG_LASTWITHTIME;
+      const bool wt = pb200::is_withtime_fn(q->aggs[a].function);
       if (c.data_type == PB200_STRING && q->aggs[a].function != PB200_AGG_DISTINCTCOUNT && !pb200::is_hll_fn(q->aggs[a].function) && !wt) { set_error("%s over STRING column", "aggregation"); return PB200_E_UNSUPPORTED; }
       if (args) dev_args[a].p = args[a].p;
       if (wt) {

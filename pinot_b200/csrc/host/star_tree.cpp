@@ -245,8 +245,7 @@ extern "C" int32_t pb200h_startree_attach(pb200_ctx* ctx, pb200h_segment* seg, c
     pack_bits(ids, bits, packed);
     bufs.push_back(std::move(packed));
     bufs.push_back(std::move(dict));
-    const std::string fn = sm.function == PB200_AGG_COUNT ? "count" : sm.function == PB200_AGG_SUM ? "sum" : sm.function == PB200_AGG_MIN ? "min" : "max";
-    names.push_back(fn + "__" + (sm.column ? sm.column : "*"));
+    names.push_back(lower_fn_name(sm.function) + "__" + (sm.column ? sm.column : "*"));
     pb200h_column c;
     memset(&c, 0, sizeof c);
     c.data_type = is_long ? PB200_LONG : PB200_DOUBLE; c.has_dictionary = 1; c.bits_per_value = bits; c.cardinality = card; c.dict_entry_bytes = 8;
@@ -328,8 +327,7 @@ extern "C" int32_t pb200h_startree_build(pb200_ctx* ctx, pb200h_segment* seg, co
     spec.metric_col.push_back(bc);
     st->metric_fn.push_back(p.function);
     st->metric_base_col.push_back(bc);
-    const char* fn = p.function == PB200_AGG_COUNT ? "count" : p.function == PB200_AGG_SUM ? "sum" : p.function == PB200_AGG_MIN ? "min" : "max";
-    metric_names.push_back(std::string(fn) + "__" + (bc < 0 ? "*" : p.column));
+    metric_names.push_back(lower_fn_name(p.function) + "__" + (bc < 0 ? "*" : p.column));
   }
   pb200::StarBuildResult res;
   if (int rc = pb200::startree_build(ctx, seg->dev, spec, &res)) return rc;

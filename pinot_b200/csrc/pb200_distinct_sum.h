@@ -13,8 +13,6 @@ namespace pb200 {
 
 typedef __int128 i128;
 
-PB200_MHD bool is_distinct_value_fn(int fn) { return fn == PB200_AGG_DISTINCTSUM || fn == PB200_AGG_DISTINCTAVG; }
-
 // special members of S
 enum : uint32_t { DS_NAN = 1, DS_POS_INF = 2, DS_NEG_INF = 4 };
 
@@ -23,11 +21,11 @@ enum : uint32_t { DS_NAN = 1, DS_POS_INF = 2, DS_NEG_INF = 4 };
 // extraction, ORDER BY and HAVING only read them.  Group-by: kDsWords words per table entry; aggregation only: kDsWords
 // per result and set.
 constexpr int kDsWords = 6;
-PB200_MHD int ds_final_word(int fn) { return fn == PB200_AGG_DISTINCTAVG ? 5 : 4; }
+PB200_HD int ds_final_word(int fn) { return fn == PB200_AGG_DISTINCTAVG ? 5 : 4; }
 
 // Decomposes a double into m * 2^x with m an odd integer, |m| < 2^53 (m = 0, x = 0 for +-0.0), so that x is the
 // exponent of its lowest set bit.  Finite values only.
-PB200_MHD void double_parts(double v, long long* m, int* x) {
+PB200_HD void double_parts(double v, long long* m, int* x) {
   unsigned long long b;
   memcpy(&b, &v, 8);
   const int be = (int)((b >> 52) & 0x7FF);
@@ -48,7 +46,7 @@ PB200_MHD void double_parts(double v, long long* m, int* x) {
 
 // One member given as a double: adds its j = v / 2^e to *sum, or returns its flag (0 for a finite member).  The value is
 // on the grid (checked when the dictionary was admitted), so the shift is exact.
-PB200_MHD uint32_t ds_add_double(double v, int e, i128* sum) {
+PB200_HD uint32_t ds_add_double(double v, int e, i128* sum) {
   if (v != v) return DS_NAN;
   if (v == (double)INFINITY) return DS_POS_INF;
   if (v == -(double)INFINITY) return DS_NEG_INF;
@@ -60,7 +58,7 @@ PB200_MHD uint32_t ds_add_double(double v, int e, i128* sum) {
 }
 
 // The final value of DISTINCTSUM / DISTINCTAVG (fn) over a row's state: its exact sum of j, |S| and flags, grid exponent e
-PB200_MHD double distinct_final(int fn, i128 sum, unsigned long long n, uint32_t flags, int e) {
+PB200_HD double distinct_final(int fn, i128 sum, unsigned long long n, uint32_t flags, int e) {
   if ((flags & DS_NAN) || ((flags & DS_POS_INF) && (flags & DS_NEG_INF))) return (double)NAN;
   if (flags & DS_POS_INF) return (double)INFINITY;
   if (flags & DS_NEG_INF) return -(double)INFINITY;
@@ -71,7 +69,7 @@ PB200_MHD double distinct_final(int fn, i128 sum, unsigned long long n, uint32_t
   return round_dyadic(neg, mag, fn == PB200_AGG_DISTINCTAVG ? n : 1ull, e);
 }
 
-PB200_MHD i128 ds_sum_of(const unsigned long long* st) { return (i128)(((u128)st[1] << 64) | (u128)st[0]); }
+PB200_HD i128 ds_sum_of(const unsigned long long* st) { return (i128)(((u128)st[1] << 64) | (u128)st[0]); }
 
 // ---- host only ----
 // Whether the sorted dictionary `dict` (native values of `stored_type`, `card` entries) qualifies, and its exponent e:

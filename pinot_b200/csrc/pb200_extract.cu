@@ -385,10 +385,8 @@ static size_t layout_result(const pb200_result::Dense& d, ExtractDesc& e, size_t
   for (int a = 0; a < e.nagg; a++) {
     const int fn = e.fn[a];
     e.off_dbl[a] = take(8, rows);
-    const bool wt = fn == PB200_AGG_FIRSTWITHTIME || fn == PB200_AGG_LASTWITHTIME;
-    e.off_lng[a] = (fn == PB200_AGG_COUNT || fn == PB200_AGG_AVG || fn == PB200_AGG_SUM || fn == PB200_AGG_DISTINCTCOUNT ||
-                    fn == PB200_AGG_PERCENTILE || is_moments_fn(fn) || reads_distinct_set(fn) || wt) ? take(8, rows) : kNoCol;
-    e.off_ids[a] = (fn == PB200_AGG_MIN || fn == PB200_AGG_MAX || fn == PB200_AGG_PERCENTILE || wt) ? take(4, rows) : kNoCol;
+    e.off_lng[a] = agg_fn(fn)->long_col ? take(8, rows) : kNoCol;
+    e.off_ids[a] = agg_fn(fn)->ids_col ? take(4, rows) : kNoCol;
     e.off_mom[a] = is_moments_fn(fn) ? take(24, rows) : kNoCol;
   }
   return off;

@@ -15,13 +15,7 @@
 #include <math.h>
 #include <stdint.h>
 
-#include "../../include/pinot_b200.h"
-
-#ifdef __CUDACC__
-#define PB200_HD __host__ __device__ __forceinline__
-#else
-#define PB200_HD inline
-#endif
+#include "pb200_aggfn.h"
 
 namespace pb200 {
 

@@ -13,15 +13,9 @@
 #include <math.h>
 #include <stdint.h>
 
-#include "pb200_distinct_sum.h"
-#include "pb200_moments.h"
+#include "pb200_aggfn.h"
 
 namespace pb200 {
-
-PB200_MHD bool is_hll_fn(int fn) { return fn == PB200_AGG_DISTINCTCOUNTHLL; }
-// a function that reads a DISTINCTCOUNT bitset it may not own (ScanPlan::ds_rep): the scan builds the set, a finalize after
-// the scan turns it into the function's value
-PB200_MHD bool reads_distinct_set(int fn) { return is_distinct_value_fn(fn) || is_hll_fn(fn); }
 
 // whether every aggregation that reads the set held by aggregation b's bitset is a DISTINCTCOUNTHLL (fns: PB200_AGG_*,
 // ds_rep: ScanPlan::ds_rep; a DISTINCTCOUNT reads its own bitset)
@@ -36,7 +30,7 @@ constexpr int kHllMinLog2m = 4, kHllMaxLog2m = 12;   // accelerated; the referen
 constexpr long long kHllSaturated = 0x7FFFFFFFFFFFFFFFll;   // Math.round(+inf)
 
 // MurmurHash.hashLong: a long's two 32-bit halves, low first
-PB200_MHD uint32_t hll_hash_long(uint64_t data) {
+PB200_HD uint32_t hll_hash_long(uint64_t data) {
   const uint32_t m = 0x5bd1e995u;
   uint32_t h = 0;
   uint32_t k = (uint32_t)data * m;
@@ -54,7 +48,7 @@ PB200_MHD uint32_t hll_hash_long(uint64_t data) {
 
 // MurmurHash.hash(byte[], length, seed): little-endian 4-byte blocks, then the 1..3 tail bytes SIGN-extended (Java's
 // byte), unlike C MurmurHash2 for bytes >= 0x80
-PB200_MHD uint32_t hll_hash_bytes(const unsigned char* b, int len, uint32_t seed) {
+PB200_HD uint32_t hll_hash_bytes(const unsigned char* b, int len, uint32_t seed) {
   const uint32_t m = 0x5bd1e995u;
   uint32_t h = seed ^ (uint32_t)len;
   const int blocks = len >> 2;
@@ -81,14 +75,14 @@ PB200_MHD uint32_t hll_hash_bytes(const unsigned char* b, int len, uint32_t seed
 
 // MurmurHash.hash(Object) of a dictionary value of a numeric stored type, given as its raw bits: INT and FLOAT
 // (floatToRawIntBits) are sign-extended to a long, LONG and DOUBLE (doubleToRawLongBits) are the long
-PB200_MHD uint32_t hll_hash_value(int stored_type, uint64_t raw) {
+PB200_HD uint32_t hll_hash_value(int stored_type, uint64_t raw) {
   if (stored_type == PB200_INT || stored_type == PB200_FLOAT) return hll_hash_long((uint64_t)(int64_t)(int32_t)(uint32_t)raw);
   return hll_hash_long(raw);
 }
 
 // Whether b[0, len) is well-formed UTF-8 (no overlong forms, no surrogates, nothing above U+10FFFF): the bytes Java's
 // new String(bytes, UTF_8).getBytes(UTF_8) gives back unchanged.  Other bytes would be hashed as U+FFFD by the reference.
-PB200_MHD bool hll_utf8_valid(const unsigned char* b, int len) {
+PB200_HD bool hll_utf8_valid(const unsigned char* b, int len) {
   int i = 0;
   while (i < len) {
     const unsigned c = b[i];
@@ -109,7 +103,7 @@ PB200_MHD bool hll_utf8_valid(const unsigned char* b, int len) {
   return true;
 }
 
-PB200_MHD int hll_clz(uint32_t x) {
+PB200_HD int hll_clz(uint32_t x) {
 #ifdef __CUDA_ARCH__
   return __clz((int)x);
 #else
@@ -119,14 +113,14 @@ PB200_MHD int hll_clz(uint32_t x) {
 
 // HyperLogLog.offerHashed: register j = x >>> (32 - p), rank r = numberOfLeadingZeros((x << p) | (1 << (p - 1)) + 1) + 1
 // (Java's precedence puts the + 1 inside the OR operand), 1 <= r <= 33 - p
-PB200_MHD uint32_t hll_index(uint32_t x, int p) { return x >> (32 - p); }
-PB200_MHD uint32_t hll_rank(uint32_t x, int p) { return (uint32_t)hll_clz((x << p) | ((1u << (p - 1)) + 1u)) + 1u; }
+PB200_HD uint32_t hll_index(uint32_t x, int p) { return x >> (32 - p); }
+PB200_HD uint32_t hll_rank(uint32_t x, int p) { return (uint32_t)hll_clz((x << p) | ((1u << (p - 1)) + 1u)) + 1u; }
 
 // one register's term of registerSum = sum 1.0 / (1 << reg[j]), scaled by 2^(33 - p): an integer
-PB200_MHD unsigned long long hll_term(uint32_t reg, int p) { return 1ull << (33 - p - (int)reg); }
+PB200_HD unsigned long long hll_term(uint32_t reg, int p) { return 1ull << (33 - p - (int)reg); }
 
 // Math.round of a finite x >= 0: floor(x + 1/2) taken exactly (x - floor(x) is exact), saturating at Long.MAX_VALUE
-PB200_MHD long long hll_round(double x) {
+PB200_HD long long hll_round(double x) {
   if (!(x < 9223372036854775807.0)) return kHllSaturated;
   const double f = floor(x);
   return (long long)f + (x - f >= 0.5 ? 1 : 0);
@@ -134,7 +128,7 @@ PB200_MHD long long hll_round(double x) {
 
 // HyperLogLog.cardinality from the registers' scaled sum and the number of zero registers.  alpha_mm = hll_alpha_mm(p);
 // linear[z] = Math.round(m * Math.log(m / z)) for z = 0..m (hll_linear_table; z = 0 gives Long.MAX_VALUE).
-PB200_MHD long long hll_estimate(unsigned long long scaled_sum, uint32_t zeros, int p, double alpha_mm, const long long* linear) {
+PB200_HD long long hll_estimate(unsigned long long scaled_sum, uint32_t zeros, int p, double alpha_mm, const long long* linear) {
   const int m = 1 << p;
   const double register_sum = ldexp((double)scaled_sum, -(33 - p));   // exact: scaled_sum < 2^34
 #ifdef __CUDA_ARCH__

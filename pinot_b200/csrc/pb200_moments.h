@@ -16,19 +16,11 @@
 #include <algorithm>
 #include <cmath>
 
-#include "../../include/pinot_b200.h"
-
-#ifdef __CUDACC__
-#define PB200_MHD __host__ __device__ __forceinline__
-#else
-#define PB200_MHD inline
-#endif
+#include "pb200_aggfn.h"
 
 namespace pb200 {
 
 typedef unsigned __int128 u128;
-
-PB200_MHD bool is_moments_fn(int fn) { return fn >= PB200_AGG_VARPOP && fn <= PB200_AGG_STDDEVSAMP; }
 
 // The grid of one dictionary: value = c + k * 2^e.  c is kept exactly as c_mant * 2^c_exp (the C-ABI's form) and, for the
 // build kernel, as the column's own type (c_int: INT / LONG, c_dbl: FLOAT / DOUBLE).
@@ -49,7 +41,7 @@ struct Moments {
 };
 
 // From the three limb SUM tables of a row (each holds sum(limb) - n * 2^31) and its row count
-PB200_MHD Moments moments_from_sums(unsigned long long n, long long sum_k, long long sum_h, long long sum_l) {
+PB200_HD Moments moments_from_sums(unsigned long long n, long long sum_k, long long sum_h, long long sum_l) {
   const unsigned long long bias = n << 31;  // n < 2^32
   Moments m;
   m.n = n;
@@ -59,7 +51,7 @@ PB200_MHD Moments moments_from_sums(unsigned long long n, long long sum_k, long 
   return m;
 }
 
-PB200_MHD int bitlen128(u128 x) {
+PB200_HD int bitlen128(u128 x) {
   const unsigned long long hi = (unsigned long long)(x >> 64), lo = (unsigned long long)x;
 #ifdef __CUDA_ARCH__
   return hi ? 128 - __clzll((long long)hi) : (lo ? 64 - __clzll((long long)lo) : 0);
@@ -72,7 +64,7 @@ PB200_MHD int bitlen128(u128 x) {
 // the subnormal range and to +-inf on overflow.  The quotient is developed bit by bit until it holds at least 55
 // significant bits (the remainder is the sticky bit); then exactly the bits the result can hold are kept -- 53, or fewer
 // where the result is subnormal -- and rounded once.
-PB200_MHD double round_dyadic(bool neg, u128 num, unsigned long long den, int scale) {
+PB200_HD double round_dyadic(bool neg, u128 num, unsigned long long den, int scale) {
   u128 q = 0, r = 0;
   for (int i = 127; i >= 0; --i) {
     r = (r << 1) | ((num >> i) & 1u);
@@ -104,10 +96,10 @@ PB200_MHD double round_dyadic(bool neg, u128 num, unsigned long long den, int sc
 }
 
 // the positive case (VAR / STDDEV)
-PB200_MHD double div_round(u128 num, unsigned long long den, int scale) { return round_dyadic(false, num, den, scale); }
+PB200_HD double div_round(u128 num, unsigned long long den, int scale) { return round_dyadic(false, num, den, scale); }
 
 // The final value of function fn (PB200_AGG_VARPOP .. STDDEVSAMP) over moments m of values on grid exponent e
-PB200_MHD double moments_final(int fn, const Moments& m, int e) {
+PB200_HD double moments_final(int fn, const Moments& m, int e) {
   const bool samp = fn == PB200_AGG_VARSAMP || fn == PB200_AGG_STDDEVSAMP;
   if (m.n == 0 || (samp && m.n == 1)) return -(double)INFINITY;
   const u128 N = (u128)m.n * m.s2 - (u128)m.s1 * m.s1;

@@ -122,6 +122,12 @@ struct ScanPlanner {
     set_error("%s over column %d: no dictIds in segment %d (raw values): not accelerated", what, col, t);
     return PB200_E_UNSUPPORTED;
   }
+  // the first aggregation before a over a's column that `shares` accepts (an earlier one whose state a shares), else -1
+  template <class Shares> int first_sharing(int a, Shares shares) const {
+    for (int b = 0; b < a; b++)
+      if (plan.aggs[b].column == plan.aggs[a].column && shares(b)) return b;
+    return -1;
+  }
   // ---- VAR / STDDEV: each column's moments are three internal INT-dictionary SUMs over its limb dictionaries
   //      (pb200_moments.h), appended behind the caller's aggregations; functions of one column share them ----
   int expand_moments() {
@@ -142,9 +148,8 @@ struct ScanPlanner {
           return PB200_E_UNSUPPORTED;
         }
       }
-      for (int b = 0; b < a && plan.mom_first[a] < 0; b++)
-        if (plan.mom_first[b] >= 0 && query->aggs[b].column == ag.column) plan.mom_first[a] = plan.mom_first[b];
-      if (plan.mom_first[a] >= 0) continue;
+      const int b = first_sharing(a, [&](int e) { return plan.mom_first[e] >= 0; });
+      if (b >= 0) { plan.mom_first[a] = plan.mom_first[b]; continue; }
       plan.mom_first[a] = (int)plan.aggs.size();
       for (int j = 0; j < 3; j++) plan.aggs.push_back(pb200_agg{PB200_AGG_SUM, ag.column});
     }
@@ -171,7 +176,7 @@ struct ScanPlanner {
   // FIRST/LASTWITHTIME: the time column t (INT / LONG with dictIds), the data column v (dictIds) and the type literal
   int check_withtime(int a, const pb200_agg_arg* wt_args) {
     const pb200_agg& ag = plan.aggs[a];
-    const char* name = ag.function == PB200_AGG_FIRSTWITHTIME ? "FIRSTWITHTIME" : "LASTWITHTIME";
+    const char* name = agg_fn(ag.function)->name;
     if (!wt_args) { set_error("unknown aggregation function %d without arguments: %s (aggregation %d) takes its time column through pb200_execute_agg_args", ag.function, name, a); return PB200_E_INVALID; }
     const int tc = wt_args[a].time_column;
     if (tc < 0 || tc >= ncols) { set_error("%s (aggregation %d): time column %d out of range", name, a, tc); return PB200_E_INVALID; }
@@ -199,7 +204,7 @@ struct ScanPlanner {
   // every segment (evaluated once per device dictionary and cached with it), and the bitset it reads
   int check_distinct_value(int a) {
     const pb200_agg& ag = plan.aggs[a];
-    const char* name = ag.function == PB200_AGG_DISTINCTSUM ? "DISTINCTSUM" : "DISTINCTAVG";
+    const char* name = agg_fn(ag.function)->name;
     for (int t = 0; t < nseg; t++) {
       DeviceColumn& c = segments[t]->cols[ag.column];
       if (c.stored_type == PB200_STRING) { set_error("%s over STRING column %d", name, ag.column); return PB200_E_UNSUPPORTED; }
@@ -226,24 +231,15 @@ struct ScanPlanner {
   // a function that reads a DISTINCTCOUNT set (reads_distinct_set): the bitset of an earlier DISTINCTCOUNT or reader of
   // the same column, else its own
   void share_distinct_set(int a) {
-    const pb200_agg& ag = plan.aggs[a];
-    plan.ds_rep[a] = a;
-    for (int b = 0; b < a; b++) {
-      const int fb = plan.aggs[b].function;
-      if (plan.aggs[b].column != ag.column || (fb != PB200_AGG_DISTINCTCOUNT && !reads_distinct_set(fb))) continue;
-      plan.ds_rep[a] = fb == PB200_AGG_DISTINCTCOUNT ? b : plan.ds_rep[b];
-      break;
-    }
+    const int b = first_sharing(a, [&](int e) { const int fb = plan.aggs[e].function; return fb == PB200_AGG_DISTINCTCOUNT || reads_distinct_set(fb); });
+    plan.ds_rep[a] = b < 0 ? a : plan.aggs[b].function == PB200_AGG_DISTINCTCOUNT ? b : plan.ds_rep[b];
   }
-  // DISTINCTCOUNTHLL: log2m from the aggregation's argument (none or 0: the default 8; the reference accepts 0..30, the
-  // registers fit the finalize's shared memory up to 12), a column with dictIds in every segment (STRING too: its UTF-8
-  // bytes are hashed), and the bitset it reads.  HLLs of one column and log2m share one estimate (hll_rep).
+  // DISTINCTCOUNTHLL: log2m from the aggregation's argument (hll_log2m), a column with dictIds in every segment (STRING
+  // too: its UTF-8 bytes are hashed), and the bitset it reads.  HLLs of one column and log2m share one estimate (hll_rep).
   int check_hll(int a, const double* agg_args) {
     const pb200_agg& ag = plan.aggs[a];
-    const double lv = agg_args ? agg_args[a] : 0.0;
-    if (!(lv >= 0.0 && lv <= 30.0) || lv != (double)(int)lv) { set_error("DISTINCTCOUNTHLL (aggregation %d): log2m %g is not an integer in 0..30", a, lv); return PB200_E_INVALID; }
-    const int p = lv == 0.0 ? kHllDefaultLog2m : (int)lv;
-    if (p < kHllMinLog2m || p > kHllMaxLog2m) { set_error("DISTINCTCOUNTHLL (aggregation %d): log2m %d outside %d..%d is not accelerated", a, p, kHllMinLog2m, kHllMaxLog2m); return PB200_E_UNSUPPORTED; }
+    int p = 0;
+    if (int rc = hll_log2m(agg_args ? agg_args[a] : 0.0, a, &p)) return rc;
     for (int t = 0; t < nseg; t++) {
       const DeviceColumn& c = segments[t]->cols[ag.column];
       if (c.bits > 31 || c.cardinality <= 0 || (c.stored_type != PB200_STRING && !c.dict_native)) {
@@ -252,9 +248,8 @@ struct ScanPlanner {
       }
     }
     plan.hll_log2m[a] = p;
-    plan.hll_rep[a] = a;
-    for (int b = 0; b < a; b++)
-      if (is_hll_fn(plan.aggs[b].function) && plan.aggs[b].column == ag.column && plan.hll_log2m[b] == p) { plan.hll_rep[a] = b; break; }
+    const int b = first_sharing(a, [&](int e) { return is_hll_fn(plan.aggs[e].function) && plan.hll_log2m[e] == p; });
+    plan.hll_rep[a] = b >= 0 ? b : a;
     share_distinct_set(a);
     return PB200_OK;
   }
@@ -289,7 +284,7 @@ struct ScanPlanner {
       const pb200_agg& ag = plan.aggs[a];
       q.aggs[a] = AggDesc{ag.function, -1, VAL_NONE, 0};
       if (ag.function == PB200_AGG_COUNT || is_moments_fn(ag.function)) continue;   // VAR / STDDEV: read their limb sums
-      if (ag.function < 0 || (ag.function > PB200_AGG_PERCENTILE && !is_withtime_fn(ag.function) && !reads_distinct_set(ag.function))) { set_error("unknown aggregation function %d", ag.function); return PB200_E_INVALID; }
+      if (!agg_fn(ag.function)) { set_error("unknown aggregation function %d", ag.function); return PB200_E_INVALID; }
       if (ag.column < 0 || ag.column >= ncols) { set_error("aggregation column %d out of range", ag.column); return PB200_E_INVALID; }
       if (reads_distinct_set(ag.function)) {
         if (int rc = is_hll_fn(ag.function) ? check_hll(a, agg_args) : check_distinct_value(a)) return rc;
@@ -304,20 +299,20 @@ struct ScanPlanner {
         continue;
       }
       if (ag.function == PB200_AGG_PERCENTILE) {
-        // the percentile travels beside the query (pb200_execute_args); PercentileAggregationFunction takes 0 <= p <= 100
+        // the percentile travels beside the query (pb200_execute_args)
         if (!agg_args) {   // pb200_execute / pb200_execute_ordered carry no percentile
           set_error("unknown aggregation function %d without arguments: PERCENTILE (aggregation %d) takes its percentile through pb200_execute_args", ag.function, a);
           return PB200_E_INVALID;
         }
         const double pv = agg_args[a];
-        if (!(pv >= 0.0 && pv <= 100.0)) { set_error("PERCENTILE (aggregation %d): percentile %g outside [0, 100]", a, pv); return PB200_E_INVALID; }
+        if (int rc = check_percentile(pv, a)) return rc;
         if (plan.defer_finalize) { set_error("PERCENTILE histograms are not reducible across GPUs (PB200_Q_DEFER_FINALIZE)"); return PB200_E_UNSUPPORTED; }
         for (int t = 0; t < nseg; t++)
           if (int rc = require_dict_ids(t, ag.column, "PERCENTILE")) return rc;
         plan.pct_p[a] = pv;
-        plan.pct_rep[a] = a;
-        for (int b = 0; b < a; b++)   // PERCENTILEs of one column share the first one's histogram
-          if (plan.aggs[b].function == PB200_AGG_PERCENTILE && plan.aggs[b].column == ag.column) { plan.pct_rep[a] = b; break; }
+        // PERCENTILEs of one column share the first one's histogram
+        const int b = first_sharing(a, [&](int e) { return plan.aggs[e].function == PB200_AGG_PERCENTILE; });
+        plan.pct_rep[a] = b >= 0 ? b : a;
       }
       if ((q.aggs[a].slot = slot_of(plan, ag.column, ROLE_AGG)) < 0) return PB200_E_UNSUPPORTED;
       const DeviceColumn& c0 = segments[0]->cols[ag.column];
@@ -865,9 +860,7 @@ struct ScanPlanner {
         const DeviceColumn& c = seg->cols[plan.aggs[a].column];
         const unsigned long long words = ((unsigned long long)c.cardinality + 31) / 32;
         if (words * (unsigned long long)t.groups > (1ull << 28)) {
-          set_error("%s with GROUP BY: %lld groups x %d dictIds exceed the device bitset budget",
-                    fn == PB200_AGG_DISTINCTCOUNT ? "DISTINCTCOUNT" : fn == PB200_AGG_DISTINCTSUM ? "DISTINCTSUM"
-                    : fn == PB200_AGG_DISTINCTAVG ? "DISTINCTAVG" : "DISTINCTCOUNTHLL", t.groups, c.cardinality);
+          set_error("%s with GROUP BY: %lld groups x %d dictIds exceed the device bitset budget", agg_fn(fn)->name, t.groups, c.cardinality);
           return PB200_E_UNSUPPORTED;
         }
         t.dwords[a] = (uint32_t)words;
@@ -931,6 +924,20 @@ struct ScanPlanner {
 
 }  // namespace
 
+int check_percentile(double p, int a) {
+  if (p >= 0.0 && p <= 100.0) return PB200_OK;
+  set_error("PERCENTILE (aggregation %d): percentile %g outside [0, 100]", a, p);
+  return PB200_E_INVALID;
+}
+
+int hll_log2m(double arg, int a, int* log2m) {
+  if (!(arg >= 0.0 && arg <= 30.0) || arg != (double)(int)arg) { set_error("DISTINCTCOUNTHLL (aggregation %d): log2m %g is not an integer in 0..30", a, arg); return PB200_E_INVALID; }
+  const int p = arg == 0.0 ? kHllDefaultLog2m : (int)arg;
+  if (p < kHllMinLog2m || p > kHllMaxLog2m) { set_error("DISTINCTCOUNTHLL (aggregation %d): log2m %d outside %d..%d is not accelerated", a, p, kHllMinLog2m, kHllMaxLog2m); return PB200_E_UNSUPPORTED; }
+  *log2m = p;
+  return PB200_OK;
+}
+
 int plan_scan(const Tuning& tune, DeviceLimits lim, const pb200_query* query, pb200_segment* const* segments, int nseg,
               bool allow_count_carrier, ScanPlan* out, const double* agg_args, const pb200_agg_arg* wt_args) {
   if (!query || !segments || !out || nseg <= 0) { set_error("invalid argument to pb200_execute"); return PB200_E_INVALID; }
@@ -952,14 +959,11 @@ int plan_scan(const Tuning& tune, DeviceLimits lim, const pb200_query* query, pb
     }
     for (int a = 0; a < nuser; a++) {
       const pb200_agg& ag = query->aggs[a];
-      if (ag.function != PB200_AGG_MIN && ag.function != PB200_AGG_MAX && ag.function != PB200_AGG_DISTINCTCOUNT &&
-          ag.function != PB200_AGG_PERCENTILE && !is_moments_fn(ag.function) && !reads_distinct_set(ag.function)) continue;
+      const AggFn* d = agg_fn(ag.function);
+      if (!d || !d->dict_ids) continue;
       if (ag.column < 0 || ag.column >= ncols) continue;
       if (segments[0]->cols[ag.column].bits == 32 && !segments[0]->cols[ag.column].dict_native) continue;  // raw values, no ids
-      const char* what = ag.function == PB200_AGG_DISTINCTCOUNT ? "DISTINCTCOUNT" : ag.function == PB200_AGG_PERCENTILE ? "PERCENTILE"
-                         : is_moments_fn(ag.function) ? "VAR/STDDEV" : is_distinct_value_fn(ag.function) ? "DISTINCTSUM/DISTINCTAVG"
-                         : is_hll_fn(ag.function) ? "DISTINCTCOUNTHLL" : "MIN/MAX";
-      if (!same_dictionary(segments, nseg, ag.column, what)) return PB200_E_UNSUPPORTED;
+      if (!same_dictionary(segments, nseg, ag.column, d->family)) return PB200_E_UNSUPPORTED;
     }
     for (int a = 0; a < nuser && wt_args; a++) {   // FIRST/LASTWITHTIME: one dictionary for the data and the time column
       const pb200_agg& ag = query->aggs[a];

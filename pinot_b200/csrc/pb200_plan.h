@@ -117,7 +117,6 @@ constexpr int kHistWarpPrivateMaxCard = 64;
 // every entry point but pb200_execute_agg_args does).
 int plan_scan(const Tuning& tune, DeviceLimits lim, const pb200_query* query, pb200_segment* const* segments, int nseg,
               bool allow_count_carrier, ScanPlan* out, const double* agg_args = nullptr, const pb200_agg_arg* wt_args = nullptr);
-inline bool is_withtime_fn(int fn) { return fn == PB200_AGG_FIRSTWITHTIME || fn == PB200_AGG_LASTWITHTIME; }
 // aggregation a of the plan sets bits in a DISTINCTCOUNT bitset of its own: a DISTINCTCOUNT, or the owner of a set that
 // DISTINCTSUM / DISTINCTAVG / DISTINCTCOUNTHLL read
 inline bool owns_bitset(const ScanPlan& p, int a) {

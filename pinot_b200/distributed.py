@@ -33,10 +33,11 @@ from __future__ import annotations
 import ctypes as C
 from typing import Dict, List, Optional, Sequence
 
-from .query import DISTINCT_SET_FUNCTIONS, HllSet, distinct_final, hll_final, is_multi_column_expression, value_key
+from .query import (DISTINCT_SET_FUNCTIONS, MOMENT_FUNCTIONS, WITHTIME_FUNCTIONS, HllSet, distinct_final, functions_where, hll_final,
+                    is_multi_column_expression, value_key)
 
 # functions whose per-rank intermediate is a set of domain ids, united on the host
-_SET_FUNCTIONS = DISTINCT_SET_FUNCTIONS + ("DISTINCTCOUNTHLL",)
+_SET_FUNCTIONS = DISTINCT_SET_FUNCTIONS + functions_where(lambda f: f.family == "DISTINCTCOUNTHLL")
 
 
 KINDS = {"i64": 0, "f64": 1, "u32max": 2, "u32min": 3}
@@ -226,7 +227,7 @@ def execute_and_combine(plan_maker_or_backend, segments: Sequence, query, dist, 
         # extraction only on one GPU, the host merge would drop it): the caller filters the combined rows
         from ._lib import E_UNSUPPORTED, UnsupportedQueryError
         raise UnsupportedQueryError(E_UNSUPPORTED, "HAVING is not combined across GPUs")
-    if any(a.function in ("FIRSTWITHTIME", "LASTWITHTIME") for a in query.aggregations):
+    if any(a.function in WITHTIME_FUNCTIONS for a in query.aggregations):
         # the winning rows of different GPUs are compared by time value on the host: the caller merges per-GPU results
         from ._lib import E_UNSUPPORTED, UnsupportedQueryError
         raise UnsupportedQueryError(E_UNSUPPORTED, "FIRSTWITHTIME / LASTWITHTIME are not combined across GPUs")
@@ -234,7 +235,7 @@ def execute_and_combine(plan_maker_or_backend, segments: Sequence, query, dist, 
         # per-GPU histograms are not reduced across GPUs: the caller runs the query per GPU and merges by value
         from ._lib import E_UNSUPPORTED, UnsupportedQueryError
         raise UnsupportedQueryError(E_UNSUPPORTED, "PERCENTILE is not combined across GPUs")
-    if any(a.function in ("VARPOP", "VARSAMP", "STDDEVPOP", "STDDEVSAMP") for a in query.aggregations):
+    if any(a.function in MOMENT_FUNCTIONS for a in query.aggregations):
         # per-GPU moments are not reduced across GPUs: the caller runs the query per GPU and merges them by value
         from ._lib import E_UNSUPPORTED, UnsupportedQueryError
         raise UnsupportedQueryError(E_UNSUPPORTED, "VAR/STDDEV is not combined across GPUs")

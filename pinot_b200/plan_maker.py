@@ -25,7 +25,7 @@ import numpy as np
 
 from . import _lib
 from ._lib import UnsupportedQueryError  # noqa: F401  (re-export)
-from .query import DISTINCT_SET_FUNCTIONS, MOMENT_FUNCTIONS, WITHTIME_FUNCTIONS, WITHTIME_TYPES, Filter, Moments, QueryContext, postfix
+from .query import DISTINCT_SET_FUNCTIONS, MOMENT_FUNCTIONS, WITHTIME_FUNCTIONS, WITHTIME_TYPES, functions_where, Filter, Moments, QueryContext, postfix
 
 
 class B200Context:
@@ -812,7 +812,8 @@ class B200PlanMaker:
             if a.function == "DISTINCTCOUNTHLL" and a.arg == 0:   # the library reads an argument of 0 as the default 8
                 raise UnsupportedQueryError(_lib.E_UNSUPPORTED, "DISTINCTCOUNTHLL with log2m 0 is not accelerated")
         # one argument per aggregation: the percentile of a PERCENTILE, the log2m of a DISTINCTCOUNTHLL
-        pct = [a.function in ("PERCENTILE", "DISTINCTCOUNTHLL") for a in query.aggregations]
+        numeric = functions_where(lambda f: f.arg in ("percentile", "log2m"))
+        pct = [a.function in numeric for a in query.aggregations]
         if any(a.function in WITHTIME_FUNCTIONS for a in query.aggregations):
             # FIRST/LASTWITHTIME: the time column and the type literal travel beside the query (pb200h_execute_agg_args)
             args = (_lib.HAggArg * len(pct))(*[

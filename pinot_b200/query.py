@@ -47,6 +47,46 @@ class Filter:
 FilterNode = Union[Filter, Predicate]
 
 
+@dataclass(frozen=True)
+class AggFunction:
+    family: str       # as a refusal shared by the family names it ("VAR/STDDEV", "MIN/MAX", ...)
+    arg: Optional[str]  # the argument besides the column: None, "percentile", "log2m" or "time" (the time column)
+    dict_ids: bool    # reads its column's dictIds: a merged submission needs one dictionary for that column
+
+
+# What each aggregation function is, in PB200_AGG_* code order (_lib.AGG_CODES): the package's half of
+# pinot_b200/csrc/pb200_aggfn.h.  FIRST/LASTWITHTIME's data column is bound with its time column, not through dict_ids.
+AGG_FUNCTIONS = {
+    "COUNT": AggFunction("COUNT", None, False),
+    "SUM": AggFunction("SUM/AVG", None, False),
+    "MIN": AggFunction("MIN/MAX", None, True),
+    "MAX": AggFunction("MIN/MAX", None, True),
+    "AVG": AggFunction("SUM/AVG", None, False),
+    "DISTINCTCOUNT": AggFunction("DISTINCTCOUNT", None, True),
+    "PERCENTILE": AggFunction("PERCENTILE", "percentile", True),
+    "VARPOP": AggFunction("VAR/STDDEV", None, True),
+    "VARSAMP": AggFunction("VAR/STDDEV", None, True),
+    "STDDEVPOP": AggFunction("VAR/STDDEV", None, True),
+    "STDDEVSAMP": AggFunction("VAR/STDDEV", None, True),
+    "FIRSTWITHTIME": AggFunction("FIRST/LASTWITHTIME", "time", False),
+    "LASTWITHTIME": AggFunction("FIRST/LASTWITHTIME", "time", False),
+    "DISTINCTSUM": AggFunction("DISTINCTSUM/DISTINCTAVG", None, True),
+    "DISTINCTAVG": AggFunction("DISTINCTSUM/DISTINCTAVG", None, True),
+    "DISTINCTCOUNTHLL": AggFunction("DISTINCTCOUNTHLL", "log2m", True),
+}
+
+
+def functions_where(test) -> tuple:
+    """The names of the functions whose AggFunction passes `test`, in code order."""
+    return tuple(name for name, f in AGG_FUNCTIONS.items() if test(f))
+
+
+WITHTIME_FUNCTIONS = functions_where(lambda f: f.arg == "time")
+MOMENT_FUNCTIONS = functions_where(lambda f: f.family == "VAR/STDDEV")
+# functions whose intermediate is the set of distinct values (merged by union)
+DISTINCT_SET_FUNCTIONS = functions_where(lambda f: f.family in ("DISTINCTCOUNT", "DISTINCTSUM/DISTINCTAVG"))
+
+
 @dataclass
 class Aggregation:
     function: str  # COUNT | SUM | MIN | MAX | AVG | DISTINCTCOUNT | PERCENTILE | VARPOP | VARSAMP | STDDEVPOP | STDDEVSAMP
@@ -72,7 +112,6 @@ class Aggregation:
         return f"{self.function.lower()}({self.column or '*'})"
 
 
-WITHTIME_FUNCTIONS = ("FIRSTWITHTIME", "LASTWITHTIME")
 # the type literal of FIRST/LASTWITHTIME -> the stored type it names (BOOLEAN is stored as INT)
 WITHTIME_TYPES = {"INT": 0, "BOOLEAN": 0, "LONG": 1, "FLOAT": 2, "DOUBLE": 3, "STRING": 4}
 
@@ -141,10 +180,6 @@ def percentile_of_counts(counts) -> float:
         if k < 0:
             return float(v)
     raise AssertionError("unreachable")
-
-
-# functions whose intermediate is the set of distinct values (merged by union)
-DISTINCT_SET_FUNCTIONS = ("DISTINCTCOUNT", "DISTINCTSUM", "DISTINCTAVG")
 
 
 def distinct_final(function: str, values) -> float:
@@ -264,9 +299,6 @@ def hll_final(values, log2m: int = HLL_DEFAULT_LOG2M, data_type: Optional[str] =
         estimate = m * math.log(m / zeros)
     f = math.floor(estimate)
     return f + (1 if estimate - f >= 0.5 else 0)
-
-
-MOMENT_FUNCTIONS = ("VARPOP", "VARSAMP", "STDDEVPOP", "STDDEVSAMP")
 
 
 @dataclass(frozen=True)

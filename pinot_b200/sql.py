@@ -45,15 +45,14 @@ import re
 from dataclasses import dataclass, field
 from typing import List, Optional
 
-from .query import HLL_DEFAULT_LOG2M, WITHTIME_FUNCTIONS, WITHTIME_TYPES, Aggregation, Filter, FilterNode, Predicate, QueryContext, flatten, optimize_filter
+from .query import AGG_FUNCTIONS, HLL_DEFAULT_LOG2M, WITHTIME_FUNCTIONS, WITHTIME_TYPES, Aggregation, Filter, FilterNode, Predicate, QueryContext, flatten, optimize_filter
 
 _TOKEN = re.compile(r"\s*(?:(\d+\.\d+(?:[eE][-+]?\d+)?|-?\d+\.\d+|-?\d+)|'((?:[^']|'')*)'|(<=|>=|<>|!=|[=<>(),*+/%-])|"
                     r"([A-Za-z_$][A-Za-z0-9_$]*))")
 
 # VarianceAggregationFunction: both spellings of each function, the underscore one canonicalised to the other
 _ALIASES = {"VAR_POP": "VARPOP", "VAR_SAMP": "VARSAMP", "STDDEV_POP": "STDDEVPOP", "STDDEV_SAMP": "STDDEVSAMP"}
-_FUNCTIONS = {"COUNT", "SUM", "MIN", "MAX", "AVG", "DISTINCTCOUNT", "DISTINCTSUM", "DISTINCTAVG", "DISTINCTCOUNTHLL", "PERCENTILE", "VARPOP",
-              "VARSAMP", "STDDEVPOP", "STDDEVSAMP", *WITHTIME_FUNCTIONS} | set(_ALIASES)
+_FUNCTIONS = set(AGG_FUNCTIONS) | set(_ALIASES)
 # FN(DISTINCT col): the function Pinot's query compiler rewrites it into
 _DISTINCT_OF = {"COUNT": "DISTINCTCOUNT", "SUM": "DISTINCTSUM", "AVG": "DISTINCTAVG"}
 _PERCENTILE_N = re.compile(r"PERCENTILE(\d+)")

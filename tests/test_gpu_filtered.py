@@ -2,13 +2,15 @@
 device submission per distinct clause over main AND clause, aligned by group key) against the oracle's restatement of
 AggregationFunctionUtils.buildFilteredAggregationInfos / FilteredGroupByOperator (tests/test_oracle_filtered.py pins that
 restatement on the reference's own FilteredAggregationsTest queries)."""
+import re
+
 import numpy as np
 import pytest
 
 from exact_ref import check_exact
 from gpu_util import assert_tables_equal, check_query, gpu_table, oracle_table, to_device
 from pinot_b200 import sql
-from pinot_b200.plan_maker import B200Context, B200PlanMaker
+from pinot_b200.plan_maker import B200Context, B200PlanMaker, UnsupportedQueryError
 
 pytestmark = pytest.mark.gpu
 
@@ -109,5 +111,27 @@ def test_filtered_result_as_datatable(oracle, ctx, pm):
         got = {(row[0],): [float(row[1]), int(row[2])] for row in table["rows"]}
         assert got == {k: [float(v[0]), int(v[1])] for k, v in want.items()}
         block.release(ctx)
+    finally:
+        dev.destroy()
+
+
+def test_refusal_does_not_depend_on_function_order(oracle, ctx, pm):
+    """A query with several functions that do not run next to FILTER clauses, or have no DataTable type, is refused for
+    the same one whichever comes first in the query."""
+    seg = _segment(oracle, 4096, 5)
+    dev = to_device(ctx, seg)
+    try:
+        for fns, family in ((["VARPOP(v)", "PERCENTILE(v, 50)"], "PERCENTILE"),
+                            (["DISTINCTCOUNTHLL(k)", "DISTINCTSUM(v)", "STDDEVSAMP(f)"], "VAR/STDDEV")):
+            for order in (fns, fns[::-1]):
+                q = sql.parse(f"SELECT {', '.join(order)}, COUNT(*) FILTER(WHERE j = 1) FROM t")
+                with pytest.raises(UnsupportedQueryError, match=re.escape(f"{family} in a query with FILTER (WHERE ...) clauses")):
+                    pm.execute_segments([dev], q)
+        for order in (["VARPOP(v)", "DISTINCTCOUNTHLL(k)"], ["DISTINCTCOUNTHLL(k)", "VARPOP(v)"]):
+            q = sql.parse(f"SELECT {', '.join(order)} FROM t")
+            block = pm.execute_segments([dev], q, keep_handle=True, defer=False)[0]
+            with pytest.raises(UnsupportedQueryError, match="DISTINCTCOUNTHLL is not written as a server DataTable"):
+                pm.to_datatable(dev, q, block)
+            block.release(ctx)
     finally:
         dev.destroy()
