@@ -8,6 +8,7 @@
 #include <chrono>
 
 #include <algorithm>
+#include <array>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
@@ -16,6 +17,7 @@
 #include <memory>
 #include <optional>
 
+#include "pb200_decode.h"
 #include "pb200_internal.h"
 #include "pb200_expr.h"
 #include "pb200_percentile.h"
@@ -821,38 +823,31 @@ namespace {
 // The accumulator block of one call: on the device, and in each half of a pooled pinned block (initial values go up and
 // results come back through it, both asynchronously on the call's stream: a pageable cudaMemcpy would synchronise the
 // device twice per query).  nres AggAccum records, then 4 words per result for the count-carrier verification {sum of
-// carried counts, largest sum field, largest carried count, unused}, then (aggregation-only PERCENTILE) per result
-// kMaxAggs selected dictIds and kMaxAggs value counts, u32 each.
-// Then (aggregation-only FIRST/LASTWITHTIME) per result kMaxAggs winning keys and kMaxAggs time values, u64 each, and
-// kMaxAggs data dictIds, u32 each.
-// Then (aggregation-only DISTINCTSUM / DISTINCTAVG) per result and aggregation the finalized state, kDsWords u64 each.
-// Then (aggregation-only expression aggregations, pb200_expr.cu) per result and aggregation one u64: the f64 sum, or the
-// Double.compare key of a MIN / MAX.
-// Then (aggregation-only DISTINCTCOUNTHLL) per result and aggregation the estimate, int64 (slot of ScanPlan::hll_rep).
+// carried counts, largest sum field, largest carried count, unused}, then per result kMaxAggs OneEntry records.
+// Aggregation only, AggAccum's fields and the OneEntry records are the result's one-entry tables: the scan and the
+// finalize stages write them like a GROUP BY result's tables, and one decoder (pb200_decode.h) reads both.
+struct OneEntry {
+  unsigned long long wt_key;         // FIRST/LASTWITHTIME: the scan's winning key...
+  long long wt_time;                 // ... and the finalize's time value ...
+  unsigned long long ds[kDsWords];   // DISTINCTSUM / DISTINCTAVG: the set's finalized state (record of ScanPlan::ds_rep)
+  unsigned long long xkey;           // expression aggregations (pb200_expr.cu): the f64 sum, or a MIN / MAX Double.compare key
+  long long hll;                     // DISTINCTCOUNTHLL: the estimate (record of ScanPlan::hll_rep)
+  uint32_t pct_id, pct_n;            // PERCENTILE: the selected dictId; values (record of the histogram's owner)
+  uint32_t wt_id;                    // FIRST/LASTWITHTIME: ... and data dictId
+};
 struct AccumLayout {
-  size_t verify_off = 0, pct_off = 0, wt_off = 0, ds_off = 0, ex_off = 0, hll_off = 0, bytes = 0;
-  int nres = 0;
+  size_t verify_off = 0, one_off = 0, bytes = 0;
   AccumLayout() = default;
-  AccumLayout(int nres, bool pct, bool wt, bool ds, bool ex, bool hll)
-      : verify_off(sizeof(AggAccum) * nres), pct_off(verify_off + 32ull * nres), wt_off(pct_off + (pct ? 8ull * kMaxAggs * nres : 0)),
-        ds_off(wt_off + (wt ? 20ull * kMaxAggs * nres : 0)), ex_off(ds_off + (ds ? 8ull * kDsWords * kMaxAggs * nres : 0)),
-        hll_off(ex_off + (ex ? 8ull * kMaxAggs * nres : 0)), bytes(hll_off + (hll ? 8ull * kMaxAggs * nres : 0)), nres(nres) {}
-  long long* hll(void* b, int r) const {
-    return reinterpret_cast<long long*>(static_cast<unsigned char*>(b) + hll_off) + (size_t)r * kMaxAggs;
-  }
-  unsigned long long* ex(void* b, int r) const {
-    return reinterpret_cast<unsigned long long*>(static_cast<unsigned char*>(b) + ex_off) + (size_t)r * kMaxAggs;
-  }
-  unsigned long long* ds(void* b, int r, int a) const {
-    return reinterpret_cast<unsigned long long*>(static_cast<unsigned char*>(b) + ds_off) + ((size_t)r * kMaxAggs + a) * kDsWords;
-  }
+  explicit AccumLayout(int nres)
+      : verify_off(sizeof(AggAccum) * nres), one_off(verify_off + 32ull * nres), bytes(one_off + sizeof(OneEntry) * kMaxAggs * nres) {}
   static AggAccum* records(void* b) { return static_cast<AggAccum*>(b); }
   unsigned long long* verify(void* b) const { return reinterpret_cast<unsigned long long*>(static_cast<unsigned char*>(b) + verify_off); }
-  uint32_t* pct(void* b) const { return reinterpret_cast<uint32_t*>(static_cast<unsigned char*>(b) + pct_off); }
-  unsigned long long* wt_key(void* b, int r) const { return reinterpret_cast<unsigned long long*>(static_cast<unsigned char*>(b) + wt_off) + (size_t)r * kMaxAggs; }
-  long long* wt_time(void* b, int r) const { return reinterpret_cast<long long*>(wt_key(b, nres)) + (size_t)r * kMaxAggs; }
-  uint32_t* wt_ids(void* b, int r) const { return reinterpret_cast<uint32_t*>(wt_time(b, nres)) + (size_t)r * kMaxAggs; }
+  OneEntry* one(void* b, int r) const { return reinterpret_cast<OneEntry*>(static_cast<unsigned char*>(b) + one_off) + (size_t)r * kMaxAggs; }
 };
+
+// The byte every entry of fn's u32 / u64 tables starts at: the min reductions (MIN, FIRSTWITHTIME keys, expression MIN
+// keys) at all ones, the rest at zero.
+int start_byte(int fn) { return fn == PB200_AGG_MIN || fn == PB200_AGG_FIRSTWITHTIME ? 0xFF : 0; }
 
 // Frees a result's group tables and PERCENTILE selections; its histograms too unless keep_hist (pb200_result_histogram).
 void release_tables(pb200_result& R, bool keep_hist) {
@@ -939,20 +934,31 @@ struct ScanCall {
       res.emplace_back(new pb200_result());
       res.back()->pct.ctx = ctx;
       for (int a = 0; a < plan.q.num_aggs; a++) res.back()->pct.rep[a] = plan.pct_rep[a];
+      describe_aggs(r);
     }
     return bind_leaf_buffers(ctx, plan, st, temps);
+  }
+  // result r's aggregations, on both routes: functions, value kinds, columns and shared states.  An expression
+  // aggregation is the function the caller asked for over a DOUBLE value (the scan runs it as COUNT(*)).
+  void describe_aggs(int r) {
+    const pb200_segment* seg = segments[plan.merge ? 0 : r];
+    pb200_result::Dense& d = res[r]->dense;
+    for (int a = 0; a < plan.num_user_aggs; a++) {
+      d.aggs.push_back(query->aggs[a]);
+      d.val_kind.push_back(plan.q.aggs[a].val_kind);
+      if (expr_fn(a) >= 0) { d.aggs[a].function = expr_fn(a); d.val_kind[a] = VAL_DICT_F64; }
+      d.agg_cols.push_back(plan.q.aggs[a].slot < 0 ? nullptr : &seg->cols[query->aggs[a].column]);
+      d.mom_first[a] = plan.mom_first[a];
+      if (plan.mom_first[a] >= 0) d.mom_e[a] = seg->cols[query->aggs[a].column].moments->grid.e;
+      d.ds_rep[a] = plan.ds_rep[a];
+      d.hll_log2m[a] = plan.hll_log2m[a];
+      d.hll_rep[a] = plan.hll_rep[a];
+    }
   }
 
   // 4. the accumulator block, initialised with one copy from the pinned block's first half
   int bind_accumulators() {
-    bool any_pct = false;
-    for (int a = 0; a < plan.q.num_aggs; a++) any_pct |= plan.pct_rep[a] >= 0;
-    bool any_ds = false;
-    for (int a = 0; a < plan.q.num_aggs; a++) any_ds |= is_distinct_value_fn(plan.q.aggs[a].function);
-    bool any_hll = false;
-    for (int a = 0; a < plan.q.num_aggs; a++) any_hll |= plan.hll_rep[a] >= 0;
-    acc = AccumLayout(plan.nres, any_pct && !plan.group_by, plan.any_wt && !plan.group_by, any_ds && !plan.group_by, ex && !plan.group_by,
-                      any_hll && !plan.group_by);
+    acc = AccumLayout(plan.nres);
     if (int rc = pinned_alloc(ctx, 2 * acc.bytes, &pin.p, &pin.bytes)) return rc;
     unsigned char* const init = static_cast<unsigned char*>(pin.p);
     back = init + acc.bytes;
@@ -960,15 +966,15 @@ struct ScanCall {
     memset(&init_acc, 0, sizeof init_acc);
     for (int a = 0; a < kMaxAggs; a++) init_acc.min_id[a] = 0xFFFFFFFFu;
     memset(init, 0, acc.bytes);
-    for (int r = 0; r < plan.nres; r++) AccumLayout::records(init)[r] = init_acc;
-    if (plan.any_wt && !plan.group_by)   // FIRSTWITHTIME keys start at u64 max (a u64 min reduction), LASTWITHTIME at 0
-      for (int r = 0; r < plan.nres; r++)
-        for (int a = 0; a < plan.q.num_aggs; a++)
-          if (plan.q.aggs[a].function == PB200_AGG_FIRSTWITHTIME) acc.wt_key(init, r)[a] = ~0ull;
-    if (ex && !plan.group_by)   // expression MIN keys start at u64 max, MAX keys at 0, sums at +0.0
-      for (int r = 0; r < plan.nres; r++)
-        for (int a = 0; a < plan.q.num_aggs; a++)
-          if (expr_fn(a) == PB200_AGG_MIN) acc.ex(init, r)[a] = kExprMinEmpty;
+    for (int r = 0; r < plan.nres; r++) {
+      AccumLayout::records(init)[r] = init_acc;
+      for (int a = 0; a < plan.num_user_aggs; a++) {
+        OneEntry& o = acc.one(init, r)[a];
+        const int fn = expr_fn(a) >= 0 ? expr_fn(a) : plan.q.aggs[a].function;
+        memset(&o.wt_key, start_byte(fn), 8);
+        memset(&o.xkey, start_byte(fn), 8);
+      }
+    }
     if (int rc = accum.alloc(acc.bytes)) return rc;
     PB200_CUDA(cudaMemcpyAsync(accum.p, init, acc.bytes, cudaMemcpyHostToDevice, st));
     for (int s = 0; s < nseg; s++) plan.segs[s].accum = AccumLayout::records(accum.p) + (plan.merge ? 0 : s);
@@ -1004,7 +1010,7 @@ struct ScanCall {
       for (int a = 0; a < nagg; a++) {
         if (distinct_bufs[r][a]) plan.segs[s].distinct_bits[a] = (uint32_t*)distinct_bufs[r][a]->p;
         if (res[r]->pct.hist[a]) plan.segs[s].distinct_bits[a] = res[r]->pct.hist[a];
-        if (plan.wt_time[a] >= 0) plan.segs[s].distinct_bits[a] = reinterpret_cast<uint32_t*>(acc.wt_key(accum.p, r) + a);
+        if (plan.wt_time[a] >= 0) plan.segs[s].distinct_bits[a] = reinterpret_cast<uint32_t*>(&acc.one(accum.p, r)[a].wt_key);
       }
     }
     return PB200_OK;
@@ -1032,8 +1038,7 @@ struct ScanCall {
     }
     return PB200_OK;
   }
-  // expression aggregations: each one's table, and the result's view of the aggregation as the function the caller asked
-  // for over a DOUBLE value (the scan ran it as COUNT(*))
+  // expression aggregations: each one's table (the function the caller asked for over a DOUBLE value)
   int build_expr_tables(int r) {
     pb200_result::Dense& d = res[r]->dense;
     for (int a = 0; a < plan.num_user_aggs; a++) {
@@ -1041,15 +1046,12 @@ struct ScanCall {
       if (fn < 0) continue;
       const size_t bytes = (size_t)d.groups * 8;
       if (int rc = dev_alloc(ctx, bytes, &d.expr_tab[a])) return rc;
-      PB200_CUDA(cudaMemsetAsync(d.expr_tab[a], fn == PB200_AGG_MIN ? 0xFF : 0, bytes, st));
-      d.aggs[a].function = fn;
-      d.val_kind[a] = VAL_DICT_F64;
+      PB200_CUDA(cudaMemsetAsync(d.expr_tab[a], start_byte(fn), bytes, st));
       if (fn == PB200_AGG_SUM || fn == PB200_AGG_AVG) d.dsum[a] = static_cast<double*>(d.expr_tab[a]);
     }
     return PB200_OK;
   }
   int build_dense(int r) {
-    const pb200_segment* seg = segments[plan.merge ? 0 : r];
     const TableLayout& t = plan.tables[r];
     const QueryDesc& q = plan.q;
     pb200_result::Dense& d = res[r]->dense;
@@ -1060,17 +1062,6 @@ struct ScanCall {
     d.stride = t.stride;
     d.live = true;
     d.num_groups_limit = query->num_groups_limit;
-    for (int a = 0; a < plan.num_user_aggs; a++) {
-      d.aggs.push_back(query->aggs[a]);
-      d.val_kind.push_back(q.aggs[a].val_kind);
-      d.agg_cols.push_back(q.aggs[a].slot < 0 ? nullptr : &seg->cols[query->aggs[a].column]);
-      d.mom_first[a] = plan.mom_first[a];
-      if (plan.mom_first[a] >= 0) d.mom_e[a] = seg->cols[query->aggs[a].column].moments->grid.e;
-      d.ds_rep[a] = plan.ds_rep[a];
-      if (plan.ds_rep[a] >= 0) d.ds_e[plan.ds_rep[a]] = seg->cols[query->aggs[a].column].moments->ds_e;
-      d.hll_log2m[a] = plan.hll_log2m[a];
-      d.hll_rep[a] = plan.hll_rep[a];
-    }
     d.pack_agg = t.carrier.agg; d.pack_shift = t.carrier.shift; d.pack_vmin = t.carrier.vmin;
     d.reduce_world = t.reduce_world;
     d.flag_slot = t.flag_slot;
@@ -1124,7 +1115,7 @@ struct ScanCall {
         if ((rc = dev_alloc(ctx, (size_t)t.groups * 4, (void**)&p.ids[a]))) return rc;
       } else if (is_withtime_fn(fn)) {  // one key per group / slot: u64 min (FIRST) starts at ~0, u64 max (LAST) at 0
         pb200_result::Wt& w = res[r]->wt;
-        if ((rc = alloc_block((void**)&w.key[a], t.groups, 8, fn == PB200_AGG_FIRSTWITHTIME ? 0xFF : 0))) return rc;
+        if ((rc = alloc_block((void**)&w.key[a], t.groups, 8, start_byte(fn)))) return rc;
         if ((rc = dev_alloc(ctx, (size_t)t.groups * 4, (void**)&w.ids[a]))) return rc;
         if ((rc = dev_alloc(ctx, (size_t)t.groups * 8, (void**)&w.time[a]))) return rc;
       }
@@ -1138,31 +1129,65 @@ struct ScanCall {
   // 7. the descriptors and every chunk's scan, between the call's two events
   int launch() { return launch_chunks(ctx, st, plan, dsegs, ev, "scan kernel", nullptr, nullptr, &t_launch); }
 
-  // 8. PERCENTILE: histograms -> selected dictIds, queued behind the scan (aggregation only: into the accumulator block;
-  //    group-by: per table entry, read by the extraction)
+  // entries of result r's tables: its group table's, or the one of an aggregation-only result
+  long long entries(int r) const { return plan.group_by ? plan.tables[r].groups : 1; }
+
+  // result r's tables as the finalize stages write them and the decoder reads them: the result's own (group-by), or its
+  // one-entry tables in the accumulator block at `block`, the device block or its pinned copy (aggregation only; the
+  // host's dictionaries)
+  std::array<AggSource, kMaxAggs> sources(int r, unsigned char* block) const {
+    std::array<AggSource, kMaxAggs> out{};
+    const pb200_result& R = *res[r];
+    if (plan.group_by) { agg_sources(R, out.data()); return out; }
+    AggAccum& rec = AccumLayout::records(block)[r];
+    OneEntry* one = acc.one(block, r);
+    const pb200_result::Dense& d = R.dense;
+    for (int a = 0; a < (int)d.aggs.size(); a++) {
+      AggSource& s = out[a];
+      const int fn = s.fn = d.aggs[a].function, vk = s.vk = d.val_kind[a];
+      if (fn == PB200_AGG_SUM || fn == PB200_AGG_AVG)
+        s.src = expr_fn(a) >= 0 ? (void*)&one[a].xkey : sum_in_double(vk) ? (void*)&rec.dsum[a] : (void*)&rec.isum[a];
+      else if (expr_fn(a) >= 0) s.xkey = &one[a].xkey;
+      else if (fn == PB200_AGG_MIN) s.src = &rec.min_id[a];
+      else if (fn == PB200_AGG_MAX) s.src = &rec.max_id_plus1[a];
+      else if (fn == PB200_AGG_PERCENTILE) { s.src = &one[a].pct_id; s.pct_n = &one[plan.pct_rep[a]].pct_n; }
+      else if (is_withtime_fn(fn)) { s.src = &one[a].wt_id; s.wt_time = &one[a].wt_time; }
+      else if (is_moments_fn(fn)) {
+        for (int j = 0; j < 3; j++) s.mom[j] = &rec.isum[d.mom_first[a] + j];
+        s.mom_e = d.mom_e[a];
+      } else if (is_distinct_value_fn(fn)) s.ds = one[d.ds_rep[a]].ds;
+      else if (is_hll_fn(fn)) s.hll = &one[d.hll_rep[a]].hll;
+      const DeviceColumn* c = d.agg_cols[a];
+      s.dict = (c && vk != VAL_RAW_I32 && !c->dict_host.empty()) ? c->dict_host.data() : nullptr;   // unbiased
+      s.counted = true;   // the matched docs (AggAccum::count)
+    }
+    return out;
+  }
+
+  // 8. PERCENTILE: histograms -> selected dictIds, queued behind the scan
   int finalize_percentiles() {
-    uint32_t* const dev_pct = acc.pct(accum.p);
-    for (int r = 0; r < plan.nres; r++)
+    for (int r = 0; r < plan.nres; r++) {
+      const auto src = sources(r, static_cast<unsigned char*>(accum.p));
       for (int a = 0; a < plan.q.num_aggs; a++) {
         pb200_result::Pct& p = res[r]->pct;
         if (!p.hist[a]) continue;
         PercentileJob job;
         job.hist = p.hist[a];
         job.E = p.entries[a];
-        job.rows = plan.group_by ? plan.tables[r].groups : 1;
-        job.n_out = plan.group_by ? p.n[a] : dev_pct + (size_t)r * 2 * kMaxAggs + kMaxAggs + a;
+        job.rows = entries(r);
+        job.n_out = src[a].pct_n;
         for (int b = 0; b < plan.q.num_aggs; b++) {
           if (plan.pct_rep[b] != a) continue;
           job.p[job.np] = plan.pct_p[b];
-          job.ids[job.np++] = plan.group_by ? p.ids[b] : dev_pct + (size_t)r * 2 * kMaxAggs + b;
+          job.ids[job.np++] = static_cast<uint32_t*>(src[b].src);
         }
         if (int rc = percentile_finalize(ctx, st, job, temps)) return rc;
       }
+    }
     return PB200_OK;
   }
 
-  // 8b. FIRST/LASTWITHTIME: winning keys -> data dictIds and time values, queued behind the scan (aggregation only: in the
-  //     accumulator block; group-by: per table entry, read by the extraction)
+  // 8b. FIRST/LASTWITHTIME: the scan's winning keys -> data dictIds and time values, queued behind the scan
   int finalize_withtime() {
     if (!plan.any_wt) return PB200_OK;
     for (int a = 0; a < plan.q.num_aggs; a++) {
@@ -1170,65 +1195,41 @@ struct ScanCall {
       const WtSeg* wsegs = nullptr;
       if (int rc = withtime_segments(ctx, st, segments, nseg, query->aggs[a].column, plan.wt_time[a], plan.wt_base, temps, &wsegs)) return rc;
       for (int r = 0; r < plan.nres; r++) {
-        WithTimeJob job;
-        if (plan.group_by) {
-          const pb200_result::Wt& w = res[r]->wt;
-          job = WithTimeJob{w.key[a], plan.tables[r].groups, w.ids[a], w.time[a]};
-        } else {
-          job = WithTimeJob{acc.wt_key(accum.p, r) + a, 1, acc.wt_ids(accum.p, r) + a, acc.wt_time(accum.p, r) + a};
-        }
+        const AggSource s = sources(r, static_cast<unsigned char*>(accum.p))[a];
+        unsigned long long* key = plan.group_by ? res[r]->wt.key[a] : &acc.one(accum.p, r)[a].wt_key;
+        const WithTimeJob job{key, entries(r), static_cast<uint32_t*>(s.src), s.wt_time};
         if (int rc = withtime_finalize(ctx, st, job, wsegs, nseg)) return rc;
       }
     }
     return PB200_OK;
   }
 
-  // 8c. DISTINCTSUM / DISTINCTAVG, aggregation only: each result's set -> its state in the accumulator block (slot of the
-  //     aggregation b whose bitset holds it, once per set), queued behind the scan (group-by: the extraction finalizes)
-  int finalize_distinct_sums() {
+  // 8c. DISTINCTSUM / DISTINCTAVG states and DISTINCTCOUNTHLL estimates, aggregation only, queued behind the scan
+  //     (group-by: the extraction finalizes them)
+  int finalize_sets() {
     if (plan.group_by) return PB200_OK;
-    for (int r = 0; r < plan.nres; r++)
-      for (int a = 0; a < plan.q.num_aggs; a++) {
-        if (!is_distinct_value_fn(plan.q.aggs[a].function)) continue;   // a set DISTINCTSUM / DISTINCTAVG read
-        const int b = plan.ds_rep[a];
-        bool done = false;
-        for (int x = 0; x < a && !done; x++) done = is_distinct_value_fn(plan.q.aggs[x].function) && plan.ds_rep[x] == b;
-        if (done) continue;
-        const DeviceColumn& c = segments[plan.merge ? 0 : r]->cols[query->aggs[a].column];
-        const DistinctSumJob job{static_cast<const uint32_t*>(distinct_bufs[r][b]->p), plan.distinct_words[r][b], 1, true,
-                                 c.dict_native, c.stored_type, c.moments->ds_e, acc.ds(accum.p, r, b)};
-        if (int rc = distinct_sum_finalize(ctx, st, job, temps)) return rc;
-      }
+    for (int r = 0; r < plan.nres; r++) {
+      const uint32_t* bits[kMaxAggs] = {};
+      for (int b = 0; b < plan.num_user_aggs; b++) bits[b] = distinct_bufs[r][b] ? static_cast<const uint32_t*>(distinct_bufs[r][b]->p) : nullptr;
+      if (int rc = pb200::finalize_sets(ctx, st, res[r]->dense, bits, plan.distinct_words[r].data(), 1, true,
+                                        sources(r, static_cast<unsigned char*>(accum.p)).data(), temps))
+        return rc;
+    }
     return PB200_OK;
   }
 
-  // 8e. DISTINCTCOUNTHLL, aggregation only: each result's set -> the estimate in the accumulator block (slot of the
-  //     first HLL of the column and log2m), queued behind the scan (group-by: the extraction finalizes)
-  int finalize_hll() {
-    if (plan.group_by) return PB200_OK;
-    for (int r = 0; r < plan.nres; r++)
-      for (int a = 0; a < plan.q.num_aggs; a++) {
-        if (plan.hll_rep[a] != a) continue;
-        const int b = plan.ds_rep[a];
-        const DeviceColumn& c = segments[plan.merge ? 0 : r]->cols[query->aggs[a].column];
-        const HllJob job{static_cast<const uint32_t*>(distinct_bufs[r][b]->p), plan.distinct_words[r][b], 1, true,
-                         c.moments->hll_hash, plan.hll_log2m[a], acc.hll(accum.p, r) + a};
-        if (int rc = hll_finalize(ctx, st, job, temps)) return rc;
-      }
-    return PB200_OK;
-  }
-
-  // 8d. expression aggregations: the mask scan and the expression pass (pb200_expr.cu), queued behind the scan into the
-  //     expression tables (group-by) or the accumulator block (aggregation only)
+  // 8d. expression aggregations: the mask scan and the expression pass (pb200_expr.cu), queued behind the scan
   int finalize_exprs() {
     if (!ex) return PB200_OK;
     std::vector<ExprOut> outs(plan.nres);
-    for (int r = 0; r < plan.nres; r++)
+    for (int r = 0; r < plan.nres; r++) {
+      const auto src = sources(r, static_cast<unsigned char*>(accum.p));
       for (int a = 0; a < plan.num_user_aggs; a++) {
         if (expr_fn(a) < 0) continue;
-        outs[r].out[a] = plan.group_by ? res[r]->dense.expr_tab[a] : static_cast<void*>(acc.ex(accum.p, r) + a);
+        outs[r].out[a] = src[a].xkey ? static_cast<void*>(src[a].xkey) : src[a].src;
         outs[r].hkeys = res[r]->dense.hkeys;
       }
+    }
     return expr_launch(ctx, st, tune, query, segments, nseg, plan, *ex, outs, temps);
   }
 
@@ -1277,91 +1278,6 @@ struct ScanCall {
     return PB200_OK;
   }
 
-  // whether only DISTINCTCOUNTHLLs read the set held by aggregation b's bitset
-  bool hll_only_set(int r, int b) const {
-    if (!distinct_bufs[r][b]) return false;
-    std::vector<int> fns(plan.q.num_aggs);
-    for (int x = 0; x < plan.q.num_aggs; x++) fns[x] = plan.q.aggs[x].function;
-    return hll_only_set_of(fns.data(), plan.ds_rep.data(), plan.q.num_aggs, b);
-  }
-
-  // 10. aggregation only: aggregation a of result r's one row, {double, long, dictId}
-  struct AggValue { double d = 0; int64_t l = 0; int32_t id = -1; };
-  int agg_value(int r, int a, AggValue* v) {
-    pb200_result& R = *res[r];
-    const AggAccum& acc_r = AccumLayout::records(back)[r];
-    const uint32_t* host_pct = acc.pct(back) + (size_t)r * 2 * kMaxAggs;
-    const int fn = plan.q.aggs[a].function, vk = plan.q.aggs[a].val_kind;
-    const DeviceColumn* c = plan.q.aggs[a].slot < 0 ? nullptr : &segments[plan.merge ? 0 : r]->cols[query->aggs[a].column];
-    auto value_of = [&](uint32_t x) -> double {
-      if (vk == VAL_RAW_I32) return (double)(int32_t)(x ^ 0x80000000u);
-      const unsigned char* h = c->dict_host.data();
-      switch (vk) {
-        case VAL_DICT_I32: { int32_t y; memcpy(&y, h + 4ull * x, 4); return (double)y; }
-        case VAL_DICT_I64: { int64_t y; memcpy(&y, h + 8ull * x, 8); return (double)y; }
-        case VAL_DICT_F32: { float y; memcpy(&y, h + 4ull * x, 4); return (double)y; }
-        default: { double y; memcpy(&y, h + 8ull * x, 8); return y; }
-      }
-    };
-    if (expr_fn(a) >= 0) {   // the expression pass's sum, or the decoded MIN / MAX key
-      const unsigned long long w = acc.ex(back, r)[a];
-      if (expr_fn(a) == PB200_AGG_SUM || expr_fn(a) == PB200_AGG_AVG) { memcpy(&v->d, &w, 8); v->l = (int64_t)acc_r.count; }
-      else v->d = expr_key_value(expr_fn(a), w);
-    } else if (fn == PB200_AGG_COUNT) { v->l = (int64_t)acc_r.count; v->d = (double)v->l; }
-    else if (is_moments_fn(fn)) {   // the exact moments from the limb sums (pb200_moments.h), rounded once
-      const int k0 = plan.mom_first[a];
-      const Moments m = moments_from_sums(acc_r.count, acc_r.isum[k0], acc_r.isum[k0 + 1], acc_r.isum[k0 + 2]);
-      v->d = moments_final(fn, m, R.mom.grid[a].e);
-      v->l = (int64_t)acc_r.count;
-      R.mom.one[a][0] = m.s1; R.mom.one[a][1] = (unsigned long long)m.s2; R.mom.one[a][2] = (unsigned long long)(m.s2 >> 64);
-    } else if (fn == PB200_AGG_SUM || fn == PB200_AGG_AVG) {
-      v->d = sum_in_double(vk) ? acc_r.dsum[a] : (double)acc_r.isum[a];
-      v->l = (int64_t)acc_r.count;
-      if (!sum_in_double(vk)) { R.exact.on[a] = true; R.exact.sum[a] = acc_r.isum[a]; }
-    } else if (fn == PB200_AGG_MIN || fn == PB200_AGG_MAX) {
-      // raw INT: 0xFFFFFFFF / 0 are INT_MAX / INT_MIN as well as "no row" (max_offset): only the count tells
-      const bool mn = fn == PB200_AGG_MIN;
-      const uint32_t x = mn ? acc_r.min_id[a] : acc_r.max_id_plus1[a] - max_offset(vk);
-      const bool empty = acc_r.count == 0 || (vk != VAL_RAW_I32 && (mn ? acc_r.min_id[a] == 0xFFFFFFFFu : acc_r.max_id_plus1[a] == 0));
-      if (empty) v->d = mn ? INFINITY : -INFINITY;
-      else { v->id = (int32_t)x; v->d = c->dict_host.empty() && vk != VAL_RAW_I32 ? (double)v->id : value_of(x); }
-    } else if (fn == PB200_AGG_PERCENTILE) {
-      const uint32_t x = host_pct[a];
-      if (x == ~0u) v->d = -INFINITY;   // no matched row
-      else { v->id = (int32_t)x; v->d = value_of(x); v->l = host_pct[kMaxAggs + plan.pct_rep[a]]; }
-    } else if (is_withtime_fn(fn)) {   // the finalize's data dictId and time value; an empty result has no row
-      const uint32_t x = acc.wt_ids(back, r)[a];
-      if (acc_r.count == 0 || x == ~0u) v->d = -INFINITY;
-      else { v->id = (int32_t)x; v->d = c->dict_host.empty() ? (double)v->id : value_of(x); v->l = acc.wt_time(back, r)[a]; }
-    } else if (is_hll_fn(fn) && hll_only_set(r, plan.ds_rep[a])) {
-      // only DISTINCTCOUNTHLLs read this set: the bitset stays on the device until pb200_result_distinct asks for it
-      const int b = plan.ds_rep[a];
-      pb200_result::LazySets& L = R.lazy;
-      if (!L.bits[b]) {
-        L.ctx = ctx;
-        L.bits[b] = static_cast<uint32_t*>(distinct_bufs[r][b]->p);
-        distinct_bufs[r][b]->p = nullptr;
-        L.words[b] = plan.distinct_words[r][b];
-        L.rows[b] = 1;
-      }
-      L.src[a] = b;
-      v->l = acc.hll(back, r)[plan.hll_rep[a]]; v->d = (double)v->l;
-    } else if (fn == PB200_AGG_DISTINCTCOUNT || reads_distinct_set(fn)) {
-      const int b = fn == PB200_AGG_DISTINCTCOUNT ? a : plan.ds_rep[a];   // the aggregation whose bitset holds the set
-      std::vector<uint32_t> bits(plan.distinct_words[r][b]);
-      PB200_CUDA(cudaMemcpy(bits.data(), distinct_bufs[r][b]->p, bits.size() * 4, cudaMemcpyDeviceToHost));
-      R.distinct[a].push_back(bitset_ids(bits.data(), bits.size()));
-      v->l = (int64_t)R.distinct[a].back().size(); v->d = (double)v->l;
-      if (is_distinct_value_fn(fn)) {
-        const unsigned long long* ds = acc.ds(back, r, b);
-        memcpy(&v->d, ds + ds_final_word(fn), 8);   // rounded once by the finalize
-      } else if (is_hll_fn(fn)) {
-        v->l = acc.hll(back, r)[plan.hll_rep[a]]; v->d = (double)v->l;
-      }
-    }
-    return PB200_OK;
-  }
-
   // 11. every result's metadata and (aggregation only) its row, then the group-by rows extracted, or left for
   //     pb200_result_finalize (deferred); per-segment results release their tables
   int fill_results_and_extract(const pb200_order_by* order, const pb200_having* having) {
@@ -1393,11 +1309,23 @@ struct ScanCall {
       }
       R.meta.num_groups = -1;
       R.meta.regime = PB200_REGIME_NONE;
+      const AggAccum& rec = AccumLayout::records(back)[r];
+      const auto src = sources(r, back);
       for (int a = 0; a < nuser; a++) {
-        AggValue v;
-        if (int rc = agg_value(r, a, &v)) return rc;
-        R.dbl[a].push_back(v.d); R.lng[a].push_back(v.l); R.ids[a].push_back(v.id);
+        double dv;
+        long long lv;
+        int32_t id;
+        agg_values(src[a], 0, count, dv, lv, id, R.mom.on[a] ? R.mom.one[a] : nullptr);
+        R.dbl[a].push_back(dv); R.lng[a].push_back(lv); R.ids[a].push_back(id);
+        const int fn = plan.q.aggs[a].function;   // an INT sum's exact value, for a cross-GPU combine
+        if ((fn == PB200_AGG_SUM || fn == PB200_AGG_AVG) && expr_fn(a) < 0 && !sum_in_double(src[a].vk)) { R.exact.on[a] = true; R.exact.sum[a] = rec.isum[a]; }
       }
+      DevBufRaw* sets[kMaxAggs] = {};
+      double* dbl[kMaxAggs] = {};
+      int64_t* lng[kMaxAggs] = {};
+      for (int a = 0; a < nuser; a++) { sets[a] = distinct_bufs[r][a].get(); dbl[a] = R.dbl[a].data(); lng[a] = R.lng[a].data(); }
+      bool kept = false;   // the sets were complete at the read-back
+      if (int rc = decode_sets(ctx, st, &R, sets, plan.distinct_words[r].data(), 1, dbl, lng, &kept)) return rc;
     }
     t_results = now_ms();
     if (!plan.group_by) return PB200_OK;
@@ -1450,8 +1378,7 @@ static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment*
   if (int rc = c.launch()) return rc;
   if (int rc = c.finalize_percentiles()) return rc;
   if (int rc = c.finalize_withtime()) return rc;
-  if (int rc = c.finalize_distinct_sums()) return rc;
-  if (int rc = c.finalize_hll()) return rc;
+  if (int rc = c.finalize_sets()) return rc;
   if (int rc = c.finalize_exprs()) return rc;
   if (int rc = c.read_back_and_verify()) return rc;   // kRetryWithoutCountCarrier: ~ScanCall frees this attempt's tables
   if (int rc = c.fill_results_and_extract(order, having)) return rc;

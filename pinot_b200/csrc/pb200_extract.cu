@@ -32,7 +32,7 @@
 #include <cstring>
 
 #include "pb200_internal.h"
-#include "pb200_expr.h"
+#include "pb200_decode.h"
 #include "pb200_having.h"
 #include "pb200_order.h"
 
@@ -50,8 +50,7 @@ struct ExtractDesc {
   const uint32_t* mink;
   const unsigned long long* hkeys;
   const unsigned long long* packed;  // count-carrying sum table (pb200_plan.cpp): sum(value - vmin) + count << shift
-  long long pack_vmin;
-  int32_t pack_agg, pack_shift;
+  int32_t pack_shift;
   long long groups;                  // table entries (dense: raw key space x stride, hash: capacity)
   int32_t stride, pad_stride;        // dense tables: only entries at multiples of `stride` are ever written
   int32_t ngb, nagg;
@@ -61,23 +60,14 @@ struct ExtractDesc {
   unsigned long long off_keys;       // int32 [rows x ngb]
   unsigned long long off_idx;        // uint32 [rows] raw key / slot (only when a per-group bitset has to be gathered), else kNoCol
   unsigned long long off_dbl[kMaxAggs], off_lng[kMaxAggs], off_ids[kMaxAggs];  // kNoCol: column not produced
-  const void* src[kMaxAggs];         // accumulator table of the aggregation (NULL: COUNT)
-  const void* dict[kMaxAggs];        // device dictionary for the MIN / MAX value lookup (NULL: the id itself is the value)
-  int32_t fn[kMaxAggs], vk[kMaxAggs];
+  unsigned long long off_mom[kMaxAggs];  // VAR / STDDEV: {s1, s2 low, s2 high} per row, for pb200_result_moments
+  AggSource agg[kMaxAggs];           // each aggregation's tables (pb200_decode.h)
   // ORDER BY only (order_idx == NULL: rows in raw-key order)
   uint32_t* order_idx;               // [idx_cap] non-empty entries in raw-key order (index-only pass), sorted in place...
   const uint32_t* order_sorted;      // ...ending up here (one of the sort's two value buffers)
   unsigned long long idx_cap;        // untrimmed row bound: min(entries, numGroupsLimit + 1)
   const uint32_t* dbits[kMaxAggs];   // DISTINCTCOUNT per-group bitsets (an ORDER BY key is the popcount of a row)
   uint32_t dwords[kMaxAggs];
-  const uint32_t* pct_n[kMaxAggs];   // PERCENTILE: values per table entry (src[a] holds the selected dictIds)
-  const long long* wt_time[kMaxAggs];  // FIRST/LASTWITHTIME: the winning row's time value per table entry (src[a]: data dictIds)
-  const long long* mom[kMaxAggs][3]; // VAR / STDDEV: the K, H, L limb sum tables (pb200_moments.h)
-  int32_t mom_e[kMaxAggs];           // ... and the grid exponent of the column
-  unsigned long long off_mom[kMaxAggs];  // ... {s1, s2 low, s2 high} per row, for pb200_result_moments
-  const unsigned long long* ds[kMaxAggs];  // DISTINCTSUM / DISTINCTAVG: the finalized state per table entry (kDsWords u64)
-  const long long* hll[kMaxAggs];    // DISTINCTCOUNTHLL: the estimate per table entry
-  const unsigned long long* xkey[kMaxAggs];  // expression MIN / MAX (pb200_expr.cu): Double.compare key per table entry
   const uint8_t* keep;               // HAVING only: bit j of byte i = entry 8i + j is a row (NULL: every non_empty() entry is)
 };
 
@@ -86,13 +76,16 @@ __device__ __forceinline__ bool non_empty(const ExtractDesc& d, long long i) {
   if (d.packed) return d.packed[i] != 0ull;
   return (d.count && d.count[i] != 0ull) || (d.seen && d.seen[i] != 0u) || (d.maxk && d.maxk[i] != 0u) || (d.mink && d.mink[i] != 0xFFFFFFFFu);
 }
-// bit j = entry base + j is a row of the result (base: a multiple of 8)
-__device__ __forceinline__ uint32_t entry_flags(const ExtractDesc& d, long long base) {
-  if (d.keep) return d.keep[base >> 3];
+// bit j = entry base + j exists (base: a multiple of 8)
+__device__ __forceinline__ uint32_t exists_flags(const ExtractDesc& d, long long base) {
   uint32_t flags = 0;
 #pragma unroll
   for (int j = 0; j < 8; ++j) flags |= ((base + j < d.groups && non_empty(d, base + j)) ? 1u : 0u) << j;
   return flags;
+}
+// bit j = entry base + j is a row of the result
+__device__ __forceinline__ uint32_t entry_flags(const ExtractDesc& d, long long base) {
+  return d.keep ? d.keep[base >> 3] : exists_flags(d, base);
 }
 __device__ __forceinline__ int find_result(const ExtractDesc* descs, int nres, uint32_t chunk) {
   int r = 0;
@@ -144,67 +137,6 @@ __device__ __forceinline__ unsigned long long group_count(const ExtractDesc& d, 
   return d.packed ? d.packed[g] >> d.pack_shift : (d.count ? d.count[g] : 0ull);
 }
 
-// aggregation a of entry g as the result's columns hold it: double value, long (count), MIN / MAX dictId.  DISTINCTCOUNT
-// leaves zeros (the set sizes are filled in on the host from the gathered bitsets)
-// value of dictId x of aggregation a's column
-__device__ __forceinline__ double dict_value(const ExtractDesc& d, int a, uint32_t x) {
-  const int vk = d.vk[a];
-  if (vk == VAL_RAW_I32) return (double)(int32_t)(x ^ 0x80000000u);
-  if (!d.dict[a]) return (double)x;
-  if (vk == VAL_DICT_I32) return (double)(int32_t)(static_cast<const uint32_t*>(d.dict[a])[x] ^ 0x80000000u);  // device copy is biased
-  if (vk == VAL_DICT_I64) return (double)static_cast<const long long*>(d.dict[a])[x];
-  if (vk == VAL_DICT_F32) return (double)static_cast<const float*>(d.dict[a])[x];
-  return static_cast<const double*>(d.dict[a])[x];
-}
-
-__device__ __forceinline__ void agg_values(const ExtractDesc& d, int a, long long g, unsigned long long cnt, double& dv,
-                                           long long& lv, int32_t& id) {
-  const int fn = d.fn[a], vk = d.vk[a];
-  dv = 0.0; lv = 0; id = -1;
-  if (fn == PB200_AGG_COUNT) { lv = (long long)cnt; dv = (double)cnt; }
-  else if (fn == PB200_AGG_SUM || fn == PB200_AGG_AVG) {
-    if (a == d.pack_agg) {  // low field = sum(value - vmin): exact integer arithmetic, then to double like every sum
-      const unsigned long long f = d.packed[g] & ((1ull << d.pack_shift) - 1ull);
-      dv = (double)((long long)f + (long long)cnt * d.pack_vmin);
-    } else {
-      dv = sum_in_double(vk) ? static_cast<const double*>(d.src[a])[g] : (double)static_cast<const long long*>(d.src[a])[g];
-    }
-    lv = (long long)cnt;
-  } else if (d.xkey[a]) {
-    dv = expr_key_value(fn, d.xkey[a][g]);
-  } else if (fn == PB200_AGG_MIN || fn == PB200_AGG_MAX) {
-    const uint32_t t = static_cast<const uint32_t*>(d.src[a])[g];
-    // every row of a submission reaches each of its functions, so a group that exists has a MIN / MAX.  Raw INT entries
-    // are all values (max_offset): 0xFFFFFFFF / 0 are INT_MAX / INT_MIN there, never "empty"
-    const bool empty = vk != VAL_RAW_I32 && (fn == PB200_AGG_MIN ? t == 0xFFFFFFFFu : t == 0u);
-    if (empty) dv = fn == PB200_AGG_MIN ? INFINITY : -INFINITY;
-    else {
-      const uint32_t x = fn == PB200_AGG_MIN ? t : t - max_offset(vk);
-      id = (int32_t)x;
-      dv = dict_value(d, a, x);
-    }
-  } else if (fn == PB200_AGG_PERCENTILE) {  // finalized from the histogram (pb200_percentile.cu): dictId, ~0 = no row
-    const uint32_t x = static_cast<const uint32_t*>(d.src[a])[g];
-    lv = d.pct_n[a][g];
-    if (x == ~0u) dv = -INFINITY;
-    else { id = (int32_t)x; dv = dict_value(d, a, x); }
-  } else if (fn == PB200_AGG_FIRSTWITHTIME || fn == PB200_AGG_LASTWITHTIME) {  // finalized (pb200_withtime.cu): ~0 = no row
-    const uint32_t x = static_cast<const uint32_t*>(d.src[a])[g];
-    if (x == ~0u) dv = -INFINITY;
-    else { id = (int32_t)x; dv = dict_value(d, a, x); lv = d.wt_time[a][g]; }
-  } else if (is_moments_fn(fn)) {  // exact moments from the group's limb sums and count, rounded once
-    dv = moments_final(fn, moments_from_sums(cnt, d.mom[a][0][g], d.mom[a][1][g], d.mom[a][2][g]), d.mom_e[a]);
-    lv = (long long)cnt;
-  } else if (is_distinct_value_fn(fn)) {  // rounded once by the finalize (pb200_distinct_sum.cu); no rounding here keeps the
-    const unsigned long long* st = d.ds[a] + (size_t)g * kDsWords;   // registers of the kernels every group-by query runs
-    dv = __longlong_as_double((long long)st[ds_final_word(fn)]);
-    lv = (long long)st[2];
-  } else if (is_hll_fn(fn)) {   // the finalize's estimate (pb200_hll.cu), in both columns
-    lv = d.hll[a][g];
-    dv = (double)lv;
-  }
-}
-
 // set size of DISTINCTCOUNT aggregation a in entry g: the popcount of its bitset row
 __device__ __forceinline__ long long distinct_size(const ExtractDesc& d, int a, long long g) {
   const uint32_t* row = d.dbits[a] + (size_t)g * d.dwords[a];
@@ -231,15 +163,11 @@ __device__ __forceinline__ void write_row(const ExtractDesc& d, unsigned long lo
     double dv;
     long long lv;
     int32_t id;
-    agg_values(d, a, g, cnt, dv, lv, id);
+    agg_values(d.agg[a], g, cnt, dv, lv, id,
+               d.off_mom[a] != kNoCol ? reinterpret_cast<unsigned long long*>(out + d.off_mom[a]) + 3 * row : nullptr);
     if (d.off_dbl[a] != kNoCol) reinterpret_cast<double*>(out + d.off_dbl[a])[row] = dv;
     if (d.off_lng[a] != kNoCol) reinterpret_cast<long long*>(out + d.off_lng[a])[row] = lv;
     if (d.off_ids[a] != kNoCol) reinterpret_cast<int32_t*>(out + d.off_ids[a])[row] = id;
-    if (d.off_mom[a] != kNoCol) {
-      const Moments m = moments_from_sums(cnt, d.mom[a][0][g], d.mom[a][1][g], d.mom[a][2][g]);
-      unsigned long long* mp = reinterpret_cast<unsigned long long*>(out + d.off_mom[a]) + 3 * row;
-      mp[0] = m.s1; mp[1] = (unsigned long long)m.s2; mp[2] = (unsigned long long)(m.s2 >> 64);
-    }
   }
 }
 
@@ -308,11 +236,11 @@ __global__ void __launch_bounds__(kExtractThreads) order_key_kernel(const Extrac
       double dv;
       long long lv;
       int32_t id;
-      if (d.fn[p.index] == PB200_AGG_DISTINCTCOUNT) {
+      if (d.agg[p.index].fn == PB200_AGG_DISTINCTCOUNT) {
         lv = distinct_size(d, p.index, g);
         dv = (double)lv;
       } else {
-        agg_values(d, p.index, g, group_count(d, g), dv, lv, id);
+        agg_values(d.agg[p.index], g, group_count(d, g), dv, lv, id, nullptr);
       }
       k = order_key(p.cmp, p.descending != 0, p.mask, dv, lv);
     } else {
@@ -339,25 +267,24 @@ __global__ void __launch_bounds__(kExtractThreads) having_kernel(const ExtractDe
   __shared__ uint32_t wsum[kExtractThreads / 32];
   const ExtractDesc& d = descs[r];
   const long long base = (long long)blockIdx.x * kChunk + threadIdx.x * 8;
-  uint32_t flags = 0, c = 0;
+  uint32_t flags = exists_flags(d, base);
+  const uint32_t c = __reduce_add_sync(0xFFFFFFFFu, __popc(flags));   // counted first: not live across the evaluations
+  if ((threadIdx.x & 31) == 0) wsum[threadIdx.x >> 5] = c;
   for (int j = 0; j < 8; ++j) {
+    if (!((flags >> j) & 1u)) continue;
     const long long g = base + j;
-    if (g >= d.groups || !non_empty(d, g)) continue;
-    ++c;
     const unsigned long long cnt = group_count(d, g);
     const bool pass = having_eval(h, [&](int a) -> double {
-      if (d.fn[a] == PB200_AGG_DISTINCTCOUNT) return (double)distinct_size(d, a, g);
+      if (d.agg[a].fn == PB200_AGG_DISTINCTCOUNT) return (double)distinct_size(d, a, g);
       double dv;
       long long lv;
       int32_t id;
-      agg_values(d, a, g, cnt, dv, lv, id);
-      return having_value(d.fn[a], dv, lv);
+      agg_values(d.agg[a], g, cnt, dv, lv, id, nullptr);
+      return having_value(d.agg[a].fn, dv, lv);
     });
-    flags |= (pass ? 1u : 0u) << j;
+    if (!pass) flags &= ~(1u << j);
   }
   keep[base >> 3] = (uint8_t)flags;
-  c = __reduce_add_sync(0xFFFFFFFFu, c);
-  if ((threadIdx.x & 31) == 0) wsum[threadIdx.x >> 5] = c;
   __syncthreads();
   if (threadIdx.x == 0) {
     unsigned long long t = 0;
@@ -380,10 +307,10 @@ static size_t layout_result(const pb200_result::Dense& d, ExtractDesc& e, size_t
   e.cap_rows = rows;
   e.off_keys = take(4, rows * (size_t)std::max(e.ngb, 1));
   bool need_idx = false;
-  for (int a = 0; a < e.nagg; a++) need_idx |= d.dbits[a] != nullptr || e.fn[a] == PB200_AGG_PERCENTILE;
+  for (int a = 0; a < e.nagg; a++) need_idx |= d.dbits[a] != nullptr || e.agg[a].fn == PB200_AGG_PERCENTILE;
   e.off_idx = need_idx ? take(4, rows) : kNoCol;
   for (int a = 0; a < e.nagg; a++) {
-    const int fn = e.fn[a];
+    const int fn = e.agg[a].fn;
     e.off_dbl[a] = take(8, rows);
     e.off_lng[a] = agg_fn(fn)->long_col ? take(8, rows) : kNoCol;
     e.off_ids[a] = agg_fn(fn)->ids_col ? take(4, rows) : kNoCol;
@@ -448,29 +375,13 @@ int extract_groups(pb200_ctx* ctx, pb200_result* const* Rs, int nres, cudaStream
     ExtractDesc& e = descs[r];
     memset(&e, 0, sizeof e);
     e.count = d.count; e.seen = d.seen; e.maxk = d.exists_max; e.mink = d.exists_min; e.hkeys = d.hkeys;
-    e.packed = d.exists_packed; e.pack_agg = d.pack_agg; e.pack_shift = d.pack_shift; e.pack_vmin = d.pack_vmin;
+    e.packed = d.exists_packed; e.pack_shift = d.pack_shift;
     e.groups = d.groups;
     e.stride = std::max(d.stride, 1);
     e.ngb = (int)d.cards.size();
     e.nagg = (int)d.aggs.size();
     for (int k = 0; k < e.ngb; k++) e.cards[k] = (uint32_t)d.cards[k];
-    for (int a = 0; a < e.nagg; a++) {
-      const int fn = d.aggs[a].function, vk = d.val_kind[a];
-      e.fn[a] = fn; e.vk[a] = vk;
-      if (fn == PB200_AGG_SUM || fn == PB200_AGG_AVG) e.src[a] = sum_in_double(vk) ? (const void*)d.dsum[a] : (const void*)d.isum[a];
-      else if (d.expr_tab[a]) e.xkey[a] = static_cast<const unsigned long long*>(d.expr_tab[a]);   // MIN / MAX of an expression
-      else if (fn == PB200_AGG_MIN) e.src[a] = d.gmin[a];
-      else if (fn == PB200_AGG_MAX) e.src[a] = d.gmax[a];
-      else if (fn == PB200_AGG_PERCENTILE) { e.src[a] = Rs[r]->pct.ids[a]; e.pct_n[a] = Rs[r]->pct.n[Rs[r]->pct.rep[a]]; }
-      else if (fn == PB200_AGG_FIRSTWITHTIME || fn == PB200_AGG_LASTWITHTIME) { e.src[a] = Rs[r]->wt.ids[a]; e.wt_time[a] = Rs[r]->wt.time[a]; }
-      else if (is_moments_fn(fn)) {
-        for (int j = 0; j < 3; j++) e.mom[a][j] = d.isum[d.mom_first[a] + j];
-        e.mom_e[a] = d.mom_e[a];
-      } else if (is_distinct_value_fn(fn)) e.ds[a] = d.ds_state[d.ds_rep[a]];
-      else if (is_hll_fn(fn)) e.hll[a] = d.hll_est[d.hll_rep[a]];
-      const DeviceColumn* c = d.agg_cols[a];
-      e.dict[a] = (c && vk != VAL_RAW_I32 && !c->dict_host.empty()) ? c->dict_native : nullptr;
-    }
+    agg_sources(*Rs[r], e.agg);
     e.first_chunk = chunks;
     e.num_chunks = (uint32_t)((d.groups + kChunk - 1) / kChunk);
     chunks += e.num_chunks;
@@ -482,7 +393,7 @@ int extract_groups(pb200_ctx* ctx, pb200_result* const* Rs, int nres, cudaStream
       for (int i = 0; i < Rs[r]->having.num_nodes; i++) {
         const pb200_having_node& hn = Rs[r]->having.nodes[i];
         const bool leaf = hn.op == PB200_HAVING_RANGE || hn.op == PB200_HAVING_EQ || hn.op == PB200_HAVING_NEQ;
-        if (leaf && e.fn[hn.agg] == PB200_AGG_DISTINCTCOUNT && !d.dbits[hn.agg]) {
+        if (leaf && e.agg[hn.agg].fn == PB200_AGG_DISTINCTCOUNT && !d.dbits[hn.agg]) {
           set_error("HAVING on a DISTINCTCOUNT without per-group sets"); return PB200_E_UNSUPPORTED;
         }
       }
@@ -490,7 +401,7 @@ int extract_groups(pb200_ctx* ctx, pb200_result* const* Rs, int nres, cudaStream
     if (Rs[r]->order.num_items > 0) {
       for (int i = 0; i < Rs[r]->order.num_items; i++) {
         const pb200_order_item& it = Rs[r]->order.items[i];
-        if (it.kind == PB200_ORDER_AGG && e.fn[it.index] == PB200_AGG_DISTINCTCOUNT && !d.dbits[it.index]) {
+        if (it.kind == PB200_ORDER_AGG && e.agg[it.index].fn == PB200_AGG_DISTINCTCOUNT && !d.dbits[it.index]) {
           set_error("ORDER BY a DISTINCTCOUNT without per-group sets"); return PB200_E_UNSUPPORTED;
         }
       }
@@ -537,23 +448,15 @@ int extract_groups(pb200_ctx* ctx, pb200_result* const* Rs, int nres, cudaStream
     for (int r = 0; r < nres; r++)
       if (Rs[r]->having.num_nodes > 0) descs[r].keep = static_cast<const uint8_t*>(dkeep.p) + 256ull * descs[r].first_chunk;
   }
-  // ---- DISTINCTSUM / DISTINCTAVG: every table entry's bitset row -> its state, before HAVING, the order keys and the rows
-  //      read it (entries without rows have an empty row and finalize to the empty state) ----
+  // ---- DISTINCTSUM / DISTINCTAVG / DISTINCTCOUNTHLL: every table entry's bitset row -> its state or estimate, before
+  //      HAVING, the order keys and the rows read it (entries without rows have an empty row and finalize to the empty
+  //      state) ----
   std::vector<std::unique_ptr<DevBufRaw>> ds_temps;
   for (int r = 0; r < nres; r++) {
     const pb200_result::Dense& d = Rs[r]->dense;
-    for (int b = 0; b < descs[r].nagg; b++) {   // one state per set: indexed by the aggregation whose bitset holds it
-      if (!d.ds_state[b]) continue;
-      const DeviceColumn& c = *d.agg_cols[b];
-      const DistinctSumJob job{d.dbits[b], d.dwords[b], d.groups, false, c.dict_native, c.stored_type, d.ds_e[b], d.ds_state[b]};
-      if ((rc = distinct_sum_finalize(ctx, st, job, ds_temps))) return rc;
-    }
-    for (int a = 0; a < descs[r].nagg; a++) {   // DISTINCTCOUNTHLL: one estimate per column and log2m
-      if (d.hll_rep[a] != a || !d.hll_est[a]) continue;
-      const int b = d.ds_rep[a];
-      const HllJob job{d.dbits[b], d.dwords[b], d.groups, false, d.agg_cols[b]->moments->hll_hash, d.hll_log2m[a], d.hll_est[a]};
-      if ((rc = hll_finalize(ctx, st, job, ds_temps))) return rc;
-    }
+    size_t words[kMaxAggs] = {};
+    for (int b = 0; b < descs[r].nagg; b++) words[b] = d.dwords[b];
+    if ((rc = finalize_sets(ctx, st, d, d.dbits, words, d.groups, false, descs[r].agg, ds_temps))) return rc;
   }
   const ExtractDesc* ddescs = (const ExtractDesc*)ddesc.p;
   PB200_CUDA(cudaMemcpyAsync(ddesc.p, descs.data(), sizeof(ExtractDesc) * nres, cudaMemcpyHostToDevice, st));
@@ -646,51 +549,112 @@ int extract_groups(pb200_ctx* ctx, pb200_result* const* Rs, int nres, cudaStream
       v.ids[a] = e.off_ids[a] == kNoCol ? nullptr : reinterpret_cast<const int32_t*>(out + e.off_ids[a]);
       R->mom.rows[a] = e.off_mom[a] == kNoCol ? nullptr : reinterpret_cast<const unsigned long long*>(out + e.off_mom[a]);
     }
-    // DISTINCTCOUNT with GROUP BY: the groups' bitset rows are gathered on the device and decoded here into dictId lists
+    // DISTINCTCOUNT with GROUP BY: the groups' bitset rows are gathered on the device and decoded into dictId lists
     // (what extractGroupByResult's value-set conversion starts from, BaseDistinctAggregateAggregationFunction :306-321)
-    // (DISTINCTSUM / DISTINCTAVG / DISTINCTCOUNTHLL: the same from the bitset that holds their set, decoded once per
-    // bitset; their columns already hold value and size.  A set only DISTINCTCOUNTHLLs read keeps its gathered rows on
-    // the device instead, for pb200_result_distinct to decode on first use.)
-    std::vector<int> decoded(nagg, -1);   // the bitset aggregation a's set was decoded from
-    std::vector<int32_t> fns(nagg);
-    for (int a = 0; a < nagg; a++) fns[a] = d.aggs[a].function;
-    for (int a = 0; a < nagg; a++) {
-      const bool value_fn = reads_distinct_set(d.aggs[a].function);
-      const int b = value_fn ? d.ds_rep[a] : a;
-      if ((d.aggs[a].function != PB200_AGG_DISTINCTCOUNT && !value_fn) || b < 0 || !d.dbits[b]) continue;
-      decoded[a] = b;
-      const bool lazy = hll_only_set_of(fns.data(), d.ds_rep, nagg, b);
-      if (lazy) R->lazy.src[a] = b;
-      const int same = (int)(std::find(decoded.begin(), decoded.begin() + a, b) - decoded.begin());
-      if (same < a) { if (!lazy) R->distinct[a] = R->distinct[same]; continue; }
-      const size_t wpg = d.dwords[b], rows = v.rows;
-      std::vector<uint32_t> bits(lazy ? 0 : rows * wpg);
-      if (rows) {
-        DevBufRaw g(ctx);
-        if ((rc = g.alloc(rows * wpg * 4))) return rc;
-        gather_bitset_rows_kernel<<<grid_for(ctx, (long long)(rows * wpg), 256), 256, 0, st>>>(d.dbits[b], reinterpret_cast<const uint32_t*>(out + e.off_idx), (long long)rows, (int)wpg, (uint32_t*)g.p);
-        if (lazy) {   // owned by the result from here on; the stream orders the gather before any later copy of it
-          pb200_result::LazySets& L = R->lazy;
-          dev_free(ctx, L.bits[b]);   // a result extracted again (pb200_result_finalize) replaces its rows
-          L.ctx = ctx; L.bits[b] = static_cast<uint32_t*>(g.p); L.words[b] = wpg; L.rows[b] = rows;
-          g.p = nullptr;
-          kept_sets = true;
-          continue;
-        }
-        PB200_CUDA(cudaMemcpyAsync(bits.data(), g.p, rows * wpg * 4, cudaMemcpyDeviceToHost, st));
-        PB200_CUDA(cudaStreamSynchronize(st));
-      }
-      if (lazy) { R->lazy.ctx = ctx; R->lazy.words[b] = wpg; R->lazy.rows[b] = 0; continue; }
-      R->distinct[a].resize(rows);
-      int64_t* sizes = const_cast<int64_t*>(v.lng[a]);   // the kernel left zeros: the set sizes go here
-      double* dsz = const_cast<double*>(v.dbl[a]);
-      for (size_t i = 0; i < rows; i++) {
-        R->distinct[a][i] = bitset_ids(bits.data() + i * wpg, wpg);
-        if (!value_fn) { sizes[i] = (int64_t)R->distinct[a][i].size(); dsz[i] = (double)sizes[i]; }
-      }
+    std::unique_ptr<DevBufRaw> gathered[kMaxAggs];
+    DevBufRaw* sets[kMaxAggs] = {};
+    size_t words[kMaxAggs] = {};
+    double* dbl[kMaxAggs] = {};
+    int64_t* lng[kMaxAggs] = {};
+    for (int b = 0; b < nagg; b++) {
+      dbl[b] = const_cast<double*>(v.dbl[b]);   // the kernel left zeros for DISTINCTCOUNT: the set sizes go here
+      lng[b] = const_cast<int64_t*>(v.lng[b]);
+      if (!d.dbits[b]) continue;
+      gathered[b].reset(new DevBufRaw(ctx));
+      sets[b] = gathered[b].get();
+      words[b] = d.dwords[b];
+      if (!v.rows) continue;
+      if ((rc = sets[b]->alloc(v.rows * words[b] * 4))) return rc;
+      gather_bitset_rows_kernel<<<grid_for(ctx, (long long)(v.rows * words[b]), 256), 256, 0, st>>>(
+          d.dbits[b], reinterpret_cast<const uint32_t*>(out + e.off_idx), (long long)v.rows, (int)words[b], (uint32_t*)sets[b]->p);
     }
+    if ((rc = decode_sets(ctx, st, R, sets, words, v.rows, dbl, lng, &kept_sets))) return rc;
   }
   if (kept_sets) PB200_CUDA(cudaStreamSynchronize(st));   // the bitset tables may be freed once this returns
+  return PB200_OK;
+}
+
+void agg_sources(const pb200_result& R, AggSource* out) {
+  const pb200_result::Dense& d = R.dense;
+  for (int a = 0; a < (int)d.aggs.size(); a++) {
+    AggSource& s = out[a];
+    s = AggSource{};
+    const int fn = s.fn = d.aggs[a].function, vk = s.vk = d.val_kind[a];
+    if (fn == PB200_AGG_SUM || fn == PB200_AGG_AVG) {
+      s.src = sum_in_double(vk) ? (void*)d.dsum[a] : (void*)d.isum[a];
+      if (a == d.pack_agg) { s.pack_shift = d.pack_shift; s.pack_vmin = d.pack_vmin; }
+    } else if (d.expr_tab[a]) s.xkey = static_cast<unsigned long long*>(d.expr_tab[a]);   // MIN / MAX of an expression
+    else if (fn == PB200_AGG_MIN) s.src = d.gmin[a];
+    else if (fn == PB200_AGG_MAX) s.src = d.gmax[a];
+    else if (fn == PB200_AGG_PERCENTILE) { s.src = R.pct.ids[a]; s.pct_n = R.pct.n[R.pct.rep[a]]; }
+    else if (is_withtime_fn(fn)) { s.src = R.wt.ids[a]; s.wt_time = R.wt.time[a]; }
+    else if (is_moments_fn(fn)) {
+      for (int j = 0; j < 3; j++) s.mom[j] = d.isum[d.mom_first[a] + j];
+      s.mom_e = d.mom_e[a];
+    } else if (is_distinct_value_fn(fn)) s.ds = d.ds_state[d.ds_rep[a]];
+    else if (is_hll_fn(fn)) s.hll = d.hll_est[d.hll_rep[a]];
+    const DeviceColumn* c = d.agg_cols[a];
+    s.dict = (c && vk != VAL_RAW_I32 && !c->dict_host.empty()) ? c->dict_native : nullptr;
+    s.dict_bias = 0x80000000u;   // the device copy of an INT dictionary is biased
+    s.counted = d.count || d.exists_packed;
+  }
+}
+
+int finalize_sets(pb200_ctx* ctx, cudaStream_t st, const pb200_result::Dense& d, const uint32_t* const* bits, const size_t* words,
+                  long long rows, bool single, const AggSource* src, std::vector<std::unique_ptr<DevBufRaw>>& temps) {
+  for (int a = 0; a < (int)d.aggs.size(); a++) {
+    const int fn = d.aggs[a].function, b = d.ds_rep[a];
+    if (!reads_distinct_set(fn)) continue;
+    const DeviceColumn& c = *d.agg_cols[b];   // a reader of another aggregation's set has no scan slot of its own
+    if (is_distinct_value_fn(fn)) {   // one state per set, in the table of the first aggregation that reads it
+      bool done = false;
+      for (int x = 0; x < a && !done; x++) done = is_distinct_value_fn(d.aggs[x].function) && d.ds_rep[x] == b;
+      if (done) continue;
+      const DistinctSumJob job{bits[b], words[b], rows, single, c.dict_native, c.stored_type, c.moments->ds_e, src[a].ds};
+      if (int rc = distinct_sum_finalize(ctx, st, job, temps)) return rc;
+    } else if (is_hll_fn(fn) && d.hll_rep[a] == a) {   // one estimate per column and log2m
+      const HllJob job{bits[b], words[b], rows, single, c.moments->hll_hash, d.hll_log2m[a], src[a].hll};
+      if (int rc = hll_finalize(ctx, st, job, temps)) return rc;
+    }
+  }
+  return PB200_OK;
+}
+
+int decode_sets(pb200_ctx* ctx, cudaStream_t st, pb200_result* R, DevBufRaw* const* sets, const size_t* words, size_t rows,
+                double* const* dbl, int64_t* const* lng, bool* kept) {
+  const pb200_result::Dense& d = R->dense;
+  const int nagg = (int)d.aggs.size();
+  std::vector<int> decoded(nagg, -1);   // the bitset aggregation a's set was decoded from
+  std::vector<int32_t> fns(nagg);
+  for (int a = 0; a < nagg; a++) fns[a] = d.aggs[a].function;
+  for (int a = 0; a < nagg; a++) {
+    const bool value_fn = reads_distinct_set(fns[a]);
+    const int b = value_fn ? d.ds_rep[a] : a;
+    if ((fns[a] != PB200_AGG_DISTINCTCOUNT && !value_fn) || b < 0 || !sets[b]) continue;
+    decoded[a] = b;
+    const bool lazy = hll_only_set_of(fns.data(), d.ds_rep, nagg, b);
+    if (lazy) R->lazy.src[a] = b;
+    const int same = (int)(std::find(decoded.begin(), decoded.begin() + a, b) - decoded.begin());
+    if (same < a) { if (!lazy) R->distinct[a] = R->distinct[same]; continue; }
+    if (lazy) {   // owned by the result from here on; the stream orders the rows' writes before any later copy of them
+      pb200_result::LazySets& L = R->lazy;
+      dev_free(ctx, L.bits[b]);   // a result extracted again (pb200_result_finalize) replaces its rows
+      L.ctx = ctx; L.bits[b] = static_cast<uint32_t*>(sets[b]->p); L.words[b] = words[b]; L.rows[b] = rows;
+      sets[b]->p = nullptr;
+      *kept |= L.bits[b] != nullptr;
+      continue;
+    }
+    std::vector<uint32_t> bits(rows * words[b]);
+    if (!bits.empty()) {
+      PB200_CUDA(cudaMemcpyAsync(bits.data(), sets[b]->p, bits.size() * 4, cudaMemcpyDeviceToHost, st));
+      PB200_CUDA(cudaStreamSynchronize(st));
+    }
+    R->distinct[a].resize(rows);
+    for (size_t i = 0; i < rows; i++) {
+      R->distinct[a][i] = bitset_ids(bits.data() + i * words[b], words[b]);
+      if (!value_fn) { lng[a][i] = (int64_t)R->distinct[a][i].size(); dbl[a][i] = (double)lng[a][i]; }
+    }
+  }
   return PB200_OK;
 }
 

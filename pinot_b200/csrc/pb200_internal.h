@@ -244,10 +244,11 @@ struct pb200_result {
   } wt;
   // VAR / STDDEV (pb200_moments.h): the grid of each such aggregation's dictionary and its exact moments per row
   struct Mom {
+    Mom() { for (int a = 0; a < pb200::kMaxAggs; a++) rows[a] = one[a]; }
     bool on[pb200::kMaxAggs] = {};
     pb200::MomentGrid grid[pb200::kMaxAggs] = {};
-    const unsigned long long* rows[pb200::kMaxAggs] = {};  // group-by: {s1, s2 low, s2 high} per row (inside view.block)
-    unsigned long long one[pb200::kMaxAggs][3] = {};        // aggregation only: the same for the one row
+    const unsigned long long* rows[pb200::kMaxAggs];      // {s1, s2 low, s2 high} per row: `one`, or (group-by) in view.block
+    unsigned long long one[pb200::kMaxAggs][3] = {};       // aggregation only: the one row's
   } mom;
   // aggregation only: the exact int64 sum behind an INT SUM / AVG (the double column holds it rounded), so that a
   // cross-GPU combine adds exact sums and rounds once (pb200_result_exact_sum, pb200_comm.cu: combine_scalars)
@@ -310,10 +311,9 @@ struct pb200_result {
     uint32_t* dbits[pb200::kMaxAggs] = {};      // DISTINCTCOUNT with GROUP BY: per-group dictId bitsets, dwords[a] words each
     uint32_t dwords[pb200::kMaxAggs] = {};
     // DISTINCTSUM / DISTINCTAVG (pb200_distinct_sum.h): the aggregation b whose bitset holds the set (-1: neither
-    // function); indexed by b, the grid exponent and the set's finalized state per table entry (kDsWords u64 each,
-    // device), shared by every function that reads the set
+    // function); indexed by b, the set's finalized state per table entry (kDsWords u64 each, device), shared by every
+    // function that reads the set
     int ds_rep[pb200::kMaxAggs];
-    int ds_e[pb200::kMaxAggs] = {};
     unsigned long long* ds_state[pb200::kMaxAggs] = {};
     // DISTINCTCOUNTHLL (pb200_hll.h): log2m of aggregation a (0: not one); indexed by the first HLL of a column and log2m
     // (ScanPlan::hll_rep), the estimate per table entry (int64, device), shared by the HLLs with that column and log2m
@@ -390,6 +390,20 @@ inline int grid_for(const pb200_ctx* ctx, long long items, int threads) {
 std::vector<int32_t> bitset_ids(const uint32_t* bits, size_t words);
 // pb200_extract.cu: non-empty groups of the results' device tables -> final layout in pinned memory (all results at once)
 int extract_groups(pb200_ctx* ctx, pb200_result* const* results, int nres, cudaStream_t st);
+struct AggSource;   // pb200_decode.h
+// The decoder's sources of a GROUP BY result's aggregations (out: one per aggregation), over its device tables.
+void agg_sources(const pb200_result& R, AggSource* out);
+// DISTINCTSUM / DISTINCTAVG states and DISTINCTCOUNTHLL estimates of one result's sets, queued on `st`: the `rows` rows of
+// set b (bits[b], words[b] u32 per row; b the aggregation whose bitset holds the set) into the tables of `src`, once per
+// set and once per column and log2m.  d: the result's aggregations.  single: the one row of an aggregation-only result.
+int finalize_sets(pb200_ctx* ctx, cudaStream_t st, const pb200_result::Dense& d, const uint32_t* const* bits, const size_t* words,
+                  long long rows, bool single, const AggSource* src, std::vector<std::unique_ptr<DevBufRaw>>& temps);
+// The value sets of R's `rows` rows: DISTINCTCOUNT's, and those DISTINCTSUM / DISTINCTAVG / DISTINCTCOUNTHLL read, decoded
+// once per set from its rows on the device (sets[b], words[b] u32 per row).  DISTINCTCOUNT's set sizes go to dbl[a] /
+// lng[a].  A set only DISTINCTCOUNTHLLs read is not decoded: R takes its device rows for pb200_result_distinct to decode
+// on first use (sets[b] gives them up; *kept is set when rows are still being written on `st`).
+int decode_sets(pb200_ctx* ctx, cudaStream_t st, pb200_result* R, DevBufRaw* const* sets, const size_t* words, size_t rows,
+                double* const* dbl, int64_t* const* lng, bool* kept);
 void result_materialize(pb200_result* R);  // view -> the std::vector fields
 // pb200_order_by checks shared by the device and host entry points: PB200_OK or PB200_E_INVALID (message set)
 int order_validate(const pb200_order_by* order, int num_aggs, int num_group_by);

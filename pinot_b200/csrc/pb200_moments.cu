@@ -94,16 +94,10 @@ extern "C" int32_t pb200_result_moments(const pb200_result* R, int32_t a, int32_
   if (!R->mom.on[a]) { set_error("aggregation %d is not VAR_POP / VAR_SAMP / STDDEV_POP / STDDEV_SAMP", a); return PB200_E_INVALID; }
   const long long rows = R->meta.num_groups < 0 ? 1 : R->meta.num_groups;
   if (row < 0 || row >= rows) { set_error("bad row %d (%lld rows)", row, rows); return PB200_E_INVALID; }
-  const unsigned long long* m;
-  long long cnt;
-  if (R->meta.num_groups < 0) {
-    m = R->mom.one[a];
-    cnt = R->lng[a][0];
-  } else {
-    if (!R->mom.rows[a] || !R->view.lng[a]) { set_error("result rows carry no moments"); return PB200_E_INVALID; }
-    m = R->mom.rows[a] + 3ull * row;
-    cnt = R->view.lng[a][row];
-  }
+  const int64_t* counts = R->meta.num_groups < 0 ? R->lng[a].data() : R->view.lng[a];
+  if (!R->mom.rows[a] || !counts) { set_error("result rows carry no moments"); return PB200_E_INVALID; }
+  const unsigned long long* m = R->mom.rows[a] + 3ull * row;
+  const long long cnt = counts[row];
   const MomentGrid& g = R->mom.grid[a];
   if (n) *n = cnt;
   if (c_mant) *c_mant = g.c_mant;
