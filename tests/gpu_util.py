@@ -16,7 +16,7 @@ SUM_REL_TOL = 1e-6
 TUNING_DEFAULTS = {"warps": 6, "defer": 1, "gb_defer": 1, "sparse_max_agg": -1, "smem_groups": 1, "smem_copies": 0,
                    "pack_count": 1, "pack_shift": 0, "dense_max": 1 << 24, "table_stride": 0, "grid": 0, "ctas_per_sm": 2,
                    "raw_dict_max": 1 << 20, "always_count": 0,
-                   "sparse_max": 4, "skip": 1, "stages": 0}
+                   "sparse_max": 4, "skip": 1, "stages": 0, "spec": 1}
 
 
 @contextlib.contextmanager

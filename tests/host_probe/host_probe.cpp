@@ -3,6 +3,7 @@
 //   * pb200h::StarTree::parse / traverse   (StarTreeFilterOperator's traversal as the product runs it)
 //   * pb200h::matching_dict_ids             (PredicateEvaluator resolution: value-space predicate -> dictIds)
 //   * pb200::plan_scan                       (every decision about a scan launch, on segments built from metadata)
+//   * probe_plan_sharing                     (which aggregation's state each aggregation reads, and the count carriers)
 //   * probe_plan_dump                        (every field of a scan, selection or DISTINCT plan as text: plan_diff.py)
 // Built by tests/test_host_logic_cpu.py with g++ against the in-tree library; nothing here ships.
 #include <algorithm>
@@ -263,6 +264,51 @@ int32_t probe_plan_scan(int32_t sm_count, int32_t max_smem_optin, const char* co
       o.seg_leaf_span[s * kMaxLeaves + l] = lf.span; o.seg_leaf_slot[s * kMaxLeaves + l] = lf.slot;
     }
   }
+  return PB200_OK;
+}
+
+// Which aggregation's state each aggregation of a plan reads, and the count carrier of each result
+// (tests/test_mixed_aggs_cpu.py).  Per-aggregation arrays are -1 past their length: mom_first has num_user_aggs entries,
+// the others num_aggs (the caller's aggregations, then the internal moment sums).
+typedef struct {
+  int64_t num_user_aggs, num_aggs, nres;
+  int64_t function[pb200::kMaxAggs], column[pb200::kMaxAggs];
+  int64_t ds_rep[pb200::kMaxAggs], hll_log2m[pb200::kMaxAggs], hll_rep[pb200::kMaxAggs], pct_rep[pb200::kMaxAggs];
+  int64_t mom_first[pb200::kMaxAggs], limb[pb200::kMaxAggs];
+  int64_t carrier_agg[PP_RES];
+} probe_sharing;
+
+int64_t probe_sharing_size(void) { return (int64_t)sizeof(probe_sharing); }
+
+// plan_scan as probe_plan_scan runs it, with the per-aggregation arguments (agg_args: PERCENTILE's p and
+// DISTINCTCOUNTHLL's log2m; wt_args: the time columns of FIRST/LASTWITHTIME; either may be NULL).  Returns its status.
+int32_t probe_plan_sharing(int32_t sm_count, int32_t max_smem_optin, const char* const* knob_names, const int64_t* knob_values,
+                           int32_t nknobs, const pb200_query* query, const double* agg_args, const pb200_agg_arg* wt_args,
+                           const probe_col* cols, int32_t ncols, const int32_t* num_docs, int32_t nseg,
+                           int32_t allow_count_carrier, probe_sharing* out) {
+  using namespace pb200;
+  pb200_ctx ctx;
+  for (int i = 0; i < nknobs; i++) if (int rc = pb200_tuning_set(&ctx, knob_names[i], knob_values[i])) return rc;
+  ProbeSegments ps(cols, ncols, num_docs, nseg);
+  ScanPlan plan;
+  const int rc = plan_scan(ctx.tune, DeviceLimits{sm_count, max_smem_optin}, query, ps.ptrs.data(), nseg, allow_count_carrier != 0,
+                           &plan, agg_args, wt_args);
+  probe_sharing& o = *out;
+  memset(&o, 0, sizeof o);
+  for (int a = 0; a < kMaxAggs; a++) {
+    o.function[a] = o.column[a] = o.ds_rep[a] = o.hll_rep[a] = o.pct_rep[a] = o.mom_first[a] = o.limb[a] = -1;
+    o.hll_log2m[a] = 0;
+  }
+  for (int r = 0; r < PP_RES; r++) o.carrier_agg[r] = -1;
+  if (rc) return rc;
+  o.num_user_aggs = plan.num_user_aggs; o.num_aggs = (int64_t)plan.aggs.size(); o.nres = plan.nres;
+  for (int a = 0; a < (int)plan.aggs.size() && a < kMaxAggs; a++) {
+    o.function[a] = plan.aggs[a].function; o.column[a] = plan.aggs[a].column;
+    o.ds_rep[a] = plan.ds_rep[a]; o.hll_log2m[a] = plan.hll_log2m[a]; o.hll_rep[a] = plan.hll_rep[a];
+    o.pct_rep[a] = plan.pct_rep[a]; o.limb[a] = plan.limb[a];
+  }
+  for (int a = 0; a < plan.num_user_aggs && a < kMaxAggs; a++) o.mom_first[a] = plan.mom_first[a];
+  for (int r = 0; r < (int)plan.tables.size() && r < PP_RES; r++) o.carrier_agg[r] = plan.tables[r].carrier.agg;
   return PB200_OK;
 }
 

@@ -1,22 +1,22 @@
-"""-m gpu: DISTINCTSUM / DISTINCTAVG (and COUNT / SUM / AVG(DISTINCT col)) against a Fraction reference over the doc set of
-tests/filter_ref.py, bit for bit, on every route.
+"""-m gpu: DISTINCTSUM / DISTINCTAVG (and COUNT / SUM / AVG(DISTINCT col)) against the Fraction reference of
+tests/distinct_value_ref.py over the doc set of tests/filter_ref.py, bit for bit, on every route.
 
 Columns: INT at INT_MIN and INT_MAX, LONG near +-2^62, grid FLOAT and DOUBLE (eighths), a raw INT column whose dictionary
 is synthesised at load, and a DATETRUNC derived column.  Routes: aggregation only (an empty filter included), the dense
 table, the spread dense table, the hash table, the scan knobs, 17 segments merged over a domain, ORDER BY ... LIMIT with
 ties, HAVING, one bitset shared with DISTINCTCOUNT.  Every refusal."""
 import math
-from fractions import Fraction
 
 import numpy as np
 import pytest
 
+from distinct_value_ref import distinct_values, ref_final
 from gpu_util import to_device, tuned
 from percentile_ref import group_values
 from pinot_b200 import cli, sql
 from pinot_b200._lib import UnsupportedQueryError
 from pinot_b200.plan_maker import B200Context, B200PlanMaker, DictionaryDomain
-from pinot_b200.query import Aggregation, Predicate, QueryContext, value_key
+from pinot_b200.query import Aggregation, Predicate, QueryContext
 
 pytestmark = pytest.mark.gpu
 
@@ -68,22 +68,6 @@ def seg(oracle, ctx):
 def _query(aggs, flt=None, group_by=(), order_by=(), limit=100_000, **kw):
     return QueryContext(aggregations=list(aggs), filter=flt, group_by=list(group_by), order_by=list(order_by), limit=limit,
                         num_groups_limit=100_000, **kw)
-
-
-def distinct_values(values):
-    """The distinct stored values: integers exactly, floats by identity (ValueKey: -0.0 and 0.0 apart, one NaN)."""
-    return {value_key(v) for v in (x.item() if hasattr(x, "item") else x for x in values)}
-
-
-def ref_final(fn, values):
-    """The exact reference: the distinct stored values summed as Fractions, rounded once."""
-    s = distinct_values(values)
-    if fn == "DISTINCTCOUNT":
-        return float(len(s))
-    if not s:
-        return 0.0 if fn == "DISTINCTSUM" else -math.inf
-    total = sum((Fraction(v) for v in s), Fraction(0))
-    return float(total / len(s) if fn == "DISTINCTAVG" else total)
 
 
 def _key_of(data, group_by, keys_row):
