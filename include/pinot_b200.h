@@ -259,9 +259,10 @@ int32_t pb200_execute(pb200_ctx* ctx, const pb200_query* query, pb200_segment* c
  * an ordered result come back in that order, and only the first trim_size of them (trim_size <= 0: all, sorted).  The
  * numGroupsLimit check applies to the untrimmed group count; num_groups is the number of rows kept. */
 #define PB200_MAX_ORDER_BY 8
-enum { PB200_ORDER_AGG = 0, PB200_ORDER_GROUP_BY = 1 };
+enum { PB200_ORDER_AGG = 0, PB200_ORDER_GROUP_BY = 1, PB200_ORDER_POST = 2 };
 typedef struct {
-  int32_t kind;       /* PB200_ORDER_AGG: index into pb200_query.aggs; PB200_ORDER_GROUP_BY: index into group_by_columns */
+  int32_t kind;       /* PB200_ORDER_AGG: index into pb200_query.aggs; PB200_ORDER_GROUP_BY: index into group_by_columns;
+                         PB200_ORDER_POST: index into pb200_post_aggs.programs (pb200_execute_post only) */
   int32_t index;
   int32_t descending; /* 0: ASC, else DESC */
 } pb200_order_item;
@@ -356,6 +357,41 @@ typedef struct {
 int32_t pb200_execute_agg_args(pb200_ctx* ctx, const pb200_query* query, const pb200_order_by* order, const pb200_agg_arg* args,
                                const pb200_having* having, pb200_segment* const* segments, int32_t num_segments,
                                pb200_result** results);
+/* ---- ORDER BY arithmetic over aggregations: SUM(a) / SUM(b), COUNT(*) * 100.0 / SUM(n) (DESIGN.md section 3.18) ----- */
+/* A post-aggregation program is POSTFIX (root last) over the FINAL values of a row's aggregations: AGG pushes the final
+ * value of aggregation `agg` (index into pb200_query.aggs) as a double -- COUNT / DISTINCTCOUNT the count, AVG sum / count
+ * (-inf at count 0), the other functions their double column, as HAVING reads them; LITERAL pushes `value` (finite);
+ * ADD, SUB, MUL, DIV pop two operands and push one IEEE-754 double operation rounded to nearest (never an FMA; x / 0 is
+ * +-inf, 0 / 0 NaN); NEG flips the sign of the top operand.  A PB200_ORDER_POST item orders rows by its program's value in
+ * Double.compare order (-0.0 before 0.0, every NaN one value after +inf); ties, trim and numGroupsLimit as for the other
+ * items. */
+#define PB200_MAX_POST_NODES 16
+enum { PB200_POST_AGG = 0, PB200_POST_LITERAL = 1, PB200_POST_ADD = 2, PB200_POST_SUB = 3, PB200_POST_MUL = 4,
+       PB200_POST_DIV = 5, PB200_POST_NEG = 6 };
+typedef struct {
+  int32_t op;           /* PB200_POST_* */
+  int32_t agg;          /* AGG: index into pb200_query.aggs */
+  double value;         /* LITERAL: the literal */
+} pb200_post_node;
+typedef struct {
+  int32_t num_nodes;    /* 1 .. PB200_MAX_POST_NODES */
+  int32_t reserved;
+  pb200_post_node nodes[PB200_MAX_POST_NODES];
+} pb200_post_program;
+typedef struct {
+  int32_t num_programs; /* 0 .. PB200_MAX_ORDER_BY */
+  int32_t reserved;
+  pb200_post_program programs[PB200_MAX_ORDER_BY];
+} pb200_post_aggs;
+/* pb200_execute_agg_args whose ORDER BY may name programs of `post` (post == NULL: exactly pb200_execute_agg_args).  A
+ * PB200_Q_DEFER_FINALIZE result keeps the programs with its order spec for pb200_result_finalize / pb200_result_combine.
+ * PB200_E_INVALID: a malformed program (unknown op, an aggregation index out of range, a stack that does not end with one
+ * value, a non-finite literal, num_nodes outside 1..16), num_programs outside 0..8, a PB200_ORDER_POST index past
+ * num_programs.  PB200_E_UNSUPPORTED: a DISTINCTCOUNT operand without per-group sets, a STRING-typed *WITHTIME operand. */
+int32_t pb200_execute_post(pb200_ctx* ctx, const pb200_query* query, const pb200_order_by* order, const pb200_agg_arg* args,
+                           const pb200_having* having, const pb200_post_aggs* post, pb200_segment* const* segments,
+                           int32_t num_segments, pb200_result** results);
+
 /* The histogram behind PERCENTILE aggregation `agg` in row `row`: its non-zero bins ascending by dictId (counts > 0), the
  * intermediate for merging per-segment results by value (the analogue of pb200_result_distinct).  Returns the number of
  * bins (or < 0 on error) and writes at most `capacity` of them; either output may be NULL.  The histograms are copied from

@@ -238,6 +238,13 @@ typedef struct {
 int32_t pb200h_execute_agg_args(pb200_ctx* ctx, const pb200h_query* query, const pb200_order_by* order, const pb200h_agg_arg* args,
                                 const pb200_having* having, pb200h_segment* const* segments, int32_t num_segments,
                                 pb200_result** results, int32_t* operator_kinds);
+/* pb200h_execute_agg_args whose ORDER BY may name post-aggregation programs (pb200_execute_post of include/pinot_b200.h;
+ * operands index query->aggs).  post == NULL: exactly pb200h_execute_agg_args.  Device results are ordered on the device;
+ * star-tree results and the aligned results of FILTER clauses on the host, by the same evaluator.  The same errors as
+ * pb200_execute_post. */
+int32_t pb200h_execute_post(pb200_ctx* ctx, const pb200h_query* query, const pb200_order_by* order, const pb200h_agg_arg* args,
+                            const pb200_having* having, const pb200_post_aggs* post, pb200h_segment* const* segments,
+                            int32_t num_segments, pb200_result** results, int32_t* operator_kinds);
 /* DISTINCTCOUNTHLL (the DISTINCTCOUNTHLL section of include/pinot_b200.h) through every entry point above, with the same
  * refusals.  A segment whose filter matches every doc is answered without a scan (PB200H_OP_NON_SCAN_AGGREGATION, as the
  * reference's NonScanBasedAggregationOperator does): the estimate over the whole dictionary, computed by the device

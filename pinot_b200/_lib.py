@@ -118,7 +118,7 @@ class HQuery(C.Structure):
 
 
 MAX_ORDER_BY = 8
-ORDER_AGG, ORDER_GROUP_BY = 0, 1
+ORDER_AGG, ORDER_GROUP_BY, ORDER_POST = 0, 1, 2
 
 
 class OrderItem(C.Structure):
@@ -141,6 +141,22 @@ class HavingNode(C.Structure):
 
 class Having(C.Structure):
     _fields_ = [("num_nodes", C.c_int32), ("reserved", C.c_int32), ("nodes", HavingNode * MAX_HAVING_NODES)]
+
+
+MAX_POST_NODES = 16
+POST_CODES = {"AGG": 0, "LIT": 1, "ADD": 2, "SUB": 3, "MUL": 4, "DIV": 5, "NEG": 6}   # PB200_POST_*
+
+
+class PostNode(C.Structure):  # pb200_post_node
+    _fields_ = [("op", C.c_int32), ("agg", C.c_int32), ("value", C.c_double)]
+
+
+class PostProgram(C.Structure):  # pb200_post_program
+    _fields_ = [("num_nodes", C.c_int32), ("reserved", C.c_int32), ("nodes", PostNode * MAX_POST_NODES)]
+
+
+class PostAggs(C.Structure):  # pb200_post_aggs
+    _fields_ = [("num_programs", C.c_int32), ("reserved", C.c_int32), ("programs", PostProgram * MAX_ORDER_BY)]
 
 
 class SelectOrder(C.Structure):
@@ -222,6 +238,7 @@ EXPORTED_SYMBOLS = [
     "pb200h_startree_build", "pb200h_startree_get",
     "pb200_execute_having", "pb200h_execute_having", "pb200_execute_agg_args", "pb200h_execute_agg_args",
     "pb200_match_pattern", "pb200_result_exact_sum", "pb200_execute_exprs", "pb200_expr_doc_masks",
+    "pb200_execute_post", "pb200h_execute_post",
 ]
 
 _LIB = None
@@ -255,6 +272,8 @@ def load() -> C.CDLL:
                                          C.POINTER(vp), i32, C.POINTER(vp)]
     L.pb200_execute_exprs.argtypes = [vp, C.POINTER(Query), C.POINTER(OrderBy), C.POINTER(AggArg), C.POINTER(Having),
                                       C.POINTER(ExprProgram), C.POINTER(vp), i32, C.POINTER(vp)]
+    L.pb200_execute_post.argtypes = [vp, C.POINTER(Query), C.POINTER(OrderBy), C.POINTER(AggArg), C.POINTER(Having),
+                                     C.POINTER(PostAggs), C.POINTER(vp), i32, C.POINTER(vp)]
     L.pb200_expr_doc_masks.argtypes = [vp, i32, C.POINTER(ExprPredicate), C.POINTER(vp), i32, C.POINTER(vp)]
     L.pb200_result_histogram.restype = i64
     L.pb200_result_histogram.argtypes = [vp, i32, i32, vp, vp, i64]
@@ -296,6 +315,8 @@ def load() -> C.CDLL:
                                         C.POINTER(vp), i32, C.POINTER(vp), C.POINTER(i32)]
     L.pb200h_execute_agg_args.argtypes = [vp, C.POINTER(HQuery), C.POINTER(OrderBy), C.POINTER(HAggArg), C.POINTER(Having),
                                           C.POINTER(vp), i32, C.POINTER(vp), C.POINTER(i32)]
+    L.pb200h_execute_post.argtypes = [vp, C.POINTER(HQuery), C.POINTER(OrderBy), C.POINTER(HAggArg), C.POINTER(Having),
+                                      C.POINTER(PostAggs), C.POINTER(vp), i32, C.POINTER(vp), C.POINTER(i32)]
     L.pb200h_explain.argtypes = [vp, C.POINTER(HQuery), vp, C.c_char_p, i32]
     L.pb200h_startree_attach.argtypes = [vp, vp, vp, C.c_uint64, i32, i32, C.POINTER(C.c_char_p), C.POINTER(vp),
                                          C.POINTER(C.c_uint64), i32, C.POINTER(HStarMetric)]

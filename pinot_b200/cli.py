@@ -8,7 +8,7 @@ and dictionary-encoded at load, star-trees attached), ``pb200h_execute`` over al
 reference's combine + broker reduce do, in a few lines of Python -- the per-segment results blocks are merged by key VALUES
 (``AggregationFunction.merge``), final results extracted (AVG = sum / count, DISTINCTCOUNT = set size, DISTINCTSUM /
 DISTINCTAVG = the set's exact sum / mean rounded once, DISTINCTCOUNTHLL = the set's estimate), filtered by HAVING,
-ordered, and the first LIMIT rows printed.  With ``--merge-on-device`` the segments are first bound to one dictionary domain
+expressions over aggregations computed, ordered, and the first LIMIT rows printed.  With ``--merge-on-device`` the segments are first bound to one dictionary domain
 and combined on the GPU, where HAVING, ORDER BY and the trim run too.
 
 Needs a GPU: the product has no CPU fallback.  Queries outside the accelerated set exit with the library's message (a Pinot
@@ -93,14 +93,29 @@ def merge_blocks(query, segments, blocks) -> Dict[tuple, list]:
     return out
 
 
+def output_columns(query) -> List[tuple]:
+    """(header, position) of each printed column; positions index a row of key values, then the final value of every
+    aggregation, then the value of every post-aggregation expression.  A query with expressions over aggregations prints
+    its SELECT list in its order; the others print the GROUP BY columns, then their aggregations.  Hidden aggregations
+    (named only in HAVING or in expressions) are never printed."""
+    k, m = len(query.group_by), len(query.aggregations)
+    if query.post_aggregations:
+        at = {"COLUMN": lambda c: query.group_by.index(c), "AGG": lambda a: k + a, "POST": lambda i: k + m + i}
+        names = {"COLUMN": str, "AGG": lambda a: str(query.aggregations[a]), "POST": lambda i: str(query.post_aggregations[i])}
+        return [(names[kind](x), at[kind](x)) for kind, x in query.select]
+    return ([(c, j) for j, c in enumerate(query.group_by)] +
+            [(str(a), k + j) for j, a in enumerate(query.aggregations) if not a.hidden])
+
+
 def final_rows(query, table: Dict[tuple, list]) -> List[list]:
     """Broker-side extraction of final results + HAVING + ORDER BY + LIMIT.  HAVING keeps the rows whose final values pass
-    it (Java's comparisons: query.having_eval).  ORDER BY compares final values (AVG = sum / count, DISTINCTCOUNT = set
-    size) and breaks ties by the key values ascending, in GROUP BY column order -- the library's order.  Without ORDER BY
-    Pinot returns an arbitrary LIMIT-sized subset; here the rows are sorted by key to make the output stable.  Hidden
-    aggregations (named only in HAVING) are left out of the rows."""
+    it (Java's comparisons: query.having_eval).  Expressions over aggregations are computed from the final values as
+    Python floats, one IEEE-754 operation per operator (query.post_eval).  ORDER BY compares final values (AVG = sum /
+    count, DISTINCTCOUNT = set size) or expression values and breaks ties by the key values ascending, in GROUP BY column
+    order -- the library's order.  Without ORDER BY Pinot returns an arbitrary LIMIT-sized subset; here the rows are sorted
+    by key to make the output stable.  Rows hold the columns of output_columns."""
     from .query import (DISTINCT_SET_FUNCTIONS, MOMENT_FUNCTIONS, distinct_final, having_eval, hll_final, moments_final, percentile_of_counts,
-                        value_order)
+                        post_eval, value_order)
     from .sql import resolve_having, resolve_order_by
     items = resolve_order_by(query) if query.is_group_by else []
     having = resolve_having(query)
@@ -127,12 +142,13 @@ def final_rows(query, table: Dict[tuple, list]) -> List[list]:
         # refuses that), so it stands in as -inf, the value the device compares for it when empty
         if having and not having_eval(having, [float("-inf") if isinstance(x, (bytes, str)) else float(x) for x in vals]):
             continue
-        rows.append(list(key) + vals)
-    k = len(query.group_by)
+        posts = [post_eval(p.program, lambda a: float(vals[a])) for p in query.post_aggregations]
+        rows.append(list(key) + vals + posts)
+    k, m = len(query.group_by), len(query.aggregations)
     for kind, index, asc in reversed(items):  # stable passes, last item first
-        col = index if kind == "GROUP_BY" else k + index
+        col = index if kind == "GROUP_BY" else k + index if kind == "AGG" else k + m + index
         rows.sort(key=lambda r: value_order(r[col]), reverse=not asc)
-    shown = list(range(k)) + [k + a for a, agg in enumerate(query.aggregations) if not agg.hidden]
+    shown = [c for _, c in output_columns(query)]
     return [[r[c] for c in shown] for r in rows[: query.limit]]
 
 
@@ -189,7 +205,7 @@ def main(argv=None) -> int:
             sys.stderr.write(f"{e}\n")
             return 2
         rows = final_rows(query, table)
-        names = list(query.group_by) + [str(a) for a in query.aggregations if not a.hidden]
+        names = [name for name, _ in output_columns(query)]
         stats = {"numDocsScanned": sum(b.stats.num_docs_scanned for b in blocks), "totalDocs": sum(s.num_docs for s in segments),
                  "numSegments": len(segments), "deviceMs": round(sum(b.device_ms for b in blocks[:1]), 4),
                  "operators": sorted({b.operator_kind for b in blocks})}

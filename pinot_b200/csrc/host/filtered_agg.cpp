@@ -43,7 +43,7 @@ struct ResultGuard {
 }  // namespace
 
 int execute_filtered(pb200_ctx* ctx, const pb200h_query& q, const pb200_order_by* order, const pb200_having* having,
-                     pb200h_segment* const* segs, int nseg, pb200_result** results, int32_t* kinds) {
+                     const pb200_post_aggs* post, pb200h_segment* const* segs, int nseg, pb200_result** results, int32_t* kinds) {
   if (q.merge_segments == 2) { set_error("FILTER clauses with a deferred (cross-GPU) combine are not accelerated"); return PB200_E_UNSUPPORTED; }
   const int nagg = q.num_aggs, ngb = q.num_group_by;
   const int nres = q.merge_segments ? 1 : nseg;
@@ -174,7 +174,7 @@ int execute_filtered(pb200_ctx* ctx, const pb200h_query& q, const pb200_order_by
     // HAVING and ORDER BY: the infos ran unfiltered and unordered (each holds partial columns, and a trimmed info could miss
     // a group of the main filter); the aligned rows are filtered, ordered and trimmed here, by the device's rules
     if (having && ngb > 0) pb200::having_rows_host(R.get(), *having, R->agg_functions.data());
-    if (order && ngb > 0) pb200::order_rows_host(R.get(), *order, R->agg_functions.data());
+    if (order && ngb > 0) pb200::order_rows_host(R.get(), *order, R->agg_functions.data(), post);
     aligned[r] = std::move(R);
   }
   for (int r = 0; r < nres; r++) results[r] = aligned[r].release();  // only when every result was built

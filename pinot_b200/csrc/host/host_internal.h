@@ -200,7 +200,7 @@ bool synthesize_dictionary(const std::vector<unsigned char>& values_be, int data
                            std::vector<unsigned char>& dict_be, std::vector<unsigned char>& fwd_packed, int* cardinality, int* bits);
 // filtered_agg.cpp: FILTER (WHERE ...) clauses = one device submission per distinct clause, aligned by group key
 int execute_filtered(pb200_ctx* ctx, const pb200h_query& q, const pb200_order_by* order, const pb200_having* having,
-                     pb200h_segment* const* segs, int nseg, pb200_result** results, int32_t* kinds);
+                     const pb200_post_aggs* post, pb200h_segment* const* segs, int nseg, pb200_result** results, int32_t* kinds);
 // ids[] storage that must outlive the pb200_execute call
 struct SegmentFilterStore { std::vector<std::unique_ptr<std::vector<int32_t>>> ids; };
 // PredicateEvaluator.getMatchingDictIds (sorted) of one predicate on a dictionary column

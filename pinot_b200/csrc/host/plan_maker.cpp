@@ -822,9 +822,15 @@ extern "C" int32_t pb200h_execute_having(pb200_ctx* ctx, const pb200h_query* q, 
 extern "C" int32_t pb200h_execute_agg_args(pb200_ctx* ctx, const pb200h_query* q, const pb200_order_by* order, const pb200h_agg_arg* args,
                                            const pb200_having* having, pb200h_segment* const* segs, int32_t nseg,
                                            pb200_result** results, int32_t* kinds) {
+  return pb200h_execute_post(ctx, q, order, args, having, nullptr, segs, nseg, results, kinds);
+}
+
+extern "C" int32_t pb200h_execute_post(pb200_ctx* ctx, const pb200h_query* q, const pb200_order_by* order, const pb200h_agg_arg* args,
+                                       const pb200_having* having, const pb200_post_aggs* post, pb200h_segment* const* segs,
+                                       int32_t nseg, pb200_result** results, int32_t* kinds) {
   if (!ctx || !q || !segs || !results || nseg <= 0) { set_error("invalid argument to pb200h_execute"); return PB200_E_INVALID; }
   if (q->num_aggs <= 0) { set_error("selection queries are outside this path"); return PB200_E_UNSUPPORTED; }
-  if (int vrc = pb200::order_validate(order, q->num_aggs, q->num_group_by)) return vrc;
+  if (int vrc = pb200::order_validate(order, q->num_aggs, q->num_group_by, post)) return vrc;
   if (int hrc = pb200::having_check(having, q->num_aggs, q->num_group_by, q->merge_segments ? 1 : nseg,
                                     q->merge_segments == 2 || q->reduce_world > 1))
     return hrc;
@@ -861,7 +867,7 @@ extern "C" int32_t pb200h_execute_agg_args(pb200_ctx* ctx, const pb200h_query* q
   if (int rc = resolve_expr_filters(ctx, *q, segs, nseg, expr_filters, true)) return rc;
   if (q->agg_filter_count && q->agg_filter_start && q->agg_filter_nodes)
     for (int a = 0; a < q->num_aggs; a++)
-      if (q->agg_filter_count[a] > 0) return execute_filtered(ctx, *q, order, having, segs, nseg, results, kinds);  // host/filtered_agg.cpp
+      if (q->agg_filter_count[a] > 0) return execute_filtered(ctx, *q, order, having, post, segs, nseg, results, kinds);  // host/filtered_agg.cpp
   const bool merge = q->merge_segments != 0;
   // resolve columns by name against segment 0 (all segments of a table share the schema)
   const pb200h_segment& s0 = *segs[0];
@@ -952,7 +958,7 @@ extern "C" int32_t pb200h_execute_agg_args(pb200_ctx* ctx, const pb200h_query* q
           std::vector<int32_t> fns(q->num_aggs);
           for (int a = 0; a < q->num_aggs; a++) fns[a] = q->aggs[a].function;
           if (having) pb200::having_rows_host(star_results[s], *having, fns.data());
-          if (order) pb200::order_rows_host(star_results[s], *order, fns.data());
+          if (order) pb200::order_rows_host(star_results[s], *order, fns.data(), post);
           break;
         }
       }
@@ -981,8 +987,8 @@ extern "C" int32_t pb200h_execute_agg_args(pb200_ctx* ctx, const pb200h_query* q
     dq.filter = flat.data();
     dq.group_by_columns = gb.data();
     dq.aggs = aggs.data();
-    int rc = any_expr ? pb200_execute_exprs(ctx, &dq, order, args ? dev_args.data() : nullptr, having, programs.data(), dsegs.data(), (int)dsegs.size(), dev_results.data())
-                      : pb200_execute_agg_args(ctx, &dq, order, args ? dev_args.data() : nullptr, having, dsegs.data(), (int)dsegs.size(), dev_results.data());
+    int rc = pb200::execute_exprs_post(ctx, &dq, order, args ? dev_args.data() : nullptr, having, any_expr ? programs.data() : nullptr, post,
+                                       dsegs.data(), (int)dsegs.size(), dev_results.data());
     if (rc) { for (auto r : star_results) if (r) pb200_result_free(r); return rc; }
     // the mask pass of each expression leaf read its leaf columns at every doc of the segment
     for (size_t k = 0; k < dev_idx.size(); k++) dev_results[merge ? 0 : k]->meta.num_entries_scanned_in_filter += expr_filter_entries(*segs[dev_idx[k]], *q);

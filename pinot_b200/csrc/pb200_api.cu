@@ -706,10 +706,11 @@ int launch_chunks(pb200_ctx* ctx, cudaStream_t st, const ScanPlan& plan, DevBufR
 constexpr int kRetryWithoutCountCarrier = 1;
 static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment* const* segments, int32_t nseg,
                         pb200_result** results, bool allow_count_carrier, const pb200_order_by* order, const double* agg_args,
-                        const pb200_having* having, const pb200_agg_arg* wt_args, const ExprCall* ex = nullptr);
+                        const pb200_having* having, const pb200_agg_arg* wt_args, const ExprCall* ex = nullptr,
+                        const pb200_post_aggs* post = nullptr);
 static int execute_checked(pb200_ctx* ctx, const pb200_query* query, const pb200_order_by* order, const pb200_agg_arg* args,
                            const pb200_having* having, pb200_segment* const* segments, int32_t nseg, pb200_result** results,
-                           const ExprCall* ex);
+                           const ExprCall* ex, const pb200_post_aggs* post = nullptr);
 
 extern "C" int32_t pb200_execute_having(pb200_ctx* ctx, const pb200_query* query, const pb200_order_by* order, const double* agg_args,
                                         const pb200_having* having, pb200_segment* const* segments, int32_t nseg,
@@ -733,28 +734,52 @@ extern "C" int32_t pb200_execute_agg_args(pb200_ctx* ctx, const pb200_query* que
   return execute_checked(ctx, query, order, args, having, segments, nseg, results, nullptr);
 }
 
-extern "C" int32_t pb200_execute_exprs(pb200_ctx* ctx, const pb200_query* query, const pb200_order_by* order, const pb200_agg_arg* args,
-                                       const pb200_having* having, const pb200_expr_program* exprs, pb200_segment* const* segments,
-                                       int32_t nseg, pb200_result** results) {
-  if (!exprs) return pb200_execute_agg_args(ctx, query, order, args, having, segments, nseg, results);
-  if (!ctx || !results) { set_error("invalid argument to pb200_execute_exprs"); return PB200_E_INVALID; }
+int pb200::execute_exprs_post(pb200_ctx* ctx, const pb200_query* query, const pb200_order_by* order, const pb200_agg_arg* args,
+                              const pb200_having* having, const pb200_expr_program* exprs, const pb200_post_aggs* post,
+                              pb200_segment* const* segments, int32_t nseg, pb200_result** results) {
+  if (!exprs && !post) return pb200_execute_agg_args(ctx, query, order, args, having, segments, nseg, results);
+  if (!ctx || !results) { set_error("invalid argument to %s", exprs ? "pb200_execute_exprs" : "pb200_execute_post"); return PB200_E_INVALID; }
+  if (post && (!query || query->num_aggs < 0 || (query->num_aggs > 0 && !query->aggs))) {
+    set_error("invalid query passed to pb200_execute_post");
+    return PB200_E_INVALID;
+  }
+  if (post && query->num_aggs > kMaxAggs) {   // as the scan planner refuses it: the stock operator runs the query
+    set_error("query exceeds device limits (aggs %d/%d)", query->num_aggs, kMaxAggs);
+    return PB200_E_UNSUPPORTED;
+  }
   ExprCall ex;
-  if (const int rc = expr_prepare(query, exprs, segments, nseg, &ex)) return rc;
-  if (!ex.count) return pb200_execute_agg_args(ctx, query, order, args, having, segments, nseg, results);
+  if (exprs)
+    if (const int rc = expr_prepare(query, exprs, segments, nseg, &ex)) return rc;
+  if (!ex.count)
+    return post ? execute_checked(ctx, query, order, args, having, segments, nseg, results, nullptr, post)
+                : pb200_execute_agg_args(ctx, query, order, args, having, segments, nseg, results);
   // the scan runs every expression aggregation as COUNT(*): its group tables and counts are what the expressions need
   pb200_query q = *query;
   pb200_agg aggs[kMaxAggs];
   for (int a = 0; a < q.num_aggs; a++) aggs[a] = ex.fn_of[a] >= 0 ? pb200_agg{PB200_AGG_COUNT, -1} : query->aggs[a];
   q.aggs = aggs;
-  return execute_checked(ctx, &q, order, args, having, segments, nseg, results, &ex);
+  return execute_checked(ctx, &q, order, args, having, segments, nseg, results, &ex, post);
+}
+
+extern "C" int32_t pb200_execute_exprs(pb200_ctx* ctx, const pb200_query* query, const pb200_order_by* order, const pb200_agg_arg* args,
+                                       const pb200_having* having, const pb200_expr_program* exprs, pb200_segment* const* segments,
+                                       int32_t nseg, pb200_result** results) {
+  return pb200::execute_exprs_post(ctx, query, order, args, having, exprs, nullptr, segments, nseg, results);
+}
+
+extern "C" int32_t pb200_execute_post(pb200_ctx* ctx, const pb200_query* query, const pb200_order_by* order, const pb200_agg_arg* args,
+                                      const pb200_having* having, const pb200_post_aggs* post, pb200_segment* const* segments,
+                                      int32_t nseg, pb200_result** results) {
+  return pb200::execute_exprs_post(ctx, query, order, args, having, nullptr, post, segments, nseg, results);
 }
 
 // pb200_execute_agg_args past its argument check (args NULL: no percentiles and no *WITHTIME), with the expression
-// aggregations of pb200_execute_exprs (ex NULL: none)
+// aggregations of pb200_execute_exprs (ex NULL: none) and the post-aggregation programs of pb200_execute_post (post NULL:
+// none)
 static int execute_checked(pb200_ctx* ctx, const pb200_query* query, const pb200_order_by* order, const pb200_agg_arg* args,
                            const pb200_having* having, pb200_segment* const* segments, int32_t nseg, pb200_result** results,
-                           const ExprCall* ex) {
-  if (const int vrc = order_validate(order, query->num_aggs, query->num_group_by)) return vrc;
+                           const ExprCall* ex, const pb200_post_aggs* post) {
+  if (const int vrc = order_validate(order, query->num_aggs, query->num_group_by, post)) return vrc;
   const int nres = (query->flags & PB200_Q_MERGE_SEGMENTS) ? 1 : nseg;
   const bool deferred = (query->flags & PB200_Q_DEFER_FINALIZE) || query->reduce_world > 1;
   if (const int hrc = having_check(having, query->num_aggs, query->num_group_by, nres, deferred)) return hrc;
@@ -769,6 +794,14 @@ static int execute_checked(pb200_ctx* ctx, const pb200_query* query, const pb200
       if (order->items[i].kind == PB200_ORDER_AGG && string_wt(order->items[i].index)) {
         set_error("ORDER BY a STRING FIRST/LASTWITHTIME is not accelerated"); return PB200_E_UNSUPPORTED;
       }
+    for (int i = 0; order && post && i < order->num_items; i++) {
+      if (order->items[i].kind != PB200_ORDER_POST) continue;
+      const pb200_post_program& pp = post->programs[order->items[i].index];
+      for (int k = 0; k < pp.num_nodes; k++)
+        if (pp.nodes[k].op == PB200_POST_AGG && string_wt(pp.nodes[k].agg)) {
+          set_error("ORDER BY an expression over a STRING FIRST/LASTWITHTIME is not accelerated"); return PB200_E_UNSUPPORTED;
+        }
+    }
     for (int i = 0; having && i < having->num_nodes; i++) {
       const pb200_having_node& hn = having->nodes[i];
       if ((hn.op == PB200_HAVING_RANGE || hn.op == PB200_HAVING_EQ || hn.op == PB200_HAVING_NEQ) && string_wt(hn.agg)) {
@@ -780,8 +813,8 @@ static int execute_checked(pb200_ctx* ctx, const pb200_query* query, const pb200
   for (int a = 0; args && a < query->num_aggs; a++) p[a] = args[a].p;
   const double* agg_args = args ? p : nullptr;
   // a retry rebuilds every table of the attempt, the expression tables included
-  int rc = execute_impl(ctx, query, segments, nseg, results, true, order, agg_args, having, args, ex);
-  if (rc == kRetryWithoutCountCarrier) rc = execute_impl(ctx, query, segments, nseg, results, false, order, agg_args, having, args, ex);
+  int rc = execute_impl(ctx, query, segments, nseg, results, true, order, agg_args, having, args, ex, post);
+  if (rc == kRetryWithoutCountCarrier) rc = execute_impl(ctx, query, segments, nseg, results, false, order, agg_args, having, args, ex, post);
   return rc;
 }
 
@@ -1280,7 +1313,7 @@ struct ScanCall {
 
   // 11. every result's metadata and (aggregation only) its row, then the group-by rows extracted, or left for
   //     pb200_result_finalize (deferred); per-segment results release their tables
-  int fill_results_and_extract(const pb200_order_by* order, const pb200_having* having) {
+  int fill_results_and_extract(const pb200_order_by* order, const pb200_having* having, const pb200_post_aggs* post) {
     const int nuser = plan.num_user_aggs;
     const float ms = ev.ms();
     for (int r = 0; r < plan.nres; r++) {
@@ -1305,6 +1338,7 @@ struct ScanCall {
         R.meta.reserved = (R.dense.pack_agg >= 0 ? 1 : 0) | (R.dense.carrier_unsafe ? 2 : 0) | (R.dense.flag_slot ? 4 : 0);  // include/pinot_b200.h
         if (order) R.order = *order;   // a deferred result keeps it for its extraction
         if (having) R.having = *having;
+        if (post) R.post = *post;
         continue;
       }
       R.meta.num_groups = -1;
@@ -1367,7 +1401,8 @@ struct ScanCall {
 
 static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment* const* segments, int32_t nseg,
                         pb200_result** results, bool allow_count_carrier, const pb200_order_by* order, const double* agg_args,
-                        const pb200_having* having, const pb200_agg_arg* wt_args, const ExprCall* ex) {
+                        const pb200_having* having, const pb200_agg_arg* wt_args, const ExprCall* ex,
+                        const pb200_post_aggs* post) {
   ScanCall c{ctx, query, segments, nseg};
   c.ex = ex;
   if (int rc = c.check_call(results)) return rc;
@@ -1381,7 +1416,7 @@ static int execute_impl(pb200_ctx* ctx, const pb200_query* query, pb200_segment*
   if (int rc = c.finalize_sets()) return rc;
   if (int rc = c.finalize_exprs()) return rc;
   if (int rc = c.read_back_and_verify()) return rc;   // kRetryWithoutCountCarrier: ~ScanCall frees this attempt's tables
-  if (int rc = c.fill_results_and_extract(order, having)) return rc;
+  if (int rc = c.fill_results_and_extract(order, having, post)) return rc;
   c.hand_out(results);
   return PB200_OK;
 }

@@ -19,7 +19,8 @@
 // compacts its non-empty entries into an index array (index-only mode), a key kernel turns each row into one u64 key per
 // pass, stable LSD radix sorts order the index by the group-key tie key first and then by the items from last to first, and
 // the write kernel writes row r from entry idx[r] for r < min(groups, trim_size).  The block is sized for the trimmed rows,
-// so a trimmed result stays on the one-synchronisation path.
+// so a trimmed result stays on the one-synchronisation path.  A PB200_ORDER_POST item's pass evaluates its program
+// (pb200_postagg.h) over the row's final values and keys the result in Double.compare order.
 // A result with a HAVING tree (pb200_having, pb200_having.h) takes one step before count: a keep kernel evaluates the tree
 // on every existing entry's final values and writes a keep bitmap (1 bit per entry, one byte per 8 consecutive entries)
 // plus the number of existing entries, which the numGroupsLimit check uses.  Count and write (also index-only) then test
@@ -35,6 +36,7 @@
 #include "pb200_decode.h"
 #include "pb200_having.h"
 #include "pb200_order.h"
+#include "pb200_postagg.h"
 
 namespace pb200 {
 
@@ -145,6 +147,17 @@ __device__ __forceinline__ long long distinct_size(const ExtractDesc& d, int a, 
   return n;
 }
 
+// final value of aggregation a in entry g as HAVING and post-aggregation programs read it (having_value); cnt = the
+// entry's group count
+__device__ __forceinline__ double final_value(const ExtractDesc& d, int a, long long g, unsigned long long cnt) {
+  if (d.agg[a].fn == PB200_AGG_DISTINCTCOUNT) return (double)distinct_size(d, a, g);
+  double dv;
+  long long lv;
+  int32_t id;
+  agg_values(d.agg[a], g, cnt, dv, lv, id, nullptr);
+  return having_value(d.agg[a].fn, dv, lv);
+}
+
 __device__ __forceinline__ unsigned long long raw_key_of(const ExtractDesc& d, long long g) {
   return d.hkeys ? d.hkeys[g] : (unsigned long long)g / (unsigned)d.stride;
 }
@@ -211,13 +224,14 @@ __global__ void __launch_bounds__(kExtractThreads) extract_write_kernel(const Ex
 }
 
 // One sort pass of an ordered result: which key, how many of its bits are in use (pb200_order.h)
-enum { PASS_TIE = 0, PASS_GROUP_BY = 1, PASS_AGG = 2 };
+enum { PASS_TIE = 0, PASS_GROUP_BY = 1, PASS_AGG = 2, PASS_POST = 3 };
 struct OrderPass {
   int32_t what, index;   // PASS_GROUP_BY: group-by column; PASS_AGG: aggregation
   int32_t cmp;           // OrderCmp of an aggregation
   int32_t descending;
   int32_t bits;
   unsigned long long mask;  // (1 << bits) - 1: the key of a padding row (past the group count: sorts last, stays last)
+  pb200_post_program prog;  // PASS_POST: the item's program
 };
 
 // keys[i] = the pass's key of row i of the current order idx[], for all idx_cap rows
@@ -243,6 +257,9 @@ __global__ void __launch_bounds__(kExtractThreads) order_key_kernel(const Extrac
         agg_values(d.agg[p.index], g, group_count(d, g), dv, lv, id, nullptr);
       }
       k = order_key(p.cmp, p.descending != 0, p.mask, dv, lv);
+    } else if (p.what == PASS_POST) {
+      const unsigned long long cnt = group_count(d, g);
+      k = order_key(ORDER_CMP_DOUBLE, p.descending != 0, p.mask, postagg_eval(p.prog, [&](int a) { return final_value(d, a, g, cnt); }), 0);
     } else {
       // raw key: column 0 least significant; tie key: column 0 most significant (= ascending key values in GROUP BY order)
       unsigned long long raw = raw_key_of(d, g), tie = 0, id = 0;
@@ -274,14 +291,7 @@ __global__ void __launch_bounds__(kExtractThreads) having_kernel(const ExtractDe
     if (!((flags >> j) & 1u)) continue;
     const long long g = base + j;
     const unsigned long long cnt = group_count(d, g);
-    const bool pass = having_eval(h, [&](int a) -> double {
-      if (d.agg[a].fn == PB200_AGG_DISTINCTCOUNT) return (double)distinct_size(d, a, g);
-      double dv;
-      long long lv;
-      int32_t id;
-      agg_values(d.agg[a], g, cnt, dv, lv, id, nullptr);
-      return having_value(d.agg[a].fn, dv, lv);
-    });
+    const bool pass = having_eval(h, [&](int a) { return final_value(d, a, g, cnt); });
     if (!pass) flags &= ~(1u << j);
   }
   keep[base >> 3] = (uint8_t)flags;
@@ -327,7 +337,7 @@ static int bits_for(unsigned long long max_value) {
 
 // The sort passes of an ordered result in the order they run: stable LSD, so the tie key first, then the items from last
 // to first.  Keys are narrowed to the bits their values can use.
-static std::vector<OrderPass> order_passes(const pb200_result::Dense& d, const pb200_order_by& o) {
+static std::vector<OrderPass> order_passes(const pb200_result::Dense& d, const pb200_order_by& o, const pb200_post_aggs& post) {
   std::vector<OrderPass> ps;
   auto add = [&](OrderPass p) { p.mask = p.bits >= 64 ? ~0ull : (1ull << p.bits) - 1ull; ps.push_back(p); };
   unsigned long long space = 1;  // raw key space: bounded like the raw key (63 bits)
@@ -343,6 +353,8 @@ static std::vector<OrderPass> order_passes(const pb200_result::Dense& d, const p
     p.descending = it.descending != 0;
     if (it.kind == PB200_ORDER_GROUP_BY) {
       p.what = PASS_GROUP_BY; p.cmp = ORDER_CMP_LONG; p.bits = bits_for((unsigned long long)std::max(d.cards[it.index] - 1, 0));
+    } else if (it.kind == PB200_ORDER_POST) {
+      p.what = PASS_POST; p.cmp = ORDER_CMP_DOUBLE; p.bits = 64; p.prog = post.programs[it.index];
     } else {
       const int fn = d.aggs[it.index].function;
       p.what = PASS_AGG; p.cmp = order_cmp_of(fn);
@@ -404,8 +416,14 @@ int extract_groups(pb200_ctx* ctx, pb200_result* const* Rs, int nres, cudaStream
         if (it.kind == PB200_ORDER_AGG && e.agg[it.index].fn == PB200_AGG_DISTINCTCOUNT && !d.dbits[it.index]) {
           set_error("ORDER BY a DISTINCTCOUNT without per-group sets"); return PB200_E_UNSUPPORTED;
         }
+        if (it.kind != PB200_ORDER_POST) continue;
+        const pb200_post_program& pp = Rs[r]->post.programs[it.index];
+        for (int k = 0; k < pp.num_nodes; k++)
+          if (pp.nodes[k].op == PB200_POST_AGG && e.agg[pp.nodes[k].agg].fn == PB200_AGG_DISTINCTCOUNT && !d.dbits[pp.nodes[k].agg]) {
+            set_error("ORDER BY an expression over a DISTINCTCOUNT without per-group sets"); return PB200_E_UNSUPPORTED;
+          }
       }
-      passes[r] = order_passes(d, Rs[r]->order);
+      passes[r] = order_passes(d, Rs[r]->order, Rs[r]->post);
       order_bytes += (cap * 24 + 255) / 256 * 256 + 256;
     }
   }
@@ -679,7 +697,15 @@ void result_materialize(pb200_result* R) {
   v = pb200_result::View();
 }
 
-int order_validate(const pb200_order_by* o, int num_aggs, int num_group_by) {
+int order_validate(const pb200_order_by* o, int num_aggs, int num_group_by, const pb200_post_aggs* post) {
+  if (post) {
+    if (post->num_programs < 0 || post->num_programs > PB200_MAX_ORDER_BY) {
+      set_error("%d post-aggregation programs (0..%d)", post->num_programs, PB200_MAX_ORDER_BY);
+      return PB200_E_INVALID;
+    }
+    for (int i = 0; i < post->num_programs; i++)
+      if (const char* why = postagg_validate(&post->programs[i], num_aggs)) { set_error("program %d: %s", i, why); return PB200_E_INVALID; }
+  }
   if (!o) return PB200_OK;
   if (o->num_items < 1 || o->num_items > PB200_MAX_ORDER_BY) {
     set_error("ORDER BY has %d items (1..%d)", o->num_items, PB200_MAX_ORDER_BY);
@@ -687,7 +713,10 @@ int order_validate(const pb200_order_by* o, int num_aggs, int num_group_by) {
   }
   for (int i = 0; i < o->num_items; i++) {
     const pb200_order_item& it = o->items[i];
-    const int bound = it.kind == PB200_ORDER_AGG ? num_aggs : it.kind == PB200_ORDER_GROUP_BY ? num_group_by : 0;
+    const int bound = it.kind == PB200_ORDER_AGG        ? num_aggs
+                      : it.kind == PB200_ORDER_GROUP_BY ? num_group_by
+                      : it.kind == PB200_ORDER_POST     ? (post ? post->num_programs : 0)
+                                                        : 0;
     if (it.index < 0 || it.index >= bound) {
       set_error("ORDER BY item %d: kind %d index %d is out of range", i, it.kind, it.index);
       return PB200_E_INVALID;
@@ -696,7 +725,7 @@ int order_validate(const pb200_order_by* o, int num_aggs, int num_group_by) {
   return PB200_OK;
 }
 
-void order_rows_host(pb200_result* R, const pb200_order_by& o, const int32_t* fns) {
+void order_rows_host(pb200_result* R, const pb200_order_by& o, const int32_t* fns, const pb200_post_aggs* post) {
   if (R->meta.num_groups < 0) return;
   const size_t rows = (size_t)R->meta.num_groups, ngb = (size_t)R->meta.num_group_by, nagg = (size_t)R->meta.num_aggs;
   const pb200_result::View& v = R->view;
@@ -717,10 +746,16 @@ void order_rows_host(pb200_result* R, const pb200_order_by& o, const int32_t* fn
   std::vector<std::vector<uint64_t>> ok(o.num_items, std::vector<uint64_t>(rows));
   for (int i = 0; i < o.num_items; i++) {
     const pb200_order_item& it = o.items[i];
-    for (size_t r = 0; r < rows; r++)
+    for (size_t r = 0; r < rows; r++) {
+      if (it.kind == PB200_ORDER_POST) {
+        const double v = postagg_eval(post->programs[it.index], [&](int a) { return having_value(fns[a], dbl[a][r], lng[a][r]); });
+        ok[i][r] = order_key(ORDER_CMP_DOUBLE, it.descending != 0, ~0ull, v, 0);
+        continue;
+      }
       ok[i][r] = it.kind == PB200_ORDER_GROUP_BY
                      ? order_key(ORDER_CMP_LONG, it.descending != 0, ~0ull, 0.0, (int64_t)(uint32_t)keys[r * ngb + it.index])
                      : order_key(order_cmp_of(fns[it.index]), it.descending != 0, ~0ull, dbl[it.index][r], lng[it.index][r]);
+    }
   }
   std::vector<size_t> perm(rows);
   for (size_t r = 0; r < rows; r++) perm[r] = r;

@@ -271,6 +271,7 @@ struct pb200_result {
   pb200_order_by order{};                      // ORDER BY spec of a group-by result (num_items 0: none), applied at extraction
   pb200_having having{};                       // HAVING of a group-by result (num_nodes 0: none), applied at extraction before
                                                // the order; set on every result whose rows it filtered
+  pb200_post_aggs post{};                      // the programs PB200_ORDER_POST items of `order` name (num_programs 0: none)
   std::vector<int32_t> agg_functions;            // PB200_AGG_* per aggregation (set by pb200_execute)
   std::vector<int32_t> keys;                     // [G x k]
   std::vector<std::vector<double>> dbl;          // per agg [rows]
@@ -405,11 +406,18 @@ int finalize_sets(pb200_ctx* ctx, cudaStream_t st, const pb200_result::Dense& d,
 int decode_sets(pb200_ctx* ctx, cudaStream_t st, pb200_result* R, DevBufRaw* const* sets, const size_t* words, size_t rows,
                 double* const* dbl, int64_t* const* lng, bool* kept);
 void result_materialize(pb200_result* R);  // view -> the std::vector fields
-// pb200_order_by checks shared by the device and host entry points: PB200_OK or PB200_E_INVALID (message set)
-int order_validate(const pb200_order_by* order, int num_aggs, int num_group_by);
+// pb200_execute_exprs (exprs NULL: no expression aggregations) whose ORDER BY may name the post-aggregation programs of
+// pb200_execute_post (post NULL: none); both NULL is pb200_execute_agg_args.  The host layer's one device entry point.
+int execute_exprs_post(pb200_ctx* ctx, const pb200_query* query, const pb200_order_by* order, const pb200_agg_arg* args,
+                       const pb200_having* having, const pb200_expr_program* exprs, const pb200_post_aggs* post,
+                       pb200_segment* const* segments, int32_t nseg, pb200_result** results);
+// pb200_order_by checks shared by the device and host entry points, with the post-aggregation programs its
+// PB200_ORDER_POST items may name (post NULL: none): PB200_OK or PB200_E_INVALID (message set)
+int order_validate(const pb200_order_by* order, int num_aggs, int num_group_by, const pb200_post_aggs* post = nullptr);
 // Orders and trims a host-built group-by result (rows in its std::vector fields or view) by `order`; fns = PB200_AGG_* per
-// aggregation.  Same keys as the device sort (pb200_order.h); the result's rows end up in its std::vector fields.
-void order_rows_host(pb200_result* R, const pb200_order_by& order, const int32_t* fns);
+// aggregation, post = the programs of its PB200_ORDER_POST items (NULL: none).  Same keys as the device sort (pb200_order.h,
+// pb200_postagg.h); the result's rows end up in its std::vector fields.
+void order_rows_host(pb200_result* R, const pb200_order_by& order, const int32_t* fns, const pb200_post_aggs* post = nullptr);
 // pb200_having checks of the device and host entry points (having may be NULL): PB200_OK, or PB200_E_INVALID /
 // PB200_E_UNSUPPORTED (message set).  nres = results the call writes, deferred = PB200_Q_DEFER_FINALIZE or reduce_world > 1.
 int having_check(const pb200_having* having, int num_aggs, int num_group_by, int nres, bool deferred);

@@ -355,7 +355,7 @@ def _order_and_trim(query, fns, keys, merged, set_final):
     the key order -- the library's tie rule.  Values compare in the reference's order (query.value_order); a key column
     compares by domain id, which is its value order."""
     from .plan_maker import order_spec
-    from .query import value_order
+    from .query import post_eval, value_order
     from .sql import resolve_order_by
 
     def final(a, v):
@@ -371,6 +371,9 @@ def _order_and_trim(query, fns, keys, merged, set_final):
     for kind, index, asc in reversed(resolve_order_by(query)):
         if kind == "GROUP_BY":
             rows.sort(key=lambda key: key[index], reverse=not asc)
+        elif kind == "POST":
+            program = query.post_aggregations[index].program
+            rows.sort(key=lambda key: value_order(post_eval(program, lambda a: float(final(a, merged[key][a])))), reverse=not asc)
         else:
             rows.sort(key=lambda key: value_order(float(final(index, merged[key][index]))), reverse=not asc)
     trim = order_spec(query, merge=True).trim_size

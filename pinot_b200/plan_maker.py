@@ -561,8 +561,32 @@ def order_spec(q: QueryContext, merge: bool):
         raise ValueError(f"ORDER BY has {len(items)} items, at most {_lib.MAX_ORDER_BY} are supported")
     option = q.min_server_group_trim_size if merge else q.min_segment_group_trim_size
     spec = _lib.OrderBy(len(items), max(5 * q.limit, option) if option > 0 else 0)
+    programs = 0   # a POST item names the next program of post_spec
     for i, (kind, index, asc) in enumerate(items):
+        if kind == "POST":
+            spec.items[i] = _lib.OrderItem(_lib.ORDER_POST, programs, int(not asc))
+            programs += 1
+            continue
         spec.items[i] = _lib.OrderItem(_lib.ORDER_GROUP_BY if kind == "GROUP_BY" else _lib.ORDER_AGG, index, int(not asc))
+    return spec
+
+
+def post_spec(q: QueryContext):
+    """pb200_post_aggs of a GROUP BY query whose ORDER BY names post-aggregation expressions (None otherwise): their
+    programs, in the order of those items (order_spec's POST items index it).  Expressions only in the SELECT list stay
+    here: the caller computes them from the final values."""
+    from .sql import resolve_order_by
+    if not q.is_group_by or not q.order_by:
+        return None
+    programs = [q.post_aggregations[index].program for kind, index, _ in resolve_order_by(q) if kind == "POST"]
+    if not programs:
+        return None
+    spec = _lib.PostAggs(len(programs), 0)
+    for i, program in enumerate(programs):
+        spec.programs[i].num_nodes = len(program)
+        for j, n in enumerate(program):
+            spec.programs[i].nodes[j] = _lib.PostNode(_lib.POST_CODES[n[0]], n[1] if n[0] == "AGG" else 0,
+                                                      n[1] if n[0] == "LIT" else 0.0)
     return spec
 
 
@@ -784,8 +808,8 @@ class B200PlanMaker:
         segments (sharing dictionaries) are combined on the device and one block is returned; with keep_handle=True as
         well, a group-by block comes back WITHOUT its groups extracted (PB200_Q_DEFER_FINALIZE): its dense device tables
         are meant to be reduced across GPUs (pinot_b200.distributed.combine_across_ranks), which extracts on the root.
-        A GROUP BY query with an ORDER BY gets its rows ordered and trimmed by the library (order_spec; a deferred block
-        when it is extracted); ordered=False returns every group in the library's row order.  A query with HAVING gets
+        A GROUP BY query with an ORDER BY gets its rows ordered and trimmed by the library (order_spec, with post_spec's
+        programs for expressions over aggregations; a deferred block when it is extracted); ordered=False returns every group in the library's row order.  A query with HAVING gets
         its rows filtered by the library before that order when the call's result is final (merge=True, or one segment,
         and ordered); per-segment blocks of several segments come back unfiltered, for the caller's merge to filter.
         Per-segment blocks carry the intermediates of a by-value merge (DISTINCTCOUNTHLL sets among them); sets=True
@@ -807,6 +831,7 @@ class B200PlanMaker:
         res = (C.c_void_p * nres)()
         kinds = (C.c_int32 * n)()
         spec = order_spec(query, merge) if ordered else None
+        post = post_spec(query) if ordered else None
         having = having_spec(query) if ordered and (merge or n == 1) else None
         for a in query.aggregations:
             if a.function == "DISTINCTCOUNTHLL" and a.arg == 0:   # the library reads an argument of 0 as the default 8
@@ -814,15 +839,21 @@ class B200PlanMaker:
         # one argument per aggregation: the percentile of a PERCENTILE, the log2m of a DISTINCTCOUNTHLL
         numeric = functions_where(lambda f: f.arg in ("percentile", "log2m"))
         pct = [a.function in numeric for a in query.aggregations]
-        if any(a.function in WITHTIME_FUNCTIONS for a in query.aggregations):
-            # FIRST/LASTWITHTIME: the time column and the type literal travel beside the query (pb200h_execute_agg_args)
+        if post is not None or any(a.function in WITHTIME_FUNCTIONS for a in query.aggregations):
+            # FIRST/LASTWITHTIME: the time column and the type literal travel beside the query (pb200h_execute_agg_args);
+            # ORDER BY expressions over aggregations: their programs (pb200h_execute_post)
             args = (_lib.HAggArg * len(pct))(*[
                 _lib.HAggArg(float(a.arg) if is_p else 0.0,
                              a.time_column.encode() if a.function in WITHTIME_FUNCTIONS else None,
                              WITHTIME_TYPES[a.value_type] if a.function in WITHTIME_FUNCTIONS else 0)
                 for a, is_p in zip(query.aggregations, pct)])
-            _lib.check(self.ctx.lib.pb200h_execute_agg_args(self.ctx.handle, C.byref(hq), C.byref(spec) if spec is not None else None,
-                                                            args, C.byref(having) if having is not None else None, segs, n, res, kinds))
+            if post is not None:
+                _lib.check(self.ctx.lib.pb200h_execute_post(self.ctx.handle, C.byref(hq), C.byref(spec), args,
+                                                            C.byref(having) if having is not None else None, C.byref(post),
+                                                            segs, n, res, kinds))
+            else:
+                _lib.check(self.ctx.lib.pb200h_execute_agg_args(self.ctx.handle, C.byref(hq), C.byref(spec) if spec is not None else None,
+                                                                args, C.byref(having) if having is not None else None, segs, n, res, kinds))
         elif having is not None:
             args = (C.c_double * max(1, len(pct)))(*[float(a.arg) if is_p else 0.0 for a, is_p in zip(query.aggregations, pct)])
             _lib.check(self.ctx.lib.pb200h_execute_having(self.ctx.handle, C.byref(hq), C.byref(spec) if spec is not None else None,

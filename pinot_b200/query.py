@@ -112,6 +112,49 @@ class Aggregation:
         return f"{self.function.lower()}({self.column or '*'})"
 
 
+@dataclass
+class PostAggregation:
+    """Arithmetic over the final values of aggregations (Pinot's post-aggregation expression), e.g. SUM(a) / SUM(b)
+    (DESIGN.md section 3.18).  `program` is postfix, root last: ("AGG", a) with a indexing QueryContext.aggregations,
+    ("LIT", float), ("NEG",), ("ADD",), ("SUB",), ("MUL",), ("DIV",).  `text` is its normalised name
+    (divide(sum(a),sum(b))): what an ORDER BY item is matched with and the CLI's column header."""
+    text: str
+    program: List[tuple]
+
+    def __str__(self):
+        return self.text
+
+
+def java_divide(x: float, y: float) -> float:
+    """x / y as one IEEE-754 double division, as Java computes it: a division by zero gives +-inf (the sign of x times
+    the sign of the zero), and NaN for 0 / 0 or a NaN operand; Python raises there instead."""
+    if y != 0.0:
+        return x / y
+    if x == 0.0 or math.isnan(x):
+        return math.nan
+    return math.copysign(math.inf, x) * math.copysign(1.0, y)
+
+
+def post_eval(program, value) -> float:
+    """The value of a post-aggregation program (PostAggregation.program) for one row; value(a) = the final value of
+    aggregation a.  Each operand is read as a float and each operator is one IEEE-754 double operation, rounded to
+    nearest (pinot_b200/csrc/pb200_postagg.h is the library's copy of this rule)."""
+    st: List[float] = []
+    for n in program:
+        op = n[0]
+        if op == "AGG":
+            st.append(float(value(n[1])))
+        elif op == "LIT":
+            st.append(float(n[1]))
+        elif op == "NEG":
+            st.append(-st.pop())
+        else:
+            y = st.pop()
+            x = st.pop()
+            st.append(x + y if op == "ADD" else x - y if op == "SUB" else x * y if op == "MUL" else java_divide(x, y))
+    return st[0]
+
+
 # the type literal of FIRST/LASTWITHTIME -> the stored type it names (BOOLEAN is stored as INT)
 WITHTIME_TYPES = {"INT": 0, "BOOLEAN": 0, "LONG": 1, "FLOAT": 2, "DOUBLE": 3, "STRING": 4}
 
@@ -363,6 +406,10 @@ class QueryContext:
     # HAVING: a filter tree whose leaves name aggregations by sql.having_name and compare them with numeric literals
     # (sql.resolve_having gives the library's postfix form); applied to final rows, before ORDER BY and LIMIT
     having: Optional[FilterNode] = None
+    # arithmetic over aggregations in the SELECT list (PostAggregation; an ORDER BY expression is one of them), and the
+    # SELECT list in its order: ("COLUMN", name), ("AGG", index into aggregations), ("POST", index into post_aggregations)
+    post_aggregations: List[PostAggregation] = field(default_factory=list)
+    select: List[tuple] = field(default_factory=list)
 
     @property
     def is_group_by(self) -> bool:

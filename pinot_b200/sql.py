@@ -8,6 +8,7 @@ stays Java).  This module exists so the parity tests read like the reference's
 
     SELECT item[, item...] FROM table [WHERE cond] [GROUP BY col[, col...] [HAVING hcond]] [ORDER BY expr [ASC|DESC], ...]
            [LIMIT n]
+    item  := agg | col | post
     item  := COUNT(*) | FN(col) | PERCENTILE(col, p) | PERCENTILE<n>(col) | FIRSTWITHTIME(col, col, 'T')
              | LASTWITHTIME(col, col, 'T') | COUNT(DISTINCT col) | SUM(DISTINCT col) | AVG(DISTINCT col) | col
              (COUNT / SUM / AVG(DISTINCT col) are DISTINCTCOUNT / DISTINCTSUM / DISTINCTAVG(col), named
@@ -32,6 +33,13 @@ stays Java).  This module exists so the parity tests read like the reference's
     hcond := cond whose left-hand sides are aggregation calls (COUNT(*), FN(col), PERCENTILE(col, p), ...) and whose
              literals are numbers.  An aggregation named only in HAVING is computed as a hidden one (Aggregation.hidden):
              ORDER BY may name it, it is never an output column.  HAVING on a column belongs in WHERE and is refused.
+    post  := arithmetic over aggregation calls, a post-aggregation expression (DESIGN.md section 3.18):
+             post := term (+|- term)* ; term := unary (*|/ unary)* ; unary := -unary | factor ;
+             factor := agg | number | (post), with at least one agg.  Numbers are finite decimals; a column, a string, %
+             or a function that is not an aggregation (ABS(SUM(x))) is refused.  Named by its normalised text
+             (QueryContext.post_aggregations): SUM(a) / SUM(b) -> divide(sum(a),sum(b)), -x -> negate(x).  An aggregation
+             named only in such expressions is a hidden one, as for HAVING.  An ORDER BY expression must be a SELECT
+             item, compared by that text.
     col   := a column, or a single-column expression wherever a column is accepted (select list, GROUP BY, aggregation
              arguments, the left-hand side of predicates, ORDER BY, selection and DISTINCT lists):
              expr := term (+|- term)* ; term := factor (*|/|% factor)* ; factor := col | number | (expr) | fn(args)
@@ -41,11 +49,13 @@ stays Java).  This module exists so the parity tests read like the reference's
 """
 from __future__ import annotations
 
+import math
 import re
 from dataclasses import dataclass, field
 from typing import List, Optional
 
-from .query import AGG_FUNCTIONS, HLL_DEFAULT_LOG2M, WITHTIME_FUNCTIONS, WITHTIME_TYPES, Aggregation, Filter, FilterNode, Predicate, QueryContext, flatten, optimize_filter
+from .query import (AGG_FUNCTIONS, HLL_DEFAULT_LOG2M, WITHTIME_FUNCTIONS, WITHTIME_TYPES, Aggregation, Filter, FilterNode, PostAggregation,
+                    Predicate, QueryContext, flatten, optimize_filter)
 
 _TOKEN = re.compile(r"\s*(?:(\d+\.\d+(?:[eE][-+]?\d+)?|-?\d+\.\d+|-?\d+)|'((?:[^']|'')*)'|(<=|>=|<>|!=|[=<>(),*+/%-])|"
                     r"([A-Za-z_$][A-Za-z0-9_$]*))")
@@ -113,6 +123,66 @@ def having_name(agg: Aggregation) -> str:
 
 
 MAX_HAVING_NODES = 32
+MAX_POST_NODES = 16   # nodes of one post-aggregation program (pb200_post_program)
+
+_POST_NAMES = {"ADD": "plus", "SUB": "minus", "MUL": "times", "DIV": "divide", "NEG": "negate"}
+
+
+def _filter_text(n) -> str:
+    """Canonical text of a FILTER clause's tree (how a filtered operand of a post-aggregation expression is named)."""
+    if isinstance(n, Filter):
+        return f"{n.type.lower()}({','.join(_filter_text(c) for c in n.children)})"
+    if n.type == "RANGE":
+        return (f"range({n.column},{'[' if n.lower_inclusive else '('}{'*' if n.lower is None else _literal_text(n.lower)},"
+                f"{'*' if n.upper is None else _literal_text(n.upper)}{']' if n.upper_inclusive else ')'})")
+    return f"{n.type.lower()}({n.column},{','.join(_literal_text(v) for v in n.values)})"
+
+
+def _post_text(t) -> str:
+    """Normalised text of a post-aggregation expression tree (_Parser.post_item): spacing, case and parentheses gone."""
+    if t[0] == "AGG":
+        return having_name(t[1]) + ("" if t[1].filter is None else f" filter({_filter_text(t[1].filter)})")
+    if t[0] == "LIT":
+        return _literal_text(t[1])
+    return f"{_POST_NAMES[t[0]]}({','.join(_post_text(c) for c in t[1:])})"
+
+
+def _post_aggs(t) -> List[Aggregation]:
+    """The aggregation calls of a post-aggregation expression tree, left to right."""
+    if t[0] == "AGG":
+        return [t[1]]
+    if t[0] in ("LIT", "COL", "STR"):
+        return []
+    return [a for c in (t[2] if t[0] == "FUNC" else t[1:]) for a in _post_aggs(c)]
+
+
+def _post_check(t):
+    """Refuses what a post-aggregation expression cannot hold (SqlError)."""
+    kind = t[0]
+    if kind == "COL":
+        raise SqlError(f"the column {t[1]} in an expression over aggregations: operands must be aggregation calls or numbers")
+    if kind == "STR":
+        raise SqlError(f"the string literal {t[1]!r} in an expression over aggregations: only numbers are supported")
+    if kind == "FUNC":
+        if _post_aggs(t):
+            raise SqlError(f"{t[1]}(...) over an aggregation: only +, -, * and / apply to aggregations")
+        raise SqlError(f"the column expression {t[1]}(...) in an expression over aggregations: operands must be aggregation calls or numbers")
+    if kind == "MOD":
+        raise SqlError("% in an expression over aggregations is not supported (only +, -, * and /)")
+    if kind == "LIT":
+        try:
+            v = float(t[1])
+        except OverflowError:
+            v = math.inf
+        if not math.isfinite(v):
+            raise SqlError(f"the literal {t[1]!r} in an expression over aggregations is not a finite number")
+        return
+    if kind == "AGG":
+        if t[1].value_type == "STRING":
+            raise SqlError(f"{having_name(t[1])} in an expression: a STRING FIRST/LASTWITHTIME is not a number")
+        return
+    for c in t[1:]:
+        _post_check(c)
 
 _REGEX_META = set("\\.^$|?*+()[]{}")
 
@@ -325,6 +395,77 @@ class _Parser:
         self.expect_op(")")
         return agg
 
+    # ---- post-aggregation expressions: arithmetic over aggregation calls -------------------------------------------
+    def post_item(self):
+        """At a SELECT or ORDER BY item: its tree when the item is arithmetic over aggregation calls (a post-aggregation
+        expression; checked by _post_check), else None with the position unchanged -- a single aggregation call, a column
+        or a single-column expression is parsed as before.  Tree nodes: ("AGG", Aggregation), ("LIT", number),
+        ("NEG", x), ("ADD" | "SUB" | "MUL" | "DIV" | "MOD", x, y) and, refused by _post_check, ("COL", name),
+        ("STR", text), ("FUNC", name, args)."""
+        start = self.i
+        try:
+            tree = self._post_additive()
+        except SqlError:
+            tree = None
+        if tree is None or not _post_aggs(tree) or (tree[0] == "AGG" and self.toks[start][0] == "id"):
+            self.i = start
+            return None
+        _post_check(tree)
+        return tree
+
+    def _post_additive(self):
+        left = self._post_term()
+        while True:
+            k, v = self.peek()
+            if k == "op" and v in ("+", "-"):
+                self.i += 1
+                left = ("ADD" if v == "+" else "SUB", left, self._post_term())
+            elif k == "num" and v < 0:   # `x -1` is tokenized as x, -1
+                self.i += 1
+                left = ("SUB", left, ("LIT", -v))
+            else:
+                return left
+
+    def _post_term(self):
+        left = self._post_unary()
+        while True:
+            k, v = self.peek()
+            if k != "op" or v not in ("*", "/", "%"):
+                return left
+            self.i += 1
+            left = ({"*": "MUL", "/": "DIV", "%": "MOD"}[v], left, self._post_unary())
+
+    def _post_unary(self):
+        if self.take_op("-"):
+            return ("NEG", self._post_unary())
+        return self._post_factor()
+
+    def _post_factor(self):
+        k, v = self.peek()
+        if k in ("num", "str"):
+            self.i += 1
+            return ("LIT" if k == "num" else "STR", v)
+        if self.take_op("("):
+            inner = self._post_additive()
+            self.expect_op(")")
+            return inner
+        name = self.ident()
+        if not self.take_op("("):
+            return ("COL", name)
+        if _is_function(name):
+            agg = self.aggregation_call()
+            if self.take_kw("FILTER"):   # SUM(x) FILTER (WHERE cond)
+                self.expect_op("(")
+                self.expect_kw("WHERE")
+                agg.filter = optimize_filter(self.cond())
+                self.expect_op(")")
+            return ("AGG", agg)
+        args = [] if self.peek() == ("op", ")") else [self._post_additive()]
+        while self.take_op(","):
+            args.append(self._post_additive())
+        self.expect_op(")")
+        return ("FUNC", name, args)
+
     def having_operand(self) -> str:
         """Left-hand side of a HAVING comparison: an aggregation call, named by having_name."""
         k, v = self.peek()
@@ -473,12 +614,17 @@ def _comparison(col: str, op: str, v) -> Predicate:
 
 def resolve_order_by(query: QueryContext) -> List[tuple]:
     """ORDER BY expressions -> [(kind, index, ascending)]: kind "GROUP_BY" indexes query.group_by, "AGG" indexes
-    query.aggregations (the first one the expression names).  Anything else is refused: ORDER BY on expressions or on
-    functions that are not in the SELECT list is outside this path."""
+    query.aggregations (the first one the expression names), "POST" indexes query.post_aggregations (an arithmetic
+    expression over aggregations of the SELECT list, matched by its normalised text).  Anything else is refused: ORDER BY
+    on column expressions or on functions that are not in the SELECT list is outside this path."""
     out = []
     for expr, asc in query.order_by:
         if expr in query.group_by:
             out.append(("GROUP_BY", query.group_by.index(expr), asc))
+            continue
+        post = next((i for i, pa in enumerate(query.post_aggregations) if pa.text == expr), None)
+        if post is not None:
+            out.append(("POST", post, asc))
             continue
         m = re.fullmatch(r"([A-Za-z_$][A-Za-z0-9_$]*)\((.+?)(?:,([-+0-9.eE]+))?\)", expr)
         found = None
@@ -553,11 +699,18 @@ def parse(sql: str, **options) -> QueryContext:
     p.expect_kw("SELECT")
     aggs: List[Aggregation] = []
     plain: List[str] = []
+    select: List[tuple] = []
+    posts: List[tuple] = []   # post-aggregation expression trees of the SELECT list
     while True:
         k, name = p.peek()
-        if k == "id" and _is_function(name) and p.toks[p.i + 1:p.i + 2] == [("op", "(")]:
+        tree = p.post_item()
+        if tree is not None:
+            select.append(("POST", len(posts)))
+            posts.append(tree)
+        elif k == "id" and _is_function(name) and p.toks[p.i + 1:p.i + 2] == [("op", "(")]:
             p.i += 2
             aggs.append(p.aggregation_call())
+            select.append(("AGG", len(aggs) - 1))
             if p.take_kw("FILTER"):   # SUM(x) FILTER (WHERE cond)
                 p.expect_op("(")
                 p.expect_kw("WHERE")
@@ -565,6 +718,7 @@ def parse(sql: str, **options) -> QueryContext:
                 p.expect_op(")")
         else:
             plain.append(p.column())
+            select.append(("COLUMN", plain[-1]))
         if not p.take_op(","):
             break
     p.expect_kw("FROM")
@@ -594,7 +748,12 @@ def parse(sql: str, **options) -> QueryContext:
         p.expect_kw("BY")
         while True:
             k, name = p.peek()
-            if k == "id" and _is_function(name) and p.toks[p.i + 1:p.i + 2] == [("op", "(")]:
+            tree = p.post_item()
+            if tree is not None:
+                expr = _post_text(tree)
+                if expr not in (_post_text(t) for t in posts):
+                    raise SqlError(f"ORDER BY {expr}: an expression over aggregations must also be a SELECT item")
+            elif k == "id" and _is_function(name) and p.toks[p.i + 1:p.i + 2] == [("op", "(")]:
                 p.i += 2
                 if name.upper().startswith("PERCENTILE"):
                     inner, pct = p.percentile_call(name)
@@ -633,13 +792,40 @@ def parse(sql: str, **options) -> QueryContext:
     for c in plain:
         if c not in group_by:
             raise SqlError(f"column {c} must appear in GROUP BY (selection queries are outside this path)")
+    post_aggregations = [_post_program(tree, aggs) for tree in posts]
     if not aggs:
         raise SqlError("only aggregation / group-by queries are on this path")
     query = QueryContext(aggregations=aggs, filter=optimize_filter(flt), group_by=group_by, table=table, limit=limit,
-                         order_by=order_by, having=having, **options)
+                         order_by=order_by, having=having, post_aggregations=post_aggregations, select=select, **options)
     resolve_order_by(query)
     resolve_having(query)
     return query
+
+
+def _post_program(tree, aggs: List[Aggregation]) -> PostAggregation:
+    """A post-aggregation expression tree -> its PostAggregation over `aggs`: each operand is the first aggregation that
+    computes it (same function, arguments and FILTER clause), or a hidden one appended to `aggs`."""
+    program: List[tuple] = []
+
+    def emit(t):
+        if t[0] == "AGG":
+            found = next((a for a, x in enumerate(aggs) if having_name(x) == having_name(t[1]) and x.filter == t[1].filter), None)
+            if found is None:
+                t[1].hidden = True
+                aggs.append(t[1])
+                found = len(aggs) - 1
+            program.append(("AGG", found))
+        elif t[0] == "LIT":
+            program.append(("LIT", float(t[1])))
+        else:
+            for c in t[1:]:
+                emit(c)
+            program.append((t[0],))
+
+    emit(tree)
+    if len(program) > MAX_POST_NODES:
+        raise SqlError(f"{_post_text(tree)} needs {len(program)} nodes, at most {MAX_POST_NODES} are supported")
+    return PostAggregation(_post_text(tree), program)
 
 
 @dataclass
