@@ -580,6 +580,43 @@ int32_t pb200_execute_exprs(pb200_ctx* ctx, const pb200_query* query, const pb20
                             const pb200_having* having, const pb200_expr_program* exprs, pb200_segment* const* segments,
                             int32_t num_segments, pb200_result** results);
 
+/* ---- CASE WHEN inside expression programs: SUM(CASE WHEN s = 'x' THEN b ELSE 0 END) (DESIGN.md section 3.19) ------- */
+/* Five more program operations, accepted by pb200_execute_exprs_cond only:
+ *   COND        a leaf: condition `i` of the call's pb200_expr_conds holds for the row (1.0) or not (0.0)
+ *   AND, OR (x, y), NOT (x)   over conditions (COND, AND, OR, NOT results) only
+ *   CASE (c, v, e)            v when the condition c holds, else e; v and e are values (never conditions).  A k-WHEN
+ *                             CASE is k nested CASE nodes: c1 v1 c2 v2 e CASE CASE.
+ * Branches are evaluated before one is selected: they have no side effects in double arithmetic.  The program's result
+ * is a value.  COND leaves count as column leaves (at most 8 with the PB200_T_COLUMN leaves; one suffices). */
+enum { PB200_T_COND = 27, PB200_T_AND = 28, PB200_T_OR = 29, PB200_T_NOT = 30, PB200_T_CASE = 31 };
+/* A condition is a set of dictIds of one column, resolved by the caller per segment: a dictId range or a bitset. */
+enum { PB200_COND_RANGE = 0, PB200_COND_BITSET = 1 };
+#define PB200_MAX_EXPR_CONDS 32 /* conditions of one call */
+typedef struct {
+  int32_t column;           /* a column with dictIds (a device dictionary, STRING included) in every segment */
+  int32_t kind;             /* PB200_COND_* */
+  /* two per segment, in submission order: RANGE: the dictIds [args[2s], args[2s+1]) (0 <= lo <= hi <= cardinality);
+     BITSET: the first word of segment s's bitset in pb200_expr_conds.words and its length in words (at least
+     ceil(cardinality / 32)); bit j of word w is dictId 32 * w + j.  A bound segment's ids are the domain's. */
+  const int64_t* args;
+} pb200_expr_cond;
+typedef struct {
+  int32_t num_conds;        /* 1 .. PB200_MAX_EXPR_CONDS */
+  int32_t reserved;         /* 0 */
+  const pb200_expr_cond* conds;
+  int64_t num_words;        /* bitset words (0 when every condition is a RANGE) */
+  const uint32_t* words;    /* host pointer */
+} pb200_expr_conds;
+/* pb200_execute_exprs whose programs may hold COND / AND / OR / NOT / CASE (conds == NULL: exactly pb200_execute_exprs).
+ * A condition's dictIds are read through the same forward index as a value leaf, once per distinct condition column
+ * and row; the device never compares values, so the caller decides what a condition means.
+ * PB200_E_INVALID as well: a condition index out of range, an operand of the wrong kind (a condition where a value
+ * belongs or the reverse), a malformed condition table (range or bitset outside its segment's cardinality or words).
+ * PB200_E_UNSUPPORTED as well: a condition column without dictIds (raw 32-bit values). */
+int32_t pb200_execute_exprs_cond(pb200_ctx* ctx, const pb200_query* query, const pb200_order_by* order, const pb200_agg_arg* args,
+                                 const pb200_having* having, const pb200_expr_program* exprs, const pb200_expr_conds* conds,
+                                 pb200_segment* const* segments, int32_t num_segments, pb200_result** results);
+
 /* ---- predicates on expressions of two or more columns: WHERE a > b, WHERE price * qty > 1000 (DESIGN.md section 3.16) -- */
 /* One predicate on the value of a pb200_expr_program (the rules of pb200_execute_exprs: 2 .. 8 column leaves by column
  * id, every leaf a double, every operation one IEEE-754 step without FMA).  The value is compared as a DOUBLE with Java's

@@ -189,6 +189,18 @@ class ExprProgram(C.Structure):  # pb200_expr_program
 
 
 EXPR_OPS = {"EQ": 0, "NEQ": 1, "IN": 2, "NOT_IN": 3, "RANGE": 4}   # PB200_EXPR_*
+T_COND, T_AND, T_OR, T_NOT, T_CASE = 27, 28, 29, 30, 31               # PB200_T_* of CASE WHEN programs
+COND_RANGE, COND_BITSET = 0, 1                                         # PB200_COND_*
+MAX_EXPR_CONDS = 32
+
+
+class ExprCond(C.Structure):  # pb200_expr_cond
+    _fields_ = [("column", C.c_int32), ("kind", C.c_int32), ("args", C.POINTER(C.c_int64))]
+
+
+class ExprConds(C.Structure):  # pb200_expr_conds
+    _fields_ = [("num_conds", C.c_int32), ("reserved", C.c_int32), ("conds", C.POINTER(ExprCond)), ("num_words", C.c_int64),
+                ("words", C.POINTER(C.c_uint32))]
 
 
 class ExprPredicate(C.Structure):  # pb200_expr_predicate
@@ -238,7 +250,7 @@ EXPORTED_SYMBOLS = [
     "pb200h_startree_build", "pb200h_startree_get",
     "pb200_execute_having", "pb200h_execute_having", "pb200_execute_agg_args", "pb200h_execute_agg_args",
     "pb200_match_pattern", "pb200_result_exact_sum", "pb200_execute_exprs", "pb200_expr_doc_masks",
-    "pb200_execute_post", "pb200h_execute_post",
+    "pb200_execute_post", "pb200h_execute_post", "pb200_execute_exprs_cond",
 ]
 
 _LIB = None
@@ -272,6 +284,8 @@ def load() -> C.CDLL:
                                          C.POINTER(vp), i32, C.POINTER(vp)]
     L.pb200_execute_exprs.argtypes = [vp, C.POINTER(Query), C.POINTER(OrderBy), C.POINTER(AggArg), C.POINTER(Having),
                                       C.POINTER(ExprProgram), C.POINTER(vp), i32, C.POINTER(vp)]
+    L.pb200_execute_exprs_cond.argtypes = [vp, C.POINTER(Query), C.POINTER(OrderBy), C.POINTER(AggArg), C.POINTER(Having),
+                                           C.POINTER(ExprProgram), C.POINTER(ExprConds), C.POINTER(vp), i32, C.POINTER(vp)]
     L.pb200_execute_post.argtypes = [vp, C.POINTER(Query), C.POINTER(OrderBy), C.POINTER(AggArg), C.POINTER(Having),
                                      C.POINTER(PostAggs), C.POINTER(vp), i32, C.POINTER(vp)]
     L.pb200_expr_doc_masks.argtypes = [vp, i32, C.POINTER(ExprPredicate), C.POINTER(vp), i32, C.POINTER(vp)]

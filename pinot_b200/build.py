@@ -18,7 +18,7 @@ SCAN_KERNELS = ["w6_agg", "w8_agg", "w8_agg_nodefer", "w6_gb1", "w8_gb1", "w6_gb
                 "w8_gb1_spec", "w6_gb2_spec"]
 SOURCES = [f"pb200_scan_k_{k}.cu" for k in SCAN_KERNELS] + ["pb200_api.cu", "pb200_plan.cpp", "pb200_select.cu", "pb200_distinct.cu", "pb200_percentile.cu", "pb200_withtime.cu", "pb200_expr.cu", "pb200_distinct_sum.cu", "pb200_hll.cu", "pb200_moments.cu", "pb200_transform.cu", "pb200_domain.cu", "pb200_extract.cu", "pb200_comm.cu", "pb200_roaring.cu", "pb200_synth.cu", "pb200_startree_build.cu", "pb200_pattern.cu",
                                                              "host/plan_maker.cpp", "host/star_tree.cpp", "host/datatable.cpp", "host/segment_cache.cpp", "host/raw_forward.cpp", "host/filtered_agg.cpp", "host/transform.cpp", "host/patterns.cpp",
-                                                             "host/expr_filters.cpp"]
+                                                             "host/expr_filters.cpp", "host/case_expr.cpp"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
          "-Xptxas", "-v", "--expt-relaxed-constexpr"]

@@ -104,7 +104,9 @@ extern "C" int64_t pb200h_result_to_datatable(const pb200h_query* q, const pb200
       std::vector<std::string> leaves;
       // an expression over several columns: written like the function over a DOUBLE column, named by its canonical text
       if (ci < 0 && expression_function(fn) && is_multi_column_expression(q->aggs[a].column)) {
-        if (int rc = compile_multi_expression(q->aggs[a].column, &arg, &ops, &leaves)) return rc;
+        std::vector<CaseCond> conds;
+        if (int rc = compile_multi_expression(q->aggs[a].column, &arg, &ops, &leaves, &conds)) return rc;
+        if (!conds.empty()) { set_error("%s", pb200::kNoDtCase); return PB200_E_UNSUPPORTED; }
       } else {
         if (ci < 0) { set_error("unknown aggregation column '%s'", q->aggs[a].column); return PB200_E_INVALID; }
         agg_cols[a] = &seg->cols[ci].decode_column();

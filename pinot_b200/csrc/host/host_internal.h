@@ -176,8 +176,43 @@ int derive_names(pb200_ctx* ctx, pb200h_segment* const* segs, int nseg, const st
 // Multi-column expressions (DESIGN.md section 3.15): `text` in the grammar of compile_expression with two or more column
 // leaves, compiled to a program whose PB200_T_COLUMN leaf k (i = k) reads column leaves[k].  PB200_E_INVALID (malformed)
 // or PB200_E_UNSUPPORTED (fewer than two or more than 8 leaves, a time function, outside the grammar), message set.
+// CASE WHEN (DESIGN.md section 3.19) compiles to COND leaves (i = k: conds[k]) and CASE / AND / OR / NOT operations; a
+// caller that passes no `conds` refuses it (PB200_E_UNSUPPORTED).  COND leaves count against the 8 column leaves, and a
+// CASE needs no second column.
+struct CaseCond {
+  std::string fn;                     // equals, not_equals, less_than, ..., between, in, not_in, like, regexp_like
+  std::string column;
+  std::vector<std::string> literals;  // as written (quotes removed)
+};
+struct CaseBranch {                   // a THEN or ELSE value: what decides whether its CASE has one result type
+  enum Kind { COLUMN, LONG_LITERAL, DOUBLE_LITERAL, ARITHMETIC } kind = COLUMN;
+  std::string column;                 // COLUMN
+  int64_t value = 0;                  // LONG_LITERAL
+};
 int compile_multi_expression(const char* text, std::string* canonical, std::vector<pb200_transform_op>* ops,
-                             std::vector<std::string>* leaves);
+                             std::vector<std::string>* leaves, std::vector<CaseCond>* conds = nullptr,
+                             std::vector<CaseBranch>* branches = nullptr);
+// case_expr.cpp: the condition table of a call's CASE conditions (their COND leaves index `conds`), resolved on every
+// segment of the call by the WHERE planner's value-to-dictId rule; LIKE / REGEXP_LIKE leaves go through `patterns`.
+// PB200_E_UNSUPPORTED for the refused conditions of DESIGN.md section 3.19 (a STRING range, a raw or NaN / -0.0
+// condition column, a non-integral literal beyond 2^53 on a LONG column, ...), PB200_E_INVALID for an unknown column.
+struct CaseTable {
+  std::vector<pb200_expr_cond> conds;
+  std::vector<std::vector<int64_t>> args;
+  std::vector<uint32_t> words;
+  pb200_expr_conds table{};
+};
+struct PatternScope;
+int resolve_case_conditions(pb200_ctx* ctx, pb200h_segment* const* segs, int nseg, const std::vector<CaseCond>& leaves,
+                            PatternScope& patterns, CaseTable& out);
+// The local dictIds (ascending) column c matches for one condition (pattern leaves: from the thread's pattern scope), with
+// the refusals that concern the column itself
+int case_condition_ids(const HostColumn& c, const CaseCond& cc, std::vector<int32_t>* ids);
+// the REGEXP_LIKE pattern of a like / regexp_like condition (LIKE as sql.py's like_to_regexp); false for a LIKE escape
+bool case_pattern(const CaseCond& cc, std::string* regex);
+// PB200_E_UNSUPPORTED for a CASE whose result type this library does not restate: a FLOAT column branch next to an INT /
+// LONG column branch or an integer literal beyond 2^24, with no DOUBLE column, decimal literal or arithmetic branch
+int case_result_type_check(const pb200h_segment& s0, const std::vector<CaseBranch>& branches, const char* text);
 // `text` compiles as a multi-column expression (the last error is left as it was)
 bool is_multi_column_expression(const char* text);
 // the functions that take a multi-column expression as their argument

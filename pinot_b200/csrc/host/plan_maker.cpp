@@ -883,13 +883,18 @@ extern "C" int32_t pb200h_execute_post(pb200_ctx* ctx, const pb200h_query* q, co
   std::vector<std::vector<pb200_transform_op>> expr_ops(q->num_aggs);
   std::vector<pb200_expr_program> programs(q->num_aggs, pb200_expr_program{0, 0, nullptr});
   std::vector<int> leaf_cols;
+  std::vector<CaseCond> case_conds;   // CASE conditions of all aggregations: a COND leaf's i indexes this call-wide list
   bool any_expr = false;
   for (int a = 0; a < q->num_aggs; a++) {
     if (!expression_function(q->aggs[a].function) || !is_multi_column_expression(q->aggs[a].column)) continue;
     std::string canonical;
     std::vector<std::string> leaves;
-    if (int rc = compile_multi_expression(q->aggs[a].column, &canonical, &expr_ops[a], &leaves)) return rc;
+    std::vector<CaseCond> conds;
+    std::vector<CaseBranch> branches;
+    if (int rc = compile_multi_expression(q->aggs[a].column, &canonical, &expr_ops[a], &leaves, &conds, &branches)) return rc;
+    if (int rc = case_result_type_check(s0, branches, q->aggs[a].column)) return rc;
     for (pb200_transform_op& o : expr_ops[a]) {
+      if (o.op == PB200_T_COND) o.i += (int64_t)case_conds.size();
       if (o.op != PB200_T_COLUMN) continue;
       const char* name = leaves[(size_t)o.i].c_str();
       const int ci = s0.column_index(name);
@@ -898,6 +903,11 @@ extern "C" int32_t pb200h_execute_post(pb200_ctx* ctx, const pb200h_query* q, co
       o.i = ci;
       leaf_cols.push_back(ci);
     }
+    for (const CaseCond& cc : conds) {
+      const int ci = s0.column_index(cc.column.c_str());
+      if (ci >= 0) leaf_cols.push_back(ci);
+    }
+    case_conds.insert(case_conds.end(), conds.begin(), conds.end());
     programs[a] = pb200_expr_program{(int32_t)expr_ops[a].size(), 0, expr_ops[a].data()};
     any_expr = true;
   }
@@ -987,8 +997,14 @@ extern "C" int32_t pb200h_execute_post(pb200_ctx* ctx, const pb200h_query* q, co
     dq.filter = flat.data();
     dq.group_by_columns = gb.data();
     dq.aggs = aggs.data();
-    int rc = pb200::execute_exprs_post(ctx, &dq, order, args ? dev_args.data() : nullptr, having, any_expr ? programs.data() : nullptr, post,
-                                       dsegs.data(), (int)dsegs.size(), dev_results.data());
+    // the CASE conditions, resolved on the segments of this submission
+    CaseTable cases;
+    std::vector<pb200h_segment*> hsegs;
+    for (int s : dev_idx) hsegs.push_back(segs[s]);
+    int rc = resolve_case_conditions(ctx, hsegs.data(), (int)hsegs.size(), case_conds, patterns, cases);
+    if (!rc)
+      rc = pb200::execute_exprs_post(ctx, &dq, order, args ? dev_args.data() : nullptr, having, any_expr ? programs.data() : nullptr,
+                                     case_conds.empty() ? nullptr : &cases.table, post, dsegs.data(), (int)dsegs.size(), dev_results.data());
     if (rc) { for (auto r : star_results) if (r) pb200_result_free(r); return rc; }
     // the mask pass of each expression leaf read its leaf columns at every doc of the segment
     for (size_t k = 0; k < dev_idx.size(); k++) dev_results[merge ? 0 : k]->meta.num_entries_scanned_in_filter += expr_filter_entries(*segs[dev_idx[k]], *q);

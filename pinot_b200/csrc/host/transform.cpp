@@ -168,9 +168,99 @@ struct Compiled {
   int columns = 0;
   bool multi = false;                  // any number of columns: leaf k (PB200_T_COLUMN i = k) reads column leaves[k]
   std::vector<std::string> leaves;
+  bool in_case = false;                // compiling a CASE's arguments (a nested CASE is refused)
+  std::vector<CaseCond> conds;         // CASE conditions: PB200_T_COND i = k tests conds[k]
+  std::vector<CaseBranch> branches;    // CASE branch values (THEN and ELSE)
 };
 
+int compile(const Node& n, Compiled& c);
+
+// a literal of a CASE condition as canonical text: quoted, '' for a quote
+std::string quoted(const std::string& t) {
+  std::string r = "'";
+  for (char ch : t) { r += ch; if (ch == '\'') r += '\''; }
+  return r + "'";
+}
+
+// CASE conditions (DESIGN.md section 3.19): the parser's function name (lower case, no '_') -> the canonical one
+const char* const kCondNames[][2] = {
+    {"and", "and"}, {"or", "or"}, {"not", "not"}, {"equals", "equals"}, {"notequals", "not_equals"},
+    {"lessthan", "less_than"}, {"lessthanorequal", "less_than_or_equal"}, {"greaterthan", "greater_than"},
+    {"greaterthanorequal", "greater_than_or_equal"}, {"between", "between"}, {"in", "in"}, {"notin", "not_in"},
+    {"like", "like"}, {"regexplike", "regexp_like"}};
+
+int compile_cond(const Node& n, Compiled& c) {
+  const char* name = nullptr;
+  if (n.call)
+    for (auto& k : kCondNames) if (n.text == k[0]) name = k[1];
+  if (!name) { set_error("a CASE condition must be a comparison, IN, BETWEEN, LIKE or REGEXP_LIKE leaf or AND / OR / NOT over them"); return PB200_E_UNSUPPORTED; }
+  const std::string fn = name;
+  const int na = (int)n.args.size();
+  auto op = [&](int code, int64_t i) { pb200_transform_op o; memset(&o, 0, sizeof o); o.op = code; o.i = i; c.ops.push_back(o); };
+  c.text += fn + "(";
+  if (fn == "and" || fn == "or" || fn == "not") {
+    if (fn == "not" ? na != 1 : na < 2) { set_error("%s takes %s arguments, not %d", name, fn == "not" ? "one" : "two or more", na); return PB200_E_UNSUPPORTED; }
+    for (int k = 0; k < na; k++) {
+      if (k) c.text += ",";
+      if (int rc = compile_cond(*n.args[k], c)) return rc;
+      if (k) op(fn == "and" ? PB200_T_AND : PB200_T_OR, 0);
+    }
+    if (fn == "not") op(PB200_T_NOT, 0);
+    c.text += ")";
+    return PB200_OK;
+  }
+  const bool many = fn == "in" || fn == "not_in";
+  const int want = fn == "between" ? 3 : 2;
+  if (many ? na < 2 : na != want) { set_error("%s takes %d arguments, not %d", name, want, na); return PB200_E_UNSUPPORTED; }
+  CaseCond cc;
+  cc.fn = fn;
+  for (int k = 0; k < na; k++) {
+    const Node& a = *n.args[k];
+    if (k == 0 ? a.call || a.literal : !a.literal) {
+      set_error("%s: a CASE condition compares one column with literals (no column against column, no expression operand)", name);
+      return PB200_E_UNSUPPORTED;
+    }
+    if (k) { c.text += "," + quoted(a.text); cc.literals.push_back(a.text); }
+    else { c.text += a.text; cc.column = a.text; }
+  }
+  c.text += ")";
+  op(PB200_T_COND, (int64_t)c.conds.size());
+  c.conds.push_back(std::move(cc));
+  return PB200_OK;
+}
+
+// case(c1,v1,c2,v2,...,e): postfix c1 v1 c2 v2 ... e CASE ... CASE (one CASE per WHEN)
+int compile_case(const Node& n, Compiled& c) {
+  if (c.in_case) { set_error("a nested CASE is not accelerated"); return PB200_E_UNSUPPORTED; }
+  const int na = (int)n.args.size();
+  if (na < 3 || na % 2 == 0) { set_error("case takes WHEN / THEN pairs and an ELSE value (an odd number of three or more arguments), not %d", na); return PB200_E_UNSUPPORTED; }
+  c.in_case = true;
+  c.text += "case(";
+  for (int k = 0; k < na; k++) {
+    if (k) c.text += ",";
+    const Node& a = *n.args[k];
+    if (k % 2 == 0 && k + 1 < na) {
+      if (int rc = compile_cond(a, c)) return rc;
+      continue;
+    }
+    CaseBranch b;
+    b.kind = a.call ? CaseBranch::ARITHMETIC : a.literal ? CaseBranch::DOUBLE_LITERAL : CaseBranch::COLUMN;
+    b.column = a.literal ? "" : a.text;
+    const size_t first = c.ops.size();
+    if (int rc = compile(a, c)) return rc;
+    if (a.literal && c.ops[first].op == PB200_T_LONG_LITERAL) { b.kind = CaseBranch::LONG_LITERAL; b.value = c.ops[first].i; }
+    c.branches.push_back(b);
+  }
+  for (int k = 0; k < na / 2; k++) {
+    pb200_transform_op o; memset(&o, 0, sizeof o); o.op = PB200_T_CASE; c.ops.push_back(o);
+  }
+  c.text += ")";
+  c.in_case = false;
+  return PB200_OK;
+}
+
 int compile(const Node& n, Compiled& c) {
+  if (n.call && c.multi && n.text == "case") return compile_case(n, c);
   auto op = [&](int code, int64_t i) { pb200_transform_op o; memset(&o, 0, sizeof o); o.op = code; o.i = i; c.ops.push_back(o); };
   if (n.literal) {
     bool is_int; int64_t i = 0; double d = 0;
@@ -251,8 +341,9 @@ int compile_text(const char* text, Compiled& c, bool multi = false) {
   if (!root->call) { set_error("'%s' is no expression", text); return PB200_E_INVALID; }
   if (int rc = compile(*root, c)) return rc;
   int operations = 0;
-  for (const auto& o : c.ops) operations += o.op > PB200_T_DOUBLE_LITERAL;
+  for (const auto& o : c.ops) operations += o.op > PB200_T_DOUBLE_LITERAL && o.op != PB200_T_COND;
   if (operations > pb200::kTransformMaxOps) { set_error("expression '%s' has %d operations (at most %d)", text, operations, pb200::kTransformMaxOps); return PB200_E_UNSUPPORTED; }
+  if ((int)c.ops.size() > pb200::kTransformMaxProgram) { set_error("expression '%s' compiles to %zu program entries (at most %d)", text, c.ops.size(), pb200::kTransformMaxProgram); return PB200_E_UNSUPPORTED; }
   return PB200_OK;
 }
 
@@ -304,22 +395,27 @@ int compile_expression(const char* text, std::string* canonical, std::vector<pb2
 }
 
 int compile_multi_expression(const char* text, std::string* canonical, std::vector<pb200_transform_op>* ops,
-                             std::vector<std::string>* leaves) {
+                             std::vector<std::string>* leaves, std::vector<CaseCond>* conds, std::vector<CaseBranch>* branches) {
   Compiled c;
   int rc = compile_text(text, c, true);
-  if (rc == PB200_OK && c.leaves.size() < 2) { set_error("'%s' has fewer than two column leaves", text); rc = PB200_E_UNSUPPORTED; }
+  if (rc == PB200_OK && !c.conds.empty() && !conds) { set_error("'%s': CASE is accelerated only as the argument of SUM, AVG, MIN, MAX or COUNT", text); rc = PB200_E_UNSUPPORTED; }
+  if (rc == PB200_OK && c.leaves.size() < 2 && c.conds.empty()) { set_error("'%s' has fewer than two column leaves", text); rc = PB200_E_UNSUPPORTED; }
   if (rc == PB200_OK)
     for (const auto& o : c.ops)
-      if (!pb200::expr_op_ok(o.op)) {
+      if (!pb200::expr_op_ok(o.op) && !pb200::expr_case_op(o.op)) {
         set_error("'%s': time functions are not accelerated inside an expression over two or more columns", text);
         rc = PB200_E_UNSUPPORTED;
         break;
       }
-  if (rc == PB200_OK && (int)c.leaves.size() > pb200::kExprMaxLeaves) {
-    set_error("'%s' has %zu column leaves (at most %d)", text, c.leaves.size(), pb200::kExprMaxLeaves);
+  if (rc == PB200_OK && (int)(c.leaves.size() + c.conds.size()) > pb200::kExprMaxLeaves) {
+    set_error("'%s' has %zu column leaves, conditions included (at most %d)", text, c.leaves.size() + c.conds.size(), pb200::kExprMaxLeaves);
     rc = PB200_E_UNSUPPORTED;
   }
-  if (rc == PB200_OK) { *canonical = c.text; *ops = c.ops; *leaves = c.leaves; }
+  if (rc == PB200_OK) {
+    *canonical = c.text; *ops = c.ops; *leaves = c.leaves;
+    if (conds) *conds = c.conds;
+    if (branches) *branches = c.branches;
+  }
   return rc;
 }
 
@@ -328,7 +424,7 @@ bool is_multi_column_expression(const char* text) {
   Compiled c;
   char saved[1024];
   memcpy(saved, pb200_last_error(), sizeof saved);  // a failed test leaves the caller's last error alone
-  const bool multi = compile_text(text, c, true) == PB200_OK && c.leaves.size() >= 2;
+  const bool multi = compile_text(text, c, true) == PB200_OK && (c.leaves.size() >= 2 || !c.conds.empty());
   set_error("%s", saved);
   return multi;
 }
@@ -340,7 +436,7 @@ bool is_expression_filter(const char* text) {
   memcpy(saved, pb200_last_error(), sizeof saved);
   bool multi = compile_text(text, c, true) == PB200_OK;
   set_error("%s", saved);
-  if (!multi) return false;
+  if (!multi || !c.conds.empty()) return false;   // a CASE leaf is derived, which refuses it
   for (const std::string& l : c.leaves) if (l != c.leaves[0]) return true;
   return false;
 }

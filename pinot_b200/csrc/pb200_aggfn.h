@@ -41,7 +41,8 @@ struct AggFn {
 constexpr const char *kNoDtPercentile = "PERCENTILE intermediates are not written as DataTable objects",
                      *kNoDtMoments = "VAR/STDDEV intermediates are not written as DataTable objects",
                      *kNoDtWithTime = "FIRST/LASTWITHTIME intermediates are not written as DataTable objects",
-                     *kNoDtHll = "DISTINCTCOUNTHLL is not written as a server DataTable (the reference's HyperLogLog bytes are not restated)";
+                     *kNoDtHll = "DISTINCTCOUNTHLL is not written as a server DataTable (the reference's HyperLogLog bytes are not restated)",
+                     *kNoDtCase = "an aggregation over CASE is not written as a server DataTable (the reference's spelling of CASE is not restated)";
 
 // FIRST/LASTWITHTIME: the data column's dictionary is checked with the time column's (plan_scan), not through dict_ids
 constexpr AggFn kAggFns[] = {

@@ -735,8 +735,8 @@ extern "C" int32_t pb200_execute_agg_args(pb200_ctx* ctx, const pb200_query* que
 }
 
 int pb200::execute_exprs_post(pb200_ctx* ctx, const pb200_query* query, const pb200_order_by* order, const pb200_agg_arg* args,
-                              const pb200_having* having, const pb200_expr_program* exprs, const pb200_post_aggs* post,
-                              pb200_segment* const* segments, int32_t nseg, pb200_result** results) {
+                              const pb200_having* having, const pb200_expr_program* exprs, const pb200_expr_conds* conds,
+                              const pb200_post_aggs* post, pb200_segment* const* segments, int32_t nseg, pb200_result** results) {
   if (!exprs && !post) return pb200_execute_agg_args(ctx, query, order, args, having, segments, nseg, results);
   if (!ctx || !results) { set_error("invalid argument to %s", exprs ? "pb200_execute_exprs" : "pb200_execute_post"); return PB200_E_INVALID; }
   if (post && (!query || query->num_aggs < 0 || (query->num_aggs > 0 && !query->aggs))) {
@@ -749,7 +749,7 @@ int pb200::execute_exprs_post(pb200_ctx* ctx, const pb200_query* query, const pb
   }
   ExprCall ex;
   if (exprs)
-    if (const int rc = expr_prepare(query, exprs, segments, nseg, &ex)) return rc;
+    if (const int rc = expr_prepare(query, exprs, conds, segments, nseg, &ex)) return rc;
   if (!ex.count)
     return post ? execute_checked(ctx, query, order, args, having, segments, nseg, results, nullptr, post)
                 : pb200_execute_agg_args(ctx, query, order, args, having, segments, nseg, results);
@@ -764,13 +764,20 @@ int pb200::execute_exprs_post(pb200_ctx* ctx, const pb200_query* query, const pb
 extern "C" int32_t pb200_execute_exprs(pb200_ctx* ctx, const pb200_query* query, const pb200_order_by* order, const pb200_agg_arg* args,
                                        const pb200_having* having, const pb200_expr_program* exprs, pb200_segment* const* segments,
                                        int32_t nseg, pb200_result** results) {
-  return pb200::execute_exprs_post(ctx, query, order, args, having, exprs, nullptr, segments, nseg, results);
+  return pb200::execute_exprs_post(ctx, query, order, args, having, exprs, nullptr, nullptr, segments, nseg, results);
+}
+
+extern "C" int32_t pb200_execute_exprs_cond(pb200_ctx* ctx, const pb200_query* query, const pb200_order_by* order, const pb200_agg_arg* args,
+                                            const pb200_having* having, const pb200_expr_program* exprs, const pb200_expr_conds* conds,
+                                            pb200_segment* const* segments, int32_t nseg, pb200_result** results) {
+  if (conds && !exprs) { set_error("invalid argument to pb200_execute_exprs_cond: conditions without programs"); return PB200_E_INVALID; }
+  return pb200::execute_exprs_post(ctx, query, order, args, having, exprs, conds, nullptr, segments, nseg, results);
 }
 
 extern "C" int32_t pb200_execute_post(pb200_ctx* ctx, const pb200_query* query, const pb200_order_by* order, const pb200_agg_arg* args,
                                       const pb200_having* having, const pb200_post_aggs* post, pb200_segment* const* segments,
                                       int32_t nseg, pb200_result** results) {
-  return pb200::execute_exprs_post(ctx, query, order, args, having, nullptr, post, segments, nseg, results);
+  return pb200::execute_exprs_post(ctx, query, order, args, having, nullptr, nullptr, post, segments, nseg, results);
 }
 
 // pb200_execute_agg_args past its argument check (args NULL: no percentiles and no *WITHTIME), with the expression
@@ -1375,10 +1382,13 @@ struct ScanCall {
     return PB200_OK;
   }
 
-  // columns read after the filter: the scan's group-by and aggregation columns, and every expression leaf, each once
+  // columns read after the filter: the scan's group-by and aggregation columns, and every expression leaf and condition
+  // column, each once
   int projected() const {
     if (!ex) return plan.projected;
     std::vector<int> cols = ex->cols;
+    for (int c : ex->ccols)
+      if (std::find(cols.begin(), cols.end(), c) == cols.end()) cols.push_back(c);
     for (int k = 0; k < plan.q.num_slots; k++)
       if ((plan.q.slot_roles[k] & (ROLE_GROUP | ROLE_AGG)) && std::find(cols.begin(), cols.end(), plan.slot_cols[k]) == cols.end())
         cols.push_back(plan.slot_cols[k]);

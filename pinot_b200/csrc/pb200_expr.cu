@@ -13,6 +13,10 @@
 //      results reduce in registers and once per block.
 // Both launches are queued on the call's stream behind the scan; neither synchronises.
 //
+// CASE WHEN (DESIGN.md section 3.19, pb200_execute_exprs_cond) runs in the same pass, in its own instantiation of the
+// kernel: per matched doc it reads each distinct condition column's dictId once, tests it against every condition of
+// that column (a dictId range, or a bit of the call's bitset buffer), and hands the row's condition word to the program.
+//
 // Predicates on such expressions (DESIGN.md section 3.16, pb200_expr_doc_masks) run before the query is planned:
 // expr_mask_kernel evaluates every doc of every segment against each predicate and writes the doc mask that the query's
 // filter tree then reads as a PB200_F_DOC_MASK leaf.
@@ -21,6 +25,7 @@
 #include <algorithm>
 #include <cstring>
 #include <memory>
+#include <type_traits>
 #include <vector>
 
 #include "pb200_expr.h"
@@ -54,6 +59,18 @@ struct ExprProg {
   pb200_transform_op ops[kMaxAggs][kTransformMaxProgram];
 };
 
+constexpr int kExprMaxConds = PB200_MAX_EXPR_CONDS;
+struct CondSeg {                      // one segment's conditions, grouped by column
+  int32_t ncc;                        // distinct condition columns
+  int32_t first[kExprMaxConds + 1];   // the conditions of column c: entries first[c] .. first[c + 1] - 1
+  SelCol ccol[kExprMaxConds];         // read_at only: the dictId
+  int32_t kind[kExprMaxConds];        // PB200_COND_*
+  int32_t slot[kExprMaxConds];        // the condition's index in the call's table: its bit in the row's condition word
+  uint32_t hi[kExprMaxConds];         // RANGE: [lo, hi)
+  uint32_t pad;
+  long long lo[kExprMaxConds];        // RANGE: lo; BITSET: the first word of this segment's bitset
+};
+
 // the table entry of the group of `doc`; false when its key is not in the hash table (only after an overflow, whose
 // result is discarded as PB200_E_LIMIT)
 __device__ __forceinline__ bool expr_entry(const ExprSeg& s, int32_t doc, unsigned long long& g) {
@@ -80,24 +97,46 @@ __device__ __forceinline__ double leaf_value(const SelCol& c, int32_t doc) {
   return c.kind == SEL_DICT_F32 || c.kind == SEL_DICT_F64 || c.kind == SEL_RAW_F32 ? __longlong_as_double((long long)w) : (double)(long long)w;
 }
 
+// bit k: condition k holds for `doc`
+__device__ __forceinline__ uint32_t cond_word(const CondSeg& cs, const uint32_t* __restrict__ bits, int32_t doc) {
+  uint32_t w = 0;
+  for (int c = 0; c < cs.ncc; ++c) {
+    const uint32_t id = read_at(cs.ccol[c], doc);
+    for (int k = cs.first[c]; k < cs.first[c + 1]; ++k) {
+      const bool hit = cs.kind[k] == PB200_COND_RANGE ? id >= (uint32_t)cs.lo[k] && id < cs.hi[k]
+                                                     : ((__ldg(bits + cs.lo[k] + (id >> 5)) >> (id & 31)) & 1u) != 0u;
+      w |= (uint32_t)hit << cs.slot[k];
+    }
+  }
+  return w;
+}
+
 __device__ __forceinline__ bool is_sum(int fn) { return fn == PB200_AGG_SUM || fn == PB200_AGG_AVG; }
 __device__ __forceinline__ unsigned long long key_of(double r) { return transform_key(TK_DOUBLE, 0, r); }
 __device__ __forceinline__ unsigned long long key_pick(int fn, unsigned long long a, unsigned long long b) {
   return fn == PB200_AGG_MIN ? (a < b ? a : b) : (a > b ? a : b);
 }
 
-// grid: (blocks per segment, segments); one warp per 32-doc mask word at a time.  GB: group-by (one instantiation each,
-// so that neither carries the other's live state)
-template <bool GB>
-__global__ void __launch_bounds__(kExprThreads) expr_kernel(const ExprSeg* __restrict__ segs, const ExprProg* __restrict__ gprog) {
+// grid: (blocks per segment, segments); one warp per 32-doc mask word at a time.  GB: group-by, COND: programs with
+// conditions (csegs: one CondSeg per segment, bits: the call's bitsets).  One instantiation each, so that none carries
+// another's live state.
+template <bool GB, bool COND>
+__global__ void __launch_bounds__(kExprThreads) expr_kernel(const ExprSeg* __restrict__ segs, const ExprProg* __restrict__ gprog,
+                                                            const CondSeg* __restrict__ csegs, const uint32_t* __restrict__ bits) {
   constexpr bool group_by = GB;
   __shared__ ExprProg prog;
   __shared__ double red_s[kExprThreads / 32][kMaxAggs];
   __shared__ unsigned long long red_k[kExprThreads / 32][kMaxAggs];
+  __shared__ std::conditional_t<COND, CondSeg, int> cs;
   {
     const uint32_t* src = reinterpret_cast<const uint32_t*>(gprog);
     uint32_t* dst = reinterpret_cast<uint32_t*>(&prog);
     for (int i = threadIdx.x; i < (int)(sizeof(ExprProg) / 4); i += blockDim.x) dst[i] = src[i];
+    if constexpr (COND) {
+      const uint32_t* csrc = reinterpret_cast<const uint32_t*>(csegs + blockIdx.y);
+      uint32_t* cdst = reinterpret_cast<uint32_t*>(&cs);
+      for (int i = threadIdx.x; i < (int)(sizeof(CondSeg) / 4); i += blockDim.x) cdst[i] = csrc[i];
+    }
   }
   __syncthreads();
   const ExprSeg& s = segs[blockIdx.y];
@@ -118,11 +157,14 @@ __global__ void __launch_bounds__(kExprThreads) expr_kernel(const ExprSeg* __res
     if (active == 0u) continue;
     if (ok)
       for (int c = 0; c < s.ncols; ++c) v[c] = leaf_value(s.col[c], doc);
+    uint32_t cw = 0;
+    if constexpr (COND)
+      if (ok) cw = cond_word(cs, bits, doc);
     if (!group_by) {
 #pragma unroll
       for (int x = 0; x < kMaxAggs; ++x) {
         if (x >= nx || !ok) continue;
-        const double r = expr_eval(prog.ops[x], prog.len[x], v);
+        const double r = expr_eval<COND>(prog.ops[x], prog.len[x], v, cw);
         if (is_sum(prog.fn[x])) acc_s[x] = t_add(acc_s[x], r);
         else acc_k[x] = key_pick(prog.fn[x], acc_k[x], key_of(r));
       }
@@ -134,7 +176,7 @@ __global__ void __launch_bounds__(kExprThreads) expr_kernel(const ExprSeg* __res
     const int leader = __ffs(ok ? peers : active) - 1;
     for (int x = 0; x < nx; ++x) {
       const int fn = prog.fn[x];
-      const double r = ok ? expr_eval(prog.ops[x], prog.len[x], v) : 0.0;
+      const double r = ok ? expr_eval<COND>(prog.ops[x], prog.len[x], v, cw) : 0.0;
       if (is_sum(fn)) {
         double t = ok ? r : 0.0;
         if (uniform) {
@@ -276,9 +318,33 @@ bool reuse_leaf_buffers(const ScanPlan& scan_plan, ScanPlan& mask_plan) {
   return true;
 }
 
+// Checks the condition table of pb200_execute_exprs_cond against the segments and collects its distinct columns
+int cond_prepare(const pb200_expr_conds& t, pb200_segment* const* segments, int nseg, int ncols, std::vector<int>& ccols) {
+  if (t.reserved != 0 || t.num_conds < 1 || t.num_conds > PB200_MAX_EXPR_CONDS || !t.conds || t.num_words < 0 || (t.num_words > 0 && !t.words)) {
+    set_error("malformed condition table"); return PB200_E_INVALID;
+  }
+  for (int k = 0; k < t.num_conds; k++) {
+    const pb200_expr_cond& c = t.conds[k];
+    if (c.column < 0 || c.column >= ncols) { set_error("condition %d: column %d out of range", k, c.column); return PB200_E_INVALID; }
+    if ((c.kind != PB200_COND_RANGE && c.kind != PB200_COND_BITSET) || !c.args) { set_error("condition %d: malformed", k); return PB200_E_INVALID; }
+    for (int s = 0; s < nseg; s++) {
+      const DeviceColumn& dc = segments[s]->cols[c.column];
+      const int kind = selection_kind(dc);
+      if (kind < 0 || kind == SEL_RAW_I32 || kind == SEL_RAW_F32) { set_error("condition %d: column %d of segment %d has no dictIds", k, c.column, s); return PB200_E_UNSUPPORTED; }
+      const long long a = c.args[2 * s], b = c.args[2 * s + 1];
+      const bool ok = c.kind == PB200_COND_RANGE ? 0 <= a && a <= b && b <= dc.cardinality
+                                                 : a >= 0 && b >= ((long long)dc.cardinality + 31) / 32 && b <= t.num_words - a;
+      if (!ok) { set_error("condition %d: %s outside segment %d's dictIds or the bitset words", k, c.kind == PB200_COND_RANGE ? "range" : "bitset", s); return PB200_E_INVALID; }
+    }
+    if (std::find(ccols.begin(), ccols.end(), c.column) == ccols.end()) ccols.push_back(c.column);
+  }
+  return PB200_OK;
+}
+
 }  // namespace
 
-int expr_prepare(const pb200_query* query, const pb200_expr_program* exprs, pb200_segment* const* segments, int nseg, ExprCall* out) {
+int expr_prepare(const pb200_query* query, const pb200_expr_program* exprs, const pb200_expr_conds* conds, pb200_segment* const* segments,
+                 int nseg, ExprCall* out) {
   ExprCall& x = *out;
   x = ExprCall();
   if (!query || !segments || nseg <= 0 || query->num_aggs < 0 || query->num_aggs > kMaxAggs || (query->num_aggs > 0 && !query->aggs)) {
@@ -286,13 +352,17 @@ int expr_prepare(const pb200_query* query, const pb200_expr_program* exprs, pb20
   }
   const int ncols = common_columns(segments, nseg);
   if (ncols < 0) { set_error("segments do not share their registered columns"); return PB200_E_INVALID; }
+  if (conds) {
+    if (int rc = cond_prepare(*conds, segments, nseg, ncols, x.ccols)) return rc;
+    x.conds = conds;
+  }
   for (int a = 0; a < query->num_aggs; a++) {
     const pb200_expr_program& e = exprs[a];
     if (e.num_ops == 0) continue;
     if (e.num_ops < 0 || !e.ops || e.reserved != 0) { set_error("aggregation %d: malformed expression program", a); return PB200_E_INVALID; }
     const char* why = "";
     int leaves = 0;
-    if (int rc = expr_check(e.ops, e.num_ops, &leaves, &why)) { set_error("aggregation %d: %s", a, why); return rc; }
+    if (int rc = expr_check(e.ops, e.num_ops, &leaves, &why, conds ? conds->num_conds : 0)) { set_error("aggregation %d: %s", a, why); return rc; }
     const int fn = query->aggs[a].function;
     if (fn == PB200_AGG_COUNT) continue;   // COUNT(expr) is COUNT(*)
     if (fn != PB200_AGG_SUM && fn != PB200_AGG_AVG && fn != PB200_AGG_MIN && fn != PB200_AGG_MAX) {
@@ -400,8 +470,42 @@ int expr_launch(pb200_ctx* ctx, cudaStream_t st, const Tuning& tune, const pb200
   PB200_CUDA(cudaMemcpyAsync(dprog, &prog, sizeof prog, cudaMemcpyHostToDevice, st));
   const long long per_seg = std::max<long long>(1, (long long)ctx->sm_count * 8 / nseg);
   const dim3 grid((unsigned)std::min<long long>((max_words + kExprThreads / 32 - 1) / (kExprThreads / 32), std::max<long long>(per_seg, 2)), (unsigned)nseg);
-  if (plan.group_by) expr_kernel<true><<<grid, kExprThreads, 0, st>>>(dsegs, dprog);
-  else expr_kernel<false><<<grid, kExprThreads, 0, st>>>(dsegs, dprog);
+  if (!x.conds) {
+    if (plan.group_by) expr_kernel<true, false><<<grid, kExprThreads, 0, st>>>(dsegs, dprog, nullptr, nullptr);
+    else expr_kernel<false, false><<<grid, kExprThreads, 0, st>>>(dsegs, dprog, nullptr, nullptr);
+    PB200_CUDA(cudaGetLastError());
+    return PB200_OK;
+  }
+  // the conditions: per segment grouped by column, and the call's bitsets in one buffer
+  const pb200_expr_conds& t = *x.conds;
+  std::vector<CondSeg> cseg(nseg);
+  for (int s = 0; s < nseg; s++) {
+    CondSeg& c = cseg[s];
+    memset(&c, 0, sizeof c);
+    c.ncc = (int)x.ccols.size();
+    int n = 0;
+    for (int j = 0; j < c.ncc; j++) {
+      const DeviceColumn& dc = segments[s]->cols[x.ccols[j]];
+      c.ccol[j] = SelCol{dc.fwd, nullptr, dc.bits, SEL_DICT_ID, 0, 0};
+      c.first[j] = n;
+      for (int k = 0; k < t.num_conds; k++) {
+        if (t.conds[k].column != x.ccols[j]) continue;
+        c.kind[n] = t.conds[k].kind;
+        c.slot[n] = k;
+        c.lo[n] = t.conds[k].args[2 * s];
+        c.hi[n] = t.conds[k].kind == PB200_COND_RANGE ? (uint32_t)t.conds[k].args[2 * s + 1] : 0u;
+        n++;
+      }
+    }
+    c.first[c.ncc] = n;
+  }
+  CondSeg* dcond = static_cast<CondSeg*>(temp(sizeof(CondSeg) * nseg));
+  uint32_t* dbits = static_cast<uint32_t*>(temp(std::max<size_t>((size_t)t.num_words, 1) * 4));
+  if (!dcond || !dbits) return PB200_E_CUDA;
+  PB200_CUDA(cudaMemcpyAsync(dcond, cseg.data(), sizeof(CondSeg) * nseg, cudaMemcpyHostToDevice, st));
+  if (t.num_words > 0) PB200_CUDA(cudaMemcpyAsync(dbits, t.words, (size_t)t.num_words * 4, cudaMemcpyHostToDevice, st));
+  if (plan.group_by) expr_kernel<true, true><<<grid, kExprThreads, 0, st>>>(dsegs, dprog, dcond, dbits);
+  else expr_kernel<false, true><<<grid, kExprThreads, 0, st>>>(dsegs, dprog, dcond, dbits);
   PB200_CUDA(cudaGetLastError());
   return PB200_OK;
 }

@@ -408,9 +408,10 @@ int decode_sets(pb200_ctx* ctx, cudaStream_t st, pb200_result* R, DevBufRaw* con
 void result_materialize(pb200_result* R);  // view -> the std::vector fields
 // pb200_execute_exprs (exprs NULL: no expression aggregations) whose ORDER BY may name the post-aggregation programs of
 // pb200_execute_post (post NULL: none); both NULL is pb200_execute_agg_args.  The host layer's one device entry point.
+// conds: the CASE WHEN conditions of the programs (pb200_execute_exprs_cond; NULL: none).
 int execute_exprs_post(pb200_ctx* ctx, const pb200_query* query, const pb200_order_by* order, const pb200_agg_arg* args,
-                       const pb200_having* having, const pb200_expr_program* exprs, const pb200_post_aggs* post,
-                       pb200_segment* const* segments, int32_t nseg, pb200_result** results);
+                       const pb200_having* having, const pb200_expr_program* exprs, const pb200_expr_conds* conds,
+                       const pb200_post_aggs* post, pb200_segment* const* segments, int32_t nseg, pb200_result** results);
 // pb200_order_by checks shared by the device and host entry points, with the post-aggregation programs its
 // PB200_ORDER_POST items may name (post NULL: none): PB200_OK or PB200_E_INVALID (message set)
 int order_validate(const pb200_order_by* order, int num_aggs, int num_group_by, const pb200_post_aggs* post = nullptr);

@@ -226,12 +226,16 @@ struct ExprCall {
   int fn_of[kMaxAggs];                           // aggregation -> PB200_AGG_SUM / AVG / MIN / MAX (-1: not an expression)
   std::vector<pb200_transform_op> ops[kMaxAggs]; // device programs: PB200_T_COLUMN i = index into cols
   std::vector<int> cols;                         // the distinct leaf column ids
+  const pb200_expr_conds* conds = nullptr;       // the call's CASE WHEN conditions (pb200_execute_exprs_cond; NULL: none)
+  std::vector<int> ccols;                        // the distinct condition column ids
 };
 // where one result's expression values go: per aggregation a table of `groups` entries (group-by) or one word
 // (aggregation only) -- f64 sums, or u64 Double.compare keys for MIN / MAX -- and the hash table keys (NULL: dense)
 struct ExprOut { void* out[kMaxAggs] = {}; const unsigned long long* hkeys = nullptr; };
-// Validates the programs against the segments and fills `out`; PB200_OK or the code of pb200_execute_exprs (no CUDA call).
-int expr_prepare(const pb200_query* query, const pb200_expr_program* exprs, pb200_segment* const* segments, int nseg, ExprCall* out);
+// Validates the programs and conditions (NULL: none) against the segments and fills `out`; PB200_OK or the code of
+// pb200_execute_exprs_cond (no CUDA call).
+int expr_prepare(const pb200_query* query, const pb200_expr_program* exprs, const pb200_expr_conds* conds, pb200_segment* const* segments,
+                 int nseg, ExprCall* out);
 // Queues the mask scan (none when the filter matches every doc) and the expression pass on `st`, behind the scan of
 // `plan`; filter_query = the query the scan ran.  Device scratch stays in `temps` until the caller's synchronisation.
 int expr_launch(pb200_ctx* ctx, cudaStream_t st, const Tuning& tune, const pb200_query* filter_query, pb200_segment* const* segments,

@@ -561,11 +561,13 @@ _EXPR_TOKEN = re.compile(r"'(?:[^']|'')*'|[A-Za-z_$][\w$.]*|[0-9.][0-9.]*(?:[eE]
 
 
 def is_multi_column_expression(function: str, column) -> bool:
-    """SUM / AVG / MIN / MAX over an expression with two or more column leaves (DESIGN.md section 3.15): computed per row
+    """SUM / AVG / MIN / MAX over an expression with two or more column leaves (DESIGN.md section 3.15) or over CASE: computed per row
     on the device, not derived; the same test as the library's (a name followed by '(' is a function, a quoted or numeric
     token a literal, any other name a column)."""
     if function not in ("SUM", "AVG", "MIN", "MAX") or not column or "(" not in column:
         return False
+    if column.startswith("case("):   # CASE WHEN (DESIGN.md section 3.19) is computed per row whatever its column count
+        return True
     tokens = _EXPR_TOKEN.findall(column)
     leaves = 0
     for k, t in enumerate(tokens):

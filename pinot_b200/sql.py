@@ -33,6 +33,13 @@ stays Java).  This module exists so the parity tests read like the reference's
     hcond := cond whose left-hand sides are aggregation calls (COUNT(*), FN(col), PERCENTILE(col, p), ...) and whose
              literals are numbers.  An aggregation named only in HAVING is computed as a hidden one (Aggregation.hidden):
              ORDER BY may name it, it is never an output column.  HAVING on a column belongs in WHERE and is refused.
+    case  := CASE WHEN ccond THEN value [WHEN ccond THEN value ...] ELSE value END, only as the whole argument of SUM,
+             AVG, MIN, MAX or COUNT (DESIGN.md section 3.19); named case(c1,v1,...,e).  value := the arithmetic of col below
+             (and a leading unary minus, times('-1',x)); ccond := AND / OR / NOT / parentheses over `col op literal`,
+             col BETWEEN a AND b, col [NOT] IN (...), col [NOT] LIKE 'p', REGEXP_LIKE(col, 'p'), spelled equals(a,'1'),
+             not_equals, less_than, less_than_or_equal, greater_than, greater_than_or_equal, between, in, not_in, like,
+             regexp_like, and, or, not.  Refused: no ELSE, a nested or simple CASE, column against column, expression
+             operands, string values, CASE anywhere else.
     post  := arithmetic over aggregation calls, a post-aggregation expression (DESIGN.md section 3.18):
              post := term (+|- term)* ; term := unary (*|/ unary)* ; unary := -unary | factor ;
              factor := agg | number | (post), with at least one agg.  Numbers are finite decimals; a column, a string, %
@@ -227,6 +234,7 @@ class _Parser:
             pos = m.end()
         self.i = 0
         self.having: Optional[List[Aggregation]] = None   # inside HAVING: the aggregations its leaves name
+        self.in_case = False   # inside a CASE's branches
 
     def peek(self):
         return self.toks[self.i] if self.i < len(self.toks) else (None, None)
@@ -331,6 +339,12 @@ class _Parser:
 
     def _factor(self):
         k, v = self.peek()
+        if k == "id" and v.upper() == "CASE":
+            if self.in_case:
+                raise SqlError("a nested CASE is not supported")
+            raise SqlError("CASE is accepted only as the whole argument of SUM, AVG, MIN, MAX or COUNT")
+        if self.in_case and self.take_op("-"):   # a negated CASE value (THEN -bytes): IEEE negation, -1 * x
+            return f"times('-1',{self._factor()[0]})", False
         if k in ("num", "str"):
             self.i += 1
             return _literal_text(v), True
@@ -390,10 +404,116 @@ class _Parser:
                 raise SqlError(f"{fn}(*) is not valid")
             agg = Aggregation("COUNT", None)
         else:
-            col = self.column()
+            col = self.case_expr() if self.kw("CASE") and fn in _CASE_FUNCTIONS else self.column()
             agg = Aggregation("COUNT", None) if fn == "COUNT" else Aggregation(fn, col)
         self.expect_op(")")
         return agg
+
+    # ---- CASE WHEN as an aggregation argument (DESIGN.md section 3.19) ----------------------------------------------
+    def case_expr(self) -> str:
+        """CASE WHEN cond THEN value [WHEN ...] ELSE value END, named case(c1,v1,...,e)."""
+        self.expect_kw("CASE")
+        if not self.kw("WHEN"):
+            raise SqlError("simple CASE (CASE x WHEN v THEN ...) is not supported: write CASE WHEN x = v THEN ...")
+        parts = []
+        self.in_case = True
+        try:
+            while self.take_kw("WHEN"):
+                parts.append(self.case_cond())
+                self.expect_kw("THEN")
+                parts.append(self._case_value())
+            if not self.take_kw("ELSE"):
+                raise SqlError("CASE without ELSE is not supported (an implicit ELSE NULL has no value without null handling)")
+            parts.append(self._case_value())
+            self.expect_kw("END")
+        finally:
+            self.in_case = False
+        return f"case({','.join(parts)})"
+
+    def _case_value(self) -> str:
+        start = self.i
+        text, is_literal = self._additive()
+        if is_literal and self.toks[start][0] == "str" and not _DECIMAL.fullmatch(self.toks[start][1]):
+            raise SqlError(f"CASE values are numbers, columns or arithmetic, got the string {self.toks[start][1]!r}")
+        return text
+
+    def case_cond(self) -> str:
+        kids = [self._case_and()]
+        while self.take_kw("OR"):
+            kids.append(self._case_and())
+        return kids[0] if len(kids) == 1 else f"or({','.join(kids)})"
+
+    def _case_and(self) -> str:
+        kids = [self._case_not()]
+        while self.take_kw("AND"):
+            kids.append(self._case_not())
+        return kids[0] if len(kids) == 1 else f"and({','.join(kids)})"
+
+    def _case_not(self) -> str:
+        if self.take_kw("NOT"):
+            return f"not({self._case_not()})"
+        if self.take_op("("):
+            inner = self.case_cond()
+            self.expect_op(")")
+            return inner
+        return self._case_leaf()
+
+    def _case_column(self) -> str:
+        k, v = self.peek()
+        nxt = self.toks[self.i + 1] if self.i + 1 < len(self.toks) else (None, None)
+        if k != "id" or nxt == ("op", "(") or (nxt[0] == "op" and nxt[1] in "+-*/%") or (nxt[0] == "num" and nxt[1] < 0):
+            raise SqlError(f"a CASE condition compares one column with literals, got {self.peek()}")
+        self.i += 1
+        return v
+
+    def _case_literal(self) -> str:
+        k, v = self.peek()
+        if k not in ("num", "str"):
+            raise SqlError(f"a CASE condition compares one column with literals (no column against column), got {self.peek()}")
+        self.i += 1
+        return _case_literal_text(v)
+
+    def _case_leaf(self) -> str:
+        k, v = self.peek()
+        if k == "id" and v.upper() == "REGEXP_LIKE" and self.toks[self.i + 1:self.i + 2] == [("op", "(")]:
+            self.i += 2
+            col = self._case_column()
+            self.expect_op(",")
+            pat = self.pattern()
+            self.expect_op(")")
+            return f"regexp_like({col},{_quote(pat)})"
+        if k in ("num", "str"):   # `literal op col` is `col op' literal`
+            lit = self._case_literal()
+            k, op = self.peek()
+            if k != "op" or op not in _FLIPPED:
+                raise SqlError(f"expected a comparison operator after the literal {lit}")
+            self.i += 1
+            return f"{_CASE_OPS[_FLIPPED[op]]}({self._case_column()},{lit})"
+        col = self._case_column()
+        if self.take_kw("BETWEEN"):
+            lo = self._case_literal()
+            self.expect_kw("AND")
+            return f"between({col},{lo},{self._case_literal()})"
+        negate = self.take_kw("NOT")
+        if self.take_kw("LIKE"):
+            pat = self.pattern()
+            like_to_regexp(pat)   # the same refusals as a WHERE leaf
+            leaf = f"like({col},{_quote(pat)})"
+            return f"not({leaf})" if negate else leaf
+        if self.take_kw("IN"):
+            self.expect_op("(")
+            vals = [self._case_literal()]
+            while self.take_op(","):
+                vals.append(self._case_literal())
+            self.expect_op(")")
+            return f"{'not_in' if negate else 'in'}({col},{','.join(vals)})"
+        if negate:
+            raise SqlError("NOT must be followed by IN or LIKE here")
+        k, op = self.peek()
+        if k != "op" or op not in _CASE_OPS:
+            raise SqlError(f"expected a comparison operator in a CASE condition, got {self.peek()}")
+        self.i += 1
+        return f"{_CASE_OPS[op]}({col},{self._case_literal()})"
 
     # ---- post-aggregation expressions: arithmetic over aggregation calls -------------------------------------------
     def post_item(self):
@@ -595,6 +715,25 @@ class _Parser:
 # `literal op x` written as `x op' literal`
 _FLIPPED = {"=": "=", "!=": "!=", "<>": "<>", "<": ">", "<=": ">=", ">": "<", ">=": "<="}
 
+# CASE WHEN (DESIGN.md section 3.19): the functions that take it, and its comparisons by canonical name
+_CASE_FUNCTIONS = ("SUM", "AVG", "MIN", "MAX", "COUNT")
+_CASE_OPS = {"=": "equals", "!=": "not_equals", "<>": "not_equals", "<": "less_than", "<=": "less_than_or_equal",
+             ">": "greater_than", ">=": "greater_than_or_equal"}
+
+
+def _quote(s: str) -> str:
+    return "'" + s.replace("'", "''") + "'"
+
+
+def _case_literal_text(v) -> str:
+    """A CASE condition literal: strings as written, numbers by value.  A decimal literal beyond 2^53 keeps a decimal
+    form ('1e+16'): it is integral as a double, and a LONG column refuses it rather than compare with its rounding."""
+    if isinstance(v, str):
+        return _quote(v)
+    if isinstance(v, float) and math.isfinite(v) and abs(v) >= 2.0 ** 53:
+        return f"'{v!r}'"
+    return _literal_text(v)
+
 
 def _comparison(col: str, op: str, v) -> Predicate:
     if op == "=":
@@ -771,7 +910,12 @@ def parse(sql: str, **options) -> QueryContext:
                     p.expect_op(")")
                     expr = f"{_DISTINCT_OF[name.upper()].lower()}({inner})"
                 else:
-                    inner = "*" if p.take_op("*") else p.column()
+                    if p.kw("CASE") and name.upper() in _CASE_FUNCTIONS:   # named as in the SELECT list
+                        inner = p.case_expr()
+                        if name.upper() == "COUNT":
+                            inner = "*"
+                    else:
+                        inner = "*" if p.take_op("*") else p.column()
                     p.expect_op(")")
                     expr = f"{name.lower()}({inner})"
             else:
